@@ -854,6 +854,16 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
             prefetch_targets(c, a.targets + ((int64_t)__ldg(a.env2task + eh) * c.nt) * 3, ct_now[h], h, tr);
         }
     }
+    // Velocity task, tile kernel: the state leaves before the observation and reward work, so that its stores drain
+    // while that work runs instead of at the end of the step.  Its ct is final here (velocity_control has no collision
+    // rule: only ct == nt and a failure end an episode, finish_step); an auto-reset rewrites the state below.
+    const bool state_first = N == 1 && !EARLY && vel;
+    if (state_first) {
+        QState s1;
+        get_lane_state(s, 0, s1);
+        if (s1.ct[0] == c.nt || fail[0]) s1.ct[0] = 0;
+        store_state(a, e, s1);
+    }
     T o[kMaxObs], reward;
     int done[N];
     bool wf[N];
@@ -875,7 +885,7 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
             if (h < nact) {
                 QState s1;
                 get_lane_state(s, h, s1);
-                store_state(a, e + h, s1);
+                if (!state_first || wf[h]) store_state(a, e + h, s1);
                 a.rew[e + h] = lane(reward, h);
                 a.done[e + h] = (uint8_t)done[h];
                 if (a.fail) a.fail[e + h] = fail[h];
@@ -921,10 +931,11 @@ __device__ __forceinline__ void publish_final(const QuadArgs &a, const float *ft
 }
 
 // Scalar step kernel, 64 envs per CTA (small batches, and batches between one wave of 512-thread CTAs and the streaming
-// regime).  EARLY: fetch the velocity-target rows before the integrator (hides their latency, +8 registers).  Right when one
-// launch is a single wave of CTAs (latency-bound, e.g. 65 536 envs); for multi-wave launches the extra registers cost one
-// resident CTA per SM and other CTAs already hide the latency, so the host picks EARLY=false.
-template <bool SIMPLE, bool EARLY>
+// regime).  The velocity-target rows are fetched after the integrator (step_body EARLY = false): fetched before it, their
+// six scattered 4-byte gathers per env meet every warp's state loads at the start of the step, and the 65 536-env step
+// measured 3 % slower that way on an H100.  For velocity_control the kernel also stores the stepped state right after
+// the integrator, before the observation work (step_body): 5 % faster together (DESIGN.md section 4).
+template <bool SIMPLE>
 __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_constant__ QuadConst c,
                                                              const __grid_constant__ QuadArgs a)
 {
@@ -953,7 +964,7 @@ __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_consta
         load_state(a, e, s);
         const float4 act = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
         const float V[4] = {act.x, act.y, act.z, act.w};
-        step_body<SIMPLE, EARLY, float>(c, a, e, 1, s, V, tile + threadIdx.x * D, ftile + threadIdx.x * D, final_mask);
+        step_body<SIMPLE, false, float>(c, a, e, 1, s, V, tile + threadIdx.x * D, ftile + threadIdx.x * D, final_mask);
     }
     publish_tile(a.obs, tile, e0, rows, D);
     publish_final(a, ftile, e, threadIdx.x, 1, final_mask, D);
@@ -1539,6 +1550,9 @@ extern "C" int mgb_quad_set_targets(mgb_quad *h, const float *tbl_dev, int32_t n
     MGB_CUDA(cudaMalloc(&h->env2task, sizeof(int32_t) * h->n));
     MGB_CUDA(cudaMemcpy(h->targets, tbl_dev, tb, cudaMemcpyDeviceToDevice));
     MGB_CUDA(cudaMemcpy(h->env2task, env2task_dev, sizeof(int32_t) * h->n, cudaMemcpyDeviceToDevice));
+    // a device-to-device cudaMemcpy may return before the copy is done, and a step launched next on a non-blocking
+    // stream would not be ordered after it
+    MGB_CUDA(cudaDeviceSynchronize());
     h->n_tasks = n_tasks;
     return MGB_OK;
 }
@@ -1599,9 +1613,9 @@ static StepKernel choose_step_kernel(const mgb_quad *h, const QuadArgs &a)
                              (reinterpret_cast<uintptr_t>(a.done) & 1u) == 0 && (reinterpret_cast<uintptr_t>(a.fail) & 7u) == 0;
         if (aligned) return STEP_PACKED;
     }
-    // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (700 W, velocity_control
-    // dt = 0.005, CUDA graphs of 256 steps), us per step tile / wide: 9 473 envs 5.41 / 3.35, 24 576 envs 5.84 / 5.09,
-    // 49 152 envs 7.84 / 6.42, but 65 536 envs 7.47 / 8.69 and 67 001 envs 8.14 / 8.53 (16 384 and 33 792 envs: within 2 %).
+    // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (400 W power limit,
+    // velocity_control dt = 0.005, CUDA graphs of 256 steps), us per step tile / wide: 9 473 envs 5.38 / 3.23, 24 576 envs
+    // 5.99 / 5.07, 49 152 envs 6.71 / 6.42, but 65 536 envs 7.49 / 8.92 and 67 001 envs 8.18 / 8.81.
     // So by default the wide kernel takes batches of up to 384 envs per SM and the 64-env tile kernel the rest.
     const bool single_wave = a.n <= (int64_t)h->num_sms * 512 && a.n >= (int64_t)h->num_sms * 64;
     const int64_t wide_max = (int64_t)h->num_sms * (h->wide_kernel > 0 ? 512 : 384);
@@ -1648,15 +1662,8 @@ static int launch_step(mgb_quad *h, const QuadArgs &a, cudaStream_t st)
             else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_wide_kernel<false>, h->c, aw));
         }
     } else {
-        // single wave (<= ~8 resident CTAs per SM) -> latency-bound -> early target fetch; otherwise favour occupancy
-        const bool early = blocks <= (unsigned)h->num_sms * 10u;
-        if (h->c.simple) {
-            if (early) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<true, true>, h->c, a));
-            else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<true, false>, h->c, a));
-        } else {
-            if (early) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<false, true>, h->c, a));
-            else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<false, false>, h->c, a));
-        }
+        if (h->c.simple) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<true>, h->c, a));
+        else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<false>, h->c, a));
     }
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
@@ -1671,7 +1678,7 @@ extern "C" const char *mgb_quad_step_kernel(const mgb_quad *h)
     case STEP_STREAM: return h->c.simple ? "quad_stream_kernel<true>" : "quad_stream_kernel<false>";
     case STEP_PACKED: return h->c.simple ? "quad_step2_kernel<true>" : "quad_step2_kernel<false>";
     case STEP_WIDE: return h->c.simple ? "quad_step_wide_kernel<true>" : "quad_step_wide_kernel<false>";
-    default: return h->c.simple ? "quad_step_kernel<true,.>" : "quad_step_kernel<false,.>";
+    default: return h->c.simple ? "quad_step_kernel<true>" : "quad_step_kernel<false>";
     }
 }
 
