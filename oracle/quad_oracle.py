@@ -4,12 +4,14 @@ Follows metagym/quadrotor/quadrotorsim.py:50-109 (_parse_cfg) for turning a simu
 exposes ``sim_step`` (quadrotorsim.py:295-304) and ``env_step`` (env.py:127-165) in three precisions:
 ``f32`` (never-reset simulator), ``mix`` (after reset(): float64 velocity vectors) and ``f64`` (arbiter).
 """
+import copy
 import ctypes
 import json
 
 import numpy as np
 
 from . import build as _build
+from . import philox
 
 TASKS = {"no_collision": 0, "hovering_control": 1, "velocity_control": 2}
 
@@ -142,6 +144,115 @@ def reset_state(cfg_params, noise):
     s[:, 3:6] = base_v + (float(iv["noisy"]) * noise[:, 3:6]) * sv
     s[:, 6:9] = base_w + (float(iw["noisy"]) * noise[:, 9:12]) * sw
     return s
+
+
+def general_params():
+    """A config that leaves the engine's specialised kernels (SIMPLE = false): off-diagonal inertia, a
+    centre-of-gravity offset, CT[2] != 0 and rotors out of the body plane."""
+    p = copy.deepcopy(DEFAULT_PARAMS)
+    p["inertia"].update(xy=0.001, xz=-0.0005, yz=0.0007)
+    p["gravity_center"] = {"x": 0.01, "y": -0.02, "z": 0.015}
+    p["thrust"]["CT"][2] = "1.0e-3"
+    for i, z in enumerate([0.02, -0.01, 0.03, 0.0]):
+        p["propeller"][i]["z"] = z
+    return p
+
+
+class StepResult(object):
+    """What OracleBatch.step returns: obs / rew / done / fail as env_step computes them, except that rows of envs an
+    auto-reset replaced hold the reset observation and `final_obs` holds their terminal one (NaN elsewhere);
+    `pre_state` / `end_state` are the states before the step and after the integrator (before any reset)."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+class OracleBatch(object):
+    """The engine's batch semantics around env_step(mode="mix"): per-env step counters `ct`, episode counters `ep`,
+    and resets whose twelve draws come from the engine's counter-based generator (oracle/philox.py), keyed by
+    `rng_seed`, the global env index env_index_base + e and `ep`.
+
+    `subset` (local env indices) makes the batch follow only those envs of an n-env batch; step() still takes the
+    actions of all n envs.  Rules for `ep`: it starts at 0; reset() without noise and every auto-reset increment it and
+    then draw; reset(noise=...) leaves it alone.  A reset state follows the engine's typing: float32 init values and
+    noise scales, one float64 expression, one rounding to float32.
+    """
+
+    def __init__(self, n, task, dt, nt, params=None, healthy=1.0, targets=None, env2task=None, map_matrix=None,
+                 rng_seed=0, env_index_base=0, auto_reset=False, subset=None):
+        self.params = DEFAULT_PARAMS if params is None else params
+        self.cfg = make_cfg(self.params)
+        self.n, self.task, self.dt, self.nt, self.healthy = int(n), task, float(dt), int(nt), float(healthy)
+        self.idx = np.arange(self.n, dtype=np.int64) if subset is None else np.asarray(subset, dtype=np.int64)
+        self.genv = int(env_index_base) + self.idx
+        self.rng_seed, self.auto_reset = int(rng_seed), bool(auto_reset)
+        self.targets = None if targets is None else np.ascontiguousarray(targets, dtype=np.float32)
+        self.env2task = None if env2task is None else np.ascontiguousarray(np.asarray(env2task, np.int32)[self.idx])
+        self.map_matrix = map_matrix
+        self.z_off = 0.0 if task == "velocity_control" else 5.0
+        self.obs_dim = 19 if task == "velocity_control" else 16
+        m = self.idx.size
+        self.state, self.ct, self.ep = zero_state(m), np.zeros(m, np.int32), np.zeros(m, np.int64)
+        iv, iw = self.params["init_velocity"], self.params["init_angular_velocity"]
+        self._base = [np.array([iv[k] for k in "xyz"], np.float32), np.array([iw[k] for k in "xyz"], np.float32)]
+        self._scale = [np.float32(iv["noisy"]), np.float32(iw["noisy"])]
+
+    def reset_rows(self, u):
+        """[k,22] reset states for the draws u [k,12] (reset_env in quad.cu)."""
+        u = np.asarray(u, dtype=np.float64).reshape(-1, 12)
+        s = zero_state(u.shape[0])
+        for blk, (sign, mag) in enumerate([(0, 3), (6, 9)]):
+            sg = np.where(u[:, sign:sign + 3] > 0.5, 1.0, -1.0)
+            x = np.float64(self._base[blk]) + (np.float64(self._scale[blk]) * u[:, mag:mag + 3]) * sg
+            s[:, 3 + 3 * blk:6 + 3 * blk] = x.astype(np.float32)
+        return s
+
+    def reset_obs(self, rows):
+        """Observation of the freshly reset envs `rows` (bool mask or indices): R = I, p = 0."""
+        s = self.state[rows]
+        o = np.zeros((s.shape[0], self.obs_dim), np.float32)
+        o[:, 0:3] = s[:, 3:6]
+        o[:, 6:8] = np.float32(0.0) * np.float32(-9.8)
+        o[:, 8] = np.float32(-9.8)
+        o[:, 9:12] = s[:, 6:9]
+        o[:, 12] = -0.0
+        o[:, 15] = np.float32(self.z_off)
+        if self.task == "velocity_control":
+            t = np.minimum(self.ct[rows], self.nt - 1)
+            o[:, 16:19] = self.targets[self.env2task[rows], t]
+        return o
+
+    def _redraw(self, rows):
+        self.ep[rows] += 1
+        self.state[rows] = self.reset_rows(philox.quad_reset_draws(self.rng_seed, self.genv[rows], self.ep[rows]))
+
+    def reset(self, mask=None, noise=None):
+        """Quadrotor.reset of the envs in `mask` ([n] over the whole batch; None = all); `noise` [n,12] replays draws.
+        ct is left alone, as in the reference.  Returns the reset observation rows (NaN for envs left alone)."""
+        rows = np.ones(self.idx.size, bool) if mask is None else np.asarray(mask, bool)[self.idx]
+        if noise is None:
+            self._redraw(rows)
+        else:
+            self.state[rows] = self.reset_rows(np.asarray(noise, np.float64).reshape(self.n, 12)[self.idx][rows])
+        o = np.full((self.idx.size, self.obs_dim), np.nan, np.float32)
+        o[rows] = self.reset_obs(rows)
+        return o
+
+    def step(self, act):
+        """One engine step of the followed envs; act [n,4] for the whole batch."""
+        act = np.ascontiguousarray(np.asarray(act, np.float32).reshape(self.n, 4)[self.idx])
+        pre = self.state.copy()
+        set_map(self.map_matrix)
+        obs, rew, done, fail, _ = env_step(self.cfg, self.state, self.ct, act, self.task, self.dt, self.nt,
+                                           self.healthy, self.targets, self.env2task, mode="mix")
+        done = done.astype(bool)
+        end = self.state.copy()
+        final = np.full_like(obs, np.nan)
+        if self.auto_reset and done.any():
+            final[done] = obs[done]
+            self._redraw(done)
+            obs[done] = self.reset_obs(done)
+        return StepResult(obs=obs, rew=rew, done=done, fail=fail, final_obs=final, pre_state=pre, end_state=end)
 
 
 def rk4_step(cfg, state, act, dt, rk4_steps=1, mode="f64"):

@@ -72,7 +72,46 @@ for task, dt in (("hovering_control", 0.01), ("velocity_control", 0.005), ("no_c
             batch[t] = max(batch[t], group_rel_err(obs.cpu().numpy()[:, :16], o_ref[:, :16], OBS_GROUPS))
         env.close()
 batch = np.maximum.accumulate(batch)
-out = {"random_batch_vs_oracle_running_max": [float(x) for x in batch],"metric": "group_rel_err over obs[:16] (tests/util.py), GPU free run vs reference golden episodes",
+# ---- the same for test_path_matrix_vs_oracle, indexed by steps since an env's last reset: its batches exactly (sizes,
+# seeds, edge states, actions; every path computes the same bits, so the default kernel stands for all), observations
+# and terminal observations of the followed envs
+import tempfile  # noqa: E402
+import test_quadrotor_gpu as tq  # noqa: E402
+from util import group_rel_err_rows  # noqa: E402
+matrix = np.zeros(20)
+tmp = tempfile.mkdtemp()
+for n in (4099, 9473, tq._stream_size()):
+    for task, terrain in tq.MATRIX_TASKS:
+        for config in ("default", "general"):
+            for drawn in ((False, True) if n == 4099 else (False,)):
+                env, ob, rng = tq._matrix_batch(n, task, terrain, config, g["map_obst"], tmp)
+                rows, since = ob.idx, np.zeros(ob.idx.size, np.int64)
+                acts = [rng.uniform(-1.0, 16.0, (n, 4)).astype(np.float32) for _ in range(20)]
+                outs = []
+                if drawn:
+                    for t0 in (0, 10):
+                        o = env.rollout(10, act_seed=tq.MATRIX_ACT_SEED, want_actions=True)
+                        for t in range(10):
+                            acts[t0 + t] = o["act"][t].cpu().numpy()
+                            outs.append((o["obs"][t].cpu().numpy(), o["done"][t].cpu().numpy(), None))
+                for t in range(20):
+                    if not drawn:
+                        obs, _, done, _ = env.step(torch.as_tensor(acts[t]).cuda())
+                        outs.append((obs.cpu().numpy(), done.cpu().numpy(), env.final_observation.cpu().numpy()))
+                    r = ob.step(acts[t])
+                    o, d, f = outs[t]
+                    o, d = o[rows], d[rows].astype(bool)
+                    assert np.array_equal(d, r.done), (n, task, terrain, config, t)
+                    e = group_rel_err_rows(o[~d, :16], r.obs[~d, :16], OBS_GROUPS)
+                    np.maximum.at(matrix, since[~d], e)
+                    if f is not None:
+                        np.maximum.at(matrix, since[d], group_rel_err_rows(f[rows][d, :16], r.final_obs[d, :16],
+                                                                           OBS_GROUPS))
+                    since = np.where(d, 0, since + 1)
+                env.close()
+matrix = np.maximum.accumulate(matrix)
+out = {"random_batch_vs_oracle_running_max": [float(x) for x in batch],
+       "path_matrix_running_max": [float(x) for x in matrix], "metric": "group_rel_err over obs[:16] (tests/util.py), GPU free run vs reference golden episodes",
        "runs": RUNS, "curve_running_max": [float(x) for x in mono], "per_run_max": {k: float(max(v)) for k, v in per_run.items()},
        "per_run_len": {k: len(v) for k, v in per_run.items()}, "device": torch.cuda.get_device_name(0)}
 with open(os.path.join(HERE, "free_run_envelope.json"), "w") as f:
@@ -80,3 +119,4 @@ with open(os.path.join(HERE, "free_run_envelope.json"), "w") as f:
 print("steps", len(mono), "err@1,10,50,100,end:", [float(mono[min(i, len(mono) - 1)]) for i in (0, 9, 49, 99, len(mono) - 1)])
 print(out["per_run_max"])
 print("random batch vs oracle, err@1,5,10,20:", [float(batch[i]) for i in (0, 4, 9, 19)])
+print("path matrix, err by steps since reset:", [float(x) for x in matrix[:7]])

@@ -10,7 +10,8 @@ f32-vs-f64 drift at 7e-6 after 100 steps).
 import numpy as np
 import pytest
 
-from util import OBS_GROUPS, QUAD_MAP_RUNS, QUAD_RUNS, STATE_GROUPS, golden_run, group_rel_err, scalar_rel_err
+from util import (OBS_GROUPS, QUAD_MAP_RUNS, QUAD_RUNS, STATE_GROUPS, golden_run, group_rel_err, group_rel_err_rows,
+                  scalar_rel_err)
 
 pytestmark = pytest.mark.gpu
 
@@ -208,24 +209,19 @@ def test_benchmark_shape_vs_oracle(torch_mod):
 
 
 def test_general_config_path_vs_oracle(torch_mod, tmp_path):
-    """A config that leaves the specialised kernel (off-diagonal inertia, raised rotors, cg offset, CT2 != 0)."""
-    import copy
+    """A config that leaves the specialised kernel (off-diagonal inertia, raised rotors, cg offset, CT2 != 0), loaded
+    from a file."""
     import json
     torch = torch_mod
     from oracle import quad_oracle as qo
-    from metagym_b200.quadrotor import DEFAULT_SIMULATOR_CONF
-    conf = copy.deepcopy(DEFAULT_SIMULATOR_CONF)
-    conf["inertia"].update(xy=0.001, xz=-0.0005, yz=0.0007)
-    conf["gravity_center"] = {"x": 0.01, "y": -0.02, "z": 0.015}
-    conf["thrust"]["CT"][2] = "1.0e-3"
-    for i, z in enumerate([0.02, -0.01, 0.03, 0.0]):
-        conf["propeller"][i]["z"] = z
+    conf = qo.general_params()
     path = tmp_path / "conf.json"
     path.write_text(json.dumps(conf))
     cfg = qo.make_cfg(conf)
     n, dt, nt = 512, 0.01, 1000
     rng = np.random.RandomState(5)
     env = make_env(n, "hovering_control", dt=dt, nt=nt, simulator_conf=str(path))
+    assert env.step_kernel_name() == "quad_step_kernel<false>"
     noise = rng.random_sample((n, 12))
     env.reset(noise=noise)
     state = qo.reset_state(conf, noise)
@@ -420,8 +416,10 @@ def test_full_size_sharding_invariance_and_rollout(torch_mod):
 
 
 def test_full_size_hover_invariants(torch_mod):
-    """4096- and 65 536-env hovering batches: outputs finite, done <=> floor contact or time limit, determinism."""
+    """4096- and 65 536-env hovering batches: outputs finite, done <=> floor contact or time limit, determinism, and
+    the device-drawn actions equal the restated counter-based draws bit for bit."""
     torch = torch_mod
+    from oracle import philox
     for N in (4096, 65536):
         a = make_env(N, "hovering_control", nt=50, auto_reset=True, rng_seed=5)
         b = make_env(N, "hovering_control", nt=50, auto_reset=True, rng_seed=5)
@@ -431,7 +429,9 @@ def test_full_size_hover_invariants(torch_mod):
         rb = b.rollout(60, act_seed=9)
         assert torch.equal(ra["obs"], rb["obs"]) and torch.equal(ra["rew"], rb["rew"])
         assert torch.isfinite(ra["obs"]).all() and torch.isfinite(ra["rew"]).all()
-        assert float(ra["act"].min()) >= 0.1 and float(ra["act"].max()) <= 15.0
+        drawn = ra["act"].cpu().numpy()
+        for t in range(60):
+            assert np.array_equal(drawn[t], philox.quad_rollout_actions(9, np.arange(N), t, 0.1, 15.0)), t
         # every env hits the nt = 50 limit once (random actions do not reach the floor 5 m below in 0.5 s)
         assert int(ra["done"].sum()) >= N
         a.close()
@@ -439,67 +439,78 @@ def test_full_size_hover_invariants(torch_mod):
 
 
 def test_auto_reset_publishes_first_obs_and_final_obs(torch_mod):
+    """Every env ends its episode at once (nt = 3): the step returns the first observation of episode 2 and the state
+    holds its reset state, both bit for bit against the restated draws; final_observation holds the terminal one."""
     torch = torch_mod
+    from oracle import quad_oracle as qo
     n = 256
     env = make_env(n, "no_collision", nt=3, auto_reset=True, rng_seed=1)
-    env.reset()
-    act = torch.full((n, 4), 5.0, device="cuda")
+    ob = qo.OracleBatch(n, "no_collision", 0.01, 3, rng_seed=1, auto_reset=True)
+    assert np.array_equal(env.reset().cpu().numpy(), ob.reset())
+    act = np.full((n, 4), 5.0, np.float32)
     for t in range(3):
-        obs, rew, done, _ = env.step(act)
-    assert bool(done.all())
-    # after auto-reset: R = I, position 0 -> body position 0, z = 5, |v| <= 2*sqrt(3), episode counter restarted
-    o = obs.cpu().numpy()
-    assert np.all(o[:, 3:6] == 0) and np.all(o[:, 15] == 5.0) and np.all(np.abs(o[:, 0:3]) <= 2.0)
-    f = env.final_observation.cpu().numpy()
-    assert np.all(np.abs(f[:, 15] - 5.0) > 0) and np.isfinite(f).all()
+        obs, rew, done, _ = env.step(torch.as_tensor(act).cuda())
+        r = ob.step(act)
+        assert group_rel_err(obs.cpu().numpy(), r.obs, OBS_GROUPS) < 1e-5
+        assert scalar_rel_err(rew.cpu().numpy(), r.rew) < 1e-5
+    assert bool(done.all()) and r.done.all()
+    assert np.array_equal(obs.cpu().numpy(), r.obs)
+    assert group_rel_err(env.final_observation.cpu().numpy(), r.final_obs, OBS_GROUPS) < 1e-5
     st, ct = get_state(env)
-    assert np.all(ct == 0) and np.all(st[:, 0:3] == 0)
+    assert np.all(ct == 0) and np.array_equal(st, ob.state)
     env.close()
 
 
 def test_streaming_kernel_equals_tile_kernel(torch_mod, monkeypatch):
     """Multi-wave launches take the persistent TMA-pipelined kernel (quad_stream_kernel); it must reproduce the plain
-    step kernel bit for bit, ragged last tile and auto-reset included (400 037 envs = 3125 full tiles + 37)."""
+    step kernel bit for bit, ragged last tile and auto-reset included (400 037 envs = 3125 full tiles + 37), in both
+    SIMPLE instantiations (the default config, then the general one)."""
     torch = torch_mod
+    from oracle import quad_oracle as qo
     N = 400037
-    kw = dict(dt=0.005, nt=6, seed=list(range(16)), auto_reset=True, rng_seed=11)
-    a = make_env(N, "velocity_control", **kw)                  # streaming kernel (default for this size)
-    assert a.step_kernel_name().startswith("quad_stream_kernel")
-    monkeypatch.setenv("MGB_STREAM_KERNEL", "0")
-    b = make_env(N, "velocity_control", **kw)                  # plain kernel
-    monkeypatch.delenv("MGB_STREAM_KERNEL")
-    assert b.step_kernel_name().startswith("quad_step_kernel")
-    g = torch.Generator(device="cuda").manual_seed(2)
-    a.reset()
-    b.reset()
-    for t in range(9):
-        act = torch.rand((N, 4), device="cuda", generator=g) * 16.0 - 0.5
-        o1, r1, d1, _ = a.step(act)
-        o2, r2, d2, _ = b.step(act)
-        assert torch.equal(o1, o2) and torch.equal(r1, r2) and torch.equal(d1, d2), t
-        if a.final_observation is not None:
-            m = d1.bool()
-            assert torch.equal(a.final_observation[m], b.final_observation[m])
-    s1, s2 = a.state_dict(), b.state_dict()
-    assert torch.equal(s1["state"], s2["state"]) and torch.equal(s1["ct"], s2["ct"])
-    a.close()
-    b.close()
+    for config in ("default", "general"):
+        kw = dict(dt=0.005, nt=6, seed=list(range(16)), auto_reset=True, rng_seed=11,
+                  simulator_conf=qo.general_params() if config == "general" else None)
+        a = make_env(N, "velocity_control", **kw)              # streaming kernel (default for this size)
+        assert a.step_kernel_name() == "quad_stream_kernel" + _kernel_suffix(config)
+        monkeypatch.setenv("MGB_STREAM_KERNEL", "0")
+        b = make_env(N, "velocity_control", **kw)              # plain kernel
+        monkeypatch.delenv("MGB_STREAM_KERNEL")
+        assert b.step_kernel_name() == "quad_step_kernel" + _kernel_suffix(config)
+        g = torch.Generator(device="cuda").manual_seed(2)
+        a.reset()
+        b.reset()
+        for t in range(9):
+            act = torch.rand((N, 4), device="cuda", generator=g) * 16.0 - 0.5
+            o1, r1, d1, _ = a.step(act)
+            o2, r2, d2, _ = b.step(act)
+            assert torch.equal(o1, o2) and torch.equal(r1, r2) and torch.equal(d1, d2), (config, t)
+            if a.final_observation is not None:
+                m = d1.bool()
+                assert torch.equal(a.final_observation[m], b.final_observation[m])
+        s1, s2 = a.state_dict(), b.state_dict()
+        assert torch.equal(s1["state"], s2["state"]) and torch.equal(s1["ct"], s2["ct"])
+        a.close()
+        b.close()
 
 
-@pytest.mark.parametrize("N", [9473, 65536, 67001])
-def test_wide_kernel_equals_tile_kernel(torch_mod, monkeypatch, N):
+@pytest.mark.parametrize("N,config", [pytest.param(N, c, id=str(N) + ("" if c == "default" else "-general"))
+                                      for N in (9473, 65536, 67001) for c in ("default", "general")])
+def test_wide_kernel_equals_tile_kernel(torch_mod, monkeypatch, N, config):
     """Single-wave launches can take the one-CTA-per-SM kernel (quad_step_wide_kernel; MGB_WIDE_KERNEL=1 selects it for
     every single-wave size); it must reproduce the 64-thread tile kernel bit for bit (ragged sizes, auto-reset, terminal
     observations).  67001 is just under the one-wave limit of an H100 (132 SMs x 512 envs)."""
     torch = torch_mod
-    kw = dict(dt=0.005, nt=5, seed=list(range(8)), auto_reset=True, rng_seed=4)
+    from oracle import quad_oracle as qo
+    kw = dict(dt=0.005, nt=5, seed=list(range(8)), auto_reset=True, rng_seed=4,
+              simulator_conf=qo.general_params() if config == "general" else None)
     monkeypatch.setenv("MGB_WIDE_KERNEL", "1")
     a = make_env(N, "velocity_control", **kw)
-    assert a.step_kernel_name().startswith("quad_step_wide_kernel")
+    assert a.step_kernel_name() == "quad_step_wide_kernel" + _kernel_suffix(config)
     monkeypatch.setenv("MGB_WIDE_KERNEL", "0")
     b = make_env(N, "velocity_control", **kw)
     monkeypatch.delenv("MGB_WIDE_KERNEL")
-    assert b.step_kernel_name().startswith("quad_step_kernel")
+    assert b.step_kernel_name() == "quad_step_kernel" + _kernel_suffix(config)
     g = torch.Generator(device="cuda").manual_seed(5)
     a.reset()
     b.reset()
@@ -516,47 +527,77 @@ def test_wide_kernel_equals_tile_kernel(torch_mod, monkeypatch, N):
     b.close()
 
 
-@pytest.mark.parametrize("task,dt,rk4_steps", [("velocity_control", 0.005, 1), ("hovering_control", 0.01, 2)])
-def test_rk4_integrator_vs_restatement(torch_mod, task, dt, rk4_steps):
+@pytest.mark.parametrize("task,dt,rk4_steps,path,config", [
+    pytest.param(task, dt, k, path, c, id="%s-%s-%d" % (task, dt, k) + ("" if (path, c) == ("tile", "default") else
+                                                                        "-%s-%s" % (path, c)))
+    for task, dt, k in (("velocity_control", 0.005, 1), ("hovering_control", 0.01, 2))
+    for path in ("tile", "wide", "stream", "rollout") for c in ("default", "general")])
+def test_rk4_integrator_vs_restatement(torch_mod, monkeypatch, task, dt, rk4_steps, path, config):
     """integrator='rk4' (BASELINE config 3 wording; no reference counterpart, parity unpinned): the float32 kernel
-    follows the float64 RK4 restatement of the same continuous-time model to 1e-5 over 20 free-running steps."""
+    follows the float64 RK4 restatement of the same continuous-time model to 1e-5 over 20 free-running steps, on every
+    path that integrates (the tile, wide and streaming step kernels and the rollout kernel) in both SIMPLE
+    instantiations.  The packed kernel has no RK4: MGB_PACKED=1 falls back to a scalar kernel."""
     torch = torch_mod
     from oracle import quad_oracle as qo
-    cfg = qo.make_cfg()
-    n, nt = 2048, 1000
+    params = qo.general_params() if config == "general" else None
+    cfg = qo.make_cfg(params)
+    n = {"wide": 9473, "stream": _stream_size()}.get(path, 2048)
+    nt = 1000
     rng = np.random.RandomState(21)
-    env = make_env(n, task, dt=dt, nt=nt, seed=[0, 1], integrator="rk4", rk4_steps=rk4_steps)
+    kw = dict(dt=dt, nt=nt, seed=[0, 1], integrator="rk4", rk4_steps=rk4_steps, simulator_conf=params)
+    monkeypatch.setenv("MGB_WIDE_KERNEL", "1" if path == "wide" else "0")
+    env = make_env(n, task, **kw)
+    kname = {"wide": "quad_step_wide_kernel", "stream": "quad_stream_kernel"}.get(path, "quad_step_kernel")
+    assert env.step_kernel_name() == kname + _kernel_suffix(config)
+    if path == "tile":
+        monkeypatch.setenv("MGB_PACKED", "1")
+        packed = make_env(n, task, **kw)
+        assert packed.step_kernel_name() == "quad_step_kernel" + _kernel_suffix(config)
+        packed.close()
+    monkeypatch.delenv("MGB_PACKED", raising=False)
+    monkeypatch.delenv("MGB_WIDE_KERNEL")
+    rows = _stream_subset(n) if path == "stream" else np.arange(n)
     noise = rng.random_sample((n, 12))
     env.reset(noise=noise)
-    state = qo.reset_state(None, noise)
+    state = qo.reset_state(params, noise[rows])
+    acts = [rng.uniform(-1.0, 16.0, (n, 4)).astype(np.float32) for _ in range(20)]
+    if path == "rollout":
+        for t0 in range(0, 20, 5):
+            out = env.rollout(5, actions=torch.as_tensor(np.stack(acts[t0:t0 + 5])).cuda())
+            assert torch.isfinite(out["obs"]).all() and not bool(out["done"].any())
     for t in range(20):
-        act = rng.uniform(-1.0, 16.0, (n, 4)).astype(np.float32)
-        obs, rew, done, _ = env.step(torch.as_tensor(act).cuda())
-        qo.rk4_step(cfg, state, act, dt, rk4_steps, "f64")
-        assert torch.isfinite(obs).all() and not bool(done.any())
+        if path != "rollout":
+            obs, rew, done, _ = env.step(torch.as_tensor(acts[t]).cuda())
+            assert torch.isfinite(obs).all() and not bool(done.any())
+        qo.rk4_step(cfg, state, acts[t][rows], dt, rk4_steps, "f64")
     st, ct = get_state(env)
-    assert group_rel_err(st, state, STATE_GROUPS) < 2e-5
+    assert group_rel_err(st[rows], state, STATE_GROUPS) < 2e-5
     assert np.all(ct == 20)
     env.close()
 
 
-@pytest.mark.parametrize("task,dt", [("velocity_control", 0.005), ("hovering_control", 0.01), ("no_collision", 0.003)])
+@pytest.mark.parametrize("task,dt,config", [
+    pytest.param(task, dt, c, id="%s-%s" % (task, dt) + ("" if c == "default" else "-general"))
+    for task, dt in (("velocity_control", 0.005), ("hovering_control", 0.01), ("no_collision", 0.003))
+    for c in ("default", "general")])
 @pytest.mark.parametrize("N", [1, 63, 9473, 65536, 70001, 151001])
-def test_packed_kernel_equals_scalar_kernel(torch_mod, monkeypatch, N, task, dt):
+def test_packed_kernel_equals_scalar_kernel(torch_mod, monkeypatch, N, task, dt, config):
     """The packed variant (MGB_PACKED=1: two envs per thread as two scalar chains; quad_step2_kernel) must reproduce the scalar
     one-env-per-thread instantiation of the same code bit for bit: ragged and odd sizes, auto-reset, terminal
     observations, fail codes, every task, and substep counts that do (5, 10) and do not (3) take the unrolled loop.
     Actions outside [0.1, 15] exercise the clamp; the long horizon lets hovering envs crash and velocity envs time out.
     This is also the guard against the compiler contracting multiply-add pairs in either lane (quad_lanes.cuh)."""
     torch = torch_mod
-    kw = dict(dt=dt, nt=5, auto_reset=True, rng_seed=4)
+    from oracle import quad_oracle as qo
+    kw = dict(dt=dt, nt=5, auto_reset=True, rng_seed=4,
+              simulator_conf=qo.general_params() if config == "general" else None)
     if task == "velocity_control":
         kw["seed"] = list(range(8))
     monkeypatch.setenv("MGB_PACKED", "1")
     a = make_env(N, task, **kw)
     monkeypatch.delenv("MGB_PACKED")
     if N > 1:
-        assert a.step_kernel_name().startswith("quad_step2_kernel")
+        assert a.step_kernel_name() == "quad_step2_kernel" + _kernel_suffix(config)
     b = make_env(N, task, **kw)
     assert not b.step_kernel_name().startswith("quad_step2_kernel")
     g = torch.Generator(device="cuda").manual_seed(5)
@@ -708,4 +749,312 @@ def test_custom_simulator_config_vs_reference(torch_mod, name, tmp_path):
     assert scalar_rel_err(rew, r["rew"]) < RTOL_STEP
     assert np.array_equal(done, r["done"]) and np.array_equal(ct, r["post_ct"])
     assert not env.fail_code.cpu().numpy().any()
+    env.close()
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# Path matrix: every way the engine reaches its outputs, against the oracle batch, through auto-resets
+# ----------------------------------------------------------------------------------------------------------------
+MATRIX_SEED = 0x9E3779B97F4A7C15          # reset draws; both 32-bit halves non-zero
+MATRIX_ACT_SEED = 0xD1B54A32D192ED03      # device-drawn rollout actions
+MATRIX_TASKS = [("no_collision", "map"), ("hovering_control", "flat"), ("hovering_control", "map"),
+                ("velocity_control", "flat")]
+# path -> (step kernel a step of this batch launches, environment settings at creation)
+MATRIX_PATHS = {
+    "tile": ("quad_step_kernel", {}),
+    "wide": ("quad_step_wide_kernel", {"MGB_WIDE_KERNEL": "1"}),
+    "packed": ("quad_step2_kernel", {"MGB_PACKED": "1"}),
+    "stream": ("quad_stream_kernel", {}),
+    "rollout": ("quad_step_kernel", {}),
+    "rollout_drawn": ("quad_step_kernel", {}),
+    "host_copy": ("quad_step_kernel", {"MGB_HOST_ZEROCOPY": "0"}),
+    "host_zerocopy": ("quad_step_kernel", {}),
+    "host_zerocopy_stream": ("quad_stream_kernel", {}),
+    "host_hybrid": ("quad_step_kernel", {"MGB_HOST_ZEROCOPY": "2"}),
+}
+
+
+def _num_sms():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _stream_size():
+    """Just over the multi-wave threshold of the 64-env tile kernel: the persistent streaming kernel takes it, and the
+    last 128-env state tile is ragged (37 envs)."""
+    return _num_sms() * 32 * 64 + 37
+
+
+def _stream_subset(n):
+    """Envs the oracle follows in a streaming-size batch: the first and last two 128-env tiles and every 97th env."""
+    last = ((n + 127) // 128 - 2) * 128
+    return np.unique(np.concatenate([np.arange(256), np.arange(last, n), np.arange(0, n, 97)]))
+
+
+def _kernel_suffix(config):
+    return "<true>" if config == "default" else "<false>"
+
+
+def _make_edge_states(st, ct, rows, task, terrain, rng, nt):
+    """Some followed envs start next to a decision, each placed decisively on one side so that float32 error cannot
+    flip it: across the range / velocity / angular-velocity limits within the first substep or not, through the floor
+    or an obstacle cell's 1 m ceiling within the step or not.  Every env starts at a random ct."""
+    ct[:] = rng.randint(0, nt - 1, ct.size)
+    kinds = {0: ((999.999, 0, 0), (1.5, None, None), None),          # range: fails in substep 1
+             1: ((999.999, 0, 0), (-1.5, None, None), None),         # range: moves away
+             2: (None, (103.0, 0.0, 0.0), None),                     # |v|: 100.4 after substep 1 (drag 2.5 / substep)
+             3: (None, (99.9995, 0.0, 0.0), None),                   # |v|: drag pulls it below at once
+             4: (None, None, (999.99, 0.0, 0.0))}                    # |w|: angular drag overshoots past -1000
+    if task != "velocity_control":
+        if terrain == "map":
+            kinds[5] = ((-1.5, -1.5, -3.995), (None, None, -2.0), None)    # over obstacle cells, z 1.005 -> 0.985
+            kinds[6] = ((-1.5, -1.5, -3.5), (None, None, 0.0), None)       # over obstacle cells, z 1.5
+            kinds[7] = ((5.5, 0.0, -4.995), (None, None, -2.0), None)      # over free cells, z 0.005 -> below 0
+        else:
+            kinds[5] = ((0.0, 0.0, -4.995), (None, None, -2.0), None)      # z 0.005 -> below the floor
+            kinds[6] = ((0.0, 0.0, -4.9), (None, None, 0.5), None)         # z 0.1, rising
+    for k, (p, v, w) in kinds.items():
+        e = rows[k::17]
+        for off, vals in ((0, p), (3, v), (6, w)):
+            for j, x in enumerate(vals or ()):
+                if x is not None:
+                    st[e, off + j] = x
+
+
+def _done_flip_is_marginal(ob, r, i, gpu_fail):
+    """A done flag the GPU and the oracle disagree on is accepted only when the oracle's deciding quantity lies within
+    1e-5 (relative) of its threshold, where the float32 error of a free run can land it: |p|^2, |v|^2, |w|^2 for a
+    failure; for a collision min(z_old, z_new) against the floor, or, over an obstacle map, the altitudes and the
+    swept cell window against the integers where the collision rule changes."""
+    rel = 1e-5
+    pre, end = r.pre_state[i], r.end_state[i]
+    if r.fail[i] or gpu_fail:
+        c = ob.cfg
+        q = [(end[0:3] @ end[0:3], c.fail_r ** 2), (end[3:6] @ end[3:6], c.fail_v ** 2),
+             (end[6:9] @ end[6:9], c.fail_w ** 2)]
+        return any(abs(a / b - 1.0) <= rel for a, b in q)
+    if ob.task == "velocity_control":
+        return False                      # only ct == nt and a failure end its episodes
+    zo = np.float32(ob.z_off)
+    z = (np.float32(pre[2]) + zo, np.float32(end[2]) + zo)
+    if ob.map_matrix is None:
+        return abs(float(min(z))) <= rel * ob.z_off
+
+    def near_int(q):
+        return abs(q - round(q)) <= rel * max(1.0, abs(q))
+    ys, xs = np.nonzero(np.asarray(ob.map_matrix) == -1)
+    x = (pre[0] + xs[0], end[0] + xs[0])
+    y = (pre[1] + ys[0], end[1] + ys[0])
+    return any(near_int(float(q)) for q in (min(z), max(z), min(x), max(x), min(y), max(y)))
+
+
+def _matrix_batch(n, task, terrain, config, map_matrix, tmp_dir):
+    """The path matrix's batch, created under the caller's environment settings, and its oracle batch: episode 1 drawn
+    on the device and compared bit for bit with the restatement, then the edge states loaded.  Returns (env, oracle
+    batch, numpy RandomState for the actions)."""
+    import os
+    from oracle import quad_oracle as qo
+    params = qo.general_params() if config == "general" else None
+    vel = task == "velocity_control"
+    dt, nt = (0.005 if vel else 0.01), 7
+    base = 2 ** 32 - 50 if vel else 0
+    kw = dict(dt=dt, nt=nt, auto_reset=True, rng_seed=MATRIX_SEED, env_index_base=base, simulator_conf=params)
+    if vel:
+        kw["seed"] = list(range(5))
+    if terrain == "map":
+        kw["map_file"] = os.path.join(tmp_dir, "map.txt")
+        with open(kw["map_file"], "w") as f:
+            f.write("".join(" ".join(str(int(v)).zfill(2) for v in row) + "\n" for row in map_matrix))
+    env = make_env(n, task, **kw)
+    ob = qo.OracleBatch(n, task, dt, nt, params=params, map_matrix=map_matrix if terrain == "map" else None,
+                        rng_seed=MATRIX_SEED, env_index_base=base, auto_reset=True,
+                        subset=_stream_subset(n) if n > 100000 else None,
+                        targets=env.velocity_targets.cpu().numpy() if vel else None,
+                        env2task=env.env2task.cpu().numpy() if vel else None)
+    rows = ob.idx
+    assert np.array_equal(env.reset().cpu().numpy()[rows], ob.reset())
+    st, ct = get_state(env)
+    assert np.array_equal(st[rows], ob.state)
+    rng = np.random.RandomState(17)
+    st = st.astype(np.float32)
+    _make_edge_states(st, ct, rows, task, terrain, rng, nt)
+    set_state(env, st, ct)
+    ob.state[:] = st[rows]
+    ob.ct[:] = ct[rows]
+    return env, ob, rng
+
+
+@pytest.mark.parametrize("config", ["default", "general"])
+@pytest.mark.parametrize("task,terrain", MATRIX_TASKS)
+@pytest.mark.parametrize("path", list(MATRIX_PATHS))
+def test_path_matrix_vs_oracle(torch_mod, quad_golden, monkeypatch, tmp_path, path, task, terrain, config):
+    """Every path to the engine's outputs -- the tile, wide, packed and streaming step kernels, the rollout kernel with
+    given and device-drawn actions, the host entry point by copies, zero-copy and hybrid -- in both SIMPLE
+    instantiations, against the oracle batch (oracle.quad_oracle.OracleBatch) for 20 steps with nt = 7, so that every env
+    auto-resets at least twice.  Per step: done and fail codes exactly; obs and reward within 2x the error envelope
+    measured on these batches (tests/golden/measure_free_run_envelope.py), indexed by steps since the env's last reset; reset observations, and the state right after a reset, bit
+    for bit against the restated counter-based draws; terminal observations within the same envelope.  At the end the
+    whole followed state within 5e-5 and ct exactly."""
+    torch = torch_mod
+    from metagym_b200 import _lib
+    from oracle import philox
+    kname, env_vars = MATRIX_PATHS[path]
+    n = {"wide": 9473, "stream": _stream_size(), "host_zerocopy_stream": _stream_size()}.get(path, 4099)
+    for k, v in env_vars.items():
+        monkeypatch.setenv(k, v)
+    env, ob, rng = _matrix_batch(n, task, terrain, config, quad_golden["map_obst"], str(tmp_path))
+    for k in env_vars:
+        monkeypatch.delenv(k)
+    assert env.step_kernel_name() == kname + _kernel_suffix(config)
+    rows, vel, base = ob.idx, task == "velocity_control", int(ob.genv[0] - ob.idx[0])
+
+    curve = _envelope("path_matrix_running_max")
+    desync = np.zeros(rows.size, bool)     # envs whose done flag flipped in this launch: resynchronised after it
+    since = np.zeros(rows.size, np.int64)  # steps since the env's last reset
+    accepted = []
+
+    def check_step(t, act, obs, rew, done, fail=None, final=None):
+        ep_before = ob.ep.copy()
+        r = ob.step(act)
+        g_obs, g_rew, g_done = obs[rows], rew[rows].astype(np.float64), done[rows].astype(bool)
+        g_fail = fail[rows] if fail is not None else np.zeros(rows.size, np.int32)
+        live = ~desync
+        flip = live & (g_done != r.done)
+        for i in np.nonzero(flip)[0]:
+            assert _done_flip_is_marginal(ob, r, i, g_fail[i]), (t, int(rows[i]), bool(g_done[i]), int(g_fail[i]))
+            accepted.append((t, int(rows[i])))
+        desync[flip] = True
+        ok = live & ~flip
+        tol = np.maximum(2.0 * curve[np.minimum(since, len(curve) - 1)], 5e-7)
+        if fail is not None:
+            assert np.array_equal(g_fail[ok], r.fail[ok]), t
+        cont, fresh = ok & ~r.done, ok & r.done
+        err = group_rel_err_rows(g_obs[cont, :16], r.obs[cont, :16], OBS_GROUPS)
+        assert (err <= tol[cont]).all(), (t, float(err.max()), rows[cont][np.argmax(err - tol[cont])])
+        if vel:
+            assert np.array_equal(g_obs[ok, 16:], r.obs[ok, 16:]), t
+        rerr = np.abs(g_rew - r.rew) / np.maximum(np.abs(r.rew), 1.0)
+        assert (rerr[ok] <= np.maximum(tol[ok], 1e-5)).all(), (t, float(rerr[ok].max()))
+        assert np.array_equal(g_obs[fresh], r.obs[fresh]), t            # reset observations, bit for bit
+        if final is not None:
+            ferr = group_rel_err_rows(final[rows][fresh, :16], r.final_obs[fresh, :16], OBS_GROUPS)
+            assert (ferr <= tol[fresh]).all(), (t, float(ferr.max()) if ferr.size else 0.0)
+        ob.ep[desync] = ep_before[desync] + g_done[desync]                 # the GPU's episode count
+        since[:] = np.where(g_done, 0, since + 1)
+        return fresh
+
+    def sync(fresh):
+        """After a launch: envs reset by its last step hold the restated reset state bit for bit; envs whose done
+        flag flipped take the GPU's state."""
+        gs, gc = get_state(env)
+        gs, gc = gs[rows], gc[rows]
+        assert np.array_equal(gs[fresh], ob.state[fresh]) and np.array_equal(gc[fresh], ob.ct[fresh])
+        ob.state[desync] = gs[desync]
+        ob.ct[desync] = gc[desync]
+        desync[:] = False
+        return gs, gc
+
+    steps = 20
+    acts = [rng.uniform(-1.0, 16.0, (n, 4)).astype(np.float32) for _ in range(steps)]
+    if path in ("rollout", "rollout_drawn"):
+        T = 5 if path == "rollout" else 10
+        genv = base + np.arange(n)
+        for t0 in range(0, steps, T):
+            if path == "rollout":
+                out = env.rollout(T, actions=torch.as_tensor(np.stack(acts[t0:t0 + T])).cuda())
+            else:
+                out = env.rollout(T, act_seed=MATRIX_ACT_SEED, want_actions=True)
+                drawn = out["act"].cpu().numpy()
+                for t in range(T):                  # t_base continues across consecutive rollouts
+                    acts[t0 + t] = philox.quad_rollout_actions(MATRIX_ACT_SEED, genv, t0 + t, env._cfg.min_voltage,
+                                                               env._cfg.max_voltage)
+                    assert np.array_equal(drawn[t], acts[t0 + t]), t0 + t
+            o, r_, d = out["obs"].cpu().numpy(), out["rew"].cpu().numpy(), out["done"].cpu().numpy()
+            for t in range(T):
+                fresh = check_step(t0 + t, acts[t0 + t], o[t], r_[t], d[t])
+            gs, gc = sync(fresh)
+    elif path.startswith("host"):
+        D = env.obs_dim
+
+        def pinned(shape, dtype):
+            return torch.zeros(shape, dtype=dtype).pin_memory()
+        h_act, h_obs, h_rew = pinned((n, 4), torch.float32), pinned((n, D), torch.float32), pinned((n,), torch.float32)
+        h_done, h_fail, h_final = pinned((n,), torch.uint8), pinned((n,), torch.int32), pinned((n, D), torch.float32)
+        for t in range(steps):
+            h_act.numpy()[:] = acts[t]
+            _lib.check(env._lib.mgb_quad_step_host(env._h, h_act.data_ptr(), h_obs.data_ptr(), h_rew.data_ptr(),
+                                                   h_done.data_ptr(), h_fail.data_ptr(), h_final.data_ptr(),
+                                                   env._stream()))
+            fresh = check_step(t, acts[t], h_obs.numpy().copy(), h_rew.numpy().copy(), h_done.numpy().copy(),
+                               h_fail.numpy().copy(), h_final.numpy().copy())
+            gs, gc = sync(fresh)
+    else:
+        for t in range(steps):
+            obs, rew, done, _ = env.step(torch.as_tensor(acts[t]).cuda())
+            fresh = check_step(t, acts[t], obs.cpu().numpy(), rew.cpu().numpy(), done.cpu().numpy(),
+                               env.fail_code.cpu().numpy(), env.final_observation.cpu().numpy())
+            gs, gc = sync(fresh)
+    assert group_rel_err(gs, ob.state, STATE_GROUPS) < 5e-5
+    assert np.array_equal(gc, ob.ct)
+    assert (ob.ep >= 3).all()              # the first reset and at least two auto-resets
+    assert len(accepted) <= 3, accepted
+    env.close()
+
+
+def test_path_matrix_covers_every_step_kernel():
+    """The kernels the path matrix asserts: all four step kernels, each in both SIMPLE instantiations."""
+    names = {MATRIX_PATHS[p][0] + _kernel_suffix(c) for p in MATRIX_PATHS for c in ("default", "general")}
+    assert names == {k + s for k in ("quad_step_kernel", "quad_step_wide_kernel", "quad_step2_kernel",
+                                     "quad_stream_kernel") for s in ("<true>", "<false>")}
+
+
+@pytest.mark.parametrize("task", ["hovering_control", "velocity_control"])
+def test_masked_reset_vs_restatement(torch_mod, task):
+    """reset(mask): masked-in envs take the restated draws of episode ep + 1, bit for bit; masked-out envs keep their
+    state, ct and episode count, and their observation equals bit for bit the one their last step returned.
+    reset(noise=..., mask) replays the draws without advancing the episode count, which the draws of the next
+    auto-reset show."""
+    torch = torch_mod
+    from oracle import quad_oracle as qo
+    n, nt, dt, seed, base = 1000, 5, 0.01, 0xC0FFEE1234567, 77
+    kw = dict(dt=dt, nt=nt, auto_reset=True, rng_seed=seed, env_index_base=base)
+    if task == "velocity_control":
+        kw["seed"] = [0, 1, 2]
+    env = make_env(n, task, **kw)
+    vel = task == "velocity_control"
+    ob = qo.OracleBatch(n, task, dt, nt, rng_seed=seed, env_index_base=base, auto_reset=True,
+                        targets=env.velocity_targets.cpu().numpy() if vel else None,
+                        env2task=env.env2task.cpu().numpy() if vel else None)
+    assert np.array_equal(env.reset().cpu().numpy(), ob.reset())
+    rng = np.random.RandomState(4)
+    for _ in range(2):
+        act = rng.uniform(0.1, 15.0, (n, 4)).astype(np.float32)
+        obs, _, done, _ = env.step(torch.as_tensor(act).cuda())
+        ob.step(act)
+    assert not bool(done.any())
+    last_obs = obs.cpu().numpy().copy()
+    st0, ct0 = get_state(env)
+    ob.state[:], ob.ct[:] = st0, ct0                  # carry on from the GPU's state: only the resets are compared
+    mask = rng.random_sample(n) < 0.4
+    o = env.reset(mask=torch.as_tensor(mask)).cpu().numpy()
+    o_ref = ob.reset(mask=mask)
+    st, ct = get_state(env)
+    assert np.array_equal(o[mask], o_ref[mask]) and np.array_equal(st[mask], ob.state[mask])
+    assert np.array_equal(st[~mask], st0[~mask]) and np.array_equal(ct, ct0)
+    assert np.array_equal(o[~mask], last_obs[~mask])
+    mask2 = rng.random_sample(n) < 0.5
+    noise = rng.random_sample((n, 12))
+    o = env.reset(mask=torch.as_tensor(mask2), noise=noise).cpu().numpy()
+    o_ref = ob.reset(mask=mask2, noise=noise)
+    st, _ = get_state(env)
+    assert np.array_equal(o[mask2], o_ref[mask2]) and np.array_equal(st[mask2], ob.state[mask2])
+    # ct is 2 everywhere: the third step from here ends every episode, and the auto-reset draws with ep + 1
+    for t in range(nt - 2):
+        act = rng.uniform(0.1, 15.0, (n, 4)).astype(np.float32)
+        obs, _, done, _ = env.step(torch.as_tensor(act).cuda())
+        r = ob.step(act)
+        assert np.array_equal(done.cpu().numpy(), r.done), t
+    assert r.done.all() and np.array_equal(np.unique(ob.ep), [2, 3])
+    st, ct = get_state(env)
+    assert np.array_equal(obs.cpu().numpy(), r.obs) and np.array_equal(st, ob.state) and (ct == 0).all()
     env.close()

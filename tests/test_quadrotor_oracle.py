@@ -253,3 +253,42 @@ def test_numpy_port_with_custom_config(conf_golden, name, np_seed):
         obs, rew, done, _ = env.step(r["act"][i])
         assert np.array_equal(obs, r["obs"][i]) and float(rew) == r["rew"][i] and bool(done) == bool(r["done"][i])
         assert np.array_equal(env.st.as_row(), r["post_state"][i])
+
+
+@pytest.mark.parametrize("general", [False, True])
+def test_oracle_batch_reset_rules(general):
+    """OracleBatch: episode counters follow the engine's rules, a reset state is float32 and within 1e-7 (relative) of
+    reset_state()'s float64 expression, and a subset follows exactly the rows of the whole batch."""
+    from oracle import philox
+    params = qo.general_params() if general else None
+    seed, base, n = (0x0123456789 << 20) | 0xABCDE, 2 ** 32 - 3, 9
+    ob = qo.OracleBatch(n, "hovering_control", 0.01, 3, params=params, rng_seed=seed, env_index_base=base,
+                        auto_reset=True)
+    sub = qo.OracleBatch(n, "hovering_control", 0.01, 3, params=params, rng_seed=seed, env_index_base=base,
+                         auto_reset=True, subset=[1, 4, 8])
+    assert (ob.ep == 0).all()
+    o = ob.reset()
+    sub.reset()
+    u = philox.quad_reset_draws(seed, base + np.arange(n), np.ones(n, np.int64))
+    assert (ob.ep == 1).all() and np.array_equal(ob.state, ob.reset_rows(u))
+    assert np.array_equal(ob.state, ob.state.astype(np.float32).astype(np.float64))
+    ref = qo.reset_state(params, u)
+    assert (np.abs(ob.state - ref) <= 1e-7 * np.maximum(np.abs(ref), 1e-30)).all()
+    assert np.array_equal(o[:, 0:3], ob.state[:, 3:6]) and np.array_equal(o[:, 9:12], ob.state[:, 6:9])
+    assert (o[:, 3:6] == 0).all() and (o[:, 8] == np.float32(-9.8)).all() and (o[:, 15] == 5.0).all()
+    ob.reset(noise=np.full((n, 12), 0.25))
+    sub.reset(noise=np.full((n, 12), 0.25))
+    assert (ob.ep == 1).all()
+    mask = np.arange(n) % 2 == 0
+    ob.reset(mask=mask)
+    sub.reset(mask=mask)
+    assert np.array_equal(ob.ep, np.where(mask, 2, 1)) and np.array_equal(sub.ep, ob.ep[[1, 4, 8]])
+    # nt = 3 steps end every episode; the auto-reset draws with ep + 1
+    for _ in range(3):
+        r = ob.step(np.full((n, 4), 5.0, np.float32))
+        rs = sub.step(np.full((n, 4), 5.0, np.float32))
+    assert r.done.all() and np.isfinite(r.final_obs).all() and np.array_equal(rs.obs, r.obs[[1, 4, 8]])
+    assert np.array_equal(ob.ep, np.where(mask, 3, 2))
+    u = philox.quad_reset_draws(seed, base + np.arange(n), ob.ep)
+    assert np.array_equal(ob.state, ob.reset_rows(u)) and np.array_equal(sub.state, ob.state[[1, 4, 8]])
+    assert np.array_equal(r.obs, ob.reset_obs(np.ones(n, bool)))

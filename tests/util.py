@@ -29,6 +29,22 @@ def group_rel_err(a, ref, groups, floor=1e-3):
     return worst
 
 
+def group_rel_err_rows(a, ref, groups, floor=1e-3):
+    """group_rel_err of every row on its own: [n]."""
+    a = np.asarray(a, dtype=np.float64)
+    ref = np.asarray(ref, dtype=np.float64)
+    a = a.reshape(-1, a.shape[-1])
+    ref = ref.reshape(-1, ref.shape[-1])
+    worst = np.zeros(a.shape[0])
+    for grp in groups:
+        lo, hi = grp[0], grp[1]
+        gfloor = grp[2] if len(grp) > 2 else floor
+        scale = np.maximum(np.abs(ref[:, lo:hi]).max(axis=1, keepdims=True), gfloor)
+        worst = np.maximum(worst, (np.abs(a[:, lo:hi] - ref[:, lo:hi]) / scale).max(axis=1))
+        assert not np.isnan(a[:, lo:hi]).any()
+    return worst
+
+
 def scalar_rel_err(a, ref, floor=1.0):
     a = np.asarray(a, dtype=np.float64).reshape(-1)
     ref = np.asarray(ref, dtype=np.float64).reshape(-1)
