@@ -289,6 +289,14 @@ int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t ac
  * what the reference computes for float32 actions (its action_space.sample()): float32 position, float64 heading. */
 int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                              void *stream);
+/* MetaMazeContinuous3D: T consecutive mgb_maze_step_continuous calls (the random-action loop of metamaze/test.py:49-67)
+ * in ONE launch of the direct renderer; auto-reset semantics as configured, state left as T steps leave it.
+ *   act_dev [T][n][2] float32 or NULL: NULL draws turn_rate and walk_speed uniform on [-1, 1) from the counter-based
+ *   generator (seed act_seed, keyed by the global env index, counted across calls), written to act_out_dev [T][n][2]
+ *   if not NULL.  obs_dev [T][n][res_h][res_v][3] (uint8, int32 or float32), rew_dev [T][n] float64,
+ *   done_dev [T][n] uint8.  Refused while output mirrors are set.  Stream-ordered, no host synchronisation. */
+int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
+                                void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream);
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

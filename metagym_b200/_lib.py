@@ -92,6 +92,7 @@ SIGNATURES = {
     "mgb_maze_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
     "mgb_maze_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
     "mgb_maze_step_continuous": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_rollout_continuous": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

@@ -111,6 +111,8 @@ struct MazeArgs {
     int32_t *act_out;
     MgbMirrors mir;              // maze2d rollout: every output is also stored at ptr + mir.delta[i]
     int auto_reset;
+    float *act_out_c;            // continuous-maze rollout: drawn actions [T][n][2] (last, so the other kernels' parameter
+                                 // offsets do not move)
 };
 
 struct Env {
@@ -566,7 +568,11 @@ __device__ __forceinline__ size_t align_up(size_t x, size_t a) { return (x + a -
 //               before any transparency, the food slot under every floor/ceiling pixel, every POSSIBLE transparent
 //               crossing of every column.  maze3d_compose_kernel then turns a pose + the env's current food state
 //               into the exact observation with integer work only (the float64 geometry is memoised).
-template <bool FILL>
+// ROLL = true (FILL = false, continuous maze): T steps per launch.  A work item is (env, t), env-major: a CTA runs
+//               t = 0..T-1 of env blockIdx.x, then of env blockIdx.x + gridDim.x, ...; so the pipelined order prepares
+//               step t + 1 under the pixels of step t.  The pixel phase reads only its record set's snapshot (transparent
+//               map, pose, life-bar end), never the env state that the next item's step logic is rewriting.
+template <bool FILL, bool ROLL>
 __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_constant__ MazeConst c,
                                                                    const __grid_constant__ MazeArgs a)
 {
@@ -646,7 +652,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     // direct renderer -- the first kGeoThreads threads (named barrier 2) while every warp paints the previous env.
     // Tile buffer bb: loaded here (pipelined mode: the other buffer is being read by the pixel warps), or already requested by
     // the previous call, which prefetches `next_e` into the other buffer after its own wait (sequential mode).
-    auto geometry = [&](int64_t e, int b, int bb, int gt, int gn, bool named, bool load_here, int64_t next_e) {
+    auto geometry = [&](int64_t e, int t, int b, int bb, int gt, int gn, bool named, bool load_here, int64_t next_e) {
         auto gsync = [&]() { if (named) asm volatile("bar.sync 2, %0;" ::"n"(kGeoThreads) : "memory"); else __syncthreads(); };
         uint8_t *s_blob = (bb ? s_blob2[1] : s_blob2[0]);
         double *s_transp = (b ? s_transp2[1] : s_transp2[0]);
@@ -677,16 +683,29 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
             if (a.do_step) {
                 double reward;
                 int done;
+                const int64_t o = ROLL ? (int64_t)t * a.n + e : e;       // [T][n] outputs and actions of a rollout
                 if (cont) {
-                    continuous_move(c, s_blob, a.act_c[2 * e], a.act_c[2 * e + 1], cp, co);
+                    float tr, ws;
+                    if (ROLL && !a.act_c) {   // uniform on [-1, 1): 2 u - 1 is exact for every 24-bit u01
+                        const int64_t genv = a.env_base + e;
+                        const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
+                                                                     a.t_base + (uint32_t)t, MGB_STREAM_ACTION),
+                                                          make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32)));
+                        tr = 2.0f * mgb_u01(r.x) - 1.0f;
+                        ws = 2.0f * mgb_u01(r.y) - 1.0f;
+                        if (a.act_out_c) { a.act_out_c[2 * o] = tr; a.act_out_c[2 * o + 1] = ws; }
+                    } else {
+                        tr = a.act_c[2 * o]; ws = a.act_c[2 * o + 1];
+                    }
+                    continuous_move(c, s_blob, tr, ws, cp, co);
                     const float csf = (float)th->cell_size;                 // get_loc_grid, maze_base.py:199-202
                     s.gx = (int)(cp[0] / csf); s.gy = (int)(cp[1] / csf);
                     maze_evaluate(c, s_blob, eaten, a.n_pad, s, reward, done);
                 } else {
                     maze_logic(c, s_blob, eaten, a.n_pad, s, a.act[e], reward, done);
                 }
-                a.rew[e] = reward;
-                a.done[e] = (uint8_t)done;
+                a.rew[o] = reward;
+                a.done[o] = (uint8_t)done;
                 if (done && a.auto_reset) {
                     env_reset(c, s_blob, eaten, a.n_pad, s);
                     if (cont) {
@@ -1183,23 +1202,49 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     const int64_t stride = gridDim.x;
     int b = 0, bb = 0;
     if (!pipe && tid == 0 && (int64_t)blockIdx.x < a.n) load_blob(blockIdx.x, 0);
-    for (int64_t e_pix = pipe ? (int64_t)blockIdx.x - stride : (int64_t)blockIdx.x; e_pix < a.n; e_pix += stride) {
-        const int64_t e_geo = pipe ? e_pix + stride : e_pix;
-        if (e_geo < a.n && (!pipe || tid < kGeoThreads)) {
-            // sequential: the other tile buffer was last read before the barrier that closed the previous env: prefetch into it
-            geometry(e_geo, pipe ? b ^ 1 : 0, pipe ? b ^ 1 : bb, tid, pipe ? kGeoThreads : (int)blockDim.x, pipe, pipe,
-                     (!pipe && e_geo + stride < a.n) ? e_geo + stride : -1);
+    if (!ROLL) {
+        for (int64_t e_pix = pipe ? (int64_t)blockIdx.x - stride : (int64_t)blockIdx.x; e_pix < a.n; e_pix += stride) {
+            const int64_t e_geo = pipe ? e_pix + stride : e_pix;
+            if (e_geo < a.n && (!pipe || tid < kGeoThreads)) {
+                // sequential: the other tile buffer was last read before the barrier that closed the previous env: prefetch into it
+                geometry(e_geo, 0, pipe ? b ^ 1 : 0, pipe ? b ^ 1 : bb, tid, pipe ? kGeoThreads : (int)blockDim.x, pipe, pipe,
+                         (!pipe && e_geo + stride < a.n) ? e_geo + stride : -1);
+            }
+            if (!pipe) {
+                if (!tex_ready) { mgb_mbar_wait(&s_bar[0], 0); tex_ready = true; }
+                __syncthreads();
+            }
+            if (e_pix >= 0) {
+                if (FILL) fill_pixels(e_pix, bb);
+                else pixels(e_pix, pipe ? b : 0, pipe ? b : bb, pipe);
+            }
+            __syncthreads();   // the record set / tile just painted from is rewritten next
+            b ^= 1; bb ^= 1;   // pipelined: the set prepared in this trip is painted in the next one
         }
-        if (!pipe) {
-            if (!tex_ready) { mgb_mbar_wait(&s_bar[0], 0); tex_ready = true; }
+    } else {
+        // the same trips over items (env, t): geometry of item (e_geo, t_geo), pixels of item (e_pix, t_pix) into frame
+        // t_pix * n + e_pix -- the same item (sequential) or the one before it (pipelined; none on the first trip).  Every
+        // item reloads its env's tile, so the tile buffers alternate exactly as above.
+        int64_t e_geo = blockIdx.x, e_pix = pipe ? -1 : e_geo;
+        int t_geo = 0, t_pix = 0;
+        while (e_pix < a.n) {
+            const bool last_t = t_geo + 1 == a.T;
+            const int64_t e_next = last_t ? e_geo + stride : e_geo;
+            const int t_next = last_t ? 0 : t_geo + 1;
+            if (e_geo < a.n && (!pipe || tid < kGeoThreads)) {
+                geometry(e_geo, t_geo, pipe ? b ^ 1 : 0, pipe ? b ^ 1 : bb, tid, pipe ? kGeoThreads : (int)blockDim.x, pipe,
+                         pipe, (!pipe && e_next < a.n) ? e_next : -1);
+            }
+            if (!pipe) {
+                if (!tex_ready) { mgb_mbar_wait(&s_bar[0], 0); tex_ready = true; }
+                __syncthreads();
+            }
+            if (e_pix >= 0) pixels((int64_t)t_pix * a.n + e_pix, pipe ? b : 0, pipe ? b : bb, pipe);
             __syncthreads();
+            b ^= 1; bb ^= 1;
+            e_pix = pipe ? e_geo : e_next; t_pix = pipe ? t_geo : t_next;
+            e_geo = e_next; t_geo = t_next;
         }
-        if (e_pix >= 0) {
-            if (FILL) fill_pixels(e_pix, bb);
-            else pixels(e_pix, pipe ? b : 0, pipe ? b : bb, pipe);
-        }
-        __syncthreads();   // the record set / tile just painted from is rewritten next
-        b ^= 1; bb ^= 1;   // pipelined: the set prepared in this trip is painted in the next one
     }
     if (!tex_ready && tid == 0) mgb_mbar_wait(&s_bar[0], 0);   // never leave a TMA load in flight
     if ((tid & 31) == 0) mgb_bulk_wait_read<0>();   // smem must outlive the copies; the kernel boundary flushes the writes
@@ -1831,7 +1876,7 @@ struct mgb_maze {
     int auto_reset = 0;
     bool has_task = false, has_tex = false;
     size_t smem3d = 0;
-    int render_attr_set[2] = {0, 0};   // maze3d_kernel<false / true>: shared-memory opt-in raised by this handle
+    int render_attr_set[3] = {0, 0, 0};   // maze3d_kernel<false / true / rollout>: shared-memory opt-in raised by this handle
     int compose_ctas_per_sm = 0;       // occupancy of maze3d_compose_kernel (queried once per handle)
     int compose_persistent = -1;       // MGB_COMPOSE_PERSISTENT
     int num_sms = 0;
@@ -2651,7 +2696,7 @@ template <class F> static cudaError_t maze_allow_max_dynamic_smem(F *kernel)
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
 }
 
-template <bool FILL>
+template <bool FILL, bool ROLL = false>
 static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStream_t st)
 {
     MazeConst &c = h->c;
@@ -2688,12 +2733,13 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
     }
     // The opt-in limit is a property of the kernel on a device, shared by every handle: each handle raises it once to the
     // device maximum (the same value from every handle and thread, so there is no ordering to get wrong and no global state).
-    if (!h->render_attr_set[FILL ? 1 : 0]) {
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL>));
-        h->render_attr_set[FILL ? 1 : 0] = 1;
+    const int attr = ROLL ? 2 : (FILL ? 1 : 0);
+    if (!h->render_attr_set[attr]) {
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL>));
+        h->render_attr_set[attr] = 1;
     }
     h->smem3d = sm;
-    maze3d_kernel<FILL><<<grid, kRenderThreads, sm, st>>>(c, a2);
+    maze3d_kernel<FILL, ROLL><<<grid, kRenderThreads, sm, st>>>(c, a2);
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -3062,6 +3108,29 @@ extern "C" int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void 
     MazeArgs a = maze_args(h);
     a.act_c = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
     return launch_observe(h, a, (cudaStream_t)stream);
+}
+
+extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
+                                           float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                           void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_continuous");
+    MGB_REQUIRE(h, "null handle");
+    MGB_REQUIRE(T > 0, "T must be positive");
+    MGB_REQUIRE(obs_dev && rew_dev && done_dev, "null argument");
+    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_rollout_continuous needs a MGB_MAZE_CONTINUOUS_3D handle");
+    int rc = maze_ready(h);
+    if (rc) return rc;
+    MGB_REQUIRE(h->mir.count == 0, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    a.act_c = act_dev; a.act_out_c = act_out_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
+    rc = launch_render<false, true>(h, a, (unsigned)(h->n < h->num_sms ? h->n : h->num_sms), (cudaStream_t)stream);
+    if (rc) return rc;
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return MGB_OK;
 }
 
 __global__ void maze_pose_kernel(MazeArgs a, float *pos_out, double *ori_out)

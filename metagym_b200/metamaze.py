@@ -528,8 +528,6 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
         """T steps in one launch on the pose cache: obs [T,N,res_h,res_v,3] (uint8 or int32), rew, done, act as for
         BatchedMetaMaze2D.rollout."""
-        if self.KIND != 1:
-            raise NotImplementedError("fused rollout: MetaMaze2D and MetaMazeDiscrete3D")
         return self._rollout(T, actions, act_seed, want_actions, out)
 
     def cache_info(self):
@@ -580,6 +578,30 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
                                                       self._rew.data_ptr(), self._done.data_ptr(), self._stream()))
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done.view(torch.bool)), info
+
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
+        """T steps in one launch of the direct renderer (mgb_maze_rollout_continuous), exactly as T step() calls.
+        actions: anything reshapeable to [T,N,2] (turn_rate, walk_speed), clipped to [-1, 1] like step(); None draws them
+        on the device, uniform on [-1, 1) like action_space.sample().  Returns dict(obs [T,N,res_h,res_v,3] in the env's
+        obs dtype, rew [T,N] f64, done [T,N] u8, act [T,N,2] f32: the drawn actions when want_actions, else None)."""
+        if self.need_reset:
+            raise Exception("Must \"reset\" before doing any actions")
+        torch = self._torch
+        T, N, dev = int(T), self.num_envs, self.device
+        if out is None:
+            out = {"obs": torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev),
+                   "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
+                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
+                   "act": torch.empty((T, N, 2), dtype=torch.float32, device=dev)
+                   if want_actions and actions is None else None}
+        a = None
+        if actions is not None:
+            a = torch.as_tensor(actions, dtype=torch.float32, device=dev).reshape(T, N, 2).contiguous()
+        drawn = out.get("act") if a is None else None
+        _lib.check(self._lib.mgb_maze_rollout_continuous(self._h, T, _lib.ptr(a), int(act_seed), _lib.ptr(drawn),
+                                                         _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
+                                                         _lib.ptr(out.get("done")), self._stream()))
+        return out
 
     def pose(self):
         """-> (pos [N,2] float32 = _agent_loc, ori [N] float64 = _agent_ori)."""
