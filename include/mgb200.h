@@ -245,7 +245,8 @@ int mgb_maze_set_cache(mgb_maze *h, int enabled);
 
 /* Pose-cache statistics after the first reset/step (reporting only): out[0] cached poses, out[1] extra variant frames,
  * out[2] variant bits in use (poses whose image depends on k <= bits foods have all 2^k finished frames), out[3] bytes,
- * out[4..12] poses by k (0..7, and 8 = eight or more), out[13] 1 if the cache is in use. */
+ * out[4..12] poses by k (0..7, and 8 = eight or more), out[13] 1 if the cache is in use; shared-memory plan of the last
+ * direct-renderer launch: out[14] 1 if the crossing lists live in a global scratch, out[15] 1 if pipelined. */
 int mgb_maze_cache_info(const mgb_maze *h, int64_t out[16]);
 
 /* Per-episode task resampling (MazeBase.set_task on a fresh TaskConfig every episode, maze_base.py:19-38, at the scale of
@@ -271,6 +272,18 @@ int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_dev, void *st
  * observation of the next episode. */
 int mgb_maze_step(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                   void *stream);
+/* mgb_maze_step with two optional outputs (NULL: not produced; both NULL is exactly mgb_maze_step):
+ *   final_obs_dev [n][obs of one env] in the obs dtype: for every env with done = 1 in this step, the observation an
+ *     auto_reset-off handle would have returned (the terminal frame, life bar included).  Rows of envs that did not
+ *     finish are left untouched.  Needs auto_reset on (MGB_ERR_ARG otherwise).
+ *   truncated_dev [n] uint8, written for every env: 1 iff done and the episode ended only through the step limit
+ *     (SURVIVAL: life >= 0; ESCAPE: not on the goal; steps > max_steps - 1), so terminated = done && !truncated.
+ * obs, rew, done and the env state are bit for bit what mgb_maze_step gives.  The fused uint8 step (pose cache) moves the
+ * terminal frames in the same launch (final_obs 16-byte aligned; otherwise the two-kernel path runs); the other 3-D paths
+ * render them in one more launch, one frame per finished env.  Stream-ordered, no host synchronisation, capturable in a
+ * CUDA graph. */
+int mgb_maze_step_ex(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                     void *final_obs_dev, uint8_t *truncated_dev, void *stream);
 int mgb_maze_set_options(mgb_maze *h, int auto_reset);
 
 /* MetaMaze2D and MetaMazeDiscrete3D: T consecutive step() calls (maze_env.py:59-75,189-206; the random-action loops of
@@ -289,6 +302,9 @@ int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t ac
  * what the reference computes for float32 actions (its action_space.sample()): float32 position, float64 heading. */
 int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                              void *stream);
+/* mgb_maze_step_continuous with the final_obs_dev and truncated_dev outputs of mgb_maze_step_ex. */
+int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                void *final_obs_dev, uint8_t *truncated_dev, void *stream);
 /* MetaMazeContinuous3D: T consecutive mgb_maze_step_continuous calls (the random-action loop of metamaze/test.py:49-67)
  * in ONE launch of the direct renderer; auto-reset semantics as configured, state left as T steps leave it.
  *   act_dev [T][n][2] float32 or NULL: NULL draws turn_rate and walk_speed uniform on [-1, 1) from the counter-based

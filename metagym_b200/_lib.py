@@ -78,6 +78,7 @@ SIGNATURES = {
     "mgb_maze_update_tasks": (ctypes.c_int, [vp, c_i32, vp, vp, vp, vp, vp, ctypes.POINTER(MazeTaskScalars), vp]),
     "mgb_maze_reset": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_step": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_step_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_set_options": (ctypes.c_int, [vp, ctypes.c_int]),
     "mgb_peer_alloc": (ctypes.c_int, [ctypes.c_int, c_u64, ctypes.POINTER(ctypes.c_void_p)]),
     "mgb_peer_free": (ctypes.c_int, [ctypes.c_int, vp]),
@@ -92,6 +93,7 @@ SIGNATURES = {
     "mgb_maze_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
     "mgb_maze_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
     "mgb_maze_step_continuous": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_step_continuous_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_rollout_continuous": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),

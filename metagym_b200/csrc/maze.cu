@@ -113,6 +113,19 @@ struct MazeArgs {
     int auto_reset;
     float *act_out_c;            // continuous-maze rollout: drawn actions [T][n][2] (last, so the other kernels' parameter
                                  // offsets do not move)
+    // terminal observations of auto-reset steps (mgb_maze_step_ex).  The step logic of a finished env appends its terminal
+    // state to a compact list before env_reset; a second pass renders the list into final_obs[fin_env[i]].
+    uint8_t *truncated;          // [n] 1: done only through the step limit; nullptr: not produced
+    void *final_obs;             // 2-D: [n][2g+1][2g+1] float32, written by the step kernel itself; 3-D: set on the list pass
+    int32_t *fin_count;          // [1] list length (zeroed before the step); nullptr: no list
+    int32_t *fin_env;            // [n] env of list entry i
+    void *fin_dyn;               // pose cache: [n] EnvDyn of the terminal state
+    int4 *fin_agent;             // direct renderer: terminal gx, gy, ori, steps ...
+    double *fin_life;            // ... life
+    int32_t *fin_eaten;          // ... food stamps [f_max][n_pad]
+    int32_t *fin_task;           // ... task slot
+    float2 *fin_cpos;            // ... continuous position
+    double *fin_cori;            // ... continuous heading
 };
 
 struct Env {
@@ -190,6 +203,16 @@ __device__ __forceinline__ void env_reset(const MazeConst &c, const uint8_t *blo
     e.gx = th->start[0]; e.gy = th->start[1]; e.ori = 0; e.steps = 0;
     e.life = th->initial_life;
     for (int f = 0; f < c.f_max; ++f) eaten[f * estride] = kNever;
+}
+
+// the episode that just ended (done) ended only through the step limit: SURVIVAL alive, ESCAPE off the goal (maze_base.py:80,
+// 91-95, 191-192).  Evaluated on the state evaluation_rule left, before any reset.
+__device__ __forceinline__ uint8_t maze_truncated(const MazeConst &c, const uint8_t *blob, const Env &e)
+{
+    const TaskHdr *th = blob_hdr(blob);
+    const bool over = e.steps > c.max_steps - 1;
+    const bool terminal = c.task_type == MGB_MAZE_SURVIVAL ? e.life < 0.0 : (e.gx == th->goal[0] && e.gy == th->goal[1]);
+    return (uint8_t)(over && !terminal);
 }
 
 // current transparent value of cell (i, j): SURVIVAL = remaining food (alias at maze_base.py:57), ESCAPE = goal one-hot
@@ -335,34 +358,38 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_kernel(const __grid_constan
         const int4 ag = a.agent[e];
         Env s = {ag.x, ag.y, ag.z, ag.w, a.life[e]};
         int32_t *eaten = a.eaten + e;
+        // update_observation, maze_2d.py:89-121
+        auto observe = [&](float *row) {
+            const int8_t *walls = reinterpret_cast<const int8_t *>(blob + c.off_walls);
+            const int n = c.n, g = c.view_grid;
+            for (int p = 0; p < W; ++p)
+                for (int q = 0; q < W; ++q) {
+                    const int x = s.gx - g + p, y = s.gy - g + q;
+                    float v = -1.0f;
+                    if (x >= 0 && x < n && y >= 0 && y < n) {
+                        v = (float)(-(int)walls[x * n + y]);
+                        if (c.task_type == MGB_MAZE_SURVIVAL)
+                            v = (float)((double)v + food_now(c, blob, eaten, a.n_pad, s.steps, x * n + y));
+                        else
+                            v = (float)((double)v + ((x == th->goal[0] && y == th->goal[1]) ? 1.0 : 0.0));
+                    }
+                    row[p * W + q] = v;
+                }
+            if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
+        };
         if (a.do_step) {
             double reward;
             int done;
             maze_logic(c, blob, eaten, a.n_pad, s, a.act[e], reward, done);
             a.rew[e] = reward;
             a.done[e] = (uint8_t)done;
+            if (a.truncated) a.truncated[e] = maze_truncated(c, blob, s);
+            if (done && a.final_obs) observe(reinterpret_cast<float *>(a.final_obs) + e * D);   // the terminal window
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
             a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
             a.life[e] = s.life;
         }
-        // update_observation, maze_2d.py:89-121
-        const int8_t *walls = reinterpret_cast<const int8_t *>(blob + c.off_walls);
-        const int n = c.n, g = c.view_grid;
-        float *row = tile2d + threadIdx.x * D;
-        for (int p = 0; p < W; ++p)
-            for (int q = 0; q < W; ++q) {
-                const int x = s.gx - g + p, y = s.gy - g + q;
-                float v = -1.0f;
-                if (x >= 0 && x < n && y >= 0 && y < n) {
-                    v = (float)(-(int)walls[x * n + y]);
-                    if (c.task_type == MGB_MAZE_SURVIVAL)
-                        v = (float)((double)v + food_now(c, blob, eaten, a.n_pad, s.steps, x * n + y));
-                    else
-                        v = (float)((double)v + ((x == th->goal[0] && y == th->goal[1]) ? 1.0 : 0.0));
-                }
-                row[p * W + q] = v;
-            }
-        if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
+        observe(tile2d + threadIdx.x * D);
     }
     float *dst = reinterpret_cast<float *>(a.obs) + e0 * D;
     const uint32_t bytes = (uint32_t)rows * (uint32_t)D * 4u;
@@ -563,6 +590,20 @@ __device__ __forceinline__ void blend(int rgb[3], double tf)
 
 __device__ __forceinline__ size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Terminal state of a finished env for the direct renderer's list pass: everything geometry() reads of an env (pose, life,
+// food stamps, task).  Called before env_reset, which clears the stamps the terminal frame still shows.
+__device__ __forceinline__ void push_terminal_state(const MazeConst &c, const MazeArgs &a, int64_t e, const Env &s,
+                                                    const int32_t *eaten, float2 cp, double co)
+{
+    const int i = atomicAdd(a.fin_count, 1);
+    a.fin_env[i] = (int32_t)e;
+    a.fin_task[i] = a.env2task[e];
+    a.fin_agent[i] = make_int4(s.gx, s.gy, s.ori, s.steps);
+    a.fin_life[i] = s.life;
+    for (int f = 0; f < c.f_max; ++f) a.fin_eaten[f * a.n_pad + i] = eaten[f * a.n_pad];
+    if (c.kind == MGB_MAZE_CONTINUOUS_3D) { a.fin_cpos[i] = cp; a.fin_cori[i] = co; }
+}
+
 // FILL = false: render the observation of every env directly (step logic + ray cast + paint).
 // FILL = true : render the STATIC layers of every cached pose (task, cell, heading) once, at set_task time: colours
 //               before any transparency, the food slot under every floor/ceiling pixel, every POSSIBLE transparent
@@ -577,6 +618,10 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                                                                    const __grid_constant__ MazeArgs a)
 {
     extern __shared__ __align__(128) uint8_t smem[];
+    // list pass (final_obs set): items are the entries of the terminal list the step logic just wrote; a CTA without one
+    // leaves before it stages the textures
+    const int64_t n_items = !FILL && a.final_obs ? (int64_t)*a.fin_count : a.n;
+    if ((int64_t)blockIdx.x >= n_items) return;
     const int n = c.n, H = c.res_h, V = c.res_v, ts = c.ts;
     const int tex_words = (c.n_tex + 1) * ts * ts;
     // ---- shared memory carve-up (mirrors maze3d_smem_bytes on the host)
@@ -706,6 +751,8 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                 }
                 a.rew[o] = reward;
                 a.done[o] = (uint8_t)done;
+                if (a.truncated) a.truncated[o] = maze_truncated(c, s_blob, s);
+                if (done && a.fin_count) push_terminal_state(c, a, e, s, eaten, make_float2(cp[0], cp[1]), co);
                 if (done && a.auto_reset) {
                     env_reset(c, s_blob, eaten, a.n_pad, s);
                     if (cont) {
@@ -905,7 +952,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
         int lb_ey = trunc_i(c.lb_sy + c.lb_w);
         if (lb_ey > V) lb_ey = V;
         const bool has_bar = c.task_type == MGB_MAZE_SURVIVAL;
-        uint8_t *gobs = reinterpret_cast<uint8_t *>(a.obs) + (size_t)e * total_px * px_bytes;
+        uint8_t *gobs = reinterpret_cast<uint8_t *>(a.obs) + (size_t)(a.final_obs ? a.fin_env[e] : e) * total_px * px_bytes;
         const int lane = tid & 31, warp = tid >> 5, n_warps = blockDim.x >> 5;
         const double inv_cell = th->inv_cell, inv_t2c = th->inv_t2c;
         const bool cell_p2 = th->cell_pow2 != 0, t2c_p2 = th->t2c_pow2 != 0, text_p2 = c.text_pow2 != 0;
@@ -1201,14 +1248,14 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     const bool pipe = !FILL && c.pipe;
     const int64_t stride = gridDim.x;
     int b = 0, bb = 0;
-    if (!pipe && tid == 0 && (int64_t)blockIdx.x < a.n) load_blob(blockIdx.x, 0);
+    if (!pipe && tid == 0 && (int64_t)blockIdx.x < n_items) load_blob(blockIdx.x, 0);
     if (!ROLL) {
-        for (int64_t e_pix = pipe ? (int64_t)blockIdx.x - stride : (int64_t)blockIdx.x; e_pix < a.n; e_pix += stride) {
+        for (int64_t e_pix = pipe ? (int64_t)blockIdx.x - stride : (int64_t)blockIdx.x; e_pix < n_items; e_pix += stride) {
             const int64_t e_geo = pipe ? e_pix + stride : e_pix;
-            if (e_geo < a.n && (!pipe || tid < kGeoThreads)) {
+            if (e_geo < n_items && (!pipe || tid < kGeoThreads)) {
                 // sequential: the other tile buffer was last read before the barrier that closed the previous env: prefetch into it
                 geometry(e_geo, 0, pipe ? b ^ 1 : 0, pipe ? b ^ 1 : bb, tid, pipe ? kGeoThreads : (int)blockDim.x, pipe, pipe,
-                         (!pipe && e_geo + stride < a.n) ? e_geo + stride : -1);
+                         (!pipe && e_geo + stride < n_items) ? e_geo + stride : -1);
             }
             if (!pipe) {
                 if (!tex_ready) { mgb_mbar_wait(&s_bar[0], 0); tex_ready = true; }
@@ -1328,6 +1375,17 @@ __device__ __forceinline__ EnvDyn make_dyn(const MazeConst &c, const MazeArgs &a
     return d;
 }
 
+// a finished env's terminal state joins the list pass of mgb_maze_step_ex (before env_reset): the pose cache keeps its EnvDyn,
+// the direct renderer everything geometry() reads
+__device__ __forceinline__ void push_terminal(const MazeConst &c, const MazeArgs &a, int64_t e, int task, const uint8_t *blob,
+                                              const Env &s, const int32_t *eaten)
+{
+    if (!a.fin_dyn) { push_terminal_state(c, a, e, s, eaten, make_float2(0.0f, 0.0f), 0.0); return; }
+    const int i = atomicAdd(a.fin_count, 1);
+    a.fin_env[i] = (int32_t)e;
+    reinterpret_cast<EnvDyn *>(a.fin_dyn)[i] = make_dyn(c, a, blob, task, s, eaten);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Pose cache path: step logic (one thread per env) + compose (static pose layers x current food state -> observation)
 // ---------------------------------------------------------------------------------------------------------------
@@ -1350,6 +1408,8 @@ __global__ void maze3d_logic_kernel(const __grid_constant__ MazeConst c, const _
         maze_logic(c, blob, eaten, a.n_pad, s, a.act[e], reward, done);
         a.rew[e] = reward;
         a.done[e] = (uint8_t)done;
+        if (a.truncated) a.truncated[e] = maze_truncated(c, blob, s);
+        if (done && a.fin_count) push_terminal(c, a, e, task, blob, s, eaten);
         if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
@@ -1426,7 +1486,8 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
     if (lb_ey > V) lb_ey = V;
     const int px_bytes = c.obs_dtype == MGB_OBS_U8 ? 3 : 12;
     const int part_px = ((total_px / kParts) + 127) / 128 * 128;          // slice boundaries stay 128-pixel aligned
-  const int64_t n_items = a.n * kParts;
+  // list pass of mgb_maze_step_ex (final_obs set): item = (terminal list entry, slice), frame into final_obs[fin_env[entry]]
+  const int64_t n_items = (a.final_obs ? (int64_t)*a.fin_count : a.n) * kParts;
   // bake mode (pose-cache build): item = pose slot, every food present, no life bar, tintable groups only
   auto fetch = [&](int64_t idx) -> EnvDyn {
       if (!a.bake) return reinterpret_cast<const EnvDyn *>(a.dyn)[idx];
@@ -1442,8 +1503,9 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
   EnvDyn d_next;
   if ((int64_t)blockIdx.x < n_items) d_next = fetch(blockIdx.x / kParts);
   for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
-    const int64_t e = item / kParts;
-    const int part = (int)(item - e * kParts);
+    const int64_t entry = item / kParts;
+    const int part = (int)(item - entry * kParts);
+    const int64_t e = a.final_obs ? (int64_t)a.fin_env[entry] : entry;
     const int q_begin = part * part_px, q_end = (part + 1) * part_px < total_px ? (part + 1) * part_px : total_px;
     // software pipeline: the next item's EnvDyn (-> pose slot -> every address below) is requested now, so the
     // dependent-load bubble at the start of an item overlaps this item's pixels
@@ -1548,8 +1610,13 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
     // The frame move is HBM-bound (every frame is read once and written once), so the step costs launch gap + logic + the
     // time HBM needs to move the frames.
     extern __shared__ __align__(128) uint8_t s_ring[];           // kStepSlots x 12 KB
-    __shared__ EnvDyn s_dyn[kStepBatch];
-    __shared__ const uint8_t *s_src[kStepBatch];                 // finished frame each env's observation starts from
+    // frames of a pass: [0, B) the pass's observations; [B, B + terminal count) with final_obs, the terminal frames of the
+    // pass's finished envs (their EnvDyn taken before env_reset), moved through the same ring into final_obs
+    __shared__ EnvDyn s_dyn[2 * kStepBatch];
+    __shared__ const uint8_t *s_src[2 * kStepBatch];             // finished frame each observation starts from
+    __shared__ uint8_t *s_dst[2 * kStepBatch];                   // where a terminal frame goes
+    __shared__ int s_nterm[2];                                   // terminal frames of the pass; by pass parity, so that
+                                                                 // the next pass's count is cleared while this one is read
     __shared__ __align__(8) uint64_t s_bar[kStepSlots];
     __shared__ __align__(8) uint64_t s_empty[kStepSlots];
     __shared__ int s_nslow;
@@ -1569,14 +1636,15 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
         for (int k = 0; k < kStepSlots; ++k) { mgb_mbar_init(&s_bar[k], 1); mgb_mbar_init(&s_empty[k], 1); }
         mgb_fence_mbar_init();
         s_nslow = 0;
+        s_nterm[0] = s_nterm[1] = 0;
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
     __syncthreads();
     uint32_t g0 = 0;                                             // chunks this CTA has moved in earlier passes (ring position)
-    for (int64_t base = blockIdx.x; base < a.n; base += (int64_t)gridDim.x * kStepBatch) {
+    int pass = 0;
+    for (int64_t base = blockIdx.x; base < a.n; base += (int64_t)gridDim.x * kStepBatch, ++pass) {
         const int64_t left = (a.n - base + gridDim.x - 1) / gridDim.x;
         const int B = (int)(left < kStepBatch ? left : kStepBatch);
-        const int M = B * n_chunks;                               // chunks of this pass
         // ---- (1) step logic of the pass's envs, one thread each (what maze3d_logic_kernel does for the two-kernel path)
         if (tid < B) {
             const int64_t e = base + (int64_t)tid * gridDim.x;
@@ -1591,6 +1659,14 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
                 maze_logic(c, blob, eaten, a.n_pad, s, a.act[e], reward, done);
                 a.rew[e] = reward;
                 a.done[e] = (uint8_t)done;
+                if (a.truncated) a.truncated[e] = maze_truncated(c, blob, s);
+                if (done && a.final_obs) {                        // the terminal state still has its food stamps
+                    const EnvDyn td = make_dyn(c, a, blob, task, s, eaten);
+                    const int j = B + atomicAdd(&s_nterm[pass & 1], 1);
+                    s_dyn[j] = td;
+                    s_src[j] = frame_of(a, td, frame_bytes);
+                    s_dst[j] = reinterpret_cast<uint8_t *>(a.final_obs) + (size_t)e * frame_bytes;
+                }
                 if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
                 a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
                 a.life[e] = s.life;
@@ -1600,6 +1676,9 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
             s_src[tid] = frame_of(a, dd, frame_bytes);
         }
         __syncthreads();
+        const int J = a.final_obs ? B + s_nterm[pass & 1] : B;    // frames of this pass
+        const int M = J * n_chunks;                               // chunks of this pass
+        if (a.final_obs && tid == 0) s_nterm[(pass + 1) & 1] = 0;  // last read in the previous pass, before its closing barrier
         const bool producer = (tid >> 5) == 1;
         const int t96 = tid < 32 ? tid : tid - 32;                 // index inside the consumer group (warps 0, 2, 3)
         if (producer) {
@@ -1618,12 +1697,12 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
                 }
             }
         } else {
-        for (int it = 0; it < B; ++it) {
+        for (int it = 0; it < J; ++it) {
             asm volatile("bar.sync 1, 96;" ::: "memory");          // frame boundary: nobody runs more than a frame ahead of warp 0
-            const int64_t e = base + (int64_t)it * gridDim.x;
             const EnvDyn d = s_dyn[it];
             const uint32_t miss_sig = (uint32_t)d.pad & 0xFFu;     // != 0: some groups need the float64 path (uniform)
-            uint8_t *gobs = reinterpret_cast<uint8_t *>(a.obs) + (size_t)e * frame_bytes;
+            uint8_t *gobs = it < B ? reinterpret_cast<uint8_t *>(a.obs) + (size_t)(base + (int64_t)it * gridDim.x) * frame_bytes
+                                   : s_dst[it];
             if (!warp0 && !miss_sig) continue;
             const uint8_t *blob = a.blobs + (int64_t)d.task * c.blob_bytes;
             const double *fval = reinterpret_cast<const double *>(blob + c.off_fval);
@@ -1884,6 +1963,13 @@ struct mgb_maze {
     uint32_t t_base = 0;
     MgbMirrors mir = {};         // mgb_maze_set_mirrors
     MgbMirrorWindow mir_win;     // mgb_maze_set_mirror_window
+    // terminal list of mgb_maze_step_ex (allocated by its first 3-D call with final_obs)
+    int32_t *fin_count = nullptr, *fin_env = nullptr, *fin_task = nullptr, *fin_eaten = nullptr;
+    EnvDyn *fin_dyn = nullptr;
+    int4 *fin_agent = nullptr;
+    double *fin_life = nullptr, *fin_cori = nullptr;
+    float2 *fin_cpos = nullptr;
+    bool list_pending = false;   // the last launch_observe left terminal states in the list
 };
 
 static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
@@ -2041,6 +2127,8 @@ extern "C" void mgb_maze_destroy(mgb_maze *h)
     cudaFree(h->c_px_all); cudaFree(h->c_fmask);
     cudaFree(h->c_vbase); cudaFree(h->c_var8); cudaFree(h->d_bake_desc); cudaFree(h->task_flags); cudaFree(h->task_epoch);
     cudaFree(h->pose_rec);
+    cudaFree(h->fin_count); cudaFree(h->fin_env); cudaFree(h->fin_task); cudaFree(h->fin_eaten); cudaFree(h->fin_dyn);
+    cudaFree(h->fin_agent); cudaFree(h->fin_life); cudaFree(h->fin_cori); cudaFree(h->fin_cpos);
     for (int i = 0; i < 2; ++i) {
         cudaFreeHost(h->h_stage[i]); cudaFree(h->d_stage[i]);
         if (h->stage_done[i]) cudaEventDestroy(h->stage_done[i]);
@@ -2074,6 +2162,8 @@ extern "C" int mgb_maze_cache_info(const mgb_maze *h, int64_t out[16])
     out[3] = (int64_t)h->cache_bytes;
     for (int k = 0; k < 9; ++k) out[4 + k] = h->k_hist[k];
     out[13] = h->cache_ready ? 1 : 0;
+    out[14] = h->c.hits_in_global;      // plan of the last direct-renderer launch: crossing lists in global scratch
+    out[15] = h->c.pipe;                // ... and geometry pipelined under the pixels
     return MGB_OK;
 }
 
@@ -2240,6 +2330,22 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     MGB_CUDA(cudaMalloc(&h->blobs, blobs.size()));
     MGB_CUDA(cudaMemcpy(h->blobs, blobs.data(), blobs.size(), cudaMemcpyHostToDevice));
     MGB_CUDA(cudaMalloc(&h->eaten, sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad));
+    if (c.kind != MGB_MAZE_2D) {     // terminal list of mgb_maze_step_ex, sized here so that its first call can be captured
+        cudaFree(h->fin_eaten); h->fin_eaten = nullptr;
+        MGB_CUDA(cudaMalloc(&h->fin_eaten, sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad));
+        if (!h->fin_count) {
+            MGB_CUDA(cudaMalloc(&h->fin_count, sizeof(int32_t)));
+            MGB_CUDA(cudaMalloc(&h->fin_env, sizeof(int32_t) * h->n));
+            MGB_CUDA(cudaMalloc(&h->fin_task, sizeof(int32_t) * h->n));
+            MGB_CUDA(cudaMalloc(&h->fin_dyn, sizeof(EnvDyn) * h->n));
+            MGB_CUDA(cudaMalloc(&h->fin_agent, sizeof(int4) * h->n));
+            MGB_CUDA(cudaMalloc(&h->fin_life, sizeof(double) * h->n));
+            if (c.kind == MGB_MAZE_CONTINUOUS_3D) {
+                MGB_CUDA(cudaMalloc(&h->fin_cpos, sizeof(float2) * h->n));
+                MGB_CUDA(cudaMalloc(&h->fin_cori, sizeof(double) * h->n));
+            }
+        }
+    }
     MGB_CUDA(cudaMemcpy(h->env2task, env2task_host, sizeof(int32_t) * h->n, cudaMemcpyHostToDevice));
     h->n_tasks = n_tasks;
     h->has_task = true;
@@ -2896,8 +3002,21 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     return MGB_OK;
 }
 
+// Paths other than the fused step keep their terminal states in a list (mgb_maze_step_ex): clear its length, and leave
+// a.final_obs to the list pass, which step_ex launches after the step.
+static int start_terminal_list(mgb_maze *h, MazeArgs &a, cudaStream_t st)
+{
+    h->list_pending = a.fin_count != nullptr;
+    a.final_obs = nullptr;
+    if (!a.fin_count) return MGB_OK;
+    MGB_CUDA(cudaMemsetAsync(a.fin_count, 0, sizeof(int32_t), st));
+    h->launches += 1;
+    return MGB_OK;
+}
+
 static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
 {
+    h->list_pending = false;
     const MazeConst &c = h->c;
     if (c.kind == MGB_MAZE_2D) {
         const int W = 2 * c.view_grid + 1;
@@ -2921,7 +3040,7 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
             const size_t frame_bytes = (size_t)c.res_h * c.res_v * 3;
             if (h->fused_step && c.obs_dtype == MGB_OBS_U8 && (c.res_v & 15) == 0 && ((size_t)c.res_h * c.res_v) % 128 == 0 &&
                 frame_bytes <= (size_t)64 * kStepChunkPx * 3 &&
-                (reinterpret_cast<uintptr_t>(a.obs) & 15u) == 0) {
+                ((reinterpret_cast<uintptr_t>(a.obs) | reinterpret_cast<uintptr_t>(a.final_obs)) & 15u) == 0) {
                 const size_t ring_bytes = (size_t)kStepSlots * kStepChunkPx * 3;       // 96 KB: two CTAs per SM
                 if (h->step_smem_set == 0) {
                     MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_step_kernel));
@@ -2939,11 +3058,13 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
                 attr[0].val.programmaticStreamSerializationAllowed = h->step_pdl ? 1 : 0;
                 cfg.attrs = attr;
                 cfg.numAttrs = 1;
-                MGB_CUDA(cudaLaunchKernelEx(&cfg, maze3d_step_kernel, c, a));
+                MGB_CUDA(cudaLaunchKernelEx(&cfg, maze3d_step_kernel, c, a));   // terminal frames in the same launch
                 MGB_CUDA(cudaGetLastError());
                 h->launches += 1;
                 return MGB_OK;
             }
+            rc = start_terminal_list(h, a, st);
+            if (rc) return rc;
             maze3d_logic_kernel<true><<<(unsigned)((h->n + 127) / 128), 128, 0, st>>>(c, a);
             MGB_CUDA(cudaGetLastError());
             {
@@ -2966,6 +3087,9 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
             }
             h->launches += 1;
         } else {
+            rc = start_terminal_list(h, a, st);
+            if (rc) return rc;
+            a.fin_dyn = nullptr;                                    // terminal list: full states for the direct renderer
             if (a.do_step && c.kind == MGB_MAZE_DISCRETE_3D) {     // logic for all envs in parallel, then render only
                 maze3d_logic_kernel<false><<<(unsigned)((h->n + 127) / 128), 128, 0, st>>>(c, a);
                 MGB_CUDA(cudaGetLastError());
@@ -2977,6 +3101,47 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
         }
     }
     MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
+// One step with the optional outputs of mgb_maze_step_ex (obs, rew, done and the state are exactly what they are without
+// them).  2-D: the step kernel writes the terminal windows itself.  Fused 3-D step: the terminal frames are extra frames of
+// the same launch.  Other 3-D paths: the step logic appends each finished env's terminal state to a list before resetting
+// it, then one more launch renders the list into final_obs: the compose kernel over the terminal EnvDyn records on the pose
+// cache, the direct renderer over the terminal states otherwise.  The list pass reads its length on the device; its grid
+// is fixed, and its work is one frame per finished env.
+static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated, cudaStream_t st)
+{
+    MGB_REQUIRE(!final_obs || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
+    a.truncated = truncated;
+    a.final_obs = final_obs;
+    if (!final_obs || h->c.kind == MGB_MAZE_2D) return launch_observe(h, a, st);
+    a.fin_count = h->fin_count; a.fin_env = h->fin_env; a.fin_dyn = h->fin_dyn;
+    a.fin_agent = h->fin_agent; a.fin_life = h->fin_life; a.fin_eaten = h->fin_eaten; a.fin_task = h->fin_task;
+    a.fin_cpos = h->fin_cpos; a.fin_cori = h->fin_cori;
+    int rc = launch_observe(h, a, st);
+    if (rc || !h->list_pending) return rc;
+    MazeArgs l = maze_args(h);
+    l.obs = final_obs; l.final_obs = final_obs; l.do_step = 0;
+    l.fin_count = h->fin_count; l.fin_env = h->fin_env;
+    if (h->cache_ready) {
+        l.dyn = h->fin_dyn;
+        l.do_parts = 16;     // a few frames per step: slices spread each over many CTAs, so the pass costs a slice, not a frame
+        int &ctas_per_sm = h->compose_ctas_per_sm;
+        if (!ctas_per_sm) {
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, maze3d_compose_kernel, kComposeThreads, 0) !=
+                    cudaSuccess || ctas_per_sm < 1) ctas_per_sm = 4;
+        }
+        const int64_t resident = (int64_t)h->num_sms * ctas_per_sm;
+        maze3d_compose_kernel<<<(unsigned)(h->n < resident ? h->n : resident), kComposeThreads, 0, st>>>(h->c, l);
+        MGB_CUDA(cudaGetLastError());
+    } else {
+        l.agent = h->fin_agent; l.life = h->fin_life; l.eaten = h->fin_eaten; l.env2task = h->fin_task;
+        l.cpos = h->fin_cpos; l.cori = h->fin_cori;
+        rc = launch_render<false>(h, l, (unsigned)(h->n < h->num_sms ? h->n : h->num_sms), st);
+        if (rc) return rc;
+    }
     h->launches += 1;
     return MGB_OK;
 }
@@ -3110,6 +3275,20 @@ extern "C" int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void 
     return launch_observe(h, a, (cudaStream_t)stream);
 }
 
+extern "C" int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev,
+                                           uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_step_continuous_ex");
+    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
+    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_step_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle");
+    int rc = maze_ready(h);
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    a.act_c = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
+}
+
 extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
                                            float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                                            void *stream)
@@ -3166,6 +3345,20 @@ extern "C" int mgb_maze_step(mgb_maze *h, const int32_t *act_dev, void *obs_dev,
     MazeArgs a = maze_args(h);
     a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
     return launch_observe(h, a, (cudaStream_t)stream);
+}
+
+extern "C" int mgb_maze_step_ex(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_step_ex");
+    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
+    MGB_REQUIRE(h->c.kind != MGB_MAZE_CONTINUOUS_3D, "use mgb_maze_step_continuous_ex for the continuous maze");
+    int rc = maze_ready(h);
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
 }
 
 extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev, void *stream)

@@ -197,9 +197,12 @@ def MazeTaskSampler(n=15, allow_loops=True, cell_size=2.0, wall_height=3.2, agen
 class _BatchedMazeBase(object):
     KIND = None
 
-    def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze):
+    def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs=False):
         import torch
         assert task_type in ("SURVIVAL", "ESCAPE")
+        if final_obs and not auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True (without auto-reset obs already is the terminal frame)")
+        self._want_final = bool(final_obs)
         self._torch = torch
         self.num_envs = int(num_envs)
         self.task_type = task_type
@@ -221,6 +224,27 @@ class _BatchedMazeBase(object):
         self._rew = torch.empty((self.num_envs,), dtype=torch.float64, device=self.device)
         self._done = torch.empty((self.num_envs,), dtype=torch.uint8, device=self.device)
         self._own_ptrs = None
+        self._final = self._trunc = None
+
+    def _alloc_final(self):
+        """Persistent final_obs / truncated buffers (final_obs=True), so that step() can be captured in a CUDA graph."""
+        if self._want_final:
+            self._final = self._torch.zeros_like(self._obs)
+            self._trunc = self._torch.zeros((self.num_envs,), dtype=self._torch.uint8, device=self.device)
+
+    @property
+    def final_observation(self):
+        """final_obs=True: [N, <obs of one env>] in the obs dtype.  After step(), row e holds the terminal observation
+        of env e if done[e] (what an auto_reset=False env would have returned; obs holds the next episode's first
+        frame).  Rows of envs that did not finish in that step are left untouched: they keep an earlier terminal frame
+        (zeros before the first).  None with final_obs=False."""
+        return None if self._final is None else self._out(self._final)
+
+    @property
+    def truncated(self):
+        """final_obs=True: [N] bool, written by every step(): True iff done and the episode ended only through the step
+        limit (max_steps), so terminated = done & ~truncated.  None with final_obs=False."""
+        return None if self._trunc is None else self._out(self._trunc.view(self._torch.bool))
 
     def _stream(self):
         return _lib.current_stream(self._torch, self.device)
@@ -376,7 +400,11 @@ class _BatchedMazeBase(object):
             self._own_ptrs = (self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr())
             self._done_bool = self._done.view(torch.bool)
         p = self._own_ptrs
-        rc = self._lib.mgb_maze_step(self._h, act.data_ptr(), p[0], p[1], p[2], self._stream())
+        if self._final is None:
+            rc = self._lib.mgb_maze_step(self._h, act.data_ptr(), p[0], p[1], p[2], self._stream())
+        else:
+            rc = self._lib.mgb_maze_step_ex(self._h, act.data_ptr(), p[0], p[1], p[2], self._final.data_ptr(),
+                                            self._trunc.data_ptr(), self._stream())
         if rc:
             _lib.check(rc)
         info = _LazySteps(self)
@@ -449,16 +477,17 @@ class BatchedMetaMaze2D(_BatchedMazeBase):
     KIND = 0
 
     def __init__(self, enable_render=False, render_scale=480, max_steps=5000, task_type="SURVIVAL", view_grid=2,
-                 num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True):
+                 num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True, final_obs=False):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
         self.view_grid = int(view_grid)
-        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze)
+        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs)
         w = 2 * self.view_grid + 1
         # the reference declares Box(-1, 1, (3,3), int32) but returns float32 (2g+1)^2 arrays (maze_2d.py:92)
         self.observation_space = Box(low=-1, high=1, shape=(w, w), dtype=np.float32)
         self._obs = self._torch.empty((self.num_envs, w, w), dtype=self._torch.float32, device=self.device)
+        self._alloc_final()
 
     def _make_cfg(self, n_cells):
         cfg = _lib.MazeCfg()
@@ -498,7 +527,8 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
 
     def __init__(self, enable_render=False, render_scale=480, resolution=(320, 320), max_steps=5000,
                  task_type="SURVIVAL", num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True,
-                 obs_dtype="int32", textures=None, max_vision_range=12.0, fol_angle=0.6 * PI, cache=None):
+                 obs_dtype="int32", textures=None, max_vision_range=12.0, fol_angle=0.6 * PI, cache=None,
+                 final_obs=False):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
@@ -508,12 +538,13 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         self.max_vision_range, self.fol_angle = max_vision_range, fol_angle
         self.cache = cache                  # None: library default (on, MGB_MAZE_CACHE); False: direct renderer only
         self.textures = textures if textures is not None else synthetic_textures(seed=0)
-        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze)
+        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs)
         torch = self._torch
         h, v = self.resolution
         self.observation_space = Box(low=0, high=256, shape=(h, v, 3), dtype=np.float32)     # maze_env.py:37-39
         self._obs = torch.empty((self.num_envs, h, v, 3), device=self.device,
                                 dtype={"int32": torch.int32, "uint8": torch.uint8, "float32": torch.float32}[obs_dtype])
+        self._alloc_final()
 
     def _make_cfg(self, n_cells):
         cfg = _lib.MazeCfg()
@@ -532,11 +563,13 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
 
     def cache_info(self):
         """Pose-cache statistics (valid after the first reset()/step()): dict(poses, variant_frames, variant_bits, bytes,
-        poses_by_food_count [k = 0..7, >= 8], in_use)."""
+        poses_by_food_count [k = 0..7, >= 8], in_use), and the shared-memory plan of the last direct-renderer launch
+        (hits_in_global: crossing lists in a global scratch; pipelined: geometry of the next env under the pixels)."""
         out = (ctypes.c_int64 * 16)()
         _lib.check(self._lib.mgb_maze_cache_info(self._h, out))
         return {"poses": int(out[0]), "variant_frames": int(out[1]), "variant_bits": int(out[2]), "bytes": int(out[3]),
-                "poses_by_food_count": [int(out[4 + k]) for k in range(9)], "in_use": bool(out[13])}
+                "poses_by_food_count": [int(out[4 + k]) for k in range(9)], "in_use": bool(out[13]),
+                "hits_in_global": bool(out[14]), "pipelined": bool(out[15])}
 
     def _after_create(self):
         if self.cache is not None:
@@ -574,8 +607,14 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         if not (hasattr(action, "is_cuda") and action.is_cuda):
             action = torch.as_tensor(np.asarray(action, dtype=np.float32).reshape(self.num_envs, 2), device=self.device)
         act = action.to(torch.float32).reshape(self.num_envs, 2).contiguous()
-        _lib.check(self._lib.mgb_maze_step_continuous(self._h, act.data_ptr(), self._obs.data_ptr(),
-                                                      self._rew.data_ptr(), self._done.data_ptr(), self._stream()))
+        if self._final is None:
+            _lib.check(self._lib.mgb_maze_step_continuous(self._h, act.data_ptr(), self._obs.data_ptr(),
+                                                          self._rew.data_ptr(), self._done.data_ptr(), self._stream()))
+        else:
+            _lib.check(self._lib.mgb_maze_step_continuous_ex(self._h, act.data_ptr(), self._obs.data_ptr(),
+                                                             self._rew.data_ptr(), self._done.data_ptr(),
+                                                             self._final.data_ptr(), self._trunc.data_ptr(),
+                                                             self._stream()))
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done.view(torch.bool)), info
 
