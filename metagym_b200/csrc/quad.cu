@@ -73,7 +73,8 @@ struct QuadArgs {
     uint8_t *done;
     int32_t *fail;
     float *final_obs;
-    const float *targets;      // [n_tasks][nt][3]
+    const float4 *targets;     // [nt][n_tasks] (x, y, z, 0): the handle's time-major copy (mgb_quad_set_targets)
+    int n_tasks;
     const int32_t *sat;        // obstacle map: summed-area table of non-zero cells [(rows+1)][(cols+1)], or null (flat)
     int map_rows, map_cols, x_off, y_off;
     const int32_t *env2task;   // [n]
@@ -609,19 +610,30 @@ __device__ __forceinline__ void philox_reset_draws(uint64_t seed, int64_t genv, 
     }
 }
 
-// Velocity-target rows an env needs this step, fetched BEFORE the integrator runs so the (dependent: env2task -> row)
-// L2 latency hides under the ~1000 arithmetic instructions of the substeps instead of stalling the epilogue.
+// Velocity-target rows an env needs this step.  The handle's table is time-major, [nt][n_tasks] float4 (x, y, z, 0), so
+// a row is ONE 16-byte load, and the lanes of a warp at the same ct (all envs of a batch that started together) read 32
+// consecutive rows: 512 contiguous bytes instead of 32 cache lines per component of the task-major [n_tasks][nt][3].
 template <class T> struct TargetRows {
     T cur[3];    // velocity_targets[ct - 1]         (env.py:153)
     T nxt[3];    // velocity_targets[min(ct, nt-1)]  (env.py:270-274)
 };
+__device__ __forceinline__ float4 target_row(const QuadArgs &a, int task, int t)
+{
+    return __ldg(a.targets + (int64_t)t * a.n_tasks + task);
+}
 template <class T>
-__device__ __forceinline__ void prefetch_targets(const QuadConst &c, const float *trow, int ct, int h, TargetRows<T> &tr)
+__device__ __forceinline__ void prefetch_targets(const QuadConst &c, const QuadArgs &a, int task, int ct, int h,
+                                                 TargetRows<T> &tr)
 {
     const int t = ct < c.nt - 1 ? ct : c.nt - 1;
-    const float *g = trow + 3 * (ct - 1), *q = trow + 3 * t;
-    set_lane(tr.cur[0], h, __ldg(g)); set_lane(tr.cur[1], h, __ldg(g + 1)); set_lane(tr.cur[2], h, __ldg(g + 2));
-    set_lane(tr.nxt[0], h, __ldg(q)); set_lane(tr.nxt[1], h, __ldg(q + 1)); set_lane(tr.nxt[2], h, __ldg(q + 2));
+    const float4 g = target_row(a, task, ct - 1), q = target_row(a, task, t);
+    set_lane(tr.cur[0], h, g.x); set_lane(tr.cur[1], h, g.y); set_lane(tr.cur[2], h, g.z);
+    set_lane(tr.nxt[0], h, q.x); set_lane(tr.nxt[1], h, q.y); set_lane(tr.nxt[2], h, q.z);
+}
+// env2task of env e (0 for the tasks without targets, whose handles have no env2task)
+__device__ __forceinline__ int env_task(const QuadConst &c, const QuadArgs &a, int64_t e)
+{
+    return c.task == MGB_TASK_VELOCITY_CONTROL ? __ldg(a.env2task + e) : 0;
 }
 
 // python slice bound for a[start:stop] on an axis of length len (negative indices wrap once, then clamp)
@@ -653,9 +665,9 @@ __device__ __forceinline__ bool map_collision(const QuadArgs &a, float x_old, fl
     return z_lo < any || z_hi < any;
 }
 
-// Observation of a freshly reset env (R = I): cheap closed form of observe().  Written into lane h of o[].
+// Observation of a freshly reset env (R = I) of task `task`: cheap closed form of observe().  Written into lane h of o[].
 template <class T>
-__device__ __forceinline__ void observe_reset(const QuadConst &c, const QuadArgs &a, int64_t e, const VState<T> &s, int h,
+__device__ __forceinline__ void observe_reset(const QuadConst &c, const QuadArgs &a, int task, const VState<T> &s, int h,
                                               T *o)
 {
     set_lane(o[0], h, lane(s.v[0], h)); set_lane(o[1], h, lane(s.v[1], h)); set_lane(o[2], h, lane(s.v[2], h));
@@ -665,10 +677,8 @@ __device__ __forceinline__ void observe_reset(const QuadConst &c, const QuadArgs
     set_lane(o[12], h, -0.f); set_lane(o[13], h, 0.f); set_lane(o[14], h, 0.f);   // arctan2(-0, 1) = -0 (:114-117 at R = I)
     set_lane(o[15], h, 0.f + c.z_off);
     if (c.task == MGB_TASK_VELOCITY_CONTROL) {
-        const float *trow = a.targets + ((int64_t)a.env2task[e] * c.nt) * 3;
-        const int t = s.ct[h] < c.nt - 1 ? s.ct[h] : c.nt - 1;
-        set_lane(o[16], h, __ldg(trow + 3 * t)); set_lane(o[17], h, __ldg(trow + 3 * t + 1));
-        set_lane(o[18], h, __ldg(trow + 3 * t + 2));
+        const float4 q = target_row(a, task, s.ct[h] < c.nt - 1 ? s.ct[h] : c.nt - 1);
+        set_lane(o[16], h, q.x); set_lane(o[17], h, q.y); set_lane(o[18], h, q.z);
     }
 }
 
@@ -785,9 +795,12 @@ __device__ __forceinline__ void publish_tile_mirrored(const MgbMirrors &m, float
 // One env.step() of Lanes<T>::N consecutive envs (e, e+1) on register state: integrate, task logic, state / reward /
 // done stores, observation rows into the CTA's shared-memory tile (trow = row of env e); frow receives the terminal
 // observation when auto-reset replaced it (bit h of final_mask).  nact = number of valid lanes (a ragged last pair has 1).
-template <bool SIMPLE, bool EARLY, class T>
+// task[h] = env2task of lane h (velocity_control only).  EARLY: the target rows are loaded before the integrator (else
+// after it); STATE_FIRST: for velocity_control the stepped state is stored before the observation work.
+template <bool SIMPLE, bool EARLY, bool STATE_FIRST, class T>
 __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a, int64_t e, int nact, VState<T> &s,
-                                          const T V[4], float *trow, float *frow, int &final_mask)
+                                          const T V[4], const int task[Lanes<T>::N], float *trow, float *frow,
+                                          int &final_mask)
 {
     constexpr int N = Lanes<T>::N;
     const int D = c.obs_dim;
@@ -803,10 +816,7 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
     const bool vel = c.task == MGB_TASK_VELOCITY_CONTROL;
     if (EARLY && vel) {
 #pragma unroll
-        for (int h = 0; h < N; ++h) {
-            const int64_t eh = h < nact ? e + h : e;
-            prefetch_targets(c, a.targets + ((int64_t)__ldg(a.env2task + eh) * c.nt) * 3, ct_now[h], h, tr);
-        }
+        for (int h = 0; h < N; ++h) prefetch_targets(c, a, task[h], ct_now[h], h, tr);
     }
     const T z_old = vadd(s.p[2], c.z_off);                  // env.py:131-133
     const T x_old = s.p[0], y_old = s.p[1];
@@ -849,15 +859,12 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
     }
     if (!EARLY && vel) {
 #pragma unroll
-        for (int h = 0; h < N; ++h) {
-            const int64_t eh = h < nact ? e + h : e;
-            prefetch_targets(c, a.targets + ((int64_t)__ldg(a.env2task + eh) * c.nt) * 3, ct_now[h], h, tr);
-        }
+        for (int h = 0; h < N; ++h) prefetch_targets(c, a, task[h], ct_now[h], h, tr);
     }
     // Velocity task, tile kernel: the state leaves before the observation and reward work, so that its stores drain
     // while that work runs instead of at the end of the step.  Its ct is final here (velocity_control has no collision
     // rule: only ct == nt and a failure end an episode, finish_step); an auto-reset rewrites the state below.
-    const bool state_first = N == 1 && !EARLY && vel;
+    const bool state_first = N == 1 && STATE_FIRST && vel;
     if (state_first) {
         QState s1;
         get_lane_state(s, 0, s1);
@@ -905,7 +912,7 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
                     if (D == 19) { fr_h[16] = lane(o[16], h); fr_h[17] = lane(o[17], h); fr_h[18] = lane(o[18], h); }
                     final_mask |= 1 << h;
                 }
-                observe_reset(c, a, e + h, s, h, o);
+                observe_reset(c, a, task[h], s, h, o);
             }
 #pragma unroll
             for (int k = 0; k < 16; ++k) tr_h[k] = lane(o[k], h);
@@ -931,10 +938,10 @@ __device__ __forceinline__ void publish_final(const QuadArgs &a, const float *ft
 }
 
 // Scalar step kernel, 64 envs per CTA (small batches, and batches between one wave of 512-thread CTAs and the streaming
-// regime).  The velocity-target rows are fetched after the integrator (step_body EARLY = false): fetched before it, their
-// six scattered 4-byte gathers per env meet every warp's state loads at the start of the step, and the 65 536-env step
-// measured 3 % slower that way on an H100.  For velocity_control the kernel also stores the stepped state right after
-// the integrator, before the observation work (step_body): 5 % faster together (DESIGN.md section 4).
+// regime).  env2task is read before the PDL wait and the two 16-byte target rows after the integrator (step_body EARLY =
+// false): issued before it, with env2task already in a register, they hold eight registers across the substeps, and the
+// 65 536-env step measured 1.5 % slower that way on an H100 (67 001 envs: 2 %).  For velocity_control the kernel also
+// stores the stepped state right after the integrator, before the observation work (step_body; DESIGN.md section 4).
 template <bool SIMPLE>
 __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_constant__ QuadConst c,
                                                              const __grid_constant__ QuadArgs a)
@@ -957,6 +964,8 @@ __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_consta
     // start before its own step k has stored its state, so the per-block latency chain -- not the grid barrier -- sets the
     // pace, and the register file holds barely more than one launch's worth of threads.  DESIGN.md section 4.)
     asm volatile("griddepcontrol.launch_dependents;");
+    // env2task is written only by mgb_quad_set_targets, which synchronises the device: it may be read before the wait
+    const int task[1] = {active ? env_task(c, a, e) : 0};
     asm volatile("griddepcontrol.wait;" ::: "memory");
 
     if (active) {
@@ -964,7 +973,8 @@ __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_consta
         load_state(a, e, s);
         const float4 act = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
         const float V[4] = {act.x, act.y, act.z, act.w};
-        step_body<SIMPLE, false, float>(c, a, e, 1, s, V, tile + threadIdx.x * D, ftile + threadIdx.x * D, final_mask);
+        step_body<SIMPLE, false, true, float>(c, a, e, 1, s, V, task, tile + threadIdx.x * D, ftile + threadIdx.x * D,
+                                              final_mask);
     }
     publish_tile(a.obs, tile, e0, rows, D);
     publish_final(a, ftile, e, threadIdx.x, 1, final_mask, D);
@@ -973,7 +983,8 @@ __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_consta
 
 // "One CTA per SM" variant for launches that fit a single wave (N <= SMs x 512): each CTA owns `per` = ceil(N / SMs)
 // envs rounded up to 4 (so that every observation tile stays 16-byte aligned for the bulk store), grid = ceil(N / per),
-// and the last CTA takes the remainder (49 152 envs on 132 SMs: 130 CTAs of 376 envs and one of 272).
+// and the last CTA takes the remainder (49 152 envs on 132 SMs: 130 CTAs of 376 envs and one of 272).  Target rows after
+// the integrator as in quad_step_kernel: before it, 24 576 envs measured 3 % and 49 152 envs 1 % slower.
 template <bool SIMPLE>
 __global__ void __launch_bounds__(512, 1) quad_step_wide_kernel(const __grid_constant__ QuadConst c,
                                                                 const __grid_constant__ QuadArgs a)
@@ -989,13 +1000,15 @@ __global__ void __launch_bounds__(512, 1) quad_step_wide_kernel(const __grid_con
     const bool active = (int)threadIdx.x < rows;
     int final_mask = 0;
     asm volatile("griddepcontrol.launch_dependents;");
+    const int task[1] = {active ? env_task(c, a, e) : 0};     // before the wait, as in quad_step_kernel
     asm volatile("griddepcontrol.wait;" ::: "memory");
     if (active) {
         QState s;
         load_state(a, e, s);
         const float4 act = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
         const float V[4] = {act.x, act.y, act.z, act.w};
-        step_body<SIMPLE, true, float>(c, a, e, 1, s, V, tile + threadIdx.x * D, ftile + threadIdx.x * D, final_mask);
+        step_body<SIMPLE, false, false, float>(c, a, e, 1, s, V, task, tile + threadIdx.x * D, ftile + threadIdx.x * D,
+                                               final_mask);
     }
     if (rows > 0) publish_tile(a.obs, tile, e0, rows, D);
     else __syncthreads();
@@ -1030,7 +1043,8 @@ __global__ void __launch_bounds__(256, 1) quad_step2_kernel(const __grid_constan
         const float4 a0 = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
         const float4 a1 = nact == 2 ? __ldg(reinterpret_cast<const float4 *>(a.act) + e + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
         const f2 V[4] = {pack2(a0.x, a1.x), pack2(a0.y, a1.y), pack2(a0.z, a1.z), pack2(a0.w, a1.w)};
-        step_body<SIMPLE, true, f2>(c, a, e, nact, s, V, tile + le * D, ftile + le * D, final_mask);
+        const int task[2] = {env_task(c, a, e), env_task(c, a, nact == 2 ? e + 1 : e)};
+        step_body<SIMPLE, true, false, f2>(c, a, e, nact, s, V, task, tile + le * D, ftile + le * D, final_mask);
     }
     if (rows > 0) publish_tile(a.obs, tile, e0, rows, D);
     else __syncthreads();
@@ -1099,7 +1113,8 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
             unpack_state(q, s);
             const float4 act = stage[st][6][tid];
             const float V[4] = {act.x, act.y, act.z, act.w};
-            step_body<SIMPLE, true, float>(c, a, e, 1, s, V, tile + tid * D, ftile + tid * D, final_mask);
+            const int task[1] = {env_task(c, a, e)};
+            step_body<SIMPLE, true, false, float>(c, a, e, 1, s, V, task, tile + tid * D, ftile + tid * D, final_mask);
         }
         publish_tile(a.obs, tile, e0, rows, D);
         publish_final(a, ftile, e, tid, 1, final_mask, D);
@@ -1110,7 +1125,8 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 
 // T env.step()s in one launch: the state never leaves registers; per step the kernel reads 16 B of action (or draws
 // it) and writes obs/reward/done.  Observation tiles are double-buffered so the bulk store of step t overlaps the
-// arithmetic of step t+1.
+// arithmetic of step t+1.  The target rows of a step are loaded after its integrator: loaded before it, the two 16-byte
+// rows stay live across the substeps of a kernel held to 128 registers, and the rollout measured 12 % slower.
 // XM: 0 = outputs stored once; 1 = also at every peer mirror (NVLink P2P); 2 = stored ONLY through the multicast
 // mapping (multimem.st: the switch replicates them into every rank's arena, this rank's included)
 template <bool SIMPLE, int XM>
@@ -1131,8 +1147,7 @@ __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_
     }
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
-    const float *trow = nullptr;
-    if (active && c.task == MGB_TASK_VELOCITY_CONTROL) trow = a.targets + ((int64_t)__ldg(a.env2task + e) * c.nt) * 3;
+    const int task = active ? env_task(c, a, e) : 0;
     // software pipeline: the action of step t+1 is requested while step t integrates
     float4 act_next = make_float4(0.f, 0.f, 0.f, 0.f);
     if (active && a.act) act_next = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
@@ -1163,18 +1178,18 @@ __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_
             }
             s.ct[0] += 1;
             TargetRows<float> tr;
-            if (c.task == MGB_TASK_VELOCITY_CONTROL) prefetch_targets(c, trow, s.ct[0], 0, tr);
             const float z_old = s.p[2] + c.z_off;
             const float x_old = s.p[0], y_old = s.p[1];
             float power;
             int fail[1];
             fail[0] = integrate1<SIMPLE>(c, s, act, adj, id, power);
+            if (c.task == MGB_TASK_VELOCITY_CONTROL) prefetch_targets(c, a, task, s.ct[0], 0, tr);
             float o[kMaxObs], reward;
             int done[1];
             bool wf[1];
             finish_step<float>(c, a, e, s, adj, id, z_old, x_old, y_old, power, fail, tr, o, reward, done, wf);
             if (wf[0]) {
-                observe_reset(c, a, e, s, 0, o);
+                observe_reset(c, a, task, s, 0, o);
                 adjugate(s.R, adj, id);
             }
             if (a.rew) {
@@ -1238,9 +1253,8 @@ __global__ void __launch_bounds__(kThreads) quad_reset_kernel(const __grid_const
         adjugate(s.R, adj, id);
         observe(c, s, adj, id, o, bv, Ri);
         if (c.task == MGB_TASK_VELOCITY_CONTROL) {
-            const float *trow = a.targets + ((int64_t)a.env2task[e] * c.nt) * 3;
-            const int t = s.ct[0] < c.nt - 1 ? s.ct[0] : c.nt - 1;
-            o[16] = trow[3 * t]; o[17] = trow[3 * t + 1]; o[18] = trow[3 * t + 2];
+            const float4 q = target_row(a, env_task(c, a, e), s.ct[0] < c.nt - 1 ? s.ct[0] : c.nt - 1);
+            o[16] = q.x; o[17] = q.y; o[18] = q.z;
         }
         float *dst = a.obs + e * c.obs_dim;
 #pragma unroll
@@ -1314,6 +1328,17 @@ __global__ void quad_targets_kernel(const __grid_constant__ QuadConst c, const f
     }
 }
 
+// mgb_quad_set_targets: task-major [n_tasks][nt][3] float32 -> the handle's time-major [nt][n_tasks] float4 (x, y, z, 0),
+// one thread per row (values copied, not recomputed)
+__global__ void quad_targets_layout_kernel(const float *__restrict__ src, int nt, int n_tasks, float4 *__restrict__ dst)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;     // = t * n_tasks + task
+    if (i >= (int64_t)nt * n_tasks) return;
+    const int64_t t = i / n_tasks, k = i % n_tasks;
+    const float *s = src + (k * nt + t) * 3;
+    dst[i] = make_float4(s[0], s[1], s[2], 0.f);
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1327,7 +1352,7 @@ struct mgb_quad {
     float4 *planes = nullptr;
     int32_t *sat = nullptr;
     int map_rows = 0, map_cols = 0, x_off = 0, y_off = 0;
-    float *targets = nullptr;
+    float4 *targets = nullptr;  // [nt][n_tasks] (x, y, z, 0), built by mgb_quad_set_targets
     int32_t *env2task = nullptr;
     int n_tasks = 0;
     int auto_reset = 0;
@@ -1360,6 +1385,7 @@ static QuadArgs base_args(const mgb_quad *h)
     a.n = h->n;
     a.env_base = h->env_base;
     a.targets = h->targets;
+    a.n_tasks = h->n_tasks;
     a.sat = h->sat; a.map_rows = h->map_rows; a.map_cols = h->map_cols; a.x_off = h->x_off; a.y_off = h->y_off;
     a.env2task = h->env2task;
     a.seed = h->seed;
@@ -1545,13 +1571,16 @@ extern "C" int mgb_quad_set_targets(mgb_quad *h, const float *tbl_dev, int32_t n
     MGB_CUDA(cudaDeviceSynchronize());
     cudaFree(h->targets); h->targets = nullptr;
     cudaFree(h->env2task); h->env2task = nullptr;
-    const size_t tb = sizeof(float) * 3 * (size_t)h->c.nt * (size_t)n_tasks;
-    MGB_CUDA(cudaMalloc(&h->targets, tb));
+    h->n_tasks = 0;
+    // the kernels read the table time-major with 16-byte rows (prefetch_targets): 16 instead of 12 bytes per row
+    const int64_t rows = (int64_t)h->c.nt * n_tasks;
+    MGB_CUDA(cudaMalloc(&h->targets, sizeof(float4) * (size_t)rows));
     MGB_CUDA(cudaMalloc(&h->env2task, sizeof(int32_t) * h->n));
-    MGB_CUDA(cudaMemcpy(h->targets, tbl_dev, tb, cudaMemcpyDeviceToDevice));
+    quad_targets_layout_kernel<<<(unsigned)((rows + 255) / 256), 256>>>(tbl_dev, h->c.nt, n_tasks, h->targets);
+    MGB_CUDA(cudaGetLastError());
     MGB_CUDA(cudaMemcpy(h->env2task, env2task_dev, sizeof(int32_t) * h->n, cudaMemcpyDeviceToDevice));
     // a device-to-device cudaMemcpy may return before the copy is done, and a step launched next on a non-blocking
-    // stream would not be ordered after it
+    // stream would not be ordered after it (nor after the layout kernel)
     MGB_CUDA(cudaDeviceSynchronize());
     h->n_tasks = n_tasks;
     return MGB_OK;
@@ -1613,9 +1642,9 @@ static StepKernel choose_step_kernel(const mgb_quad *h, const QuadArgs &a)
                              (reinterpret_cast<uintptr_t>(a.done) & 1u) == 0 && (reinterpret_cast<uintptr_t>(a.fail) & 7u) == 0;
         if (aligned) return STEP_PACKED;
     }
-    // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (400 W power limit,
-    // velocity_control dt = 0.005, CUDA graphs of 256 steps), us per step tile / wide: 9 473 envs 5.38 / 3.23, 24 576 envs
-    // 5.99 / 5.07, 49 152 envs 6.71 / 6.42, but 65 536 envs 7.49 / 8.92 and 67 001 envs 8.18 / 8.81.
+    // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (700 W power limit,
+    // velocity_control dt = 0.005, CUDA graphs of 256 steps, medians of 3 runs), us per step tile / wide: 9 473 envs
+    // 4.87 / 3.09, 24 576 envs 5.26 / 4.73, 49 152 envs 6.88 / 5.89, but 65 536 envs 6.79 / 8.09 and 67 001 envs 7.39 / 7.90.
     // So by default the wide kernel takes batches of up to 384 envs per SM and the 64-env tile kernel the rest.
     const bool single_wave = a.n <= (int64_t)h->num_sms * 512 && a.n >= (int64_t)h->num_sms * 64;
     const int64_t wide_max = (int64_t)h->num_sms * (h->wide_kernel > 0 ? 512 : 384);
