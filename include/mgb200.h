@@ -129,6 +129,14 @@ int mgb_quad_reset(mgb_quad *h, const uint8_t *mask_dev, const double *noise_dev
  *   final_obs_dev [n][obs_dim] or NULL (terminal observation of envs that finished, when auto_reset is on) */
 int mgb_quad_step(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
                   int32_t *fail_dev, float *final_obs_dev, void *stream);
+/* mgb_quad_step with one more optional output (NULL: not produced, and the call is exactly mgb_quad_step):
+ *   truncated_dev [n] uint8, written for every env: 1 iff done and the episode ended through the time limit alone,
+ *     `ct == nt` (env.py:159-161).  A collision in the same step is terminal: its branch (env.py:144-150) clears ct
+ *     before the time-limit check.  A failure (MGB_FAIL_*, where the reference raises) is terminal.  So
+ *     terminated = done && !truncated; for velocity_control, truncated = done && fail == MGB_FAIL_NONE.
+ * obs, rew, done, fail, final_obs and the env state are bit for bit what mgb_quad_step gives. */
+int mgb_quad_step_ex(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                     int32_t *fail_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream);
 
 /* T consecutive Quadrotor.step calls (env.py:127-165; the rollout loop of quadrotor/tests/test_env.py:22-28) in ONE launch
  * with the state held in registers (auto-reset semantics as configured).
@@ -137,6 +145,16 @@ int mgb_quad_step(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_
  *   obs_dev [T][n][obs_dim], rew_dev [T][n], done_dev [T][n]; any of them may be NULL to skip that output. */
 int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
                      float *obs_dev, float *rew_dev, uint8_t *done_dev, void *stream);
+/* mgb_quad_rollout with two optional outputs (both NULL: exactly mgb_quad_rollout):
+ *   final_obs_dev [T][n][obs_dim] float32: row (t, e) is written only when done[t][e] = 1, with the observation an
+ *     auto_reset-off handle would have returned at step t (the terminal one, env.py:163-165).  Rows with done = 0 are
+ *     not written.  Needs auto_reset on (MGB_ERR_ARG otherwise).
+ *   truncated_dev [T][n] uint8, written for every (t, e): as mgb_quad_step_ex's truncated_dev (env.py:144-161).
+ * obs, rew, done, the drawn actions and the env state are bit for bit what mgb_quad_rollout gives.  Either output while
+ * output mirrors or multicast are set is MGB_ERR_ARG. */
+int mgb_quad_rollout_ex(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
+                        float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                        void *stream);
 
 /* Quadrotor.step as the reference's numpy users call it (env.py:127-165: ndarray in, ndarray out).
  * Same as mgb_quad_step with HOST buffers: stages through pinned memory (or, for pinned caller buffers, lets the kernel
@@ -147,6 +165,10 @@ int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_
  * This is the call a numpy user of the reference API makes. */
 int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs_host, float *rew_host, uint8_t *done_host,
                        int32_t *fail_host, float *final_obs_host, void *stream);
+/* mgb_quad_step_host with truncated_host [n] uint8 (NULL: not produced): what mgb_quad_step_ex's truncated_dev reports
+ * (env.py:144-161), through the same zero-copy, copy and hybrid paths (a pageable truncated_host takes the copy path). */
+int mgb_quad_step_host_ex(mgb_quad *h, const float *act_host, float *obs_host, float *rew_host, uint8_t *done_host,
+                          int32_t *fail_host, float *final_obs_host, uint8_t *truncated_host, void *stream);
 
 /* Checkpoint / inspection (quadrotorsim.py:30-48 _save_state/_restore_state): state_dev [n][22] float32 row-major
  * = p3 v3 w3 prop4 R9, ct_dev [n] int32.  load = 0 copies handle -> buffers, 1 buffers -> handle. */
@@ -298,6 +320,18 @@ int mgb_maze_set_options(mgb_maze *h, int auto_reset);
  *   rew_dev [T][n] float64, done_dev [T][n] uint8 (any may be NULL). */
 int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
                      void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream);
+/* mgb_maze_rollout with the two optional outputs of mgb_maze_step_ex, per step (both NULL: exactly mgb_maze_rollout).
+ * MetaMaze2D only: a MetaMazeDiscrete3D handle given either one returns MGB_ERR_ARG.
+ *   final_obs_dev [T][n][2g+1][2g+1] float32: row (t, e) is written only when done[t][e] = 1, with the terminal window
+ *     (update_observation, maze_2d.py:89-121, on the state evaluation_rule left).  Rows with done = 0 are not written.
+ *     Needs auto_reset on (MGB_ERR_ARG otherwise).
+ *   truncated_dev [T][n] uint8, written for every (t, e): 1 iff done and the episode ended only through the step limit
+ *     (maze_base.py:80,91-95,191-192).
+ * obs, rew, done, the drawn actions and the env state are bit for bit what mgb_maze_rollout gives.  Either output while
+ * output mirrors or multicast are set is MGB_ERR_ARG. */
+int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
+                        void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
+                        void *stream);
 
 /* MetaMazeContinuous3D.step (maze_env.py:129-146 -> maze_continuous_3d.py:47-56, dynamics.py:58-92): act_dev [n][2]
  * float32 = (turn_rate, walk_speed), clipped to [-1, 1] like the reference; ten 10 ms sub-steps of turn/walk with the

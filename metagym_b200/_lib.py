@@ -63,6 +63,9 @@ SIGNATURES = {
     "mgb_quad_step": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_quad_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
     "mgb_quad_step_host": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_quad_step_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_quad_step_host_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_quad_rollout_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_quad_state": (ctypes.c_int, [vp, vp, vp, ctypes.c_int, vp]),
     "mgb_quad_launch_count": (c_i64, [vp]),
     "mgb_quad_step_kernel": (ctypes.c_char_p, [vp]),
@@ -92,6 +95,7 @@ SIGNATURES = {
     "mgb_quad_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
     "mgb_maze_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
     "mgb_maze_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
+    "mgb_maze_rollout_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_step_continuous": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
     "mgb_maze_step_continuous_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_rollout_continuous": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),

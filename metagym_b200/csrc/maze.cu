@@ -408,9 +408,37 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_kernel(const __grid_constan
 }
 
 
+// update_observation (maze_2d.py:89-121) of one env into row: the terminal windows of maze2d_rollout_kernel<0, true>.  The
+// rollout's observation tile writes the same loop out: routed through a shared helper, the instantiations without FIN
+// were scheduled differently (same instructions, other order), and they are kept exactly as they were.
+__device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t *blob, const int32_t *eaten,
+                                              int64_t estride, const Env &s, float *row)
+{
+    const TaskHdr *th = blob_hdr(blob);
+    const int8_t *walls = reinterpret_cast<const int8_t *>(blob + c.off_walls);
+    const int n = c.n, g = c.view_grid, W = 2 * g + 1;
+    for (int p = 0; p < W; ++p)
+        for (int q = 0; q < W; ++q) {
+            const int x = s.gx - g + p, y = s.gy - g + q;
+            float v = -1.0f;
+            if (x >= 0 && x < n && y >= 0 && y < n) {
+                v = (float)(-(int)walls[x * n + y]);
+                if (c.task_type == MGB_MAZE_SURVIVAL)
+                    v = (float)((double)v + food_now(c, blob, eaten, estride, s.steps, x * n + y));
+                else
+                    v = (float)((double)v + ((x == th->goal[0] && y == th->goal[1]) ? 1.0 : 0.0));
+            }
+            row[p * W + q] = v;
+        }
+    if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
+}
+
 // T MetaMaze2D steps in one launch: the agent (cell, step counter, life) stays in registers, food stamps stay in their
 // SoA slots, each step's observation tile of the CTA leaves through double-buffered shared memory + one bulk store.
-template <int XM>   // 0 plain, 1 peer mirrors, 2 multicast-only stores (see quad_rollout_kernel)
+// XM: 0 plain, 1 peer mirrors, 2 multicast-only stores (see quad_rollout_kernel).  FIN (XM == 0 only, mgb_maze_rollout_ex):
+// also store the truncation byte of every (t, e), and the terminal window of every env that finished at step t to
+// final_obs + (t n + e) D, both before env_reset; rows of envs that did not finish are not written.
+template <int XM, bool FIN>
 __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid_constant__ MazeConst c,
                                                                     const __grid_constant__ MazeArgs a)
 {
@@ -456,6 +484,12 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
             double reward;
             int done;
             maze_logic(c, blob, eaten, a.n_pad, s, action, reward, done);
+            if (FIN) {
+                static_assert(!FIN || XM == 0, "terminal rows and truncation flags are not mirrored");
+                if (a.truncated) a.truncated[(int64_t)t * a.n + e] = maze_truncated(c, blob, s);
+                if (done && a.final_obs)
+                    maze2d_window(c, blob, eaten, a.n_pad, s, reinterpret_cast<float *>(a.final_obs) + ((int64_t)t * a.n + e) * D);
+            }
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
             if (a.rew) {
                 if (XM == 2) mgb_mc_st(mgb_shift(a.rew + (int64_t)t * a.n + e, a.mir.delta[0]), reward);
@@ -3166,14 +3200,19 @@ extern "C" int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_de
     return MGB_OK;
 }
 
-extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                                void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream)
+static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
+                   void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
+                   void *stream)
 {
-    MgbRange nvtx_range("mgb_maze_rollout");
     MGB_REQUIRE(h, "null handle");
     MGB_REQUIRE(T > 0, "T must be positive");
     MGB_REQUIRE(h->c.kind == MGB_MAZE_2D || h->c.kind == MGB_MAZE_DISCRETE_3D,
                 "mgb_maze_rollout serves MetaMaze2D and MetaMazeDiscrete3D");
+    const bool fin = final_obs_dev || truncated_dev;
+    MGB_REQUIRE(!fin || h->c.kind == MGB_MAZE_2D, "final_obs / truncated of a rollout are produced for MetaMaze2D only");
+    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
+    MGB_REQUIRE(!fin || h->mir.count == 0,
+                "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
     int rc = maze_ready(h);
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
@@ -3212,21 +3251,42 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, 
     const size_t sm = (size_t)2 * k2dThreads * W * W * 4;
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     if (sm > 48 * 1024) {
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0>));
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<1>));
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<2>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<1, false>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<2, false>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true>));
     }
     if (h->mir.count == MGB_MIRROR_MULTICAST) {
         MGB_REQUIRE(h->n % 4 == 0, "multicast outputs need num_envs % 4 == 0");
         MGB_REQUIRE((((uintptr_t)done_dev | (uintptr_t)obs_dev | (uintptr_t)act_out_dev) & 3) == 0 && ((uintptr_t)rew_dev & 7) == 0,
                     "multicast outputs must be 4-byte (rewards: 8-byte) aligned");
-        maze2d_rollout_kernel<2><<<blocks, k2dThreads, sm, st>>>(h->c, a);
-    } else if (h->mir.count > 0) maze2d_rollout_kernel<1><<<blocks, k2dThreads, sm, st>>>(h->c, a);
-    else maze2d_rollout_kernel<0><<<blocks, k2dThreads, sm, st>>>(h->c, a);
+        maze2d_rollout_kernel<2, false><<<blocks, k2dThreads, sm, st>>>(h->c, a);
+    } else if (h->mir.count > 0) maze2d_rollout_kernel<1, false><<<blocks, k2dThreads, sm, st>>>(h->c, a);
+    else if (fin) {
+        a.final_obs = final_obs_dev;
+        a.truncated = truncated_dev;
+        maze2d_rollout_kernel<0, true><<<blocks, k2dThreads, sm, st>>>(h->c, a);
+    } else maze2d_rollout_kernel<0, false><<<blocks, k2dThreads, sm, st>>>(h->c, a);
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
+}
+
+extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
+                                void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout");
+    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
+}
+
+extern "C" int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
+                                   int32_t *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                   void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_ex");
+    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
+                   stream);
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)

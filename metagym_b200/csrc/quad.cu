@@ -87,6 +87,9 @@ struct QuadArgs {
     uint32_t t_base;
     float *act_out;
     MgbMirrors mir;            // rollout only: every output is also stored at ptr + mir.delta[i]
+    // [n] (rollout: [T][n]) uint8, 1 where done came only from ct == nt (env.py:159-161); null: not produced.  Last, so
+    // that the parameter offsets of the fields above do not move.
+    uint8_t *truncated;
 };
 
 // Register state of Lanes<T>::N envs
@@ -684,12 +687,14 @@ __device__ __forceinline__ void observe_reset(const QuadConst &c, const QuadArgs
 
 // Task logic after the integrator: observation, reward, collision, done, counters, optional auto-reset.
 // o[] receives the observation of the (pre-reset) end state; lane h of env e + h.  write_final[h]: auto-reset replaced
-// the env, o[] is its terminal observation and the caller must publish observe_reset() instead.
+// the env, o[] is its terminal observation and the caller must publish observe_reset() instead.  trunc[h]: the episode
+// ended through ct == nt alone (env.py:159-161): a collision clears ct first (env.py:144-150) and a failure is terminal.
 template <class T>
 __device__ __forceinline__ void finish_step(const QuadConst &c, const QuadArgs &a, int64_t e, VState<T> &s,
                                             const T adj[9], T id, T z_old, T x_old, T y_old, T power,
                                             const int fail[Lanes<T>::N], const TargetRows<T> &tr, T *o, T &reward,
-                                            int done_flag[Lanes<T>::N], bool write_final[Lanes<T>::N])
+                                            int done_flag[Lanes<T>::N], bool write_final[Lanes<T>::N],
+                                            int trunc[Lanes<T>::N])
 {
     constexpr int N = Lanes<T>::N;
     T bv[3], Ri[9];
@@ -737,6 +742,7 @@ __device__ __forceinline__ void finish_step(const QuadConst &c, const QuadArgs &
     }
 #pragma unroll
     for (int h = 0; h < N; ++h) {
+        trunc[h] = s.ct[h] == c.nt && !fail[h];                   // before the counters are cleared
         if (s.ct[h] == c.nt) { done[h] = 1; s.ct[h] = 0; }        // env.py:159-161
         if (fail[h]) { done[h] = 1; s.ct[h] = 0; }                // the reference raises (quadrotorsim.py:212-221)
         done_flag[h] = done[h];
@@ -872,10 +878,10 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
         store_state(a, e, s1);
     }
     T o[kMaxObs], reward;
-    int done[N];
+    int done[N], trunc[N];
     bool wf[N];
-    finish_step(c, a, e, s, adj, id, z_old, x_old, y_old, power, fail, tr, o, reward, done, wf);
-    // ---- state / reward / done / fail stores
+    finish_step(c, a, e, s, adj, id, z_old, x_old, y_old, power, fail, tr, o, reward, done, wf, trunc);
+    // ---- state / reward / done / fail / truncated stores
     bool stored = false;
     if constexpr (N == 2) {
         if (nact == 2) {
@@ -883,6 +889,7 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
             *reinterpret_cast<float2 *>(a.rew + e) = reward.v;
             *reinterpret_cast<uchar2 *>(a.done + e) = make_uchar2((uint8_t)done[0], (uint8_t)done[1]);
             if (a.fail) *reinterpret_cast<int2 *>(a.fail + e) = make_int2(fail[0], fail[1]);
+            if (a.truncated) *reinterpret_cast<uchar2 *>(a.truncated + e) = make_uchar2((uint8_t)trunc[0], (uint8_t)trunc[1]);
             stored = true;
         }
     }
@@ -896,6 +903,7 @@ __device__ __forceinline__ void step_body(const QuadConst &c, const QuadArgs &a,
                 a.rew[e + h] = lane(reward, h);
                 a.done[e + h] = (uint8_t)done[h];
                 if (a.fail) a.fail[e + h] = fail[h];
+                if (a.truncated) a.truncated[e + h] = (uint8_t)trunc[h];
             }
         }
     }
@@ -1129,7 +1137,10 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 // rows stay live across the substeps of a kernel held to 128 registers, and the rollout measured 12 % slower.
 // XM: 0 = outputs stored once; 1 = also at every peer mirror (NVLink P2P); 2 = stored ONLY through the multicast
 // mapping (multimem.st: the switch replicates them into every rank's arena, this rank's included)
-template <bool SIMPLE, int XM>
+// FIN (XM == 0 only, mgb_quad_rollout_ex): also store the truncation byte of every (t, e), and the terminal observation of
+// every env an auto-reset replaced at step t to final_obs + (t n + e) D, straight from registers before observe_reset
+// overwrites them.  Rows of envs that did not finish are not written.
+template <bool SIMPLE, int XM, bool FIN>
 __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_constant__ QuadConst c,
                                                                 const __grid_constant__ QuadArgs a)
 {
@@ -1185,9 +1196,19 @@ __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_
             fail[0] = integrate1<SIMPLE>(c, s, act, adj, id, power);
             if (c.task == MGB_TASK_VELOCITY_CONTROL) prefetch_targets(c, a, task, s.ct[0], 0, tr);
             float o[kMaxObs], reward;
-            int done[1];
+            int done[1], trunc[1];
             bool wf[1];
-            finish_step<float>(c, a, e, s, adj, id, z_old, x_old, y_old, power, fail, tr, o, reward, done, wf);
+            finish_step<float>(c, a, e, s, adj, id, z_old, x_old, y_old, power, fail, tr, o, reward, done, wf, trunc);
+            if (FIN) {
+                static_assert(!FIN || XM == 0, "terminal rows and truncation flags are not mirrored");
+                if (a.truncated) a.truncated[(int64_t)t * a.n + e] = (uint8_t)trunc[0];
+                if (wf[0] && a.final_obs) {
+                    float *frow = a.final_obs + ((int64_t)t * a.n + e) * D;
+#pragma unroll
+                    for (int k = 0; k < 16; ++k) frow[k] = o[k];
+                    if (D == 19) { frow[16] = o[16]; frow[17] = o[17]; frow[18] = o[18]; }
+                }
+            }
             if (wf[0]) {
                 observe_reset(c, a, task, s, 0, o);
                 adjugate(s.R, adj, id);
@@ -1369,10 +1390,10 @@ struct mgb_quad {
     MgbMirrorWindow mir_win;   // mgb_quad_set_mirror_window
     // host staging for *_host entry points
     float *h_act = nullptr, *h_obs = nullptr, *h_rew = nullptr, *h_final = nullptr;
-    uint8_t *h_done = nullptr;
+    uint8_t *h_done = nullptr, *h_trunc = nullptr;
     int32_t *h_fail = nullptr;
     float *d_act = nullptr, *d_obs = nullptr, *d_rew = nullptr, *d_final = nullptr;
-    uint8_t *d_done = nullptr;
+    uint8_t *d_done = nullptr, *d_trunc = nullptr;
     int32_t *d_fail = nullptr;
 };
 
@@ -1516,9 +1537,9 @@ extern "C" void mgb_quad_destroy(mgb_quad *h)
     cudaFree(h->targets);
     cudaFree(h->env2task);
     cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_done);
-    cudaFree(h->d_fail); cudaFree(h->d_final);
+    cudaFree(h->d_fail); cudaFree(h->d_final); cudaFree(h->d_trunc);
     cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_done);
-    cudaFreeHost(h->h_fail); cudaFreeHost(h->h_final);
+    cudaFreeHost(h->h_fail); cudaFreeHost(h->h_final); cudaFreeHost(h->h_trunc);
     delete h;
 }
 
@@ -1637,9 +1658,10 @@ static StepKernel choose_step_kernel(const mgb_quad *h, const QuadArgs &a)
     // multi-wave launches stream: persistent CTAs + TMA double buffering (quad_stream_kernel)
     if (h->stream_kernel && (int64_t)blocks > (int64_t)h->num_sms * 32 && act16) return STEP_STREAM;
     if (h->packed && h->c.rk4_steps == 0 && a.n >= 2) {
-        // the packed kernel stores reward / done / fail of an env pair with one 8 / 2 / 8-byte access
+        // the packed kernel stores reward / done / fail / truncated of an env pair with one 8 / 2 / 8 / 2-byte access
         const bool aligned = act16 && (reinterpret_cast<uintptr_t>(a.rew) & 7u) == 0 &&
-                             (reinterpret_cast<uintptr_t>(a.done) & 1u) == 0 && (reinterpret_cast<uintptr_t>(a.fail) & 7u) == 0;
+                             (reinterpret_cast<uintptr_t>(a.done) & 1u) == 0 && (reinterpret_cast<uintptr_t>(a.fail) & 7u) == 0 &&
+                             (reinterpret_cast<uintptr_t>(a.truncated) & 1u) == 0;
         if (aligned) return STEP_PACKED;
     }
     // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (700 W power limit,
@@ -1711,10 +1733,9 @@ extern "C" const char *mgb_quad_step_kernel(const mgb_quad *h)
     }
 }
 
-extern "C" int mgb_quad_step(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
-                             int32_t *fail_dev, float *final_obs_dev, void *stream)
+static int step_dev(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                    int32_t *fail_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
-    MgbRange nvtx_range("mgb_quad_step");
     MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
     MGB_REQUIRE((reinterpret_cast<uintptr_t>(act_dev) & 15u) == 0, "act_dev must be 16-byte aligned");
     int rc = check_ready(h);
@@ -1723,22 +1744,41 @@ extern "C" int mgb_quad_step(mgb_quad *h, const float *act_dev, float *obs_dev, 
     QuadArgs a = base_args(h);
     a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.fail = fail_dev;
     a.final_obs = final_obs_dev;
+    a.truncated = truncated_dev;
     return launch_step(h, a, (cudaStream_t)stream);
 }
 
-extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
-                                float *obs_dev, float *rew_dev, uint8_t *done_dev, void *stream)
+extern "C" int mgb_quad_step(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                             int32_t *fail_dev, float *final_obs_dev, void *stream)
 {
-    MgbRange nvtx_range("mgb_quad_rollout");
+    MgbRange nvtx_range("mgb_quad_step");
+    return step_dev(h, act_dev, obs_dev, rew_dev, done_dev, fail_dev, final_obs_dev, nullptr, stream);
+}
+
+extern "C" int mgb_quad_step_ex(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                                int32_t *fail_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_step_ex");
+    return step_dev(h, act_dev, obs_dev, rew_dev, done_dev, fail_dev, final_obs_dev, truncated_dev, stream);
+}
+
+static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev, float *obs_dev,
+                   float *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
     MGB_REQUIRE(h, "null handle");
     MGB_REQUIRE(T > 0, "T must be positive");
     MGB_REQUIRE((reinterpret_cast<uintptr_t>(act_dev) & 15u) == 0, "act_dev must be 16-byte aligned");
+    const bool fin = final_obs_dev || truncated_dev;
+    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal observation)");
+    MGB_REQUIRE(!fin || h->mir.count == 0,
+                "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
     int rc = check_ready(h);
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
     QuadArgs a = base_args(h);
     a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev;
     a.T = T; a.act_seed = act_seed; a.t_base = h->t_base; a.act_out = act_out_dev;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
     const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
     a.mir = h->mir;
     if (h->mir.count != 0)
@@ -1750,19 +1790,38 @@ extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, ui
         MGB_REQUIRE(h->n % 4 == 0, "multicast outputs need num_envs % 4 == 0");
         MGB_REQUIRE((((uintptr_t)done_dev | (uintptr_t)rew_dev | (uintptr_t)obs_dev) & 3) == 0 && ((uintptr_t)act_out_dev & 15) == 0,
                     "multicast outputs must be 4-byte (actions: 16-byte) aligned");
-        if (h->c.simple) quad_rollout_kernel<true, 2><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 2><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        if (h->c.simple) quad_rollout_kernel<true, 2, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        else quad_rollout_kernel<false, 2, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
     } else if (h->mir.count > 0) {
-        if (h->c.simple) quad_rollout_kernel<true, 1><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 1><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        if (h->c.simple) quad_rollout_kernel<true, 1, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        else quad_rollout_kernel<false, 1, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+    } else if (fin) {
+        if (h->c.simple) quad_rollout_kernel<true, 0, true><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        else quad_rollout_kernel<false, 0, true><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
     } else {
-        if (h->c.simple) quad_rollout_kernel<true, 0><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 0><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        if (h->c.simple) quad_rollout_kernel<true, 0, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+        else quad_rollout_kernel<false, 0, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
     }
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
+}
+
+extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
+                                float *obs_dev, float *rew_dev, uint8_t *done_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout");
+    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
+}
+
+extern "C" int mgb_quad_rollout_ex(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
+                                   float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                                   uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_ex");
+    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
+                   stream);
 }
 
 extern "C" int mgb_quad_set_mirrors(mgb_quad *h, int count, const int64_t *byte_delta)
@@ -1807,6 +1866,8 @@ static int ensure_host_staging(mgb_quad *h)
     MGB_CUDA(cudaMalloc(&h->d_done, n));
     MGB_CUDA(cudaMalloc(&h->d_fail, n * 4));
     MGB_CUDA(cudaMalloc(&h->d_final, n * D * 4));
+    MGB_CUDA(cudaMalloc(&h->d_trunc, n));
+    MGB_CUDA(cudaMallocHost(&h->h_trunc, n));
     MGB_CUDA(cudaMemset(h->d_fail, 0, n * 4));
     MGB_CUDA(cudaMemset(h->d_final, 0, n * D * 4));     // rows keep the last terminal observation seen, like final_obs_dev
     MGB_CUDA(cudaMallocHost(&h->h_act, n * 16));
@@ -1827,10 +1888,9 @@ static void *pinned_device_alias(const void *p)
     return at.devicePointer;
 }
 
-extern "C" int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs_host, float *rew_host,
-                                  uint8_t *done_host, int32_t *fail_host, float *final_obs_host, void *stream)
+static int step_host(mgb_quad *h, const float *act_host, float *obs_host, float *rew_host, uint8_t *done_host,
+                     int32_t *fail_host, float *final_obs_host, uint8_t *truncated_host, void *stream)
 {
-    MgbRange nvtx_range("mgb_quad_step_host");
     MGB_REQUIRE(h && act_host && obs_host && rew_host && done_host, "null argument");
     int rc = check_ready(h);
     if (rc) return rc;
@@ -1848,11 +1908,12 @@ extern "C" int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs
          *dd = pinned_device_alias(done_host);
     void *df = fail_host ? pinned_device_alias(fail_host) : nullptr;
     void *dfo = final_obs_host ? pinned_device_alias(final_obs_host) : nullptr;
-    const bool opt_ok = (!fail_host || df) && (!final_obs_host || dfo);
+    void *dtr = truncated_host ? pinned_device_alias(truncated_host) : nullptr;
+    const bool opt_ok = (!fail_host || df) && (!final_obs_host || dfo) && (!truncated_host || dtr);
     if (h->zerocopy && da && dob && dr && dd && opt_ok && (reinterpret_cast<uintptr_t>(da) & 15u) == 0) {
         QuadArgs a = base_args(h);
         a.act = (const float *)da; a.obs = (float *)dob; a.rew = (float *)dr; a.done = (uint8_t *)dd;
-        a.fail = (int32_t *)df; a.final_obs = (float *)dfo;
+        a.fail = (int32_t *)df; a.final_obs = (float *)dfo; a.truncated = (uint8_t *)dtr;
         if (h->zerocopy == 2) {
             // hybrid: actions by DMA (copy engine), outputs written to host memory by the kernel
             MGB_CUDA(cudaMemcpyAsync(h->d_act, act_host, n * 16, cudaMemcpyHostToDevice, st));
@@ -1873,6 +1934,7 @@ extern "C" int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs
     a.act = h->d_act; a.obs = h->d_obs; a.rew = h->d_rew; a.done = h->d_done;
     a.fail = fail_host ? h->d_fail : nullptr;
     a.final_obs = final_obs_host ? h->d_final : nullptr;
+    a.truncated = truncated_host ? h->d_trunc : nullptr;
     rc = launch_step(h, a, st);
     if (rc) return rc;
     float *o = pin_out ? obs_host : h->h_obs;
@@ -1884,6 +1946,8 @@ extern "C" int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs
     if (fail_host) MGB_CUDA(cudaMemcpyAsync(pin_out ? fail_host : h->h_fail, h->d_fail, n * 4, cudaMemcpyDeviceToHost, st));
     if (final_obs_host)
         MGB_CUDA(cudaMemcpyAsync(pin_out ? final_obs_host : h->h_final, h->d_final, n * D * 4, cudaMemcpyDeviceToHost, st));
+    if (truncated_host)
+        MGB_CUDA(cudaMemcpyAsync(pin_out ? truncated_host : h->h_trunc, h->d_trunc, n, cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
     if (!pin_out) {
         memcpy(obs_host, h->h_obs, n * D * 4);
@@ -1891,8 +1955,24 @@ extern "C" int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs
         memcpy(done_host, h->h_done, n);
         if (fail_host) memcpy(fail_host, h->h_fail, n * 4);
         if (final_obs_host) memcpy(final_obs_host, h->h_final, n * D * 4);
+        if (truncated_host) memcpy(truncated_host, h->h_trunc, n);
     }
     return MGB_OK;
+}
+
+extern "C" int mgb_quad_step_host(mgb_quad *h, const float *act_host, float *obs_host, float *rew_host,
+                                  uint8_t *done_host, int32_t *fail_host, float *final_obs_host, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_step_host");
+    return step_host(h, act_host, obs_host, rew_host, done_host, fail_host, final_obs_host, nullptr, stream);
+}
+
+extern "C" int mgb_quad_step_host_ex(mgb_quad *h, const float *act_host, float *obs_host, float *rew_host,
+                                     uint8_t *done_host, int32_t *fail_host, float *final_obs_host,
+                                     uint8_t *truncated_host, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_step_host_ex");
+    return step_host(h, act_host, obs_host, rew_host, done_host, fail_host, final_obs_host, truncated_host, stream);
 }
 
 extern "C" int mgb_quad_state(mgb_quad *h, float *state_dev, int32_t *ct_dev, int load, void *stream)

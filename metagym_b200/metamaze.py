@@ -410,7 +410,8 @@ class _BatchedMazeBase(object):
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done_bool), info
 
-    def _rollout(self, T, actions, act_seed, want_actions, out):
+    def _rollout(self, T, actions, act_seed, want_actions, out, final=False):
+        """final: also produce the "final_obs" / "truncated" entries (MetaMaze2D with final_obs=True)."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -420,10 +421,20 @@ class _BatchedMazeBase(object):
                    "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
                    "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
                    "act": torch.empty((T, N), dtype=torch.int32, device=dev) if want_actions else None}
+            if final:
+                out["final_obs"] = torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
         a = None if actions is None else actions.to(torch.int32).reshape(T, N).contiguous()
-        _lib.check(self._lib.mgb_maze_rollout(self._h, int(T), _lib.ptr(a), int(act_seed), _lib.ptr(out.get("act")),
-                                              _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
-                                              _lib.ptr(out.get("done")), self._stream()))
+        if not final:
+            _lib.check(self._lib.mgb_maze_rollout(self._h, int(T), _lib.ptr(a), int(act_seed),
+                                                  _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
+                                                  _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")), self._stream()))
+        else:
+            _lib.check(self._lib.mgb_maze_rollout_ex(self._h, int(T), _lib.ptr(a), int(act_seed),
+                                                     _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
+                                                     _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
+                                                     _lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated")),
+                                                     self._stream()))
         return out
 
     def agent_state(self):
@@ -514,8 +525,14 @@ class BatchedMetaMaze2D(_BatchedMazeBase):
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
-        {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None)."""
-        return self._rollout(T, actions, act_seed, want_actions, out)
+        {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None).
+
+        With final_obs=True the dict also holds "final_obs" [T,N,<obs of one env>] float32: row (t, e) is the
+        terminal window of env e where done[t, e] (what step() reports as final_observation); it is allocated with
+        torch.empty, and rows with done 0 are not written, so they hold whatever the buffer held.  And "truncated"
+        [T,N] uint8, written for every step: 1 iff done and the episode ended only through max_steps.  A
+        caller-supplied `out` may omit either entry, and that output is then not produced."""
+        return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final)
 
 
 class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
@@ -558,7 +575,8 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
         """T steps in one launch on the pose cache: obs [T,N,res_h,res_v,3] (uint8 or int32), rew, done, act as for
-        BatchedMetaMaze2D.rollout."""
+        BatchedMetaMaze2D.rollout.  It does not return "final_obs" or "truncated", even with final_obs=True (those
+        are step() outputs here)."""
         return self._rollout(T, actions, act_seed, want_actions, out)
 
     def cache_info(self):
@@ -622,7 +640,8 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         """T steps in one launch of the direct renderer (mgb_maze_rollout_continuous), exactly as T step() calls.
         actions: anything reshapeable to [T,N,2] (turn_rate, walk_speed), clipped to [-1, 1] like step(); None draws them
         on the device, uniform on [-1, 1) like action_space.sample().  Returns dict(obs [T,N,res_h,res_v,3] in the env's
-        obs dtype, rew [T,N] f64, done [T,N] u8, act [T,N,2] f32: the drawn actions when want_actions, else None)."""
+        obs dtype, rew [T,N] f64, done [T,N] u8, act [T,N,2] f32: the drawn actions when want_actions, else None).
+        It does not return "final_obs" or "truncated", even with final_obs=True (those are step() outputs here)."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch

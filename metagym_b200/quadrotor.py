@@ -133,14 +133,19 @@ class BatchedQuadrotor(object):
     parity-checked; 'rk4' = classical RK4 with rk4_steps steps per env step, validated by convergence only).
     velocity_control: `seed` may be an int (as in the reference) or a sequence of seeds = distinct tasks; env i
     flies task `env2task[i]` (default i % n_tasks).
+    final_obs=True (needs auto_reset=True): every step() also reports `truncated`, and rollout() also returns the
+    terminal observations and truncation flags of its steps.
     """
     metadata = {"render.modes": []}
 
     def __init__(self, dt=0.01, nt=1000, seed=0, task="no_collision", map_file=None, simulator_conf=None,
                  healthy_reward=1.0, num_envs=1, device=0, auto_reset=False, rng_seed=0, env_index_base=0,
-                 env2task=None, squeeze=True, integrator="euler", rk4_steps=1, **kwargs):
+                 env2task=None, squeeze=True, integrator="euler", rk4_steps=1, final_obs=False, **kwargs):
         import torch
         assert task in ["velocity_control", "no_collision", "hovering_control"], "Invalid task setting"  # env.py:55
+        if final_obs and not auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True (without auto-reset obs already is the terminal frame)")
+        self._want_final = bool(final_obs)
         self.dt, self.nt, self.task, self.healthy_reward = dt, nt, task, healthy_reward
         self.num_envs = int(num_envs)
         self._squeeze = bool(squeeze) and self.num_envs == 1
@@ -184,6 +189,8 @@ class BatchedQuadrotor(object):
         self._own_ptrs = None
         self._host_results = False            # True after a host-path step: fail_code / final_observation are numpy
         self._final_obs = torch.zeros((N, D), dtype=torch.float32, device=dev) if self.auto_reset else None
+        # persistent, so that a step with final_obs=True can be captured in a CUDA graph
+        self._trunc = torch.zeros((N,), dtype=torch.uint8, device=dev) if self._want_final else None
         if self.map_matrix is not None and map_file is not None:
             m = np.ascontiguousarray(self.map_matrix, dtype=np.int32)
             _lib.check(self._lib.mgb_quad_set_map(self._h, m.ctypes.data, m.shape[0], m.shape[1]))
@@ -286,15 +293,25 @@ class BatchedQuadrotor(object):
                                   self._fail.data_ptr(), _lib.ptr(self._final_obs))
                 self._done_bool = self._done.view(torch.bool)
             p = self._own_ptrs
-            rc = self._lib.mgb_quad_step(self._h, act.data_ptr(), p[0], p[1], p[2], p[3], p[4], self._stream())
+            if self._trunc is None:
+                rc = self._lib.mgb_quad_step(self._h, act.data_ptr(), p[0], p[1], p[2], p[3], p[4], self._stream())
+            else:
+                rc = self._lib.mgb_quad_step_ex(self._h, act.data_ptr(), p[0], p[1], p[2], p[3], p[4],
+                                                self._trunc.data_ptr(), self._stream())
             if rc:
                 _lib.check(rc)
             obs, rew, done_b = self._obs, self._rew, self._done_bool
         else:
             obs, rew, done = out
-            _lib.check(self._lib.mgb_quad_step(self._h, act.data_ptr(), obs.data_ptr(), rew.data_ptr(),
-                                               done.data_ptr(), self._fail.data_ptr(), _lib.ptr(self._final_obs),
-                                               self._stream()))
+            if self._trunc is None:
+                _lib.check(self._lib.mgb_quad_step(self._h, act.data_ptr(), obs.data_ptr(), rew.data_ptr(),
+                                                   done.data_ptr(), self._fail.data_ptr(), _lib.ptr(self._final_obs),
+                                                   self._stream()))
+            else:
+                _lib.check(self._lib.mgb_quad_step_ex(self._h, act.data_ptr(), obs.data_ptr(), rew.data_ptr(),
+                                                      done.data_ptr(), self._fail.data_ptr(),
+                                                      _lib.ptr(self._final_obs), self._trunc.data_ptr(),
+                                                      self._stream()))
             done_b = done.view(torch.bool)
         info = QuadInfo(obs, self.obs_keys)
         return self._out(obs), self._out(rew), self._out(done_b), info
@@ -307,10 +324,17 @@ class BatchedQuadrotor(object):
             self._h_done = np.empty((self.num_envs,), dtype=np.uint8)
             self._h_fail = np.zeros((self.num_envs,), dtype=np.int32)
             self._h_final = np.zeros((self.num_envs, self.obs_dim), dtype=np.float32) if self.auto_reset else None
+            self._h_trunc = np.zeros((self.num_envs,), dtype=np.uint8) if self._want_final else None
         # enqueued on torch's current stream: ordered after a preceding reset() / rollout() / load_state_dict()
-        _lib.check(self._lib.mgb_quad_step_host(self._h, act.ctypes.data, self._h_obs.ctypes.data,
-                                                self._h_rew.ctypes.data, self._h_done.ctypes.data,
-                                                self._h_fail.ctypes.data, _lib.ptr(self._h_final), self._stream()))
+        if self._h_trunc is None:
+            _lib.check(self._lib.mgb_quad_step_host(self._h, act.ctypes.data, self._h_obs.ctypes.data,
+                                                    self._h_rew.ctypes.data, self._h_done.ctypes.data,
+                                                    self._h_fail.ctypes.data, _lib.ptr(self._h_final), self._stream()))
+        else:
+            _lib.check(self._lib.mgb_quad_step_host_ex(self._h, act.ctypes.data, self._h_obs.ctypes.data,
+                                                       self._h_rew.ctypes.data, self._h_done.ctypes.data,
+                                                       self._h_fail.ctypes.data, _lib.ptr(self._h_final),
+                                                       self._h_trunc.ctypes.data, self._stream()))
         self._host_results = True
         info = QuadInfo(self._h_obs, self.obs_keys)
         return (self._out(self._h_obs), self._out(self._h_rew), self._out(self._h_done.view(np.bool_)), info)
@@ -322,7 +346,13 @@ class BatchedQuadrotor(object):
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
         """T steps in one launch (state stays in registers).  actions: [T,N,4] CUDA tensor or None (device-drawn
-        U(min_voltage, max_voltage)).  Returns dict(obs [T,N,D], rew [T,N], done [T,N], act [T,N,4] or None)."""
+        U(min_voltage, max_voltage)).  Returns dict(obs [T,N,D], rew [T,N], done [T,N], act [T,N,4] or None).
+
+        With final_obs=True the dict also holds "final_obs" [T,N,D] float32: row (t, e) is the terminal observation
+        of env e where done[t, e] (what step() reports as final_observation); it is allocated with torch.empty, and
+        rows with done 0 are not written, so they hold whatever the buffer held.  And "truncated" [T,N] uint8, written
+        for every step: 1 iff done and the episode ended through the time limit nt alone.  A caller-supplied `out` may
+        omit either entry, and that output is then not produced."""
         torch = self._torch
         N, D, dev = self.num_envs, self.obs_dim, self.device
         if out is None:
@@ -330,12 +360,22 @@ class BatchedQuadrotor(object):
                    "rew": torch.empty((T, N), dtype=torch.float32, device=dev),
                    "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
                    "act": torch.empty((T, N, 4), dtype=torch.float32, device=dev) if want_actions else None}
+            if self._want_final:
+                out["final_obs"] = torch.empty((T, N, D), dtype=torch.float32, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
         a = None
         if actions is not None:
             a = actions.to(torch.float32).reshape(T, N, 4).contiguous()
-        _lib.check(self._lib.mgb_quad_rollout(self._h, int(T), _lib.ptr(a), int(act_seed), _lib.ptr(out.get("act")),
-                                              _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
-                                              _lib.ptr(out.get("done")), self._stream()))
+        if not self._want_final:
+            _lib.check(self._lib.mgb_quad_rollout(self._h, int(T), _lib.ptr(a), int(act_seed),
+                                                  _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
+                                                  _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")), self._stream()))
+        else:
+            _lib.check(self._lib.mgb_quad_rollout_ex(self._h, int(T), _lib.ptr(a), int(act_seed),
+                                                     _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
+                                                     _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
+                                                     _lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated")),
+                                                     self._stream()))
         return out
 
     def _set_window(self, window):
@@ -366,6 +406,16 @@ class BatchedQuadrotor(object):
     @property
     def final_observation(self):
         return self._h_final if self._host_results else self._final_obs
+
+    @property
+    def truncated(self):
+        """final_obs=True: [N] bool, written by every step(): True iff done and the episode ended through ct == nt
+        alone (env.py:159-161); a collision or a failure in that step is terminal.  So terminated = done & ~truncated.
+        A torch tensor after a device step, a numpy array after a host step.  None with final_obs=False."""
+        if self._trunc is None:
+            return None
+        t = self._h_trunc.view(np.bool_) if self._host_results else self._trunc.view(self._torch.bool)
+        return self._out(t)
 
     def raise_on_failure(self):
         """Strict mode helper: re-raise the reference's exception for the first failed env of the last step."""
