@@ -332,6 +332,21 @@ int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t ac
 int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
                         void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
                         void *stream);
+/* mgb_maze_rollout of a MetaMazeDiscrete3D handle (pose cache) with the two optional outputs of mgb_maze_step_ex, per step
+ * (both NULL: exactly mgb_maze_rollout).  Any other handle kind is MGB_ERR_ARG.
+ *   final_obs_dev [T][n][res_h][res_v][3] in the obs dtype: row (t, e) is written only when done[t][e] = 1, with the frame
+ *     an auto_reset-off handle would have returned at step t (update_observation, maze_discrete_3d.py:113-127, on the state
+ *     evaluation_rule left: the food it left and the life bar at the terminal life).  Rows with done = 0 are not written.
+ *     Needs auto_reset on (MGB_ERR_ARG otherwise).
+ *   truncated_dev [T][n] uint8, written for every (t, e): 1 iff done and the episode ended only through the step limit
+ *     (maze_base.py:80,91-95,191-192).
+ * obs_dev may be NULL (then only the terminal frames and the flags are produced).  obs, rew, done, the drawn actions, the
+ * generator's step counter and the env state are bit for bit what mgb_maze_rollout gives.  Either output while output
+ * mirrors or multicast are set is MGB_ERR_ARG; so is a handle without a pose cache.  Stream-ordered, no host
+ * synchronisation, no allocation: capturable in a CUDA graph. */
+int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
+                                 void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                                 uint8_t *truncated_dev, void *stream);
 
 /* MetaMazeContinuous3D.step (maze_env.py:129-146 -> maze_continuous_3d.py:47-56, dynamics.py:58-92): act_dev [n][2]
  * float32 = (turn_rate, walk_speed), clipped to [-1, 1] like the reference; ten 10 ms sub-steps of turn/walk with the
@@ -350,6 +365,20 @@ int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, void *obs_dev
  *   done_dev [T][n] uint8.  Refused while output mirrors are set.  Stream-ordered, no host synchronisation. */
 int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
                                 void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream);
+/* mgb_maze_rollout_continuous with the two optional outputs of mgb_maze_step_continuous_ex, per step (both NULL: exactly
+ * mgb_maze_rollout_continuous).  Any other handle kind is MGB_ERR_ARG.
+ *   final_obs_dev [T][n][res_h][res_v][3] in the obs dtype: row (t, e) is written only when done[t][e] = 1, with the frame
+ *     an auto_reset-off handle would have returned at step t (maze_continuous_3d.py:47-56 then the ray-cast observation on
+ *     the state evaluation_rule left, maze_base.py:65-95).  Rows with done = 0 are not written.  Needs auto_reset on.
+ *   truncated_dev [T][n] uint8, written for every (t, e): 1 iff done and the episode ended only through the step limit
+ *     (maze_base.py:80,91-95,191-192).
+ * A finished env costs one more frame in the same launch.  obs, rew, done, the drawn actions, the generator's step counter,
+ * the env state and the pose are bit for bit what mgb_maze_rollout_continuous gives.  Refused while output mirrors or
+ * multicast are set.  Stream-ordered, no host synchronisation, no allocation after the first call of the handle's
+ * renderer (reset() makes it): capturable in a CUDA graph. */
+int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
+                                   void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                                   uint8_t *truncated_dev, void *stream);
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

@@ -647,14 +647,21 @@ __device__ __forceinline__ void push_terminal_state(const MazeConst &c, const Ma
 //               t = 0..T-1 of env blockIdx.x, then of env blockIdx.x + gridDim.x, ...; so the pipelined order prepares
 //               step t + 1 under the pixels of step t.  The pixel phase reads only its record set's snapshot (transparent
 //               map, pose, life-bar end), never the env state that the next item's step logic is rewriting.
-template <bool FILL, bool ROLL>
+// FIN (ROLL only, mgb_maze_rollout_continuous_ex): the step logic of item (env, t) also stores truncated[t][env].  When the
+//               env finished and final_obs is wanted it does NOT reset: the item's record set is built from the terminal
+//               state and its pixels go to final_obs[t][env]; the next item is then (env, t, reset), whose geometry runs
+//               env_reset, stores the state and builds the record set of the new episode's first frame for obs[t][env].
+//               The destination travels with the record set; whether a reset item follows is published in shared memory
+//               before the trip's closing barrier, so every thread takes the same next item.
+template <bool FILL, bool ROLL, bool FIN = false>
 __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_constant__ MazeConst c,
                                                                    const __grid_constant__ MazeArgs a)
 {
+    static_assert(!FIN || (ROLL && !FILL), "terminal frames are a rollout output");
     extern __shared__ __align__(128) uint8_t smem[];
     // list pass (final_obs set): items are the entries of the terminal list the step logic just wrote; a CTA without one
     // leaves before it stages the textures
-    const int64_t n_items = !FILL && a.final_obs ? (int64_t)*a.fin_count : a.n;
+    const int64_t n_items = !FILL && !FIN && a.final_obs ? (int64_t)*a.fin_count : a.n;
     if ((int64_t)blockIdx.x >= n_items) return;
     const int n = c.n, H = c.res_h, V = c.res_v, ts = c.ts;
     const int tex_words = (c.n_tex + 1) * ts * ts;
@@ -693,6 +700,10 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     s_env2[0] = reinterpret_cast<int *>(smem + off);      s_pose2[0] = reinterpret_cast<double *>(smem + off + 32);
     s_env2[1] = reinterpret_cast<int *>(smem + off + 64); s_pose2[1] = reinterpret_cast<double *>(smem + off + 96);
     int *s_runctr = reinterpret_cast<int *>(smem + off + 128);            // [b]: next column run of record set b (pipelined mode)
+    // FIN: [2 + bb] = 1 when the item whose geometry used tile buffer bb is followed by its reset item (one slot per trip
+    // parity: a slot is rewritten two trips later, after every thread has read it); the destination of record set b is the
+    // pointer at s_env2[b] + 6 (bytes 24..31 of the record set's int block)
+    int *s_split = s_runctr + 2;
 
     const int tid = threadIdx.x;
     // screen-row centre above the horizon, half_v - (d_v + 0.5) * pixel_size: the wall texel's row term (:184), pose independent
@@ -730,7 +741,9 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     // threads (gt = index among them) that synchronise among themselves: the whole CTA (__syncthreads), or -- pipelined
     // direct renderer -- the first kGeoThreads threads (named barrier 2) while every warp paints the previous env.
     // Tile buffer bb: loaded here (pipelined mode: the other buffer is being read by the pixel warps), or already requested by
-    // the previous call, which prefetches `next_e` into the other buffer after its own wait (sequential mode).
+    // the previous call, which prefetches `next_e` into the other buffer after its own wait (sequential mode).  FIN:
+    // geo_reset marks the reset item of (e, t).
+    bool geo_reset = false;
     auto geometry = [&](int64_t e, int t, int b, int bb, int gt, int gn, bool named, bool load_here, int64_t next_e) {
         auto gsync = [&]() { if (named) asm volatile("bar.sync 2, %0;" ::"n"(kGeoThreads) : "memory"); else __syncthreads(); };
         uint8_t *s_blob = (bb ? s_blob2[1] : s_blob2[0]);
@@ -743,7 +756,10 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
         if (gt == 0) { if (load_here) load_blob(e, bb); s_runctr[b] = 0; }
         mgb_mbar_wait(&s_bar[1 + bb], (blob_phase >> bb) & 1u);
         blob_phase ^= 1u << bb;
-        if (gt == 0 && next_e >= 0) load_blob(next_e, bb ^ 1);
+        // FIN, sequential: when env e finishes here its reset item comes next and needs e's tile, not next_e's; which one is
+        // known only after the step logic, so a prefetch of another env waits for it
+        const bool late = FIN && !load_here && !geo_reset && next_e != e;
+        if (gt == 0 && next_e >= 0 && !late) load_blob(next_e, bb ^ 1);
         const TaskHdr *th = blob_hdr(s_blob);
         // ---- step logic (one thread), then publish agent pose to the CTA
         if (FILL) {
@@ -763,31 +779,37 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                 double reward;
                 int done;
                 const int64_t o = ROLL ? (int64_t)t * a.n + e : e;       // [T][n] outputs and actions of a rollout
-                if (cont) {
-                    float tr, ws;
-                    if (ROLL && !a.act_c) {   // uniform on [-1, 1): 2 u - 1 is exact for every 24-bit u01
-                        const int64_t genv = a.env_base + e;
-                        const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
-                                                                     a.t_base + (uint32_t)t, MGB_STREAM_ACTION),
-                                                          make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32)));
-                        tr = 2.0f * mgb_u01(r.x) - 1.0f;
-                        ws = 2.0f * mgb_u01(r.y) - 1.0f;
-                        if (a.act_out_c) { a.act_out_c[2 * o] = tr; a.act_out_c[2 * o + 1] = ws; }
-                    } else {
-                        tr = a.act_c[2 * o]; ws = a.act_c[2 * o + 1];
-                    }
-                    continuous_move(c, s_blob, tr, ws, cp, co);
-                    const float csf = (float)th->cell_size;                 // get_loc_grid, maze_base.py:199-202
-                    s.gx = (int)(cp[0] / csf); s.gy = (int)(cp[1] / csf);
-                    maze_evaluate(c, s_blob, eaten, a.n_pad, s, reward, done);
+                bool split = false;                                      // FIN: terminal frame now, reset item next
+                if (FIN && geo_reset) {
+                    done = 1;                                            // the reset that the step logic of (e, t) deferred
                 } else {
-                    maze_logic(c, s_blob, eaten, a.n_pad, s, a.act[e], reward, done);
+                    if (cont) {
+                        float tr, ws;
+                        if (ROLL && !a.act_c) {   // uniform on [-1, 1): 2 u - 1 is exact for every 24-bit u01
+                            const int64_t genv = a.env_base + e;
+                            const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
+                                                                         a.t_base + (uint32_t)t, MGB_STREAM_ACTION),
+                                                              make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32)));
+                            tr = 2.0f * mgb_u01(r.x) - 1.0f;
+                            ws = 2.0f * mgb_u01(r.y) - 1.0f;
+                            if (a.act_out_c) { a.act_out_c[2 * o] = tr; a.act_out_c[2 * o + 1] = ws; }
+                        } else {
+                            tr = a.act_c[2 * o]; ws = a.act_c[2 * o + 1];
+                        }
+                        continuous_move(c, s_blob, tr, ws, cp, co);
+                        const float csf = (float)th->cell_size;                 // get_loc_grid, maze_base.py:199-202
+                        s.gx = (int)(cp[0] / csf); s.gy = (int)(cp[1] / csf);
+                        maze_evaluate(c, s_blob, eaten, a.n_pad, s, reward, done);
+                    } else {
+                        maze_logic(c, s_blob, eaten, a.n_pad, s, a.act[e], reward, done);
+                    }
+                    a.rew[o] = reward;
+                    a.done[o] = (uint8_t)done;
+                    if (a.truncated) a.truncated[o] = maze_truncated(c, s_blob, s);
+                    if (done && a.fin_count) push_terminal_state(c, a, e, s, eaten, make_float2(cp[0], cp[1]), co);
+                    split = FIN && done && a.final_obs && a.auto_reset;
                 }
-                a.rew[o] = reward;
-                a.done[o] = (uint8_t)done;
-                if (a.truncated) a.truncated[o] = maze_truncated(c, s_blob, s);
-                if (done && a.fin_count) push_terminal_state(c, a, e, s, eaten, make_float2(cp[0], cp[1]), co);
-                if (done && a.auto_reset) {
+                if (done && a.auto_reset && !split) {
                     env_reset(c, s_blob, eaten, a.n_pad, s);
                     if (cont) {
                         cp[0] = (float)(s.gx * th->cell_size + 0.5 * th->cell_size);
@@ -798,6 +820,13 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                 a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
                 a.life[e] = s.life;
                 if (cont) { a.cpos[e] = make_float2(cp[0], cp[1]); a.cori[e] = co; }
+                if (FIN) {
+                    s_split[bb] = split;
+                    *reinterpret_cast<uint8_t **>(s_env + 6) =
+                        reinterpret_cast<uint8_t *>(split ? a.final_obs : a.obs) + (size_t)o * H * V * px_bytes;
+                    const int64_t ne = split ? e : next_e;
+                    if (late && ne >= 0) load_blob(ne, bb ^ 1);
+                }
             }
             if (cont) {          // publish the pose: position promoted from float32, sin/cos of the float64 heading
                 s_pose[0] = (double)cp[0]; s_pose[1] = (double)cp[1]; s_pose[2] = sin(co); s_pose[3] = cos(co);
@@ -986,7 +1015,8 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
         int lb_ey = trunc_i(c.lb_sy + c.lb_w);
         if (lb_ey > V) lb_ey = V;
         const bool has_bar = c.task_type == MGB_MAZE_SURVIVAL;
-        uint8_t *gobs = reinterpret_cast<uint8_t *>(a.obs) + (size_t)(a.final_obs ? a.fin_env[e] : e) * total_px * px_bytes;
+        uint8_t *gobs = FIN ? *reinterpret_cast<uint8_t *const *>(s_env + 6)   // FIN: the record set's destination
+                            : reinterpret_cast<uint8_t *>(a.obs) + (size_t)(a.final_obs ? a.fin_env[e] : e) * total_px * px_bytes;
         const int lane = tid & 31, warp = tid >> 5, n_warps = blockDim.x >> 5;
         const double inv_cell = th->inv_cell, inv_t2c = th->inv_t2c;
         const bool cell_p2 = th->cell_pow2 != 0, t2c_p2 = th->t2c_pow2 != 0, text_p2 = c.text_pow2 != 0;
@@ -1301,6 +1331,35 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
             }
             __syncthreads();   // the record set / tile just painted from is rewritten next
             b ^= 1; bb ^= 1;   // pipelined: the set prepared in this trip is painted in the next one
+        }
+    } else if (FIN) {
+        // the same trips over items (env, t) and, after an item whose env finished, (env, t, reset).  The pixels of an item
+        // go where its record set says; whether the item just prepared is followed by its reset item is read after the
+        // trip's closing barrier from the slot of this trip's tile buffer, so that every thread takes the same next item.
+        int64_t e_geo = blockIdx.x;
+        int t_geo = 0;
+        bool pix = false;              // pipelined: the record set prepared in the previous trip is painted in this one
+        while (e_geo < a.n || (pipe && pix)) {
+            const bool geo = e_geo < a.n;
+            const bool last_t = t_geo + 1 == a.T;
+            const int64_t e_next = last_t ? e_geo + stride : e_geo;     // the next item unless e_geo finishes here
+            const int gslot = pipe ? b ^ 1 : bb;                        // tile buffer of this trip's geometry
+            if (geo && (!pipe || tid < kGeoThreads)) {
+                geometry(e_geo, t_geo, pipe ? b ^ 1 : 0, gslot, tid, pipe ? kGeoThreads : (int)blockDim.x, pipe, pipe,
+                         (!pipe && e_next < a.n) ? e_next : -1);
+            }
+            if (!pipe) {
+                if (!tex_ready) { mgb_mbar_wait(&s_bar[0], 0); tex_ready = true; }
+                __syncthreads();
+            }
+            if (pipe ? pix : geo) pixels(0, pipe ? b : 0, pipe ? b : bb, pipe);
+            __syncthreads();
+            b ^= 1; bb ^= 1;
+            pix = geo;
+            if (geo) {
+                if (!geo_reset && s_split[gslot]) geo_reset = true;
+                else { geo_reset = false; e_geo = e_next; t_geo = last_t ? 0 : t_geo + 1; }
+            }
         }
     } else {
         // the same trips over items (env, t): geometry of item (e_geo, t_geo), pixels of item (e_pix, t_pix) into frame
@@ -1824,11 +1883,18 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
 // T MetaMazeDiscrete3D steps in one launch (pose-cache path): one CTA per env; thread 0 runs the step logic and leaves the
 // env's EnvDyn in shared memory, then the whole CTA composes frame t straight into obs[t][env].  No logic launch, no
 // EnvDyn round trip through global memory, and the logic of one env overlaps the pixels of the others on the SM.
+// FIN (mgb_maze_rollout_discrete_ex): thread 0 also stores the truncation byte of every (t, env) and, for an env that
+// finished at step t, publishes the EnvDyn of its terminal state in a second slot -- both before env_reset, which clears the
+// food stamps the terminal frame still shows.  The CTA then composes that frame into final_obs + (t n + env) frame, a
+// barrier later the usual observation: one compose body, one deferred-tint queue, two passes.
+template <bool FIN>
 __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(const __grid_constant__ MazeConst c,
                                                                             const __grid_constant__ MazeArgs a)
 {
     __shared__ EnvDyn s_dyn;
     __shared__ int s_nslow;
+    __shared__ EnvDyn s_tdyn;                           // FIN: the terminal state's EnvDyn ...
+    __shared__ int s_term;                              // ... valid when 1 (done and final_obs wanted)
     extern __shared__ int s_slow[];                     // total_px / 4 entries: queued tinted groups of the current frame
     bool deferred_pass = false;
     const int H = c.res_h, V = c.res_v, total_px = H * V;
@@ -1861,6 +1927,11 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(cons
                 double reward;
                 int done;
                 maze_logic(c, eblob, eaten, a.n_pad, s, action, reward, done);
+                if (FIN) {
+                    if (a.truncated) a.truncated[(int64_t)t * a.n + env] = maze_truncated(c, eblob, s);
+                    s_term = done && a.final_obs;
+                    if (done && a.final_obs) s_tdyn = make_dyn(c, a, eblob, task, s, eaten);
+                }
                 if (done && a.auto_reset) env_reset(c, eblob, eaten, a.n_pad, s);
                 if (a.rew) a.rew[(int64_t)t * a.n + env] = reward;
                 if (a.done) a.done[(int64_t)t * a.n + env] = (uint8_t)done;
@@ -1868,7 +1939,26 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(cons
                 s_nslow = 0;
             }
             __syncthreads();
-            if (a.obs) {
+            if (FIN) {
+                // pass 0: the terminal frame (finished envs only), pass 1: the observation; both decisions are CTA-uniform
+                const bool term = s_term != 0;
+                for (int pass = term ? 0 : 1; pass < 2; ++pass) {
+                    void *dst = pass == 0 ? a.final_obs : a.obs;
+                    if (!dst) continue;
+                    if (pass == 1 && term) {                          // the queue of pass 0 has been read by every thread
+                        __syncthreads();
+                        if (threadIdx.x == 0) s_nslow = 0;
+                        __syncthreads();
+                    }
+                    const EnvDyn d = pass == 0 ? s_tdyn : s_dyn;
+                    const int64_t e = (int64_t)t * a.n + env;         // frame index of the included body
+                    const int q_begin = 0, q_end = total_px;
+#define MGB_COMPOSE_DEFER_SLOW 1
+#define MGB_COMPOSE_OBS dst
+#include "maze_compose_body.inc"
+#undef MGB_COMPOSE_DEFER_SLOW
+                }
+            } else if (a.obs) {
                 const EnvDyn d = s_dyn;
                 const int64_t e = (int64_t)t * a.n + env;             // frame index of the included body
                 const int q_begin = 0, q_end = total_px;
@@ -1989,7 +2079,8 @@ struct mgb_maze {
     int auto_reset = 0;
     bool has_task = false, has_tex = false;
     size_t smem3d = 0;
-    int render_attr_set[3] = {0, 0, 0};   // maze3d_kernel<false / true / rollout>: shared-memory opt-in raised by this handle
+    int render_attr_set[4] = {0, 0, 0, 0};   // maze3d_kernel<false / true / rollout / rollout with terminal frames>:
+                                             // shared-memory opt-in raised by this handle
     int compose_ctas_per_sm = 0;       // occupancy of maze3d_compose_kernel (queried once per handle)
     int compose_persistent = -1;       // MGB_COMPOSE_PERSISTENT
     int num_sms = 0;
@@ -2836,7 +2927,7 @@ template <class F> static cudaError_t maze_allow_max_dynamic_smem(F *kernel)
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
 }
 
-template <bool FILL, bool ROLL = false>
+template <bool FILL, bool ROLL = false, bool FIN = false>
 static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStream_t st)
 {
     MazeConst &c = h->c;
@@ -2873,13 +2964,13 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
     }
     // The opt-in limit is a property of the kernel on a device, shared by every handle: each handle raises it once to the
     // device maximum (the same value from every handle and thread, so there is no ordering to get wrong and no global state).
-    const int attr = ROLL ? 2 : (FILL ? 1 : 0);
+    const int attr = FIN ? 3 : (ROLL ? 2 : (FILL ? 1 : 0));
     if (!h->render_attr_set[attr]) {
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL, FIN>));
         h->render_attr_set[attr] = 1;
     }
     h->smem3d = sm;
-    maze3d_kernel<FILL, ROLL><<<grid, kRenderThreads, sm, st>>>(c, a2);
+    maze3d_kernel<FILL, ROLL, FIN><<<grid, kRenderThreads, sm, st>>>(c, a2);
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -3202,14 +3293,17 @@ extern "C" int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_de
 
 static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
                    void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
-                   void *stream)
+                   void *stream, bool discrete_ex = false)
 {
     MGB_REQUIRE(h, "null handle");
     MGB_REQUIRE(T > 0, "T must be positive");
+    if (discrete_ex)
+        MGB_REQUIRE(h->c.kind == MGB_MAZE_DISCRETE_3D, "mgb_maze_rollout_discrete_ex needs a MGB_MAZE_DISCRETE_3D handle");
     MGB_REQUIRE(h->c.kind == MGB_MAZE_2D || h->c.kind == MGB_MAZE_DISCRETE_3D,
                 "mgb_maze_rollout serves MetaMaze2D and MetaMazeDiscrete3D");
     const bool fin = final_obs_dev || truncated_dev;
-    MGB_REQUIRE(!fin || h->c.kind == MGB_MAZE_2D, "final_obs / truncated of a rollout are produced for MetaMaze2D only");
+    MGB_REQUIRE(!fin || discrete_ex || h->c.kind == MGB_MAZE_2D,
+                "final_obs / truncated of a rollout are produced for MetaMaze2D only");
     MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
     MGB_REQUIRE(!fin || h->mir.count == 0,
                 "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
@@ -3236,12 +3330,21 @@ static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_
         a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask;
         a.c_vbase = h->c_vbase; a.c_var8 = h->c_var8; a.pose_rec = h->pose_rec;
         a.bake = 0;
-        const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers, no spills
+        const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers
         const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
         MGB_REQUIRE(qbytes <= 200 * 1024, "screen too large for the fused rollout's group queue");
-        if (qbytes > 40 * 1024)
-            MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel));
-        maze3d_rollout_kernel<<<(unsigned)(h->n < resident ? h->n : resident), kComposeThreads, qbytes, st>>>(h->c, a);
+        const unsigned grid = (unsigned)(h->n < resident ? h->n : resident);
+        if (fin) {
+            if (qbytes > 40 * 1024)
+                MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<true>));
+            a.final_obs = final_obs_dev;
+            a.truncated = truncated_dev;
+            maze3d_rollout_kernel<true><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
+        } else {
+            if (qbytes > 40 * 1024)
+                MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<false>));
+            maze3d_rollout_kernel<false><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
+        }
         MGB_CUDA(cudaGetLastError());
         h->t_base += (uint32_t)T;
         h->launches += 1;
@@ -3287,6 +3390,15 @@ extern "C" int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_de
     MgbRange nvtx_range("mgb_maze_rollout_ex");
     return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
                    stream);
+}
+
+extern "C" int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
+                                            int32_t *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                            void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_discrete_ex");
+    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
+                   stream, true);
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)
@@ -3349,6 +3461,31 @@ extern "C" int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, vo
     return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
 }
 
+// Launch of the continuous-maze rollout once its entry point has checked the arguments (each entry point checks them
+// itself, so that every refusal names the call that made it).  With final_obs or truncated: maze3d_kernel<.., FIN>.
+static int rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
+                              void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                              uint8_t *truncated_dev, void *stream)
+{
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    a.act_c = act_dev; a.act_out_c = act_out_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
+    const unsigned grid = (unsigned)(h->n < h->num_sms ? h->n : h->num_sms);
+    int rc;
+    if (final_obs_dev || truncated_dev) {
+        a.final_obs = final_obs_dev;
+        a.truncated = truncated_dev;
+        rc = launch_render<false, true, true>(h, a, grid, (cudaStream_t)stream);
+    } else {
+        rc = launch_render<false, true>(h, a, grid, (cudaStream_t)stream);
+    }
+    if (rc) return rc;
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return MGB_OK;
+}
+
 extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
                                            float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                                            void *stream)
@@ -3361,15 +3498,26 @@ extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *
     int rc = maze_ready(h);
     if (rc) return rc;
     MGB_REQUIRE(h->mir.count == 0, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    a.act_c = act_dev; a.act_out_c = act_out_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
-    rc = launch_render<false, true>(h, a, (unsigned)(h->n < h->num_sms ? h->n : h->num_sms), (cudaStream_t)stream);
+    return rollout_continuous(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
+}
+
+extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
+                                              float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                              void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_continuous_ex");
+    MGB_REQUIRE(h, "null handle");
+    MGB_REQUIRE(T > 0, "T must be positive");
+    MGB_REQUIRE(obs_dev && rew_dev && done_dev, "null argument");
+    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_rollout_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle");
+    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
+    MGB_REQUIRE(!(final_obs_dev || truncated_dev) || h->mir.count == 0,
+                "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
+    int rc = maze_ready(h);
     if (rc) return rc;
-    h->t_base += (uint32_t)T;
-    h->launches += 1;
-    return MGB_OK;
+    MGB_REQUIRE(h->mir.count == 0, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
+    return rollout_continuous(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev,
+                              truncated_dev, stream);
 }
 
 __global__ void maze_pose_kernel(MazeArgs a, float *pos_out, double *ori_out)

@@ -410,8 +410,9 @@ class _BatchedMazeBase(object):
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done_bool), info
 
-    def _rollout(self, T, actions, act_seed, want_actions, out, final=False):
-        """final: also produce the "final_obs" / "truncated" entries (MetaMaze2D with final_obs=True)."""
+    def _rollout(self, T, actions, act_seed, want_actions, out, final=False, entry="mgb_maze_rollout_ex"):
+        """final: also produce the "final_obs" / "truncated" entries through `entry` (mgb_maze_rollout_ex for MetaMaze2D,
+        mgb_maze_rollout_discrete_ex for MetaMazeDiscrete3D)."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -430,12 +431,18 @@ class _BatchedMazeBase(object):
                                                   _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
                                                   _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")), self._stream()))
         else:
-            _lib.check(self._lib.mgb_maze_rollout_ex(self._h, int(T), _lib.ptr(a), int(act_seed),
-                                                     _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
-                                                     _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
-                                                     _lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated")),
-                                                     self._stream()))
+            _lib.check(getattr(self._lib, entry)(self._h, int(T), _lib.ptr(a), int(act_seed),
+                                                 _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
+                                                 _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
+                                                 _lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated")),
+                                                 self._stream()))
         return out
+
+    def _check_rollout_final(self, final_obs):
+        """rollout(..., final_obs=True) of the 3-D envs: the constructor's rule, per call."""
+        if final_obs and not self.auto_reset:
+            raise ValueError("final_obs=True needs auto_reset=True (without auto-reset obs already is the terminal frame)")
+        return bool(final_obs)
 
     def agent_state(self):
         """-> (agent [N,4] int32 = grid_x, grid_y, ori_index, steps ; life [N] float64)."""
@@ -573,11 +580,18 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         cfg.l_focal, cfg.text_size = 0.20, 1.0                                # maze_discrete_3d.py:116
         return cfg
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
-        """T steps in one launch on the pose cache: obs [T,N,res_h,res_v,3] (uint8 or int32), rew, done, act as for
-        BatchedMetaMaze2D.rollout.  It does not return "final_obs" or "truncated", even with final_obs=True (those
-        are step() outputs here)."""
-        return self._rollout(T, actions, act_seed, want_actions, out)
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False):
+        """T steps in one launch on the pose cache: obs [T,N,res_h,res_v,3] (uint8, int32 or float32), rew, done, act as
+        for BatchedMetaMaze2D.rollout.
+
+        final_obs (per call, independent of the constructor's final_obs, which concerns step()): False returns only the
+        entries above.  True needs auto_reset=True (ValueError otherwise) and calls mgb_maze_rollout_discrete_ex: the
+        dict also holds "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e
+        if done[t, e] (what step() reports as final_observation; allocated with torch.empty, rows with done 0 are not
+        written), and "truncated" [T,N] uint8, written for every step: 1 iff done and the episode ended only through
+        max_steps.  A caller-supplied `out` may omit either entry, and that output is then not produced."""
+        final = self._check_rollout_final(final_obs)
+        return self._rollout(T, actions, act_seed, want_actions, out, final=final, entry="mgb_maze_rollout_discrete_ex")
 
     def cache_info(self):
         """Pose-cache statistics (valid after the first reset()/step()): dict(poses, variant_frames, variant_bits, bytes,
@@ -636,12 +650,18 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done.view(torch.bool)), info
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False):
         """T steps in one launch of the direct renderer (mgb_maze_rollout_continuous), exactly as T step() calls.
         actions: anything reshapeable to [T,N,2] (turn_rate, walk_speed), clipped to [-1, 1] like step(); None draws them
         on the device, uniform on [-1, 1) like action_space.sample().  Returns dict(obs [T,N,res_h,res_v,3] in the env's
         obs dtype, rew [T,N] f64, done [T,N] u8, act [T,N,2] f32: the drawn actions when want_actions, else None).
-        It does not return "final_obs" or "truncated", even with final_obs=True (those are step() outputs here)."""
+
+        final_obs (per call, independent of the constructor's final_obs, which concerns step()): True needs
+        auto_reset=True (ValueError otherwise) and calls mgb_maze_rollout_continuous_ex: the dict also holds
+        "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e if done[t, e]
+        (allocated with torch.empty, rows with done 0 are not written), and "truncated" [T,N] uint8, written for every
+        step.  A caller-supplied `out` may omit either entry, and that output is then not produced."""
+        final = self._check_rollout_final(final_obs)
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -652,13 +672,22 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
                    "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
                    "act": torch.empty((T, N, 2), dtype=torch.float32, device=dev)
                    if want_actions and actions is None else None}
+            if final:
+                out["final_obs"] = torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
         a = None
         if actions is not None:
             a = torch.as_tensor(actions, dtype=torch.float32, device=dev).reshape(T, N, 2).contiguous()
         drawn = out.get("act") if a is None else None
-        _lib.check(self._lib.mgb_maze_rollout_continuous(self._h, T, _lib.ptr(a), int(act_seed), _lib.ptr(drawn),
-                                                         _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
-                                                         _lib.ptr(out.get("done")), self._stream()))
+        if not final:
+            _lib.check(self._lib.mgb_maze_rollout_continuous(self._h, T, _lib.ptr(a), int(act_seed), _lib.ptr(drawn),
+                                                             _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
+                                                             _lib.ptr(out.get("done")), self._stream()))
+        else:
+            _lib.check(self._lib.mgb_maze_rollout_continuous_ex(self._h, T, _lib.ptr(a), int(act_seed), _lib.ptr(drawn),
+                                                                _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
+                                                                _lib.ptr(out.get("done")), _lib.ptr(out.get("final_obs")),
+                                                                _lib.ptr(out.get("truncated")), self._stream()))
         return out
 
     def pose(self):

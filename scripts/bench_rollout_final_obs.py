@@ -1,5 +1,6 @@
 """Cost of the terminal observations and truncation flags of the fused rollouts (mgb_quad_rollout_ex,
-mgb_maze_rollout_ex) and of the quadrotor step's truncation flag (mgb_quad_step_ex).
+mgb_maze_rollout_ex, mgb_maze_rollout_discrete_ex, mgb_maze_rollout_continuous_ex) and of the quadrotor step's truncation
+flag (mgb_quad_step_ex).
 
 Two handles per case, final_obs off and on, same configuration and seeds.  Each arm replays a CUDA graph, like bench.py:
 one rollout of T steps (device-drawn actions), or T single steps for the step case.  The arms alternate for --runs runs
@@ -8,7 +9,11 @@ step of the "on" arm, and the card's name and power limit.  One JSON line per ca
   quad_hover_nt1000 / quad_hover_nt50   hovering_control, 65 536 envs, rollout T = 32, nt = 1000 / 50
   quad_velocity                          velocity_control, dt = 0.005, 65 536 envs, rollout T = 32
   quad_step                              the 65 536-env velocity_control step (dt = 0.005), without / with truncated
-  maze2d_max200 / maze2d_max10           MetaMaze2D, 16 384 envs, view_grid = 1, ESCAPE, rollout T = 32"""
+  maze2d_max200 / maze2d_max10           MetaMaze2D, 16 384 envs, view_grid = 1, ESCAPE, rollout T = 32
+  maze3d_max200 / maze3d_max10           MetaMazeDiscrete3D (pose cache), 1024 envs, 64 tasks, 128x128 uint8, SURVIVAL,
+                                         rollout T = 32 (the shape of bench.py --workload maze3d)
+  cont3d_max200 / cont3d_max10           MetaMazeContinuous3D, the same shape (direct renderer)
+For the 3-D cases both arms are the same kind of handle; "on" calls rollout(..., final_obs=True)."""
 import argparse
 import json
 import os
@@ -20,7 +25,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 import torch
-from metagym_b200 import BatchedMetaMaze2D, BatchedQuadrotor, MazeTaskSampler
+from metagym_b200 import (BatchedMetaMaze2D, BatchedMetaMazeContinuous3D, BatchedMetaMazeDiscrete3D, BatchedQuadrotor,
+                          MazeTaskSampler)
 
 
 def power_limit_w():
@@ -48,13 +54,18 @@ def make(case, final_obs, tasks):
         env = BatchedMetaMaze2D(view_grid=1, task_type="ESCAPE", num_envs=16384, squeeze=False, auto_reset=True,
                                 final_obs=final_obs, **kw)
         env.set_task(tasks)
+    elif kind in ("maze3d", "cont3d"):
+        cls = BatchedMetaMazeDiscrete3D if kind == "maze3d" else BatchedMetaMazeContinuous3D
+        env = cls(resolution=(128, 128), obs_dtype="uint8", task_type="SURVIVAL", num_envs=1024, squeeze=False,
+                  auto_reset=True, **kw)
+        env.set_task(tasks)
     else:
         env = BatchedQuadrotor(num_envs=65536, squeeze=False, auto_reset=True, rng_seed=3, final_obs=final_obs, **kw)
     env.reset()
     return env
 
 
-def capture(case, env, T):
+def capture(case, env, T, final_obs):
     """-> (graph, count): count() = number of done flags over the T steps of the graph's last replay (the step case
     counts them on T eager steps, so that its graph holds nothing but the steps)."""
     if case == "quad_step":
@@ -68,11 +79,12 @@ def capture(case, env, T):
             for t in range(T):
                 env.step(acts[t])
         return graph, lambda: sum(int(env.step(acts[t])[2].sum()) for t in range(T))
-    out = env.rollout(T, act_seed=7)                         # warm-up; its buffers are the graph's
+    kw = {"final_obs": True} if final_obs and CASES[case][0] in ("maze3d", "cont3d") else {}
+    out = env.rollout(T, act_seed=7, **kw)                   # warm-up; its buffers are the graph's
     torch.cuda.synchronize()
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        env.rollout(T, act_seed=7, out=out)
+        env.rollout(T, act_seed=7, out=out, **kw)
     return graph, lambda: int(out["done"].sum())
 
 
@@ -83,6 +95,10 @@ CASES = {
     "quad_step": ("quad", {"task": "velocity_control", "dt": 0.005, "seed": list(range(64))}),
     "maze2d_max200": ("maze", {"max_steps": 200}),
     "maze2d_max10": ("maze", {"max_steps": 10}),
+    "maze3d_max200": ("maze3d", {"max_steps": 200}),
+    "maze3d_max10": ("maze3d", {"max_steps": 10}),
+    "cont3d_max200": ("cont3d", {"max_steps": 200}),
+    "cont3d_max10": ("cont3d", {"max_steps": 10}),
 }
 
 
@@ -90,7 +106,7 @@ def run_case(case, T, K, runs, tasks):
     envs, graphs, dones = {}, {}, {}
     for arm in ("off", "on"):
         env = make(case, arm == "on", tasks)
-        graphs[arm], dones[arm] = capture(case, env, T)
+        graphs[arm], dones[arm] = capture(case, env, T, arm == "on")
         envs[arm] = env
 
     def runner(arm):

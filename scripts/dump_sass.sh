@@ -14,11 +14,11 @@ for line in sys.stdin:
     if line.strip():
         print(line)
 ' > /tmp/mgb_all.sass
-for k in quad_step_wide_kernel quad_stream_kernel quad_step2_kernel quad_rollout_kernel maze3d_step_kernel maze3d_compose_kernel maze3d_kernel; do
+for k in quad_step_wide_kernel quad_stream_kernel quad_step2_kernel quad_rollout_kernel maze3d_step_kernel maze3d_compose_kernel maze3d_rollout_kernel maze3d_kernel; do
     f="profiles/sass/${pfx}_$k.sass"
     awk -v k="$k" '/Function : /{f = index($0, k "I") > 0 || index($0, k "E") > 0} f' /tmp/mgb_all.sass > "$f"
     echo "$k: $(grep -c 'Function : ' $f) instantiation(s), $(wc -l < $f) lines;" \
          "UBLKCP $(grep -c UBLKCP $f || true), SYNCS $(grep -c SYNCS $f || true)," \
          "DFMA/DMUL/DADD $(grep -cE 'DFMA|DMUL|DADD' $f || true)"
 done | tee "profiles/sass/${pfx}_summary.txt"
-for k in quad_step2_kernel quad_rollout_kernel maze3d_compose_kernel maze3d_kernel; do gzip -nf "profiles/sass/${pfx}_$k.sass"; done
+for k in quad_step2_kernel quad_rollout_kernel maze3d_compose_kernel maze3d_rollout_kernel maze3d_kernel; do gzip -nf "profiles/sass/${pfx}_$k.sass"; done
