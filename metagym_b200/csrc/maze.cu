@@ -30,7 +30,7 @@ constexpr int kMaxN = 31;
 constexpr int kNever = INT_MIN / 2;
 constexpr int kRenderThreads = 512;
 constexpr int kGeoThreads = 128;            // direct renderer, pipelined: threads that prepare the next env's records
-constexpr int kMaxHitsCap = 48;
+constexpr int kMaxHitsCap = 2 * kMaxN - 1;   // a ray enters at most 2 n - 1 cells of an n x n grid
 
 struct TaskHdr {                 // 112 bytes, head of every task blob
     int32_t start[2], goal[2];
@@ -1578,7 +1578,8 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
     int lb_ey = trunc_i(c.lb_sy + c.lb_w);
     if (lb_ey > V) lb_ey = V;
     const int px_bytes = c.obs_dtype == MGB_OBS_U8 ? 3 : 12;
-    const int part_px = ((total_px / kParts) + 127) / 128 * 128;          // slice boundaries stay 128-pixel aligned
+    // slice boundaries stay 128-pixel aligned; the slices cover the frame even when it has fewer pixels than slices
+    const int part_px = ((total_px + kParts - 1) / kParts + 127) / 128 * 128;
   // list pass of mgb_maze_step_ex (final_obs set): item = (terminal list entry, slice), frame into final_obs[fin_env[entry]]
   const int64_t n_items = (a.final_obs ? (int64_t)*a.fin_count : a.n) * kParts;
   // bake mode (pose-cache build): item = pose slot, every food present, no life bar, tintable groups only
@@ -2038,6 +2039,7 @@ struct mgb_maze {
     int fused_step = 1;            // MGB_MAZE_FUSED_STEP=0: logic kernel + compose kernel instead of maze3d_step_kernel
     size_t step_smem_set = 0, m2d_smem_set = 0;
     int cache_enabled = 1;         // MGB_MAZE_CACHE=0 disables (direct renderer only)
+    int tex_max = 255;             // brightest channel value of the loaded textures
     double cache_budget_gb = 24.0; // MGB_MAZE_CACHE_GB
     bool cache_ready = false, cache_dirty = true;
     int64_t n_poses = 0;
@@ -2323,6 +2325,9 @@ extern "C" int mgb_maze_set_textures(mgb_maze *h, const uint8_t *grounds_host, i
     MGB_CUDA(cudaMalloc(&h->tex, packed.size() * 4));
     MGB_CUDA(cudaMemcpy(h->tex, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice));
     h->c.n_tex = n_tex; h->c.ts = tex_size;
+    h->tex_max = 0;
+    for (size_t i = 0; i < 3 * (size_t)n_tex * px; ++i) h->tex_max = grounds_host[i] > h->tex_max ? grounds_host[i] : h->tex_max;
+    for (size_t i = 0; i < 3 * px; ++i) h->tex_max = ceil_host[i] > h->tex_max ? ceil_host[i] : h->tex_max;
     h->has_tex = true;
     h->cache_dirty = true;
     return MGB_OK;
@@ -2412,12 +2417,14 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     }
     c.f_max = f_max;
     // A ray is followed for max_vision at most, i.e. through <= 2 * max_vision / cell_size + 2 cells (one per DDA step
-    // plus the start cell): that bounds the transparent crossings a column can record (ray_caster_utils.py:24-61).
+    // plus the start cell), and it moves monotonically in i and j, so it enters at most 2 n - 1 cells of the grid: both
+    // bound the transparent crossings a column records (ray_caster_utils.py:24-61), and the reference blends every one.
     double min_cell = scalars_host[0].cell_size;
     for (int t = 1; t < n_tasks; ++t) min_cell = scalars_host[t].cell_size < min_cell ? scalars_host[t].cell_size : min_cell;
     h->min_cell = min_cell;
     const int geo = (int)ceil(2.0 * c.max_vision / min_cell) + 3;
     int mh = f_max < geo ? f_max : geo;
+    mh = mh < 2 * n - 1 ? mh : 2 * n - 1;
     if (mh < 1) mh = 1;
     if (c.task_type == MGB_MAZE_ESCAPE) mh = 2;
     c.max_hits = mh > kMaxHitsCap ? kMaxHitsCap : mh;
@@ -2986,7 +2993,11 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     const size_t slots = h->host_poses.size(), px = (size_t)c.res_h * c.res_v;
     const double bytes = (double)slots * (px * (c.obs_dtype == MGB_OBS_U8 ? 8.0 : 12.0) + px / 4.0 + 16.0 +
                                           c.res_h * (1.0 + (double)c.max_hits * sizeof(HitRec)));
-    if (bytes > h->cache_budget_gb * 1e9) { h->cache_dirty = false; h->cache_would_fit = false; return MGB_OK; }   // a decision, not a failure
+    // c_px packs 10 bits per channel.  Floor and ceiling texels are lit by v_screen / l_focal (ray_caster_utils.py:99,132),
+    // up to (half_v - pixel_size / 2) / l_focal; times the brightest texel that can pass 1023 on tall screens, and those
+    // screens render directly.
+    const bool packs = (c.half_v - 0.5 * c.pixel_size) / c.l_focal * h->tex_max < 1024.0;
+    if (bytes > h->cache_budget_gb * 1e9 || !packs) { h->cache_dirty = false; h->cache_would_fit = false; return MGB_OK; }   // a decision, not a failure
     // From here on a failure (capture in progress, out of memory) leaves cache_dirty set: the next call retries instead of
     // silently rendering every frame with the slow direct renderer (round-1 advice).
     // cudaMalloc/cudaFree synchronise; a capture in progress cannot build the cache

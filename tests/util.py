@@ -73,6 +73,10 @@ MazeTask = namedtuple("MazeTask", ["start", "goal", "cell_walls", "cell_texts", 
                                    "agent_height", "initial_life", "max_life", "step_reward", "goal_reward",
                                    "food_rewards", "food_interval"])
 MAZE_CASES = ["m2d_surv", "m2d_surv_g2", "m2d_esc", "m3d_surv", "m3d_esc", "m3d_big"]
+# tests/golden/maze_optics_golden.npz (gen_maze_optics.py): non-default vision range / field of view, odd, tall and
+# degenerate screens, and an arena with more transparent crossings per column than any sampled task
+OPTICS_CASES = ["o3d_near", "o3d_wide", "o3d_esc", "o3d_tall", "o3d_dot1", "o3d_dot3", "xings"]
+OPTICS_CONT_CASES = ["oc3d", "xings_c"]
 
 
 def task_from_arrays(walls, texts, food, interval, scalars):
@@ -94,6 +98,11 @@ def maze_case(g, name):
     d["task"] = task_from_arrays(d["task.walls"], d["task.texts"], d["task.food"], d["task.interval"],
                                  d["task.scalars"])
     return d
+
+
+def optics_kw(c):
+    """OracleMaze keyword arguments of a case's optics (the reference defaults when the fixture has none)."""
+    return {} if "optics" not in c else dict(max_vision=float(c["optics"][0]), fov=float(c["optics"][1]))
 
 
 def cont_case(g, name):
