@@ -321,12 +321,17 @@ __device__ void continuous_move(const MazeConst &c, const uint8_t *blob, float t
 // ---------------------------------------------------------------------------------------------------------------
 // state-only kernels
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void maze_reset_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a)
+// Envs start a new episode: every env, or only those with a.mask[e] set, or (task_flags) only those whose task-table slot
+// was just replaced (set_task leaves an env at its start state, maze_env.py:44-50).
+__global__ void maze_reset_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a,
+                                  const uint8_t *task_flags)
 {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.n) return;
     if (a.mask && !a.mask[e]) return;
-    const uint8_t *blob = a.blobs + (int64_t)a.env2task[e] * c.blob_bytes;
+    const int task = a.env2task[e];
+    if (task_flags && !task_flags[task]) return;
+    const uint8_t *blob = a.blobs + (int64_t)task * c.blob_bytes;
     Env s;
     env_reset(c, blob, a.eaten + e, a.n_pad, s);
     a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
@@ -1725,14 +1730,12 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
     const int tid = threadIdx.x, lane = tid & 31;
     const bool warp0 = tid < 32;
     const int v_shift = (V & (V - 1)) == 0 ? 31 - __clz(V) : -1;
-    asm volatile("griddepcontrol.launch_dependents;");
     if (tid == 0) {
         for (int k = 0; k < kStepSlots; ++k) { mgb_mbar_init(&s_bar[k], 1); mgb_mbar_init(&s_empty[k], 1); }
         mgb_fence_mbar_init();
         s_nslow = 0;
         s_nterm[0] = s_nterm[1] = 0;
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
     __syncthreads();
     uint32_t g0 = 0;                                             // chunks this CTA has moved in earlier passes (ring position)
     int pass = 0;
@@ -2034,7 +2037,6 @@ struct mgb_maze {
     double *cori = nullptr;
     double *coltab_d = nullptr;
     // pose cache
-    int step_pdl = 0;              // MGB_MAZE_PDL=1: programmatic dependent launch between consecutive fused steps
     int render_pipe = 1;           // MGB_MAZE_RENDER_PIPE=0: direct renderer without the geometry / pixel software pipeline
     int fused_step = 1;            // MGB_MAZE_FUSED_STEP=0: logic kernel + compose kernel instead of maze3d_step_kernel
     size_t step_smem_set = 0, m2d_smem_set = 0;
@@ -2084,7 +2086,6 @@ struct mgb_maze {
     int render_attr_set[4] = {0, 0, 0, 0};   // maze3d_kernel<false / true / rollout / rollout with terminal frames>:
                                              // shared-memory opt-in raised by this handle
     int compose_ctas_per_sm = 0;       // occupancy of maze3d_compose_kernel (queried once per handle)
-    int compose_persistent = -1;       // MGB_COMPOSE_PERSISTENT
     int num_sms = 0;
     int64_t launches = 0;
     uint32_t t_base = 0;
@@ -2096,7 +2097,6 @@ struct mgb_maze {
     int4 *fin_agent = nullptr;
     double *fin_life = nullptr, *fin_cori = nullptr;
     float2 *fin_cpos = nullptr;
-    bool list_pending = false;   // the last launch_observe left terminal states in the list
 };
 
 static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
@@ -2120,17 +2120,16 @@ static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
     return off;
 }
 
-static MazeArgs maze_args(const mgb_maze *h);
-static MazeArgs maze_args_impl(const mgb_maze *h);
-static MazeArgs maze_args(const mgb_maze *h)
+// The pose-cache tables of h, into args filled before ensure_pose_cache (re)built them
+static void bind_pose_cache(const mgb_maze *h, MazeArgs &a)
 {
-    MazeArgs a = maze_args_impl(h);
-    a.c_vbase = h->c_vbase;
-    a.pose_rec = h->pose_rec;
-    a.c_var8 = h->c_var8;
-    return a;
+    a.poses = h->poses; a.pose_index = h->pose_index; a.pose_rec = h->pose_rec; a.c_px = h->c_px; a.c_fid = h->c_fid;
+    a.c_colhits = h->c_colhits; a.c_hits = h->c_hits; a.dyn = h->dyn; a.c_rgb8 = h->c_rgb8; a.c_gsig = h->c_gsig;
+    a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask; a.c_vbase = h->c_vbase; a.c_var8 = h->c_var8;
 }
-static MazeArgs maze_args_impl(const mgb_maze *h)
+
+// Kernel arguments of the handle's state; every per-call field is zero
+static MazeArgs maze_args(const mgb_maze *h)
 {
     MazeArgs a;
     memset(&a, 0, sizeof(a));
@@ -2138,9 +2137,7 @@ static MazeArgs maze_args_impl(const mgb_maze *h)
     a.agent = h->agent; a.life = h->life; a.eaten = h->eaten; a.env2task = h->env2task; a.blobs = h->blobs;
     a.tex = h->tex; a.coltab = h->coltab; a.efftab = h->efftab; a.fogtab = h->fogtab; a.auto_reset = h->auto_reset;
     a.cpos = h->cpos; a.cori = h->cori; a.coltab_d = h->coltab_d;
-    a.poses = h->poses; a.pose_index = h->pose_index; a.c_px = h->c_px; a.c_fid = h->c_fid;
-    a.c_colhits = h->c_colhits; a.c_hits = h->c_hits; a.dyn = h->dyn; a.c_rgb8 = h->c_rgb8; a.c_gsig = h->c_gsig;
-    a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask;
+    bind_pose_cache(h, a);
     return a;
 }
 
@@ -2183,7 +2180,6 @@ extern "C" int mgb_maze_create(mgb_maze **out, int64_t n_envs, const mgb_maze_cf
     MGB_CUDA(cudaGetDeviceProperties(&prop, device));
     h->num_sms = prop.multiProcessorCount;
     if (const char *ev = getenv("MGB_MAZE_FUSED_STEP")) h->fused_step = atoi(ev) != 0;
-    if (const char *ev = getenv("MGB_MAZE_PDL")) h->step_pdl = atoi(ev) != 0;
     if (const char *ev = getenv("MGB_MAZE_RENDER_PIPE")) h->render_pipe = atoi(ev) != 0;
     if (const char *ev = getenv("MGB_MAZE_VARIANT_BITS")) {
         h->variant_bits = atoi(ev);
@@ -2520,7 +2516,7 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     }
     // set_task leaves the env in "need reset" state (maze_env.py:44-50): initialise it so a stray step is harmless
     MazeArgs a = maze_args(h);
-    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(c, a);
+    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(c, a, nullptr);
     MGB_CUDA(cudaDeviceSynchronize());
     h->launches += 1;
     return MGB_OK;
@@ -2727,26 +2723,6 @@ __global__ void maze_scatter_tasks_kernel(const __grid_constant__ MazeConst c, u
     for (int i = threadIdx.x; i < c.blob_bytes / 16; i += blockDim.x) dst[i] = src[i];
     if (threadIdx.x == 0) task_flags[slots[blockIdx.x]] = 1;
 }
-// envs whose task was replaced start a new episode on it (set_task leaves an env at its start state, maze_env.py:44-50)
-__global__ void maze_reset_flagged_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a,
-                                          const uint8_t *task_flags)
-{
-    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= a.n) return;
-    const int task = a.env2task[e];
-    if (!task_flags[task]) return;
-    const uint8_t *blob = a.blobs + (int64_t)task * c.blob_bytes;
-    Env s;
-    env_reset(c, blob, a.eaten + e, a.n_pad, s);
-    a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
-    a.life[e] = s.life;
-    if (c.kind == MGB_MAZE_CONTINUOUS_3D) {             // get_cell_center(start), heading 0 (maze_base.py:41,50)
-        const TaskHdr *th = blob_hdr(blob);
-        a.cpos[e] = make_float2((float)(s.gx * th->cell_size + 0.5 * th->cell_size),
-                                (float)(s.gy * th->cell_size + 0.5 * th->cell_size));
-        a.cori[e] = 0.0;
-    }
-}
 __global__ void maze_clear_flags_kernel(uint8_t *task_flags, int n)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2815,7 +2791,7 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     MGB_CUDA(cudaEventRecord(h->stage_done[sb], st));
     maze_scatter_tasks_kernel<<<(unsigned)count, 128, 0, st>>>(c, h->blobs, h->d_stage[sb], count, h->task_flags);
     MazeArgs a = maze_args(h);
-    maze_reset_flagged_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(c, a, h->task_flags);
+    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(c, a, h->task_flags);
     maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags, h->n_tasks);
     MGB_CUDA(cudaGetLastError());
     h->launches += 3;
@@ -3139,20 +3115,33 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
 }
 
 // Paths other than the fused step keep their terminal states in a list (mgb_maze_step_ex): clear its length, and leave
-// a.final_obs to the list pass, which step_ex launches after the step.
-static int start_terminal_list(mgb_maze *h, MazeArgs &a, cudaStream_t st)
+// a.final_obs to the list pass, which step_ex launches after the step.  `listed`: a list was started.
+static int start_terminal_list(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t st)
 {
-    h->list_pending = a.fin_count != nullptr;
+    listed = a.fin_count != nullptr;
     a.final_obs = nullptr;
-    if (!a.fin_count) return MGB_OK;
+    if (!listed) return MGB_OK;
     MGB_CUDA(cudaMemsetAsync(a.fin_count, 0, sizeof(int32_t), st));
     h->launches += 1;
     return MGB_OK;
 }
 
-static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
+// Resident CTAs of maze3d_compose_kernel on the handle's device (occupancy queried once per handle)
+static int64_t compose_resident_ctas(mgb_maze *h)
 {
-    h->list_pending = false;
+    int &ctas_per_sm = h->compose_ctas_per_sm;
+    if (!ctas_per_sm) {
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, maze3d_compose_kernel, kComposeThreads, 0) !=
+                cudaSuccess || ctas_per_sm < 1) ctas_per_sm = 4;
+    }
+    return (int64_t)h->num_sms * ctas_per_sm;
+}
+
+// Observe (a.do_step = 0) or step then observe every env.  `listed`: the step left its finished envs' terminal states in
+// the list for step_ex's list pass.
+static int launch_observe(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t st)
+{
+    listed = false;
     const MazeConst &c = h->c;
     if (c.kind == MGB_MAZE_2D) {
         const int W = 2 * c.view_grid + 1;
@@ -3168,10 +3157,7 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
         if (rc) return rc;
         if (h->cache_ready) {
             // memoised path: integer step logic, then compose static pose layers with the current food state
-            a.poses = h->poses; a.pose_index = h->pose_index; a.c_px = h->c_px; a.c_fid = h->c_fid;
-            a.c_colhits = h->c_colhits; a.c_hits = h->c_hits; a.dyn = h->dyn; a.c_rgb8 = h->c_rgb8; a.c_gsig = h->c_gsig;
-            a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask;
-            a.c_vbase = h->c_vbase; a.c_var8 = h->c_var8; a.pose_rec = h->pose_rec;   // (re)built by ensure_pose_cache just above
+            bind_pose_cache(h, a);
             // uint8 frames whose columns are whole 16-pixel runs: ONE fused launch (logic + TMA-moved frame)
             const size_t frame_bytes = (size_t)c.res_h * c.res_v * 3;
             if (h->fused_step && c.obs_dtype == MGB_OBS_U8 && (c.res_v & 15) == 0 && ((size_t)c.res_h * c.res_v) % 128 == 0 &&
@@ -3183,47 +3169,23 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, cudaStream_t st)
                     h->step_smem_set = ring_bytes;
                 }
                 const int64_t grid = (int64_t)h->num_sms * 2;
-                cudaLaunchConfig_t cfg;
-                memset(&cfg, 0, sizeof(cfg));
-                cfg.gridDim = dim3((unsigned)(h->n < grid ? h->n : grid));
-                cfg.blockDim = dim3(kStepThreads);
-                cfg.dynamicSmemBytes = ring_bytes;
-                cfg.stream = st;
-                cudaLaunchAttribute attr[1];
-                attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-                attr[0].val.programmaticStreamSerializationAllowed = h->step_pdl ? 1 : 0;
-                cfg.attrs = attr;
-                cfg.numAttrs = 1;
-                MGB_CUDA(cudaLaunchKernelEx(&cfg, maze3d_step_kernel, c, a));   // terminal frames in the same launch
+                // terminal frames in the same launch
+                maze3d_step_kernel<<<(unsigned)(h->n < grid ? h->n : grid), kStepThreads, ring_bytes, st>>>(c, a);
                 MGB_CUDA(cudaGetLastError());
                 h->launches += 1;
                 return MGB_OK;
             }
-            rc = start_terminal_list(h, a, st);
+            rc = start_terminal_list(h, a, listed, st);
             if (rc) return rc;
             maze3d_logic_kernel<true><<<(unsigned)((h->n + 127) / 128), 128, 0, st>>>(c, a);
             MGB_CUDA(cudaGetLastError());
-            {
-                int &ctas_per_sm = h->compose_ctas_per_sm;
-                if (!ctas_per_sm) {
-                    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, maze3d_compose_kernel, kComposeThreads, 0) !=
-                            cudaSuccess || ctas_per_sm < 1) ctas_per_sm = 4;
-                }
-                const int64_t resident = (int64_t)h->num_sms * ctas_per_sm;
-                int64_t parts = (4 * resident + h->n - 1) / h->n;  // aim at >= 4 work items per resident CTA
-                parts = parts < 1 ? 1 : (parts > 4 ? 4 : parts);
-                a.do_parts = (int)parts;
-                int64_t items = h->n * parts;
-                int &persistent = h->compose_persistent;
-                if (persistent < 0) { const char *ev = getenv("MGB_COMPOSE_PERSISTENT"); persistent = ev ? atoi(ev) : 0; }   // plain grid by default
-                if (!persistent) items = items < resident ? items : 0x7fffffff;   // plain grid: one CTA per item
-                if (!persistent) { maze3d_compose_kernel<<<(unsigned)(h->n * parts), kComposeThreads, 0, st>>>(c, a); }
-                else
-                maze3d_compose_kernel<<<(unsigned)(items < resident ? items : resident), kComposeThreads, 0, st>>>(c, a);
-            }
+            int64_t parts = (4 * compose_resident_ctas(h) + h->n - 1) / h->n;   // aim at >= 4 work items per resident CTA
+            parts = parts < 1 ? 1 : (parts > 4 ? 4 : parts);
+            a.do_parts = (int)parts;
+            maze3d_compose_kernel<<<(unsigned)(h->n * parts), kComposeThreads, 0, st>>>(c, a);   // one CTA per item
             h->launches += 1;
         } else {
-            rc = start_terminal_list(h, a, st);
+            rc = start_terminal_list(h, a, listed, st);
             if (rc) return rc;
             a.fin_dyn = nullptr;                                    // terminal list: full states for the direct renderer
             if (a.do_step && c.kind == MGB_MAZE_DISCRETE_3D) {     // logic for all envs in parallel, then render only
@@ -3252,24 +3214,21 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     MGB_REQUIRE(!final_obs || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
     a.truncated = truncated;
     a.final_obs = final_obs;
-    if (!final_obs || h->c.kind == MGB_MAZE_2D) return launch_observe(h, a, st);
-    a.fin_count = h->fin_count; a.fin_env = h->fin_env; a.fin_dyn = h->fin_dyn;
-    a.fin_agent = h->fin_agent; a.fin_life = h->fin_life; a.fin_eaten = h->fin_eaten; a.fin_task = h->fin_task;
-    a.fin_cpos = h->fin_cpos; a.fin_cori = h->fin_cori;
-    int rc = launch_observe(h, a, st);
-    if (rc || !h->list_pending) return rc;
+    if (final_obs && h->c.kind != MGB_MAZE_2D) {
+        a.fin_count = h->fin_count; a.fin_env = h->fin_env; a.fin_dyn = h->fin_dyn;
+        a.fin_agent = h->fin_agent; a.fin_life = h->fin_life; a.fin_eaten = h->fin_eaten; a.fin_task = h->fin_task;
+        a.fin_cpos = h->fin_cpos; a.fin_cori = h->fin_cori;
+    }
+    bool listed;
+    int rc = launch_observe(h, a, listed, st);
+    if (rc || !listed) return rc;
     MazeArgs l = maze_args(h);
     l.obs = final_obs; l.final_obs = final_obs; l.do_step = 0;
     l.fin_count = h->fin_count; l.fin_env = h->fin_env;
     if (h->cache_ready) {
         l.dyn = h->fin_dyn;
         l.do_parts = 16;     // a few frames per step: slices spread each over many CTAs, so the pass costs a slice, not a frame
-        int &ctas_per_sm = h->compose_ctas_per_sm;
-        if (!ctas_per_sm) {
-            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, maze3d_compose_kernel, kComposeThreads, 0) !=
-                    cudaSuccess || ctas_per_sm < 1) ctas_per_sm = 4;
-        }
-        const int64_t resident = (int64_t)h->num_sms * ctas_per_sm;
+        const int64_t resident = compose_resident_ctas(h);
         maze3d_compose_kernel<<<(unsigned)(h->n < resident ? h->n : resident), kComposeThreads, 0, st>>>(h->c, l);
         MGB_CUDA(cudaGetLastError());
     } else {
@@ -3282,6 +3241,30 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     return MGB_OK;
 }
 
+// What MGB_REQUIRE does, for a refusal made on behalf of the function `fn`
+static int maze_refuse(const char *fn, const char *msg)
+{
+    mgb_set_error("%s: %s", fn, msg);
+    return MGB_ERR_ARG;
+}
+
+// The four single-step entry points: refusals are made as `fn`, with kind_msg for a handle of the other action type
+// (`continuous`: float [n][2] actions of a MGB_MAZE_CONTINUOUS_3D handle; otherwise int32 [n] actions).
+static int step(const char *fn, bool continuous, const char *kind_msg, mgb_maze *h, const void *act_dev, void *obs_dev,
+                double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    if (!(h && act_dev && obs_dev && rew_dev && done_dev)) return maze_refuse(fn, "null argument");
+    if ((h->c.kind == MGB_MAZE_CONTINUOUS_3D) != continuous) return maze_refuse(fn, kind_msg);
+    int rc = maze_ready(h);
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    if (continuous) a.act_c = static_cast<const float *>(act_dev);
+    else a.act = static_cast<const int32_t *>(act_dev);
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
+}
+
 extern "C" int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_reset");
@@ -3292,34 +3275,41 @@ extern "C" int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_de
     cudaStream_t st = (cudaStream_t)stream;
     MazeArgs a = maze_args(h);
     a.mask = mask_dev;
-    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c, a);
+    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c, a, nullptr);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     if (obs_dev) {
         a.obs = obs_dev; a.do_step = 0; a.mask = nullptr;
-        return launch_observe(h, a, st);
+        bool listed;
+        return launch_observe(h, a, listed, st);
     }
     return MGB_OK;
 }
 
+// The checks of every rollout entry point, in the order it makes them: the handle, T, the entry point's own checks
+// (own() returns the refusal, or nullptr), the optional outputs, then the handle's state.  Refusals are made as `fn`.
+template <class Own>
+static int check_rollout(const char *fn, const mgb_maze *h, int32_t T, const void *final_obs, const void *truncated, Own own)
+{
+    if (!h) return maze_refuse(fn, "null handle");
+    if (T <= 0) return maze_refuse(fn, "T must be positive");
+    if (const char *why = own()) return maze_refuse(fn, why);
+    if (final_obs && !h->auto_reset)
+        return maze_refuse(fn, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
+    if ((final_obs || truncated) && h->mir.count != 0)
+        return maze_refuse(fn, "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
+    return maze_ready(h);
+}
+
+// Rollout of a MetaMaze2D or MetaMazeDiscrete3D handle; `own`: the entry point's kind checks (see check_rollout)
+template <class Own>
 static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
                    void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
-                   void *stream, bool discrete_ex = false)
+                   void *stream, Own own)
 {
-    MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE(T > 0, "T must be positive");
-    if (discrete_ex)
-        MGB_REQUIRE(h->c.kind == MGB_MAZE_DISCRETE_3D, "mgb_maze_rollout_discrete_ex needs a MGB_MAZE_DISCRETE_3D handle");
-    MGB_REQUIRE(h->c.kind == MGB_MAZE_2D || h->c.kind == MGB_MAZE_DISCRETE_3D,
-                "mgb_maze_rollout serves MetaMaze2D and MetaMazeDiscrete3D");
-    const bool fin = final_obs_dev || truncated_dev;
-    MGB_REQUIRE(!fin || discrete_ex || h->c.kind == MGB_MAZE_2D,
-                "final_obs / truncated of a rollout are produced for MetaMaze2D only");
-    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
-    MGB_REQUIRE(!fin || h->mir.count == 0,
-                "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
-    int rc = maze_ready(h);
+    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, own);
     if (rc) return rc;
+    const bool fin = final_obs_dev || truncated_dev;
     MgbDeviceGuard guard(h->device);
     MazeArgs a = maze_args(h);
     a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
@@ -3336,11 +3326,7 @@ static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_
         rc = ensure_pose_cache(h, st);
         if (rc) return rc;
         MGB_REQUIRE(h->cache_ready, "the fused 3-D rollout runs on the pose cache (MGB_MAZE_CACHE=0 or cache budget too small)");
-        a.poses = h->poses; a.pose_index = h->pose_index; a.c_px = h->c_px; a.c_fid = h->c_fid;
-        a.c_colhits = h->c_colhits; a.c_hits = h->c_hits; a.dyn = h->dyn; a.c_rgb8 = h->c_rgb8; a.c_gsig = h->c_gsig;
-        a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask;
-        a.c_vbase = h->c_vbase; a.c_var8 = h->c_var8; a.pose_rec = h->pose_rec;
-        a.bake = 0;
+        bind_pose_cache(h, a);
         const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers
         const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
         MGB_REQUIRE(qbytes <= 200 * 1024, "screen too large for the fused rollout's group queue");
@@ -3387,11 +3373,20 @@ static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_
     return MGB_OK;
 }
 
+// The handle kinds of mgb_maze_rollout and mgb_maze_rollout_ex (fin: final_obs or truncated requested)
+static const char *grid_rollout_refusal(const mgb_maze *h, bool fin)
+{
+    if (h->c.kind != MGB_MAZE_2D && h->c.kind != MGB_MAZE_DISCRETE_3D)
+        return "mgb_maze_rollout serves MetaMaze2D and MetaMazeDiscrete3D";
+    return fin && h->c.kind != MGB_MAZE_2D ? "final_obs / truncated of a rollout are produced for MetaMaze2D only" : nullptr;
+}
+
 extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
                                 void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout");
-    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
+    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream,
+                   [h] { return grid_rollout_refusal(h, false); });
 }
 
 extern "C" int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
@@ -3400,7 +3395,7 @@ extern "C" int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_de
 {
     MgbRange nvtx_range("mgb_maze_rollout_ex");
     return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
-                   stream);
+                   stream, [=] { return grid_rollout_refusal(h, final_obs_dev || truncated_dev); });
 }
 
 extern "C" int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
@@ -3409,7 +3404,10 @@ extern "C" int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_
 {
     MgbRange nvtx_range("mgb_maze_rollout_discrete_ex");
     return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
-                   stream, true);
+                   stream, [h]() -> const char * {
+        if (h->c.kind != MGB_MAZE_DISCRETE_3D) return "mgb_maze_rollout_discrete_ex needs a MGB_MAZE_DISCRETE_3D handle";
+        return nullptr;
+    });
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)
@@ -3448,42 +3446,36 @@ extern "C" int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void 
                                         uint8_t *done_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_step_continuous");
-    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
-    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_step_continuous needs a MGB_MAZE_CONTINUOUS_3D handle");
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    a.act_c = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    return launch_observe(h, a, (cudaStream_t)stream);
+    return step(__func__, true, "mgb_maze_step_continuous needs a MGB_MAZE_CONTINUOUS_3D handle", h, act_dev, obs_dev,
+                rew_dev, done_dev, nullptr, nullptr, stream);
 }
 
 extern "C" int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev,
                                            uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_step_continuous_ex");
-    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
-    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_step_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle");
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    a.act_c = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
+    return step(__func__, true, "mgb_maze_step_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle", h, act_dev, obs_dev,
+                rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
 }
 
-// Launch of the continuous-maze rollout once its entry point has checked the arguments (each entry point checks them
-// itself, so that every refusal names the call that made it).  With final_obs or truncated: maze3d_kernel<.., FIN>.
-static int rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
-                              void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
-                              uint8_t *truncated_dev, void *stream)
+// The continuous-maze rollout entry points; refusals are made as `fn`, with kind_msg for a handle of another kind.
+// With final_obs or truncated: maze3d_kernel<.., FIN>.
+static int rollout_continuous(const char *fn, const char *kind_msg, mgb_maze *h, int32_t T, const float *act_dev,
+                              uint64_t act_seed, float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                              void *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
+    int rc = check_rollout(fn, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
+        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
+        return h->c.kind == MGB_MAZE_CONTINUOUS_3D ? nullptr : kind_msg;
+    });
+    if (rc) return rc;
+    if (h->mir.count != 0)
+        return maze_refuse(fn, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
     MgbDeviceGuard guard(h->device);
     MazeArgs a = maze_args(h);
     a.act_c = act_dev; a.act_out_c = act_out_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
     a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
     const unsigned grid = (unsigned)(h->n < h->num_sms ? h->n : h->num_sms);
-    int rc;
     if (final_obs_dev || truncated_dev) {
         a.final_obs = final_obs_dev;
         a.truncated = truncated_dev;
@@ -3502,14 +3494,8 @@ extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *
                                            void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout_continuous");
-    MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE(T > 0, "T must be positive");
-    MGB_REQUIRE(obs_dev && rew_dev && done_dev, "null argument");
-    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_rollout_continuous needs a MGB_MAZE_CONTINUOUS_3D handle");
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MGB_REQUIRE(h->mir.count == 0, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
-    return rollout_continuous(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
+    return rollout_continuous(__func__, "mgb_maze_rollout_continuous needs a MGB_MAZE_CONTINUOUS_3D handle", h, T,
+                              act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
 }
 
 extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
@@ -3517,18 +3503,9 @@ extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const floa
                                               void *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout_continuous_ex");
-    MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE(T > 0, "T must be positive");
-    MGB_REQUIRE(obs_dev && rew_dev && done_dev, "null argument");
-    MGB_REQUIRE(h->c.kind == MGB_MAZE_CONTINUOUS_3D, "mgb_maze_rollout_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle");
-    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
-    MGB_REQUIRE(!(final_obs_dev || truncated_dev) || h->mir.count == 0,
-                "final_obs / truncated are not delivered through output mirrors or multicast (set_mirrors([]) first)");
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MGB_REQUIRE(h->mir.count == 0, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
-    return rollout_continuous(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev,
-                              truncated_dev, stream);
+    return rollout_continuous(__func__, "mgb_maze_rollout_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle", h, T,
+                              act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
+                              stream);
 }
 
 __global__ void maze_pose_kernel(MazeArgs a, float *pos_out, double *ori_out)
@@ -3556,28 +3533,16 @@ extern "C" int mgb_maze_step(mgb_maze *h, const int32_t *act_dev, void *obs_dev,
                              void *stream)
 {
     MgbRange nvtx_range("mgb_maze_step");
-    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
-    MGB_REQUIRE(h->c.kind != MGB_MAZE_CONTINUOUS_3D, "use mgb_maze_step_continuous for the continuous maze");
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    return launch_observe(h, a, (cudaStream_t)stream);
+    return step(__func__, false, "use mgb_maze_step_continuous for the continuous maze", h, act_dev, obs_dev, rew_dev,
+                done_dev, nullptr, nullptr, stream);
 }
 
 extern "C" int mgb_maze_step_ex(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                                 void *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_step_ex");
-    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
-    MGB_REQUIRE(h->c.kind != MGB_MAZE_CONTINUOUS_3D, "use mgb_maze_step_continuous_ex for the continuous maze");
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
+    return step(__func__, false, "use mgb_maze_step_continuous_ex for the continuous maze", h, act_dev, obs_dev, rew_dev,
+                done_dev, final_obs_dev, truncated_dev, stream);
 }
 
 extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev, void *stream)

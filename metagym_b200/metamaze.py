@@ -269,6 +269,23 @@ class _BatchedMazeBase(object):
         _lib.check(self._lib.mgb_maze_set_options(self._h, int(self.auto_reset)))
         self._after_create()
 
+    @staticmethod
+    def _pack_tasks(tasks):
+        """TaskConfigs -> the C ABI's task arrays: walls, texts [K,n,n] int8, food [K,n,n] float64, interval [K,n,n]
+        int32, and a MazeTaskScalars[K]."""
+        walls = np.ascontiguousarray(np.stack([np.asarray(t.cell_walls) for t in tasks]).astype(np.int8))
+        texts = np.ascontiguousarray(np.stack([np.asarray(t.cell_texts) for t in tasks]).astype(np.int8))
+        food = np.ascontiguousarray(np.stack([np.asarray(t.food_rewards, dtype=np.float64) for t in tasks]))
+        itv = np.ascontiguousarray(np.stack([np.asarray(t.food_interval) for t in tasks]).astype(np.int32))
+        sc = (_lib.MazeTaskScalars * len(tasks))()
+        for k, t in enumerate(tasks):
+            sc[k].start[:] = [int(t.start[0]), int(t.start[1])]
+            sc[k].goal[:] = [int(t.goal[0]), int(t.goal[1])]
+            sc[k].cell_size, sc[k].wall_height, sc[k].agent_height = t.cell_size, t.wall_height, t.agent_height
+            sc[k].initial_life, sc[k].max_life = t.initial_life, t.max_life
+            sc[k].step_reward, sc[k].goal_reward = t.step_reward, t.goal_reward
+        return walls, texts, food, itv, sc
+
     def set_task(self, task_config, env2task=None):
         """MazeBase.set_task (maze_base.py:19-38).  `task_config`: one TaskConfig (all envs) or a sequence of them;
         env i then runs task env2task[i] (default: (env_index_base + i) % n_tasks)."""
@@ -283,17 +300,7 @@ class _BatchedMazeBase(object):
             assert w.shape[0] == n, "all tasks of one batch must share the maze size"
         self._create(n)
         K = len(tasks)
-        walls = np.ascontiguousarray(np.stack([np.asarray(t.cell_walls) for t in tasks]).astype(np.int8))
-        texts = np.ascontiguousarray(np.stack([np.asarray(t.cell_texts) for t in tasks]).astype(np.int8))
-        food = np.ascontiguousarray(np.stack([np.asarray(t.food_rewards, dtype=np.float64) for t in tasks]))
-        itv = np.ascontiguousarray(np.stack([np.asarray(t.food_interval) for t in tasks]).astype(np.int32))
-        sc = (_lib.MazeTaskScalars * K)()
-        for k, t in enumerate(tasks):
-            sc[k].start[:] = [int(t.start[0]), int(t.start[1])]
-            sc[k].goal[:] = [int(t.goal[0]), int(t.goal[1])]
-            sc[k].cell_size, sc[k].wall_height, sc[k].agent_height = t.cell_size, t.wall_height, t.agent_height
-            sc[k].initial_life, sc[k].max_life = t.initial_life, t.max_life
-            sc[k].step_reward, sc[k].goal_reward = t.step_reward, t.goal_reward
+        walls, texts, food, itv, sc = self._pack_tasks(tasks)
         if env2task is None:
             env2task = (np.arange(self.num_envs, dtype=np.int64) + self.env_index_base) % K
         e2t = np.ascontiguousarray(np.asarray(env2task, dtype=np.int32))
@@ -314,19 +321,10 @@ class _BatchedMazeBase(object):
         tasks = [task_configs] if hasattr(task_configs, "cell_walls") else list(task_configs)
         K = len(tasks)
         assert slots.shape == (K,), "one task per slot"
-        walls = np.ascontiguousarray(np.stack([np.asarray(t.cell_walls) for t in tasks]).astype(np.int8))
-        texts = np.ascontiguousarray(np.stack([np.asarray(t.cell_texts) for t in tasks]).astype(np.int8))
-        food = np.ascontiguousarray(np.stack([np.asarray(t.food_rewards, dtype=np.float64) for t in tasks]))
-        itv = np.ascontiguousarray(np.stack([np.asarray(t.food_interval) for t in tasks]).astype(np.int32))
+        walls, texts, food, itv, sc = self._pack_tasks(tasks)
         assert walls.shape[1:] == (self._n_cells, self._n_cells), "all tasks of one batch must share the maze size"
-        sc = (_lib.MazeTaskScalars * K)()
-        for k, t in enumerate(tasks):
+        for t in tasks:
             assert t.agent_height < t.wall_height and t.agent_height > 0, "the agent height must be > 0 and < wall height"
-            sc[k].start[:] = [int(t.start[0]), int(t.start[1])]
-            sc[k].goal[:] = [int(t.goal[0]), int(t.goal[1])]
-            sc[k].cell_size, sc[k].wall_height, sc[k].agent_height = t.cell_size, t.wall_height, t.agent_height
-            sc[k].initial_life, sc[k].max_life = t.initial_life, t.max_life
-            sc[k].step_reward, sc[k].goal_reward = t.step_reward, t.goal_reward
         _lib.check(self._lib.mgb_maze_update_tasks(self._h, K, slots.ctypes.data, walls.ctypes.data, texts.ctypes.data,
                                                    food.ctypes.data, itv.ctypes.data, sc, self._stream()))
         for k, sl in enumerate(slots):
@@ -410,32 +408,36 @@ class _BatchedMazeBase(object):
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done_bool), info
 
-    def _rollout(self, T, actions, act_seed, want_actions, out, final=False, entry="mgb_maze_rollout_ex"):
-        """final: also produce the "final_obs" / "truncated" entries through `entry` (mgb_maze_rollout_ex for MetaMaze2D,
-        mgb_maze_rollout_discrete_ex for MetaMazeDiscrete3D)."""
+    # rollout(): the C entry points without / with the final_obs and truncated outputs, the layout of one step's
+    # actions, and whether the "act" output also records actions the caller passed in (or only device-drawn ones)
+    _ROLLOUT_ENTRIES = ("mgb_maze_rollout", "mgb_maze_rollout_ex")
+    _ACT_DTYPE, _ACT_SHAPE = "int32", ()
+    _RECORDS_GIVEN_ACTIONS = True
+
+    def _rollout(self, T, actions, act_seed, want_actions, out, final=False):
+        """final: also produce the "final_obs" / "truncated" entries (through _ROLLOUT_ENTRIES[1])."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
-        N, dev = self.num_envs, self.device
+        T, N, dev = int(T), self.num_envs, self.device
+        act_dtype, act_shape = getattr(torch, self._ACT_DTYPE), (T, N) + self._ACT_SHAPE
+        record = actions is None or self._RECORDS_GIVEN_ACTIONS
         if out is None:
             out = {"obs": torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev),
                    "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
                    "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
-                   "act": torch.empty((T, N), dtype=torch.int32, device=dev) if want_actions else None}
+                   "act": torch.empty(act_shape, dtype=act_dtype, device=dev) if want_actions and record else None}
             if final:
                 out["final_obs"] = torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev)
                 out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
-        a = None if actions is None else actions.to(torch.int32).reshape(T, N).contiguous()
-        if not final:
-            _lib.check(self._lib.mgb_maze_rollout(self._h, int(T), _lib.ptr(a), int(act_seed),
-                                                  _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
-                                                  _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")), self._stream()))
-        else:
-            _lib.check(getattr(self._lib, entry)(self._h, int(T), _lib.ptr(a), int(act_seed),
-                                                 _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
-                                                 _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
-                                                 _lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated")),
-                                                 self._stream()))
+        a = None
+        if actions is not None:
+            a = torch.as_tensor(actions, dtype=act_dtype, device=dev).reshape(act_shape).contiguous()
+        args = [_lib.ptr(a), int(act_seed), _lib.ptr(out.get("act") if record else None), _lib.ptr(out.get("obs")),
+                _lib.ptr(out.get("rew")), _lib.ptr(out.get("done"))]
+        if final:
+            args += [_lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated"))]
+        _lib.check(getattr(self._lib, self._ROLLOUT_ENTRIES[final])(self._h, T, *args, self._stream()))
         return out
 
     def _check_rollout_final(self, final_obs):
@@ -548,6 +550,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     same values in the dtype the reference's observation_space declares (maze_env.py:37-39), 'uint8' = min(value, 255).
     textures: (grounds uint8 [n_tex,64,64,3], ceil uint8 [64,64,3]); default = procedural set."""
     KIND = 1
+    _ROLLOUT_ENTRIES = ("mgb_maze_rollout", "mgb_maze_rollout_discrete_ex")
 
     def __init__(self, enable_render=False, render_scale=480, resolution=(320, 320), max_steps=5000,
                  task_type="SURVIVAL", num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True,
@@ -590,8 +593,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         if done[t, e] (what step() reports as final_observation; allocated with torch.empty, rows with done 0 are not
         written), and "truncated" [T,N] uint8, written for every step: 1 iff done and the episode ended only through
         max_steps.  A caller-supplied `out` may omit either entry, and that output is then not produced."""
-        final = self._check_rollout_final(final_obs)
-        return self._rollout(T, actions, act_seed, want_actions, out, final=final, entry="mgb_maze_rollout_discrete_ex")
+        return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs))
 
     def cache_info(self):
         """Pose-cache statistics (valid after the first reset()/step()): dict(poses, variant_frames, variant_bits, bytes,
@@ -620,6 +622,9 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
     maze_continuous_3d.py:48-49); float32 position / float64 heading exactly as the reference computes them for
     float32 actions.  Every pose is unique, so this env always uses the direct float64 renderer."""
     KIND = 2
+    _ROLLOUT_ENTRIES = ("mgb_maze_rollout_continuous", "mgb_maze_rollout_continuous_ex")
+    _ACT_DTYPE, _ACT_SHAPE = "float32", (2,)
+    _RECORDS_GIVEN_ACTIONS = False
 
     def __init__(self, *args, **kwargs):
         BatchedMetaMazeDiscrete3D.__init__(self, *args, **kwargs)
@@ -661,34 +666,7 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e if done[t, e]
         (allocated with torch.empty, rows with done 0 are not written), and "truncated" [T,N] uint8, written for every
         step.  A caller-supplied `out` may omit either entry, and that output is then not produced."""
-        final = self._check_rollout_final(final_obs)
-        if self.need_reset:
-            raise Exception("Must \"reset\" before doing any actions")
-        torch = self._torch
-        T, N, dev = int(T), self.num_envs, self.device
-        if out is None:
-            out = {"obs": torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev),
-                   "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
-                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
-                   "act": torch.empty((T, N, 2), dtype=torch.float32, device=dev)
-                   if want_actions and actions is None else None}
-            if final:
-                out["final_obs"] = torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev)
-                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
-        a = None
-        if actions is not None:
-            a = torch.as_tensor(actions, dtype=torch.float32, device=dev).reshape(T, N, 2).contiguous()
-        drawn = out.get("act") if a is None else None
-        if not final:
-            _lib.check(self._lib.mgb_maze_rollout_continuous(self._h, T, _lib.ptr(a), int(act_seed), _lib.ptr(drawn),
-                                                             _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
-                                                             _lib.ptr(out.get("done")), self._stream()))
-        else:
-            _lib.check(self._lib.mgb_maze_rollout_continuous_ex(self._h, T, _lib.ptr(a), int(act_seed), _lib.ptr(drawn),
-                                                                _lib.ptr(out.get("obs")), _lib.ptr(out.get("rew")),
-                                                                _lib.ptr(out.get("done")), _lib.ptr(out.get("final_obs")),
-                                                                _lib.ptr(out.get("truncated")), self._stream()))
-        return out
+        return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs))
 
     def pose(self):
         """-> (pos [N,2] float32 = _agent_loc, ori [N] float64 = _agent_ori)."""
