@@ -174,6 +174,25 @@ int mgb_quad_step_host_ex(mgb_quad *h, const float *act_host, float *obs_host, f
  * = p3 v3 w3 prop4 R9, ct_dev [n] int32.  load = 0 copies handle -> buffers, 1 buffers -> handle. */
 int mgb_quad_state(mgb_quad *h, float *state_dev, int32_t *ct_dev, int load, void *stream);
 
+/* Exact snapshot / restore of env state (DESIGN.md "Snapshot, restore and clone").  A record is a fixed-size,
+ * 16-byte-aligned row of mgb_quad_record_bytes(h) bytes per env: the six float4 state planes of the env (22 state floats,
+ * ct, episode counter) and its velocity task index.  Records carry no env index: the caller matches them to envs.
+ *   mgb_quad_snapshot: rec_dev [n][B] receives the record of every local env.
+ *   mgb_quad_restore: row_of_env_dev [n] int64 gives, for each local env e, the row of rec_dev [n_rec][B] to load into
+ *     it; a row outside [0, n_rec) leaves env e untouched.  Rows must come from a handle with the same fingerprint.  A
+ *     task index outside the handle's target table leaves env2task[e] as it was.
+ * Both are stream-ordered kernels, with no host synchronisation and no allocation (capturable in a CUDA graph).
+ *   mgb_quad_counters: set = 0 reads the handle's rollout action counter (the step index that keys device-drawn rollout
+ *     actions) into *t_base, set = 1 writes it.  Host-only, immediate.
+ *   mgb_quad_fingerprint: out[MGB_FINGERPRINT_WORDS] = what a handle restoring these records must share: out[0] config
+ *     (mgb_quad_cfg, auto_reset, rng seed, record size), out[1] obstacle map, out[2] velocity-target table, out[3] 0. */
+#define MGB_FINGERPRINT_WORDS 4
+int64_t mgb_quad_record_bytes(const mgb_quad *h);
+int mgb_quad_snapshot(mgb_quad *h, uint8_t *rec_dev, void *stream);
+int mgb_quad_restore(mgb_quad *h, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row_of_env_dev, void *stream);
+int mgb_quad_counters(mgb_quad *h, uint64_t *t_base, int set);
+int mgb_quad_fingerprint(const mgb_quad *h, uint64_t *out);
+
 /* Number of kernel launches issued through this handle so far (bench.py reports it as gpu_launches). */
 int64_t mgb_quad_launch_count(const mgb_quad *h);
 
@@ -387,6 +406,21 @@ int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);
  * int32 = grid_x, grid_y, ori_index, steps; life [n] float64. */
 int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev, void *stream);
 int64_t mgb_maze_launch_count(const mgb_maze *h);
+
+/* Exact snapshot / restore of env state, as mgb_quad_snapshot / mgb_quad_restore (same row map and stream rules).  A
+ * record of mgb_maze_record_bytes(h) bytes (after mgb_maze_set_task) holds agent (int4), life, the env's resample count,
+ * its task-table slot, the continuous pose, the food stamps of every food slot and -- when the handle owns one table
+ * slot per env and can re-task envs on the device (injective env2task, direct renderer) -- the whole task of the env's
+ * slot.  Restore then writes that task into the destination env's own slot; otherwise the table is shared, the fingerprint
+ * covers it, and restore points env2task[e] at the record's slot.  mgb_maze_restore is synchronous the first time it
+ * finds the pose cache to be built (like the first reset); after that it is stream-ordered.
+ *   mgb_maze_fingerprint: out[0] config (mgb_maze_cfg, auto_reset, table shape, record layout), out[1] textures,
+ *     out[2] the shared task table (0 when records carry their tasks), out[3] 1 when records carry their tasks. */
+int64_t mgb_maze_record_bytes(const mgb_maze *h);
+int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream);
+int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row_of_env_dev, void *stream);
+int mgb_maze_counters(mgb_maze *h, uint64_t *t_base, int set);
+int mgb_maze_fingerprint(const mgb_maze *h, uint64_t *out);
 
 /* ------------------------------------------------------------------------------------------------------------ */
 const char *mgb_last_error(void);

@@ -104,6 +104,16 @@ SIGNATURES = {
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),
+    "mgb_quad_record_bytes": (c_i64, [vp]),
+    "mgb_quad_snapshot": (ctypes.c_int, [vp, vp, vp]),
+    "mgb_quad_restore": (ctypes.c_int, [vp, vp, c_i64, vp, vp]),
+    "mgb_quad_counters": (ctypes.c_int, [vp, ctypes.POINTER(c_u64), ctypes.c_int]),
+    "mgb_quad_fingerprint": (ctypes.c_int, [vp, ctypes.POINTER(c_u64)]),
+    "mgb_maze_record_bytes": (c_i64, [vp]),
+    "mgb_maze_snapshot": (ctypes.c_int, [vp, vp, vp]),
+    "mgb_maze_restore": (ctypes.c_int, [vp, vp, c_i64, vp, vp]),
+    "mgb_maze_counters": (ctypes.c_int, [vp, ctypes.POINTER(c_u64), ctypes.c_int]),
+    "mgb_maze_fingerprint": (ctypes.c_int, [vp, ctypes.POINTER(c_u64)]),
     "mgb_last_error": (ctypes.c_char_p, []),
     "mgb_version": (ctypes.c_char_p, []),
     "mgb_device_count": (ctypes.c_int, []),

@@ -2089,6 +2089,8 @@ struct mgb_maze {
     int num_sms = 0;
     int64_t launches = 0;
     uint32_t t_base = 0;
+    uint64_t fp_tex = 0;                      // fingerprint of the loaded textures (mgb_maze_fingerprint)
+    std::vector<uint64_t> slot_fp;            // fingerprint of every task-table slot as set_task / update_tasks wrote it
     MgbMirrors mir = {};         // mgb_maze_set_mirrors
     MgbMirrorWindow mir_win;     // mgb_maze_set_mirror_window
     // terminal list of mgb_maze_step_ex (allocated by its first 3-D call with final_obs)
@@ -2321,6 +2323,8 @@ extern "C" int mgb_maze_set_textures(mgb_maze *h, const uint8_t *grounds_host, i
     MGB_CUDA(cudaMalloc(&h->tex, packed.size() * 4));
     MGB_CUDA(cudaMemcpy(h->tex, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice));
     h->c.n_tex = n_tex; h->c.ts = tex_size;
+    h->fp_tex = mgb_fnv(mgb_fnv(mgb_fnv(MGB_FNV_BASIS, &n_tex, sizeof(n_tex)), &tex_size, sizeof(tex_size)), packed.data(),
+                        packed.size() * 4);
     h->tex_max = 0;
     for (size_t i = 0; i < 3 * (size_t)n_tex * px; ++i) h->tex_max = grounds_host[i] > h->tex_max ? grounds_host[i] : h->tex_max;
     for (size_t i = 0; i < 3 * px; ++i) h->tex_max = ceil_host[i] > h->tex_max ? ceil_host[i] : h->tex_max;
@@ -2457,6 +2461,9 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     cudaFree(h->eaten); h->eaten = nullptr;
     MGB_CUDA(cudaMalloc(&h->blobs, blobs.size()));
     MGB_CUDA(cudaMemcpy(h->blobs, blobs.data(), blobs.size(), cudaMemcpyHostToDevice));
+    h->slot_fp.assign((size_t)n_tasks, 0);
+    for (int t = 0; t < n_tasks; ++t)
+        h->slot_fp[t] = mgb_fnv(MGB_FNV_BASIS, blobs.data() + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
     MGB_CUDA(cudaMalloc(&h->eaten, sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad));
     if (c.kind != MGB_MAZE_2D) {     // terminal list of mgb_maze_step_ex, sized here so that its first call can be captured
         cudaFree(h->fin_eaten); h->fin_eaten = nullptr;
@@ -2786,6 +2793,8 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
         fill_task_blob(c, hs + head + (size_t)t * c.blob_bytes, walls_host + (size_t)t * nn, texts_host + (size_t)t * nn,
                        food_rewards_host + (size_t)t * nn, food_interval_host + (size_t)t * nn, scalars_host[t], h->cls_heights,
                        false);
+    for (int t = 0; t < count; ++t)
+        h->slot_fp[task_slots_host[t]] = mgb_fnv(MGB_FNV_BASIS, hs + head + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
     cudaStream_t st = (cudaStream_t)stream;
     MGB_CUDA(cudaMemcpyAsync(h->d_stage[sb], hs, need, cudaMemcpyHostToDevice, st));
     MGB_CUDA(cudaEventRecord(h->stage_done[sb], st));
@@ -2795,6 +2804,15 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags, h->n_tasks);
     MGB_CUDA(cudaGetLastError());
     h->launches += 3;
+    return MGB_OK;
+}
+
+// The per-env resample counts, zero until the first mgb_maze_resample_tasks (or a restore) needs them
+static int ensure_task_epoch(mgb_maze *h)
+{
+    if (h->task_epoch) return MGB_OK;
+    MGB_CUDA(cudaMalloc(&h->task_epoch, sizeof(uint32_t) * (size_t)h->n_pad));
+    MGB_CUDA(cudaMemset(h->task_epoch, 0, sizeof(uint32_t) * (size_t)h->n_pad));
     return MGB_OK;
 }
 
@@ -2826,10 +2844,8 @@ extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, con
     sc.cls = -1;
     for (size_t k = 0; k < h->cls_heights.size() / 2; ++k)
         if (h->cls_heights[2 * k] == cfg->agent_height && h->cls_heights[2 * k + 1] == cfg->wall_height) sc.cls = (int)k;
-    if (!h->task_epoch) {
-        MGB_CUDA(cudaMalloc(&h->task_epoch, sizeof(uint32_t) * (size_t)h->n_pad));
-        MGB_CUDA(cudaMemset(h->task_epoch, 0, sizeof(uint32_t) * (size_t)h->n_pad));
-    }
+    int rc = ensure_task_epoch(h);
+    if (rc) return rc;
     MazeArgs a = maze_args(h);
     maze_sample_tasks_kernel<<<(unsigned)((h->n + kSamplerWarps - 1) / kSamplerWarps), 32 * kSamplerWarps, 0, (cudaStream_t)stream>>>(c, a, h->blobs, mask_dev, h->task_epoch,
                                                                                         sc, seed);
@@ -2960,6 +2976,20 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
 
 // (Re)build the pose cache when tasks or textures changed: every free cell x 4 headings of every task is rendered once
 // into its static layers.  Skipped (direct renderer used instead) when disabled or over the memory budget.
+// Bytes of the pose cache of the handle's task table, and whether the cache can serve it: within the budget, and every
+// lit texel fits the 10 bits per channel c_px packs.  Floor and ceiling texels are lit by v_screen / l_focal
+// (ray_caster_utils.py:99,132), up to (half_v - pixel_size / 2) / l_focal; times the brightest texel that can pass 1023 on
+// tall screens, and those screens render directly.
+static bool pose_cache_fits(const mgb_maze *h, double &bytes)
+{
+    const MazeConst &c = h->c;
+    const size_t slots = h->host_poses.size(), px = (size_t)c.res_h * c.res_v;
+    bytes = (double)slots * (px * (c.obs_dtype == MGB_OBS_U8 ? 8.0 : 12.0) + px / 4.0 + 16.0 +
+                             c.res_h * (1.0 + (double)c.max_hits * sizeof(HitRec)));
+    const bool packs = (c.half_v - 0.5 * c.pixel_size) / c.l_focal * h->tex_max < 1024.0;
+    return bytes <= h->cache_budget_gb * 1e9 && packs;
+}
+
 static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
 {
     if (!h->cache_dirty) return MGB_OK;
@@ -2967,13 +2997,8 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     MazeConst &c = h->c;
     if (!h->cache_enabled || c.kind != MGB_MAZE_DISCRETE_3D || h->host_poses.empty()) { h->cache_dirty = false; return MGB_OK; }
     const size_t slots = h->host_poses.size(), px = (size_t)c.res_h * c.res_v;
-    const double bytes = (double)slots * (px * (c.obs_dtype == MGB_OBS_U8 ? 8.0 : 12.0) + px / 4.0 + 16.0 +
-                                          c.res_h * (1.0 + (double)c.max_hits * sizeof(HitRec)));
-    // c_px packs 10 bits per channel.  Floor and ceiling texels are lit by v_screen / l_focal (ray_caster_utils.py:99,132),
-    // up to (half_v - pixel_size / 2) / l_focal; times the brightest texel that can pass 1023 on tall screens, and those
-    // screens render directly.
-    const bool packs = (c.half_v - 0.5 * c.pixel_size) / c.l_focal * h->tex_max < 1024.0;
-    if (bytes > h->cache_budget_gb * 1e9 || !packs) { h->cache_dirty = false; h->cache_would_fit = false; return MGB_OK; }   // a decision, not a failure
+    double bytes;
+    if (!pose_cache_fits(h, bytes)) { h->cache_dirty = false; h->cache_would_fit = false; return MGB_OK; }   // a decision, not a failure
     // From here on a failure (capture in progress, out of memory) leaves cache_dirty set: the next call retries instead of
     // silently rendering every frame with the slow direct renderer (round-1 advice).
     // cudaMalloc/cudaFree synchronise; a capture in progress cannot build the cache
@@ -3553,5 +3578,206 @@ extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev,
     maze_state_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, agent_dev, life_dev);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
+    return MGB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Snapshot / restore records (DESIGN.md "Snapshot, restore and clone").  A record is
+//   [0, 16)   agent int4 (gx, gy, ori, steps)
+//   [16, 32)  life f64 | resample count u32 | task-table slot i32
+//   [32, 48)  continuous position f32 x 2 | heading f64 (zero for the other kinds)
+//   [48, ..)  food stamps int32 [f_max], in groups of four (16 bytes each, unused tail zero)
+//   [tail, ..) the task of the env's slot, blob_bytes, when records carry their tasks
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int64_t kMazeRecHead = 48;
+
+__global__ void maze_snapshot_kernel(int f_max, const __grid_constant__ MazeArgs a, const uint32_t *__restrict__ epoch,
+                                     uint8_t *__restrict__ rec, int64_t rec_bytes)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n) return;
+    uint4 *r = reinterpret_cast<uint4 *>(rec + e * rec_bytes);
+    const int4 ag = a.agent[e];
+    const double life = a.life[e];
+    r[0] = make_uint4((uint32_t)ag.x, (uint32_t)ag.y, (uint32_t)ag.z, (uint32_t)ag.w);
+    r[1] = make_uint4((uint32_t)__double2loint(life), (uint32_t)__double2hiint(life), epoch ? epoch[e] : 0u,
+                      (uint32_t)a.env2task[e]);
+    const float2 p = a.cpos ? a.cpos[e] : make_float2(0.f, 0.f);
+    const double o = a.cori ? a.cori[e] : 0.0;
+    r[2] = make_uint4(__float_as_uint(p.x), __float_as_uint(p.y), (uint32_t)__double2loint(o), (uint32_t)__double2hiint(o));
+    for (int f = 0; f < f_max; f += 4) {
+        uint32_t v[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) v[j] = f + j < f_max ? (uint32_t)a.eaten[(int64_t)(f + j) * a.n_pad + e] : 0u;
+        r[3 + f / 4] = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+}
+
+// env2task_w: null when records carry their tasks (the env keeps its own slot)
+__global__ void maze_restore_kernel(int f_max, const __grid_constant__ MazeArgs a, uint32_t *__restrict__ epoch,
+                                    int32_t *__restrict__ env2task_w, int n_tasks, const uint8_t *__restrict__ rec,
+                                    int64_t rec_bytes, int64_t n_rec, const int64_t *__restrict__ row)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n) return;
+    const int64_t rw = row[e];
+    if (rw < 0 || rw >= n_rec) return;
+    const uint4 *s = reinterpret_cast<const uint4 *>(rec + rw * rec_bytes);
+    const uint4 h0 = s[0], h1 = s[1], h2 = s[2];
+    a.agent[e] = make_int4((int)h0.x, (int)h0.y, (int)h0.z, (int)h0.w);
+    a.life[e] = __hiloint2double((int)h1.y, (int)h1.x);
+    epoch[e] = h1.z;
+    if (env2task_w && (int)h1.w >= 0 && (int)h1.w < n_tasks) env2task_w[e] = (int)h1.w;
+    if (a.cpos) {
+        a.cpos[e] = make_float2(__uint_as_float(h2.x), __uint_as_float(h2.y));
+        a.cori[e] = __hiloint2double((int)h2.w, (int)h2.z);
+    }
+    for (int f = 0; f < f_max; f += 4) {
+        const uint4 u = s[3 + f / 4];
+        const uint32_t v[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (f + j < f_max) a.eaten[(int64_t)(f + j) * a.n_pad + e] = (int32_t)v[j];
+    }
+}
+
+// The task of every env's own slot <-> the tail of its record: one uint4 per thread over all (env, uint4) pairs, so that
+// both sides are read and written contiguously.  LOAD: restore (row map as for maze_restore_kernel), else snapshot.
+template <bool LOAD>
+__global__ void maze_record_tasks_kernel(int64_t n, int blob_bytes, const int32_t *__restrict__ env2task, uint8_t *blobs,
+                                         uint8_t *rec, int64_t rec_bytes, int64_t tail, int64_t n_rec,
+                                         const int64_t *__restrict__ row)
+{
+    const int64_t q = blob_bytes / 16, total = n * q;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t e = i / q, k = i - e * q;
+        uint4 *blob = reinterpret_cast<uint4 *>(blobs + (int64_t)env2task[e] * blob_bytes) + k;
+        if (LOAD) {
+            const int64_t rw = row[e];
+            if (rw >= 0 && rw < n_rec) *blob = reinterpret_cast<const uint4 *>(rec + rw * rec_bytes + tail)[k];
+        } else {
+            reinterpret_cast<uint4 *>(rec + e * rec_bytes + tail)[k] = *blob;
+        }
+    }
+}
+
+}  // namespace
+
+// Records carry their env's whole task when the env owns its table slot and the table can change on the device
+// (resample_tasks / update_tasks need the direct renderer).  Otherwise the table is shared, and fingerprinted.
+static bool records_carry_tasks(const mgb_maze *h)
+{
+    double bytes;
+    const bool cached = h->c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() &&
+                        pose_cache_fits(h, bytes);
+    return h->slot_per_env && !cached;
+}
+
+static int64_t record_tail(const mgb_maze *h) { return kMazeRecHead + (int64_t)(h->c.f_max + 3) / 4 * 16; }
+
+static int64_t record_bytes(const mgb_maze *h)
+{
+    return record_tail(h) + (records_carry_tasks(h) ? h->c.blob_bytes : 0);
+}
+
+extern "C" int64_t mgb_maze_record_bytes(const mgb_maze *h)
+{
+    MGB_REQUIRE(h, "null handle");
+    MGB_REQUIRE(h->has_task, "call mgb_maze_set_task first (it fixes the record layout)");
+    return record_bytes(h);
+}
+
+extern "C" int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_snapshot");
+    MGB_REQUIRE(h && rec_dev, "null argument");
+    MGB_REQUIRE((reinterpret_cast<uintptr_t>(rec_dev) & 15u) == 0, "rec_dev must be 16-byte aligned");
+    MGB_REQUIRE(h->has_task, "call mgb_maze_set_task first (it fixes the record layout)");
+    MgbDeviceGuard guard(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const MazeArgs a = maze_args(h);
+    const int64_t rb = record_bytes(h);
+    maze_snapshot_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch, rec_dev, rb);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    if (records_carry_tasks(h)) {
+        const int64_t total = h->n * (h->c.blob_bytes / 16), cap = (int64_t)h->num_sms * 16;
+        const int64_t grid = (total + 255) / 256 < cap ? (total + 255) / 256 : cap;
+        maze_record_tasks_kernel<false><<<(unsigned)grid, 256, 0, st>>>(h->n, h->c.blob_bytes, h->env2task, h->blobs, rec_dev,
+                                                                       rb, record_tail(h), 0, nullptr);
+        MGB_CUDA(cudaGetLastError());
+        h->launches += 1;
+    }
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row_of_env_dev,
+                                void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_restore");
+    MGB_REQUIRE(h && rec_dev && row_of_env_dev, "null argument");
+    MGB_REQUIRE(n_rec >= 0, "n_rec must not be negative");
+    MGB_REQUIRE((reinterpret_cast<uintptr_t>(rec_dev) & 15u) == 0, "rec_dev must be 16-byte aligned");
+    int rc = maze_ready(h);
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    // what the first reset() builds, so that a handle restored right after set_task steps (and can be captured) like a
+    // reset one
+    if (h->c.kind != MGB_MAZE_2D && (rc = ensure_pose_cache(h, st))) return rc;
+    if ((rc = ensure_task_epoch(h))) return rc;
+    const bool carry = records_carry_tasks(h);
+    const int64_t rb = record_bytes(h);
+    const MazeArgs a = maze_args(h);
+    maze_restore_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch,
+                                                                        carry ? nullptr : h->env2task, h->n_tasks, rec_dev,
+                                                                        rb, n_rec, row_of_env_dev);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    if (carry) {
+        const int64_t total = h->n * (h->c.blob_bytes / 16), cap = (int64_t)h->num_sms * 16;
+        const int64_t grid = (total + 255) / 256 < cap ? (total + 255) / 256 : cap;
+        maze_record_tasks_kernel<true><<<(unsigned)grid, 256, 0, st>>>(h->n, h->c.blob_bytes, h->env2task, h->blobs,
+                                                                      const_cast<uint8_t *>(rec_dev), rb, record_tail(h),
+                                                                      n_rec, row_of_env_dev);
+        MGB_CUDA(cudaGetLastError());
+        h->launches += 1;
+    }
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_counters(mgb_maze *h, uint64_t *t_base, int set)
+{
+    MGB_REQUIRE(h && t_base, "null argument");
+    if (set) h->t_base = (uint32_t)*t_base;
+    else *t_base = h->t_base;
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_fingerprint(const mgb_maze *h, uint64_t *out)
+{
+    MGB_REQUIRE(h && out, "null argument");
+    MGB_REQUIRE(h->has_task, "call mgb_maze_set_task first (it fixes the record layout)");
+    const MazeConst &c = h->c;
+    const bool carry = records_carry_tasks(h);
+    const int64_t rb = record_bytes(h);
+    uint64_t f = mgb_fnv(MGB_FNV_BASIS, &h->cfg, sizeof(h->cfg));
+    f = mgb_fnv(f, &h->auto_reset, sizeof(h->auto_reset));
+    f = mgb_fnv(f, &c.f_max, sizeof(c.f_max));
+    f = mgb_fnv(f, &c.blob_bytes, sizeof(c.blob_bytes));
+    f = mgb_fnv(f, &c.max_hits, sizeof(c.max_hits));
+    f = mgb_fnv(f, &h->min_cell, sizeof(h->min_cell));
+    f = mgb_fnv(f, h->cls_heights.data(), h->cls_heights.size() * sizeof(double));
+    out[0] = mgb_fnv(f, &rb, sizeof(rb));
+    out[1] = h->fp_tex;
+    uint64_t t = 0;
+    if (!carry) {
+        t = mgb_fnv(MGB_FNV_BASIS, &h->n_tasks, sizeof(h->n_tasks));
+        t = mgb_fnv(t, h->slot_fp.data(), h->slot_fp.size() * sizeof(uint64_t));
+    }
+    out[2] = t;
+    out[3] = carry ? 1 : 0;
     return MGB_OK;
 }

@@ -35,6 +35,15 @@ struct MgbRange {
         }                                                                                                \
     } while (0)
 
+// FNV-1a over bytes, chained through h (start from MGB_FNV_BASIS): the host-side fingerprints of mgb_*_fingerprint
+#define MGB_FNV_BASIS 0xcbf29ce484222325ull
+static inline uint64_t mgb_fnv(uint64_t h, const void *p, size_t bytes)
+{
+    const unsigned char *b = static_cast<const unsigned char *>(p);
+    for (size_t i = 0; i < bytes; ++i) h = (h ^ b[i]) * 0x100000001b3ull;
+    return h;
+}
+
 // RAII "make this device current for the duration of the call"
 struct MgbDeviceGuard {
     int prev = -1;

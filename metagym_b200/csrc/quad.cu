@@ -972,7 +972,8 @@ __global__ void __launch_bounds__(kThreads) quad_step_kernel(const __grid_consta
     // start before its own step k has stored its state, so the per-block latency chain -- not the grid barrier -- sets the
     // pace, and the register file holds barely more than one launch's worth of threads.  DESIGN.md section 4.)
     asm volatile("griddepcontrol.launch_dependents;");
-    // env2task is written only by mgb_quad_set_targets, which synchronises the device: it may be read before the wait
+    // env2task is written only by mgb_quad_set_targets, which synchronises the device, and by the first of mgb_quad_restore's
+    // two kernels, never the kernel right before a step: it may be read before the wait
     const int task[1] = {active ? env_task(c, a, e) : 0};
     asm volatile("griddepcontrol.wait;" ::: "memory");
 
@@ -1386,6 +1387,7 @@ struct mgb_quad {
     uint64_t seed = 0;
     uint32_t t_base = 0;
     int64_t launches = 0;
+    uint64_t fp_map = 0, fp_targets = 0;   // fingerprints of the map (0: flat) and the target table (mgb_quad_fingerprint)
     MgbMirrors mir = {};       // mgb_quad_set_mirrors
     MgbMirrorWindow mir_win;   // mgb_quad_set_mirror_window
     // host staging for *_host entry points
@@ -1563,6 +1565,7 @@ extern "C" int mgb_quad_set_map(mgb_quad *h, const int32_t *map_host, int32_t ro
     cudaFree(h->sat);
     h->sat = nullptr;
     h->map_rows = h->map_cols = h->x_off = h->y_off = 0;
+    h->fp_map = 0;
     if (!map_host) return MGB_OK;                               // flat default map, env.py:295-298
     MGB_REQUIRE(h->c.task != MGB_TASK_VELOCITY_CONTROL, "velocity_control has no map (env.py:101-104)");
     MGB_REQUIRE(rows > 0 && cols > 0 && rows <= 8192 && cols <= 8192, "map size out of range");
@@ -1581,6 +1584,8 @@ extern "C" int mgb_quad_set_map(mgb_quad *h, const int32_t *map_host, int32_t ro
     MGB_CUDA(cudaMalloc(&h->sat, sat.size() * sizeof(int32_t)));
     MGB_CUDA(cudaMemcpy(h->sat, sat.data(), sat.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
     h->map_rows = rows; h->map_cols = cols; h->x_off = sc; h->y_off = sr;
+    h->fp_map = mgb_fnv(mgb_fnv(mgb_fnv(MGB_FNV_BASIS, &rows, sizeof(rows)), &cols, sizeof(cols)), map_host,
+                        (size_t)rows * cols * sizeof(int32_t));
     return MGB_OK;
 }
 
@@ -1604,6 +1609,9 @@ extern "C" int mgb_quad_set_targets(mgb_quad *h, const float *tbl_dev, int32_t n
     // stream would not be ordered after it (nor after the layout kernel)
     MGB_CUDA(cudaDeviceSynchronize());
     h->n_tasks = n_tasks;
+    std::vector<float4> tbl((size_t)rows);
+    MGB_CUDA(cudaMemcpy(tbl.data(), h->targets, tbl.size() * sizeof(float4), cudaMemcpyDeviceToHost));
+    h->fp_targets = mgb_fnv(mgb_fnv(MGB_FNV_BASIS, &n_tasks, sizeof(n_tasks)), tbl.data(), tbl.size() * sizeof(float4));
     return MGB_OK;
 }
 
@@ -1984,5 +1992,123 @@ extern "C" int mgb_quad_state(mgb_quad *h, float *state_dev, int32_t *ct_dev, in
     quad_state_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, state_dev, ct_dev, load);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
+    return MGB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Snapshot / restore records (DESIGN.md "Snapshot, restore and clone"): the six state planes of an env as they are in
+// HBM, then (velocity task, 0, 0, 0).  One thread per env, 16-byte loads and stores on both sides.
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int kRecordQuads = kPlanes + 1;     // uint4 per record
+
+__global__ void quad_snapshot_kernel(QuadArgs a, uint4 *__restrict__ rec)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n) return;
+    QState s;
+    load_state(a, e, s);
+    float4 q[kPlanes];
+    pack_state(s, q);
+    uint4 *r = rec + e * kRecordQuads;
+#pragma unroll
+    for (int k = 0; k < kPlanes; ++k) r[k] = make_uint4(__float_as_uint(q[k].x), __float_as_uint(q[k].y),
+                                                       __float_as_uint(q[k].z), __float_as_uint(q[k].w));
+    r[kPlanes] = make_uint4(a.env2task ? (uint32_t)a.env2task[e] : 0u, 0u, 0u, 0u);
+}
+
+// env2task gets a kernel of its own, launched before quad_restore_kernel: the step kernels read env2task before their
+// griddepcontrol.wait, so the kernel right before a step must not write it
+__global__ void quad_restore_task_kernel(int64_t n, int32_t *__restrict__ env2task, int n_tasks, const uint4 *__restrict__ rec,
+                                         int64_t n_rec, const int64_t *__restrict__ row)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const int64_t r = row[e];
+    if (r < 0 || r >= n_rec) return;
+    const int t = (int)rec[r * kRecordQuads + kPlanes].x;
+    if (t >= 0 && t < n_tasks) env2task[e] = t;
+}
+
+__global__ void quad_restore_kernel(QuadArgs a, const uint4 *__restrict__ rec, int64_t n_rec, const int64_t *__restrict__ row)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n) return;
+    const int64_t r = row[e];
+    if (r < 0 || r >= n_rec) return;
+    const uint4 *src = rec + r * kRecordQuads;
+    float4 q[kPlanes];
+#pragma unroll
+    for (int k = 0; k < kPlanes; ++k) {
+        const uint4 u = src[k];
+        q[k] = make_float4(__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w));
+    }
+    QState s;
+    unpack_state(q, s);
+    store_state(a, e, s);
+}
+
+}  // namespace
+
+extern "C" int64_t mgb_quad_record_bytes(const mgb_quad *h) { return h ? (int64_t)kRecordQuads * 16 : MGB_ERR_ARG; }
+
+extern "C" int mgb_quad_snapshot(mgb_quad *h, uint8_t *rec_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_snapshot");
+    MGB_REQUIRE(h && rec_dev, "null argument");
+    MGB_REQUIRE((reinterpret_cast<uintptr_t>(rec_dev) & 15u) == 0, "rec_dev must be 16-byte aligned");
+    MgbDeviceGuard guard(h->device);
+    QuadArgs a = base_args(h);
+    quad_snapshot_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, reinterpret_cast<uint4 *>(rec_dev));
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
+extern "C" int mgb_quad_restore(mgb_quad *h, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row_of_env_dev,
+                                void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_restore");
+    MGB_REQUIRE(h && rec_dev && row_of_env_dev, "null argument");
+    MGB_REQUIRE(n_rec >= 0, "n_rec must not be negative");
+    MGB_REQUIRE((reinterpret_cast<uintptr_t>(rec_dev) & 15u) == 0, "rec_dev must be 16-byte aligned");
+    int rc = check_ready(h);
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned blocks = (unsigned)((h->n + 255) / 256);
+    const uint4 *rec = reinterpret_cast<const uint4 *>(rec_dev);
+    if (h->env2task) {
+        quad_restore_task_kernel<<<blocks, 256, 0, st>>>(h->n, h->env2task, h->n_tasks, rec, n_rec, row_of_env_dev);
+        MGB_CUDA(cudaGetLastError());
+        h->launches += 1;
+    }
+    QuadArgs a = base_args(h);
+    quad_restore_kernel<<<blocks, 256, 0, st>>>(a, rec, n_rec, row_of_env_dev);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
+extern "C" int mgb_quad_counters(mgb_quad *h, uint64_t *t_base, int set)
+{
+    MGB_REQUIRE(h && t_base, "null argument");
+    if (set) h->t_base = (uint32_t)*t_base;
+    else *t_base = h->t_base;
+    return MGB_OK;
+}
+
+extern "C" int mgb_quad_fingerprint(const mgb_quad *h, uint64_t *out)
+{
+    MGB_REQUIRE(h && out, "null argument");
+    const int64_t rec_bytes = (int64_t)kRecordQuads * 16;
+    uint64_t f = mgb_fnv(MGB_FNV_BASIS, &h->cfg, sizeof(h->cfg));
+    f = mgb_fnv(f, &h->auto_reset, sizeof(h->auto_reset));
+    f = mgb_fnv(f, &h->seed, sizeof(h->seed));
+    out[0] = mgb_fnv(f, &rec_bytes, sizeof(rec_bytes));
+    out[1] = h->fp_map;
+    out[2] = h->fp_targets;
+    out[3] = 0;
     return MGB_OK;
 }

@@ -12,6 +12,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import _lib
+from .snapshot import Snapshots
 from .spaces import Box, Discrete
 from .textures import synthetic_textures
 
@@ -194,8 +195,25 @@ def MazeTaskSampler(n=15, allow_loops=True, cell_size=2.0, wall_height=3.2, agen
                       food_interval=interval)
 
 
-class _BatchedMazeBase(object):
+class _BatchedMazeBase(Snapshots):
+    """snapshot() / restore() / clone_envs() (metagym_b200/snapshot.py): exact checkpoint and resume of agent, life, food,
+    resample counts, continuous pose, task slot (and, for one table slot per env on the direct renderer, the task itself)
+    and the rollout action counter.  A restore clears need_reset."""
     KIND = None
+    _SNAP_PREFIX = "mgb_maze"
+    _FINGERPRINT_PARTS = ("configuration (kind, task type, max_steps, view, resolution, obs dtype, optics, auto_reset, "
+                          "table shape)", "textures", "task table", "record mode (per-env tasks or a shared table)")
+
+    def _snap_kind(self):
+        return ("maze2d", "maze_discrete_3d", "maze_continuous_3d")[self.KIND]
+
+    def _after_restore(self, rec, row_dev, row):
+        """A shared-table restore points env2task at the records' slots (int32 7 of a record)."""
+        self.need_reset = False
+        if self._fingerprint()[3] == 0 and rec.shape[0]:
+            slot = rec.view(self._torch.int32)[:, 7].cpu().numpy()
+            self.env2task = np.ascontiguousarray(np.where(row >= 0, slot[np.maximum(row, 0)], self.env2task),
+                                                 dtype=np.int32)
 
     def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs=False):
         import torch

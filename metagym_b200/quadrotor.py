@@ -11,6 +11,7 @@ import os
 import numpy as np
 
 from . import _lib
+from .snapshot import Snapshots
 from .spaces import Box, Space
 
 TASKS = {"no_collision": 0, "hovering_control": 1, "velocity_control": 2}
@@ -124,7 +125,7 @@ class QuadInfo(dict):
         return list(self._keys)
 
 
-class BatchedQuadrotor(object):
+class BatchedQuadrotor(Snapshots):
     """`Quadrotor(dt, nt, seed, task, map_file, simulator_conf, healthy_reward)` x num_envs on one H100.
 
     Extra kwargs: num_envs, device (int or 'cuda:k'), auto_reset (finished envs restart inside the step launch),
@@ -135,8 +136,13 @@ class BatchedQuadrotor(object):
     flies task `env2task[i]` (default i % n_tasks).
     final_obs=True (needs auto_reset=True): every step() also reports `truncated`, and rollout() also returns the
     terminal observations and truncation flags of its steps.
+    snapshot() / restore() / clone_envs(): exact checkpoint and resume of the whole env state -- rigid body, ct, episode
+    counter, velocity task and the rollout action counter -- also into another sharding (metagym_b200/snapshot.py).
     """
     metadata = {"render.modes": []}
+    _SNAP_PREFIX = "mgb_quad"
+    _FINGERPRINT_PARTS = ("configuration (physics, dt, nt, task, integrator, auto_reset, rng_seed)", "obstacle map",
+                          "velocity-target table", "record layout")
 
     def __init__(self, dt=0.01, nt=1000, seed=0, task="no_collision", map_file=None, simulator_conf=None,
                  healthy_reward=1.0, num_envs=1, device=0, auto_reset=False, rng_seed=0, env_index_base=0,
@@ -443,6 +449,18 @@ class BatchedQuadrotor(object):
             ct = torch.as_tensor(ct, device=self.device).to(torch.int32).contiguous()
         _lib.check(self._lib.mgb_quad_state(self._h, st.data_ptr(), _lib.ptr(ct), 1, self._stream()))
         torch.cuda.current_stream(self.device).synchronize()
+
+    def _snap_kind(self):
+        return "quadrotor"
+
+    def _after_restore(self, rec, row_dev, row):
+        """env2task follows the restored velocity tasks (int32 24 of a record; mgb_quad_restore skips invalid ones)."""
+        if self.task != "velocity_control" or rec.shape[0] == 0:
+            return
+        torch = self._torch
+        task = rec.view(torch.int32)[:, 24][row_dev.clamp(min=0)]
+        take = (row_dev >= 0) & (task >= 0) & (task < self.velocity_targets.shape[0])
+        self.env2task = torch.where(take, task, self.env2task)
 
     @property
     def launch_count(self):
