@@ -407,6 +407,21 @@ int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);
 int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev, void *stream);
 int64_t mgb_maze_launch_count(const mgb_maze *h);
 
+/* God view (the right-hand panel that MazeBase.render_init + render_update draw, maze_base.py:100-157, with the agent
+ * marker of maze_2d.py:73-75 / maze_discrete_3d.py:88-99 / maze_continuous_3d.py:63-74) of `count` envs in one launch:
+ * white floor, black walls, the ESCAPE goal in green, SURVIVAL food as (f, 255, f) with f = int(255 - 255 food) on the
+ * live food state, then the agent (2-D: red cell; 3-D: green disc and heading line).  The text labels are not drawn.
+ *   envs_dev [count] int32 local env indices, or NULL for envs 0 .. count-1 (count <= n_envs); an index outside
+ *     [0, n_envs) gives an all-zero frame.
+ *   view_size S in [1, 4096]: the reference's render_scale; cell size S / n_cells, need not be an integer.
+ *   out_dev [count][S][S][3] uint8, IMAGE ROWS TOP TO BOTTOM: out[k][y][x] is pygame pixel (x, y) of the panel, as a saved
+ *     PNG shows it.  This is transposed against the x-major observation arrays ([res_h][res_v][3]).
+ * mode: MGB_GOD_LIVE (the current state; nothing needs recording).  Pixel rules: DESIGN.md "God view".  Stream-ordered,
+ * no host synchronisation, no allocation: capturable in a CUDA graph. */
+#define MGB_GOD_LIVE 0
+int mgb_maze_god_view(mgb_maze *h, int32_t count, const int32_t *envs_dev, int32_t view_size, int32_t mode,
+                      uint8_t *out_dev, void *stream);
+
 /* Exact snapshot / restore of env state, as mgb_quad_snapshot / mgb_quad_restore (same row map and stream rules).  A
  * record of mgb_maze_record_bytes(h) bytes (after mgb_maze_set_task) holds agent (int4), life, the env's resample count,
  * its task-table slot, the continuous pose, the food stamps of every food slot and -- when the handle owns one table

@@ -3533,6 +3533,313 @@ extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const floa
                               stream);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// God view: the right-hand panel of the reference window (MazeBase.render_init + render_update, maze_base.py:100-157,
+// with the agent marker of maze_2d.py:73-75, maze_discrete_3d.py:83-99 and maze_continuous_3d.py:58-74) for many envs per
+// launch.  One CTA (or a few, for small batches) per env: the env's cells and the pixel -> cell tables are staged in shared
+// memory, then every thread colours 16 pixels at a time and stores them as three 16-byte words.  The pixel rules (rect by
+// pixel centre, disc and Bresenham line on truncated coordinates) are DESIGN.md "God view"; oracle/maze_godview.py states
+// them again in numpy.
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr int kGodThreads = 256;
+constexpr int kGodPx = 16;                       // pixels per item: 48 bytes, three 16-byte stores
+constexpr int kGodMaxView = 4096;
+constexpr uint32_t kGodNone = 0xFFFFFFFFu;       // colours are 0x00BBGGRR: the bytes leave in R, G, B order
+constexpr uint32_t kGodWhite = 0xFFFFFFu, kGodBlack = 0u, kGodGreen = 0x00FF00u, kGodRed = 0x0000FFu;
+
+struct GodEnv {
+    int valid;                   // 0: env index out of range, the frame is written as zeros
+    int gx, gy;                  // 2-D: the red agent cell
+    int dcx, dcy, dr2;           // 3-D: disc centre and squared radius (dr2 < 0: nothing drawn)
+    int lx0, ly0, lx1, ly1;      // 3-D: heading line end points
+    int bx0, by0, bx1, by1;      // 3-D: bounding box of disc and line (empty for 2-D)
+};
+
+// int() of a screen coordinate; far-off values are clamped so that the integer arithmetic below cannot overflow
+__device__ __forceinline__ int god_trunc(double v)
+{
+    return (int)(v < -1.0e9 ? -1.0e9 : (v > 1.0e9 ? 1.0e9 : v));
+}
+
+// Bresenham: the major axis steps by one from the start point; at step i the minor offset is i d_minor / d_major rounded
+// half up (a tie moves toward the end point)
+__device__ __forceinline__ bool god_on_line(int px, int py, const GodEnv &g)
+{
+    const int dx = abs(g.lx1 - g.lx0), dy = abs(g.ly1 - g.ly0);
+    const int sx = g.lx1 >= g.lx0 ? 1 : -1, sy = g.ly1 >= g.ly0 ? 1 : -1;
+    if (dx >= dy) {
+        const int i = (px - g.lx0) * sx;
+        if (i < 0 || i > dx) return false;
+        if (dx == 0) return py == g.ly0;
+        return py == g.ly0 + sy * (int)((2LL * i * dy + dx) / (2LL * dx));
+    }
+    const int i = (py - g.ly0) * sy;
+    if (i < 0 || i > dy) return false;
+    return px == g.lx0 + sx * (int)((2LL * i * dx + dy) / (2LL * dy));
+}
+
+__device__ __forceinline__ void god_push(char2 &v, int cell)
+{
+    if (v.x < 0) v.x = (char)cell; else if (v.y < 0) v.y = (char)cell;
+}
+
+// The agent marker of one env in panel coordinates, typed like the reference computes it: the discrete 3-D env and a
+// continuous env at reset hold python floats as position (float64) and the continuous env's position after a step is a
+// float32 array, so `agent_pos = pos * pos_conversion` and `agent_pos + view_size` are float32 there; after a step the
+// discrete heading is a float32 table entry, so its cos / sin and `ori_size * cos` are float32 too.  Right after a reset
+// both 3-D envs have the heading 0.0 that MazeBase.reset leaves.
+// heading: cos / sin of the four float32 heading table entries (computed once on the host, mgb_maze_god_view).
+__device__ void god_marker(const MazeConst &c, const MazeArgs &a, const TaskHdr *th, int64_t e, int S,
+                           const float4 &hcos, const float4 &hsin, GodEnv &g)
+{
+    const int4 ag = a.agent[e];
+    g.gx = ag.x; g.gy = ag.y;
+    g.dr2 = -1;
+    g.bx0 = g.by0 = 1; g.bx1 = g.by1 = 0;
+    if (c.kind == MGB_MAZE_2D) return;
+    const double rcs = (double)S / (double)c.n;                   // render_init: view_size / self._n
+    const double pc = rcs / th->cell_size;                        // self._pos_conversion
+    const double ori_size = 0.60 * pc;
+    double cx, cy, ex, ey;
+    if (c.kind == MGB_MAZE_CONTINUOUS_3D && ag.w > 0) {
+        const float2 p = a.cpos[e];
+        const float ax = p.x * (float)pc, ay = p.y * (float)pc;
+        const float fcx = ax + (float)S, fcy = (float)S - ay;
+        const double o = a.cori[e];
+        cx = (double)fcx; cy = (double)fcy;
+        ex = cx + ori_size * cos(o);
+        ey = cy - ori_size * sin(o);
+    } else {
+        const double ax = (ag.x * th->cell_size + 0.5 * th->cell_size) * pc;   // get_cell_center, maze_base.py:194-197
+        const double ay = (ag.y * th->cell_size + 0.5 * th->cell_size) * pc;
+        cx = ax + (double)S; cy = (double)S - ay;
+        if (c.kind == MGB_MAZE_DISCRETE_3D && ag.w > 0) {
+            const int k = ag.z & 3;
+            const float co = k == 0 ? hcos.x : (k == 1 ? hcos.y : (k == 2 ? hcos.z : hcos.w));
+            const float si = k == 0 ? hsin.x : (k == 1 ? hsin.y : (k == 2 ? hsin.z : hsin.w));
+            ex = cx + (double)((float)ori_size * co);
+            ey = cy - (double)((float)ori_size * si);
+        } else {                                                   // heading 0.0 after reset (maze_base.py:50)
+            ex = cx + ori_size * 1.0;
+            ey = cy - ori_size * 0.0;
+        }
+    }
+    const int r = god_trunc(0.15 * pc);
+    g.dcx = god_trunc(cx) - S; g.dcy = god_trunc(cy);
+    g.dr2 = r >= 1 ? r * r : -1;
+    g.lx0 = g.dcx; g.ly0 = g.dcy;
+    g.lx1 = god_trunc(ex) - S; g.ly1 = god_trunc(ey);
+    const int rr = r >= 1 ? r : 0;
+    g.bx0 = min(min(g.lx0, g.lx1), g.dcx - rr); g.bx1 = max(max(g.lx0, g.lx1), g.dcx + rr);
+    g.by0 = min(min(g.ly0, g.ly1), g.dcy - rr); g.by1 = max(max(g.ly0, g.ly1), g.dcy + rr);
+}
+
+__global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid_constant__ MazeConst c,
+                                                                    const __grid_constant__ MazeArgs a,
+                                                                    const int32_t *__restrict__ envs, int S,
+                                                                    const float4 hcos, const float4 hsin,
+                                                                    uint8_t *__restrict__ out)
+{
+    extern __shared__ __align__(16) uint32_t god_smem[];
+    __shared__ GodEnv g;
+    __shared__ uint4 stage[kGodThreads / 32][3 * 32];              // per warp: 32 items of 48 bytes, stored coalesced
+    const int n = c.n, nn = n * n;
+    uint32_t *base = god_smem;                                     // [nn] wall / goal colour or kGodNone
+    uint32_t *food = god_smem + nn;                                // [nn] food colour or kGodNone
+    uint32_t *cell = god_smem + 2 * nn;                            // [nn] final colour of a pixel inside this cell only
+    char2 *xg = reinterpret_cast<char2 *>(god_smem + 3 * nn);      // [S] cells whose rect holds the pixel column (_surf_god)
+    char2 *xs = xg + S;                                            // [S] the same for rects drawn on the screen (x + view_size)
+    char2 *yc = xs + S;                                            // [S] cells whose rect holds the pixel row
+    // [S] each: the one cell holding the column (in both xg and xs) / the row, or -1 when a pixel there can lie in none or
+    // in two cells' rects (a cell edge within rounding of a pixel centre): such pixels take the general path
+    int8_t *colx = reinterpret_cast<int8_t *>(yc + S);
+    int8_t *rowy = colx + S;
+    const int64_t k = blockIdx.x;
+    const int64_t e = envs ? (int64_t)envs[k] : k;
+    const bool valid = e >= 0 && e < a.n;
+    const uint8_t *blob = valid ? a.blobs + (int64_t)a.env2task[e] * c.blob_bytes : nullptr;
+    const TaskHdr *th = valid ? blob_hdr(blob) : nullptr;
+    if (threadIdx.x == 0) {
+        g.valid = valid;
+        if (valid) god_marker(c, a, th, e, S, hcos, hsin, g);
+    }
+    if (valid) {
+        const int8_t *walls = reinterpret_cast<const int8_t *>(blob + c.off_walls);
+        const int4 ag = a.agent[e];
+        const int steps = ag.w;
+        for (int i = threadIdx.x; i < nn; i += blockDim.x) {      // render_init (walls, ESCAPE goal) and draw_food
+            const int x = i / n, y = i - x * n;
+            uint32_t b = walls[i] > 0 ? kGodBlack : kGodNone;
+            if (c.task_type == MGB_MAZE_ESCAPE && x == th->goal[0] && y == th->goal[1]) b = kGodGreen;
+            uint32_t f = kGodNone;
+            if (c.task_type == MGB_MAZE_SURVIVAL) {
+                const double v = food_now(c, blob, a.eaten + e, a.n_pad, steps, i);
+                if (v > 1.0e-2) {
+                    const double fv = 255.0 - 255.0 * v;          // int(255 - 255 * food), clamped to a colour
+                    const uint32_t q = fv <= 0.0 ? 0u : (fv >= 255.0 ? 255u : (uint32_t)fv);
+                    f = q | (255u << 8) | (q << 16);
+                }
+            }
+            base[i] = b; food[i] = f;
+            uint32_t v = f != kGodNone ? f : (b != kGodNone ? b : kGodWhite);
+            if (c.kind == MGB_MAZE_2D && x == ag.x && y == ag.y) v = kGodRed;
+            cell[i] = v;
+        }
+        const double rcs = (double)S / (double)n;
+        for (int p = threadIdx.x; p < S; p += blockDim.x) {
+            const double pcen = (double)p + 0.5;
+            const int cx0 = (int)(pcen / rcs), cy0 = (int)(((double)S - pcen) / rcs);   // y points up
+            char2 vg = make_char2(-1, -1), vs = make_char2(-1, -1), vy = make_char2(-1, -1);
+            for (int d = -1; d <= 1; ++d) {
+                const int q = cx0 + d, r = cy0 + d;
+                if (q >= 0 && q < n) {
+                    const double x0 = q * rcs;                     // x * self._render_cell_size
+                    if (x0 <= pcen && pcen < x0 + rcs) god_push(vg, q);
+                    const double x1 = q * rcs + (double)S;         // ... + offset[0] (draw_food, the 2-D agent rect)
+                    if (x1 <= pcen + (double)S && pcen + (double)S < x1 + rcs) god_push(vs, q);
+                }
+                if (r >= 0 && r < n) {
+                    const double y0 = (double)S - (r + 1) * rcs;   // view_size - (y + 1) * self._render_cell_size
+                    if (y0 <= pcen && pcen < y0 + rcs) god_push(vy, r);
+                }
+            }
+            xg[p] = vg; xs[p] = vs; yc[p] = vy;
+            colx[p] = (vg.x >= 0 && vg.y < 0 && vs.y < 0 && vs.x == vg.x) ? vg.x : (int8_t)-1;
+            rowy[p] = (vy.x >= 0 && vy.y < 0) ? vy.x : (int8_t)-1;
+        }
+    }
+    __syncthreads();
+    const GodEnv ge = g;
+    const bool is2d = c.kind == MGB_MAZE_2D, surv = c.task_type == MGB_MAZE_SURVIVAL;
+    // every primitive that can cover the pixel, in the reference's draw order (used where a pixel is not inside one cell)
+    auto general = [&](int row, int col) -> uint32_t {
+        uint32_t v = kGodWhite;
+        const char2 cy = yc[row], cg = xg[col], cs = xs[col];
+        const int ys[2] = {cy.x, cy.y}, gs[2] = {cg.x, cg.y}, ss[2] = {cs.x, cs.y};
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+                if (gs[i] >= 0 && ys[j] >= 0) {
+                    const uint32_t b = base[gs[i] * n + ys[j]];
+                    if (b != kGodNone) v = b;
+                }
+        if (surv) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 2; ++j)
+                    if (ss[i] >= 0 && ys[j] >= 0) {
+                        const uint32_t f = food[ss[i] * n + ys[j]];
+                        if (f != kGodNone) v = f;
+                    }
+        }
+        if (is2d && (ss[0] == ge.gx || ss[1] == ge.gx) && (ys[0] == ge.gy || ys[1] == ge.gy)) v = kGodRed;
+        return v;
+    };
+    auto colour = [&](int row, int col, int cy) -> uint32_t {
+        if (!ge.valid) return 0u;
+        const int cx = colx[col];
+        uint32_t v = (cx >= 0 && cy >= 0) ? cell[cx * n + cy] : general(row, col);
+        if (col >= ge.bx0 && col <= ge.bx1 && row >= ge.by0 && row <= ge.by1) {    // 3-D agent marker
+            const int64_t dx = col - ge.dcx, dy = row - ge.dcy;
+            if (dx * dx + dy * dy <= (int64_t)ge.dr2 || god_on_line(col, row, ge)) v = kGodGreen;
+        }
+        return v;
+    };
+    const int64_t npx = (int64_t)S * S;
+    uint8_t *frame = out + k * npx * 3;
+    const int64_t items = (npx + kGodPx - 1) / kGodPx;
+    const int64_t full = (reinterpret_cast<uintptr_t>(frame) & 15u) == 0 ? npx / kGodPx : 0;   // items stored as 16-byte words
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = kGodThreads / 32;
+    // a warp takes 32 consecutive items (1536 contiguous bytes): each lane colours 16 pixels, the warp's words go through
+    // shared memory so that each of its three store instructions writes 512 contiguous bytes
+    for (int64_t wb = ((int64_t)blockIdx.y * nwarps + warp) * 32; wb < items; wb += (int64_t)gridDim.y * nwarps * 32) {
+        const int64_t it = wb + lane;
+        if (it >= items) continue;
+        const int64_t p0 = it * kGodPx;
+        int row = (int)(p0 / S), col = (int)(p0 - (int64_t)row * S);
+        uint32_t px[kGodPx];
+        int cy = rowy[row];                                        // the row's cell, reloaded only where the row changes
+#pragma unroll
+        for (int j = 0; j < kGodPx; ++j) {
+            px[j] = row < S ? colour(row, col, cy) : 0u;
+            if (++col == S) { col = 0; ++row; cy = row < S ? rowy[row] : -1; }
+        }
+        if (it < full) {
+            uint32_t w[12];
+#pragma unroll
+            for (int i = 0; i < 12; ++i) {
+                uint32_t v = 0;
+#pragma unroll
+                for (int b = 0; b < 4; ++b) v |= ((px[(4 * i + b) / 3] >> (8 * ((4 * i + b) % 3))) & 0xFFu) << (8 * b);
+                w[i] = v;
+            }
+            if (wb + 32 <= full) {                                 // warp-uniform: all 32 items are whole words
+                stage[warp][3 * lane] = make_uint4(w[0], w[1], w[2], w[3]);
+                stage[warp][3 * lane + 1] = make_uint4(w[4], w[5], w[6], w[7]);
+                stage[warp][3 * lane + 2] = make_uint4(w[8], w[9], w[10], w[11]);
+                __syncwarp();
+                uint4 *dst = reinterpret_cast<uint4 *>(frame + wb * kGodPx * 3);
+#pragma unroll
+                for (int i = 0; i < 3; ++i) __stcs(dst + i * 32 + lane, stage[warp][i * 32 + lane]);
+                __syncwarp();
+            } else {
+                uint4 *dst = reinterpret_cast<uint4 *>(frame + p0 * 3);
+                __stcs(dst, make_uint4(w[0], w[1], w[2], w[3]));
+                __stcs(dst + 1, make_uint4(w[4], w[5], w[6], w[7]));
+                __stcs(dst + 2, make_uint4(w[8], w[9], w[10], w[11]));
+            }
+        } else {
+            for (int j = 0; j < kGodPx && p0 + j < npx; ++j) {
+                uint8_t *d = frame + (p0 + j) * 3;
+                d[0] = (uint8_t)px[j]; d[1] = (uint8_t)(px[j] >> 8); d[2] = (uint8_t)(px[j] >> 16);
+            }
+        }
+    }
+}
+
+}  // namespace
+
+extern "C" int mgb_maze_god_view(mgb_maze *h, int32_t count, const int32_t *envs_dev, int32_t view_size, int32_t mode,
+                                 uint8_t *out_dev, void *stream)
+{
+    MGB_REQUIRE(h, "null argument");
+    MGB_REQUIRE(mode == MGB_GOD_LIVE, "mgb_maze_god_view: mode must be MGB_GOD_LIVE");
+    MGB_REQUIRE(count >= 0 && count <= INT_MAX / 2, "mgb_maze_god_view: count out of range");
+    MGB_REQUIRE(view_size >= 1 && view_size <= kGodMaxView, "mgb_maze_god_view: view_size must be in [1, 4096]");
+    MGB_REQUIRE(h->has_task, "mgb_maze_god_view: set a task first");
+    if (count == 0) return MGB_OK;
+    MGB_REQUIRE(out_dev, "mgb_maze_god_view: null output");
+    MGB_REQUIRE(envs_dev || count <= h->n, "mgb_maze_god_view: count exceeds the env count (pass envs_dev)");
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    const int64_t items = ((int64_t)view_size * view_size + kGodPx - 1) / kGodPx;
+    // enough CTAs to fill the GPU when the batch is small; one CTA per env otherwise
+    const int64_t want = (int64_t)(h->num_sms > 0 ? h->num_sms : 132) * 8;
+    int64_t split = (want + count - 1) / count;
+    const int64_t most = (items + kGodThreads - 1) / kGodThreads;
+    split = split < most ? split : most;
+    split = split < 65535 ? split : 65535;
+    // maze_discrete_3d.py:46: float32 table entries k * 0.5 * PI, and numpy's float32 cos / sin of them.  Computed here so
+    // that the kernel needs no device trig table (which would renumber the module's constant-bank entries that the other
+    // kernels reference).
+    float hc[4], hs[4];
+    for (int k = 0; k < 4; ++k) {
+        const float o = (float)(0.5 * k) * (float)3.1415926;
+        hc[k] = cosf(o); hs[k] = sinf(o);
+    }
+    const size_t smem = (size_t)3 * h->c.n * h->c.n * 4 + (size_t)3 * view_size * sizeof(char2) + (size_t)2 * view_size;
+    maze_god_view_kernel<<<dim3((unsigned)count, (unsigned)split), kGodThreads, smem, (cudaStream_t)stream>>>(
+        h->c, a, envs_dev, view_size, make_float4(hc[0], hc[1], hc[2], hc[3]), make_float4(hs[0], hs[1], hs[2], hs[3]),
+        out_dev);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
 __global__ void maze_pose_kernel(MazeArgs a, float *pos_out, double *ori_out)
 {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

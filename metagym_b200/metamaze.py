@@ -476,8 +476,50 @@ class _BatchedMazeBase(Snapshots):
     def launch_count(self):
         return int(self._lib.mgb_maze_launch_count(self._h)) if self._h else 0
 
+    def god_view(self, envs=None, view_size=None, out=None):
+        """Top-down views of many envs in one launch (mgb_maze_god_view): the god panel of the reference window
+        (render_init + render_update, maze_base.py:100-157): white floor, black walls, the ESCAPE goal in green, SURVIVAL
+        food in (f, 255, f) with f = int(255 - 255 food), and the agent (2-D: red cell; 3-D: green disc and heading line).
+        The text labels are not drawn.
+
+        envs: local env indices (default: all), a host sequence (checked) or a CUDA tensor, moved to the env's device as
+        int32 (not checked: an index out of range gives an all-zero frame; no host synchronisation, so the call can be
+        captured in a CUDA graph).
+        view_size: the panel's side S in pixels (default: the constructor's render_scale).  Returns (or fills `out`) a
+        CUDA uint8 tensor [K, S, S, 3] with image rows top to bottom, as a saved picture shows it: out[k, y, x] is pixel
+        (x, y) of the panel, so it is transposed against the x-major 3-D observations."""
+        if self.need_set_task:
+            raise Exception("Must call \"set_task\" before reset")
+        torch = self._torch
+        S = self.render_scale if view_size is None else view_size
+        if int(S) != S or not 1 <= int(S) <= 4096:
+            raise ValueError("view_size must be an integer in [1, 4096], got %r" % (view_size,))
+        S = int(S)
+        e = None
+        K = self.num_envs
+        if envs is not None:
+            if hasattr(envs, "is_cuda") and envs.is_cuda:
+                e = envs.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
+            else:
+                idx = np.asarray(envs, dtype=np.int64).reshape(-1)
+                if idx.size and (idx.min() < 0 or idx.max() >= self.num_envs):
+                    raise IndexError("env index out of range [0, %d)" % self.num_envs)
+                e = torch.as_tensor(idx.astype(np.int32), device=self.device)
+            K = int(e.numel())
+        if out is None:
+            out = torch.empty((K, S, S, 3), dtype=torch.uint8, device=self.device)
+        elif (tuple(out.shape) != (K, S, S, 3) or out.dtype != torch.uint8 or out.device != self.device
+              or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous uint8 tensor of shape %s on %s" % ((K, S, S, 3), self.device))
+        _lib.check(self._lib.mgb_maze_god_view(self._h, K, _lib.ptr(e), S, 0, _lib.ptr(out), self._stream()))
+        return out
+
     def render(self, mode="human"):
-        raise NotImplementedError("the pygame god-view (maze_base.py:100-189) is out of scope for the batched engine")
+        """mode="rgb_array": god_view() of every env at render_scale ([S, S, 3] for num_envs=1 with squeeze).  The
+        reference's window (mode "human") needs a display, which the batched engine does not have."""
+        if mode != "rgb_array":
+            raise NotImplementedError("render(mode=%r): the batched engine is headless; use mode=\"rgb_array\"" % (mode,))
+        return self._out(self.god_view())
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h:
@@ -519,6 +561,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
+        self.render_scale = int(render_scale)
         self.view_grid = int(view_grid)
         self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs)
         w = 2 * self.view_grid + 1
@@ -577,6 +620,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
+        self.render_scale = int(render_scale)
         self.resolution = (int(resolution[0]), int(resolution[1]))
         assert obs_dtype in ("int32", "uint8", "float32")
         self.obs_dtype = obs_dtype
