@@ -3341,9 +3341,8 @@ static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_
     a.T = T; a.act_seed = act_seed; a.t_base = h->t_base; a.act_out = act_out_dev;
     a.mir = h->mir;
     if (h->mir.count != 0)
-        MGB_REQUIRE(h->mir_win.holds(obs_dev, (uint64_t)T * h->n * (uint64_t)mgb_maze_obs_bytes_per_env(h)) &&
-                        h->mir_win.holds(rew_dev, (uint64_t)T * h->n * 8) && h->mir_win.holds(done_dev, (uint64_t)T * h->n) &&
-                        h->mir_win.holds(act_out_dev, (uint64_t)T * h->n * 4),
+        MGB_REQUIRE(h->mir_win.holds_rollout((uint64_t)T * h->n, obs_dev, (uint64_t)mgb_maze_obs_bytes_per_env(h), rew_dev, 8,
+                                             done_dev, act_out_dev, 4),
                     "mirrors are on but an output lies outside the mirrored arena (set_mirrors([]) first)");
     cudaStream_t st = (cudaStream_t)stream;
     if (h->c.kind == MGB_MAZE_DISCRETE_3D) {
@@ -3438,32 +3437,23 @@ extern "C" int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)
 {
     MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE(count >= 0 && count <= MGB_MAX_MIRRORS && (count == 0 || byte_delta), "count out of range");
-    MgbMirrors m = {};
-    for (int i = 0; i < count; ++i) {
-        MGB_REQUIRE((byte_delta[i] & 15) == 0, "mirror deltas must be multiples of 16 bytes");
-        m.delta[i] = byte_delta[i];
-    }
-    m.count = count;
-    h->mir = m;
+    const char *why = h->mir.set_peers(count, byte_delta);
+    MGB_REQUIRE(!why, why);
     return MGB_OK;
 }
 
 extern "C" int mgb_maze_set_mirror_window(mgb_maze *h, const void *base, uint64_t bytes)
 {
     MGB_REQUIRE(h, "null handle");
-    h->mir_win.base = reinterpret_cast<uintptr_t>(base);
-    h->mir_win.bytes = bytes;
+    h->mir_win.set(base, bytes);
     return MGB_OK;
 }
 
 extern "C" int mgb_maze_set_multicast(mgb_maze *h, int64_t byte_delta)
 {
     MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE((byte_delta & 15) == 0, "multicast delta must be a multiple of 16 bytes");
-    MgbMirrors m = {};
-    if (byte_delta != 0) { m.count = MGB_MIRROR_MULTICAST; m.delta[0] = byte_delta; }
-    h->mir = m;
+    const char *why = h->mir.set_multicast(byte_delta);
+    MGB_REQUIRE(!why, why);
     return MGB_OK;
 }
 

@@ -129,16 +129,52 @@ struct MgbMirrors {
     int count;                        // > 0: peer mirrors; MGB_MIRROR_MULTICAST: delta[0] = multicast base - local base
 #define MGB_MIRROR_MULTICAST (-1)
     int64_t delta[MGB_MAX_MIRRORS];   // bytes
+
+    // The bodies of mgb_*_set_mirrors and mgb_*_set_multicast: the refusal, or nullptr once *this holds the new
+    // mirrors (left unchanged on a refusal).  The callers refuse in their own name.
+    const char *set_peers(int n, const int64_t *byte_delta)
+    {
+        if (!(n >= 0 && n <= MGB_MAX_MIRRORS && (n == 0 || byte_delta))) return "count out of range";
+        MgbMirrors m = {};
+        for (int i = 0; i < n; ++i) {
+            if ((byte_delta[i] & 15) != 0) return "mirror deltas must be multiples of 16 bytes";
+            m.delta[i] = byte_delta[i];
+        }
+        m.count = n;
+        *this = m;
+        return nullptr;
+    }
+    const char *set_multicast(int64_t byte_delta)
+    {
+        if ((byte_delta & 15) != 0) return "multicast delta must be a multiple of 16 bytes";
+        MgbMirrors m = {};
+        if (byte_delta != 0) { m.count = MGB_MIRROR_MULTICAST; m.delta[0] = byte_delta; }
+        *this = m;
+        return nullptr;
+    }
 };
 struct MgbMirrorWindow {             // host side: where mirrored outputs must lie (0 bytes = unchecked)
     uintptr_t base = 0;
     uint64_t bytes = 0;
+    void set(const void *p, uint64_t len)
+    {
+        base = reinterpret_cast<uintptr_t>(p);
+        bytes = len;
+    }
     // the whole extent [p, p + len) must lie inside the window: a rollout with a larger T or N than the arena slot was
     // laid out for would otherwise store `ptr + delta` past the peer's slot
     bool holds(const void *p, uint64_t len) const
     {
         const uintptr_t q = reinterpret_cast<uintptr_t>(p);
         return p == nullptr || bytes == 0 || (q >= base && len <= bytes && q - base <= bytes - len);
+    }
+    // every output of a rollout of `env_steps` = T x n env-steps: observations, rewards, done flags and recorded
+    // actions of obs_bytes / rew_bytes / 1 / act_bytes bytes per env-step
+    bool holds_rollout(uint64_t env_steps, const void *obs, uint64_t obs_bytes, const void *rew, uint64_t rew_bytes,
+                       const void *done, const void *act, uint64_t act_bytes) const
+    {
+        return holds(obs, env_steps * obs_bytes) && holds(rew, env_steps * rew_bytes) && holds(done, env_steps) &&
+               holds(act, env_steps * act_bytes);
     }
 };
 template <typename T> __device__ __forceinline__ void mgb_mirror_store(const MgbMirrors &m, T *p, const T v)

@@ -22,6 +22,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include "mgb_common.cuh"
@@ -1379,7 +1380,7 @@ struct mgb_quad {
     int n_tasks = 0;
     int auto_reset = 0;
     int num_sms = 132;
-    int wide_kernel = -1;      // MGB_WIDE_KERNEL: unset = by batch size (choose_step_kernel), 1 = every single-wave launch, 0 = never
+    int wide_kernel = -1;      // MGB_WIDE_KERNEL: unset = by batch size (plan_step), 1 = every single-wave launch, 0 = never
     int packed = 0;            // MGB_PACKED=1: two envs per thread (bit-identical to one env per thread)
     int stream_kernel = 1;     // persistent TMA-pipelined kernel for multi-wave launches (MGB_STREAM_KERNEL=0 disables)
     int pdl = 1;               // programmatic dependent launch of consecutive step kernels (MGB_PDL=0 disables)
@@ -1414,6 +1415,13 @@ static QuadArgs base_args(const mgb_quad *h)
     a.seed = h->seed;
     a.auto_reset = h->auto_reset;
     return a;
+}
+
+// Calls f(std::true_type()) for a handle whose configuration takes the simplified dynamics (QuadConst::simple), else
+// f(std::false_type()): the one place where the SIMPLE argument of a kernel template is chosen
+template <class F> static auto with_simple(const mgb_quad *h, F &&f)
+{
+    return h->c.simple ? f(std::true_type()) : f(std::false_type());
 }
 
 static int derive_constants(const mgb_quad_cfg *g, QuadConst *c)
@@ -1497,12 +1505,12 @@ extern "C" int mgb_quad_create(mgb_quad **out, int64_t n_envs, const mgb_quad_cf
     {
         // the one-CTA-per-SM step kernels need up to 2 x 512 x 19 floats of dynamic shared memory; the attribute is per
         // function and device, idempotent, and set to the maximum so that handles never lower each other's limit (round-1
-        // advice: the process-global high-water mark it replaces was not thread-safe)
+        // advice: the process-global high-water mark it replaces was not thread-safe), for the kernels this handle launches
         const int max_smem = 512 * kMaxObs * 4 * 2;
-        cudaFuncSetAttribute(quad_step_wide_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        cudaFuncSetAttribute(quad_step_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        cudaFuncSetAttribute(quad_step2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-        cudaFuncSetAttribute(quad_step2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
+        with_simple(h, [&](auto simple) {
+            cudaFuncSetAttribute(quad_step_wide_kernel<simple>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
+            cudaFuncSetAttribute(quad_step2_kernel<simple>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
+        });
         if (cudaGetLastError() != cudaSuccess) {
             mgb_set_error("cudaFuncSetAttribute(quad_step_wide_kernel, %d bytes of shared memory) failed", max_smem);
             delete h;
@@ -1632,8 +1640,9 @@ extern "C" int mgb_quad_make_targets(mgb_quad *h, const float *act_dev, int32_t 
     MgbDeviceGuard guard(h->device);
     cudaStream_t st = (cudaStream_t)stream;
     const int threads = 32, blocks = (n_tasks + threads - 1) / threads;
-    if (h->c.simple) quad_targets_kernel<true><<<blocks, threads, 0, st>>>(h->c, act_dev, n_tasks, tbl_dev);
-    else quad_targets_kernel<false><<<blocks, threads, 0, st>>>(h->c, act_dev, n_tasks, tbl_dev);
+    with_simple(h, [&](auto simple) {
+        quad_targets_kernel<simple><<<blocks, threads, 0, st>>>(h->c, act_dev, n_tasks, tbl_dev);
+    });
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     return MGB_OK;
@@ -1656,90 +1665,70 @@ extern "C" int mgb_quad_reset(mgb_quad *h, const uint8_t *mask_dev, const double
     return MGB_OK;
 }
 
-// Which step kernel a launch of this handle takes (also reported through mgb_quad_step_kernel for the bench line)
-enum StepKernel { STEP_TILE = 0, STEP_WIDE = 1, STEP_STREAM = 2, STEP_PACKED = 3 };
+// A step launch of this handle: the kernel and its name (mgb_quad_step_kernel reports it for the bench line), the launch
+// shape, and QuadArgs::per_cta of the one-CTA-per-SM kernels (0 for the others)
+struct StepPlan {
+    void (*kernel)(QuadConst, QuadArgs);
+    const char *name;
+    dim3 grid, block;
+    size_t smem = 0;
+    int per_cta = 0;
+};
 
-static StepKernel choose_step_kernel(const mgb_quad *h, const QuadArgs &a)
+static StepPlan plan_step(const mgb_quad *h, const QuadArgs &a)
 {
-    const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
-    const bool act16 = (reinterpret_cast<uintptr_t>(a.act) & 15u) == 0;
-    // multi-wave launches stream: persistent CTAs + TMA double buffering (quad_stream_kernel)
-    if (h->stream_kernel && (int64_t)blocks > (int64_t)h->num_sms * 32 && act16) return STEP_STREAM;
-    if (h->packed && h->c.rk4_steps == 0 && a.n >= 2) {
+#define STEP_KERNEL(k) k<simple>, simple ? #k "<true>" : #k "<false>"
+    return with_simple(h, [&](auto simple) {
+        const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
+        const bool act16 = (reinterpret_cast<uintptr_t>(a.act) & 15u) == 0;
+        // multi-wave launches stream: persistent CTAs + TMA double buffering (quad_stream_kernel)
+        if (h->stream_kernel && (int64_t)blocks > (int64_t)h->num_sms * 32 && act16)
+            return StepPlan{STEP_KERNEL(quad_stream_kernel), dim3((unsigned)(h->num_sms * 4)), dim3(kStreamThreads)};
         // the packed kernel stores reward / done / fail / truncated of an env pair with one 8 / 2 / 8 / 2-byte access
-        const bool aligned = act16 && (reinterpret_cast<uintptr_t>(a.rew) & 7u) == 0 &&
-                             (reinterpret_cast<uintptr_t>(a.done) & 1u) == 0 && (reinterpret_cast<uintptr_t>(a.fail) & 7u) == 0 &&
-                             (reinterpret_cast<uintptr_t>(a.truncated) & 1u) == 0;
-        if (aligned) return STEP_PACKED;
-    }
-    // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (700 W power limit,
-    // velocity_control dt = 0.005, CUDA graphs of 256 steps, medians of 3 runs), us per step tile / wide: 9 473 envs
-    // 4.87 / 3.09, 24 576 envs 5.26 / 4.73, 49 152 envs 6.88 / 5.89, but 65 536 envs 6.79 / 8.09 and 67 001 envs 7.39 / 7.90.
-    // So by default the wide kernel takes batches of up to 384 envs per SM and the 64-env tile kernel the rest.
-    const bool single_wave = a.n <= (int64_t)h->num_sms * 512 && a.n >= (int64_t)h->num_sms * 64;
-    const int64_t wide_max = (int64_t)h->num_sms * (h->wide_kernel > 0 ? 512 : 384);
-    if (h->wide_kernel != 0 && single_wave && a.n <= wide_max) return STEP_WIDE;
-    return STEP_TILE;
+        const bool packed = h->packed && h->c.rk4_steps == 0 && a.n >= 2 && act16 &&
+                            (reinterpret_cast<uintptr_t>(a.rew) & 7u) == 0 && (reinterpret_cast<uintptr_t>(a.done) & 1u) == 0 &&
+                            (reinterpret_cast<uintptr_t>(a.fail) & 7u) == 0 && (reinterpret_cast<uintptr_t>(a.truncated) & 1u) == 0;
+        // launches that fit one wave of 512-thread CTAs: one CTA per SM.  Measured on an H100 80GB HBM3 (700 W power limit,
+        // velocity_control dt = 0.005, CUDA graphs of 256 steps, medians of 3 runs), us per step tile / wide: 9 473 envs
+        // 4.87 / 3.09, 24 576 envs 5.26 / 4.73, 49 152 envs 6.88 / 5.89, but 65 536 envs 6.79 / 8.09 and 67 001 envs 7.39 / 7.90.
+        // So by default the wide kernel takes batches of up to 384 envs per SM and the 64-env tile kernel the rest.
+        const bool single_wave = a.n <= (int64_t)h->num_sms * 512 && a.n >= (int64_t)h->num_sms * 64;
+        const int64_t wide_max = (int64_t)h->num_sms * (h->wide_kernel > 0 ? 512 : 384);
+        if (!packed && !(h->wide_kernel != 0 && single_wave && a.n <= wide_max))
+            return StepPlan{STEP_KERNEL(quad_step_kernel), dim3(blocks), dim3(kThreads)};
+        // envs per CTA: one CTA per SM when the launch fits a single wave; the packed kernel also serves the other sizes
+        int per = single_wave ? (int)((a.n + h->num_sms - 1) / h->num_sms) : a.n < (int64_t)h->num_sms * 64 ? 64 : 256;
+        per = (per + 3) / 4 * 4;
+        const dim3 grid((unsigned)((a.n + per - 1) / per)), block((unsigned)((per / (packed ? 2 : 1) + 31) / 32 * 32));
+        const size_t smem = (size_t)per * kMaxObs * 4 * 2;
+        if (packed) return StepPlan{STEP_KERNEL(quad_step2_kernel), grid, block, smem, per};
+        return StepPlan{STEP_KERNEL(quad_step_wide_kernel), grid, block, smem, per};
+    });
+#undef STEP_KERNEL
 }
 
-static int launch_step(mgb_quad *h, const QuadArgs &a, cudaStream_t st)
+static int launch_step(mgb_quad *h, QuadArgs a, cudaStream_t st)
 {
-    const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
+    const StepPlan p = plan_step(h, a);
+    a.per_cta = p.per_cta;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(blocks);
-    cfg.blockDim = dim3(kThreads);
+    cfg.gridDim = p.grid;
+    cfg.blockDim = p.block;
+    cfg.dynamicSmemBytes = p.smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = h->pdl ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    const StepKernel which = choose_step_kernel(h, a);
-    if (which == STEP_STREAM) {
-        cfg.gridDim = dim3((unsigned)(h->num_sms * 4));
-        cfg.blockDim = dim3(kStreamThreads);
-        if (h->c.simple) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_stream_kernel<true>, h->c, a));
-        else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_stream_kernel<false>, h->c, a));
-    } else if (which == STEP_WIDE || which == STEP_PACKED) {
-        // envs per CTA: one CTA per SM when the launch fits a single wave; the packed kernel also serves the other sizes
-        const int lanes = which == STEP_PACKED ? 2 : 1;
-        int per;
-        if (a.n <= (int64_t)h->num_sms * 512 && a.n >= (int64_t)h->num_sms * 64) per = (int)((a.n + h->num_sms - 1) / h->num_sms);
-        else per = a.n < (int64_t)h->num_sms * 64 ? 64 : 256;        // packed only
-        per = (per + 3) / 4 * 4;
-        QuadArgs aw = a;
-        aw.per_cta = per;
-        cfg.gridDim = dim3((unsigned)((a.n + per - 1) / per));
-        cfg.blockDim = dim3((unsigned)((per / lanes + 31) / 32 * 32));
-        cfg.dynamicSmemBytes = (size_t)per * kMaxObs * 4 * 2;
-        if (which == STEP_PACKED) {
-            if (h->c.simple) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step2_kernel<true>, h->c, aw));
-            else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step2_kernel<false>, h->c, aw));
-        } else {
-            if (h->c.simple) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_wide_kernel<true>, h->c, aw));
-            else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_wide_kernel<false>, h->c, aw));
-        }
-    } else {
-        if (h->c.simple) MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<true>, h->c, a));
-        else MGB_CUDA(cudaLaunchKernelEx(&cfg, quad_step_kernel<false>, h->c, a));
-    }
+    MGB_CUDA(cudaLaunchKernelEx(&cfg, p.kernel, h->c, a));
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     return MGB_OK;
 }
 
-extern "C" const char *mgb_quad_step_kernel(const mgb_quad *h)
-{
-    if (!h) return "";
-    QuadArgs a = base_args(h);
-    switch (choose_step_kernel(h, a)) {
-    case STEP_STREAM: return h->c.simple ? "quad_stream_kernel<true>" : "quad_stream_kernel<false>";
-    case STEP_PACKED: return h->c.simple ? "quad_step2_kernel<true>" : "quad_step2_kernel<false>";
-    case STEP_WIDE: return h->c.simple ? "quad_step_wide_kernel<true>" : "quad_step_wide_kernel<false>";
-    default: return h->c.simple ? "quad_step_kernel<true>" : "quad_step_kernel<false>";
-    }
-}
+extern "C" const char *mgb_quad_step_kernel(const mgb_quad *h) { return h ? plan_step(h, base_args(h)).name : ""; }
 
 static int step_dev(mgb_quad *h, const float *act_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
                     int32_t *fail_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
@@ -1790,26 +1779,20 @@ static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_se
     const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
     a.mir = h->mir;
     if (h->mir.count != 0)
-        MGB_REQUIRE(h->mir_win.holds(obs_dev, (uint64_t)T * h->n * h->c.obs_dim * 4) &&
-                        h->mir_win.holds(rew_dev, (uint64_t)T * h->n * 4) && h->mir_win.holds(done_dev, (uint64_t)T * h->n) &&
-                        h->mir_win.holds(act_out_dev, (uint64_t)T * h->n * 16),
+        MGB_REQUIRE(h->mir_win.holds_rollout((uint64_t)T * h->n, obs_dev, (uint64_t)h->c.obs_dim * 4, rew_dev, 4, done_dev,
+                                             act_out_dev, 16),
                     "mirrors are on but an output lies outside the mirrored arena (set_mirrors([]) first)");
-    if (h->mir.count == MGB_MIRROR_MULTICAST) {
+    const int xm = h->mir.count == MGB_MIRROR_MULTICAST ? 2 : h->mir.count > 0 ? 1 : 0;
+    if (xm == 2) {
         MGB_REQUIRE(h->n % 4 == 0, "multicast outputs need num_envs % 4 == 0");
         MGB_REQUIRE((((uintptr_t)done_dev | (uintptr_t)rew_dev | (uintptr_t)obs_dev) & 3) == 0 && ((uintptr_t)act_out_dev & 15) == 0,
                     "multicast outputs must be 4-byte (actions: 16-byte) aligned");
-        if (h->c.simple) quad_rollout_kernel<true, 2, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 2, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-    } else if (h->mir.count > 0) {
-        if (h->c.simple) quad_rollout_kernel<true, 1, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 1, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-    } else if (fin) {
-        if (h->c.simple) quad_rollout_kernel<true, 0, true><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 0, true><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-    } else {
-        if (h->c.simple) quad_rollout_kernel<true, 0, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
-        else quad_rollout_kernel<false, 0, false><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
     }
+    const auto kernel = with_simple(h, [&](auto simple) {
+        return xm == 2 ? quad_rollout_kernel<simple, 2, false> : xm == 1 ? quad_rollout_kernel<simple, 1, false>
+               : fin   ? quad_rollout_kernel<simple, 0, true>  : quad_rollout_kernel<simple, 0, false>;
+    });
+    kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;
@@ -1835,32 +1818,23 @@ extern "C" int mgb_quad_rollout_ex(mgb_quad *h, int32_t T, const float *act_dev,
 extern "C" int mgb_quad_set_mirrors(mgb_quad *h, int count, const int64_t *byte_delta)
 {
     MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE(count >= 0 && count <= MGB_MAX_MIRRORS && (count == 0 || byte_delta), "count out of range");
-    MgbMirrors m = {};
-    for (int i = 0; i < count; ++i) {
-        MGB_REQUIRE((byte_delta[i] & 15) == 0, "mirror deltas must be multiples of 16 bytes");
-        m.delta[i] = byte_delta[i];
-    }
-    m.count = count;
-    h->mir = m;
+    const char *why = h->mir.set_peers(count, byte_delta);
+    MGB_REQUIRE(!why, why);
     return MGB_OK;
 }
 
 extern "C" int mgb_quad_set_mirror_window(mgb_quad *h, const void *base, uint64_t bytes)
 {
     MGB_REQUIRE(h, "null handle");
-    h->mir_win.base = reinterpret_cast<uintptr_t>(base);
-    h->mir_win.bytes = bytes;
+    h->mir_win.set(base, bytes);
     return MGB_OK;
 }
 
 extern "C" int mgb_quad_set_multicast(mgb_quad *h, int64_t byte_delta)
 {
     MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE((byte_delta & 15) == 0, "multicast delta must be a multiple of 16 bytes");
-    MgbMirrors m = {};
-    if (byte_delta != 0) { m.count = MGB_MIRROR_MULTICAST; m.delta[0] = byte_delta; }
-    h->mir = m;
+    const char *why = h->mir.set_multicast(byte_delta);
+    MGB_REQUIRE(!why, why);
     return MGB_OK;
 }
 

@@ -12,6 +12,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import _lib
+from .rollout import Mirrored
 from .snapshot import Snapshots
 from .spaces import Box, Discrete
 from .textures import synthetic_textures
@@ -407,29 +408,30 @@ class _BatchedMazeBase(Snapshots):
         if action is None:
             raise NotImplementedError("keyboard control (action=None) is display-only in the reference")
         torch = self._torch
+        act_dtype, shape = getattr(torch, self._ACT_DTYPE), (self.num_envs,) + self._ACT_SHAPE
         if not (hasattr(action, "is_cuda") and action.is_cuda):
-            action = torch.as_tensor(np.asarray(action).reshape(self.num_envs), device=self.device)
+            action = torch.as_tensor(np.asarray(action, dtype=self._ACT_HOST_DTYPE).reshape(shape), device=self.device)
         act = action
-        if act.dtype is not torch.int32 or not act.is_contiguous() or act.numel() != self.num_envs:
-            act = action.to(torch.int32).reshape(self.num_envs).contiguous()
+        if act.dtype is not act_dtype or not act.is_contiguous() or act.shape != shape:
+            act = action.to(act_dtype).reshape(shape).contiguous()
         if self._own_ptrs is None or self._own_ptrs[0] != self._obs.data_ptr():
             self._own_ptrs = (self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr())
+            if self._final is not None:
+                self._own_ptrs += (self._final.data_ptr(), self._trunc.data_ptr())
+            self._step_fn = getattr(self._lib, self._STEP_ENTRIES[self._final is not None])
             self._done_bool = self._done.view(torch.bool)
-        p = self._own_ptrs
-        if self._final is None:
-            rc = self._lib.mgb_maze_step(self._h, act.data_ptr(), p[0], p[1], p[2], self._stream())
-        else:
-            rc = self._lib.mgb_maze_step_ex(self._h, act.data_ptr(), p[0], p[1], p[2], self._final.data_ptr(),
-                                            self._trunc.data_ptr(), self._stream())
+        rc = self._step_fn(self._h, act.data_ptr(), *self._own_ptrs, self._stream())
         if rc:
             _lib.check(rc)
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done_bool), info
 
-    # rollout(): the C entry points without / with the final_obs and truncated outputs, the layout of one step's
-    # actions, and whether the "act" output also records actions the caller passed in (or only device-drawn ones)
+    # step() and rollout(): the C entry points without / with the final_obs and truncated outputs, the layout of one
+    # env's action, the numpy dtype host actions are read as (None: as given), and whether the "act" output also
+    # records actions the caller passed in (or only device-drawn ones)
+    _STEP_ENTRIES = ("mgb_maze_step", "mgb_maze_step_ex")
     _ROLLOUT_ENTRIES = ("mgb_maze_rollout", "mgb_maze_rollout_ex")
-    _ACT_DTYPE, _ACT_SHAPE = "int32", ()
+    _ACT_DTYPE, _ACT_SHAPE, _ACT_HOST_DTYPE = "int32", (), None
     _RECORDS_GIVEN_ACTIONS = True
 
     def _rollout(self, T, actions, act_seed, want_actions, out, final=False):
@@ -552,9 +554,10 @@ class _LazySteps(dict):
         return k == "steps"
 
 
-class BatchedMetaMaze2D(_BatchedMazeBase):
+class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
     """MetaMaze2D(enable_render, render_scale, max_steps, task_type, view_grid) x num_envs (maze_env.py:155-172)."""
     KIND = 0
+    _MIRROR_PREFIX = "mgb_maze"
 
     def __init__(self, enable_render=False, render_scale=480, max_steps=5000, task_type="SURVIVAL", view_grid=2,
                  num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True, final_obs=False):
@@ -575,23 +578,6 @@ class BatchedMetaMaze2D(_BatchedMazeBase):
         cfg.kind, cfg.task_type = 0, {"SURVIVAL": 0, "ESCAPE": 1}[self.task_type]
         cfg.n_cells, cfg.max_steps, cfg.view_grid = n_cells, self.max_steps, self.view_grid
         return cfg
-
-    def _set_window(self, window):
-        """window = (base address, bytes) of this rank's arena slot: rollouts writing elsewhere are refused while
-        mirrors are on (arena.attach(env) passes it)."""
-        base, nbytes = (0, 0) if window is None else (int(window[0]), int(window[1]))
-        _lib.check(self._lib.mgb_maze_set_mirror_window(self._h, base, nbytes))
-
-    def set_mirrors(self, byte_deltas, window=None):
-        """Every output of rollout() is also stored at `pointer + delta` (see rollout.PeerArena)."""
-        self._set_window(window)
-        d = np.ascontiguousarray(np.asarray(list(byte_deltas), dtype=np.int64))
-        _lib.check(self._lib.mgb_maze_set_mirrors(self._h, int(d.size), _lib.ptr(d) if d.size else None))
-
-    def set_multicast(self, byte_delta, window=None):
-        """rollout() outputs go through an NVSwitch multicast mapping at `pointer + byte_delta` (rollout.MulticastArena)."""
-        self._set_window(window)
-        _lib.check(self._lib.mgb_maze_set_multicast(self._h, int(byte_delta)))
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
@@ -684,8 +670,9 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
     maze_continuous_3d.py:48-49); float32 position / float64 heading exactly as the reference computes them for
     float32 actions.  Every pose is unique, so this env always uses the direct float64 renderer."""
     KIND = 2
+    _STEP_ENTRIES = ("mgb_maze_step_continuous", "mgb_maze_step_continuous_ex")
     _ROLLOUT_ENTRIES = ("mgb_maze_rollout_continuous", "mgb_maze_rollout_continuous_ex")
-    _ACT_DTYPE, _ACT_SHAPE = "float32", (2,)
+    _ACT_DTYPE, _ACT_SHAPE, _ACT_HOST_DTYPE = "float32", (2,), np.float32
     _RECORDS_GIVEN_ACTIONS = False
 
     def __init__(self, *args, **kwargs):
@@ -696,26 +683,6 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         cfg = BatchedMetaMazeDiscrete3D._make_cfg(self, n_cells)
         cfg.kind = 2
         return cfg
-
-    def step(self, action=None):
-        if self.need_reset:
-            raise Exception("Must \"reset\" before doing any actions")              # maze_env.py:130-131
-        if action is None:
-            raise NotImplementedError("keyboard control (action=None) is display-only in the reference")
-        torch = self._torch
-        if not (hasattr(action, "is_cuda") and action.is_cuda):
-            action = torch.as_tensor(np.asarray(action, dtype=np.float32).reshape(self.num_envs, 2), device=self.device)
-        act = action.to(torch.float32).reshape(self.num_envs, 2).contiguous()
-        if self._final is None:
-            _lib.check(self._lib.mgb_maze_step_continuous(self._h, act.data_ptr(), self._obs.data_ptr(),
-                                                          self._rew.data_ptr(), self._done.data_ptr(), self._stream()))
-        else:
-            _lib.check(self._lib.mgb_maze_step_continuous_ex(self._h, act.data_ptr(), self._obs.data_ptr(),
-                                                             self._rew.data_ptr(), self._done.data_ptr(),
-                                                             self._final.data_ptr(), self._trunc.data_ptr(),
-                                                             self._stream()))
-        info = _LazySteps(self)
-        return self._out(self._obs), self._out(self._rew), self._out(self._done.view(torch.bool)), info
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False):
         """T steps in one launch of the direct renderer (mgb_maze_rollout_continuous), exactly as T step() calls.

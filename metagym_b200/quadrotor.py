@@ -11,6 +11,7 @@ import os
 import numpy as np
 
 from . import _lib
+from .rollout import Mirrored
 from .snapshot import Snapshots
 from .spaces import Box, Space
 
@@ -125,7 +126,7 @@ class QuadInfo(dict):
         return list(self._keys)
 
 
-class BatchedQuadrotor(Snapshots):
+class BatchedQuadrotor(Snapshots, Mirrored):
     """`Quadrotor(dt, nt, seed, task, map_file, simulator_conf, healthy_reward)` x num_envs on one H100.
 
     Extra kwargs: num_envs, device (int or 'cuda:k'), auto_reset (finished envs restart inside the step launch),
@@ -140,7 +141,7 @@ class BatchedQuadrotor(Snapshots):
     counter, velocity task and the rollout action counter -- also into another sharding (metagym_b200/snapshot.py).
     """
     metadata = {"render.modes": []}
-    _SNAP_PREFIX = "mgb_quad"
+    _SNAP_PREFIX = _MIRROR_PREFIX = "mgb_quad"
     _FINGERPRINT_PARTS = ("configuration (physics, dt, nt, task, integrator, auto_reset, rng_seed)", "obstacle map",
                           "velocity-target table", "record layout")
 
@@ -197,6 +198,12 @@ class BatchedQuadrotor(Snapshots):
         self._final_obs = torch.zeros((N, D), dtype=torch.float32, device=dev) if self.auto_reset else None
         # persistent, so that a step with final_obs=True can be captured in a CUDA graph
         self._trunc = torch.zeros((N,), dtype=torch.uint8, device=dev) if self._want_final else None
+        # final_obs=True: steps and rollouts go through the *_ex entry points, which also take the truncated output
+        ex = "_ex" if self._want_final else ""
+        self._step_fn = getattr(self._lib, "mgb_quad_step" + ex)
+        self._step_host_fn = getattr(self._lib, "mgb_quad_step_host" + ex)
+        self._rollout_fn = getattr(self._lib, "mgb_quad_rollout" + ex)
+        self._trunc_ptr = (self._trunc.data_ptr(),) if self._want_final else ()
         if self.map_matrix is not None and map_file is not None:
             m = np.ascontiguousarray(self.map_matrix, dtype=np.int32)
             _lib.check(self._lib.mgb_quad_set_map(self._h, m.ctypes.data, m.shape[0], m.shape[1]))
@@ -296,29 +303,18 @@ class BatchedQuadrotor(Snapshots):
         if out is None:                       # the env's own output tensors: addresses and views are fixed
             if self._own_ptrs is None:
                 self._own_ptrs = (self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr(),
-                                  self._fail.data_ptr(), _lib.ptr(self._final_obs))
+                                  self._fail.data_ptr(), _lib.ptr(self._final_obs)) + self._trunc_ptr
                 self._done_bool = self._done.view(torch.bool)
             p = self._own_ptrs
-            if self._trunc is None:
-                rc = self._lib.mgb_quad_step(self._h, act.data_ptr(), p[0], p[1], p[2], p[3], p[4], self._stream())
-            else:
-                rc = self._lib.mgb_quad_step_ex(self._h, act.data_ptr(), p[0], p[1], p[2], p[3], p[4],
-                                                self._trunc.data_ptr(), self._stream())
-            if rc:
-                _lib.check(rc)
-            obs, rew, done_b = self._obs, self._rew, self._done_bool
+            obs, rew, done = self._obs, self._rew, None
         else:
             obs, rew, done = out
-            if self._trunc is None:
-                _lib.check(self._lib.mgb_quad_step(self._h, act.data_ptr(), obs.data_ptr(), rew.data_ptr(),
-                                                   done.data_ptr(), self._fail.data_ptr(), _lib.ptr(self._final_obs),
-                                                   self._stream()))
-            else:
-                _lib.check(self._lib.mgb_quad_step_ex(self._h, act.data_ptr(), obs.data_ptr(), rew.data_ptr(),
-                                                      done.data_ptr(), self._fail.data_ptr(),
-                                                      _lib.ptr(self._final_obs), self._trunc.data_ptr(),
-                                                      self._stream()))
-            done_b = done.view(torch.bool)
+            p = (obs.data_ptr(), rew.data_ptr(), done.data_ptr(), self._fail.data_ptr(),
+                 _lib.ptr(self._final_obs)) + self._trunc_ptr
+        rc = self._step_fn(self._h, act.data_ptr(), *p, self._stream())
+        if rc:
+            _lib.check(rc)
+        done_b = self._done_bool if done is None else done.view(torch.bool)
         info = QuadInfo(obs, self.obs_keys)
         return self._out(obs), self._out(rew), self._out(done_b), info
 
@@ -331,16 +327,11 @@ class BatchedQuadrotor(Snapshots):
             self._h_fail = np.zeros((self.num_envs,), dtype=np.int32)
             self._h_final = np.zeros((self.num_envs, self.obs_dim), dtype=np.float32) if self.auto_reset else None
             self._h_trunc = np.zeros((self.num_envs,), dtype=np.uint8) if self._want_final else None
+            trunc = (self._h_trunc.ctypes.data,) if self._want_final else ()
+            self._h_ptrs = (self._h_obs.ctypes.data, self._h_rew.ctypes.data, self._h_done.ctypes.data,
+                            self._h_fail.ctypes.data, _lib.ptr(self._h_final)) + trunc
         # enqueued on torch's current stream: ordered after a preceding reset() / rollout() / load_state_dict()
-        if self._h_trunc is None:
-            _lib.check(self._lib.mgb_quad_step_host(self._h, act.ctypes.data, self._h_obs.ctypes.data,
-                                                    self._h_rew.ctypes.data, self._h_done.ctypes.data,
-                                                    self._h_fail.ctypes.data, _lib.ptr(self._h_final), self._stream()))
-        else:
-            _lib.check(self._lib.mgb_quad_step_host_ex(self._h, act.ctypes.data, self._h_obs.ctypes.data,
-                                                       self._h_rew.ctypes.data, self._h_done.ctypes.data,
-                                                       self._h_fail.ctypes.data, _lib.ptr(self._h_final),
-                                                       self._h_trunc.ctypes.data, self._stream()))
+        _lib.check(self._step_host_fn(self._h, act.ctypes.data, *self._h_ptrs, self._stream()))
         self._host_results = True
         info = QuadInfo(self._h_obs, self.obs_keys)
         return (self._out(self._h_obs), self._out(self._h_rew), self._out(self._h_done.view(np.bool_)), info)
@@ -372,36 +363,10 @@ class BatchedQuadrotor(Snapshots):
         a = None
         if actions is not None:
             a = actions.to(torch.float32).reshape(T, N, 4).contiguous()
-        if not self._want_final:
-            _lib.check(self._lib.mgb_quad_rollout(self._h, int(T), _lib.ptr(a), int(act_seed),
-                                                  _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
-                                                  _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")), self._stream()))
-        else:
-            _lib.check(self._lib.mgb_quad_rollout_ex(self._h, int(T), _lib.ptr(a), int(act_seed),
-                                                     _lib.ptr(out.get("act")), _lib.ptr(out.get("obs")),
-                                                     _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
-                                                     _lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated")),
-                                                     self._stream()))
+        keys = ("act", "obs", "rew", "done") + (("final_obs", "truncated") if self._want_final else ())
+        _lib.check(self._rollout_fn(self._h, int(T), _lib.ptr(a), int(act_seed), *[_lib.ptr(out.get(k)) for k in keys],
+                                    self._stream()))
         return out
-
-    def _set_window(self, window):
-        """window = (base address, bytes) of this rank's arena slot: rollouts writing elsewhere are refused while
-        mirrors are on (arena.attach(env) passes it)."""
-        base, nbytes = (0, 0) if window is None else (int(window[0]), int(window[1]))
-        _lib.check(self._lib.mgb_quad_set_mirror_window(self._h, base, nbytes))
-
-    def set_mirrors(self, byte_deltas, window=None):
-        """Every output of rollout() is also stored at `pointer + delta` for each delta (rollout.PeerArena.mirrors:
-        the kernel then writes the trajectory straight into the other ranks' receive arenas over NVLink)."""
-        self._set_window(window)
-        d = np.ascontiguousarray(np.asarray(list(byte_deltas), dtype=np.int64))
-        _lib.check(self._lib.mgb_quad_set_mirrors(self._h, int(d.size), _lib.ptr(d) if d.size else None))
-
-    def set_multicast(self, byte_delta, window=None):
-        """rollout() outputs are stored through an NVSwitch multicast mapping at `pointer + byte_delta`
-        (rollout.MulticastArena.multicast_delta); 0 switches it off."""
-        self._set_window(window)
-        _lib.check(self._lib.mgb_quad_set_multicast(self._h, int(byte_delta)))
 
     @property
     def fail_code(self):

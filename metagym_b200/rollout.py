@@ -8,6 +8,10 @@ same code runs on gloo for the CPU tests).
 """
 import os
 
+import numpy as np
+
+from . import _lib
+
 
 def shard_range(num_envs_global, rank, world_size):
     """Contiguous block of global env indices owned by `rank` -> (base, count).  Remainder goes to the low ranks."""
@@ -115,6 +119,32 @@ class RolloutArena:
         """[world, T, n, ...] -> [T, world*n, ...] (global env order; this one copies)."""
         return {k: v.movedim(0, 1).reshape((v.shape[1], v.shape[0] * v.shape[2]) + tuple(v.shape[3:]))
                 for k, v in views.items()}
+
+
+class Mirrored(object):
+    """set_mirrors() / set_multicast() of an env whose fused rollout can store its outputs into every rank's slot of a
+    PeerArena or MulticastArena.  The class sets _MIRROR_PREFIX (C entry points <prefix>_set_mirrors ...)."""
+    _MIRROR_PREFIX = None
+
+    def _set_window(self, window):
+        """window = (base address, bytes) of this rank's arena slot: rollouts writing elsewhere are refused while
+        mirrors are on (arena.attach(env) passes it)."""
+        base, nbytes = (0, 0) if window is None else (int(window[0]), int(window[1]))
+        _lib.check(getattr(self._lib, self._MIRROR_PREFIX + "_set_mirror_window")(self._h, base, nbytes))
+
+    def set_mirrors(self, byte_deltas, window=None):
+        """Every output of rollout() is also stored at `pointer + delta` for each delta (PeerArena.mirrors: the kernel
+        then writes the trajectory straight into the other ranks' receive arenas over NVLink)."""
+        self._set_window(window)
+        d = np.ascontiguousarray(np.asarray(list(byte_deltas), dtype=np.int64))
+        _lib.check(getattr(self._lib, self._MIRROR_PREFIX + "_set_mirrors")(self._h, int(d.size),
+                                                                              _lib.ptr(d) if d.size else None))
+
+    def set_multicast(self, byte_delta, window=None):
+        """rollout() outputs are stored through an NVSwitch multicast mapping at `pointer + byte_delta`
+        (MulticastArena.multicast_delta); 0 switches it off."""
+        self._set_window(window)
+        _lib.check(getattr(self._lib, self._MIRROR_PREFIX + "_set_multicast")(self._h, int(byte_delta)))
 
 
 class _RawDeviceMemory:
