@@ -416,11 +416,27 @@ int64_t mgb_maze_launch_count(const mgb_maze *h);
  *   view_size S in [1, 4096]: the reference's render_scale; cell size S / n_cells, need not be an integer.
  *   out_dev [count][S][S][3] uint8, IMAGE ROWS TOP TO BOTTOM: out[k][y][x] is pygame pixel (x, y) of the panel, as a saved
  *     PNG shows it.  This is transposed against the x-major observation arrays ([res_h][res_v][3]).
- * mode: MGB_GOD_LIVE (the current state; nothing needs recording).  Pixel rules: DESIGN.md "God view".  Stream-ordered,
- * no host synchronisation, no allocation: capturable in a CUDA graph. */
+ * mode: MGB_GOD_LIVE (the current state; nothing needs recording) or MGB_GOD_TRAJECTORY (the picture of
+ *   MazeBase.render_trajectory with additional=None, maze_base.py:159-189: white fill, walls and ESCAPE goal, a red agent
+ *   rect at the current cell for every kind, SURVIVAL food over it, then red width-3 lines between the centres of
+ *   consecutive cells of the env's current-episode path; needs mgb_maze_set_path, else MGB_ERR_ARG).  Pixel rules:
+ *   DESIGN.md "God view".  Stream-ordered, no host synchronisation, no allocation: capturable in a CUDA graph. */
 #define MGB_GOD_LIVE 0
+#define MGB_GOD_TRAJECTORY 1
 int mgb_maze_god_view(mgb_maze *h, int32_t count, const int32_t *envs_dev, int32_t view_size, int32_t mode,
                       uint8_t *out_dev, void *stream);
+
+/* Path recording (MazeBase._agent_trajectory, maze_base.py:44,67), off by default; call after mgb_maze_create, like
+ * mgb_maze_set_options.  enabled = 1 allocates [max_steps + 1][n_envs] int8 cell pairs, step-major; every kernel that
+ * leaves env e with step count s then stores the agent's cell as entry (s, e), so the current episode's path is entries
+ * 0 .. min(s, max_steps).  Steps past max_steps (auto_reset off, stepping on after done) are not stored.  Switching it on
+ * mid-episode records the current cell; earlier entries read (-1, -1).  Observations, rewards, dones and state are
+ * bit-identical with recording on and off.  Synchronous; enabled = 0 frees the buffer.
+ *   mgb_maze_path: cells_out [count][max_steps + 1][2] int8 (entries at and past len_out[k] are not written) and len_out
+ *   [count] int32 of envs envs_dev (as for mgb_maze_god_view; an index outside [0, n_envs) has length 0).  Stream-ordered,
+ *   no host synchronisation. */
+int mgb_maze_set_path(mgb_maze *h, int enabled);
+int mgb_maze_path(mgb_maze *h, int32_t count, const int32_t *envs_dev, int8_t *cells_out, int32_t *len_out, void *stream);
 
 /* Exact snapshot / restore of env state, as mgb_quad_snapshot / mgb_quad_restore (same row map and stream rules).  A
  * record of mgb_maze_record_bytes(h) bytes (after mgb_maze_set_task) holds agent (int4), life, the env's resample count,
@@ -428,8 +444,9 @@ int mgb_maze_god_view(mgb_maze *h, int32_t count, const int32_t *envs_dev, int32
  * slot per env and can re-task envs on the device (injective env2task, direct renderer) -- the whole task of the env's
  * slot.  Restore then writes that task into the destination env's own slot; otherwise the table is shared, the fingerprint
  * covers it, and restore points env2task[e] at the record's slot.  mgb_maze_restore is synchronous the first time it
- * finds the pose cache to be built (like the first reset); after that it is stream-ordered.
- *   mgb_maze_fingerprint: out[0] config (mgb_maze_cfg, auto_reset, table shape, record layout), out[1] textures,
+ * finds the pose cache to be built (like the first reset); after that it is stream-ordered.  A recording handle
+ * (mgb_maze_set_path) appends the env's path entries to its records (2 (max_steps + 1) bytes, padded to 16).
+ *   mgb_maze_fingerprint: out[0] config (mgb_maze_cfg, auto_reset, table shape, path recording, record layout), out[1] textures,
  *     out[2] the shared task table (0 when records carry their tasks), out[3] 1 when records carry their tasks. */
 int64_t mgb_maze_record_bytes(const mgb_maze *h);
 int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream);

@@ -105,6 +105,8 @@ SIGNATURES = {
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),
     "mgb_maze_god_view": (ctypes.c_int, [vp, c_i32, vp, c_i32, c_i32, vp, vp]),
+    "mgb_maze_set_path": (ctypes.c_int, [vp, ctypes.c_int]),
+    "mgb_maze_path": (ctypes.c_int, [vp, c_i32, vp, vp, vp, vp]),
     "mgb_quad_record_bytes": (c_i64, [vp]),
     "mgb_quad_snapshot": (ctypes.c_int, [vp, vp, vp]),
     "mgb_quad_restore": (ctypes.c_int, [vp, vp, c_i64, vp, vp]),

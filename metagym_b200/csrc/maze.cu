@@ -126,6 +126,9 @@ struct MazeArgs {
     int32_t *fin_task;           // ... task slot
     float2 *fin_cpos;            // ... continuous position
     double *fin_cori;            // ... continuous heading
+    // path recording (mgb_maze_set_path): [max_steps + 1][n_pad] grid cells, step-major.  Whenever a kernel leaves env e
+    // with step count s, entry (s, e) holds the agent's cell; nullptr: recording off, nothing is stored
+    char2 *path;
 };
 
 struct Env {
@@ -213,6 +216,14 @@ __device__ __forceinline__ uint8_t maze_truncated(const MazeConst &c, const uint
     const bool over = e.steps > c.max_steps - 1;
     const bool terminal = c.task_type == MGB_MAZE_SURVIVAL ? e.life < 0.0 : (e.gx == th->goal[0] && e.gy == th->goal[1]);
     return (uint8_t)(over && !terminal);
+}
+
+// _agent_trajectory (maze_base.py:44,67): the agent's cell becomes entry (steps, e) of the path record.  The entry index is
+// the step count the env carries, so an episode's path is entries 0 .. steps; steps past the capacity (an env without
+// auto-reset stepped on after done) are not stored.
+__device__ __forceinline__ void path_store(const MazeConst &c, const MazeArgs &a, int64_t e, const Env &s)
+{
+    if (a.path && s.steps <= c.max_steps) a.path[(int64_t)s.steps * a.n_pad + e] = make_char2((char)s.gx, (char)s.gy);
 }
 
 // current transparent value of cell (i, j): SURVIVAL = remaining food (alias at maze_base.py:57), ESCAPE = goal one-hot
@@ -336,6 +347,7 @@ __global__ void maze_reset_kernel(const __grid_constant__ MazeConst c, const __g
     env_reset(c, blob, a.eaten + e, a.n_pad, s);
     a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
     a.life[e] = s.life;
+    path_store(c, a, e, s);
     if (c.kind == MGB_MAZE_CONTINUOUS_3D) {             // get_cell_center(start), heading 0 (maze_base.py:41,50)
         const TaskHdr *th = blob_hdr(blob);
         a.cpos[e] = make_float2((float)(s.gx * th->cell_size + 0.5 * th->cell_size),
@@ -393,6 +405,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_kernel(const __grid_constan
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
             a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
             a.life[e] = s.life;
+            path_store(c, a, e, s);
         }
         observe(tile2d + threadIdx.x * D);
     }
@@ -442,8 +455,9 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // SoA slots, each step's observation tile of the CTA leaves through double-buffered shared memory + one bulk store.
 // XM: 0 plain, 1 peer mirrors, 2 multicast-only stores (see quad_rollout_kernel).  FIN (XM == 0 only, mgb_maze_rollout_ex):
 // also store the truncation byte of every (t, e), and the terminal window of every env that finished at step t to
-// final_obs + (t n + e) D, both before env_reset; rows of envs that did not finish are not written.
-template <int XM, bool FIN>
+// final_obs + (t n + e) D, both before env_reset; rows of envs that did not finish are not written.  REC: path recording on
+// (a.path set); the instantiations without it have no store and no test of a.path in their loop.
+template <int XM, bool FIN, bool REC>
 __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid_constant__ MazeConst c,
                                                                     const __grid_constant__ MazeArgs a)
 {
@@ -496,6 +510,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
                     maze2d_window(c, blob, eaten, a.n_pad, s, reinterpret_cast<float *>(a.final_obs) + ((int64_t)t * a.n + e) * D);
             }
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
+            if (REC) path_store(c, a, e, s);
             if (a.rew) {
                 if (XM == 2) mgb_mc_st(mgb_shift(a.rew + (int64_t)t * a.n + e, a.mir.delta[0]), reward);
                 else a.rew[(int64_t)t * a.n + e] = reward;
@@ -824,6 +839,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                 }
                 a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
                 a.life[e] = s.life;
+                path_store(c, a, e, s);
                 if (cont) { a.cpos[e] = make_float2(cp[0], cp[1]); a.cori[e] = co; }
                 if (FIN) {
                     s_split[bb] = split;
@@ -1511,6 +1527,7 @@ __global__ void maze3d_logic_kernel(const __grid_constant__ MazeConst c, const _
         if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
+        path_store(c, a, e, s);
     }
     if (DYN) {
         const EnvDyn d = make_dyn(c, a, blob, task, s, eaten);
@@ -1694,6 +1711,7 @@ constexpr int kStepBatch = 16;              // envs whose step logic one CTA run
 constexpr int kStepSlots = 8;               // 12 KB chunk slots of a CTA's shared-memory ring
 constexpr int kStepSlack = 3;               // bulk stores that may still be reading their slot before it is handed back
 
+template <bool REC>          // path recording on (a.path set): without it the kernel neither tests a.path nor stores
 __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __grid_constant__ MazeConst c,
                                                                       const __grid_constant__ MazeArgs a)
 {
@@ -1767,6 +1785,7 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
                 if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
                 a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
                 a.life[e] = s.life;
+                if (REC) path_store(c, a, e, s);
             }
             const EnvDyn dd = make_dyn(c, a, blob, task, s, eaten);
             s_dyn[tid] = dd;
@@ -1937,6 +1956,7 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(cons
                     if (done && a.final_obs) s_tdyn = make_dyn(c, a, eblob, task, s, eaten);
                 }
                 if (done && a.auto_reset) env_reset(c, eblob, eaten, a.n_pad, s);
+                path_store(c, a, env, s);
                 if (a.rew) a.rew[(int64_t)t * a.n + env] = reward;
                 if (a.done) a.done[(int64_t)t * a.n + env] = (uint8_t)done;
                 s_dyn = make_dyn(c, a, eblob, task, s, eaten);
@@ -2099,7 +2119,11 @@ struct mgb_maze {
     int4 *fin_agent = nullptr;
     double *fin_life = nullptr, *fin_cori = nullptr;
     float2 *fin_cpos = nullptr;
+    char2 *path = nullptr;         // mgb_maze_set_path: [max_steps + 1][n_pad] recorded cells, nullptr when not recording
 };
+
+// entries of one env's path record: an episode ends at steps <= max_steps
+static int64_t path_cap(const mgb_maze *h) { return (int64_t)h->c.max_steps + 1; }
 
 static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
 {
@@ -2139,6 +2163,7 @@ static MazeArgs maze_args(const mgb_maze *h)
     a.agent = h->agent; a.life = h->life; a.eaten = h->eaten; a.env2task = h->env2task; a.blobs = h->blobs;
     a.tex = h->tex; a.coltab = h->coltab; a.efftab = h->efftab; a.fogtab = h->fogtab; a.auto_reset = h->auto_reset;
     a.cpos = h->cpos; a.cori = h->cori; a.coltab_d = h->coltab_d;
+    a.path = h->path;
     bind_pose_cache(h, a);
     return a;
 }
@@ -2254,6 +2279,7 @@ extern "C" void mgb_maze_destroy(mgb_maze *h)
     cudaFree(h->pose_rec);
     cudaFree(h->fin_count); cudaFree(h->fin_env); cudaFree(h->fin_task); cudaFree(h->fin_eaten); cudaFree(h->fin_dyn);
     cudaFree(h->fin_agent); cudaFree(h->fin_life); cudaFree(h->fin_cori); cudaFree(h->fin_cpos);
+    cudaFree(h->path);
     for (int i = 0; i < 2; ++i) {
         cudaFreeHost(h->h_stage[i]); cudaFree(h->d_stage[i]);
         if (h->stage_done[i]) cudaEventDestroy(h->stage_done[i]);
@@ -2299,6 +2325,39 @@ extern "C" int mgb_maze_set_cache(mgb_maze *h, int enabled)
         h->cache_enabled = enabled ? 1 : 0;
         h->cache_dirty = true;            // rebuilt (or dropped) at the next reset / step
     }
+    return MGB_OK;
+}
+
+namespace {
+// entry (steps, e) of every env from its current state: what a step would have stored there
+__global__ void maze_path_seed_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n) return;
+    const int4 ag = a.agent[e];
+    const Env s = {ag.x, ag.y, ag.z, ag.w, 0.0};
+    path_store(c, a, e, s);
+}
+}  // namespace
+
+extern "C" int mgb_maze_set_path(mgb_maze *h, int enabled)
+{
+    MGB_REQUIRE(h, "null handle");
+    MgbDeviceGuard guard(h->device);
+    if ((h->path != nullptr) == (enabled != 0)) return MGB_OK;
+    MGB_CUDA(cudaDeviceSynchronize());
+    if (!enabled) {
+        MGB_CUDA(cudaFree(h->path));
+        h->path = nullptr;
+        return MGB_OK;
+    }
+    const size_t bytes = sizeof(char2) * (size_t)path_cap(h) * (size_t)h->n_pad;
+    MGB_CUDA(cudaMalloc(&h->path, bytes));
+    MGB_CUDA(cudaMemset(h->path, 0xFF, bytes));             // cells (-1, -1): not recorded
+    maze_path_seed_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(h->c, maze_args(h));
+    MGB_CUDA(cudaGetLastError());
+    MGB_CUDA(cudaDeviceSynchronize());
+    h->launches += 1;
     return MGB_OK;
 }
 
@@ -2711,6 +2770,7 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
     env_reset(c, b, a.eaten + e, a.n_pad, s);
     a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
     a.life[e] = s.life;
+    path_store(c, a, e, s);
     if (c.kind == MGB_MAZE_CONTINUOUS_3D) {
         a.cpos[e] = make_float2((float)(s.gx * sc.cell_size + 0.5 * sc.cell_size), (float)(s.gy * sc.cell_size + 0.5 * sc.cell_size));
         a.cori[e] = 0.0;
@@ -3190,12 +3250,15 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t s
                 ((reinterpret_cast<uintptr_t>(a.obs) | reinterpret_cast<uintptr_t>(a.final_obs)) & 15u) == 0) {
                 const size_t ring_bytes = (size_t)kStepSlots * kStepChunkPx * 3;       // 96 KB: two CTAs per SM
                 if (h->step_smem_set == 0) {
-                    MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_step_kernel));
+                    MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_step_kernel<false>));
+                    MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_step_kernel<true>));
                     h->step_smem_set = ring_bytes;
                 }
                 const int64_t grid = (int64_t)h->num_sms * 2;
                 // terminal frames in the same launch
-                maze3d_step_kernel<<<(unsigned)(h->n < grid ? h->n : grid), kStepThreads, ring_bytes, st>>>(c, a);
+                const unsigned ctas = (unsigned)(h->n < grid ? h->n : grid);
+                if (a.path) maze3d_step_kernel<true><<<ctas, kStepThreads, ring_bytes, st>>>(c, a);
+                else maze3d_step_kernel<false><<<ctas, kStepThreads, ring_bytes, st>>>(c, a);
                 MGB_CUDA(cudaGetLastError());
                 h->launches += 1;
                 return MGB_OK;
@@ -3249,6 +3312,7 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     if (rc || !listed) return rc;
     MazeArgs l = maze_args(h);
     l.obs = final_obs; l.final_obs = final_obs; l.do_step = 0;
+    l.path = nullptr;                                           // the list holds terminal copies, not env state
     l.fin_count = h->fin_count; l.fin_env = h->fin_env;
     if (h->cache_ready) {
         l.dyn = h->fin_dyn;
@@ -3326,6 +3390,25 @@ static int check_rollout(const char *fn, const mgb_maze *h, int32_t T, const voi
     return maze_ready(h);
 }
 
+// maze2d_rollout_kernel<xm, fin, REC> over the handle's envs (xm: 0 plain, 1 peer mirrors, 2 multicast; fin: XM 0 only)
+template <bool REC>
+static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArgs &a, unsigned blocks, size_t sm,
+                             cudaStream_t st)
+{
+    if (sm > 48 * 1024) {
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false, REC>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<1, false, REC>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<2, false, REC>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC>));
+    }
+    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
+    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
+    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
+    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
+    MGB_CUDA(cudaGetLastError());
+    return MGB_OK;
+}
+
 // Rollout of a MetaMaze2D or MetaMazeDiscrete3D handle; `own`: the entry point's kind checks (see check_rollout)
 template <class Own>
 static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
@@ -3374,24 +3457,19 @@ static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_
     const int W = 2 * h->c.view_grid + 1;
     const size_t sm = (size_t)2 * k2dThreads * W * W * 4;
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
-    if (sm > 48 * 1024) {
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false>));
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<1, false>));
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<2, false>));
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true>));
-    }
     if (h->mir.count == MGB_MIRROR_MULTICAST) {
         MGB_REQUIRE(h->n % 4 == 0, "multicast outputs need num_envs % 4 == 0");
         MGB_REQUIRE((((uintptr_t)done_dev | (uintptr_t)obs_dev | (uintptr_t)act_out_dev) & 3) == 0 && ((uintptr_t)rew_dev & 7) == 0,
                     "multicast outputs must be 4-byte (rewards: 8-byte) aligned");
-        maze2d_rollout_kernel<2, false><<<blocks, k2dThreads, sm, st>>>(h->c, a);
-    } else if (h->mir.count > 0) maze2d_rollout_kernel<1, false><<<blocks, k2dThreads, sm, st>>>(h->c, a);
-    else if (fin) {
+    }
+    if (fin) {
         a.final_obs = final_obs_dev;
         a.truncated = truncated_dev;
-        maze2d_rollout_kernel<0, true><<<blocks, k2dThreads, sm, st>>>(h->c, a);
-    } else maze2d_rollout_kernel<0, false><<<blocks, k2dThreads, sm, st>>>(h->c, a);
-    MGB_CUDA(cudaGetLastError());
+    }
+    const int xm = h->mir.count == MGB_MIRROR_MULTICAST ? 2 : (h->mir.count > 0 ? 1 : 0);
+    rc = h->path ? launch_2d_rollout<true>(h->c, xm, fin, a, blocks, sm, st)
+                 : launch_2d_rollout<false>(h->c, xm, fin, a, blocks, sm, st);
+    if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
@@ -3529,7 +3607,9 @@ extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const floa
 // launch.  One CTA (or a few, for small batches) per env: the env's cells and the pixel -> cell tables are staged in shared
 // memory, then every thread colours 16 pixels at a time and stores them as three 16-byte words.  The pixel rules (rect by
 // pixel centre, disc and Bresenham line on truncated coordinates) are DESIGN.md "God view"; oracle/maze_godview.py states
-// them again in numpy.
+// them again in numpy.  The trajectory view (MazeBase.render_trajectory, maze_base.py:159-189) is the same kernel in its
+// trajectory mode followed by maze_god_path_kernel, which draws the recorded path as width-3 lines
+// (tests/trajectory_view.py restates that picture).
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
 
@@ -3630,8 +3710,10 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
                                                                     const __grid_constant__ MazeArgs a,
                                                                     const int32_t *__restrict__ envs, int S,
                                                                     const float4 hcos, const float4 hsin,
-                                                                    uint8_t *__restrict__ out)
+                                                                    uint8_t *__restrict__ out, int traj)
 {
+    // traj: the panel of render_trajectory (maze_base.py:159-176) under its path lines: walls and goal, a red agent rect
+    // at the current cell for every kind, then the food, all on the panel's own coordinates; no 3-D disc or heading line
     extern __shared__ __align__(16) uint32_t god_smem[];
     __shared__ GodEnv g;
     __shared__ uint4 stage[kGodThreads / 32][3 * 32];              // per warp: 32 items of 48 bytes, stored coalesced
@@ -3653,7 +3735,14 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
     const TaskHdr *th = valid ? blob_hdr(blob) : nullptr;
     if (threadIdx.x == 0) {
         g.valid = valid;
-        if (valid) god_marker(c, a, th, e, S, hcos, hsin, g);
+        if (valid && traj) {
+            const int4 ag = a.agent[e];
+            g.gx = ag.x; g.gy = ag.y;
+            g.dr2 = -1;
+            g.bx0 = g.by0 = 1; g.bx1 = g.by1 = 0;
+        } else if (valid) {
+            god_marker(c, a, th, e, S, hcos, hsin, g);
+        }
     }
     if (valid) {
         const int8_t *walls = reinterpret_cast<const int8_t *>(blob + c.off_walls);
@@ -3673,11 +3762,18 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
                 }
             }
             base[i] = b; food[i] = f;
-            uint32_t v = f != kGodNone ? f : (b != kGodNone ? b : kGodWhite);
-            if (c.kind == MGB_MAZE_2D && x == ag.x && y == ag.y) v = kGodRed;
+            const bool at_agent = x == ag.x && y == ag.y;
+            uint32_t v;
+            if (traj) {
+                v = f != kGodNone ? f : (at_agent ? kGodRed : (b != kGodNone ? b : kGodWhite));
+            } else {
+                v = f != kGodNone ? f : (b != kGodNone ? b : kGodWhite);
+                if (c.kind == MGB_MAZE_2D && at_agent) v = kGodRed;
+            }
             cell[i] = v;
         }
         const double rcs = (double)S / (double)n;
+        const double soff = traj ? 0.0 : (double)S;                // x offset of the rects drawn on the screen
         for (int p = threadIdx.x; p < S; p += blockDim.x) {
             const double pcen = (double)p + 0.5;
             const int cx0 = (int)(pcen / rcs), cy0 = (int)(((double)S - pcen) / rcs);   // y points up
@@ -3687,8 +3783,8 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
                 if (q >= 0 && q < n) {
                     const double x0 = q * rcs;                     // x * self._render_cell_size
                     if (x0 <= pcen && pcen < x0 + rcs) god_push(vg, q);
-                    const double x1 = q * rcs + (double)S;         // ... + offset[0] (draw_food, the 2-D agent rect)
-                    if (x1 <= pcen + (double)S && pcen + (double)S < x1 + rcs) god_push(vs, q);
+                    const double x1 = q * rcs + soff;              // ... + offset[0] (draw_food, the 2-D agent rect)
+                    if (x1 <= pcen + soff && pcen + soff < x1 + rcs) god_push(vs, q);
                 }
                 if (r >= 0 && r < n) {
                     const double y0 = (double)S - (r + 1) * rcs;   // view_size - (y + 1) * self._render_cell_size
@@ -3716,6 +3812,7 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
                     const uint32_t b = base[gs[i] * n + ys[j]];
                     if (b != kGodNone) v = b;
                 }
+        if (traj && (gs[0] == ge.gx || gs[1] == ge.gx) && (ys[0] == ge.gy || ys[1] == ge.gy)) v = kGodRed;
         if (surv) {
 #pragma unroll
             for (int i = 0; i < 2; ++i)
@@ -3726,7 +3823,7 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
                         if (f != kGodNone) v = f;
                     }
         }
-        if (is2d && (ss[0] == ge.gx || ss[1] == ge.gx) && (ys[0] == ge.gy || ys[1] == ge.gy)) v = kGodRed;
+        if (is2d && !traj && (ss[0] == ge.gx || ss[1] == ge.gx) && (ys[0] == ge.gy || ys[1] == ge.gy)) v = kGodRed;
         return v;
     };
     auto colour = [&](int row, int col, int cy) -> uint32_t {
@@ -3791,13 +3888,107 @@ __global__ void __launch_bounds__(kGodThreads) maze_god_view_kernel(const __grid
     }
 }
 
+// pygame.draw.line(surface, red, p, q, width=3) between the centres of cells (x0, y0) and (x1, y1): the Bresenham pixels of
+// the truncated end points, each widened into a 3-pixel span across the minor axis (along x when |dx| <= |dy|, along y
+// otherwise; a zero-length segment is one span).  Pixels outside the panel are dropped.
+// Pixels i0, i0 + di, ... of the line: one thread walks a whole segment with (0, 1), a warp's lanes share one with
+// (lane, 32), so that the warp's stores of a step lie side by side.
+__device__ void god_wide_line(uint8_t *frame, int S, double rcs, int x0c, int y0c, int x1c, int y1c, int i0 = 0, int di = 1)
+{
+    const int x0 = god_trunc((x0c + 0.5) * rcs), y0 = god_trunc((double)S - (y0c + 0.5) * rcs);
+    const int x1 = god_trunc((x1c + 0.5) * rcs), y1 = god_trunc((double)S - (y1c + 0.5) * rcs);
+    const int dx = abs(x1 - x0), dy = abs(y1 - y0);
+    const int sx = x1 >= x0 ? 1 : -1, sy = y1 >= y0 ? 1 : -1;
+    const bool span_x = dx <= dy;
+    const int len = dx >= dy ? dx : dy;
+    for (int i = i0; i <= len; i += di) {
+        int px, py;
+        if (dx >= dy) { px = x0 + sx * i; py = dx == 0 ? y0 : y0 + sy * (int)((2LL * i * dy + dx) / (2LL * dx)); }
+        else { py = y0 + sy * i; px = x0 + sx * (int)((2LL * i * dx + dy) / (2LL * dy)); }
+        for (int k = -1; k <= 1; ++k) {
+            const int qx = span_x ? px + k : px, qy = span_x ? py : py + k;
+            if (qx < 0 || qx >= S || qy < 0 || qy >= S) continue;
+            uint8_t *d = frame + ((int64_t)qy * S + qx) * 3;
+            d[0] = 255; d[1] = 0; d[2] = 0;
+        }
+    }
+}
+
+// The path lines of render_trajectory (maze_base.py:178-183) over the panel maze_god_view_kernel<traj> left in `out`: one
+// CTA per env.  Every line is the same red, so the picture depends only on the set of distinct segments: segments between
+// neighbouring cells (every discrete move) are collected as direction bits per cell in shared memory and drawn once each;
+// longer ones (a continuous env crossing more than one cell in a step) are drawn where they are found.  A segment with an
+// end that was never recorded ((-1, -1), recording switched on mid-episode) is skipped.
+__global__ void __launch_bounds__(kGodThreads) maze_god_path_kernel(const __grid_constant__ MazeConst c,
+                                                                    const __grid_constant__ MazeArgs a,
+                                                                    const int32_t *__restrict__ envs, int S,
+                                                                    uint8_t *__restrict__ out)
+{
+    __shared__ uint32_t s_dirs[kMaxN * kMaxN];     // bit (dy + 1) * 3 + dx + 1: the segment from the cell to (x + dx, y + dy)
+    __shared__ uint16_t s_segs[kMaxN * kMaxN * 9]; // the set bits as cell * 9 + bit, in no particular order
+    __shared__ int s_nseg;
+    const int64_t k = blockIdx.x;
+    const int64_t e = envs ? (int64_t)envs[k] : k;
+    if (e < 0 || e >= a.n) return;                 // the frame stays all zero
+    const int n = c.n, nn = n * n;
+    for (int i = threadIdx.x; i < nn; i += blockDim.x) s_dirs[i] = 0u;
+    if (threadIdx.x == 0) s_nseg = 0;
+    __syncthreads();
+    const int steps = a.agent[e].w;
+    const int len = (steps < c.max_steps ? steps : c.max_steps) + 1;
+    uint8_t *frame = out + k * (int64_t)S * S * 3;
+    const double rcs = (double)S / (double)n;      // render_init: view_size / self._n
+    for (int i = threadIdx.x; i + 1 < len; i += blockDim.x) {
+        const char2 p = a.path[(int64_t)i * a.n_pad + e], q = a.path[(int64_t)(i + 1) * a.n_pad + e];
+        if (p.x < 0 || p.y < 0 || q.x < 0 || q.y < 0) continue;
+        const int dx = q.x - p.x, dy = q.y - p.y;
+        if (dx >= -1 && dx <= 1 && dy >= -1 && dy <= 1 && p.x < n && p.y < n)
+            atomicOr(&s_dirs[p.x * n + p.y], 1u << ((dy + 1) * 3 + dx + 1));
+        else
+            god_wide_line(frame, S, rcs, p.x, p.y, q.x, q.y);
+    }
+    __syncthreads();
+    for (int cl = threadIdx.x; cl < nn; cl += blockDim.x) {
+        uint32_t m = s_dirs[cl];
+        if (!m) continue;
+        int j = atomicAdd(&s_nseg, __popc(m));
+        for (; m; m &= m - 1) s_segs[j++] = (uint16_t)(cl * 9 + __ffs(m) - 1);
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nseg = s_nseg;
+    for (int j = warp; j < nseg; j += kGodThreads / 32) {         // one warp per segment, lanes along it
+        const int cl = s_segs[j] / 9, d = s_segs[j] - cl * 9;
+        const int x = cl / n, y = cl - x * n;
+        god_wide_line(frame, S, rcs, x, y, x + d % 3 - 1, y + d / 3 - 1, lane, 32);
+    }
+}
+
+// mgb_maze_path: env envs[k]'s current-episode path -> cells[k][0 .. len), len[k]
+__global__ void maze_path_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a,
+                                 const int32_t *__restrict__ envs, int64_t cap, char2 *__restrict__ cells,
+                                 int32_t *__restrict__ lens)
+{
+    const int64_t k = blockIdx.x;
+    const int64_t e = envs ? (int64_t)envs[k] : k;
+    int len = 0;
+    if (e >= 0 && e < a.n) {
+        const int steps = a.agent[e].w;
+        len = (steps < c.max_steps ? steps : c.max_steps) + 1;
+    }
+    if (threadIdx.x == 0) lens[k] = len;
+    for (int i = threadIdx.x; i < len; i += blockDim.x) cells[k * cap + i] = a.path[(int64_t)i * a.n_pad + e];
+}
+
 }  // namespace
 
 extern "C" int mgb_maze_god_view(mgb_maze *h, int32_t count, const int32_t *envs_dev, int32_t view_size, int32_t mode,
                                  uint8_t *out_dev, void *stream)
 {
     MGB_REQUIRE(h, "null argument");
-    MGB_REQUIRE(mode == MGB_GOD_LIVE, "mgb_maze_god_view: mode must be MGB_GOD_LIVE");
+    MGB_REQUIRE(mode == MGB_GOD_LIVE || mode == MGB_GOD_TRAJECTORY,
+                "mgb_maze_god_view: mode must be MGB_GOD_LIVE or MGB_GOD_TRAJECTORY");
+    MGB_REQUIRE(mode != MGB_GOD_TRAJECTORY || h->path,
+                "mgb_maze_god_view: MGB_GOD_TRAJECTORY needs path recording (mgb_maze_set_path)");
     MGB_REQUIRE(count >= 0 && count <= INT_MAX / 2, "mgb_maze_god_view: count out of range");
     MGB_REQUIRE(view_size >= 1 && view_size <= kGodMaxView, "mgb_maze_god_view: view_size must be in [1, 4096]");
     MGB_REQUIRE(h->has_task, "mgb_maze_god_view: set a task first");
@@ -3824,7 +4015,29 @@ extern "C" int mgb_maze_god_view(mgb_maze *h, int32_t count, const int32_t *envs
     const size_t smem = (size_t)3 * h->c.n * h->c.n * 4 + (size_t)3 * view_size * sizeof(char2) + (size_t)2 * view_size;
     maze_god_view_kernel<<<dim3((unsigned)count, (unsigned)split), kGodThreads, smem, (cudaStream_t)stream>>>(
         h->c, a, envs_dev, view_size, make_float4(hc[0], hc[1], hc[2], hc[3]), make_float4(hs[0], hs[1], hs[2], hs[3]),
-        out_dev);
+        out_dev, mode == MGB_GOD_TRAJECTORY);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    if (mode == MGB_GOD_TRAJECTORY) {
+        maze_god_path_kernel<<<(unsigned)count, kGodThreads, 0, (cudaStream_t)stream>>>(h->c, a, envs_dev, view_size, out_dev);
+        MGB_CUDA(cudaGetLastError());
+        h->launches += 1;
+    }
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_path(mgb_maze *h, int32_t count, const int32_t *envs_dev, int8_t *cells_out, int32_t *len_out,
+                             void *stream)
+{
+    MGB_REQUIRE(h, "null argument");
+    MGB_REQUIRE(h->path, "mgb_maze_path: path recording is off (mgb_maze_set_path)");
+    MGB_REQUIRE(count >= 0 && count <= INT_MAX / 2, "mgb_maze_path: count out of range");
+    if (count == 0) return MGB_OK;
+    MGB_REQUIRE(cells_out && len_out, "mgb_maze_path: null output");
+    MGB_REQUIRE(envs_dev || count <= h->n, "mgb_maze_path: count exceeds the env count (pass envs_dev)");
+    MgbDeviceGuard guard(h->device);
+    maze_path_kernel<<<(unsigned)count, 256, 0, (cudaStream_t)stream>>>(h->c, maze_args(h), envs_dev, path_cap(h),
+                                                                         reinterpret_cast<char2 *>(cells_out), len_out);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     return MGB_OK;
@@ -3885,6 +4098,7 @@ extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev,
 //   [32, 48)  continuous position f32 x 2 | heading f64 (zero for the other kinds)
 //   [48, ..)  food stamps int32 [f_max], in groups of four (16 bytes each, unused tail zero)
 //   [tail, ..) the task of the env's slot, blob_bytes, when records carry their tasks
+//   [.., ..)  path recording on: the path entries char2 [max_steps + 1], padded to 16 bytes
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
 
@@ -3960,6 +4174,25 @@ __global__ void maze_record_tasks_kernel(int64_t n, int blob_bytes, const int32_
     }
 }
 
+// Every env's path entries <-> its record at byte `off`, over all (entry, env) pairs, env fastest (the path is
+// step-major).  LOAD: restore (row map as for maze_restore_kernel), else snapshot.
+template <bool LOAD>
+__global__ void maze_record_path_kernel(int64_t n, int64_t n_pad, int64_t cap, char2 *path, uint8_t *rec, int64_t rec_bytes,
+                                        int64_t off, int64_t n_rec, const int64_t *__restrict__ row)
+{
+    const int64_t total = n * cap;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t s = i / n, e = i - s * n;
+        char2 *p = path + s * n_pad + e;
+        if (LOAD) {
+            const int64_t rw = row[e];
+            if (rw >= 0 && rw < n_rec) *p = reinterpret_cast<const char2 *>(rec + rw * rec_bytes + off)[s];
+        } else {
+            reinterpret_cast<char2 *>(rec + e * rec_bytes + off)[s] = *p;
+        }
+    }
+}
+
 }  // namespace
 
 // Records carry their env's whole task when the env owns its table slot and the table can change on the device
@@ -3974,9 +4207,33 @@ static bool records_carry_tasks(const mgb_maze *h)
 
 static int64_t record_tail(const mgb_maze *h) { return kMazeRecHead + (int64_t)(h->c.f_max + 3) / 4 * 16; }
 
-static int64_t record_bytes(const mgb_maze *h)
+// where the path entries start in a record (recording on)
+static int64_t record_path_off(const mgb_maze *h)
 {
     return record_tail(h) + (records_carry_tasks(h) ? h->c.blob_bytes : 0);
+}
+
+static int64_t record_bytes(const mgb_maze *h)
+{
+    return record_path_off(h) + (h->path ? (path_cap(h) * 2 + 15) / 16 * 16 : 0);
+}
+
+// snapshot (LOAD false) or restore the path entries of the records
+static int record_paths(mgb_maze *h, bool load, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row, cudaStream_t st)
+{
+    if (!h->path) return MGB_OK;
+    const int64_t total = h->n * path_cap(h), most = (int64_t)h->num_sms * 16;
+    const int64_t grid = (total + 255) / 256 < most ? (total + 255) / 256 : most;
+    uint8_t *rec = const_cast<uint8_t *>(rec_dev);
+    if (load)
+        maze_record_path_kernel<true><<<(unsigned)grid, 256, 0, st>>>(h->n, h->n_pad, path_cap(h), h->path, rec,
+                                                                     record_bytes(h), record_path_off(h), n_rec, row);
+    else
+        maze_record_path_kernel<false><<<(unsigned)grid, 256, 0, st>>>(h->n, h->n_pad, path_cap(h), h->path, rec,
+                                                                      record_bytes(h), record_path_off(h), 0, nullptr);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
 }
 
 extern "C" int64_t mgb_maze_record_bytes(const mgb_maze *h)
@@ -4007,7 +4264,7 @@ extern "C" int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream)
         MGB_CUDA(cudaGetLastError());
         h->launches += 1;
     }
-    return MGB_OK;
+    return record_paths(h, false, rec_dev, 0, nullptr, st);
 }
 
 extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row_of_env_dev,
@@ -4042,7 +4299,7 @@ extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_r
         MGB_CUDA(cudaGetLastError());
         h->launches += 1;
     }
-    return MGB_OK;
+    return record_paths(h, true, rec_dev, n_rec, row_of_env_dev, st);
 }
 
 extern "C" int mgb_maze_counters(mgb_maze *h, uint64_t *t_base, int set)
@@ -4067,6 +4324,11 @@ extern "C" int mgb_maze_fingerprint(const mgb_maze *h, uint64_t *out)
     f = mgb_fnv(f, &c.max_hits, sizeof(c.max_hits));
     f = mgb_fnv(f, &h->min_cell, sizeof(h->min_cell));
     f = mgb_fnv(f, h->cls_heights.data(), h->cls_heights.size() * sizeof(double));
+    if (h->path) {                              // path recording and its capacity (a handle without it hashes as before)
+        const int64_t cap = path_cap(h);
+        f = mgb_fnv(f, "path", 4);
+        f = mgb_fnv(f, &cap, sizeof(cap));
+    }
     out[0] = mgb_fnv(f, &rb, sizeof(rb));
     out[1] = h->fp_tex;
     uint64_t t = 0;

@@ -203,7 +203,7 @@ class _BatchedMazeBase(Snapshots):
     KIND = None
     _SNAP_PREFIX = "mgb_maze"
     _FINGERPRINT_PARTS = ("configuration (kind, task type, max_steps, view, resolution, obs dtype, optics, auto_reset, "
-                          "table shape)", "textures", "task table", "record mode (per-env tasks or a shared table)")
+                          "table shape, path recording)", "textures", "task table", "record mode (per-env tasks or a shared table)")
 
     def _snap_kind(self):
         return ("maze2d", "maze_discrete_3d", "maze_continuous_3d")[self.KIND]
@@ -216,12 +216,14 @@ class _BatchedMazeBase(Snapshots):
             self.env2task = np.ascontiguousarray(np.where(row >= 0, slot[np.maximum(row, 0)], self.env2task),
                                                  dtype=np.int32)
 
-    def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs=False):
+    def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs=False,
+               record_path=False):
         import torch
         assert task_type in ("SURVIVAL", "ESCAPE")
         if final_obs and not auto_reset:
             raise ValueError("final_obs=True needs auto_reset=True (without auto-reset obs already is the terminal frame)")
         self._want_final = bool(final_obs)
+        self.record_path = bool(record_path)
         self._torch = torch
         self.num_envs = int(num_envs)
         self.task_type = task_type
@@ -286,6 +288,8 @@ class _BatchedMazeBase(Snapshots):
                                              self.env_index_base))
         self._h, self._n_cells = h, n_cells
         _lib.check(self._lib.mgb_maze_set_options(self._h, int(self.auto_reset)))
+        if self.record_path:
+            _lib.check(self._lib.mgb_maze_set_path(self._h, 1))
         self._after_create()
 
     @staticmethod
@@ -478,11 +482,34 @@ class _BatchedMazeBase(Snapshots):
     def launch_count(self):
         return int(self._lib.mgb_maze_launch_count(self._h)) if self._h else 0
 
-    def god_view(self, envs=None, view_size=None, out=None):
+    def _env_index(self, envs):
+        """envs -> (int32 CUDA tensor or None for all envs, K).  A host sequence is range-checked; a CUDA tensor is moved
+        to the env's device unchecked (no host synchronisation)."""
+        if envs is None:
+            return None, self.num_envs
+        if hasattr(envs, "is_cuda") and envs.is_cuda:
+            e = envs.to(device=self.device, dtype=self._torch.int32).reshape(-1).contiguous()
+        else:
+            idx = np.asarray(envs, dtype=np.int64).reshape(-1)
+            if idx.size and (idx.min() < 0 or idx.max() >= self.num_envs):
+                raise IndexError("env index out of range [0, %d)" % self.num_envs)
+            e = self._torch.as_tensor(idx.astype(np.int32), device=self.device)
+        return e, int(e.numel())
+
+    def _require_path(self, what):
+        if not self.record_path:
+            raise ValueError("%s needs path recording: construct the env with record_path=True" % what)
+
+    def god_view(self, envs=None, view_size=None, out=None, trajectory=False):
         """Top-down views of many envs in one launch (mgb_maze_god_view): the god panel of the reference window
         (render_init + render_update, maze_base.py:100-157): white floor, black walls, the ESCAPE goal in green, SURVIVAL
         food in (f, 255, f) with f = int(255 - 255 food), and the agent (2-D: red cell; 3-D: green disc and heading line).
         The text labels are not drawn.
+
+        trajectory=True (needs record_path=True): the picture of the reference's save_trajectory() instead
+        (MazeBase.render_trajectory, maze_base.py:159-189): walls and goal, a red rect at the agent's cell for every kind,
+        SURVIVAL food over it, and red lines of width 3 between the centres of consecutive cells of the current episode's
+        path.
 
         envs: local env indices (default: all), a host sequence (checked) or a CUDA tensor, moved to the env's device as
         int32 (not checked: an index out of range gives an all-zero frame; no host synchronisation, so the call can be
@@ -492,29 +519,78 @@ class _BatchedMazeBase(Snapshots):
         (x, y) of the panel, so it is transposed against the x-major 3-D observations."""
         if self.need_set_task:
             raise Exception("Must call \"set_task\" before reset")
+        if trajectory:
+            self._require_path("god_view(trajectory=True)")
         torch = self._torch
         S = self.render_scale if view_size is None else view_size
         if int(S) != S or not 1 <= int(S) <= 4096:
             raise ValueError("view_size must be an integer in [1, 4096], got %r" % (view_size,))
         S = int(S)
-        e = None
-        K = self.num_envs
-        if envs is not None:
-            if hasattr(envs, "is_cuda") and envs.is_cuda:
-                e = envs.to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
-            else:
-                idx = np.asarray(envs, dtype=np.int64).reshape(-1)
-                if idx.size and (idx.min() < 0 or idx.max() >= self.num_envs):
-                    raise IndexError("env index out of range [0, %d)" % self.num_envs)
-                e = torch.as_tensor(idx.astype(np.int32), device=self.device)
-            K = int(e.numel())
+        e, K = self._env_index(envs)
         if out is None:
             out = torch.empty((K, S, S, 3), dtype=torch.uint8, device=self.device)
         elif (tuple(out.shape) != (K, S, S, 3) or out.dtype != torch.uint8 or out.device != self.device
               or not out.is_contiguous()):
             raise ValueError("out must be a contiguous uint8 tensor of shape %s on %s" % ((K, S, S, 3), self.device))
-        _lib.check(self._lib.mgb_maze_god_view(self._h, K, _lib.ptr(e), S, 0, _lib.ptr(out), self._stream()))
+        _lib.check(self._lib.mgb_maze_god_view(self._h, K, _lib.ptr(e), S, 1 if trajectory else 0, _lib.ptr(out),
+                                               self._stream()))
         return out
+
+    def trajectory(self, envs=None):
+        """The current episode's path of each env (record_path=True): MazeBase._agent_trajectory, the start cell and the
+        agent's cell after every step since the last reset (maze_base.py:44,67).  envs as for god_view().  Returns CUDA
+        tensors (cells int32 [K, max_steps + 1, 2] = (grid_x, grid_y), -1 past each env's length; lengths int32 [K]),
+        without a host synchronisation.  An env without auto-reset stepped on past max_steps keeps max_steps + 1 cells."""
+        if self.need_set_task:
+            raise Exception("Must call \"set_task\" before reset")
+        self._require_path("trajectory()")
+        torch = self._torch
+        e, K = self._env_index(envs)
+        cap = int(self.max_steps) + 1
+        cells = torch.empty((K, cap, 2), dtype=torch.int8, device=self.device)
+        lens = torch.empty((K,), dtype=torch.int32, device=self.device)
+        _lib.check(self._lib.mgb_maze_path(self._h, K, _lib.ptr(e), _lib.ptr(cells), _lib.ptr(lens), self._stream()))
+        valid = torch.arange(cap, device=self.device)[None, :, None] < lens[:, None, None]
+        return torch.where(valid, cells.to(torch.int32), torch.full_like(cells, -1, dtype=torch.int32)), lens
+
+    def save_trajectory(self, file_name, envs=None):
+        """The reference's save_trajectory(file_name) (maze_env.py:82,152; MazeBase.render_trajectory): PNG files of
+        god_view(trajectory=True) at render_scale.  With num_envs == 1 and squeeze the file is `file_name`; otherwise
+        one file per selected env (envs: host indices, default all), <file_name without extension>_<env index>.png.
+        Returns the list of files written."""
+        return self._save_trajectory(file_name, envs, None)
+
+    def _save_trajectory(self, file_name, envs, additional):
+        import os
+        from .png import write_png
+        idx = list(range(self.num_envs)) if envs is None else [int(v) for v in np.asarray(envs).reshape(-1)]
+        frames = self.god_view(envs=idx, trajectory=True).cpu().numpy()
+        if self._squeeze and envs is None:
+            names, stems = [file_name], [file_name.split(".")[0]]       # the reference's names (maze_base.py:185,187)
+        else:
+            stem, _ = os.path.splitext(file_name)
+            stems = ["%s_%d" % (stem, e) for e in idx]
+            names = [s + ".png" for s in stems]
+        written = []
+        for name, base, panel in zip(names, stems, frames):
+            if additional is None:
+                write_png(name, panel)
+                written.append(name)
+                continue
+            # render_trajectory with additional (maze_base.py:161-187): a white (S + aw) x max(S, ah) canvas, the panel
+            # at (0, 0), each surface blitted at (S, 0) over the previous one and saved as stem + file_names[i] + ".png"
+            surfaces = [np.asarray(s, dtype=np.uint8) for s in additional["surfaces"]]
+            S = panel.shape[0]
+            ah, aw = surfaces[0].shape[:2]
+            canvas = np.full((max(S, ah), S + aw, 3), 255, dtype=np.uint8)
+            canvas[:S, :S] = panel
+            for surf, suffix in zip(surfaces, additional["file_names"]):
+                h, w = min(surf.shape[0], canvas.shape[0]), min(surf.shape[1], aw)
+                canvas[:h, S:S + w] = surf[:h, :w]
+                out = base + suffix + ".png"
+                write_png(out, canvas)
+                written.append(out)
+        return written
 
     def render(self, mode="human"):
         """mode="rgb_array": god_view() of every env at render_scale ([S, S, 3] for num_envs=1 with squeeze).  The
@@ -560,13 +636,14 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
     _MIRROR_PREFIX = "mgb_maze"
 
     def __init__(self, enable_render=False, render_scale=480, max_steps=5000, task_type="SURVIVAL", view_grid=2,
-                 num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True, final_obs=False):
+                 num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True, final_obs=False,
+                 record_path=False):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
         self.render_scale = int(render_scale)
         self.view_grid = int(view_grid)
-        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs)
+        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path)
         w = 2 * self.view_grid + 1
         # the reference declares Box(-1, 1, (3,3), int32) but returns float32 (2g+1)^2 arrays (maze_2d.py:92)
         self.observation_space = Box(low=-1, high=1, shape=(w, w), dtype=np.float32)
@@ -590,6 +667,13 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         caller-supplied `out` may omit either entry, and that output is then not produced."""
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final)
 
+    def save_trajectory(self, file_name, envs=None, additional=None):
+        """MetaMaze2D.save_trajectory(file_name, additional) (maze_env.py:211-212), file names as for the 3-D envs.
+        additional = {"surfaces": [uint8 [H, W, 3] images], "file_names": [suffixes]}: each surface is placed right of the
+        panel on a white (S + W) x max(S, H) canvas (W, H of the first surface), and the canvas is saved as the file
+        name before its first "." + file_names[i] + ".png", as the reference does."""
+        return self._save_trajectory(file_name, envs, additional)
+
 
 class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     """MetaMazeDiscrete3D(enable_render, render_scale, resolution, max_steps, task_type) x num_envs
@@ -602,7 +686,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     def __init__(self, enable_render=False, render_scale=480, resolution=(320, 320), max_steps=5000,
                  task_type="SURVIVAL", num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True,
                  obs_dtype="int32", textures=None, max_vision_range=12.0, fol_angle=0.6 * PI, cache=None,
-                 final_obs=False):
+                 final_obs=False, record_path=False):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
@@ -613,7 +697,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         self.max_vision_range, self.fol_angle = max_vision_range, fol_angle
         self.cache = cache                  # None: library default (on, MGB_MAZE_CACHE); False: direct renderer only
         self.textures = textures if textures is not None else synthetic_textures(seed=0)
-        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs)
+        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path)
         torch = self._torch
         h, v = self.resolution
         self.observation_space = Box(low=0, high=256, shape=(h, v, 3), dtype=np.float32)     # maze_env.py:37-39
