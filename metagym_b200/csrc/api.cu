@@ -35,11 +35,11 @@ extern "C" int mgb_peer_alloc(int device, uint64_t bytes, void **ptr_out)
     MGB_REQUIRE(ptr_out && bytes > 0, "bad argument");
     MgbDeviceGuard guard(device);
     MGB_REQUIRE(guard.ok, "cannot select device");
-    void *p = nullptr;
-    MGB_CUDA(cudaMalloc(&p, bytes));          // plain cudaMalloc: the only kind cudaIpcGetMemHandle accepts
-    MGB_CUDA(cudaMemset(p, 0, bytes));
+    MgbDev<uint8_t> p;
+    MGB_CUDA(p.alloc(bytes));                 // plain cudaMalloc: the only kind cudaIpcGetMemHandle accepts
+    MGB_CUDA(cudaMemset(p.get(), 0, bytes));
     MGB_CUDA(cudaDeviceSynchronize());
-    *ptr_out = p;
+    *ptr_out = p.release();                   // the caller owns it from here (mgb_peer_free)
     return MGB_OK;
 }
 

@@ -19,7 +19,9 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <memory>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "mgb_common.cuh"
@@ -2040,22 +2042,53 @@ __global__ void maze_state_kernel(MazeArgs a, int32_t *agent_out, double *life_o
 // ---------------------------------------------------------------------------------------------------------------
 // handle + C ABI
 // ---------------------------------------------------------------------------------------------------------------
+struct MazeFinal {                 // the terminal list of mgb_maze_step_ex (MazeArgs::fin_*, 3-D kinds)
+    MgbDev<int32_t> count, env, task, eaten;
+    MgbDev<EnvDyn> dyn;
+    MgbDev<int4> agent;
+    MgbDev<double> life, cori;
+    MgbDev<float2> cpos;
+};
+
+struct MazeTasks {                 // what mgb_maze_set_task sizes by its table; the terminal list too, so that step_ex can be captured
+    MgbDev<uint8_t> blobs;
+    MgbDev<int32_t> eaten;
+    MgbDev<double> efftab, fogtab;
+    MazeFinal fin;
+};
+
+struct MazePoseCache {             // built by ensure_pose_cache (MazeArgs describes each table)
+    MgbDev<int4> poses;
+    MgbDev<int32_t> pose_index, c_vbase;
+    MgbDev<uint32_t> c_px, c_px_all;
+    MgbDev<uint8_t> c_fid, c_colhits, c_rgb8, c_gsig, c_var8;
+    MgbDev<uint64_t> c_fmask;
+    MgbDev<HitRec> c_hits;
+    MgbDev<EnvDyn> dyn;
+    MgbDev<BakeDesc> bake_desc;
+    MgbDev<PoseRec> pose_rec;      // built after the variant frames
+};
+
+struct MazeStage {                 // one half of the double-buffered staging of mgb_maze_update_tasks
+    MgbPinned<uint8_t> host;
+    MgbDev<uint8_t> dev;
+    size_t bytes = 0;
+    MgbEvent copied;               // recorded after the copy from `host`
+};
+
 struct mgb_maze {
     int device = 0;
     int64_t n = 0, n_pad = 0, env_base = 0;
     mgb_maze_cfg cfg;
     MazeConst c;
-    int4 *agent = nullptr;
-    double *life = nullptr;
-    int32_t *eaten = nullptr;
-    int32_t *env2task = nullptr;
-    uint8_t *blobs = nullptr;
-    uint32_t *tex = nullptr;
-    float *coltab = nullptr;
-    double *efftab = nullptr, *fogtab = nullptr;
-    float2 *cpos = nullptr;        // continuous maze pose
-    double *cori = nullptr;
-    double *coltab_d = nullptr;
+    MgbDev<int4> agent;
+    MgbDev<double> life;
+    MgbDev<int32_t> env2task;
+    MazeTasks tasks;
+    MgbDev<uint32_t> tex;
+    MgbDev<float> coltab;
+    MgbDev<float2> cpos;           // continuous maze pose
+    MgbDev<double> cori, coltab_d;
     // pose cache
     int render_pipe = 1;           // MGB_MAZE_RENDER_PIPE=0: direct renderer without the geometry / pixel software pipeline
     int fused_step = 1;            // MGB_MAZE_FUSED_STEP=0: logic kernel + compose kernel instead of maze3d_step_kernel
@@ -2065,37 +2098,21 @@ struct mgb_maze {
     double cache_budget_gb = 24.0; // MGB_MAZE_CACHE_GB
     bool cache_ready = false, cache_dirty = true;
     int64_t n_poses = 0;
-    int4 *poses = nullptr;
-    int32_t *pose_index = nullptr;
-    uint32_t *c_px = nullptr;
-    uint8_t *c_fid = nullptr, *c_colhits = nullptr, *c_rgb8 = nullptr;
-    uint32_t *c_px_all = nullptr;
-    uint64_t *c_fmask = nullptr;
-    uint32_t *task_epoch = nullptr;           // [n_pad] how often each env's task has been resampled on the device
+    MazePoseCache cache;
+    MgbDev<uint32_t> task_epoch;              // [n_pad] how often each env's task has been resampled on the device
     bool slot_per_env = false;                // env2task is injective: every env owns its task-table slot
-    uint8_t *task_flags = nullptr;            // [n_tasks] scratch of mgb_maze_update_tasks
-    int task_flags_n = 0;
+    MgbDev<uint8_t> task_flags;               // [n_tasks] scratch of mgb_maze_update_tasks
     bool cache_would_fit = true;              // last ensure_pose_cache decision (false: over budget -> direct renderer)
     std::vector<double> cls_heights;          // eff-table classes of the current task table
     double min_cell = 0.0;                    // smallest cell_size of the table (bounds the crossings a ray can record)
-    uint8_t *h_stage[2] = {nullptr, nullptr}; // pinned staging of mgb_maze_update_tasks (double-buffered)
-    uint8_t *d_stage[2] = {nullptr, nullptr};
-    size_t stage_bytes[2] = {0, 0};
-    cudaEvent_t stage_done[2] = {nullptr, nullptr};
+    MazeStage stage[2];
     int stage_next = 0;
-    int32_t *c_vbase = nullptr;
-    void *pose_rec = nullptr;      // PoseRec table, built after the variant frames
-    uint8_t *c_var8 = nullptr;
-    void *d_bake_desc = nullptr;
     int64_t n_var_frames = 0;
     int64_t k_hist[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // poses by the number of foods their image depends on (8 = 8 or more)
     int variant_bits_used = 0;
     double cache_bytes = 0.0;
     int variant_bits = 7;          // MGB_MAZE_VARIANT_BITS: poses that depend on <= this many foods get all 2^k frames (0 = off)
-    uint8_t *c_gsig = nullptr;
-    HitRec *c_hits = nullptr;
-    EnvDyn *dyn = nullptr;
-    void *hit_scratch = nullptr;
+    MgbDev<uint8_t> hit_scratch;
     size_t hit_scratch_bytes = 0;
     std::vector<int4> host_poses;
     std::vector<int32_t> host_pose_index;
@@ -2113,13 +2130,7 @@ struct mgb_maze {
     std::vector<uint64_t> slot_fp;            // fingerprint of every task-table slot as set_task / update_tasks wrote it
     MgbMirrors mir = {};         // mgb_maze_set_mirrors
     MgbMirrorWindow mir_win;     // mgb_maze_set_mirror_window
-    // terminal list of mgb_maze_step_ex (allocated by its first 3-D call with final_obs)
-    int32_t *fin_count = nullptr, *fin_env = nullptr, *fin_task = nullptr, *fin_eaten = nullptr;
-    EnvDyn *fin_dyn = nullptr;
-    int4 *fin_agent = nullptr;
-    double *fin_life = nullptr, *fin_cori = nullptr;
-    float2 *fin_cpos = nullptr;
-    char2 *path = nullptr;         // mgb_maze_set_path: [max_steps + 1][n_pad] recorded cells, nullptr when not recording
+    MgbDev<char2> path;            // mgb_maze_set_path: [max_steps + 1][n_pad] recorded cells, empty when not recording
 };
 
 // entries of one env's path record: an episode ends at steps <= max_steps
@@ -2146,12 +2157,12 @@ static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
     return off;
 }
 
-// The pose-cache tables of h, into args filled before ensure_pose_cache (re)built them
-static void bind_pose_cache(const mgb_maze *h, MazeArgs &a)
+// The tables of a pose cache, into args filled before ensure_pose_cache (re)built it
+static void bind_pose_cache(const MazePoseCache &pc, MazeArgs &a)
 {
-    a.poses = h->poses; a.pose_index = h->pose_index; a.pose_rec = h->pose_rec; a.c_px = h->c_px; a.c_fid = h->c_fid;
-    a.c_colhits = h->c_colhits; a.c_hits = h->c_hits; a.dyn = h->dyn; a.c_rgb8 = h->c_rgb8; a.c_gsig = h->c_gsig;
-    a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask; a.c_vbase = h->c_vbase; a.c_var8 = h->c_var8;
+    a.poses = pc.poses.get(); a.pose_index = pc.pose_index.get(); a.pose_rec = pc.pose_rec.get(); a.c_px = pc.c_px.get(); a.c_fid = pc.c_fid.get();
+    a.c_colhits = pc.c_colhits.get(); a.c_hits = pc.c_hits.get(); a.dyn = pc.dyn.get(); a.c_rgb8 = pc.c_rgb8.get(); a.c_gsig = pc.c_gsig.get();
+    a.c_px_all = pc.c_px_all.get(); a.c_fmask = pc.c_fmask.get(); a.c_vbase = pc.c_vbase.get(); a.c_var8 = pc.c_var8.get();
 }
 
 // Kernel arguments of the handle's state; every per-call field is zero
@@ -2160,11 +2171,11 @@ static MazeArgs maze_args(const mgb_maze *h)
     MazeArgs a;
     memset(&a, 0, sizeof(a));
     a.n = h->n; a.n_pad = h->n_pad; a.env_base = h->env_base;
-    a.agent = h->agent; a.life = h->life; a.eaten = h->eaten; a.env2task = h->env2task; a.blobs = h->blobs;
-    a.tex = h->tex; a.coltab = h->coltab; a.efftab = h->efftab; a.fogtab = h->fogtab; a.auto_reset = h->auto_reset;
-    a.cpos = h->cpos; a.cori = h->cori; a.coltab_d = h->coltab_d;
-    a.path = h->path;
-    bind_pose_cache(h, a);
+    a.agent = h->agent.get(); a.life = h->life.get(); a.eaten = h->tasks.eaten.get(); a.env2task = h->env2task.get(); a.blobs = h->tasks.blobs.get();
+    a.tex = h->tex.get(); a.coltab = h->coltab.get(); a.efftab = h->tasks.efftab.get(); a.fogtab = h->tasks.fogtab.get(); a.auto_reset = h->auto_reset;
+    a.cpos = h->cpos.get(); a.cori = h->cori.get(); a.coltab_d = h->coltab_d.get();
+    a.path = h->path.get();
+    bind_pose_cache(h->cache, a);
     return a;
 }
 
@@ -2189,7 +2200,7 @@ extern "C" int mgb_maze_create(mgb_maze **out, int64_t n_envs, const mgb_maze_cf
     MGB_CUDA(cudaGetDeviceCount(&ndev));
     MGB_REQUIRE(device >= 0 && device < ndev, "device index out of range");
     MgbDeviceGuard guard(device);
-    mgb_maze *h = new (std::nothrow) mgb_maze();
+    std::unique_ptr<mgb_maze> h(new (std::nothrow) mgb_maze());    // deleted with its buffers on every error exit
     MGB_REQUIRE(h, "out of host memory");
     h->device = device; h->n = n_envs; h->n_pad = (n_envs + 127) / 128 * 128; h->env_base = env_index_base;
     h->cfg = *cfg;
@@ -2215,11 +2226,11 @@ extern "C" int mgb_maze_create(mgb_maze **out, int64_t n_envs, const mgb_maze_cf
     }
     if (const char *ev = getenv("MGB_MAZE_CACHE")) h->cache_enabled = atoi(ev) != 0;
     if (const char *ev = getenv("MGB_MAZE_CACHE_GB")) h->cache_budget_gb = atof(ev);
-    MGB_CUDA(cudaMalloc(&h->agent, sizeof(int4) * h->n_pad));
-    MGB_CUDA(cudaMalloc(&h->life, sizeof(double) * h->n_pad));
-    MGB_CUDA(cudaMalloc(&h->env2task, sizeof(int32_t) * h->n_pad));
-    MGB_CUDA(cudaMemset(h->agent, 0, sizeof(int4) * h->n_pad));
-    MGB_CUDA(cudaMemset(h->life, 0, sizeof(double) * h->n_pad));
+    MGB_CUDA(h->agent.alloc(sizeof(int4) * h->n_pad));
+    MGB_CUDA(h->life.alloc(sizeof(double) * h->n_pad));
+    MGB_CUDA(h->env2task.alloc(sizeof(int32_t) * h->n_pad));
+    MGB_CUDA(cudaMemset(h->agent.get(), 0, sizeof(int4) * h->n_pad));
+    MGB_CUDA(cudaMemset(h->life.get(), 0, sizeof(double) * h->n_pad));
     if (cfg->kind != MGB_MAZE_2D) {
         // screen geometry and the per-heading column tables, exactly as maze_view computes them
         // (ray_caster_utils.py:68-92): float64 arithmetic, float32 sin/cos of the float32 heading, float32 tables.
@@ -2250,18 +2261,18 @@ extern "C" int mgb_maze_create(mgb_maze **out, int64_t n_envs, const mgb_maze_cf
                 tab[((size_t)k * 3 + 2) * H + d] = (float)(a1 + a2);
             }
         }
-        MGB_CUDA(cudaMalloc(&h->coltab, tab.size() * sizeof(float)));
-        MGB_CUDA(cudaMemcpy(h->coltab, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+        MGB_CUDA(h->coltab.alloc(tab.size() * sizeof(float)));
+        MGB_CUDA(cudaMemcpy(h->coltab.get(), tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
         if (cfg->kind == MGB_MAZE_CONTINUOUS_3D) {
-            MGB_CUDA(cudaMalloc(&h->coltab_d, tab_d.size() * sizeof(double)));
-            MGB_CUDA(cudaMemcpy(h->coltab_d, tab_d.data(), tab_d.size() * sizeof(double), cudaMemcpyHostToDevice));
-            MGB_CUDA(cudaMalloc(&h->cpos, sizeof(float2) * h->n_pad));
-            MGB_CUDA(cudaMalloc(&h->cori, sizeof(double) * h->n_pad));
-            MGB_CUDA(cudaMemset(h->cpos, 0, sizeof(float2) * h->n_pad));
-            MGB_CUDA(cudaMemset(h->cori, 0, sizeof(double) * h->n_pad));
+            MGB_CUDA(h->coltab_d.alloc(tab_d.size() * sizeof(double)));
+            MGB_CUDA(cudaMemcpy(h->coltab_d.get(), tab_d.data(), tab_d.size() * sizeof(double), cudaMemcpyHostToDevice));
+            MGB_CUDA(h->cpos.alloc(sizeof(float2) * h->n_pad));
+            MGB_CUDA(h->cori.alloc(sizeof(double) * h->n_pad));
+            MGB_CUDA(cudaMemset(h->cpos.get(), 0, sizeof(float2) * h->n_pad));
+            MGB_CUDA(cudaMemset(h->cori.get(), 0, sizeof(double) * h->n_pad));
         }
     }
-    *out = h;
+    *out = h.release();
     return MGB_OK;
 }
 
@@ -2270,21 +2281,7 @@ extern "C" void mgb_maze_destroy(mgb_maze *h)
     if (!h) return;
     MgbDeviceGuard guard(h->device);
     cudaDeviceSynchronize();
-    cudaFree(h->agent); cudaFree(h->life); cudaFree(h->eaten); cudaFree(h->env2task); cudaFree(h->blobs);
-    cudaFree(h->tex); cudaFree(h->coltab); cudaFree(h->efftab); cudaFree(h->fogtab); cudaFree(h->cpos); cudaFree(h->cori); cudaFree(h->coltab_d);
-    cudaFree(h->poses); cudaFree(h->pose_index); cudaFree(h->c_px); cudaFree(h->c_fid); cudaFree(h->c_colhits);
-    cudaFree(h->c_hits); cudaFree(h->dyn); cudaFree(h->c_rgb8); cudaFree(h->c_gsig); cudaFree(h->hit_scratch);
-    cudaFree(h->c_px_all); cudaFree(h->c_fmask);
-    cudaFree(h->c_vbase); cudaFree(h->c_var8); cudaFree(h->d_bake_desc); cudaFree(h->task_flags); cudaFree(h->task_epoch);
-    cudaFree(h->pose_rec);
-    cudaFree(h->fin_count); cudaFree(h->fin_env); cudaFree(h->fin_task); cudaFree(h->fin_eaten); cudaFree(h->fin_dyn);
-    cudaFree(h->fin_agent); cudaFree(h->fin_life); cudaFree(h->fin_cori); cudaFree(h->fin_cpos);
-    cudaFree(h->path);
-    for (int i = 0; i < 2; ++i) {
-        cudaFreeHost(h->h_stage[i]); cudaFree(h->d_stage[i]);
-        if (h->stage_done[i]) cudaEventDestroy(h->stage_done[i]);
-    }
-    delete h;
+    delete h;                  // the members free the handle's buffers while its device is current
 }
 
 extern "C" int64_t mgb_maze_obs_bytes_per_env(const mgb_maze *h)
@@ -2344,20 +2341,20 @@ extern "C" int mgb_maze_set_path(mgb_maze *h, int enabled)
 {
     MGB_REQUIRE(h, "null handle");
     MgbDeviceGuard guard(h->device);
-    if ((h->path != nullptr) == (enabled != 0)) return MGB_OK;
+    if ((bool)h->path == (enabled != 0)) return MGB_OK;
     MGB_CUDA(cudaDeviceSynchronize());
-    if (!enabled) {
-        MGB_CUDA(cudaFree(h->path));
-        h->path = nullptr;
-        return MGB_OK;
-    }
+    if (!enabled) { h->path.reset(); return MGB_OK; }
     const size_t bytes = sizeof(char2) * (size_t)path_cap(h) * (size_t)h->n_pad;
-    MGB_CUDA(cudaMalloc(&h->path, bytes));
-    MGB_CUDA(cudaMemset(h->path, 0xFF, bytes));             // cells (-1, -1): not recorded
-    maze_path_seed_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(h->c, maze_args(h));
+    MgbDev<char2> path;
+    MGB_CUDA(path.alloc(bytes));
+    MGB_CUDA(cudaMemset(path.get(), 0xFF, bytes));          // cells (-1, -1): not recorded
+    MazeArgs a = maze_args(h);
+    a.path = path.get();                                    // the new buffer, the handle's once it is seeded
+    maze_path_seed_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(h->c, a);
     MGB_CUDA(cudaGetLastError());
     MGB_CUDA(cudaDeviceSynchronize());
     h->launches += 1;
+    h->path = std::move(path);
     return MGB_OK;
 }
 
@@ -2378,9 +2375,10 @@ extern "C" int mgb_maze_set_textures(mgb_maze *h, const uint8_t *grounds_host, i
     for (size_t i = 0; i < px; ++i)
         packed[(size_t)n_tex * px + i] = (uint32_t)ceil_host[3 * i] | ((uint32_t)ceil_host[3 * i + 1] << 8) |
                                          ((uint32_t)ceil_host[3 * i + 2] << 16);
-    cudaFree(h->tex); h->tex = nullptr;
-    MGB_CUDA(cudaMalloc(&h->tex, packed.size() * 4));
-    MGB_CUDA(cudaMemcpy(h->tex, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice));
+    MgbDev<uint32_t> tex;
+    MGB_CUDA(tex.alloc(packed.size() * 4));
+    MGB_CUDA(cudaMemcpy(tex.get(), packed.data(), packed.size() * 4, cudaMemcpyHostToDevice));
+    h->tex = std::move(tex);
     h->c.n_tex = n_tex; h->c.ts = tex_size;
     h->fp_tex = mgb_fnv(mgb_fnv(mgb_fnv(MGB_FNV_BASIS, &n_tex, sizeof(n_tex)), &tex_size, sizeof(tex_size)), packed.data(),
                         packed.size() * 4);
@@ -2449,7 +2447,8 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     MGB_REQUIRE(n_tasks > 0, "n_tasks must be positive");
     MgbDeviceGuard guard(h->device);
     MGB_CUDA(cudaDeviceSynchronize());
-    MazeConst &c = h->c;
+    // Everything the table decides is computed into locals and checked first: a refused call leaves the handle as it was
+    MazeConst c = h->c;
     const int n = c.n, nn = n * n;
     // food slots: every cell with a positive reward (the ceiling tint of ray_caster_utils.py:150 tests "> 0")
     int f_max = 0;
@@ -2466,11 +2465,11 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     }
     MGB_REQUIRE(f_max <= 127, "at most 127 food cells per task are supported");
     for (int e = 0; e < h->n; ++e) MGB_REQUIRE(env2task_host[e] >= 0 && env2task_host[e] < n_tasks, "env2task out of range");
+    bool slot_per_env = true;
     {
         std::vector<uint8_t> used((size_t)n_tasks, 0);
-        h->slot_per_env = true;
         for (int e = 0; e < h->n; ++e) {
-            if (used[env2task_host[e]]) { h->slot_per_env = false; break; }
+            if (used[env2task_host[e]]) { slot_per_env = false; break; }
             used[env2task_host[e]] = 1;
         }
     }
@@ -2480,7 +2479,6 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     // bound the transparent crossings a column records (ray_caster_utils.py:24-61), and the reference blends every one.
     double min_cell = scalars_host[0].cell_size;
     for (int t = 1; t < n_tasks; ++t) min_cell = scalars_host[t].cell_size < min_cell ? scalars_host[t].cell_size : min_cell;
-    h->min_cell = min_cell;
     const int geo = (int)ceil(2.0 * c.max_vision / min_cell) + 3;
     int mh = f_max < geo ? f_max : geo;
     mh = mh < 2 * n - 1 ? mh : 2 * n - 1;
@@ -2503,8 +2501,7 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     c.off_fint = (int)off;  off += (size_t)(f_max > 0 ? f_max : 1) * 4;
     c.blob_bytes = (int)((off + 15) / 16 * 16);
     std::vector<uint8_t> blobs((size_t)n_tasks * c.blob_bytes, 0);
-    std::vector<double> &cls_heights = h->cls_heights;   // distinct (agent_height, wall_height) pairs, at most 8 get an eff table
-    cls_heights.clear();
+    std::vector<double> cls_heights;     // distinct (agent_height, wall_height) pairs, at most 8 get an eff table
     for (int t = 0; t < n_tasks; ++t)
         fill_task_blob(c, blobs.data() + (size_t)t * c.blob_bytes, walls_host + (size_t)t * nn, texts_host + (size_t)t * nn,
                        food_rewards_host + (size_t)t * nn, food_interval_host + (size_t)t * nn, scalars_host[t], cls_heights,
@@ -2516,34 +2513,53 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
                 MGB_REQUIRE(id >= 0 && (!h->has_tex || id < c.n_tex), "cell_texts refers to a texture that is not loaded");
             }
     }
-    cudaFree(h->blobs); h->blobs = nullptr;
-    cudaFree(h->eaten); h->eaten = nullptr;
-    MGB_CUDA(cudaMalloc(&h->blobs, blobs.size()));
-    MGB_CUDA(cudaMemcpy(h->blobs, blobs.data(), blobs.size(), cudaMemcpyHostToDevice));
+    // The old table goes before the new one is allocated (HBM never holds both); until the new one is complete every
+    // step refuses with "Must call set_task" instead of reading a half-built table.
+    h->has_task = false; h->tasks = MazeTasks();
+    const size_t eaten_bytes = sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad;
+    MazeTasks tasks;
+    MGB_CUDA(tasks.blobs.alloc(blobs.size()));
+    MGB_CUDA(cudaMemcpy(tasks.blobs.get(), blobs.data(), blobs.size(), cudaMemcpyHostToDevice));
+    MGB_CUDA(tasks.eaten.alloc(eaten_bytes));
+    MazeFinal &fin = tasks.fin;
+    if (c.kind != MGB_MAZE_2D) {
+        MGB_CUDA(fin.count.alloc(sizeof(int32_t)));
+        MGB_CUDA(fin.env.alloc(sizeof(int32_t) * h->n));
+        MGB_CUDA(fin.task.alloc(sizeof(int32_t) * h->n));
+        MGB_CUDA(fin.eaten.alloc(eaten_bytes));
+        MGB_CUDA(fin.dyn.alloc(sizeof(EnvDyn) * h->n));
+        MGB_CUDA(fin.agent.alloc(sizeof(int4) * h->n));
+        MGB_CUDA(fin.life.alloc(sizeof(double) * h->n));
+        if (c.kind == MGB_MAZE_CONTINUOUS_3D) {
+            MGB_CUDA(fin.cpos.alloc(sizeof(float2) * h->n));
+            MGB_CUDA(fin.cori.alloc(sizeof(double) * h->n));
+        }
+    }
+    MGB_CUDA(cudaMemcpy(h->env2task.get(), env2task_host, sizeof(int32_t) * h->n, cudaMemcpyHostToDevice));
+    c.n_cls = 0;
+    if (c.kind != MGB_MAZE_2D && !cls_heights.empty()) {
+        const int n_cls = (int)(cls_heights.size() / 2);
+        const size_t cells = (size_t)n_cls * c.res_h * c.res_v;
+        MgbDev<double> d_heights;
+        MGB_CUDA(tasks.efftab.alloc(cells * sizeof(double)));
+        MGB_CUDA(tasks.fogtab.alloc(cells * sizeof(double)));
+        MGB_CUDA(d_heights.alloc(cls_heights.size() * sizeof(double)));
+        MGB_CUDA(cudaMemcpy(d_heights.get(), cls_heights.data(), cls_heights.size() * sizeof(double), cudaMemcpyHostToDevice));
+        maze_efftab_kernel<<<(unsigned)((cells + 255) / 256), 256>>>(c, h->coltab.get(), d_heights.get(), n_cls, tasks.efftab.get(), tasks.fogtab.get());
+        MGB_CUDA(cudaDeviceSynchronize());
+        c.n_cls = n_cls;
+        h->launches += 1;
+    }
+    h->c = c;
+    h->tasks = std::move(tasks);
+    h->cls_heights = std::move(cls_heights);
+    h->min_cell = min_cell; h->slot_per_env = slot_per_env;
     h->slot_fp.assign((size_t)n_tasks, 0);
     for (int t = 0; t < n_tasks; ++t)
         h->slot_fp[t] = mgb_fnv(MGB_FNV_BASIS, blobs.data() + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
-    MGB_CUDA(cudaMalloc(&h->eaten, sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad));
-    if (c.kind != MGB_MAZE_2D) {     // terminal list of mgb_maze_step_ex, sized here so that its first call can be captured
-        cudaFree(h->fin_eaten); h->fin_eaten = nullptr;
-        MGB_CUDA(cudaMalloc(&h->fin_eaten, sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad));
-        if (!h->fin_count) {
-            MGB_CUDA(cudaMalloc(&h->fin_count, sizeof(int32_t)));
-            MGB_CUDA(cudaMalloc(&h->fin_env, sizeof(int32_t) * h->n));
-            MGB_CUDA(cudaMalloc(&h->fin_task, sizeof(int32_t) * h->n));
-            MGB_CUDA(cudaMalloc(&h->fin_dyn, sizeof(EnvDyn) * h->n));
-            MGB_CUDA(cudaMalloc(&h->fin_agent, sizeof(int4) * h->n));
-            MGB_CUDA(cudaMalloc(&h->fin_life, sizeof(double) * h->n));
-            if (c.kind == MGB_MAZE_CONTINUOUS_3D) {
-                MGB_CUDA(cudaMalloc(&h->fin_cpos, sizeof(float2) * h->n));
-                MGB_CUDA(cudaMalloc(&h->fin_cori, sizeof(double) * h->n));
-            }
-        }
-    }
-    MGB_CUDA(cudaMemcpy(h->env2task, env2task_host, sizeof(int32_t) * h->n, cudaMemcpyHostToDevice));
     h->n_tasks = n_tasks;
     h->has_task = true;
-    cudaFree(h->task_flags); h->task_flags = nullptr; h->task_flags_n = 0;
+    h->task_flags.reset();
     h->cache_would_fit = true;
     // pose list of the cache: every free cell (the agent can never stand inside a wall, maze_discrete_3d.py:63-65) x 4
     h->host_poses.clear();
@@ -2563,26 +2579,9 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
             }
         }
     }
-    cudaFree(h->efftab); h->efftab = nullptr;
-    cudaFree(h->fogtab); h->fogtab = nullptr;
-    c.n_cls = 0;
-    if (c.kind != MGB_MAZE_2D && !cls_heights.empty()) {
-        const int n_cls = (int)(cls_heights.size() / 2);
-        const size_t cells = (size_t)n_cls * c.res_h * c.res_v;
-        double *d_heights = nullptr;
-        MGB_CUDA(cudaMalloc(&h->efftab, cells * sizeof(double)));
-        MGB_CUDA(cudaMalloc(&h->fogtab, cells * sizeof(double)));
-        MGB_CUDA(cudaMalloc(&d_heights, cls_heights.size() * sizeof(double)));
-        MGB_CUDA(cudaMemcpy(d_heights, cls_heights.data(), cls_heights.size() * sizeof(double), cudaMemcpyHostToDevice));
-        maze_efftab_kernel<<<(unsigned)((cells + 255) / 256), 256>>>(c, h->coltab, d_heights, n_cls, h->efftab, h->fogtab);
-        MGB_CUDA(cudaDeviceSynchronize());
-        cudaFree(d_heights);
-        c.n_cls = n_cls;
-        h->launches += 1;
-    }
     // set_task leaves the env in "need reset" state (maze_env.py:44-50): initialise it so a stray step is harmless
     MazeArgs a = maze_args(h);
-    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(c, a, nullptr);
+    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(h->c, a, nullptr);
     MGB_CUDA(cudaDeviceSynchronize());
     h->launches += 1;
     return MGB_OK;
@@ -2828,42 +2827,44 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
         MGB_REQUIRE(s.cell_size >= h->min_cell, "a replacement task may not have smaller cells than the table's smallest");
     }
     // pinned staging, double-buffered: the host waits only for the COPY of the call before last, never for the device
-    const int sb = h->stage_next;
-    h->stage_next ^= 1;
+    MazeStage &s = h->stage[h->stage_next];
     const size_t head = (((size_t)count * 4 + 15) / 16) * 16, need = head + (size_t)count * c.blob_bytes;
-    if (!h->stage_done[sb]) MGB_CUDA(cudaEventCreateWithFlags(&h->stage_done[sb], cudaEventDisableTiming));
-    else MGB_CUDA(cudaEventSynchronize(h->stage_done[sb]));
-    if (need > h->stage_bytes[sb]) {
-        cudaFreeHost(h->h_stage[sb]); cudaFree(h->d_stage[sb]);
-        h->h_stage[sb] = nullptr; h->d_stage[sb] = nullptr; h->stage_bytes[sb] = 0;
+    if (!s.copied) MGB_CUDA(s.copied.create(cudaEventDisableTiming));
+    else MGB_CUDA(cudaEventSynchronize(s.copied.get()));
+    if (need > s.bytes) {
         const size_t cap = need * 2;
-        MGB_CUDA(cudaMallocHost(&h->h_stage[sb], cap));
-        MGB_CUDA(cudaMalloc(&h->d_stage[sb], cap));
-        h->stage_bytes[sb] = cap;
+        MgbPinned<uint8_t> host;
+        MgbDev<uint8_t> dev;
+        MGB_CUDA(host.alloc(cap));
+        MGB_CUDA(dev.alloc(cap));
+        s.host = std::move(host); s.dev = std::move(dev); s.bytes = cap;
     }
     if (!h->task_flags) {
-        MGB_CUDA(cudaMalloc(&h->task_flags, (size_t)h->n_tasks));
-        MGB_CUDA(cudaMemset(h->task_flags, 0, (size_t)h->n_tasks));
-        h->task_flags_n = h->n_tasks;
+        MgbDev<uint8_t> flags;
+        MGB_CUDA(flags.alloc((size_t)h->n_tasks));
+        MGB_CUDA(cudaMemset(flags.get(), 0, (size_t)h->n_tasks));
+        h->task_flags = std::move(flags);
     }
-    uint8_t *hs = h->h_stage[sb];
+    uint8_t *hs = s.host.get();
     memset(hs, 0, need);
     memcpy(hs, task_slots_host, (size_t)count * 4);
     for (int t = 0; t < count; ++t)
         fill_task_blob(c, hs + head + (size_t)t * c.blob_bytes, walls_host + (size_t)t * nn, texts_host + (size_t)t * nn,
                        food_rewards_host + (size_t)t * nn, food_interval_host + (size_t)t * nn, scalars_host[t], h->cls_heights,
                        false);
-    for (int t = 0; t < count; ++t)
-        h->slot_fp[task_slots_host[t]] = mgb_fnv(MGB_FNV_BASIS, hs + head + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
     cudaStream_t st = (cudaStream_t)stream;
-    MGB_CUDA(cudaMemcpyAsync(h->d_stage[sb], hs, need, cudaMemcpyHostToDevice, st));
-    MGB_CUDA(cudaEventRecord(h->stage_done[sb], st));
-    maze_scatter_tasks_kernel<<<(unsigned)count, 128, 0, st>>>(c, h->blobs, h->d_stage[sb], count, h->task_flags);
+    MGB_CUDA(cudaMemcpyAsync(s.dev.get(), hs, need, cudaMemcpyHostToDevice, st));
+    MGB_CUDA(cudaEventRecord(s.copied.get(), st));
+    h->stage_next ^= 1;
+    maze_scatter_tasks_kernel<<<(unsigned)count, 128, 0, st>>>(c, h->tasks.blobs.get(), s.dev.get(), count, h->task_flags.get());
     MazeArgs a = maze_args(h);
-    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(c, a, h->task_flags);
-    maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags, h->n_tasks);
+    maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(c, a, h->task_flags.get());
+    maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags.get(), h->n_tasks);
     MGB_CUDA(cudaGetLastError());
     h->launches += 3;
+    // the slots' fingerprints change once their new blobs are on their way
+    for (int t = 0; t < count; ++t)
+        h->slot_fp[task_slots_host[t]] = mgb_fnv(MGB_FNV_BASIS, hs + head + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
     return MGB_OK;
 }
 
@@ -2871,8 +2872,10 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
 static int ensure_task_epoch(mgb_maze *h)
 {
     if (h->task_epoch) return MGB_OK;
-    MGB_CUDA(cudaMalloc(&h->task_epoch, sizeof(uint32_t) * (size_t)h->n_pad));
-    MGB_CUDA(cudaMemset(h->task_epoch, 0, sizeof(uint32_t) * (size_t)h->n_pad));
+    MgbDev<uint32_t> epoch;
+    MGB_CUDA(epoch.alloc(sizeof(uint32_t) * (size_t)h->n_pad));
+    MGB_CUDA(cudaMemset(epoch.get(), 0, sizeof(uint32_t) * (size_t)h->n_pad));
+    h->task_epoch = std::move(epoch);
     return MGB_OK;
 }
 
@@ -2907,7 +2910,7 @@ extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, con
     int rc = ensure_task_epoch(h);
     if (rc) return rc;
     MazeArgs a = maze_args(h);
-    maze_sample_tasks_kernel<<<(unsigned)((h->n + kSamplerWarps - 1) / kSamplerWarps), 32 * kSamplerWarps, 0, (cudaStream_t)stream>>>(c, a, h->blobs, mask_dev, h->task_epoch,
+    maze_sample_tasks_kernel<<<(unsigned)((h->n + kSamplerWarps - 1) / kSamplerWarps), 32 * kSamplerWarps, 0, (cudaStream_t)stream>>>(c, a, h->tasks.blobs.get(), mask_dev, h->task_epoch.get(),
                                                                                         sc, seed);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
@@ -2928,7 +2931,7 @@ extern "C" int mgb_maze_get_tasks(mgb_maze *h, int32_t count, const int32_t *tas
     std::vector<uint8_t> blob((size_t)c.blob_bytes);
     for (int t = 0; t < count; ++t) {
         MGB_REQUIRE(task_slots_host[t] >= 0 && task_slots_host[t] < h->n_tasks, "task slot out of range");
-        MGB_CUDA(cudaMemcpy(blob.data(), h->blobs + (size_t)task_slots_host[t] * c.blob_bytes, blob.size(), cudaMemcpyDeviceToHost));
+        MGB_CUDA(cudaMemcpy(blob.data(), h->tasks.blobs.get() + (size_t)task_slots_host[t] * c.blob_bytes, blob.size(), cudaMemcpyDeviceToHost));
         TaskHdr hd;
         memcpy(&hd, blob.data(), sizeof(hd));
         const int8_t *fidx = reinterpret_cast<const int8_t *>(blob.data() + c.off_fidx);
@@ -3014,12 +3017,11 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
                 return MGB_ERR_STATE;
             }
             MGB_CUDA(cudaStreamSynchronize(st));
-            cudaFree(h->hit_scratch);
-            h->hit_scratch = nullptr;
-            MGB_CUDA(cudaMalloc(&h->hit_scratch, need));
+            h->hit_scratch_bytes = 0;                   // alloc() frees the smaller scratch first
+            MGB_CUDA(h->hit_scratch.alloc(need));
             h->hit_scratch_bytes = need;
         }
-        a2.hit_scratch = h->hit_scratch;
+        a2.hit_scratch = h->hit_scratch.get();
     }
     // The opt-in limit is a property of the kernel on a device, shared by every handle: each handle raises it once to the
     // device maximum (the same value from every handle and thread, so there is no ordering to get wrong and no global state).
@@ -3067,31 +3069,26 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
         mgb_set_error("maze pose cache must be built before stream capture: call reset() once first");
         return MGB_ERR_STATE;
     }
-    cudaFree(h->poses); cudaFree(h->pose_index); cudaFree(h->c_px); cudaFree(h->c_fid); cudaFree(h->c_colhits);
-    cudaFree(h->c_hits); cudaFree(h->dyn); cudaFree(h->c_rgb8); cudaFree(h->c_gsig);
-    cudaFree(h->c_px_all); cudaFree(h->c_fmask);
-    cudaFree(h->c_vbase); cudaFree(h->c_var8); cudaFree(h->d_bake_desc); cudaFree(h->pose_rec);
-    h->pose_rec = nullptr;
-    h->c_vbase = nullptr; h->c_var8 = nullptr; h->d_bake_desc = nullptr; h->n_var_frames = 0;
-    h->c_px_all = nullptr; h->c_fmask = nullptr;
-    h->poses = nullptr; h->pose_index = nullptr; h->c_px = nullptr; h->c_fid = nullptr; h->c_colhits = nullptr;
-    h->c_hits = nullptr; h->dyn = nullptr; h->c_rgb8 = nullptr; h->c_gsig = nullptr;
-    MGB_CUDA(cudaMalloc(&h->poses, slots * sizeof(int4)));
-    MGB_CUDA(cudaMalloc(&h->pose_index, h->host_pose_index.size() * sizeof(int32_t)));
-    MGB_CUDA(cudaMalloc(&h->c_px, slots * px * sizeof(uint32_t)));
-    MGB_CUDA(cudaMalloc(&h->c_fid, slots * px));
-    MGB_CUDA(cudaMalloc(&h->c_colhits, slots * c.res_h));
-    MGB_CUDA(cudaMalloc(&h->c_hits, slots * c.res_h * c.max_hits * sizeof(HitRec)));
-    MGB_CUDA(cudaMalloc(&h->dyn, (size_t)h->n_pad * sizeof(EnvDyn)));
-    MGB_CUDA(cudaMalloc(&h->c_rgb8, slots * px * 3));
-    MGB_CUDA(cudaMalloc(&h->c_gsig, slots * ((px + 3) / 4)));
-    MGB_CUDA(cudaMemsetAsync(h->c_gsig, 0xFF, slots * ((px + 3) / 4), st));
-    MGB_CUDA(cudaMalloc(&h->c_fmask, slots * 2 * sizeof(uint64_t)));
-    if (c.obs_dtype != MGB_OBS_U8) MGB_CUDA(cudaMalloc(&h->c_px_all, slots * px * sizeof(uint32_t)));
-    MGB_CUDA(cudaMemcpy(h->poses, h->host_poses.data(), slots * sizeof(int4), cudaMemcpyHostToDevice));
-    MGB_CUDA(cudaMemcpy(h->pose_index, h->host_pose_index.data(), h->host_pose_index.size() * sizeof(int32_t),
+    // the old cache goes before the new one (up to the whole budget) is built in `pc`, the handle's once it is complete
+    h->cache = MazePoseCache();
+    MazePoseCache pc;
+    MGB_CUDA(pc.poses.alloc(slots * sizeof(int4)));
+    MGB_CUDA(pc.pose_index.alloc(h->host_pose_index.size() * sizeof(int32_t)));
+    MGB_CUDA(pc.c_px.alloc(slots * px * sizeof(uint32_t)));
+    MGB_CUDA(pc.c_fid.alloc(slots * px));
+    MGB_CUDA(pc.c_colhits.alloc(slots * c.res_h));
+    MGB_CUDA(pc.c_hits.alloc(slots * c.res_h * c.max_hits * sizeof(HitRec)));
+    MGB_CUDA(pc.dyn.alloc((size_t)h->n_pad * sizeof(EnvDyn)));
+    MGB_CUDA(pc.c_rgb8.alloc(slots * px * 3));
+    MGB_CUDA(pc.c_gsig.alloc(slots * ((px + 3) / 4)));
+    MGB_CUDA(cudaMemsetAsync(pc.c_gsig.get(), 0xFF, slots * ((px + 3) / 4), st));
+    MGB_CUDA(pc.c_fmask.alloc(slots * 2 * sizeof(uint64_t)));
+    if (c.obs_dtype != MGB_OBS_U8) MGB_CUDA(pc.c_px_all.alloc(slots * px * sizeof(uint32_t)));
+    MGB_CUDA(cudaMemcpy(pc.poses.get(), h->host_poses.data(), slots * sizeof(int4), cudaMemcpyHostToDevice));
+    MGB_CUDA(cudaMemcpy(pc.pose_index.get(), h->host_pose_index.data(), h->host_pose_index.size() * sizeof(int32_t),
                         cudaMemcpyHostToDevice));
     MazeArgs a = maze_args(h);
+    bind_pose_cache(pc, a);
     a.n = (int64_t)slots;
     a.do_step = 0;
     int rc = launch_render<true>(h, a, (unsigned)(slots < (size_t)h->num_sms ? slots : (size_t)h->num_sms), st);
@@ -3099,19 +3096,18 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     // "all present" frames: which foods can change a pose's image at all, and the finished pixels with all of them
     // present (the compose kernel itself, fed one synthetic env per pose slot).  Screens the 4-pixel-group path cannot
     // take keep an all-ones mask, i.e. never use the baked frame.
-    a.c_px_all = h->c_px_all; a.c_fmask = h->c_fmask;
+    std::vector<BakeDesc> descs;
     if ((c.res_v & 3) == 0 && (px & 127) == 0) {
-        MGB_CUDA(cudaMemsetAsync(h->c_fmask, 0, slots * 2 * sizeof(uint64_t), st));
+        MGB_CUDA(cudaMemsetAsync(pc.c_fmask.get(), 0, slots * 2 * sizeof(uint64_t), st));
         maze3d_sig_kernel<<<(unsigned)slots, 256, 0, st>>>(c, a);
         MGB_CUDA(cudaGetLastError());
-        if (h->c_px_all) MGB_CUDA(cudaMemcpyAsync(h->c_px_all, h->c_px, slots * px * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+        if (pc.c_px_all) MGB_CUDA(cudaMemcpyAsync(pc.c_px_all.get(), pc.c_px.get(), slots * px * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
         // ---- variant frames: every pose whose image depends on k <= variant_bits foods gets its other 2^k - 1 finished
         // frames too (the all-visible one is c_rgb8[slot]); bits = the pose's foods in ascending slot order
-        std::vector<BakeDesc> descs;
         if (h->variant_bits > 0 && c.obs_dtype == MGB_OBS_U8 && c.task_type == MGB_MAZE_SURVIVAL && (px * 3) % 16 == 0) {
             std::vector<uint64_t> fm(slots * 2);
             MGB_CUDA(cudaStreamSynchronize(st));
-            MGB_CUDA(cudaMemcpy(fm.data(), h->c_fmask, slots * 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+            MGB_CUDA(cudaMemcpy(fm.data(), pc.c_fmask.get(), slots * 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
             auto popc = [](uint64_t x) { int n = 0; while (x) { x &= x - 1; ++n; } return n; };
             for (int k = 0; k < 9; ++k) h->k_hist[k] = 0;
             for (size_t sl = 0; sl < slots; ++sl) {
@@ -3154,14 +3150,13 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
                         descs.push_back(bd);
                     }
                 }
-                MGB_CUDA(cudaMalloc(&h->c_vbase, slots * sizeof(int32_t)));
-                MGB_CUDA(cudaMalloc(&h->c_var8, descs.size() * px * 3));
-                MGB_CUDA(cudaMalloc(&h->d_bake_desc, descs.size() * sizeof(BakeDesc)));
-                MGB_CUDA(cudaMemcpy(h->c_vbase, vbase.data(), slots * sizeof(int32_t), cudaMemcpyHostToDevice));
-                MGB_CUDA(cudaMemcpy(h->d_bake_desc, descs.data(), descs.size() * sizeof(BakeDesc), cudaMemcpyHostToDevice));
-                h->n_var_frames = (int64_t)descs.size();
+                MGB_CUDA(pc.c_vbase.alloc(slots * sizeof(int32_t)));
+                MGB_CUDA(pc.c_var8.alloc(descs.size() * px * 3));
+                MGB_CUDA(pc.bake_desc.alloc(descs.size() * sizeof(BakeDesc)));
+                MGB_CUDA(cudaMemcpy(pc.c_vbase.get(), vbase.data(), slots * sizeof(int32_t), cudaMemcpyHostToDevice));
+                MGB_CUDA(cudaMemcpy(pc.bake_desc.get(), descs.data(), descs.size() * sizeof(BakeDesc), cudaMemcpyHostToDevice));
                 MazeArgs av = a;
-                av.c_var8 = h->c_var8; av.bake_desc = h->d_bake_desc;
+                av.c_var8 = pc.c_var8.get(); av.bake_desc = pc.bake_desc.get();
                 maze3d_varinit_kernel<<<(unsigned)descs.size(), 256, 0, st>>>(c, av);      // static colours first ...
                 MGB_CUDA(cudaGetLastError());
             }
@@ -3173,7 +3168,7 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
         if (!descs.empty()) {                               // ... then each variant's tints (compose kernel, bake mode)
             MazeArgs av = a;
             av.n = (int64_t)descs.size();
-            av.c_rgb8 = h->c_var8; av.bake_desc = h->d_bake_desc;
+            av.c_rgb8 = pc.c_var8.get(); av.bake_desc = pc.bake_desc.get();
             maze3d_compose_kernel<<<(unsigned)descs.size(), kComposeThreads, 0, st>>>(c, av);
             MGB_CUDA(cudaGetLastError());
             h->launches += 2;
@@ -3181,17 +3176,19 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
         a.bake = 0;
         h->launches += 2;
     } else {
-        MGB_CUDA(cudaMemsetAsync(h->c_fmask, 0xFF, slots * 2 * sizeof(uint64_t), st));
+        MGB_CUDA(cudaMemsetAsync(pc.c_fmask.get(), 0xFF, slots * 2 * sizeof(uint64_t), st));
     }
     {   // merged per-pose records for the step logic (after c_fmask and c_vbase are final)
         const int64_t count = (int64_t)h->host_pose_index.size();
-        MGB_CUDA(cudaMalloc(&h->pose_rec, (size_t)count * sizeof(PoseRec)));
-        maze_pose_rec_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(h->pose_index, h->c_fmask, h->c_vbase,
-                                                                            reinterpret_cast<PoseRec *>(h->pose_rec), count);
+        MGB_CUDA(pc.pose_rec.alloc((size_t)count * sizeof(PoseRec)));
+        maze_pose_rec_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(pc.pose_index.get(), pc.c_fmask.get(),
+                                                                            pc.c_vbase.get(), pc.pose_rec.get(), count);
         MGB_CUDA(cudaGetLastError());
     }
     MGB_CUDA(cudaStreamSynchronize(st));
+    h->cache = std::move(pc);
     h->n_poses = (int64_t)slots;
+    h->n_var_frames = (int64_t)descs.size();
     h->cache_bytes = bytes + (double)h->n_var_frames * (double)(px * 3);
     h->cache_ready = true;
     h->cache_dirty = false;
@@ -3242,7 +3239,7 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t s
         if (rc) return rc;
         if (h->cache_ready) {
             // memoised path: integer step logic, then compose static pose layers with the current food state
-            bind_pose_cache(h, a);
+            bind_pose_cache(h->cache, a);
             // uint8 frames whose columns are whole 16-pixel runs: ONE fused launch (logic + TMA-moved frame)
             const size_t frame_bytes = (size_t)c.res_h * c.res_v * 3;
             if (h->fused_step && c.obs_dtype == MGB_OBS_U8 && (c.res_v & 15) == 0 && ((size_t)c.res_h * c.res_v) % 128 == 0 &&
@@ -3302,10 +3299,11 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     MGB_REQUIRE(!final_obs || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
     a.truncated = truncated;
     a.final_obs = final_obs;
+    const MazeFinal &fin = h->tasks.fin;
     if (final_obs && h->c.kind != MGB_MAZE_2D) {
-        a.fin_count = h->fin_count; a.fin_env = h->fin_env; a.fin_dyn = h->fin_dyn;
-        a.fin_agent = h->fin_agent; a.fin_life = h->fin_life; a.fin_eaten = h->fin_eaten; a.fin_task = h->fin_task;
-        a.fin_cpos = h->fin_cpos; a.fin_cori = h->fin_cori;
+        a.fin_count = fin.count.get(); a.fin_env = fin.env.get(); a.fin_dyn = fin.dyn.get();
+        a.fin_agent = fin.agent.get(); a.fin_life = fin.life.get(); a.fin_eaten = fin.eaten.get(); a.fin_task = fin.task.get();
+        a.fin_cpos = fin.cpos.get(); a.fin_cori = fin.cori.get();
     }
     bool listed;
     int rc = launch_observe(h, a, listed, st);
@@ -3313,16 +3311,16 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     MazeArgs l = maze_args(h);
     l.obs = final_obs; l.final_obs = final_obs; l.do_step = 0;
     l.path = nullptr;                                           // the list holds terminal copies, not env state
-    l.fin_count = h->fin_count; l.fin_env = h->fin_env;
+    l.fin_count = fin.count.get(); l.fin_env = fin.env.get();
     if (h->cache_ready) {
-        l.dyn = h->fin_dyn;
+        l.dyn = fin.dyn.get();
         l.do_parts = 16;     // a few frames per step: slices spread each over many CTAs, so the pass costs a slice, not a frame
         const int64_t resident = compose_resident_ctas(h);
         maze3d_compose_kernel<<<(unsigned)(h->n < resident ? h->n : resident), kComposeThreads, 0, st>>>(h->c, l);
         MGB_CUDA(cudaGetLastError());
     } else {
-        l.agent = h->fin_agent; l.life = h->fin_life; l.eaten = h->fin_eaten; l.env2task = h->fin_task;
-        l.cpos = h->fin_cpos; l.cori = h->fin_cori;
+        l.agent = fin.agent.get(); l.life = fin.life.get(); l.eaten = fin.eaten.get(); l.env2task = fin.task.get();
+        l.cpos = fin.cpos.get(); l.cori = fin.cori.get();
         rc = launch_render<false>(h, l, (unsigned)(h->n < h->num_sms ? h->n : h->num_sms), st);
         if (rc) return rc;
     }
@@ -3433,7 +3431,7 @@ static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_
         rc = ensure_pose_cache(h, st);
         if (rc) return rc;
         MGB_REQUIRE(h->cache_ready, "the fused 3-D rollout runs on the pose cache (MGB_MAZE_CACHE=0 or cache budget too small)");
-        bind_pose_cache(h, a);
+        bind_pose_cache(h->cache, a);
         const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers
         const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
         MGB_REQUIRE(qbytes <= 200 * 1024, "screen too large for the fused rollout's group queue");
@@ -4226,10 +4224,10 @@ static int record_paths(mgb_maze *h, bool load, const uint8_t *rec_dev, int64_t 
     const int64_t grid = (total + 255) / 256 < most ? (total + 255) / 256 : most;
     uint8_t *rec = const_cast<uint8_t *>(rec_dev);
     if (load)
-        maze_record_path_kernel<true><<<(unsigned)grid, 256, 0, st>>>(h->n, h->n_pad, path_cap(h), h->path, rec,
+        maze_record_path_kernel<true><<<(unsigned)grid, 256, 0, st>>>(h->n, h->n_pad, path_cap(h), h->path.get(), rec,
                                                                      record_bytes(h), record_path_off(h), n_rec, row);
     else
-        maze_record_path_kernel<false><<<(unsigned)grid, 256, 0, st>>>(h->n, h->n_pad, path_cap(h), h->path, rec,
+        maze_record_path_kernel<false><<<(unsigned)grid, 256, 0, st>>>(h->n, h->n_pad, path_cap(h), h->path.get(), rec,
                                                                       record_bytes(h), record_path_off(h), 0, nullptr);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
@@ -4253,13 +4251,13 @@ extern "C" int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream)
     cudaStream_t st = (cudaStream_t)stream;
     const MazeArgs a = maze_args(h);
     const int64_t rb = record_bytes(h);
-    maze_snapshot_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch, rec_dev, rb);
+    maze_snapshot_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch.get(), rec_dev, rb);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     if (records_carry_tasks(h)) {
         const int64_t total = h->n * (h->c.blob_bytes / 16), cap = (int64_t)h->num_sms * 16;
         const int64_t grid = (total + 255) / 256 < cap ? (total + 255) / 256 : cap;
-        maze_record_tasks_kernel<false><<<(unsigned)grid, 256, 0, st>>>(h->n, h->c.blob_bytes, h->env2task, h->blobs, rec_dev,
+        maze_record_tasks_kernel<false><<<(unsigned)grid, 256, 0, st>>>(h->n, h->c.blob_bytes, h->env2task.get(), h->tasks.blobs.get(), rec_dev,
                                                                        rb, record_tail(h), 0, nullptr);
         MGB_CUDA(cudaGetLastError());
         h->launches += 1;
@@ -4285,15 +4283,15 @@ extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_r
     const bool carry = records_carry_tasks(h);
     const int64_t rb = record_bytes(h);
     const MazeArgs a = maze_args(h);
-    maze_restore_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch,
-                                                                        carry ? nullptr : h->env2task, h->n_tasks, rec_dev,
+    maze_restore_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch.get(),
+                                                                        carry ? nullptr : h->env2task.get(), h->n_tasks, rec_dev,
                                                                         rb, n_rec, row_of_env_dev);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     if (carry) {
         const int64_t total = h->n * (h->c.blob_bytes / 16), cap = (int64_t)h->num_sms * 16;
         const int64_t grid = (total + 255) / 256 < cap ? (total + 255) / 256 : cap;
-        maze_record_tasks_kernel<true><<<(unsigned)grid, 256, 0, st>>>(h->n, h->c.blob_bytes, h->env2task, h->blobs,
+        maze_record_tasks_kernel<true><<<(unsigned)grid, 256, 0, st>>>(h->n, h->c.blob_bytes, h->env2task.get(), h->tasks.blobs.get(),
                                                                       const_cast<uint8_t *>(rec_dev), rb, record_tail(h),
                                                                       n_rec, row_of_env_dev);
         MGB_CUDA(cudaGetLastError());

@@ -59,6 +59,87 @@ struct MgbDeviceGuard {
     int want = -1;
 };
 
+// Owner of one buffer from Mem::alloc (device memory: MgbDev, pinned host memory: MgbPinned).  Handles keep every buffer
+// in one of these, so an error exit, a replaced buffer or a destroyed handle frees it exactly once.  A buffer is freed
+// when it is reset, assigned over or destroyed, which must happen with the buffer's device current: the entry points'
+// MgbDeviceGuard.
+struct MgbDeviceMem {
+    static cudaError_t alloc(void **p, size_t bytes) { return cudaMalloc(p, bytes); }
+    static void free(void *p) { cudaFree(p); }
+};
+struct MgbPinnedMem {
+    static cudaError_t alloc(void **p, size_t bytes) { return cudaMallocHost(p, bytes); }
+    static void free(void *p) { cudaFreeHost(p); }
+};
+template <typename T, class Mem> class MgbBuf {
+  public:
+    MgbBuf() = default;
+    MgbBuf(const MgbBuf &) = delete;
+    MgbBuf &operator=(const MgbBuf &) = delete;
+    MgbBuf(MgbBuf &&o) noexcept : p_(o.release()) {}
+    MgbBuf &operator=(MgbBuf &&o) noexcept
+    {
+        if (this != &o) {
+            reset();
+            p_ = o.release();
+        }
+        return *this;
+    }
+    ~MgbBuf() { reset(); }
+
+    T *get() const { return p_; }
+    explicit operator bool() const { return p_ != nullptr; }
+    // frees the buffer held, then allocates `bytes`; on an error the owner holds nothing
+    cudaError_t alloc(size_t bytes)
+    {
+        reset();
+        void *p = nullptr;
+        const cudaError_t e = Mem::alloc(&p, bytes);
+        if (e == cudaSuccess) p_ = static_cast<T *>(p);
+        return e;
+    }
+    void reset()
+    {
+        if (p_) Mem::free(p_);
+        p_ = nullptr;
+    }
+    T *release()
+    {
+        T *p = p_;
+        p_ = nullptr;
+        return p;
+    }
+
+  private:
+    T *p_ = nullptr;
+};
+template <typename T> using MgbDev = MgbBuf<T, MgbDeviceMem>;
+template <typename T> using MgbPinned = MgbBuf<T, MgbPinnedMem>;
+
+// Owner of one cudaEvent_t, destroyed like an MgbBuf is freed
+class MgbEvent {
+  public:
+    MgbEvent() = default;
+    MgbEvent(const MgbEvent &) = delete;
+    MgbEvent &operator=(const MgbEvent &) = delete;
+    ~MgbEvent()
+    {
+        if (e_) cudaEventDestroy(e_);
+    }
+
+    cudaEvent_t get() const { return e_; }
+    explicit operator bool() const { return e_ != nullptr; }
+    cudaError_t create(unsigned flags)
+    {
+        if (e_) cudaEventDestroy(e_);
+        e_ = nullptr;
+        return cudaEventCreateWithFlags(&e_, flags);
+    }
+
+  private:
+    cudaEvent_t e_ = nullptr;
+};
+
 // ---------------------------------------------------------------------------------------------------------------
 // Philox4x32-10 (Salmon et al., SC'11): counter-based, so every env owns a stream keyed by its GLOBAL index and the
 // results do not depend on how envs are sharded over GPUs or blocks.

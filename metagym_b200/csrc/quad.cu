@@ -21,8 +21,10 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <memory>
 #include <new>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "mgb_common.cuh"
@@ -1367,16 +1369,26 @@ __global__ void quad_targets_layout_kernel(const float *__restrict__ src, int nt
 // ---------------------------------------------------------------------------------------------------------------
 // handle + C ABI
 // ---------------------------------------------------------------------------------------------------------------
+// host staging of the *_host entry points: device buffers d_*, pinned host buffers h_*
+struct QuadStaging {
+    MgbDev<float> d_act, d_obs, d_rew, d_final;
+    MgbDev<uint8_t> d_done, d_trunc;
+    MgbDev<int32_t> d_fail;
+    MgbPinned<float> h_act, h_obs, h_rew, h_final;
+    MgbPinned<uint8_t> h_done, h_trunc;
+    MgbPinned<int32_t> h_fail;
+};
+
 struct mgb_quad {
     int device = 0;
     int64_t n = 0, n_pad = 0, env_base = 0;
     mgb_quad_cfg cfg;
     QuadConst c;
-    float4 *planes = nullptr;
-    int32_t *sat = nullptr;
+    MgbDev<float4> planes;
+    MgbDev<int32_t> sat;
     int map_rows = 0, map_cols = 0, x_off = 0, y_off = 0;
-    float4 *targets = nullptr;  // [nt][n_tasks] (x, y, z, 0), built by mgb_quad_set_targets
-    int32_t *env2task = nullptr;
+    MgbDev<float4> targets;     // [nt][n_tasks] (x, y, z, 0), built by mgb_quad_set_targets
+    MgbDev<int32_t> env2task;
     int n_tasks = 0;
     int auto_reset = 0;
     int num_sms = 132;
@@ -1391,27 +1403,21 @@ struct mgb_quad {
     uint64_t fp_map = 0, fp_targets = 0;   // fingerprints of the map (0: flat) and the target table (mgb_quad_fingerprint)
     MgbMirrors mir = {};       // mgb_quad_set_mirrors
     MgbMirrorWindow mir_win;   // mgb_quad_set_mirror_window
-    // host staging for *_host entry points
-    float *h_act = nullptr, *h_obs = nullptr, *h_rew = nullptr, *h_final = nullptr;
-    uint8_t *h_done = nullptr, *h_trunc = nullptr;
-    int32_t *h_fail = nullptr;
-    float *d_act = nullptr, *d_obs = nullptr, *d_rew = nullptr, *d_final = nullptr;
-    uint8_t *d_done = nullptr, *d_trunc = nullptr;
-    int32_t *d_fail = nullptr;
+    QuadStaging stage;         // allocated by the first *_host call
 };
 
 static QuadArgs base_args(const mgb_quad *h)
 {
     QuadArgs a;
     memset(&a, 0, sizeof(a));
-    a.planes = h->planes;
+    a.planes = h->planes.get();
     a.n_pad = h->n_pad;
     a.n = h->n;
     a.env_base = h->env_base;
-    a.targets = h->targets;
+    a.targets = h->targets.get();
     a.n_tasks = h->n_tasks;
-    a.sat = h->sat; a.map_rows = h->map_rows; a.map_cols = h->map_cols; a.x_off = h->x_off; a.y_off = h->y_off;
-    a.env2task = h->env2task;
+    a.sat = h->sat.get(); a.map_rows = h->map_rows; a.map_cols = h->map_cols; a.x_off = h->x_off; a.y_off = h->y_off;
+    a.env2task = h->env2task.get();
     a.seed = h->seed;
     a.auto_reset = h->auto_reset;
     return a;
@@ -1485,7 +1491,7 @@ extern "C" int mgb_quad_create(mgb_quad **out, int64_t n_envs, const mgb_quad_cf
     MGB_CUDA(cudaGetDeviceCount(&ndev));
     MGB_REQUIRE(device >= 0 && device < ndev, "device index out of range");
     MgbDeviceGuard guard(device);
-    mgb_quad *h = new (std::nothrow) mgb_quad();
+    std::unique_ptr<mgb_quad> h(new (std::nothrow) mgb_quad());    // deleted with its buffers on every error exit
     MGB_REQUIRE(h, "out of host memory");
     h->device = device;
     h->n = n_envs;
@@ -1507,33 +1513,20 @@ extern "C" int mgb_quad_create(mgb_quad **out, int64_t n_envs, const mgb_quad_cf
         // function and device, idempotent, and set to the maximum so that handles never lower each other's limit (round-1
         // advice: the process-global high-water mark it replaces was not thread-safe), for the kernels this handle launches
         const int max_smem = 512 * kMaxObs * 4 * 2;
-        with_simple(h, [&](auto simple) {
+        with_simple(h.get(), [&](auto simple) {
             cudaFuncSetAttribute(quad_step_wide_kernel<simple>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
             cudaFuncSetAttribute(quad_step2_kernel<simple>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
         });
         if (cudaGetLastError() != cudaSuccess) {
             mgb_set_error("cudaFuncSetAttribute(quad_step_wide_kernel, %d bytes of shared memory) failed", max_smem);
-            delete h;
             return MGB_ERR_CUDA;
         }
     }
-    cudaError_t e = cudaMalloc(&h->planes, sizeof(float4) * 6 * h->n_pad);
-    if (e != cudaSuccess) {
-        mgb_set_error("cudaMalloc(state planes, %lld envs) -> %s", (long long)n_envs, cudaGetErrorString(e));
-        delete h;
-        return MGB_ERR_CUDA;
-    }
-    QuadArgs a = base_args(h);
-    quad_init_kernel<<<(unsigned)((h->n_pad + 255) / 256), 256>>>(a);
-    e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-        mgb_set_error("state init -> %s", cudaGetErrorString(e));
-        cudaFree(h->planes);
-        delete h;
-        return MGB_ERR_CUDA;
-    }
+    MGB_CUDA(h->planes.alloc(sizeof(float4) * 6 * h->n_pad));        // the state planes
+    quad_init_kernel<<<(unsigned)((h->n_pad + 255) / 256), 256>>>(base_args(h.get()));
+    MGB_CUDA(cudaDeviceSynchronize());
     h->launches += 1;
-    *out = h;
+    *out = h.release();
     return MGB_OK;
 }
 
@@ -1542,15 +1535,7 @@ extern "C" void mgb_quad_destroy(mgb_quad *h)
     if (!h) return;
     MgbDeviceGuard guard(h->device);
     cudaDeviceSynchronize();
-    cudaFree(h->planes);
-    cudaFree(h->sat);
-    cudaFree(h->targets);
-    cudaFree(h->env2task);
-    cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_done);
-    cudaFree(h->d_fail); cudaFree(h->d_final); cudaFree(h->d_trunc);
-    cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_done);
-    cudaFreeHost(h->h_fail); cudaFreeHost(h->h_final); cudaFreeHost(h->h_trunc);
-    delete h;
+    delete h;                  // the members free the handle's buffers while its device is current
 }
 
 extern "C" int mgb_quad_obs_dim(const mgb_quad *h) { return h ? h->c.obs_dim : MGB_ERR_ARG; }
@@ -1570,11 +1555,12 @@ extern "C" int mgb_quad_set_map(mgb_quad *h, const int32_t *map_host, int32_t ro
     MGB_REQUIRE(h, "null handle");
     MgbDeviceGuard guard(h->device);
     MGB_CUDA(cudaDeviceSynchronize());
-    cudaFree(h->sat);
-    h->sat = nullptr;
-    h->map_rows = h->map_cols = h->x_off = h->y_off = 0;
-    h->fp_map = 0;
-    if (!map_host) return MGB_OK;                               // flat default map, env.py:295-298
+    if (!map_host) {                                            // flat default map, env.py:295-298
+        h->sat.reset();
+        h->map_rows = h->map_cols = h->x_off = h->y_off = 0;
+        h->fp_map = 0;
+        return MGB_OK;
+    }
     MGB_REQUIRE(h->c.task != MGB_TASK_VELOCITY_CONTROL, "velocity_control has no map (env.py:101-104)");
     MGB_REQUIRE(rows > 0 && cols > 0 && rows <= 8192 && cols <= 8192, "map size out of range");
     int starts = 0, sr = 0, sc = 0;
@@ -1589,8 +1575,10 @@ extern "C" int mgb_quad_set_map(mgb_quad *h, const int32_t *map_host, int32_t ro
             sat[(size_t)(r + 1) * (cols + 1) + q + 1] = (v != 0 ? 1 : 0) + sat[(size_t)r * (cols + 1) + q + 1] +
                                                         sat[(size_t)(r + 1) * (cols + 1) + q] - sat[(size_t)r * (cols + 1) + q];
         }
-    MGB_CUDA(cudaMalloc(&h->sat, sat.size() * sizeof(int32_t)));
-    MGB_CUDA(cudaMemcpy(h->sat, sat.data(), sat.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    MgbDev<int32_t> d_sat;
+    MGB_CUDA(d_sat.alloc(sat.size() * sizeof(int32_t)));
+    MGB_CUDA(cudaMemcpy(d_sat.get(), sat.data(), sat.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    h->sat = std::move(d_sat);
     h->map_rows = rows; h->map_cols = cols; h->x_off = sc; h->y_off = sr;
     h->fp_map = mgb_fnv(mgb_fnv(mgb_fnv(MGB_FNV_BASIS, &rows, sizeof(rows)), &cols, sizeof(cols)), map_host,
                         (size_t)rows * cols * sizeof(int32_t));
@@ -1603,22 +1591,22 @@ extern "C" int mgb_quad_set_targets(mgb_quad *h, const float *tbl_dev, int32_t n
     MGB_REQUIRE(n_tasks > 0, "n_tasks must be positive");
     MgbDeviceGuard guard(h->device);
     MGB_CUDA(cudaDeviceSynchronize());
-    cudaFree(h->targets); h->targets = nullptr;
-    cudaFree(h->env2task); h->env2task = nullptr;
-    h->n_tasks = 0;
     // the kernels read the table time-major with 16-byte rows (prefetch_targets): 16 instead of 12 bytes per row
     const int64_t rows = (int64_t)h->c.nt * n_tasks;
-    MGB_CUDA(cudaMalloc(&h->targets, sizeof(float4) * (size_t)rows));
-    MGB_CUDA(cudaMalloc(&h->env2task, sizeof(int32_t) * h->n));
-    quad_targets_layout_kernel<<<(unsigned)((rows + 255) / 256), 256>>>(tbl_dev, h->c.nt, n_tasks, h->targets);
+    MgbDev<float4> targets;
+    MgbDev<int32_t> env2task;
+    MGB_CUDA(targets.alloc(sizeof(float4) * (size_t)rows));
+    MGB_CUDA(env2task.alloc(sizeof(int32_t) * h->n));
+    quad_targets_layout_kernel<<<(unsigned)((rows + 255) / 256), 256>>>(tbl_dev, h->c.nt, n_tasks, targets.get());
     MGB_CUDA(cudaGetLastError());
-    MGB_CUDA(cudaMemcpy(h->env2task, env2task_dev, sizeof(int32_t) * h->n, cudaMemcpyDeviceToDevice));
+    MGB_CUDA(cudaMemcpy(env2task.get(), env2task_dev, sizeof(int32_t) * h->n, cudaMemcpyDeviceToDevice));
     // a device-to-device cudaMemcpy may return before the copy is done, and a step launched next on a non-blocking
     // stream would not be ordered after it (nor after the layout kernel)
     MGB_CUDA(cudaDeviceSynchronize());
-    h->n_tasks = n_tasks;
     std::vector<float4> tbl((size_t)rows);
-    MGB_CUDA(cudaMemcpy(tbl.data(), h->targets, tbl.size() * sizeof(float4), cudaMemcpyDeviceToHost));
+    MGB_CUDA(cudaMemcpy(tbl.data(), targets.get(), tbl.size() * sizeof(float4), cudaMemcpyDeviceToHost));
+    h->targets = std::move(targets); h->env2task = std::move(env2task);
+    h->n_tasks = n_tasks;
     h->fp_targets = mgb_fnv(mgb_fnv(MGB_FNV_BASIS, &n_tasks, sizeof(n_tasks)), tbl.data(), tbl.size() * sizeof(float4));
     return MGB_OK;
 }
@@ -1840,24 +1828,26 @@ extern "C" int mgb_quad_set_multicast(mgb_quad *h, int64_t byte_delta)
 
 static int ensure_host_staging(mgb_quad *h)
 {
-    if (h->d_act) return MGB_OK;
+    if (h->stage.d_act) return MGB_OK;
     const size_t n = (size_t)h->n, D = (size_t)h->c.obs_dim;
-    MGB_CUDA(cudaMalloc(&h->d_act, n * 16));
-    MGB_CUDA(cudaMalloc(&h->d_obs, n * D * 4));
-    MGB_CUDA(cudaMalloc(&h->d_rew, n * 4));
-    MGB_CUDA(cudaMalloc(&h->d_done, n));
-    MGB_CUDA(cudaMalloc(&h->d_fail, n * 4));
-    MGB_CUDA(cudaMalloc(&h->d_final, n * D * 4));
-    MGB_CUDA(cudaMalloc(&h->d_trunc, n));
-    MGB_CUDA(cudaMallocHost(&h->h_trunc, n));
-    MGB_CUDA(cudaMemset(h->d_fail, 0, n * 4));
-    MGB_CUDA(cudaMemset(h->d_final, 0, n * D * 4));     // rows keep the last terminal observation seen, like final_obs_dev
-    MGB_CUDA(cudaMallocHost(&h->h_act, n * 16));
-    MGB_CUDA(cudaMallocHost(&h->h_obs, n * D * 4));
-    MGB_CUDA(cudaMallocHost(&h->h_rew, n * 4));
-    MGB_CUDA(cudaMallocHost(&h->h_done, n));
-    MGB_CUDA(cudaMallocHost(&h->h_fail, n * 4));
-    MGB_CUDA(cudaMallocHost(&h->h_final, n * D * 4));
+    QuadStaging s;
+    MGB_CUDA(s.d_act.alloc(n * 16));
+    MGB_CUDA(s.d_obs.alloc(n * D * 4));
+    MGB_CUDA(s.d_rew.alloc(n * 4));
+    MGB_CUDA(s.d_done.alloc(n));
+    MGB_CUDA(s.d_fail.alloc(n * 4));
+    MGB_CUDA(s.d_final.alloc(n * D * 4));
+    MGB_CUDA(s.d_trunc.alloc(n));
+    MGB_CUDA(s.h_trunc.alloc(n));
+    MGB_CUDA(cudaMemset(s.d_fail.get(), 0, n * 4));
+    MGB_CUDA(cudaMemset(s.d_final.get(), 0, n * D * 4));   // rows keep the last terminal observation seen, like final_obs_dev
+    MGB_CUDA(s.h_act.alloc(n * 16));
+    MGB_CUDA(s.h_obs.alloc(n * D * 4));
+    MGB_CUDA(s.h_rew.alloc(n * 4));
+    MGB_CUDA(s.h_done.alloc(n));
+    MGB_CUDA(s.h_fail.alloc(n * 4));
+    MGB_CUDA(s.h_final.alloc(n * D * 4));
+    h->stage = std::move(s);
     return MGB_OK;
 }
 
@@ -1880,6 +1870,7 @@ static int step_host(mgb_quad *h, const float *act_host, float *obs_host, float 
     rc = ensure_host_staging(h);
     if (rc) return rc;
     const size_t n = (size_t)h->n, D = (size_t)h->c.obs_dim;
+    const QuadStaging &s = h->stage;
     // Everything is enqueued on the CALLER's stream, so the step is ordered after whatever the caller enqueued before
     // (reset, rollout, load_state ...) exactly like mgb_quad_step; the call then waits for that stream.
     cudaStream_t st = (cudaStream_t)stream;
@@ -1898,8 +1889,8 @@ static int step_host(mgb_quad *h, const float *act_host, float *obs_host, float 
         a.fail = (int32_t *)df; a.final_obs = (float *)dfo; a.truncated = (uint8_t *)dtr;
         if (h->zerocopy == 2) {
             // hybrid: actions by DMA (copy engine), outputs written to host memory by the kernel
-            MGB_CUDA(cudaMemcpyAsync(h->d_act, act_host, n * 16, cudaMemcpyHostToDevice, st));
-            a.act = h->d_act;
+            MGB_CUDA(cudaMemcpyAsync(s.d_act.get(), act_host, n * 16, cudaMemcpyHostToDevice, st));
+            a.act = s.d_act.get();
         }
         rc = launch_step(h, a, st);
         if (rc) return rc;
@@ -1910,34 +1901,34 @@ static int step_host(mgb_quad *h, const float *act_host, float *obs_host, float 
     const bool pin_in = da != nullptr;
     const bool pin_out = dob && dr && dd && opt_ok;
     const float *src = act_host;
-    if (!pin_in) { memcpy(h->h_act, act_host, n * 16); src = h->h_act; }
-    MGB_CUDA(cudaMemcpyAsync(h->d_act, src, n * 16, cudaMemcpyHostToDevice, st));
+    if (!pin_in) { memcpy(s.h_act.get(), act_host, n * 16); src = s.h_act.get(); }
+    MGB_CUDA(cudaMemcpyAsync(s.d_act.get(), src, n * 16, cudaMemcpyHostToDevice, st));
     QuadArgs a = base_args(h);
-    a.act = h->d_act; a.obs = h->d_obs; a.rew = h->d_rew; a.done = h->d_done;
-    a.fail = fail_host ? h->d_fail : nullptr;
-    a.final_obs = final_obs_host ? h->d_final : nullptr;
-    a.truncated = truncated_host ? h->d_trunc : nullptr;
+    a.act = s.d_act.get(); a.obs = s.d_obs.get(); a.rew = s.d_rew.get(); a.done = s.d_done.get();
+    a.fail = fail_host ? s.d_fail.get() : nullptr;
+    a.final_obs = final_obs_host ? s.d_final.get() : nullptr;
+    a.truncated = truncated_host ? s.d_trunc.get() : nullptr;
     rc = launch_step(h, a, st);
     if (rc) return rc;
-    float *o = pin_out ? obs_host : h->h_obs;
-    float *r = pin_out ? rew_host : h->h_rew;
-    uint8_t *d = pin_out ? done_host : h->h_done;
-    MGB_CUDA(cudaMemcpyAsync(o, h->d_obs, n * D * 4, cudaMemcpyDeviceToHost, st));
-    MGB_CUDA(cudaMemcpyAsync(r, h->d_rew, n * 4, cudaMemcpyDeviceToHost, st));
-    MGB_CUDA(cudaMemcpyAsync(d, h->d_done, n, cudaMemcpyDeviceToHost, st));
-    if (fail_host) MGB_CUDA(cudaMemcpyAsync(pin_out ? fail_host : h->h_fail, h->d_fail, n * 4, cudaMemcpyDeviceToHost, st));
+    float *o = pin_out ? obs_host : s.h_obs.get();
+    float *r = pin_out ? rew_host : s.h_rew.get();
+    uint8_t *d = pin_out ? done_host : s.h_done.get();
+    MGB_CUDA(cudaMemcpyAsync(o, s.d_obs.get(), n * D * 4, cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaMemcpyAsync(r, s.d_rew.get(), n * 4, cudaMemcpyDeviceToHost, st));
+    MGB_CUDA(cudaMemcpyAsync(d, s.d_done.get(), n, cudaMemcpyDeviceToHost, st));
+    if (fail_host) MGB_CUDA(cudaMemcpyAsync(pin_out ? fail_host : s.h_fail.get(), s.d_fail.get(), n * 4, cudaMemcpyDeviceToHost, st));
     if (final_obs_host)
-        MGB_CUDA(cudaMemcpyAsync(pin_out ? final_obs_host : h->h_final, h->d_final, n * D * 4, cudaMemcpyDeviceToHost, st));
+        MGB_CUDA(cudaMemcpyAsync(pin_out ? final_obs_host : s.h_final.get(), s.d_final.get(), n * D * 4, cudaMemcpyDeviceToHost, st));
     if (truncated_host)
-        MGB_CUDA(cudaMemcpyAsync(pin_out ? truncated_host : h->h_trunc, h->d_trunc, n, cudaMemcpyDeviceToHost, st));
+        MGB_CUDA(cudaMemcpyAsync(pin_out ? truncated_host : s.h_trunc.get(), s.d_trunc.get(), n, cudaMemcpyDeviceToHost, st));
     MGB_CUDA(cudaStreamSynchronize(st));
     if (!pin_out) {
-        memcpy(obs_host, h->h_obs, n * D * 4);
-        memcpy(rew_host, h->h_rew, n * 4);
-        memcpy(done_host, h->h_done, n);
-        if (fail_host) memcpy(fail_host, h->h_fail, n * 4);
-        if (final_obs_host) memcpy(final_obs_host, h->h_final, n * D * 4);
-        if (truncated_host) memcpy(truncated_host, h->h_trunc, n);
+        memcpy(obs_host, s.h_obs.get(), n * D * 4);
+        memcpy(rew_host, s.h_rew.get(), n * 4);
+        memcpy(done_host, s.h_done.get(), n);
+        if (fail_host) memcpy(fail_host, s.h_fail.get(), n * 4);
+        if (final_obs_host) memcpy(final_obs_host, s.h_final.get(), n * D * 4);
+        if (truncated_host) memcpy(truncated_host, s.h_trunc.get(), n);
     }
     return MGB_OK;
 }
@@ -2054,7 +2045,7 @@ extern "C" int mgb_quad_restore(mgb_quad *h, const uint8_t *rec_dev, int64_t n_r
     const unsigned blocks = (unsigned)((h->n + 255) / 256);
     const uint4 *rec = reinterpret_cast<const uint4 *>(rec_dev);
     if (h->env2task) {
-        quad_restore_task_kernel<<<blocks, 256, 0, st>>>(h->n, h->env2task, h->n_tasks, rec, n_rec, row_of_env_dev);
+        quad_restore_task_kernel<<<blocks, 256, 0, st>>>(h->n, h->env2task.get(), h->n_tasks, rec, n_rec, row_of_env_dev);
         MGB_CUDA(cudaGetLastError());
         h->launches += 1;
     }

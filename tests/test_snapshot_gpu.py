@@ -440,6 +440,32 @@ def test_refusals_leave_the_handle_untouched(torch_mod, maze_tasks, textures):
         assert np.array_equal(step_once(dst, 3), step_once(twin, 3))
     with pytest.raises(ValueError, match="quadrotor"):
         make_maze("d3_direct", maze_tasks, textures, n=6).restore(make_quad(n=6).snapshot())
+    # a refused set_task: a table with more food cells (a new layout) and a texture id no loaded texture has
+    from metagym_b200._lib import MgbError
+    dst, twin = [make_maze("d3_direct", maze_tasks, textures, n=6) for _ in range(2)]
+    dst.reset()
+    twin.reset()
+    t = maze_tasks[0]
+    food = np.where(np.asarray(t.cell_walls) == 0, 0.3, 0.0)
+    texts = np.asarray(t.cell_texts).copy()
+    texts[0, 0] = 15                                       # n_tex <= 15
+    with pytest.raises(MgbError, match="texture that is not loaded"):
+        dst.set_task([t._replace(food_rewards=food, cell_texts=texts)])
+    assert np.array_equal(dst._fingerprint(), twin._fingerprint()) and dst._record_bytes() == twin._record_bytes()
+    act = torch_mod.from_numpy(maze_actions(dst, 3, 6)).cuda()
+    assert same(*[[x.cpu().numpy() for x in env.step(act)[:3]] for env in (dst, twin)])
+    # a refused quadrotor map (two start cells) keeps the map the handle has
+    dst, twin = make_quad("hovering_control", n=16), make_quad("hovering_control", n=16)
+    grid = np.zeros((6, 6), dtype=np.int32)
+    grid[2, 3], grid[4, 1] = -1, 1
+    for env in (dst, twin):
+        assert env._lib.mgb_quad_set_map(env._h, grid.ctypes.data, 6, 6) == 0
+        env.reset()
+    bad = grid.copy()
+    bad[0, 0] = -1
+    assert dst._lib.mgb_quad_set_map(dst._h, bad.ctypes.data, 6, 6) < 0
+    assert dst._fingerprint()[1] == twin._fingerprint()[1] != 0
+    assert np.array_equal(step_once(dst, 3), step_once(twin, 3))
 
 
 # ---------------------------------------------------------------------------------------------------------------
