@@ -273,8 +273,11 @@ typedef struct mgb_maze_sampler_cfg {
  * come from a counter-based generator keyed by (seed, global env index, how often the env has been resampled), so results
  * do not depend on sharding.  The distribution family is MazeTaskSampler's (spanning tree of the room lattice, loops down
  * to crowd_ratio, textures, start/goal, thinned food); it is NOT sample-identical to the reference, which draws from
- * Python's and numpy's global MT19937 streams.  Needs one table slot per env (mgb_maze_set_task with an injective
- * env2task) and the direct renderer; food cells per task are capped at the table's largest task. */
+ * Python's and numpy's global MT19937 streams.  Food values are clip(U * food_reward, 0.10, food_reward) in np.clip's
+ * order and a food cell's interval is food_interval where its value is above 1e-3, else 0, as in MazeTaskSampler.  Needs
+ * one table slot per env (mgb_maze_set_task with an injective env2task) and the direct renderer; food cells per task are
+ * capped at the table's largest task.  Allocates nothing (mgb_maze_set_task allocates the resample counts), so it can be
+ * captured in a CUDA graph. */
 int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, const mgb_maze_sampler_cfg *cfg, uint64_t seed,
                             void *stream);
 

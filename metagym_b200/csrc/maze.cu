@@ -34,7 +34,7 @@ constexpr int kRenderThreads = 512;
 constexpr int kGeoThreads = 128;            // direct renderer, pipelined: threads that prepare the next env's records
 constexpr int kMaxHitsCap = 2 * kMaxN - 1;   // a ray enters at most 2 n - 1 cells of an n x n grid
 
-struct TaskHdr {                 // 112 bytes, head of every task blob
+struct TaskHdr {                 // 104 bytes, head of every task blob
     int32_t start[2], goal[2];
     double cell_size, wall_height, agent_height, initial_life, max_life, step_reward, goal_reward;
     int32_t n_food;
@@ -2513,6 +2513,14 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
                 MGB_REQUIRE(id >= 0 && (!h->has_tex || id < c.n_tex), "cell_texts refers to a texture that is not loaded");
             }
     }
+    // The per-env resample counts, zero from here on and kept by a later set_task.  They are allocated here, where the
+    // call is synchronous anyway, for every table: restore writes them in either record mode, and neither it nor
+    // resample_tasks may allocate or touch the legacy stream (both are stream-ordered and can be captured).
+    MgbDev<uint32_t> epoch;
+    if (!h->task_epoch) {
+        MGB_CUDA(epoch.alloc(sizeof(uint32_t) * (size_t)h->n_pad));
+        MGB_CUDA(cudaMemset(epoch.get(), 0, sizeof(uint32_t) * (size_t)h->n_pad));
+    }
     // The old table goes before the new one is allocated (HBM never holds both); until the new one is complete every
     // step refuses with "Must call set_task" instead of reading a half-built table.
     h->has_task = false; h->tasks = MazeTasks();
@@ -2552,6 +2560,7 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     }
     h->c = c;
     h->tasks = std::move(tasks);
+    if (epoch) h->task_epoch = std::move(epoch);
     h->cls_heights = std::move(cls_heights);
     h->min_cell = min_cell; h->slot_per_env = slot_per_env;
     h->slot_fp.assign((size_t)n_tasks, 0);
@@ -2593,10 +2602,12 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
 // deliver 700 (reference random streams) to 4 200 (numpy RandomState) tasks/s.  This kernel draws a fresh maze per finished
 // env -- one thread per env, Philox keyed by (seed, global env index, resample count) -- from the same distribution family
 // as MazeTaskSampler(rng=...) (metagym_b200/metamaze.py; the reference's maze_task.py:41-190 draws from Python's and
-// numpy's global MT19937 streams, which a device cannot replay: parity here is distributional and structural, asserted
-// in tests/test_maze_gpu.py: rooms on odd coordinates, border walls, a spanning tree of the room lattice by randomised
-// Kruskal, loops knocked out down to crowd_ratio, textures 1..n_texts-1 on walls, start/goal rooms > 0.45 n apart, food
-// values clip(U * food_reward, 0.1, food_reward) thinned by 0.9 per round until their sum is <= (n-1)^2 food_density).
+// numpy's global MT19937 streams, which a device cannot replay: parity with the reference is distributional and
+// structural: rooms on odd coordinates, border walls, a spanning tree of the room lattice by randomised Kruskal, loops
+// knocked out down to crowd_ratio, textures 1..n_texts-1 on walls, start/goal rooms > 0.45 n apart, food values
+// np.clip(U * food_reward, 0.1, food_reward) thinned by 0.9 per round until their sum is <= (n-1)^2 food_density, an
+// interval where a value is above 1e-3).  The draws themselves are restated exactly in tests/maze_sampler_draws.py, and
+// the tests compare every sampled task with that restatement.
 // ---------------------------------------------------------------------------------------------------------------
 struct SamplerCfg {          // mgb_maze_sampler_cfg + derived fields
     int allow_loops, n_texts, food_interval, cls;
@@ -2706,9 +2717,10 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
     __syncwarp();
     // ---- textures + food values, one cell per lane and pass
     uint8_t *b = blobs + (size_t)a.env2task[e] * c.blob_bytes;
-    auto value_of = [&](uint32_t u24) {                               // clip(food_reward * U, 0.10, food_reward)
+    auto value_of = [&](uint32_t u24) {      // np.clip(food_reward * U, 0.10, food_reward): below 0.10, food_reward wins
         const double v = (double)u24 * (1.0 / 16777216.0) * sc.food_reward;
-        return v < 0.10 ? 0.10 : (v > sc.food_reward ? sc.food_reward : v);
+        const double lo = v < 0.10 ? 0.10 : v;
+        return lo > sc.food_reward ? sc.food_reward : lo;
     };
     double total = 0.0;
     int alive = 0;
@@ -2747,10 +2759,16 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
     {
         int cnt = 0;
         for (int k = 0; k < nn; ++k) {                                 // food slots numbered in cell order
-            if (walls[k] & 2) { fidx[k] = (int8_t)cnt; fval[cnt] = value_of(val[k]); fint[cnt] = sc.food_interval; ++cnt; }
-            else fidx[k] = -1;
+            if (walls[k] & 2) {
+                const double v = value_of(val[k]);
+                fidx[k] = (int8_t)cnt; fval[cnt] = v; fint[cnt] = v > 1.0e-3 ? sc.food_interval : 0;   // maze_task.py:174
+                ++cnt;
+            } else fidx[k] = -1;
         }
-        TaskHdr hd;
+        // the slots past n_food and the header hold zeros, as fill_task_blob writes them: a sampled blob is byte for
+        // byte the blob of the same task given to set_task / update_tasks
+        for (int f = cnt; f < c.f_max; ++f) { fval[f] = 0.0; fint[f] = 0; }
+        TaskHdr hd = {};
         hd.start[0] = sx; hd.start[1] = sy; hd.goal[0] = gx; hd.goal[1] = gy;
         hd.cell_size = sc.cell_size; hd.wall_height = sc.wall_height; hd.agent_height = sc.agent_height;
         hd.initial_life = sc.initial_life; hd.max_life = sc.max_life; hd.step_reward = sc.step_reward;
@@ -2868,17 +2886,6 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     return MGB_OK;
 }
 
-// The per-env resample counts, zero until the first mgb_maze_resample_tasks (or a restore) needs them
-static int ensure_task_epoch(mgb_maze *h)
-{
-    if (h->task_epoch) return MGB_OK;
-    MgbDev<uint32_t> epoch;
-    MGB_CUDA(epoch.alloc(sizeof(uint32_t) * (size_t)h->n_pad));
-    MGB_CUDA(cudaMemset(epoch.get(), 0, sizeof(uint32_t) * (size_t)h->n_pad));
-    h->task_epoch = std::move(epoch);
-    return MGB_OK;
-}
-
 extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, const mgb_maze_sampler_cfg *cfg, uint64_t seed,
                                        void *stream)
 {
@@ -2907,8 +2914,6 @@ extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, con
     sc.cls = -1;
     for (size_t k = 0; k < h->cls_heights.size() / 2; ++k)
         if (h->cls_heights[2 * k] == cfg->agent_height && h->cls_heights[2 * k + 1] == cfg->wall_height) sc.cls = (int)k;
-    int rc = ensure_task_epoch(h);
-    if (rc) return rc;
     MazeArgs a = maze_args(h);
     maze_sample_tasks_kernel<<<(unsigned)((h->n + kSamplerWarps - 1) / kSamplerWarps), 32 * kSamplerWarps, 0, (cudaStream_t)stream>>>(c, a, h->tasks.blobs.get(), mask_dev, h->task_epoch.get(),
                                                                                         sc, seed);
@@ -4279,7 +4284,6 @@ extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_r
     // what the first reset() builds, so that a handle restored right after set_task steps (and can be captured) like a
     // reset one
     if (h->c.kind != MGB_MAZE_2D && (rc = ensure_pose_cache(h, st))) return rc;
-    if ((rc = ensure_task_epoch(h))) return rc;
     const bool carry = records_carry_tasks(h);
     const int64_t rb = record_bytes(h);
     const MazeArgs a = maze_args(h);

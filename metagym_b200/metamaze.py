@@ -360,7 +360,10 @@ class _BatchedMazeBase(Snapshots):
         gets a freshly drawn maze (MazeTaskSampler's keyword arguments and distribution family; counter-based draws keyed
         by (seed, global env index, resample count)) and restarts on it.  One stream-ordered kernel; typical use:
         `obs, rew, done, _ = env.step(a); env.resample_tasks(done)`.  Needs set_task() with one table slot per env
-        (env2task = arange) and the direct renderer (cache=False)."""
+        (env2task = arange) and the direct renderer (cache=False).  goal_reward None is the reference's default
+        -sqrt(n) * n * step_reward; an explicit goal_reward <= 0 raises ValueError, as MazeTaskSampler refuses it."""
+        if goal_reward is not None and not goal_reward > 0:
+            raise ValueError("goal reward must be > 0")
         m = None
         if mask is not None:
             m = self._torch.as_tensor(mask, device=self.device).to(self._torch.uint8).contiguous()
