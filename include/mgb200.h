@@ -287,10 +287,13 @@ int mgb_maze_get_tasks(mgb_maze *h, int32_t count, const int32_t *task_slots_hos
 
 /* MetaMazeDiscrete3D renderer choice.  enabled = 1 (default): static layers of every (task, cell, heading) are rendered once
  * and memoised (pose cache, within MGB_MAZE_CACHE_GB), a step composes / copies; 0: every frame is ray-cast directly
- * (ray_caster_utils.py:66-209 per frame, like the reference) -- the mode for task tables that change every episode. */
+ * (ray_caster_utils.py:66-209 per frame, like the reference) -- the mode for task tables that change every episode
+ * (mgb_maze_resample_tasks).  The cache is laid out per task slot (S = 4 x the most free cells of a set_task task pose
+ * slots, V variant frames each), so mgb_maze_update_tasks rebuilds only the replaced tasks. */
 int mgb_maze_set_cache(mgb_maze *h, int enabled);
 
-/* Pose-cache statistics after the first reset/step (reporting only): out[0] cached poses, out[1] extra variant frames,
+/* Pose-cache statistics after the first reset/step (reporting only; synchronises the device to read the counts of
+ * tasks mgb_maze_update_tasks rebuilt back): out[0] cached poses, out[1] extra variant frames,
  * out[2] variant bits in use (poses whose image depends on k <= bits foods have all 2^k finished frames), out[3] bytes,
  * out[4..12] poses by k (0..7, and 8 = eight or more), out[13] 1 if the cache is in use; shared-memory plan of the last
  * direct-renderer launch: out[14] 1 if the crossing lists live in a global scratch, out[15] 1 if pipelined. */
@@ -302,8 +305,11 @@ int mgb_maze_cache_info(const mgb_maze *h, int64_t out[16]);
  * (one pinned-staged copy + three small kernels on `stream`).  Every env whose env2task entry is one of the replaced slots
  * starts a new episode on its new task (agent at start, life = initial_life, food restored), like set_task + reset of that
  * env; other envs are untouched.  The table's shape is fixed by mgb_maze_set_task: a replacement may not have more food
- * cells than the table's largest task nor smaller cells than its smallest.  Needs the direct renderer (the pose cache
- * memoises whole task tables): create the env with the cache off or with more tasks than the cache budget holds. */
+ * cells than the table's largest task nor smaller cells than its smallest.  MetaMazeDiscrete3D on the pose cache: the
+ * replaced tasks' poses and frames are rebuilt in place in the same stream order (FILL pass, signatures, device-planned
+ * variant frames, bakes, pose records; no allocation), and a replacement may not have more free cells (start cell
+ * included) than the largest task of mgb_maze_set_task, nor may a slot appear twice in one call.  Before the cache's first
+ * build (set_task without reset yet) only the table changes, and the first build covers it. */
 int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *task_slots_host, const int8_t *walls_host,
                           const int8_t *texts_host, const double *food_rewards_host, const int32_t *food_interval_host,
                           const mgb_maze_task_scalars *scalars_host, void *stream);

@@ -87,7 +87,7 @@ struct MazeArgs {
     // variant frames (uint8 SURVIVAL): a pose whose image depends on k <= kVariantBits foods has all 2^k finished frames
     // baked, so a step never recomputes a pixel -- it picks the frame of the foods currently visible
     const int32_t *c_vbase;      // [n_slots] index of the pose's first extra frame in c_var8, or -1 (all-present frame only)
-    uint8_t *c_var8;             // [n_var_frames][H*V*3]; variant v of a pose = frame c_vbase + v, v = the visible foods'
+    uint8_t *c_var8;             // [n_tasks * V][H*V*3]; variant v of a pose = frame c_vbase + v, v = the visible foods'
                                  // bits compacted in ascending slot order; the all-visible variant is c_rgb8[slot] itself
     const void *bake_desc;       // bake mode over variant frames: [n_items] BakeDesc (slot, presence mask)
     int bake;                    // compose kernel: items are pose slots, output goes to c_rgb8 / c_px_all
@@ -131,6 +131,16 @@ struct MazeArgs {
     // path recording (mgb_maze_set_path): [max_steps + 1][n_pad] grid cells, step-major.  Whenever a kernel leaves env e
     // with step count s, entry (s, e) holds the agent's cell; nullptr: recording off, nothing is stored
     char2 *path;
+    // pose-cache build of a region of the task table (ensure_pose_cache: every task; mgb_maze_update_tasks: the replaced
+    // ones).  Task slot t owns the pose slots [t S, t S + S) and the variant frames [t V, t V + V); a region kernel's item i
+    // is entry i % region_ext of task region[i / region_ext] (region_ext = S or V), the FILL pass renders the pose slots
+    // fill_slot[0 .. n).  Unused pose slots have poses[slot].x = -1; a task's frames past task_frames[t] are unused.
+    const int32_t *region;       // [K] task slots
+    const int32_t *fill_slot;    // [n] pose slots of the region's tasks
+    const int32_t *task_frames;  // [n_tasks] variant frames planned for each task
+    int region_ext;
+    int pose_stride, var_stride; // S, V
+    int var_bits;                // variant bits of the table: a task takes the largest bits <= var_bits whose frames fit V
 };
 
 struct Env {
@@ -752,8 +762,9 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     int run_parity = 0;
 
     // ---- maze tiles (walls, texture ids, food table) arrive by TMA one env ahead of their use
+    auto slot_of = [&](int64_t e) -> int64_t { return FILL ? (int64_t)a.fill_slot[e] : e; };   // FILL: item -> pose slot
     auto load_blob = [&](int64_t e, int b) {
-        const int task_id = FILL ? a.poses[e].x : a.env2task[e];
+        const int task_id = FILL ? a.poses[slot_of(e)].x : a.env2task[e];
         const uint8_t *src = a.blobs + (int64_t)task_id * c.blob_bytes;
         mgb_mbar_expect_tx(&s_bar[1 + b], (uint32_t)c.blob_bytes);
         mgb_bulk_load(b ? s_blob2[1] : s_blob2[0], src, (uint32_t)c.blob_bytes, &s_bar[1 + b]);
@@ -786,7 +797,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
         // ---- step logic (one thread), then publish agent pose to the CTA
         if (FILL) {
             if (gt == 0) {
-                const int4 ps = a.poses[e];
+                const int4 ps = a.poses[slot_of(e)];
                 s_env[0] = ps.y; s_env[1] = ps.z; s_env[2] = ps.w; s_env[3] = 0; s_env[4] = 0;
             }
         } else if (gt == 0) {
@@ -999,8 +1010,8 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
             }
             s_col[d_h] = cr;
             if (FILL) {
-                a.c_colhits[(size_t)e * H + d_h] = (uint8_t)cr.n_hits;
-                HitRec *gh = reinterpret_cast<HitRec *>(a.c_hits) + ((size_t)e * H + d_h) * c.max_hits;
+                a.c_colhits[(size_t)slot_of(e) * H + d_h] = (uint8_t)cr.n_hits;
+                HitRec *gh = reinterpret_cast<HitRec *>(a.c_hits) + ((size_t)slot_of(e) * H + d_h) * c.max_hits;
                 for (int k = 0; k < cr.n_hits; ++k) gh[k] = hits[k];
             }
         }
@@ -1272,8 +1283,9 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
             const double dts = (double)ts;
             const int8_t *fidx = reinterpret_cast<const int8_t *>(s_blob + c.off_fidx);
             const int goal_cell = th->goal[0] * n + th->goal[1];
-            uint32_t *gpx = a.c_px + (size_t)e * total_px;
-            uint8_t *gfid = a.c_fid + (size_t)e * total_px;
+            const size_t slot = (size_t)slot_of(e);
+            uint32_t *gpx = a.c_px + slot * total_px;
+            uint8_t *gfid = a.c_fid + slot * total_px;
             for (int q = tid; q < total_px; q += blockDim.x) {
                 const int d_h = q / V, d_v = q - d_h * V;
                 const ColRec &cr = s_col[d_h];
@@ -1322,7 +1334,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                 }
                 gpx[q] = (uint32_t)rgb[0] | ((uint32_t)rgb[1] << 10) | ((uint32_t)rgb[2] << 20) | (in_wall ? (1u << 30) : 0u);
                 gfid[q] = (uint8_t)fid;
-                uint8_t *g8 = a.c_rgb8 + ((size_t)e * total_px + q) * 3;
+                uint8_t *g8 = a.c_rgb8 + (slot * total_px + q) * 3;
                 g8[0] = (uint8_t)(rgb[0] > 255 ? 255 : rgb[0]);
                 g8[1] = (uint8_t)(rgb[1] > 255 ? 255 : rgb[1]);
                 g8[2] = (uint8_t)(rgb[2] > 255 ? 255 : rgb[2]);
@@ -1540,12 +1552,18 @@ __global__ void maze3d_logic_kernel(const __grid_constant__ MazeConst c, const _
 // per pose slot, after the FILL render: (1) c_fmask = the food slots that can change this pose's image at all (under a
 // pixel or in a crossing record); (2) c_gsig = one byte per 4-pixel group, OR of 1 << (f & 7) over the food slots f that
 // can tint a pixel of the group (floor/ceiling cell under it, or a crossing span over it).  0 = never tinted.  An env
-// whose missing foods have the 8-bit signature S needs the float64 path only for groups with (gsig & S) != 0.
+// whose missing foods have the 8-bit signature S needs the float64 path only for groups with (gsig & S) != 0.  Block b
+// serves pose slot a.fill_slot[b]; int32 screens (a.c_px_all set) also start its all-present colours as the static ones.
 __global__ void __launch_bounds__(256) maze3d_sig_kernel(const __grid_constant__ MazeConst c,
                                                          const __grid_constant__ MazeArgs a)
 {
-    const int64_t slot = blockIdx.x;
+    const int64_t slot = a.fill_slot[blockIdx.x];
     const int V = c.res_v, total_px = c.res_h * V;
+    if (a.c_px_all) {
+        const uint4 *src = reinterpret_cast<const uint4 *>(a.c_px + (size_t)slot * total_px);
+        uint4 *dst = reinterpret_cast<uint4 *>(a.c_px_all + (size_t)slot * total_px);
+        for (int i = threadIdx.x; i < total_px / 4; i += blockDim.x) dst[i] = src[i];
+    }
     const uint8_t *gfid = a.c_fid + (size_t)slot * total_px;
     const uint8_t *colhits = a.c_colhits + (size_t)slot * c.res_h;
     const HitRec *ghits = reinterpret_cast<const HitRec *>(a.c_hits) + (size_t)slot * c.res_h * c.max_hits;
@@ -1569,19 +1587,103 @@ __global__ void __launch_bounds__(256) maze3d_sig_kernel(const __grid_constant__
         gsig[g] = (uint8_t)sig;
     }
     for (int o = 16; o > 0; o >>= 1) { m0 |= __shfl_xor_sync(0xffffffffu, m0, o); m1 |= __shfl_xor_sync(0xffffffffu, m1, o); }
-    if ((threadIdx.x & 31) == 0) {
-        if (m0) atomicOr(reinterpret_cast<unsigned long long *>(a.c_fmask + slot * 2), (unsigned long long)m0);
-        if (m1) atomicOr(reinterpret_cast<unsigned long long *>(a.c_fmask + slot * 2 + 1), (unsigned long long)m1);
+    __shared__ uint64_t s_m[256 / 32][2];
+    if ((threadIdx.x & 31) == 0) { s_m[threadIdx.x >> 5][0] = m0; s_m[threadIdx.x >> 5][1] = m1; }
+    __syncthreads();
+    if (threadIdx.x == 0) {                  // the whole mask is written: a rebuilt slot keeps nothing of its previous pose
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) { m0 |= s_m[w][0]; m1 |= s_m[w][1]; }
+        a.c_fmask[slot * 2] = m0;
+        a.c_fmask[slot * 2 + 1] = m1;
     }
 }
 
-// variant frames start as copies of the pose's STATIC frame (what the FILL render left in c_rgb8, before any tint is baked)
+// Item i of a region kernel (see MazeArgs::region): the pose slot (pose bake) or the variant frame (a.bake_desc set) it
+// stands for, -1 when the task has no such pose or frame
+__device__ __forceinline__ int64_t region_item(const MazeArgs &a, int64_t i)
+{
+    const int64_t k = i / a.region_ext, j = i - k * a.region_ext;
+    const int64_t t = a.region[k], r = t * a.region_ext + j;
+    if (a.bake_desc) return j < a.task_frames[t] ? r : -1;
+    return a.poses[r].x >= 0 ? r : -1;
+}
+
+// Variant frames of the region's tasks, planned on the device from c_fmask (one warp per task, block = a.region entry): a
+// pose whose image depends on k foods, 1 <= k <= bits, gets the 2^k - 1 frames vbase .. vbase + 2^k - 2 (the all-visible
+// one is c_rgb8[slot]), in ascending pose-slot order from the task's first frame t V.  bits is the largest <= a.var_bits
+// whose frames fit the task's V frames, so a task of the table ensure_pose_cache sized V by takes a.var_bits itself.
+__global__ void __launch_bounds__(32) maze3d_plan_kernel(const __grid_constant__ MazeArgs a, int32_t *vbase, BakeDesc *desc,
+                                                         int32_t *task_frames)
+{
+    const int64_t t = a.region[blockIdx.x], S = a.pose_stride, V = a.var_stride;
+    const int lane = threadIdx.x;
+    auto foods = [&](int64_t j, uint64_t fm[2]) -> int {
+        fm[0] = fm[1] = 0;
+        if (j >= S || a.poses[t * S + j].x < 0) return 0;
+        fm[0] = a.c_fmask[(t * S + j) * 2]; fm[1] = a.c_fmask[(t * S + j) * 2 + 1];
+        return __popcll(fm[0]) + __popcll(fm[1]);
+    };
+    int64_t need[kVariantBitsMax + 1];
+#pragma unroll
+    for (int b = 0; b <= kVariantBitsMax; ++b) need[b] = 0;
+    for (int64_t j = lane; j < S; j += 32) {
+        uint64_t fm[2];
+        const int k = foods(j, fm);
+#pragma unroll
+        for (int b = 1; b <= kVariantBitsMax; ++b)
+            if (k >= 1 && k <= b) need[b] += ((int64_t)1 << k) - 1;
+    }
+    int bits = 0;
+    int64_t frames = 0;
+#pragma unroll
+    for (int b = 1; b <= kVariantBitsMax; ++b) {
+        int64_t s = need[b];
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (b <= a.var_bits && s <= V) { bits = b; frames = s; }     // need[] grows with b
+    }
+    int64_t run = t * V;
+    for (int64_t j0 = 0; j0 < S; j0 += 32) {
+        const int64_t j = j0 + lane;
+        uint64_t fm[2];
+        const int k = foods(j, fm);
+        const int own = (k >= 1 && k <= bits) ? (1 << k) - 1 : 0;
+        int incl = own;
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+        }
+        const int64_t base = run + incl - own;
+        if (j < S) vbase[t * S + j] = own ? (int32_t)base : -1;
+        for (int v = 0; v < own; ++v) {
+            BakeDesc bd;
+            bd.slot = (int32_t)(t * S + j); bd.pad = 0;
+            bd.present[0] = ~fm[0]; bd.present[1] = ~fm[1];            // foods this pose never shows: irrelevant
+            int bit = 0;
+            for (int w = 0; w < 2; ++w) {
+                uint64_t m = fm[w];
+                while (m) {
+                    const uint64_t low = m & (~m + 1);
+                    m &= m - 1;
+                    if ((v >> bit) & 1) bd.present[w] |= low;
+                    ++bit;
+                }
+            }
+            desc[base + v] = bd;
+        }
+        run += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (lane == 0) task_frames[t] = (int32_t)frames;
+}
+
+// variant frames start as copies of the pose's STATIC frame (what the FILL render left in c_rgb8, before any tint is baked);
+// block = region item over the tasks' variant frames
 __global__ void __launch_bounds__(256) maze3d_varinit_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a)
 {
+    const int64_t f = region_item(a, blockIdx.x);
+    if (f < 0) return;
     const size_t frame16 = (size_t)c.res_h * c.res_v * 3 / 16;
-    const BakeDesc bd = reinterpret_cast<const BakeDesc *>(a.bake_desc)[blockIdx.x];
+    const BakeDesc bd = reinterpret_cast<const BakeDesc *>(a.bake_desc)[f];
     const uint4 *src = reinterpret_cast<const uint4 *>(a.c_rgb8) + (size_t)bd.slot * frame16;
-    uint4 *dst = reinterpret_cast<uint4 *>(a.c_var8) + (size_t)blockIdx.x * frame16;
+    uint4 *dst = reinterpret_cast<uint4 *>(a.c_var8) + (size_t)f * frame16;
     for (size_t i = threadIdx.x; i < frame16; i += blockDim.x) dst[i] = src[i];
 }
 
@@ -1590,6 +1692,9 @@ constexpr int kComposeThreads = 256;
 // Work item = (env, image slice).  Pixels no missing food can tint are copied from the pose's baked all-present frame;
 // the others take the cached static layers (packed colour + in-wall flag, food slot under the pixel, crossing records
 // of the column) through the reference's float64 blend with the env's 128-bit food presence mask.
+// REGION (pose-cache build, bake mode): items are region items (MazeArgs::region) that skip the poses / frames a task
+// does not have; the step's instantiation stays the plain one.
+template <bool REGION>
 __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(const __grid_constant__ MazeConst c,
                                                                          const __grid_constant__ MazeArgs a)
 {
@@ -1610,6 +1715,10 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
   auto fetch = [&](int64_t idx) -> EnvDyn {
       if (!a.bake) return reinterpret_cast<const EnvDyn *>(a.dyn)[idx];
       EnvDyn b;
+      if (REGION) {
+          idx = region_item(a, idx);
+          if (idx < 0) { b.slot = 0; b.task = 0; return b; }     // skipped by the loop below
+      }
       b.slot = (int32_t)idx; b.bar_end = 0; b.present[0] = b.present[1] = ~0ull; b.pad = 0xFF; b.vframe = -1; b.pad2 = 0;
       if (a.bake_desc) {               // variant frames: item = frame, its pose slot and presence mask come from the descriptor
           const BakeDesc bd = reinterpret_cast<const BakeDesc *>(a.bake_desc)[idx];
@@ -1623,13 +1732,13 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
   for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int64_t entry = item / kParts;
     const int part = (int)(item - entry * kParts);
-    const int64_t e = a.final_obs ? (int64_t)a.fin_env[entry] : entry;
+    const int64_t e = REGION ? region_item(a, entry) : (a.final_obs ? (int64_t)a.fin_env[entry] : entry);
     const int q_begin = part * part_px, q_end = (part + 1) * part_px < total_px ? (part + 1) * part_px : total_px;
     // software pipeline: the next item's EnvDyn (-> pose slot -> every address below) is requested now, so the
     // dependent-load bubble at the start of an item overlaps this item's pixels
     const EnvDyn d = d_next;
     if (item + gridDim.x < n_items) d_next = fetch((item + gridDim.x) / kParts);
-    if (q_begin >= total_px) continue;
+    if (q_begin >= total_px || (REGION && e < 0)) continue;
 #include "maze_compose_body.inc"
   }
 }
@@ -2066,6 +2175,7 @@ struct MazePoseCache {             // built by ensure_pose_cache (MazeArgs descr
     MgbDev<HitRec> c_hits;
     MgbDev<EnvDyn> dyn;
     MgbDev<BakeDesc> bake_desc;
+    MgbDev<int32_t> task_frames;   // [n_tasks] variant frames of each task slot (maze3d_plan_kernel)
     MgbDev<PoseRec> pose_rec;      // built after the variant frames
 };
 
@@ -2107,15 +2217,19 @@ struct mgb_maze {
     double min_cell = 0.0;                    // smallest cell_size of the table (bounds the crossings a ray can record)
     MazeStage stage[2];
     int stage_next = 0;
-    int64_t n_var_frames = 0;
-    int64_t k_hist[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // poses by the number of foods their image depends on (8 = 8 or more)
     int variant_bits_used = 0;
+    bool var_planned = false;      // the last build read c_fmask back and planned variant frames (cache_info reports them)
     double cache_bytes = 0.0;
     int variant_bits = 7;          // MGB_MAZE_VARIANT_BITS: poses that depend on <= this many foods get all 2^k frames (0 = off)
     MgbDev<uint8_t> hit_scratch;
     size_t hit_scratch_bytes = 0;
-    std::vector<int4> host_poses;
-    std::vector<int32_t> host_pose_index;
+    // pose list of the cache, slot-strided: task slot t owns the pose slots [t S, t S + S), S = pose_stride (4 x the most
+    // free cells of a task); unused slots hold task -1.  var_stride V: variant frames per task slot, fixed by the first build
+    std::vector<int4> host_poses;             // [n_tasks * S]
+    std::vector<int32_t> host_pose_index;     // [n_tasks][n * n * 4] -> pose slot or -1
+    std::vector<int32_t> task_poses;          // [n_tasks] used pose slots of each task
+    int pose_stride = 0;
+    int64_t var_stride = 0;
     int n_tasks = 0;
     int auto_reset = 0;
     bool has_task = false, has_tex = false;
@@ -2305,10 +2419,25 @@ extern "C" int mgb_maze_cache_info(const mgb_maze *h, int64_t out[16])
     MGB_REQUIRE(h && out, "null argument");
     for (int i = 0; i < 16; ++i) out[i] = 0;
     out[0] = h->cache_ready ? h->n_poses : 0;
-    out[1] = h->cache_ready ? h->n_var_frames : 0;
+    if (h->cache_ready && h->var_planned) {
+        // update_tasks replans the frames of its tasks on the device: read the counts back (reporting only)
+        MgbDeviceGuard guard(h->device);
+        MGB_CUDA(cudaDeviceSynchronize());
+        std::vector<uint64_t> fm(h->host_poses.size() * 2);
+        MGB_CUDA(cudaMemcpy(fm.data(), h->cache.c_fmask.get(), fm.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        for (size_t sl = 0; sl < h->host_poses.size(); ++sl) {
+            if (h->host_poses[sl].x < 0) continue;
+            const int k = __builtin_popcountll(fm[2 * sl]) + __builtin_popcountll(fm[2 * sl + 1]);
+            out[4 + (k < 8 ? k : 8)] += 1;
+        }
+        if (h->cache.task_frames) {
+            std::vector<int32_t> frames((size_t)h->n_tasks);
+            MGB_CUDA(cudaMemcpy(frames.data(), h->cache.task_frames.get(), frames.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+            for (int32_t f : frames) out[1] += f;
+        }
+    }
     out[2] = h->variant_bits_used;
     out[3] = (int64_t)h->cache_bytes;
-    for (int k = 0; k < 9; ++k) out[4 + k] = h->k_hist[k];
     out[13] = h->cache_ready ? 1 : 0;
     out[14] = h->c.hits_in_global;      // plan of the last direct-renderer launch: crossing lists in global scratch
     out[15] = h->c.pipe;                // ... and geometry pipelined under the pixels
@@ -2435,6 +2564,32 @@ static void fill_task_blob(const MazeConst &c, uint8_t *b, const int8_t *walls, 
     }
     hd.n_food = cnt;
     memcpy(b, &hd, sizeof(hd));
+}
+
+// Free cells of a task: the agent can never stand inside a wall (maze_discrete_3d.py:63-65); the start cell counts as free
+static int task_free_cells(const MazeConst &c, const int8_t *walls, const mgb_maze_task_scalars &s)
+{
+    int cnt = 0;
+    for (int k = 0; k < c.n * c.n; ++k) cnt += (walls[k] == 0 || k == s.start[0] * c.n + s.start[1]) ? 1 : 0;
+    return cnt;
+}
+
+// Pose-cache rows of task slot t: every free cell x 4 headings in cell order at pose slots t S + j (rows[j]); the task's
+// other S - 4 x free slots are unused (task -1).  index: the task's [n * n * 4] pose_index row.  Returns the pose count.
+static int task_pose_rows(const MazeConst &c, int S, int t, const int8_t *walls, const mgb_maze_task_scalars &s, int4 *rows,
+                          int32_t *index)
+{
+    const int n = c.n, nn = n * n;
+    int j = 0;
+    for (int k = 0; k < nn; ++k) {
+        const bool free = walls[k] == 0 || k == s.start[0] * n + s.start[1];
+        for (int o = 0; o < 4; ++o) {
+            index[k * 4 + o] = free ? (int32_t)((int64_t)t * S + j) : -1;
+            if (free) rows[j++] = make_int4(t, k / n, k % n, o);
+        }
+    }
+    for (int u = j; u < S; ++u) rows[u] = make_int4(-1, 0, 0, 0);
+    return j;
 }
 
 extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *walls_host, const int8_t *texts_host,
@@ -2570,23 +2725,26 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     h->has_task = true;
     h->task_flags.reset();
     h->cache_would_fit = true;
-    // pose list of the cache: every free cell (the agent can never stand inside a wall, maze_discrete_3d.py:63-65) x 4
+    // pose list of the cache: every free cell x 4 headings of every task, S = 4 x the most free cells of a task per task
+    // slot, so that update_tasks can rebuild one task's poses in place
     h->host_poses.clear();
     h->host_pose_index.assign((size_t)n_tasks * nn * 4, -1);
+    h->task_poses.assign((size_t)n_tasks, 0);
+    h->pose_stride = 0;
     h->cache_dirty = true;
     h->cache_ready = false;
     if (c.kind == MGB_MAZE_DISCRETE_3D) {
+        int most = 0;
         for (int t = 0; t < n_tasks; ++t) {
-            const mgb_maze_task_scalars &sc = scalars_host[t];
-            for (int k = 0; k < nn; ++k) {
-                const bool is_start = (k == sc.start[0] * n + sc.start[1]);
-                if (walls_host[(size_t)t * nn + k] != 0 && !is_start) continue;
-                for (int o = 0; o < 4; ++o) {
-                    h->host_pose_index[((size_t)t * nn + k) * 4 + o] = (int32_t)h->host_poses.size();
-                    h->host_poses.push_back(make_int4(t, k / n, k % n, o));
-                }
-            }
+            const int f = task_free_cells(c, walls_host + (size_t)t * nn, scalars_host[t]);
+            most = f > most ? f : most;
         }
+        h->pose_stride = 4 * most;
+        h->host_poses.resize((size_t)n_tasks * h->pose_stride);
+        for (int t = 0; t < n_tasks; ++t)
+            h->task_poses[t] = task_pose_rows(c, h->pose_stride, t, walls_host + (size_t)t * nn, scalars_host[t],
+                                              h->host_poses.data() + (size_t)t * h->pose_stride,
+                                              h->host_pose_index.data() + (size_t)t * nn * 4);
     }
     // set_task leaves the env in "need reset" state (maze_env.py:44-50): initialise it so a stray step is harmless
     MazeArgs a = maze_args(h);
@@ -2797,21 +2955,50 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
 // ---------------------------------------------------------------------------------------------------------------
 // Partial, stream-ordered task replacement (per-episode task resampling, SURVEY.md 8f row 3 / maze_base.py:19-38)
 // ---------------------------------------------------------------------------------------------------------------
-// staging layout: [count] int32 table slots | pad to 16 | [count] blobs
+// staging layout: [count] int32 table slots | pad to 16 | [count] blobs | with pose lists (discrete 3-D): [count][S] int4
+// pose rows | [count][n * n * 4] int32 pose_index rows | [n_fill] int32 pose slots of the replaced tasks.  poses: the
+// cache's tables to scatter the rows into (nullptr: no cache built)
 __global__ void maze_scatter_tasks_kernel(const __grid_constant__ MazeConst c, uint8_t *blobs, const uint8_t *stage, int count,
-                                          uint8_t *task_flags)
+                                          uint8_t *task_flags, int4 *poses, int32_t *pose_index, int S)
 {
     const int32_t *slots = reinterpret_cast<const int32_t *>(stage);
-    const uint4 *src = reinterpret_cast<const uint4 *>(stage + (((size_t)count * 4 + 15) / 16) * 16) + (size_t)blockIdx.x * (c.blob_bytes / 16);
-    uint4 *dst = reinterpret_cast<uint4 *>(blobs + (size_t)slots[blockIdx.x] * c.blob_bytes);
+    const uint8_t *blob0 = stage + (((size_t)count * 4 + 15) / 16) * 16;
+    const uint4 *src = reinterpret_cast<const uint4 *>(blob0) + (size_t)blockIdx.x * (c.blob_bytes / 16);
+    const int64_t t = slots[blockIdx.x];
+    uint4 *dst = reinterpret_cast<uint4 *>(blobs + (size_t)t * c.blob_bytes);
     for (int i = threadIdx.x; i < c.blob_bytes / 16; i += blockDim.x) dst[i] = src[i];
-    if (threadIdx.x == 0) task_flags[slots[blockIdx.x]] = 1;
+    if (poses) {
+        const int per = c.n * c.n * 4;
+        const int4 *prow = reinterpret_cast<const int4 *>(blob0 + (size_t)count * c.blob_bytes);
+        const int32_t *irow = reinterpret_cast<const int32_t *>(prow + (size_t)count * S) + (size_t)blockIdx.x * per;
+        prow += (size_t)blockIdx.x * S;
+        for (int i = threadIdx.x; i < S; i += blockDim.x) poses[t * S + i] = prow[i];
+        for (int i = threadIdx.x; i < per; i += blockDim.x) pose_index[t * per + i] = irow[i];
+    }
+    if (threadIdx.x == 0) task_flags[t] = 1;
 }
 __global__ void maze_clear_flags_kernel(uint8_t *task_flags, int n)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) task_flags[i] = 0;
 }
+
+// Lay the host pose lists out at the larger stride S (a handle on the direct renderer took a task with more free cells
+// than the table's largest; a cache enabled later is built at the new stride)
+static void relayout_poses(mgb_maze *h, int S)
+{
+    const int old = h->pose_stride;
+    std::vector<int4> rows((size_t)h->n_tasks * S, make_int4(-1, 0, 0, 0));
+    for (int t = 0; t < h->n_tasks; ++t)
+        for (int j = 0; j < h->task_poses[t]; ++j) rows[(size_t)t * S + j] = h->host_poses[(size_t)t * old + j];
+    for (int32_t &v : h->host_pose_index)
+        if (v >= 0) v = (int32_t)((int64_t)(v / old) * S + v % old);
+    h->host_poses = std::move(rows);
+    h->pose_stride = S;
+}
+
+static int render_region(mgb_maze *h, const MazeArgs &a, int K, int64_t n_fill, cudaStream_t st);
+static int bake_region(mgb_maze *h, MazePoseCache &pc, MazeArgs a, int K, cudaStream_t st);
 
 extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *task_slots_host, const int8_t *walls_host,
                                      const int8_t *texts_host, const double *food_rewards_host,
@@ -2825,10 +3012,13 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     MGB_REQUIRE(h->has_task, "call mgb_maze_set_task first (it sizes the task table)");
     MgbDeviceGuard guard(h->device);
     MazeConst &c = h->c;
-    MGB_REQUIRE(!(c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() && h->cache_would_fit),
-                "partial task updates need the direct renderer: create the env with the pose cache off (MGB_MAZE_CACHE=0 / "
-                "cache=False) -- the cache memoises whole task tables");
     const int n = c.n, nn = n * n;
+    // discrete 3-D tables keep the cache's pose lists; a handle that serves (or will serve) them from the pose cache
+    // rebuilds the replaced tasks' region in place, which needs every task within the table's S / 4 free cells
+    const bool poses_kept = c.kind == MGB_MAZE_DISCRETE_3D && !h->host_poses.empty();
+    const bool cached = poses_kept && h->cache_enabled && h->cache_would_fit;
+    int most = 0;
+    int64_t n_fill = 0;
     for (int t = 0; t < count; ++t) {
         MGB_REQUIRE(task_slots_host[t] >= 0 && task_slots_host[t] < h->n_tasks, "task slot out of range");
         int cnt = 0;
@@ -2843,10 +3033,30 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
         MGB_REQUIRE(s.goal[0] >= 0 && s.goal[0] < n && s.goal[1] >= 0 && s.goal[1] < n, "goal outside the maze");
         MGB_REQUIRE(s.agent_height < s.wall_height && s.agent_height > 0, "the agent height must be > 0 and < wall height");
         MGB_REQUIRE(s.cell_size >= h->min_cell, "a replacement task may not have smaller cells than the table's smallest");
+        if (poses_kept) {
+            const int f = task_free_cells(c, walls_host + (size_t)t * nn, s);
+            MGB_REQUIRE(!cached || 4 * f <= h->pose_stride,
+                        "a replacement task may not have more free cells than the largest task of set_task (pose cache)");
+            most = f > most ? f : most;
+            n_fill += 4 * f;
+        }
     }
+    if (cached) {
+        std::vector<uint8_t> seen((size_t)h->n_tasks, 0);
+        for (int t = 0; t < count; ++t) {
+            MGB_REQUIRE(!seen[task_slots_host[t]], "a task slot may be replaced only once per call (pose cache)");
+            seen[task_slots_host[t]] = 1;
+        }
+    }
+    if (poses_kept && 4 * most > h->pose_stride) relayout_poses(h, 4 * most);
+    const int S = h->pose_stride, per = nn * 4;
+    const bool rebuild = cached && h->cache_ready && !h->cache_dirty;   // before the first build the build covers the change
     // pinned staging, double-buffered: the host waits only for the COPY of the call before last, never for the device
     MazeStage &s = h->stage[h->stage_next];
-    const size_t head = (((size_t)count * 4 + 15) / 16) * 16, need = head + (size_t)count * c.blob_bytes;
+    const size_t head = (((size_t)count * 4 + 15) / 16) * 16, rows_off = head + (size_t)count * c.blob_bytes;
+    const size_t index_off = rows_off + (poses_kept ? (size_t)count * S * sizeof(int4) : 0);
+    const size_t fill_off = index_off + (poses_kept ? (size_t)count * per * sizeof(int32_t) : 0);
+    const size_t need = fill_off + (size_t)n_fill * sizeof(int32_t);
     if (!s.copied) MGB_CUDA(s.copied.create(cudaEventDisableTiming));
     else MGB_CUDA(cudaEventSynchronize(s.copied.get()));
     if (need > s.bytes) {
@@ -2870,19 +3080,51 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
         fill_task_blob(c, hs + head + (size_t)t * c.blob_bytes, walls_host + (size_t)t * nn, texts_host + (size_t)t * nn,
                        food_rewards_host + (size_t)t * nn, food_interval_host + (size_t)t * nn, scalars_host[t], h->cls_heights,
                        false);
+    int4 *rows = reinterpret_cast<int4 *>(hs + rows_off);
+    int32_t *index = reinterpret_cast<int32_t *>(hs + index_off), *fill = reinterpret_cast<int32_t *>(hs + fill_off);
+    std::vector<int32_t> task_n((size_t)count, 0);
+    if (poses_kept) {
+        int64_t k = 0;
+        for (int t = 0; t < count; ++t) {
+            const int64_t slot = task_slots_host[t];
+            task_n[t] = task_pose_rows(c, S, (int)slot, walls_host + (size_t)t * nn, scalars_host[t], rows + (size_t)t * S,
+                                        index + (size_t)t * per);
+            for (int j = 0; j < task_n[t]; ++j) fill[k++] = (int32_t)(slot * S + j);
+        }
+    }
     cudaStream_t st = (cudaStream_t)stream;
     MGB_CUDA(cudaMemcpyAsync(s.dev.get(), hs, need, cudaMemcpyHostToDevice, st));
     MGB_CUDA(cudaEventRecord(s.copied.get(), st));
     h->stage_next ^= 1;
-    maze_scatter_tasks_kernel<<<(unsigned)count, 128, 0, st>>>(c, h->tasks.blobs.get(), s.dev.get(), count, h->task_flags.get());
+    maze_scatter_tasks_kernel<<<(unsigned)count, 128, 0, st>>>(c, h->tasks.blobs.get(), s.dev.get(), count, h->task_flags.get(),
+                                                               rebuild ? h->cache.poses.get() : nullptr,
+                                                               rebuild ? h->cache.pose_index.get() : nullptr, S);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    if (rebuild) {
+        MazeArgs ar = maze_args(h);
+        ar.region = reinterpret_cast<const int32_t *>(s.dev.get());
+        ar.fill_slot = reinterpret_cast<const int32_t *>(s.dev.get() + fill_off);
+        int rc = render_region(h, ar, count, n_fill, st);
+        if (rc) return rc;
+        rc = bake_region(h, h->cache, ar, count, st);
+        if (rc) return rc;
+    }
     MazeArgs a = maze_args(h);
     maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(c, a, h->task_flags.get());
     maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags.get(), h->n_tasks);
     MGB_CUDA(cudaGetLastError());
-    h->launches += 3;
-    // the slots' fingerprints change once their new blobs are on their way
-    for (int t = 0; t < count; ++t)
-        h->slot_fp[task_slots_host[t]] = mgb_fnv(MGB_FNV_BASIS, hs + head + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
+    h->launches += 2;
+    // the slots' fingerprints and pose lists change once their new blobs are on their way
+    for (int t = 0; t < count; ++t) {
+        const int64_t slot = task_slots_host[t];
+        h->slot_fp[slot] = mgb_fnv(MGB_FNV_BASIS, hs + head + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
+        if (!poses_kept) continue;
+        memcpy(h->host_poses.data() + slot * S, rows + (size_t)t * S, (size_t)S * sizeof(int4));
+        memcpy(h->host_pose_index.data() + slot * per, index + (size_t)t * per, (size_t)per * sizeof(int32_t));
+        h->n_poses += task_n[t] - h->task_poses[slot];
+        h->task_poses[slot] = task_n[t];
+    }
     return MGB_OK;
 }
 
@@ -2967,18 +3209,20 @@ static int maze_ready(const mgb_maze *h)
     return MGB_OK;
 }
 
-// pose_index + c_fmask + c_vbase -> one PoseRec per (task, cell, heading)
-__global__ void maze_pose_rec_kernel(const int32_t *pose_index, const uint64_t *fmask, const int32_t *vbase, PoseRec *rec, int64_t count)
+// pose_index + c_fmask + c_vbase -> one PoseRec per (task, cell, heading), for the `per` = n * n * 4 entries of each task
+// of the region
+__global__ void maze_pose_rec_kernel(const __grid_constant__ MazeArgs a, PoseRec *rec, int64_t per, int64_t count)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
+    const int64_t k = i / per, idx = (int64_t)a.region[k] * per + (i - k * per);
     PoseRec r;
-    r.slot = pose_index[i]; r.vbase = -1; r.fmask[0] = r.fmask[1] = 0; r.pad = 0;
+    r.slot = a.pose_index[idx]; r.vbase = -1; r.fmask[0] = r.fmask[1] = 0; r.pad = 0;
     if (r.slot >= 0) {
-        r.fmask[0] = fmask[(size_t)r.slot * 2]; r.fmask[1] = fmask[(size_t)r.slot * 2 + 1];
-        if (vbase) r.vbase = vbase[r.slot];
+        r.fmask[0] = a.c_fmask[(size_t)r.slot * 2]; r.fmask[1] = a.c_fmask[(size_t)r.slot * 2 + 1];
+        if (a.c_vbase) r.vbase = a.c_vbase[r.slot];
     }
-    rec[i] = r;
+    rec[idx] = r;
 }
 
 // Raise a kernel's dynamic shared-memory opt-in to everything the device allows next to the kernel's static shared memory.
@@ -3041,12 +3285,10 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
     return MGB_OK;
 }
 
-// (Re)build the pose cache when tasks or textures changed: every free cell x 4 headings of every task is rendered once
-// into its static layers.  Skipped (direct renderer used instead) when disabled or over the memory budget.
-// Bytes of the pose cache of the handle's task table, and whether the cache can serve it: within the budget, and every
-// lit texel fits the 10 bits per channel c_px packs.  Floor and ceiling texels are lit by v_screen / l_focal
-// (ray_caster_utils.py:99,132), up to (half_v - pixel_size / 2) / l_focal; times the brightest texel that can pass 1023 on
-// tall screens, and those screens render directly.
+// Bytes of the pose cache of the handle's task table (slot-strided: n_tasks x S pose slots), and whether the cache can
+// serve it: within the budget, and every lit texel fits the 10 bits per channel c_px packs.  Floor and ceiling texels are
+// lit by v_screen / l_focal (ray_caster_utils.py:99,132), up to (half_v - pixel_size / 2) / l_focal; times the brightest
+// texel that can pass 1023 on tall screens, and those screens render directly.
 static bool pose_cache_fits(const mgb_maze *h, double &bytes)
 {
     const MazeConst &c = h->c;
@@ -3057,6 +3299,80 @@ static bool pose_cache_fits(const mgb_maze *h, double &bytes)
     return bytes <= h->cache_budget_gb * 1e9 && packs;
 }
 
+// screens whose columns are whole 4-pixel groups get signatures, baked all-present frames and (uint8 SURVIVAL) variant frames
+static bool cache_bakes(const MazeConst &c)
+{
+    const size_t px = (size_t)c.res_h * c.res_v;
+    return (c.res_v & 3) == 0 && (px & 127) == 0;
+}
+static bool cache_has_variants(const mgb_maze *h)
+{
+    const MazeConst &c = h->c;
+    return cache_bakes(c) && h->variant_bits > 0 && c.obs_dtype == MGB_OBS_U8 && c.task_type == MGB_MAZE_SURVIVAL &&
+           ((size_t)c.res_h * c.res_v * 3) % 16 == 0;
+}
+
+// The build of the cache region of K tasks (a.region, a bound to the cache), one path for the whole table and for the tasks
+// update_tasks replaced, in two halves around the first build's read-back of c_fmask.  First half: the FILL pass over the
+// n_fill pose slots a.fill_slot lists, then their signatures.  Grids come from host-known sizes (K S, K V); region items a
+// task does not have exit at once.
+static int render_region(mgb_maze *h, const MazeArgs &a, int K, int64_t n_fill, cudaStream_t st)
+{
+    MazeArgs af = a;
+    af.n = n_fill;
+    af.do_step = 0;
+    // the grid depends on K S, not n_fill: the first build (every task) sizes the renderer's scratch for every later region
+    const int64_t span = (int64_t)K * h->pose_stride;
+    int rc = launch_render<true>(h, af, (unsigned)(span < h->num_sms ? span : h->num_sms), st);
+    if (rc) return rc;
+    h->launches += 1;
+    if (cache_bakes(h->c)) {
+        maze3d_sig_kernel<<<(unsigned)n_fill, 256, 0, st>>>(h->c, af);
+        MGB_CUDA(cudaGetLastError());
+        h->launches += 1;
+    }
+    return MGB_OK;
+}
+
+// Second half: variant planning (device), the variant frames' static copies, the all-present bake (compose kernel, one
+// synthetic env per pose slot, every food present), each variant's tints, then the tasks' PoseRec rows.
+static int bake_region(mgb_maze *h, MazePoseCache &pc, MazeArgs a, int K, cudaStream_t st)
+{
+    const MazeConst &c = h->c;
+    const int64_t S = h->pose_stride, V = h->var_stride;
+    a.pose_stride = (int)S; a.var_stride = (int)V; a.var_bits = h->variant_bits_used; a.task_frames = pc.task_frames.get();
+    if (cache_bakes(c)) {
+        if (pc.c_vbase) {
+            maze3d_plan_kernel<<<(unsigned)K, 32, 0, st>>>(a, pc.c_vbase.get(), pc.bake_desc.get(), pc.task_frames.get());
+            MGB_CUDA(cudaGetLastError());
+            MazeArgs av = a;
+            av.bake_desc = pc.bake_desc.get(); av.region_ext = (int)V;
+            maze3d_varinit_kernel<<<(unsigned)(K * V), 256, 0, st>>>(c, av);      // static colours first ...
+            MGB_CUDA(cudaGetLastError());
+            h->launches += 2;
+        }
+        MazeArgs ab = a;
+        ab.bake = 1; ab.do_parts = 1; ab.region_ext = (int)S; ab.n = K * S;
+        maze3d_compose_kernel<true><<<(unsigned)(K * S), kComposeThreads, 0, st>>>(c, ab);
+        MGB_CUDA(cudaGetLastError());
+        h->launches += 1;
+        if (pc.c_vbase) {                                 // ... then each variant's tints
+            ab.region_ext = (int)V; ab.n = K * V;
+            ab.c_rgb8 = pc.c_var8.get(); ab.bake_desc = pc.bake_desc.get();
+            maze3d_compose_kernel<true><<<(unsigned)(K * V), kComposeThreads, 0, st>>>(c, ab);
+            MGB_CUDA(cudaGetLastError());
+            h->launches += 1;
+        }
+    }
+    const int64_t per = (int64_t)c.n * c.n * 4, count = K * per;     // merged per-pose records, after c_fmask and c_vbase
+    maze_pose_rec_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(a, pc.pose_rec.get(), per, count);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
+// (Re)build the pose cache when tasks or textures changed: every free cell x 4 headings of every task is rendered once
+// into its static layers.  Skipped (direct renderer used instead) when disabled or over the memory budget.
 static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
 {
     if (!h->cache_dirty) return MGB_OK;
@@ -3088,116 +3404,79 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     MGB_CUDA(pc.c_gsig.alloc(slots * ((px + 3) / 4)));
     MGB_CUDA(cudaMemsetAsync(pc.c_gsig.get(), 0xFF, slots * ((px + 3) / 4), st));
     MGB_CUDA(pc.c_fmask.alloc(slots * 2 * sizeof(uint64_t)));
+    // screens the 4-pixel-group path cannot take keep an all-ones mask, i.e. never use the baked frame; the others get
+    // every used slot's mask from the signature kernel
+    if (!cache_bakes(c)) MGB_CUDA(cudaMemsetAsync(pc.c_fmask.get(), 0xFF, slots * 2 * sizeof(uint64_t), st));
     if (c.obs_dtype != MGB_OBS_U8) MGB_CUDA(pc.c_px_all.alloc(slots * px * sizeof(uint32_t)));
+    MGB_CUDA(pc.task_frames.alloc((size_t)h->n_tasks * sizeof(int32_t)));
+    MGB_CUDA(cudaMemsetAsync(pc.task_frames.get(), 0, (size_t)h->n_tasks * sizeof(int32_t), st));
+    MGB_CUDA(pc.pose_rec.alloc(h->host_pose_index.size() * sizeof(PoseRec)));
     MGB_CUDA(cudaMemcpy(pc.poses.get(), h->host_poses.data(), slots * sizeof(int4), cudaMemcpyHostToDevice));
     MGB_CUDA(cudaMemcpy(pc.pose_index.get(), h->host_pose_index.data(), h->host_pose_index.size() * sizeof(int32_t),
                         cudaMemcpyHostToDevice));
+    // the region of the whole table: every task slot, every used pose slot
+    const int K = h->n_tasks;
+    const int64_t S = h->pose_stride;
+    std::vector<int32_t> region((size_t)K), fill;
+    for (int t = 0; t < K; ++t) {
+        region[t] = t;
+        for (int j = 0; j < h->task_poses[t]; ++j) fill.push_back((int32_t)(t * S + j));
+    }
+    MgbDev<int32_t> d_region, d_fill;
+    MGB_CUDA(d_region.alloc(region.size() * sizeof(int32_t)));
+    MGB_CUDA(d_fill.alloc(fill.size() * sizeof(int32_t)));
+    MGB_CUDA(cudaMemcpy(d_region.get(), region.data(), region.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    MGB_CUDA(cudaMemcpy(d_fill.get(), fill.data(), fill.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
     MazeArgs a = maze_args(h);
     bind_pose_cache(pc, a);
-    a.n = (int64_t)slots;
-    a.do_step = 0;
-    int rc = launch_render<true>(h, a, (unsigned)(slots < (size_t)h->num_sms ? slots : (size_t)h->num_sms), st);
+    a.region = d_region.get(); a.fill_slot = d_fill.get();
+    int rc = render_region(h, a, K, (int64_t)fill.size(), st);
     if (rc) return rc;
-    // "all present" frames: which foods can change a pose's image at all, and the finished pixels with all of them
-    // present (the compose kernel itself, fed one synthetic env per pose slot).  Screens the 4-pixel-group path cannot
-    // take keep an all-ones mask, i.e. never use the baked frame.
-    std::vector<BakeDesc> descs;
-    if ((c.res_v & 3) == 0 && (px & 127) == 0) {
-        MGB_CUDA(cudaMemsetAsync(pc.c_fmask.get(), 0, slots * 2 * sizeof(uint64_t), st));
-        maze3d_sig_kernel<<<(unsigned)slots, 256, 0, st>>>(c, a);
-        MGB_CUDA(cudaGetLastError());
-        if (pc.c_px_all) MGB_CUDA(cudaMemcpyAsync(pc.c_px_all.get(), pc.c_px.get(), slots * px * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
-        // ---- variant frames: every pose whose image depends on k <= variant_bits foods gets its other 2^k - 1 finished
-        // frames too (the all-visible one is c_rgb8[slot]); bits = the pose's foods in ascending slot order
-        if (h->variant_bits > 0 && c.obs_dtype == MGB_OBS_U8 && c.task_type == MGB_MAZE_SURVIVAL && (px * 3) % 16 == 0) {
-            std::vector<uint64_t> fm(slots * 2);
-            MGB_CUDA(cudaStreamSynchronize(st));
-            MGB_CUDA(cudaMemcpy(fm.data(), pc.c_fmask.get(), slots * 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-            auto popc = [](uint64_t x) { int n = 0; while (x) { x &= x - 1; ++n; } return n; };
-            for (int k = 0; k < 9; ++k) h->k_hist[k] = 0;
-            for (size_t sl = 0; sl < slots; ++sl) {
-                const int k = popc(fm[2 * sl]) + popc(fm[2 * sl + 1]);
-                h->k_hist[k < 8 ? k : 8] += 1;
-            }
-            int bits = h->variant_bits;
-            const double room = h->cache_budget_gb * 1e9 - bytes;
-            size_t frames = 0;
-            for (; bits > 0; --bits) {                     // largest k whose frames fit the cache budget
-                frames = 0;
-                for (size_t sl = 0; sl < slots; ++sl) {
-                    const int k = popc(fm[2 * sl]) + popc(fm[2 * sl + 1]);
-                    if (k >= 1 && k <= bits) frames += ((size_t)1 << k) - 1;
-                }
-                if ((double)frames * (double)(px * 3) <= room) break;
-            }
-            h->variant_bits_used = bits;
-            if (bits > 0 && frames > 0) {
-                std::vector<int32_t> vbase(slots, -1);
-                descs.reserve(frames);
-                for (size_t sl = 0; sl < slots; ++sl) {
-                    const int k = popc(fm[2 * sl]) + popc(fm[2 * sl + 1]);
-                    if (k < 1 || k > bits) continue;
-                    vbase[sl] = (int32_t)descs.size();
-                    for (int v = 0; v < (1 << k) - 1; ++v) {
-                        BakeDesc bd;
-                        bd.slot = (int32_t)sl; bd.pad = 0;
-                        bd.present[0] = ~fm[2 * sl]; bd.present[1] = ~fm[2 * sl + 1];   // foods this pose never shows: irrelevant
-                        int bit = 0;
-                        for (int w = 0; w < 2; ++w) {
-                            uint64_t m = fm[2 * sl + w];
-                            while (m) {
-                                const uint64_t low = m & (~m + 1);
-                                m &= m - 1;
-                                if ((v >> bit) & 1) bd.present[w] |= low;
-                                ++bit;
-                            }
-                        }
-                        descs.push_back(bd);
-                    }
-                }
-                MGB_CUDA(pc.c_vbase.alloc(slots * sizeof(int32_t)));
-                MGB_CUDA(pc.c_var8.alloc(descs.size() * px * 3));
-                MGB_CUDA(pc.bake_desc.alloc(descs.size() * sizeof(BakeDesc)));
-                MGB_CUDA(cudaMemcpy(pc.c_vbase.get(), vbase.data(), slots * sizeof(int32_t), cudaMemcpyHostToDevice));
-                MGB_CUDA(cudaMemcpy(pc.bake_desc.get(), descs.data(), descs.size() * sizeof(BakeDesc), cudaMemcpyHostToDevice));
-                MazeArgs av = a;
-                av.c_var8 = pc.c_var8.get(); av.bake_desc = pc.bake_desc.get();
-                maze3d_varinit_kernel<<<(unsigned)descs.size(), 256, 0, st>>>(c, av);      // static colours first ...
-                MGB_CUDA(cudaGetLastError());
-            }
+    // ---- variant frames: every pose whose image depends on k <= variant_bits foods gets its other 2^k - 1 finished frames
+    // too (the all-visible one is c_rgb8[slot]).  Each task slot gets V frames, V = the most frames a task of this table
+    // needs at the largest bits whose n_tasks x V frames fit the budget; the device plans them per task (maze3d_plan_kernel).
+    h->variant_bits_used = 0;
+    h->var_stride = 0;
+    h->var_planned = cache_has_variants(h);
+    if (h->var_planned) {
+        std::vector<uint64_t> fm(slots * 2);
+        MGB_CUDA(cudaStreamSynchronize(st));
+        MGB_CUDA(cudaMemcpy(fm.data(), pc.c_fmask.get(), slots * 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        std::vector<int64_t> k_tasks((size_t)K * (kVariantBitsMax + 1), 0);     // [task][k] poses depending on k foods
+        for (size_t sl = 0; sl < slots; ++sl) {
+            if (h->host_poses[sl].x < 0) continue;
+            const int k = __builtin_popcountll(fm[2 * sl]) + __builtin_popcountll(fm[2 * sl + 1]);
+            if (k <= kVariantBitsMax) k_tasks[(size_t)(sl / S) * (kVariantBitsMax + 1) + k] += 1;
         }
-        a.bake = 1;
-        a.do_parts = 1;
-        maze3d_compose_kernel<<<(unsigned)slots, kComposeThreads, 0, st>>>(c, a);
-        MGB_CUDA(cudaGetLastError());
-        if (!descs.empty()) {                               // ... then each variant's tints (compose kernel, bake mode)
-            MazeArgs av = a;
-            av.n = (int64_t)descs.size();
-            av.c_rgb8 = pc.c_var8.get(); av.bake_desc = pc.bake_desc.get();
-            maze3d_compose_kernel<<<(unsigned)descs.size(), kComposeThreads, 0, st>>>(c, av);
-            MGB_CUDA(cudaGetLastError());
-            h->launches += 2;
+        int bits = h->variant_bits;
+        const double room = h->cache_budget_gb * 1e9 - bytes;
+        int64_t V = 0;
+        for (; bits > 0; --bits) {                         // largest k whose frames fit the cache budget
+            V = 0;
+            for (int t = 0; t < K; ++t) {
+                int64_t frames = 0;
+                for (int k = 1; k <= bits; ++k) frames += k_tasks[(size_t)t * (kVariantBitsMax + 1) + k] * (((int64_t)1 << k) - 1);
+                V = frames > V ? frames : V;
+            }
+            if ((double)K * (double)V * (double)(px * 3) <= room) break;
         }
-        a.bake = 0;
-        h->launches += 2;
-    } else {
-        MGB_CUDA(cudaMemsetAsync(pc.c_fmask.get(), 0xFF, slots * 2 * sizeof(uint64_t), st));
+        h->variant_bits_used = bits;
+        if (bits > 0 && V > 0) {
+            h->var_stride = V;
+            MGB_CUDA(pc.c_vbase.alloc(slots * sizeof(int32_t)));
+            MGB_CUDA(pc.c_var8.alloc((size_t)K * V * px * 3));
+            MGB_CUDA(pc.bake_desc.alloc((size_t)K * V * sizeof(BakeDesc)));
+            a.c_vbase = pc.c_vbase.get(); a.c_var8 = pc.c_var8.get();
+        }
     }
-    {   // merged per-pose records for the step logic (after c_fmask and c_vbase are final)
-        const int64_t count = (int64_t)h->host_pose_index.size();
-        MGB_CUDA(pc.pose_rec.alloc((size_t)count * sizeof(PoseRec)));
-        maze_pose_rec_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(pc.pose_index.get(), pc.c_fmask.get(),
-                                                                            pc.c_vbase.get(), pc.pose_rec.get(), count);
-        MGB_CUDA(cudaGetLastError());
-    }
+    rc = bake_region(h, pc, a, K, st);
+    if (rc) return rc;
     MGB_CUDA(cudaStreamSynchronize(st));
     h->cache = std::move(pc);
-    h->n_poses = (int64_t)slots;
-    h->n_var_frames = (int64_t)descs.size();
-    h->cache_bytes = bytes + (double)h->n_var_frames * (double)(px * 3);
+    h->n_poses = (int64_t)fill.size();
+    h->cache_bytes = bytes + (double)K * (double)h->var_stride * (double)(px * 3);
     h->cache_ready = true;
     h->cache_dirty = false;
-    h->launches += 1;
     return MGB_OK;
 }
 
@@ -3218,7 +3497,7 @@ static int64_t compose_resident_ctas(mgb_maze *h)
 {
     int &ctas_per_sm = h->compose_ctas_per_sm;
     if (!ctas_per_sm) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, maze3d_compose_kernel, kComposeThreads, 0) !=
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, maze3d_compose_kernel<false>, kComposeThreads, 0) !=
                 cudaSuccess || ctas_per_sm < 1) ctas_per_sm = 4;
     }
     return (int64_t)h->num_sms * ctas_per_sm;
@@ -3272,7 +3551,7 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t s
             int64_t parts = (4 * compose_resident_ctas(h) + h->n - 1) / h->n;   // aim at >= 4 work items per resident CTA
             parts = parts < 1 ? 1 : (parts > 4 ? 4 : parts);
             a.do_parts = (int)parts;
-            maze3d_compose_kernel<<<(unsigned)(h->n * parts), kComposeThreads, 0, st>>>(c, a);   // one CTA per item
+            maze3d_compose_kernel<false><<<(unsigned)(h->n * parts), kComposeThreads, 0, st>>>(c, a);   // one CTA per item
             h->launches += 1;
         } else {
             rc = start_terminal_list(h, a, listed, st);
@@ -3321,7 +3600,7 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
         l.dyn = fin.dyn.get();
         l.do_parts = 16;     // a few frames per step: slices spread each over many CTAs, so the pass costs a slice, not a frame
         const int64_t resident = compose_resident_ctas(h);
-        maze3d_compose_kernel<<<(unsigned)(h->n < resident ? h->n : resident), kComposeThreads, 0, st>>>(h->c, l);
+        maze3d_compose_kernel<false><<<(unsigned)(h->n < resident ? h->n : resident), kComposeThreads, 0, st>>>(h->c, l);
         MGB_CUDA(cudaGetLastError());
     } else {
         l.agent = fin.agent.get(); l.life = fin.life.get(); l.eaten = fin.eaten.get(); l.env2task = fin.task.get();
@@ -4199,7 +4478,7 @@ __global__ void maze_record_path_kernel(int64_t n, int64_t n_pad, int64_t cap, c
 }  // namespace
 
 // Records carry their env's whole task when the env owns its table slot and the table can change on the device
-// (resample_tasks / update_tasks need the direct renderer).  Otherwise the table is shared, and fingerprinted.
+// (resample_tasks needs the direct renderer).  Otherwise the table is shared, and fingerprinted.
 static bool records_carry_tasks(const mgb_maze *h)
 {
     double bytes;

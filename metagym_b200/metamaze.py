@@ -339,7 +339,9 @@ class _BatchedMazeBase(Snapshots):
         """Per-episode task resampling: replace entries `task_slots` of the task table by `task_configs`, stream-ordered
         and without a device synchronisation (mgb_maze_update_tasks).  Envs flying a replaced slot restart on the new task.
         With set_task(tasks) of one task per env (env2task = arange), `update_tasks(env_ids, new_tasks)` re-tasks exactly
-        those envs.  Needs the direct renderer (cache=False / more tasks than the pose-cache budget)."""
+        those envs.  On the pose cache (MetaMazeDiscrete3D) the replaced tasks' poses and frames are rebuilt in place on
+        the stream; there a replacement may not have more free cells (the start cell included) than the largest task
+        set_task was given, and a slot may appear only once per call."""
         slots = np.ascontiguousarray(np.asarray(task_slots, dtype=np.int32).reshape(-1))
         tasks = [task_configs] if hasattr(task_configs, "cell_walls") else list(task_configs)
         K = len(tasks)
@@ -731,7 +733,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs))
 
     def cache_info(self):
-        """Pose-cache statistics (valid after the first reset()/step()): dict(poses, variant_frames, variant_bits, bytes,
+        """Pose-cache statistics (valid after the first reset()/step(); synchronises the device): dict(poses, variant_frames, variant_bits, bytes,
         poses_by_food_count [k = 0..7, >= 8], in_use), and the shared-memory plan of the last direct-renderer launch
         (hits_in_global: crossing lists in a global scratch; pipelined: geometry of the next env under the pixels)."""
         out = (ctypes.c_int64 * 16)()
