@@ -32,7 +32,7 @@ def needs_build():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.inc")) + [os.path.join(ROOT, "include", "mgb200.h")]
+    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(ROOT, "include", "mgb200.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

@@ -1689,9 +1689,264 @@ __global__ void __launch_bounds__(256) maze3d_varinit_kernel(const __grid_consta
 
 constexpr int kComposeThreads = 256;
 
-// Work item = (env, image slice).  Pixels no missing food can tint are copied from the pose's baked all-present frame;
-// the others take the cached static layers (packed colour + in-wall flag, food slot under the pixel, crossing records
-// of the column) through the reference's float64 blend with the env's 128-bit food presence mask.
+// Screen and life-bar constants of a pose-cache frame (the bar's end column is per env: EnvDyn::bar_end)
+struct FrameConst {
+    int H, V, total_px;
+    bool survival;               // SURVIVAL task: food values tint, the life bar is drawn
+    int lb_sx, lb_sy, lb_ey;     // life bar: first column, rows [lb_sy, lb_ey)
+    int px_bytes;                // bytes of one output pixel: 3 (uint8) or 12 (int32 / float32 words)
+    int v_shift;                 // log2(V) when V is a power of two, else -1
+};
+__device__ __forceinline__ FrameConst frame_const(const MazeConst &c)
+{
+    FrameConst f;
+    f.H = c.res_h; f.V = c.res_v; f.total_px = f.H * f.V;
+    f.survival = c.task_type == MGB_MAZE_SURVIVAL;
+    f.lb_sx = trunc_i(c.lb_sx); f.lb_sy = trunc_i(c.lb_sy);
+    f.lb_ey = trunc_i(c.lb_sy + c.lb_w);
+    if (f.lb_ey > f.V) f.lb_ey = f.V;
+    f.px_bytes = c.obs_dtype == MGB_OBS_U8 ? 3 : 12;
+    f.v_shift = (f.V & (f.V - 1)) == 0 ? 31 - __clz(f.V) : -1;
+    return f;
+}
+
+// The cached static layers of one pose and the food values of its task
+struct PoseLayers {
+    const double *fval;          // food values of the task
+    const uint32_t *px;          // packed colour (10 bits per channel) + in-wall flag, per pixel
+    const uint8_t *fid;          // food slot under the pixel, 0xFF: none
+    const uint8_t *colhits;      // transparent crossings per column
+    const HitRec *hits;          // c.max_hits crossing records per column
+};
+__device__ __forceinline__ PoseLayers pose_layers(const MazeConst &c, const MazeArgs &a, const FrameConst &f, const EnvDyn &d)
+{
+    const uint8_t *blob = a.blobs + (int64_t)d.task * c.blob_bytes;
+    return {reinterpret_cast<const double *>(blob + c.off_fval), a.c_px + (size_t)d.slot * f.total_px,
+            a.c_fid + (size_t)d.slot * f.total_px, a.c_colhits + (size_t)d.slot * f.H,
+            reinterpret_cast<const HitRec *>(a.c_hits) + (size_t)d.slot * f.H * c.max_hits};
+}
+
+template <int N>
+struct PixelGroup {
+    int rgb[N][3];
+};
+// N pixels of ONE screen column (pixel q and the N - 1 after it, rows d_v0 ..): cached static colour -> floor/ceiling
+// tint -> crossings of the column -> life bar (ray_caster_utils.py:118-205, maze_discrete_3d.py:118-126).  The channel
+// values are not clamped; the caller packs them.  Each crossing record of the column is loaded once for the N pixels
+// (they share the column), in ascending order, so every pixel sees the blends in the reference's order.  R records are
+// loaded per round trip: 4-pixel groups in the 48-register compose kernels spill with more than one in flight.
+template <int N, int R>
+__device__ __forceinline__ PixelGroup<N> tint_group(const MazeConst &c, const FrameConst &f, const EnvDyn &d, const PoseLayers &L,
+                                                    int q, int d_h, int d_v0)
+{
+    static_assert(N == 1 || N == 4, "a group is one pixel or four");
+    PixelGroup<N> g;
+    auto &rgb = g.rgb;
+    uint32_t w[N], fids;
+    if constexpr (N == 4) {
+        const uint4 w4 = __ldg(reinterpret_cast<const uint4 *>(L.px + q));
+        w[0] = w4.x; w[1] = w4.y; w[2] = w4.z; w[3] = w4.w;
+        fids = __ldg(reinterpret_cast<const uint32_t *>(L.fid + q));
+    } else {
+        w[0] = __ldg(L.px + q);
+        fids = __ldg(L.fid + q);
+    }
+    const int n_hits = L.colhits[d_h];
+    bool mark[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        const int d_v = d_v0 + k, fd = (int)((fids >> (8 * k)) & 0xFFu);
+        rgb[k][0] = (int)(w[k] & 1023u); rgb[k][1] = (int)((w[k] >> 10) & 1023u); rgb[k][2] = (int)((w[k] >> 20) & 1023u);
+        const bool in_wall = (w[k] >> 30) & 1u;
+        mark[k] = false;
+        if (fd != 0xFF && ((d.present[fd >> 6] >> (fd & 63)) & 1ull)) {
+            const double tv = f.survival ? __ldg(L.fval + fd) : 1.0;
+            if (d_v > c.res_v / 2 ? tv > 0.01 : tv > 0) {    // floor tests > 0.01 (:119), ceiling > 0 (:150)
+                if (!in_wall) blend(rgb[k], tv * 0.50 + 0.10);
+                mark[k] = true;
+            }
+        }
+    }
+    if (n_hits > 0 && !(mark[0] && mark[1 % N] && mark[2 % N] && mark[3 % N])) {    // N = 1: mark[0] four times
+        const int4 *hits = reinterpret_cast<const int4 *>(L.hits + (size_t)d_h * c.max_hits);
+        for (int j0 = 0; j0 < n_hits; j0 += R) {                      // R records per round trip
+            int4 raw[R];
+#pragma unroll
+            for (int u = 0; u < R; ++u) raw[u] = __ldg(hits + (j0 + u < n_hits ? j0 + u : n_hits - 1));
+#pragma unroll
+            for (int u = 0; u < R; ++u) {
+                if (j0 + u >= n_hits) break;
+                const double tf = __hiloint2double(raw[u].y, raw[u].x);
+                const int v_s = (int)(int16_t)(raw[u].z & 0xFFFF), v_e = (int)(int16_t)((uint32_t)raw[u].z >> 16), fid = raw[u].w;
+                if (!((d.present[fid >> 6] >> (fid & 63)) & 1ull)) continue;
+#pragma unroll
+                for (int k = 0; k < N; ++k)
+                    if (!mark[k] && d_v0 + k >= v_s && d_v0 + k < v_e) blend(rgb[k], tf);
+            }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        const int d_v = d_v0 + k;
+        if (f.survival && d_h >= f.lb_sx && d_h < d.bar_end && d_v >= f.lb_sy && d_v < f.lb_ey) { rgb[k][0] = 255; rgb[k][1] = 0; rgb[k][2] = 0; }
+    }
+    return g;
+}
+
+// four pixels' channels as 12 uint8 (values above 255 clamp: MGB_OBS_U8)
+__device__ __forceinline__ void pack_u8x4(const int rgb[4][3], uint32_t pk[3])
+{
+    pk[0] = pk[1] = pk[2] = 0u;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) {
+            const int idx = 3 * k + b;
+            pk[idx >> 2] |= (uint32_t)(rgb[k][b] > 255 ? 255 : rgb[k][b]) << (8 * (idx & 3));
+        }
+}
+
+// One compose work item: pixels [q_begin, q_end) of the frame of env state d, into frame e of `obs` (bake mode: pose slot
+// e of the cache).  Pixels no missing food can tint are copied from the pose's baked all-present frame; the others take
+// the cached static layers through tint_group with the env's 128-bit food presence mask.  Called by all kComposeThreads
+// threads of the CTA.  DEFER (rollout kernel: one CTA = one env per step): tinted groups cluster in a few columns, i.e.
+// in a few threads; they are queued in s_slow (total_px / 4 entries, *s_nslow = 0 on entry) and shared out evenly once
+// the copies are done.
+template <bool DEFER>
+__device__ __forceinline__ void compose_item(const MazeConst &c, const MazeArgs &a, const FrameConst &f, const EnvDyn &d,
+                                             void *obs, int64_t e, int q_begin, int q_end, int *s_slow = nullptr,
+                                             int *s_nslow = nullptr)
+{
+    const int V = f.V, total_px = f.total_px;
+    const PoseLayers L = pose_layers(c, a, f, d);
+    const int lb_ex = d.bar_end;
+    uint8_t *gobs = reinterpret_cast<uint8_t *>(obs) + (size_t)e * total_px * f.px_bytes;
+    if (a.bake) gobs = c.obs_dtype == MGB_OBS_U8 ? a.c_rgb8 + (size_t)e * total_px * 3 : nullptr;
+    uint32_t *bake_px = a.bake && c.obs_dtype != MGB_OBS_U8 ? a.c_px_all + (size_t)e * total_px : nullptr;
+    const uint32_t miss_sig = (uint32_t)d.pad & 0xFFu;
+
+    if ((V & 3) == 0 && (total_px & 127) == 0 && (reinterpret_cast<uintptr_t>(a.bake ? (void *)a.c_rgb8 : (void *)gobs) & 15u) == 0) {
+        // G consecutive 4-row groups of one column per thread and iteration (G = 4 when V % 16 == 0, else 1).
+        // FAST PATH: no food that could tint the group(s) is missing -> the baked all-present pixels are final, up to the
+        // life bar, which is drawn last (maze_discrete_3d.py:118-126) and simply overwrites them: uint8 copies G x 12
+        // finished bytes (three 16-byte words when G = 4), int32 unpacks.  Otherwise: 16 B + 4 B in, tint_group.
+        const uint8_t *gsig = a.c_gsig + (size_t)d.slot * (total_px / 4);
+        const uint8_t *g8 = frame_of(a, d, (size_t)total_px * 3);
+        const uint32_t *gall = a.c_px_all + (size_t)d.slot * total_px;
+        bool deferred_pass = false;
+        auto one_group = [&](int q, int d_h, int d_v0, bool slow) {
+            if (a.bake && !slow) return;                     // bake: untinted groups already hold their final value
+            if (!slow) {
+                const bool bar = f.survival && d_h >= f.lb_sx && d_h < lb_ex && d_v0 + 3 >= f.lb_sy && d_v0 < f.lb_ey;
+                if (c.obs_dtype == MGB_OBS_U8) {
+                    const uint32_t *src = reinterpret_cast<const uint32_t *>(g8 + (size_t)q * 3);
+                    uint32_t *dst = reinterpret_cast<uint32_t *>(gobs + (size_t)q * 3);
+                    uint32_t b[3] = {__ldg(src), __ldg(src + 1), __ldg(src + 2)};
+                    if (bar) {
+                        uint8_t px[12];
+                        memcpy(px, b, 12);
+                        for (int k = 0; k < 4; ++k)
+                            if (d_v0 + k >= f.lb_sy && d_v0 + k < f.lb_ey) { px[3 * k] = 255; px[3 * k + 1] = 0; px[3 * k + 2] = 0; }
+                        memcpy(b, px, 12);
+                    }
+                    dst[0] = b[0]; dst[1] = b[1]; dst[2] = b[2];
+                } else {
+                    const uint4 w4 = __ldg(reinterpret_cast<const uint4 *>(gall + q));
+                    int o[12] = {(int)(w4.x & 1023u), (int)((w4.x >> 10) & 1023u), (int)((w4.x >> 20) & 1023u),
+                                 (int)(w4.y & 1023u), (int)((w4.y >> 10) & 1023u), (int)((w4.y >> 20) & 1023u),
+                                 (int)(w4.z & 1023u), (int)((w4.z >> 10) & 1023u), (int)((w4.z >> 20) & 1023u),
+                                 (int)(w4.w & 1023u), (int)((w4.w >> 10) & 1023u), (int)((w4.w >> 20) & 1023u)};
+                    if (bar) {
+                        for (int k = 0; k < 4; ++k)
+                            if (d_v0 + k >= f.lb_sy && d_v0 + k < f.lb_ey) { o[3 * k] = 255; o[3 * k + 1] = 0; o[3 * k + 2] = 0; }
+                    }
+                    int4 *dst = reinterpret_cast<int4 *>(gobs + (size_t)q * 12);
+                    if (c.obs_dtype == MGB_OBS_F32)
+                        for (int k = 0; k < 12; ++k) o[k] = __float_as_int((float)o[k]);
+                    dst[0] = make_int4(o[0], o[1], o[2], o[3]);
+                    dst[1] = make_int4(o[4], o[5], o[6], o[7]);
+                    dst[2] = make_int4(o[8], o[9], o[10], o[11]);
+                }
+                return;
+            }
+            if constexpr (DEFER) {
+                if (!deferred_pass) { s_slow[atomicAdd(s_nslow, 1)] = q; return; }
+            }
+            const PixelGroup<4> g = tint_group<4, 1>(c, f, d, L, q, d_h, d_v0);
+            const auto &rgb = g.rgb;
+            if (c.obs_dtype == MGB_OBS_U8) {
+                uint32_t pk[3];
+                pack_u8x4(rgb, pk);
+                uint32_t *dst = reinterpret_cast<uint32_t *>(gobs + (size_t)q * 3);
+                dst[0] = pk[0]; dst[1] = pk[1]; dst[2] = pk[2];
+            } else if (bake_px) {
+                uint4 pw;
+                pw.x = (uint32_t)rgb[0][0] | ((uint32_t)rgb[0][1] << 10) | ((uint32_t)rgb[0][2] << 20);
+                pw.y = (uint32_t)rgb[1][0] | ((uint32_t)rgb[1][1] << 10) | ((uint32_t)rgb[1][2] << 20);
+                pw.z = (uint32_t)rgb[2][0] | ((uint32_t)rgb[2][1] << 10) | ((uint32_t)rgb[2][2] << 20);
+                pw.w = (uint32_t)rgb[3][0] | ((uint32_t)rgb[3][1] << 10) | ((uint32_t)rgb[3][2] << 20);
+                *reinterpret_cast<uint4 *>(bake_px + q) = pw;
+            } else {
+                int out[12];
+                for (int k = 0; k < 12; ++k) out[k] = MGB_OBS_WORD(c, rgb[k / 3][k % 3]);
+                int4 *dst = reinterpret_cast<int4 *>(gobs + (size_t)q * 12);
+                dst[0] = make_int4(out[0], out[1], out[2], out[3]);
+                dst[1] = make_int4(out[4], out[5], out[6], out[7]);
+                dst[2] = make_int4(out[8], out[9], out[10], out[11]);
+            }
+        };
+        if ((V & 15) == 0 && c.obs_dtype == MGB_OBS_U8) {      // int32: the 4-pixel loop
+            const uint32_t miss4 = miss_sig * 0x01010101u;
+            for (int q = q_begin + threadIdx.x * 16; q < q_end; q += kComposeThreads * 16) {
+                const int d_h = f.v_shift >= 0 ? (q >> f.v_shift) : q / V;
+                const int d_v0 = q - d_h * V;
+                uint32_t hit = 0;
+                if (miss_sig) hit = __ldg(reinterpret_cast<const uint32_t *>(gsig + (q >> 2))) & miss4;
+                const bool bar = f.survival && d_h >= f.lb_sx && d_h < lb_ex && d_v0 + 15 >= f.lb_sy && d_v0 < f.lb_ey;
+                if (!hit && !bar && !a.bake && c.obs_dtype == MGB_OBS_U8) {
+                    const uint4 *src = reinterpret_cast<const uint4 *>(g8 + (size_t)q * 3);
+                    uint4 *dst = reinterpret_cast<uint4 *>(gobs + (size_t)q * 3);
+                    const uint4 x0 = __ldg(src), x1 = __ldg(src + 1), x2 = __ldg(src + 2);
+                    dst[0] = x0; dst[1] = x1; dst[2] = x2;
+                    continue;
+                }
+#pragma unroll 1
+                for (int g = 0; g < 4; ++g) one_group(q + 4 * g, d_h, d_v0 + 4 * g, ((hit >> (8 * g)) & 0xFFu) != 0);
+            }
+        } else {
+            for (int q = q_begin + threadIdx.x * 4; q < q_end; q += kComposeThreads * 4) {
+                const int d_h = f.v_shift >= 0 ? (q >> f.v_shift) : q / V;
+                const int d_v0 = q - d_h * V;
+                bool slow = false;
+                if (miss_sig) slow = (__ldg(gsig + (q >> 2)) & miss_sig) != 0;
+                one_group(q, d_h, d_v0, slow);
+            }
+        }
+        if constexpr (DEFER) {
+            __syncthreads();
+            deferred_pass = true;
+            for (int i = threadIdx.x; i < *s_nslow; i += kComposeThreads) {
+                const int q = s_slow[i];
+                const int d_h = f.v_shift >= 0 ? (q >> f.v_shift) : q / V;
+                one_group(q, d_h, q - d_h * V, true);
+            }
+        }
+    } else {
+        for (int q = q_begin + threadIdx.x; q < q_end; q += kComposeThreads) {
+            const int d_h = q / V, d_v = q - d_h * V;
+            const PixelGroup<1> g = tint_group<1, 4>(c, f, d, L, q, d_h, d_v);
+            const auto &rgb = g.rgb;
+            if (c.obs_dtype == MGB_OBS_U8) {
+                for (int k = 0; k < 3; ++k) gobs[(size_t)q * 3 + k] = (uint8_t)(rgb[0][k] > 255 ? 255 : rgb[0][k]);
+            } else {
+                int32_t *o = reinterpret_cast<int32_t *>(gobs) + (size_t)q * 3;
+                o[0] = MGB_OBS_WORD(c, rgb[0][0]); o[1] = MGB_OBS_WORD(c, rgb[0][1]); o[2] = MGB_OBS_WORD(c, rgb[0][2]);
+            }
+        }
+    }
+}
+
+// Work item = (env, image slice), composed by compose_item.
 // REGION (pose-cache build, bake mode): items are region items (MazeArgs::region) that skip the poses / frames a task
 // does not have; the step's instantiation stays the plain one.
 template <bool REGION>
@@ -1701,12 +1956,8 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
     // persistent CTAs: work item = (env, one of kParts slices of its image); grid = resident CTA count, so there is
     // no partial last wave (1024 envs as 1024 CTAs ran 1.15 waves = almost twice the time of one)
     const int kParts = a.do_parts;      // 1..4 image slices per env, chosen by the host so that items >> resident CTAs
-    const int H = c.res_h, V = c.res_v, total_px = H * V;
-    const bool survival = c.task_type == MGB_MAZE_SURVIVAL;
-    const int lb_sx = trunc_i(c.lb_sx), lb_sy = trunc_i(c.lb_sy);
-    int lb_ey = trunc_i(c.lb_sy + c.lb_w);
-    if (lb_ey > V) lb_ey = V;
-    const int px_bytes = c.obs_dtype == MGB_OBS_U8 ? 3 : 12;
+    const FrameConst f = frame_const(c);
+    const int total_px = f.total_px;
     // slice boundaries stay 128-pixel aligned; the slices cover the frame even when it has fewer pixels than slices
     const int part_px = ((total_px + kParts - 1) / kParts + 127) / 128 * 128;
   // list pass of mgb_maze_step_ex (final_obs set): item = (terminal list entry, slice), frame into final_obs[fin_env[entry]]
@@ -1739,7 +1990,7 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
     const EnvDyn d = d_next;
     if (item + gridDim.x < n_items) d_next = fetch((item + gridDim.x) / kParts);
     if (q_begin >= total_px || (REGION && e < 0)) continue;
-#include "maze_compose_body.inc"
+    compose_item<false>(c, a, f, d, a.obs, e, q_begin, q_end);
   }
 }
 
@@ -1748,7 +1999,7 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
 // the TMA engine.  One CTA per env: thread 0 runs the step logic (action, evaluation rule, auto-reset, pose-cache lookup) and
 // immediately issues bulk copies (cp.async.bulk + mbarrier, 12 KB chunks) of the pose's baked all-present frame into shared
 // memory; as each chunk lands the CTA patches, in shared memory, the few 4-pixel groups a currently missing food can tint
-// (float64 blend of the cached static layers, exactly the compose kernel's slow path) and the life bar, and one bulk store
+// (tint_group: float64 blend of the cached static layers, as in the compose kernel) and the life bar, and one bulk store
 // sends the chunk to `obs`.  The 49 KB of a frame are in flight without passing through registers (the compose kernel's 256
 // threads of dependent 16-byte loads were 48 % long-scoreboard stalls), the separate logic launch and its EnvDyn round trip
 // through global memory are gone, and four CTAs per SM overlap one env's logic latency with the others' copies.
@@ -1756,67 +2007,6 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kStepThreads = 128;
 constexpr int kStepChunkPx = 4096;          // pixels per bulk copy: 12 KB of uint8 RGB
-
-// one tinted 4-pixel group (4 consecutive rows of ONE screen column): cached static colour -> floor/ceiling tint ->
-// crossings of the column -> life bar (ray_caster_utils.py:118-205), packed to 12 uint8 (values above 255 clamp: MGB_OBS_U8).
-// Each crossing record of the column is loaded once for the four pixels (they share the column), in ascending order, so
-// every pixel sees the blends in the reference's order.
-__device__ __forceinline__ void compose_group_u8(const MazeConst &c, const EnvDyn &d, const uint32_t *gpx, const uint8_t *gfid,
-                                                 const uint8_t *colhits, const HitRec *ghits, const double *fval,
-                                                 bool survival, int q, int d_h, int d_v0, int lb_sx, int lb_sy, int lb_ey,
-                                                 uint32_t pk[3])
-{
-    const int V = c.res_v;
-    const uint4 w4 = __ldg(reinterpret_cast<const uint4 *>(gpx + q));
-    const uint32_t f4 = __ldg(reinterpret_cast<const uint32_t *>(gfid + q));
-    const int n_hits = colhits[d_h];
-    const uint32_t w[4] = {w4.x, w4.y, w4.z, w4.w};
-    int rgb[4][3];
-    bool mark[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int d_v = d_v0 + k, f = (int)((f4 >> (8 * k)) & 0xFFu);
-        rgb[k][0] = (int)(w[k] & 1023u); rgb[k][1] = (int)((w[k] >> 10) & 1023u); rgb[k][2] = (int)((w[k] >> 20) & 1023u);
-        const bool in_wall = (w[k] >> 30) & 1u;
-        mark[k] = false;
-        if (f != 0xFF && ((d.present[f >> 6] >> (f & 63)) & 1ull)) {
-            const double tv = survival ? __ldg(fval + f) : 1.0;
-            if (d_v > V / 2 ? tv > 0.01 : tv > 0) {          // floor tests > 0.01 (:119), ceiling > 0 (:150)
-                if (!in_wall) blend(rgb[k], tv * 0.50 + 0.10);
-                mark[k] = true;
-            }
-        }
-    }
-    if (n_hits > 0 && !(mark[0] && mark[1] && mark[2] && mark[3])) {
-        const int4 *hits = reinterpret_cast<const int4 *>(ghits + (size_t)d_h * c.max_hits);
-        for (int j0 = 0; j0 < n_hits; j0 += 4) {                      // four records per round trip
-            int4 raw[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) raw[u] = __ldg(hits + (j0 + u < n_hits ? j0 + u : n_hits - 1));
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                if (j0 + u >= n_hits) break;
-                const double tf = __hiloint2double(raw[u].y, raw[u].x);
-                const int v_s = (int)(int16_t)(raw[u].z & 0xFFFF), v_e = (int)(int16_t)((uint32_t)raw[u].z >> 16), fid = raw[u].w;
-                if (!((d.present[fid >> 6] >> (fid & 63)) & 1ull)) continue;
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    if (!mark[k] && d_v0 + k >= v_s && d_v0 + k < v_e) blend(rgb[k], tf);
-            }
-        }
-    }
-    pk[0] = pk[1] = pk[2] = 0u;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int d_v = d_v0 + k;
-        if (survival && d_h >= lb_sx && d_h < d.bar_end && d_v >= lb_sy && d_v < lb_ey) { rgb[k][0] = 255; rgb[k][1] = 0; rgb[k][2] = 0; }
-#pragma unroll
-        for (int b = 0; b < 3; ++b) {
-            const int idx = 3 * k + b;
-            pk[idx >> 2] |= (uint32_t)(rgb[k][b] > 255 ? 255 : rgb[k][b]) << (8 * (idx & 3));
-        }
-    }
-}
 
 constexpr int kStepBatch = 16;              // envs whose step logic one CTA runs side by side before moving their frames
 constexpr int kStepSlots = 8;               // 12 KB chunk slots of a CTA's shared-memory ring
@@ -1849,16 +2039,12 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
     __shared__ __align__(8) uint64_t s_empty[kStepSlots];
     __shared__ int s_nslow;
     __shared__ uint16_t s_slow[1024];                            // queued tinted groups of one chunk (group index in the chunk)
-    const int H = c.res_h, V = c.res_v, total_px = H * V;
+    const int n_chunks = (c.res_h * c.res_v + kStepChunkPx - 1) / kStepChunkPx;
+    const FrameConst f = frame_const(c);
+    const int V = f.V, total_px = f.total_px;
     const uint32_t frame_bytes = (uint32_t)total_px * 3u;
-    const int n_chunks = (total_px + kStepChunkPx - 1) / kStepChunkPx;
-    const bool survival = c.task_type == MGB_MAZE_SURVIVAL;
-    const int lb_sx = trunc_i(c.lb_sx), lb_sy = trunc_i(c.lb_sy);
-    int lb_ey = trunc_i(c.lb_sy + c.lb_w);
-    if (lb_ey > V) lb_ey = V;
     const int tid = threadIdx.x, lane = tid & 31;
     const bool warp0 = tid < 32;
-    const int v_shift = (V & (V - 1)) == 0 ? 31 - __clz(V) : -1;
     if (tid == 0) {
         for (int k = 0; k < kStepSlots; ++k) { mgb_mbar_init(&s_bar[k], 1); mgb_mbar_init(&s_empty[k], 1); }
         mgb_fence_mbar_init();
@@ -1931,12 +2117,7 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
             uint8_t *gobs = it < B ? reinterpret_cast<uint8_t *>(a.obs) + (size_t)(base + (int64_t)it * gridDim.x) * frame_bytes
                                    : s_dst[it];
             if (!warp0 && !miss_sig) continue;
-            const uint8_t *blob = a.blobs + (int64_t)d.task * c.blob_bytes;
-            const double *fval = reinterpret_cast<const double *>(blob + c.off_fval);
-            const uint32_t *gpx = a.c_px + (size_t)d.slot * total_px;
-            const uint8_t *gfid = a.c_fid + (size_t)d.slot * total_px;
-            const uint8_t *colhits = a.c_colhits + (size_t)d.slot * H;
-            const HitRec *ghits = reinterpret_cast<const HitRec *>(a.c_hits) + (size_t)d.slot * H * c.max_hits;
+            const PoseLayers L = pose_layers(c, a, f, d);
             const uint8_t *gsig = a.c_gsig + (size_t)d.slot * (total_px / 4);
             const uint32_t miss4 = miss_sig * 0x01010101u;
             for (int k = 0; k < n_chunks; ++k) {
@@ -1963,9 +2144,10 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
                     // ... and share them out evenly: float64 blends of the cached static layers over the baked pixels
                     for (int i = t96; i < n_slow; i += 96) {
                         const int q = q0 + 4 * (int)s_slow[i];
-                        const int d_h = v_shift >= 0 ? (q >> v_shift) : q / V;
+                        const int d_h = f.v_shift >= 0 ? (q >> f.v_shift) : q / V;
+                        const PixelGroup<4> g = tint_group<4, 4>(c, f, d, L, q, d_h, q - d_h * V);
                         uint32_t pk[3];
-                        compose_group_u8(c, d, gpx, gfid, colhits, ghits, fval, survival, q, d_h, q - d_h * V, lb_sx, lb_sy, lb_ey, pk);
+                        pack_u8x4(g.rgb, pk);
                         uint32_t *dst = reinterpret_cast<uint32_t *>(s_chunk + (size_t)(q - q0) * 3);
                         dst[0] = pk[0]; dst[1] = pk[1]; dst[2] = pk[2];
                     }
@@ -1977,12 +2159,12 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
                     if (!miss_sig) mgb_mbar_wait(&s_bar[slot], parity);
                     // life bar columns inside this chunk (drawn last, maze_discrete_3d.py:118-126)
                     const int h0 = q0 / V, h1 = (q1 + V - 1) / V;      // columns [h0, h1) intersect the chunk
-                    const int bh0 = lb_sx > h0 ? lb_sx : h0, bh1 = d.bar_end < h1 ? d.bar_end : h1;
-                    if (survival && bh0 < bh1 && lb_sy < lb_ey) {
+                    const int bh0 = f.lb_sx > h0 ? f.lb_sx : h0, bh1 = d.bar_end < h1 ? d.bar_end : h1;
+                    if (f.survival && bh0 < bh1 && f.lb_sy < f.lb_ey) {
                         // one lane per column, rows walked in order: no integer division on the warp that feeds the ring
                         for (int d_h = bh0 + lane; d_h < bh1; d_h += 32) {
                             const int qc = d_h * V - q0;                // the column's first pixel, relative to the chunk
-                            int v0 = lb_sy, v1 = lb_ey;                 // rows whose pixel lies inside [q0, q1)
+                            int v0 = f.lb_sy, v1 = f.lb_ey;             // rows whose pixel lies inside [q0, q1)
                             if (qc + v0 < 0) v0 = -qc;
                             if (qc + v1 > q1 - q0) v1 = q1 - q0 - qc;
                             uint8_t *px = s_chunk + (size_t)(qc + v0) * 3;
@@ -2020,7 +2202,7 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
 // FIN (mgb_maze_rollout_discrete_ex): thread 0 also stores the truncation byte of every (t, env) and, for an env that
 // finished at step t, publishes the EnvDyn of its terminal state in a second slot -- both before env_reset, which clears the
 // food stamps the terminal frame still shows.  The CTA then composes that frame into final_obs + (t n + env) frame, a
-// barrier later the usual observation: one compose body, one deferred-tint queue, two passes.
+// barrier later the usual observation: one compose_item per pass, one deferred-tint queue.
 template <bool FIN>
 __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(const __grid_constant__ MazeConst c,
                                                                             const __grid_constant__ MazeArgs a)
@@ -2030,13 +2212,7 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(cons
     __shared__ EnvDyn s_tdyn;                           // FIN: the terminal state's EnvDyn ...
     __shared__ int s_term;                              // ... valid when 1 (done and final_obs wanted)
     extern __shared__ int s_slow[];                     // total_px / 4 entries: queued tinted groups of the current frame
-    bool deferred_pass = false;
-    const int H = c.res_h, V = c.res_v, total_px = H * V;
-    const bool survival = c.task_type == MGB_MAZE_SURVIVAL;
-    const int lb_sx = trunc_i(c.lb_sx), lb_sy = trunc_i(c.lb_sy);
-    int lb_ey = trunc_i(c.lb_sy + c.lb_w);
-    if (lb_ey > V) lb_ey = V;
-    const int px_bytes = c.obs_dtype == MGB_OBS_U8 ? 3 : 12;
+    const FrameConst f = frame_const(c);
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     for (int64_t env = blockIdx.x; env < a.n; env += gridDim.x) {
         const int task = a.env2task[env];
@@ -2086,20 +2262,11 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(cons
                         __syncthreads();
                     }
                     const EnvDyn d = pass == 0 ? s_tdyn : s_dyn;
-                    const int64_t e = (int64_t)t * a.n + env;         // frame index of the included body
-                    const int q_begin = 0, q_end = total_px;
-#define MGB_COMPOSE_DEFER_SLOW 1
-#define MGB_COMPOSE_OBS dst
-#include "maze_compose_body.inc"
-#undef MGB_COMPOSE_DEFER_SLOW
+                    compose_item<true>(c, a, f, d, dst, (int64_t)t * a.n + env, 0, f.total_px, s_slow, &s_nslow);
                 }
             } else if (a.obs) {
                 const EnvDyn d = s_dyn;
-                const int64_t e = (int64_t)t * a.n + env;             // frame index of the included body
-                const int q_begin = 0, q_end = total_px;
-#define MGB_COMPOSE_DEFER_SLOW 1
-#include "maze_compose_body.inc"
-#undef MGB_COMPOSE_DEFER_SLOW
+                compose_item<true>(c, a, f, d, a.obs, (int64_t)t * a.n + env, 0, f.total_px, s_slow, &s_nslow);
             }
             __syncthreads();                                          // s_dyn is rewritten by the next step
         }
