@@ -113,3 +113,87 @@ def cont_case(g, name):
     d["max_steps"], d["resolution"] = max_steps, (rh, rv)
     d["task"] = task_from_arrays(d["task.walls"], d["task.texts"], d["task.food"], d["task.interval"], d["task.scalars"])
     return d
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# outputs past 32-bit offsets (tests/test_large_index_gpu.py, checked on the CPU by tests/test_large_index_layout.py)
+# ---------------------------------------------------------------------------------------------------------------
+B31, B32, E31 = "byte 2^31", "byte 2^32", "element 2^31"
+
+
+def layout_bytes(T, n, row_bytes):
+    """Bytes of a [T, n, row_bytes] output (T None: [n, row_bytes])."""
+    return (1 if T is None else int(T)) * int(n) * int(row_bytes)
+
+
+def crossings(T, n, row_bytes, elem_bytes):
+    """The boundaries among B31, B32 and E31 (element index 2^31, elements of elem_bytes) that lie inside the output:
+    the offset of its last byte / element is at least the boundary, so a 32-bit offset of that kind wraps there."""
+    total = layout_bytes(T, n, row_bytes)
+    out = set()
+    if total > 1 << 31:
+        out.add(B31)
+    if total > 1 << 32:
+        out.add(B32)
+    if total // elem_bytes > 1 << 31:
+        out.add(E31)
+    return out
+
+
+def straddle_rows(T, n, row_bytes, elem_bytes, seed=0, n_random=12):
+    """(t, env) rows of a [T, n, row_bytes] output (t = 0 throughout when T is None) worth comparing env for env: the row
+    holding each boundary of crossings() and the rows on either side of it, envs 0, 1, n - 2 and n - 1 at the first and
+    the last t, and n_random seeded random rows.  Returns (sorted list of distinct (t, env), {boundary: (t, env) of the
+    row holding it})."""
+    TT, n = (1 if T is None else int(T)), int(n)
+    rows = TT * n
+    held = {}
+    pick = set()
+    for name in sorted(crossings(T, n, row_bytes, elem_bytes)):
+        byte = (1 << 31) * (elem_bytes if name == E31 else 1) if name != B32 else 1 << 32
+        r = byte // row_bytes
+        held[name] = (r // n, r % n)
+        pick.update(q for q in (r - 1, r, r + 1) if 0 <= q < rows)
+    for t in {0, TT - 1}:
+        pick.update(t * n + e for e in (0, 1, n - 2, n - 1) if 0 <= e < n)
+    rs = np.random.RandomState(seed)
+    pick.update(int(r) for r in rs.randint(0, rows, n_random))
+    return sorted((r // n, r % n) for r in pick), held
+
+
+def twin_bases(envs, n, width=3):
+    """env_index_base of the width-env twins that hold every env of `envs` (one twin per env not yet covered; a twin
+    starts one env before the env it is built for, clamped into [0, n - width])."""
+    bases = []
+    for e in sorted(set(int(e) for e in envs)):
+        if any(b <= e < b + width for b in bases):
+            continue
+        bases.append(min(max(e - 1, 0), n - width))
+    return bases
+
+
+# name -> outputs (name, T, n, row_bytes, elem_bytes, boundaries the test exists to cross).  Row sizes: quadrotor
+# velocity_control obs 19 float32; state planes 6 float4 per env of n padded to 128; MetaMaze 3-D 128 x 128 RGB frames
+# (uint8 or int32 words); 2-D view_grid 5 windows of 11 x 11 float32; god views 480 x 480 RGB; the path record
+# [max_steps + 1][n padded to 128] char2.
+QUAD_BIG_N = (1 << 25) + 37
+QUAD_BENCH_N = 4194304
+FRAME_U8, FRAME_I32 = 128 * 128 * 3, 128 * 128 * 3 * 4
+PATH_N = 2200000
+LARGE_SHAPES = {
+    "quad_step_stream": [("obs", None, QUAD_BIG_N, 76, 4, {B31}), ("final_obs", None, QUAD_BIG_N, 76, 4, {B31}),
+                         ("planes", None, (QUAD_BIG_N + 127) // 128 * 128, 96, 16, {B31})],
+    "quad_step_bench": [("obs", None, QUAD_BENCH_N, 76, 4, set())],
+    "quad_rollout": [("obs", 28, QUAD_BENCH_N, 76, 4, {B31, B32, E31}), ("act", 28, QUAD_BENCH_N, 16, 4, set())],
+    "quad_rollout_final": [("obs", 14, QUAD_BENCH_N, 76, 4, {B31, B32}),
+                           ("final_obs", 14, QUAD_BENCH_N, 76, 4, {B31, B32})],
+    "maze3d_step_u8": [("obs", None, 90000, FRAME_U8, 1, {B31, B32, E31}),
+                       ("final_obs", None, 90000, FRAME_U8, 1, {B31, B32, E31})],
+    "maze3d_rollout_u8": [("obs", 12, 8192, FRAME_U8, 1, {B31, B32, E31}),
+                          ("final_obs", 12, 8192, FRAME_U8, 1, {B31, B32, E31})],
+    "maze3d_rollout_i32": [("obs", 6, 8192, FRAME_I32, 4, {B31, B32, E31})],
+    "mazec3d_rollout_u8": [("obs", 12, 8192, FRAME_U8, 1, {B31, B32, E31})],
+    "maze2d_rollout": [("obs", 280, 65536, 11 * 11 * 4, 4, {B31, B32, E31})],
+    "god_view": [("views", None, 6300, 480 * 480 * 3, 1, {B31, B32, E31})],
+    "path": [("path", 1001, (PATH_N + 127) // 128 * 128, 2, 2, {B31, B32, E31})],
+}
