@@ -407,6 +407,28 @@ int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, ui
 int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
                                    void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
                                    uint8_t *truncated_dev, void *stream);
+/* T consecutive steps of a MetaMazeDiscrete3D or MetaMazeContinuous3D handle in ONE launch of the direct renderer (every
+ * frame ray-cast; a discrete handle's pose cache, if any, is not used), optionally giving every env whose episode ends a
+ * freshly drawn maze in the same launch -- the data-generation loop of meta-RL over an endless stream of tasks.
+ *   act_dev: discrete int32 [T][n] in 0..3, continuous float32 [T][n][2]; NULL draws the actions exactly as
+ *   mgb_maze_rollout (discrete) or mgb_maze_rollout_continuous (continuous) do for the same act_seed and step counter,
+ *   written to act_out_dev (same shape) if not NULL.  obs_dev [T][n][res_h][res_v][3], rew_dev [T][n] float64,
+ *   done_dev [T][n] uint8; final_obs_dev / truncated_dev as in mgb_maze_rollout_discrete_ex (NULL: not produced).
+ *   resample_cfg NULL: no resampling; this is then a plain rollout whose outputs and state are bit for bit those of T
+ *   step() calls (discrete) or of mgb_maze_rollout_continuous_ex (continuous).
+ *   resample_cfg set: when env e finishes at step t (done, auto-reset on), it gets the task mgb_maze_resample_tasks(mask
+ *   with only e set, resample_cfg, resample_seed) would give it -- written into its table slot, resample count + 1 -- and
+ *   starts its next episode on it: obs[t][e] is the first frame on the NEW maze, final_obs[t][e] the terminal frame on the
+ *   old one.  That equals, step for step, step_ex + resample_tasks(done) + reset(mask = done) (without the extra render).
+ * Refused (MGB_ERR_ARG, handle untouched): a MetaMaze2D handle, T <= 0, output mirrors or multicast set, final_obs without
+ * auto-reset; with resample_cfg also auto-reset off and every refusal of mgb_maze_resample_tasks (one slot per env, a
+ * discrete handle whose pose cache is in use, the cfg checks) with the same messages.
+ * Advances the step counter by T.  Stream-ordered, no host synchronisation, no allocation after the handle's first
+ * reset(): capturable in a CUDA graph. */
+int mgb_maze_rollout_direct(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
+                            void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                            uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                            void *stream);
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

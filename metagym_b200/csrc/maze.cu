@@ -34,6 +34,11 @@ constexpr int kRenderThreads = 512;
 constexpr int kGeoThreads = 128;            // direct renderer, pipelined: threads that prepare the next env's records
 constexpr int kMaxHitsCap = 2 * kMaxN - 1;   // a ray enters at most 2 n - 1 cells of an n x n grid
 
+// shared-memory workspace of one warp of the task sampler (maze_sample_task): per cell a 32-bit value draw, a 16-bit order
+// entry and a wall/food byte, then one union-find byte per room; rounded up to 16
+constexpr int sampler_ws_bytes(int n) { return (7 * n * n + ((n - 1) / 2) * ((n - 1) / 2) + 15) / 16 * 16; }
+constexpr int kSamplerWsMax = sampler_ws_bytes(kMaxN);
+
 struct TaskHdr {                 // 104 bytes, head of every task blob
     int32_t start[2], goal[2];
     double cell_size, wall_height, agent_height, initial_life, max_life, step_reward, goal_reward;
@@ -62,6 +67,12 @@ struct MazeConst {
     double half_h, half_v, pixel_size;                        // host-computed like ray_caster_utils.py:68-70
     // life bar (maze_discrete_3d.py:42-45)
     double lb_sx, lb_sy, lb_w, lb_l;
+};
+
+struct SamplerCfg {          // mgb_maze_sampler_cfg + derived fields (sampler_cfg)
+    int allow_loops, n_texts, food_interval, cls;
+    double cell_size, wall_height, agent_height, step_reward, goal_reward, food_reward, initial_life, max_life, food_density,
+        crowd_ratio;
 };
 
 struct MazeArgs {
@@ -141,6 +152,15 @@ struct MazeArgs {
     int region_ext;
     int pose_stride, var_stride; // S, V
     int var_bits;                // variant bits of the table: a task takes the largest bits <= var_bits whose frames fit V
+};
+
+// in-launch task resampling (maze3d_kernel<.., RS>, mgb_maze_rollout_direct): an env whose episode ends gets the task
+// mgb_maze_resample_tasks would draw for it.  A parameter of maze3d_kernel after MazeArgs, so that no other kernel's
+// parameter offsets move.
+struct MazeResample {
+    SamplerCfg cfg;
+    uint64_t seed;
+    uint32_t *epoch;             // [n] resample count of every env
 };
 
 struct Env {
@@ -670,12 +690,15 @@ __device__ __forceinline__ void push_terminal_state(const MazeConst &c, const Ma
     if (c.kind == MGB_MAZE_CONTINUOUS_3D) { a.fin_cpos[i] = cp; a.fin_cori[i] = co; }
 }
 
+__device__ __noinline__ void maze_sample_task(const MazeConst &c, const SamplerCfg &sc, uint64_t seed, int64_t genv,
+                                              uint32_t *epoch, uint8_t *ws, uint8_t *b);
+
 // FILL = false: render the observation of every env directly (step logic + ray cast + paint).
 // FILL = true : render the STATIC layers of every cached pose (task, cell, heading) once, at set_task time: colours
 //               before any transparency, the food slot under every floor/ceiling pixel, every POSSIBLE transparent
 //               crossing of every column.  maze3d_compose_kernel then turns a pose + the env's current food state
 //               into the exact observation with integer work only (the float64 geometry is memoised).
-// ROLL = true (FILL = false, continuous maze): T steps per launch.  A work item is (env, t), env-major: a CTA runs
+// ROLL = true (FILL = false, both 3-D kinds): T steps per launch.  A work item is (env, t), env-major: a CTA runs
 //               t = 0..T-1 of env blockIdx.x, then of env blockIdx.x + gridDim.x, ...; so the pipelined order prepares
 //               step t + 1 under the pixels of step t.  The pixel phase reads only its record set's snapshot (transparent
 //               map, pose, life-bar end), never the env state that the next item's step logic is rewriting.
@@ -685,11 +708,20 @@ __device__ __forceinline__ void push_terminal_state(const MazeConst &c, const Ma
 //               env_reset, stores the state and builds the record set of the new episode's first frame for obs[t][env].
 //               The destination travels with the record set; whether a reset item follows is published in shared memory
 //               before the trip's closing barrier, so every thread takes the same next item.
-template <bool FILL, bool ROLL, bool FIN = false>
+// ROLL entry points: mgb_maze_rollout_direct and mgb_maze_rollout_continuous[_ex]; a discrete item reads the action
+//               act[t][env] or draws it like maze3d_rollout_kernel.
+// RS (ROLL only, mgb_maze_rollout_direct with a sampler cfg): an item that resets its env (the item itself, or with FIN its
+//               reset item) first gives the env a new task: warp 0 of the geometry group draws it into the item's tile
+//               buffer (maze_sample_task), copies the tile to the env's table slot and fences the generic writes against
+//               the bulk copies that load the slot later; thread 0 then resets the env on the new tile.  The next item's
+//               tile is requested only after that (sequential mode), since it may be the same env.
+template <bool FILL, bool ROLL, bool FIN = false, bool RS = false>
 __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_constant__ MazeConst c,
-                                                                   const __grid_constant__ MazeArgs a)
+                                                                   const __grid_constant__ MazeArgs a,
+                                                                   const __grid_constant__ MazeResample rs)
 {
     static_assert(!FIN || (ROLL && !FILL), "terminal frames are a rollout output");
+    static_assert(!RS || (ROLL && !FILL), "tasks are resampled in a rollout");
     extern __shared__ __align__(128) uint8_t smem[];
     // list pass (final_obs set): items are the entries of the terminal list the step logic just wrote; a CTA without one
     // leaves before it stages the textures
@@ -736,6 +768,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
     // parity: a slot is rewritten two trips later, after every thread has read it); the destination of record set b is the
     // pointer at s_env2[b] + 6 (bytes 24..31 of the record set's int block)
     int *s_split = s_runctr + 2;
+    uint8_t *s_rsws = smem + off + 144;                                   // RS: the sampler's workspace (sampler_ws_bytes)
 
     const int tid = threadIdx.x;
     // screen-row centre above the horizon, half_v - (d_v + 0.5) * pixel_size: the wall texel's row term (:184), pose independent
@@ -791,9 +824,11 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
         blob_phase ^= 1u << bb;
         // FIN, sequential: when env e finishes here its reset item comes next and needs e's tile, not next_e's; which one is
         // known only after the step logic, so a prefetch of another env waits for it
-        const bool late = FIN && !load_here && !geo_reset && next_e != e;
+        // RS, sequential: the next item may be this env on the task it is about to draw, so every prefetch waits for the draw
+        const bool late = RS ? !load_here : (FIN && !load_here && !geo_reset && next_e != e);
         if (gt == 0 && next_e >= 0 && !late) load_blob(next_e, bb ^ 1);
         const TaskHdr *th = blob_hdr(s_blob);
+        bool rs_env = false;                                             // RS: env e starts an episode on a new task
         // ---- step logic (one thread), then publish agent pose to the CTA
         if (FILL) {
             if (gt == 0) {
@@ -833,8 +868,20 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                         const float csf = (float)th->cell_size;                 // get_loc_grid, maze_base.py:199-202
                         s.gx = (int)(cp[0] / csf); s.gy = (int)(cp[1] / csf);
                         maze_evaluate(c, s_blob, eaten, a.n_pad, s, reward, done);
-                    } else {
+                    } else if (!ROLL) {
                         maze_logic(c, s_blob, eaten, a.n_pad, s, a.act[e], reward, done);
+                    } else {
+                        int action;
+                        if (a.act) action = a.act[o];
+                        else {      // the draw of maze3d_rollout_kernel / maze2d_rollout_kernel
+                            const int64_t genv = a.env_base + e;
+                            const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
+                                                                         a.t_base + (uint32_t)t, MGB_STREAM_ACTION),
+                                                              make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32)));
+                            action = (int)(r.x >> 30);
+                            if (a.act_out) a.act_out[o] = action;
+                        }
+                        maze_logic(c, s_blob, eaten, a.n_pad, s, action, reward, done);
                     }
                     a.rew[o] = reward;
                     a.done[o] = (uint8_t)done;
@@ -843,6 +890,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                     split = FIN && done && a.final_obs && a.auto_reset;
                 }
                 if (done && a.auto_reset && !split) {
+                    rs_env = RS;
                     env_reset(c, s_blob, eaten, a.n_pad, s);
                     if (cont) {
                         cp[0] = (float)(s.gx * th->cell_size + 0.5 * th->cell_size);
@@ -859,7 +907,7 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                     *reinterpret_cast<uint8_t **>(s_env + 6) =
                         reinterpret_cast<uint8_t *>(split ? a.final_obs : a.obs) + (size_t)o * H * V * px_bytes;
                     const int64_t ne = split ? e : next_e;
-                    if (late && ne >= 0) load_blob(ne, bb ^ 1);
+                    if (!RS && late && ne >= 0) load_blob(ne, bb ^ 1);
                 }
             }
             if (cont) {          // publish the pose: position promoted from float32, sin/cos of the float64 heading
@@ -871,6 +919,43 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
             if (ex < 0) { ex += H; if (ex < 0) ex = 0; }
             if (ex > H) ex = H;
             s_env[4] = ex;
+        }
+        if (RS && gt < 32) {
+            // the state just stored and published is the reset on the old task: draw the new one into this item's tile
+            // buffer (pipelined mode: the pixel warps read the other one), then reset and publish again
+            if (__shfl_sync(0xffffffffu, (int)rs_env, 0)) {
+                maze_sample_task(c, rs.cfg, rs.seed, a.env_base + e, rs.epoch + e, s_rsws, s_blob);
+                __syncwarp();
+                uint4 *slot = reinterpret_cast<uint4 *>(const_cast<uint8_t *>(a.blobs) + (size_t)a.env2task[e] * c.blob_bytes);
+                for (int i = gt; i < c.blob_bytes / 16; i += 32) slot[i] = reinterpret_cast<const uint4 *>(s_blob)[i];
+                // the slot (global) and the tile (shared) were written through the generic proxy; later bulk copies read
+                // the slot and overwrite the tile
+                asm volatile("fence.proxy.async;" ::: "memory");
+                __syncwarp();
+                if (gt == 0) {
+                    Env s;
+                    env_reset(c, s_blob, a.eaten + e, a.n_pad, s);
+                    a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
+                    a.life[e] = s.life;
+                    path_store(c, a, e, s);
+                    if (c.kind == MGB_MAZE_CONTINUOUS_3D) {
+                        const float2 p2 = make_float2((float)(s.gx * th->cell_size + 0.5 * th->cell_size),
+                                                      (float)(s.gy * th->cell_size + 0.5 * th->cell_size));
+                        a.cpos[e] = p2; a.cori[e] = 0.0;
+                        s_pose[0] = (double)p2.x; s_pose[1] = (double)p2.y; s_pose[2] = 0.0; s_pose[3] = 1.0;   // heading 0
+                    }
+                    s_env[0] = s.gx; s_env[1] = s.gy; s_env[2] = s.ori; s_env[3] = s.steps;
+                    int ex = trunc_i(c.lb_sx + s.life / th->max_life * c.lb_l);
+                    if (ex < 0) { ex += H; if (ex < 0) ex = 0; }
+                    if (ex > H) ex = H;
+                    s_env[4] = ex;
+                }
+            }
+            // the prefetch the step logic deferred: this env's tile again when its reset item follows, else the next item's
+            if (gt == 0 && late) {
+                const int64_t ne = FIN && s_split[bb] ? e : next_e;
+                if (ne >= 0) load_blob(ne, bb ^ 1);
+            }
         }
         gsync();
         const int gx = s_env[0], gy = s_env[1], ori = s_env[2], steps = s_env[3];
@@ -2401,8 +2486,8 @@ struct mgb_maze {
     int auto_reset = 0;
     bool has_task = false, has_tex = false;
     size_t smem3d = 0;
-    int render_attr_set[4] = {0, 0, 0, 0};   // maze3d_kernel<false / true / rollout / rollout with terminal frames>:
-                                             // shared-memory opt-in raised by this handle
+    int render_attr_set[8] = {};             // maze3d_kernel<false / true / rollout / rollout with terminal frames>, then the
+                                             // two rollouts with resampling (4 + ...): shared-memory opt-in raised by this handle
     int compose_ctas_per_sm = 0;       // occupancy of maze3d_compose_kernel (queried once per handle)
     int num_sms = 0;
     int64_t launches = 0;
@@ -2417,7 +2502,7 @@ struct mgb_maze {
 // entries of one env's path record: an episode ends at steps <= max_steps
 static int64_t path_cap(const mgb_maze *h) { return (int64_t)h->c.max_steps + 1; }
 
-static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
+static size_t maze3d_smem_bytes(const MazeConst &c, bool fill, bool rs = false)
 {
     auto up = [](size_t x, size_t a) { return (x + a - 1) / a * a; };
     size_t off = 0;
@@ -2435,6 +2520,7 @@ static size_t maze3d_smem_bytes(const MazeConst &c, bool fill)
     const size_t px = c.obs_dtype == MGB_OBS_U8 ? 3 : 12;
     off = up(off + (size_t)(kRenderThreads / 32) * (c.obs_dtype == MGB_OBS_U8 ? 2 : 1) * c.run_px * px, 128);
     off += 32 + 128 + 16;
+    if (rs) off += sampler_ws_bytes(c.n);      // maze3d_kernel<.., RS>: one warp's sampler workspace
     return off;
 }
 
@@ -2934,11 +3020,6 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
 // interval where a value is above 1e-3).  The draws themselves are restated exactly in tests/maze_sampler_draws.py, and
 // the tests compare every sampled task with that restatement.
 // ---------------------------------------------------------------------------------------------------------------
-struct SamplerCfg {          // mgb_maze_sampler_cfg + derived fields
-    int allow_loops, n_texts, food_interval, cls;
-    double cell_size, wall_height, agent_height, step_reward, goal_reward, food_reward, initial_life, max_life, food_density,
-        crowd_ratio;
-};
 struct PhiloxStream {
     uint2 key;
     uint4 ctr;
@@ -2961,28 +3042,22 @@ constexpr int kSamplerWarps = 4;
 // lives in shared memory); textures, food values and the food thinning rounds are counter-based per cell -- Philox keyed by
 // (seed; global env, resample count, cell, purpose) -- so the 32 lanes take cells side by side instead of one
 // thread walking them serially (the thinning alone is 20 rounds x n^2 draws).
-__global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(const __grid_constant__ MazeConst c,
-                                                                              const __grid_constant__ MazeArgs a,
-                                                                              uint8_t *blobs, const uint8_t *mask, uint32_t *epoch,
-                                                                              const __grid_constant__ SamplerCfg sc, uint64_t seed)
+namespace {
+// The draw of one env's task by one whole warp (all 32 lanes call it): the resample count *epoch goes up by one and the
+// task is written to the blob b (global memory: the env's table slot; shared memory: a tile that the caller copies there).
+// ws: the warp's workspace of sampler_ws_bytes(n) bytes, 16-byte aligned.  Lane 0 returns after the other lanes.
+__device__ __noinline__ void maze_sample_task(const MazeConst &c, const SamplerCfg &sc, uint64_t seed, int64_t genv,
+                                              uint32_t *epoch, uint8_t *ws, uint8_t *b)
 {
-    __shared__ uint8_t s_walls[kSamplerWarps][kMaxN * kMaxN];      // bit 0 wall, bit 1 food alive
-    __shared__ uint8_t s_parent[kSamplerWarps][((kMaxN - 1) / 2) * ((kMaxN - 1) / 2)];
-    __shared__ uint16_t s_order[kSamplerWarps][kMaxN * kMaxN];
-    __shared__ uint32_t s_val[kSamplerWarps][kMaxN * kMaxN];       // 24-bit draw behind every cell's food value
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t e = (int64_t)blockIdx.x * kSamplerWarps + w;
-    if (e >= a.n) return;                                          // warp-uniform exits: no block-wide barrier below
-    if (mask && !mask[e]) return;
-    uint8_t *walls = s_walls[w];
-    uint8_t *parent = s_parent[w];
-    uint16_t *order = s_order[w];
-    uint32_t *val = s_val[w];
+    const int lane = threadIdx.x & 31;
     const int n = c.n, nn = n * n, m = (n - 1) / 2;
-    const uint32_t ep = epoch[e] + 1u;
+    uint32_t *val = reinterpret_cast<uint32_t *>(ws);               // 24-bit draw behind every cell's food value
+    uint16_t *order = reinterpret_cast<uint16_t *>(ws + 4 * nn);
+    uint8_t *walls = ws + 6 * nn;                                   // bit 0 wall, bit 1 food alive
+    uint8_t *parent = ws + 7 * nn;
+    const uint32_t ep = *epoch + 1u;
     __syncwarp();
-    if (lane == 0) epoch[e] = ep;
-    const int64_t genv = a.env_base + e;
+    if (lane == 0) *epoch = ep;
     const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
     const uint32_t hi = (uint32_t)((uint64_t)genv >> 32);
     // per-cell draws: ctr = (env, resample count, cell, purpose)
@@ -3041,7 +3116,6 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
     }
     __syncwarp();
     // ---- textures + food values, one cell per lane and pass
-    uint8_t *b = blobs + (size_t)a.env2task[e] * c.blob_bytes;
     auto value_of = [&](uint32_t u24) {      // np.clip(food_reward * U, 0.10, food_reward): below 0.10, food_reward wins
         const double v = (double)u24 * (1.0 / 16777216.0) * sc.food_reward;
         const double lo = v < 0.10 ? 0.10 : v;
@@ -3107,6 +3181,22 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
         hd.inv_t2c = 1.0 / t2c;
         *reinterpret_cast<TaskHdr *>(b) = hd;
     }
+}
+}  // namespace
+
+__global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(const __grid_constant__ MazeConst c,
+                                                                              const __grid_constant__ MazeArgs a,
+                                                                              uint8_t *blobs, const uint8_t *mask, uint32_t *epoch,
+                                                                              const __grid_constant__ SamplerCfg sc, uint64_t seed)
+{
+    __shared__ __align__(16) uint8_t s_ws[kSamplerWarps][kSamplerWsMax];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t e = (int64_t)blockIdx.x * kSamplerWarps + w;
+    if (e >= a.n) return;                                          // warp-uniform exits: no block-wide barrier below
+    if (mask && !mask[e]) return;
+    uint8_t *b = blobs + (size_t)a.env2task[e] * c.blob_bytes;
+    maze_sample_task(c, sc, seed, a.env_base + e, epoch + e, s_ws[w], b);
+    if (lane != 0) return;
     // ---- the env starts an episode on its new task (set_task + reset of that env, maze_env.py:44-57)
     Env s;
     env_reset(c, b, a.eaten + e, a.n_pad, s);
@@ -3295,25 +3385,30 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     return MGB_OK;
 }
 
-extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, const mgb_maze_sampler_cfg *cfg, uint64_t seed,
-                                       void *stream)
+// What MGB_REQUIRE does, for a refusal made on behalf of the function `fn`
+static int maze_refuse(const char *fn, const char *msg)
 {
-    MgbRange nvtx_range("mgb_maze_resample_tasks");
-    MGB_REQUIRE(h && cfg, "null argument");
-    MGB_REQUIRE(h->has_task, "call mgb_maze_set_task first (it sizes the task table)");
-    MGB_REQUIRE(h->slot_per_env, "device resampling needs one task-table slot per env (mgb_maze_set_task with n_tasks >= n_envs "
-                                 "and an injective env2task)");
-    MgbDeviceGuard guard(h->device);
-    MazeConst &c = h->c;
-    MGB_REQUIRE(!(c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() && h->cache_would_fit),
-                "device resampling needs the direct renderer: create the env with the pose cache off (cache=False)");
-    MGB_REQUIRE(c.n % 2 == 1 && c.n > 6, "Cell Numbers can only be odd, minimum 7 (maze_task.py:57-58)");
-    MGB_REQUIRE(cfg->step_reward < 0, "step_reward must be < 0 (maze_task.py:59)");
-    MGB_REQUIRE(cfg->agent_height < cfg->wall_height && cfg->agent_height > 0, "the agent height must be > 0 and < wall height");
-    MGB_REQUIRE(cfg->cell_size >= h->min_cell, "resampled tasks may not have smaller cells than the table's smallest");
-    MGB_REQUIRE(cfg->n_texts >= 2 && (c.kind == MGB_MAZE_2D || !h->has_tex || cfg->n_texts <= c.n_tex), "n_texts out of range");
-    MGB_REQUIRE(cfg->food_reward > 0 && cfg->food_density >= 0 && cfg->crowd_ratio >= 0, "invalid sampler parameters");
-    SamplerCfg sc;
+    mgb_set_error("%s: %s", fn, msg);
+    return MGB_ERR_ARG;
+}
+
+// What device resampling needs of the handle and of the sampler cfg (mgb_maze_resample_tasks, mgb_maze_rollout_direct):
+// the refusal, or nullptr with sc derived from cfg
+static const char *sampler_cfg(const mgb_maze *h, const mgb_maze_sampler_cfg *cfg, SamplerCfg &sc)
+{
+    if (!h->has_task) return "call mgb_maze_set_task first (it sizes the task table)";
+    if (!h->slot_per_env)
+        return "device resampling needs one task-table slot per env (mgb_maze_set_task with n_tasks >= n_envs and an injective "
+               "env2task)";
+    const MazeConst &c = h->c;
+    if (c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() && h->cache_would_fit)
+        return "device resampling needs the direct renderer: create the env with the pose cache off (cache=False)";
+    if (!(c.n % 2 == 1 && c.n > 6)) return "Cell Numbers can only be odd, minimum 7 (maze_task.py:57-58)";
+    if (!(cfg->step_reward < 0)) return "step_reward must be < 0 (maze_task.py:59)";
+    if (!(cfg->agent_height < cfg->wall_height && cfg->agent_height > 0)) return "the agent height must be > 0 and < wall height";
+    if (!(cfg->cell_size >= h->min_cell)) return "resampled tasks may not have smaller cells than the table's smallest";
+    if (!(cfg->n_texts >= 2 && (c.kind == MGB_MAZE_2D || !h->has_tex || cfg->n_texts <= c.n_tex))) return "n_texts out of range";
+    if (!(cfg->food_reward > 0 && cfg->food_density >= 0 && cfg->crowd_ratio >= 0)) return "invalid sampler parameters";
     sc.allow_loops = cfg->allow_loops; sc.n_texts = cfg->n_texts; sc.food_interval = cfg->food_interval;
     sc.cell_size = cfg->cell_size; sc.wall_height = cfg->wall_height; sc.agent_height = cfg->agent_height;
     sc.step_reward = cfg->step_reward;
@@ -3323,6 +3418,18 @@ extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, con
     sc.cls = -1;
     for (size_t k = 0; k < h->cls_heights.size() / 2; ++k)
         if (h->cls_heights[2 * k] == cfg->agent_height && h->cls_heights[2 * k + 1] == cfg->wall_height) sc.cls = (int)k;
+    return nullptr;
+}
+
+extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, const mgb_maze_sampler_cfg *cfg, uint64_t seed,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_resample_tasks");
+    MGB_REQUIRE(h && cfg, "null argument");
+    SamplerCfg sc;
+    if (const char *why = sampler_cfg(h, cfg, sc)) return maze_refuse(__func__, why);
+    MgbDeviceGuard guard(h->device);
+    const MazeConst &c = h->c;
     MazeArgs a = maze_args(h);
     maze_sample_tasks_kernel<<<(unsigned)((h->n + kSamplerWarps - 1) / kSamplerWarps), 32 * kSamplerWarps, 0, (cudaStream_t)stream>>>(c, a, h->tasks.blobs.get(), mask_dev, h->task_epoch.get(),
                                                                                         sc, seed);
@@ -3405,8 +3512,8 @@ template <class F> static cudaError_t maze_allow_max_dynamic_smem(F *kernel)
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
 }
 
-template <bool FILL, bool ROLL = false, bool FIN = false>
-static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStream_t st)
+template <bool FILL, bool ROLL = false, bool FIN = false, bool RS = false>
+static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStream_t st, const MazeResample &rs = {})
 {
     MazeConst &c = h->c;
     // shared-memory plan, most wanted first: (direct renderer) two record sets with the crossing lists in shared memory,
@@ -3416,7 +3523,7 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
     for (int k = 0; k < 4; ++k) {
         if (plans[k][0] && (FILL || !h->render_pipe)) continue;
         c.pipe = plans[k][0]; c.hits_in_global = plans[k][1];
-        sm = maze3d_smem_bytes(c, FILL);
+        sm = maze3d_smem_bytes(c, FILL, RS);
         if (sm <= 227 * 1024) break;
     }
     if (sm > 227 * 1024) {
@@ -3441,13 +3548,13 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
     }
     // The opt-in limit is a property of the kernel on a device, shared by every handle: each handle raises it once to the
     // device maximum (the same value from every handle and thread, so there is no ordering to get wrong and no global state).
-    const int attr = FIN ? 3 : (ROLL ? 2 : (FILL ? 1 : 0));
+    const int attr = (RS ? 4 : 0) + (FIN ? 3 : (ROLL ? 2 : (FILL ? 1 : 0)));
     if (!h->render_attr_set[attr]) {
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL, FIN>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL, FIN, RS>));
         h->render_attr_set[attr] = 1;
     }
     h->smem3d = sm;
-    maze3d_kernel<FILL, ROLL, FIN><<<grid, kRenderThreads, sm, st>>>(c, a2);
+    maze3d_kernel<FILL, ROLL, FIN, RS><<<grid, kRenderThreads, sm, st>>>(c, a2, rs);
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -3779,12 +3886,6 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     return MGB_OK;
 }
 
-// What MGB_REQUIRE does, for a refusal made on behalf of the function `fn`
-static int maze_refuse(const char *fn, const char *msg)
-{
-    mgb_set_error("%s: %s", fn, msg);
-    return MGB_ERR_ARG;
-}
 
 // The four single-step entry points: refusals are made as `fn`, with kind_msg for a handle of the other action type
 // (`continuous`: float [n][2] actions of a MGB_MAZE_CONTINUOUS_3D handle; otherwise int32 [n] actions).
@@ -4000,30 +4101,38 @@ extern "C" int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, vo
                 rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
 }
 
-// The continuous-maze rollout entry points; refusals are made as `fn`, with kind_msg for a handle of another kind.
-// With final_obs or truncated: maze3d_kernel<.., FIN>.
-static int rollout_continuous(const char *fn, const char *kind_msg, mgb_maze *h, int32_t T, const float *act_dev,
-                              uint64_t act_seed, float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                              void *final_obs_dev, uint8_t *truncated_dev, void *stream)
+// The rollouts on the direct renderer (maze3d_kernel<false, true, ..>): mgb_maze_rollout_direct (both 3-D kinds) and the
+// continuous-maze entry points.  Refusals are made as `fn`: own() makes the entry point's kind checks (see check_rollout),
+// mirror_msg refuses output mirrors.  act / act_out: int32 [T][n] (discrete) or float32 [T][n][2] (continuous).  With
+// final_obs or truncated: maze3d_kernel<.., FIN>; with rs (the derived sampler cfg): maze3d_kernel<.., RS>.
+template <class Own>
+static int rollout_continuous(const char *fn, const char *mirror_msg, mgb_maze *h, int32_t T, const void *act_dev,
+                              uint64_t act_seed, void *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                              void *final_obs_dev, uint8_t *truncated_dev, const SamplerCfg *rs, uint64_t rs_seed,
+                              void *stream, Own own)
 {
-    int rc = check_rollout(fn, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
-        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
-        return h->c.kind == MGB_MAZE_CONTINUOUS_3D ? nullptr : kind_msg;
-    });
+    int rc = check_rollout(fn, h, T, final_obs_dev, truncated_dev, own);
     if (rc) return rc;
-    if (h->mir.count != 0)
-        return maze_refuse(fn, "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)");
+    if (h->mir.count != 0) return maze_refuse(fn, mirror_msg);
     MgbDeviceGuard guard(h->device);
     MazeArgs a = maze_args(h);
-    a.act_c = act_dev; a.act_out_c = act_out_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    if (h->c.kind == MGB_MAZE_CONTINUOUS_3D) {
+        a.act_c = static_cast<const float *>(act_dev); a.act_out_c = static_cast<float *>(act_out_dev);
+    } else {
+        a.act = static_cast<const int32_t *>(act_dev); a.act_out = static_cast<int32_t *>(act_out_dev);
+    }
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
     a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
+    MazeResample r = {};
+    if (rs) { r.cfg = *rs; r.seed = rs_seed; r.epoch = h->task_epoch.get(); }
     const unsigned grid = (unsigned)(h->n < h->num_sms ? h->n : h->num_sms);
+    const cudaStream_t st = (cudaStream_t)stream;
     if (final_obs_dev || truncated_dev) {
         a.final_obs = final_obs_dev;
         a.truncated = truncated_dev;
-        rc = launch_render<false, true, true>(h, a, grid, (cudaStream_t)stream);
+        rc = rs ? launch_render<false, true, true, true>(h, a, grid, st, r) : launch_render<false, true, true>(h, a, grid, st);
     } else {
-        rc = launch_render<false, true>(h, a, grid, (cudaStream_t)stream);
+        rc = rs ? launch_render<false, true, false, true>(h, a, grid, st, r) : launch_render<false, true>(h, a, grid, st);
     }
     if (rc) return rc;
     h->t_base += (uint32_t)T;
@@ -4031,13 +4140,19 @@ static int rollout_continuous(const char *fn, const char *kind_msg, mgb_maze *h,
     return MGB_OK;
 }
 
+static const char *const kContinuousMirrors =
+    "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)";
+
 extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
                                            float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
                                            void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout_continuous");
-    return rollout_continuous(__func__, "mgb_maze_rollout_continuous needs a MGB_MAZE_CONTINUOUS_3D handle", h, T,
-                              act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream);
+    return rollout_continuous(__func__, kContinuousMirrors, h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev,
+                              nullptr, nullptr, nullptr, 0, stream, [&]() -> const char * {
+        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
+        return h->c.kind == MGB_MAZE_CONTINUOUS_3D ? nullptr : "mgb_maze_rollout_continuous needs a MGB_MAZE_CONTINUOUS_3D handle";
+    });
 }
 
 extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
@@ -4045,9 +4160,29 @@ extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const floa
                                               void *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout_continuous_ex");
-    return rollout_continuous(__func__, "mgb_maze_rollout_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle", h, T,
+    return rollout_continuous(__func__, kContinuousMirrors, h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev,
+                              final_obs_dev, truncated_dev, nullptr, 0, stream, [&]() -> const char * {
+        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
+        return h->c.kind == MGB_MAZE_CONTINUOUS_3D ? nullptr : "mgb_maze_rollout_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle";
+    });
+}
+
+extern "C" int mgb_maze_rollout_direct(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
+                                       void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                                       uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_direct");
+    SamplerCfg sc;
+    return rollout_continuous(__func__, "output mirrors are not implemented for the 3-D rollouts (set_mirrors([]) first)", h, T,
                               act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
-                              stream);
+                              resample_cfg ? &sc : nullptr, resample_seed, stream, [&]() -> const char * {
+        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
+        if (h->c.kind == MGB_MAZE_2D) return "mgb_maze_rollout_direct serves MetaMazeDiscrete3D and MetaMazeContinuous3D";
+        if (!resample_cfg) return nullptr;
+        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";
+        return sampler_cfg(h, resample_cfg, sc);
+    });
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -355,27 +355,41 @@ class _BatchedMazeBase(Snapshots):
         for k, sl in enumerate(slots):
             self.tasks[int(sl)] = tasks[k]
 
-    def resample_tasks(self, mask=None, seed=0, allow_loops=True, cell_size=2.0, wall_height=3.2, agent_height=1.6,
-                       step_reward=-0.01, goal_reward=None, food_reward=0.50, initial_life=1.0, max_life=2.0,
-                       food_density=0.010, food_interval=100, crowd_ratio=0.0, n_texts=7):
-        """Per-episode task resampling on the device (mgb_maze_resample_tasks): every env with mask[e] != 0 (None: all)
-        gets a freshly drawn maze (MazeTaskSampler's keyword arguments and distribution family; counter-based draws keyed
-        by (seed, global env index, resample count)) and restarts on it.  One stream-ordered kernel; typical use:
-        `obs, rew, done, _ = env.step(a); env.resample_tasks(done)`.  Needs set_task() with one table slot per env
-        (env2task = arange) and the direct renderer (cache=False).  goal_reward None is the reference's default
-        -sqrt(n) * n * step_reward; an explicit goal_reward <= 0 raises ValueError, as MazeTaskSampler refuses it."""
+    @staticmethod
+    def _sampler_cfg(seed=0, allow_loops=True, cell_size=2.0, wall_height=3.2, agent_height=1.6, step_reward=-0.01,
+                     goal_reward=None, food_reward=0.50, initial_life=1.0, max_life=2.0, food_density=0.010,
+                     food_interval=100, crowd_ratio=0.0, n_texts=7):
+        """resample_tasks' keyword arguments -> (MazeSamplerCfg, seed), for resample_tasks and rollout(resample=...)."""
         if goal_reward is not None and not goal_reward > 0:
             raise ValueError("goal reward must be > 0")
-        m = None
-        if mask is not None:
-            m = self._torch.as_tensor(mask, device=self.device).to(self._torch.uint8).contiguous()
         cfg = _lib.MazeSamplerCfg()
         cfg.allow_loops, cfg.n_texts, cfg.food_interval = int(bool(allow_loops)), int(n_texts), int(food_interval)
         cfg.cell_size, cfg.wall_height, cfg.agent_height = cell_size, wall_height, agent_height
         cfg.step_reward, cfg.goal_reward = step_reward, (0.0 if goal_reward is None else goal_reward)
         cfg.food_reward, cfg.initial_life, cfg.max_life = food_reward, initial_life, max_life
         cfg.food_density, cfg.crowd_ratio = food_density, crowd_ratio
-        _lib.check(self._lib.mgb_maze_resample_tasks(self._h, _lib.ptr(m), ctypes.byref(cfg), int(seed), self._stream()))
+        return cfg, int(seed)
+
+    def resample_tasks(self, mask=None, seed=0, allow_loops=True, cell_size=2.0, wall_height=3.2, agent_height=1.6,
+                       step_reward=-0.01, goal_reward=None, food_reward=0.50, initial_life=1.0, max_life=2.0,
+                       food_density=0.010, food_interval=100, crowd_ratio=0.0, n_texts=7):
+        """Per-episode task resampling on the device (mgb_maze_resample_tasks): every env with mask[e] != 0 (None: all)
+        gets a freshly drawn maze (MazeTaskSampler's keyword arguments and distribution family; counter-based draws keyed
+        by (seed, global env index, resample count)) and restarts on it.  One stream-ordered kernel.  Needs set_task() with one table slot per env (env2task = arange) and the direct renderer (cache=False).
+        goal_reward None is the reference's default -sqrt(n) * n * step_reward; an explicit goal_reward <= 0 raises
+        ValueError, as MazeTaskSampler refuses it.
+
+        This call renders nothing.  In the loop `obs, rew, done, _ = env.step(a); env.resample_tasks(done)` with
+        auto_reset on, the step has already reset every finished env on its OLD maze, so `obs` shows a re-tasked env in a
+        maze it no longer is in.  For the frame on the new maze, follow with `obs = env.reset(mask=done)` (which renders
+        every env once more), or let the 3-D envs' `rollout(T, resample=dict(seed=..., ...))` draw the new maze inside
+        the rollout, where obs[t] of a finished env already is its first frame on the new maze."""
+        m = None
+        if mask is not None:
+            m = self._torch.as_tensor(mask, device=self.device).to(self._torch.uint8).contiguous()
+        cfg, seed = self._sampler_cfg(seed, allow_loops, cell_size, wall_height, agent_height, step_reward, goal_reward,
+                                      food_reward, initial_life, max_life, food_density, food_interval, crowd_ratio, n_texts)
+        _lib.check(self._lib.mgb_maze_resample_tasks(self._h, _lib.ptr(m), ctypes.byref(cfg), seed, self._stream()))
         self.need_reset = False
 
     def get_tasks(self, task_slots):
@@ -443,8 +457,10 @@ class _BatchedMazeBase(Snapshots):
     _ACT_DTYPE, _ACT_SHAPE, _ACT_HOST_DTYPE = "int32", (), None
     _RECORDS_GIVEN_ACTIONS = True
 
-    def _rollout(self, T, actions, act_seed, want_actions, out, final=False):
-        """final: also produce the "final_obs" / "truncated" entries (through _ROLLOUT_ENTRIES[1])."""
+    def _rollout(self, T, actions, act_seed, want_actions, out, final=False, direct=False, resample=None):
+        """final: also produce the "final_obs" / "truncated" entries (through _ROLLOUT_ENTRIES[1]).  direct (3-D kinds):
+        run mgb_maze_rollout_direct instead, resampling finished envs' tasks when `resample` (resample_tasks' keyword
+        arguments with seed) is given."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -464,6 +480,12 @@ class _BatchedMazeBase(Snapshots):
             a = torch.as_tensor(actions, dtype=act_dtype, device=dev).reshape(act_shape).contiguous()
         args = [_lib.ptr(a), int(act_seed), _lib.ptr(out.get("act") if record else None), _lib.ptr(out.get("obs")),
                 _lib.ptr(out.get("rew")), _lib.ptr(out.get("done"))]
+        if direct:
+            cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+            args += [_lib.ptr(out.get("final_obs") if final else None), _lib.ptr(out.get("truncated") if final else None),
+                     None if cfg is None else ctypes.byref(cfg), seed]
+            _lib.check(self._lib.mgb_maze_rollout_direct(self._h, T, *args, self._stream()))
+            return out
         if final:
             args += [_lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated"))]
         _lib.check(getattr(self._lib, self._ROLLOUT_ENTRIES[final])(self._h, T, *args, self._stream()))
@@ -720,17 +742,24 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         cfg.l_focal, cfg.text_size = 0.20, 1.0                                # maze_discrete_3d.py:116
         return cfg
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False):
-        """T steps in one launch on the pose cache: obs [T,N,res_h,res_v,3] (uint8, int32 or float32), rew, done, act as
-        for BatchedMetaMaze2D.rollout.
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False, resample=None):
+        """T steps in one launch: obs [T,N,res_h,res_v,3] (uint8, int32 or float32), rew, done, act as for
+        BatchedMetaMaze2D.rollout.  Runs on the pose cache, or on the direct raycaster (mgb_maze_rollout_direct) for an
+        env created with cache=False or when `resample` is given; both give the same results.
 
         final_obs (per call, independent of the constructor's final_obs, which concerns step()): False returns only the
         entries above.  True needs auto_reset=True (ValueError otherwise) and calls mgb_maze_rollout_discrete_ex: the
         dict also holds "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e
         if done[t, e] (what step() reports as final_observation; allocated with torch.empty, rows with done 0 are not
         written), and "truncated" [T,N] uint8, written for every step: 1 iff done and the episode ended only through
-        max_steps.  A caller-supplied `out` may omit either entry, and that output is then not produced."""
-        return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs))
+        max_steps.  A caller-supplied `out` may omit either entry, and that output is then not produced.
+
+        resample: None, or resample_tasks' keyword arguments with its seed, e.g. dict(seed=5, crowd_ratio=0.35).  Every
+        env whose episode ends at step t then gets the maze resample_tasks(done, **resample) would give it, in the same
+        launch: obs[t] is its first frame on the new maze, final_obs[t] the terminal frame on the old one.  Needs
+        auto_reset=True, cache=False and set_task() with one table slot per env, like resample_tasks."""
+        return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs),
+                             direct=resample is not None or self.cache is False, resample=resample)
 
     def cache_info(self):
         """Pose-cache statistics (valid after the first reset()/step(); synchronises the device): dict(poses, variant_frames, variant_bits, bytes,
@@ -773,7 +802,7 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         cfg.kind = 2
         return cfg
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False, resample=None):
         """T steps in one launch of the direct renderer (mgb_maze_rollout_continuous), exactly as T step() calls.
         actions: anything reshapeable to [T,N,2] (turn_rate, walk_speed), clipped to [-1, 1] like step(); None draws them
         on the device, uniform on [-1, 1) like action_space.sample().  Returns dict(obs [T,N,res_h,res_v,3] in the env's
@@ -783,8 +812,12 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         auto_reset=True (ValueError otherwise) and calls mgb_maze_rollout_continuous_ex: the dict also holds
         "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e if done[t, e]
         (allocated with torch.empty, rows with done 0 are not written), and "truncated" [T,N] uint8, written for every
-        step.  A caller-supplied `out` may omit either entry, and that output is then not produced."""
-        return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs))
+        step.  A caller-supplied `out` may omit either entry, and that output is then not produced.
+
+        resample: as for BatchedMetaMazeDiscrete3D.rollout (mgb_maze_rollout_direct): every env whose episode ends at
+        step t gets a freshly drawn maze in the same launch, and obs[t] is its first frame on it."""
+        return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs),
+                             direct=resample is not None, resample=resample)
 
     def pose(self):
         """-> (pos [N,2] float32 = _agent_loc, ori [N] float64 = _agent_ori)."""
