@@ -375,6 +375,22 @@ int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t
 int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
                                  void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
                                  uint8_t *truncated_dev, void *stream);
+/* mgb_maze_rollout_ex of a MetaMaze2D handle that gives every env whose episode ends a freshly drawn maze in the same
+ * launch -- the meta-RL data loop over an endless stream of tasks.  Actions (given or drawn) and the outputs (any may be
+ * NULL) are those of mgb_maze_rollout_ex.  When env e finishes at step t, its reward, done, truncated[t][e] and the
+ * terminal window final_obs[t][e] come from the old task; then it gets the task mgb_maze_resample_tasks(mask with only e
+ * set, resample_cfg, resample_seed) would give it -- written into its table slot, resample count + 1 -- and starts its next
+ * episode on it (start cell, initial_life, every food present): obs[t][e] is its first window on the NEW maze.  That equals,
+ * step for step, step_ex + resample_tasks(done) + reset(mask = done).
+ * Refused (MGB_ERR_ARG, handle untouched): a 3-D handle (use mgb_maze_rollout_direct), T <= 0, resample_cfg NULL,
+ * auto-reset off, output mirrors or multicast set, shared memory per CTA (two tiles of 128 windows plus four sampler
+ * workspaces) beyond the device's opt-in limit (n = 31 needs view_grid <= 6), and every refusal of
+ * mgb_maze_resample_tasks (one slot per env, the cfg checks) with the same messages.
+ * Advances the step counter by T.  Stream-ordered, no host synchronisation, no allocation: capturable in a CUDA graph. */
+int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
+                              void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                              uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                              void *stream);
 
 /* MetaMazeContinuous3D.step (maze_env.py:129-146 -> maze_continuous_3d.py:47-56, dynamics.py:58-92): act_dev [n][2]
  * float32 = (turn_rate, walk_speed), clipped to [-1, 1] like the reference; ten 10 ms sub-steps of turn/walk with the

@@ -103,6 +103,8 @@ SIGNATURES = {
     "mgb_maze_rollout_continuous_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_rollout_direct": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp,
                                                ctypes.POINTER(MazeSamplerCfg), c_u64, vp]),
+    "mgb_maze_rollout_resample": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp,
+                                                 ctypes.POINTER(MazeSamplerCfg), c_u64, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

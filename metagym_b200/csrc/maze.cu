@@ -36,7 +36,7 @@ constexpr int kMaxHitsCap = 2 * kMaxN - 1;   // a ray enters at most 2 n - 1 cel
 
 // shared-memory workspace of one warp of the task sampler (maze_sample_task): per cell a 32-bit value draw, a 16-bit order
 // entry and a wall/food byte, then one union-find byte per room; rounded up to 16
-constexpr int sampler_ws_bytes(int n) { return (7 * n * n + ((n - 1) / 2) * ((n - 1) / 2) + 15) / 16 * 16; }
+__host__ __device__ constexpr int sampler_ws_bytes(int n) { return (7 * n * n + ((n - 1) / 2) * ((n - 1) / 2) + 15) / 16 * 16; }
 constexpr int kSamplerWsMax = sampler_ws_bytes(kMaxN);
 
 struct TaskHdr {                 // 104 bytes, head of every task blob
@@ -154,14 +154,17 @@ struct MazeArgs {
     int var_bits;                // variant bits of the table: a task takes the largest bits <= var_bits whose frames fit V
 };
 
-// in-launch task resampling (maze3d_kernel<.., RS>, mgb_maze_rollout_direct): an env whose episode ends gets the task
-// mgb_maze_resample_tasks would draw for it.  A parameter of maze3d_kernel after MazeArgs, so that no other kernel's
-// parameter offsets move.
+// in-launch task resampling (maze3d_kernel<.., RS>, mgb_maze_rollout_direct; maze2d_rollout_kernel<0, .., RS>,
+// mgb_maze_rollout_resample): an env whose episode ends gets the task mgb_maze_resample_tasks would draw for it.  A
+// parameter of those kernels after MazeArgs, so that no other parameter offsets move.
 struct MazeResample {
     SamplerCfg cfg;
     uint64_t seed;
     uint32_t *epoch;             // [n] resample count of every env
 };
+
+__device__ __noinline__ void maze_sample_task(const MazeConst &c, const SamplerCfg &sc, uint64_t seed, int64_t genv,
+                                              uint32_t *epoch, uint8_t *ws, uint8_t *b);
 
 struct Env {
     int gx, gy, ori, steps;
@@ -489,10 +492,19 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // also store the truncation byte of every (t, e), and the terminal window of every env that finished at step t to
 // final_obs + (t n + e) D, both before env_reset; rows of envs that did not finish are not written.  REC: path recording on
 // (a.path set); the instantiations without it have no store and no test of a.path in their loop.
-template <int XM, bool FIN, bool REC>
+// RS (XM == 0 only, mgb_maze_rollout_resample): an env that finishes at step t gets the task mgb_maze_resample_tasks would
+// draw for it (after its reward, done, truncation byte and terminal window, all on the old task) and restarts on it, so
+// obs[t] is its first window on the new maze.  The sampler is warp-collective: the done ballot is taken by all 32 lanes
+// (the tail warp's lanes past n included), the warp draws one task per finished lane in lane order into that lane's table
+// slot with its workspace behind the two tiles, and after a __syncwarp each owner resets on its new blob.  Each warp then
+// publishes its own 32 rows of the tile with its own bulk store, so no step waits at a CTA barrier for another warp's
+// carving.
+template <int XM, bool FIN, bool REC, bool RS = false>
 __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid_constant__ MazeConst c,
-                                                                    const __grid_constant__ MazeArgs a)
+                                                                    const __grid_constant__ MazeArgs a,
+                                                                    const __grid_constant__ MazeResample rs)
 {
+    static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
     const int64_t e0 = (int64_t)blockIdx.x * k2dThreads;
     const int64_t e = e0 + threadIdx.x;
@@ -516,8 +528,13 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
     const int n = c.n, g = c.view_grid;
     for (int t = 0; t < a.T; ++t) {
         float *tile = tile2d + (size_t)(t & 1) * k2dThreads * D;
-        if (threadIdx.x == 0) mgb_bulk_wait_read<1>();      // the store issued two steps ago has read this tile
-        __syncthreads();
+        if constexpr (RS) {                                 // per warp: the warp's rows and their store are its own
+            if ((threadIdx.x & 31) == 0) mgb_bulk_wait_read<1>();
+            __syncwarp();
+        } else {
+            if (threadIdx.x == 0) mgb_bulk_wait_read<1>();  // the store issued two steps ago has read this tile
+            __syncthreads();
+        }
         uint32_t done_byte = 0;
         if (active) {
             int action;
@@ -571,12 +588,54 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
                 if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
             }
         }
+        if constexpr (RS) {
+            // auto-reset is on (the host requires it).  The step above left every finished env reset on its old task, with
+            // that task's window in the tile and its path entry 0 stored; that step code stays as the other instantiations
+            // compile it, and the few finished envs redo the three on the new task here.
+            uint32_t fin = __ballot_sync(0xffffffffu, done_byte != 0);
+            if (fin) {
+                uint8_t *ws = reinterpret_cast<uint8_t *>(tile2d + 2 * k2dThreads * D) +
+                              (threadIdx.x >> 5) * sampler_ws_bytes(c.n);
+                const int64_t lane0_env = e - (threadIdx.x & 31);
+                for (; fin; fin &= fin - 1) {
+                    const int64_t el = lane0_env + (__ffs(fin) - 1);
+                    maze_sample_task(c, rs.cfg, rs.seed, a.env_base + el, rs.epoch + el, ws,
+                                     const_cast<uint8_t *>(a.blobs) + (int64_t)a.env2task[el] * c.blob_bytes);
+                }
+                __syncwarp();   // the new blobs, written by every lane, are read by their owners below
+                if (done_byte) {
+                    env_reset(c, blob, eaten, a.n_pad, s);
+                    if (REC) path_store(c, a, e, s);
+                    if (a.obs) maze2d_window(c, blob, eaten, a.n_pad, s, tile + threadIdx.x * D);
+                }
+            }
+        }
         if (XM == 2) {
             if (a.done) mgb_mc_st_bytes(mgb_shift(a.done + (int64_t)t * a.n + e, a.mir.delta[0]), done_byte, active);
             if (a.obs) {
                 __syncthreads();
                 mgb_mc_copy_tile(mgb_shift(reinterpret_cast<float *>(a.obs) + ((int64_t)t * a.n + e0) * D, a.mir.delta[0]),
                                  tile, (uint32_t)rows * (uint32_t)D * 4u);
+            }
+        } else if constexpr (RS) {
+            // the warp's rows: 32 D 4 bytes, a multiple of 16, except in the tail warp
+            const int w0 = threadIdx.x & ~31, lane = threadIdx.x & 31;
+            const int wrows = rows - w0 < 32 ? rows - w0 : 32;
+            if (a.obs && wrows > 0) {
+                float *dst = reinterpret_cast<float *>(a.obs) + ((int64_t)t * a.n + e0 + w0) * D;
+                const float *src = tile + w0 * D;
+                const uint32_t bytes = (uint32_t)wrows * (uint32_t)D * 4u;
+                if ((bytes & 15u) == 0 && ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0)) {
+                    mgb_fence_proxy_async();
+                    __syncwarp();
+                    if (lane == 0) {
+                        mgb_bulk_store(dst, src, bytes);
+                        mgb_bulk_commit();
+                    }
+                } else {
+                    __syncwarp();
+                    for (int i = lane; i < wrows * D; i += 32) dst[i] = src[i];
+                }
             }
         } else if (a.obs) {
             float *dst = reinterpret_cast<float *>(a.obs) + ((int64_t)t * a.n + e0) * D;
@@ -602,7 +661,11 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
     }
-    if (threadIdx.x == 0) mgb_bulk_wait_read<0>();
+    if constexpr (RS) {
+        if ((threadIdx.x & 31) == 0) mgb_bulk_wait_read<0>();
+    } else {
+        if (threadIdx.x == 0) mgb_bulk_wait_read<0>();
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -689,9 +752,6 @@ __device__ __forceinline__ void push_terminal_state(const MazeConst &c, const Ma
     for (int f = 0; f < c.f_max; ++f) a.fin_eaten[f * a.n_pad + i] = eaten[f * a.n_pad];
     if (c.kind == MGB_MAZE_CONTINUOUS_3D) { a.fin_cpos[i] = cp; a.fin_cori[i] = co; }
 }
-
-__device__ __noinline__ void maze_sample_task(const MazeConst &c, const SamplerCfg &sc, uint64_t seed, int64_t genv,
-                                              uint32_t *epoch, uint8_t *ws, uint8_t *b);
 
 // FILL = false: render the observation of every env directly (step logic + ray cast + paint).
 // FILL = true : render the STATIC layers of every cached pose (task, cell, heading) once, at set_task time: colours
@@ -3940,21 +4000,33 @@ static int check_rollout(const char *fn, const mgb_maze *h, int32_t T, const voi
     return maze_ready(h);
 }
 
-// maze2d_rollout_kernel<xm, fin, REC> over the handle's envs (xm: 0 plain, 1 peer mirrors, 2 multicast; fin: XM 0 only)
+// maze2d_rollout_kernel<xm, fin, REC> over the handle's envs (xm: 0 plain, 1 peer mirrors, 2 multicast; fin: XM 0 only);
+// with rs (xm 0 only): maze2d_rollout_kernel<0, fin, REC, true>, whose sm includes the sampler workspaces
 template <bool REC>
 static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArgs &a, unsigned blocks, size_t sm,
-                             cudaStream_t st)
+                             cudaStream_t st, const MazeResample *rs = nullptr)
 {
+    if (rs) {
+        if (sm > 48 * 1024) {
+            MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false, REC, true>));
+            MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC, true>));
+        }
+        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs);
+        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs);
+        MGB_CUDA(cudaGetLastError());
+        return MGB_OK;
+    }
     if (sm > 48 * 1024) {
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false, REC>));
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<1, false, REC>));
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<2, false, REC>));
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC>));
     }
-    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
-    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
-    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
-    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a);
+    const MazeResample none = {};
+    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
+    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
+    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
+    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -4060,6 +4132,52 @@ extern "C" int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_
         if (h->c.kind != MGB_MAZE_DISCRETE_3D) return "mgb_maze_rollout_discrete_ex needs a MGB_MAZE_DISCRETE_3D handle";
         return nullptr;
     });
+}
+
+extern "C" int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
+                                         int32_t *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                         void *final_obs_dev, uint8_t *truncated_dev,
+                                         const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_resample");
+    SamplerCfg sc;
+    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
+        if (h->c.kind != MGB_MAZE_2D)
+            return "mgb_maze_rollout_resample serves MetaMaze2D (the 3-D envs resample in mgb_maze_rollout_direct)";
+        if (!resample_cfg) return "null argument: resample_cfg is required";
+        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";
+        if (h->mir.count != 0)
+            return "output mirrors and multicast are not implemented for the resampling rollout (set_mirrors([]) first)";
+        return sampler_cfg(h, resample_cfg, sc);
+    });
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    // two observation tiles, then one sampler workspace per warp (16-byte multiples)
+    const int W = 2 * h->c.view_grid + 1;
+    const size_t sm = (size_t)2 * k2dThreads * W * W * 4 + (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
+    int optin = 0;
+    MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    if (sm > (size_t)optin) {
+        mgb_set_error("%s: the resampling rollout needs %zu bytes of shared memory per CTA at n = %d and view_grid = %d, "
+                      "more than the %d the device allows (use a smaller view_grid)", __func__, sm, h->c.n, h->c.view_grid,
+                      optin);
+        return MGB_ERR_ARG;
+    }
+    MazeArgs a = maze_args(h);
+    a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base; a.act_out = act_out_dev;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+    MazeResample r = {};
+    r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
+    const bool fin = final_obs_dev || truncated_dev;
+    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
+    const cudaStream_t st = (cudaStream_t)stream;
+    rc = h->path ? launch_2d_rollout<true>(h->c, 0, fin, a, blocks, sm, st, &r)
+                 : launch_2d_rollout<false>(h->c, 0, fin, a, blocks, sm, st, &r);
+    if (rc) return rc;
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return MGB_OK;
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)

@@ -382,7 +382,7 @@ class _BatchedMazeBase(Snapshots):
         This call renders nothing.  In the loop `obs, rew, done, _ = env.step(a); env.resample_tasks(done)` with
         auto_reset on, the step has already reset every finished env on its OLD maze, so `obs` shows a re-tasked env in a
         maze it no longer is in.  For the frame on the new maze, follow with `obs = env.reset(mask=done)` (which renders
-        every env once more), or let the 3-D envs' `rollout(T, resample=dict(seed=..., ...))` draw the new maze inside
+        every env once more), or let `rollout(T, resample=dict(seed=..., ...))` (every env kind) draw the new maze inside
         the rollout, where obs[t] of a finished env already is its first frame on the new maze."""
         m = None
         if mask is not None:
@@ -460,7 +460,7 @@ class _BatchedMazeBase(Snapshots):
     def _rollout(self, T, actions, act_seed, want_actions, out, final=False, direct=False, resample=None):
         """final: also produce the "final_obs" / "truncated" entries (through _ROLLOUT_ENTRIES[1]).  direct (3-D kinds):
         run mgb_maze_rollout_direct instead, resampling finished envs' tasks when `resample` (resample_tasks' keyword
-        arguments with seed) is given."""
+        arguments with seed) is given.  MetaMaze2D with `resample`: mgb_maze_rollout_resample."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -480,11 +480,12 @@ class _BatchedMazeBase(Snapshots):
             a = torch.as_tensor(actions, dtype=act_dtype, device=dev).reshape(act_shape).contiguous()
         args = [_lib.ptr(a), int(act_seed), _lib.ptr(out.get("act") if record else None), _lib.ptr(out.get("obs")),
                 _lib.ptr(out.get("rew")), _lib.ptr(out.get("done"))]
-        if direct:
+        if direct or resample is not None:
             cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
             args += [_lib.ptr(out.get("final_obs") if final else None), _lib.ptr(out.get("truncated") if final else None),
                      None if cfg is None else ctypes.byref(cfg), seed]
-            _lib.check(self._lib.mgb_maze_rollout_direct(self._h, T, *args, self._stream()))
+            entry = self._lib.mgb_maze_rollout_direct if direct else self._lib.mgb_maze_rollout_resample
+            _lib.check(entry(self._h, T, *args, self._stream()))
             return out
         if final:
             args += [_lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated"))]
@@ -683,7 +684,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         cfg.n_cells, cfg.max_steps, cfg.view_grid = n_cells, self.max_steps, self.view_grid
         return cfg
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, resample=None):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
         {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None).
 
@@ -691,8 +692,14 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         terminal window of env e where done[t, e] (what step() reports as final_observation); it is allocated with
         torch.empty, and rows with done 0 are not written, so they hold whatever the buffer held.  And "truncated"
         [T,N] uint8, written for every step: 1 iff done and the episode ended only through max_steps.  A
-        caller-supplied `out` may omit either entry, and that output is then not produced."""
-        return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final)
+        caller-supplied `out` may omit either entry, and that output is then not produced.
+
+        resample: None, or resample_tasks' keyword arguments with its seed, e.g. dict(seed=5, crowd_ratio=0.35)
+        (mgb_maze_rollout_resample).  Every env whose episode ends at step t then gets the maze resample_tasks(done,
+        **resample) would give it, in the same launch: obs[t] is its first window on the new maze, final_obs[t] the
+        terminal window on the old one.  Needs auto_reset=True and set_task() with one table slot per env, like
+        resample_tasks; with n = 31 the view_grid may be at most 6."""
+        return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
 
     def save_trajectory(self, file_name, envs=None, additional=None):
         """MetaMaze2D.save_trajectory(file_name, additional) (maze_env.py:211-212), file names as for the 3-D envs.
