@@ -156,6 +156,48 @@ int mgb_quad_rollout_ex(mgb_quad *h, int32_t T, const float *act_dev, uint64_t a
                         float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
                         void *stream);
 
+/* ---- policy-driven rollouts (DESIGN.md "Policy-driven rollouts") ------------------------------------------------
+ * A multi-layer perceptron evaluated inside the rollout launch: the action of step t is drawn from the policy's output
+ * on the observation the env holds before step t.
+ *   params_dev: float32 on the handle's device, read at every launch (so a captured graph sees an in-place update).
+ *     Layers in torch.nn.Linear order, first hidden layer to output layer: W [out][in] row-major, then b [out].  The
+ *     input width is the obs dim, the output width 4.  The quadrotor buffer then ends with log_std [4].
+ *   n_hidden 0..3, width[k] 1..64 for k < n_hidden, activation MGB_ACT_* (every hidden layer), mode MGB_POLICY_*.
+ *   The maze buffer has no log_std: its four outputs are the logits of the actions 0..3.
+ * Numerical contract: float32 throughout, each output a fused multiply-add chain from the bias over the inputs in index
+ * order, accurate tanhf / expf / logf (no approximate instructions, no tensor cores).  Draws: Philox4x32-10, counter
+ * (genv lo, genv hi, t_base + t, MGB_STREAM_POLICY = 0x400), key = seed. */
+#define MGB_ACT_TANH 0
+#define MGB_ACT_RELU 1
+#define MGB_POLICY_SAMPLE 0   /* stochastic: Gaussian (quadrotor) / categorical (maze 2-D) */
+#define MGB_POLICY_MEAN 1     /* deterministic: the mean (quadrotor) / argmax of the logits (maze 2-D) */
+#define MGB_POLICY_MAX_HIDDEN 3
+#define MGB_POLICY_MAX_WIDTH 64
+
+typedef struct mgb_policy {
+    const float *params_dev;  /* packed float32 on the handle's device, read at every launch */
+    int32_t n_hidden;         /* 0..3 hidden layers */
+    int32_t width[3];         /* 1..64 each (entries past n_hidden are ignored) */
+    int32_t activation;       /* MGB_ACT_*, the same for every hidden layer */
+    int32_t mode;             /* MGB_POLICY_* */
+} mgb_policy;
+
+/* mgb_quad_rollout_ex with actions from a Gaussian MLP policy instead of a fixed tensor.
+ *   Sampling: for the four Philox words (x, y, z, w), Box-Muller per pair: u1 = ((x >> 8) + 1) 2^-24 in (0, 1],
+ *   u2 = (y >> 8) 2^-24, z0 = sqrt(-2 log u1) cos(2 pi u2), z1 = sqrt(-2 log u1) sin(2 pi u2); likewise z2, z3 from
+ *   (z, w).  a_k = mean_k + exp(log_std_k) z_k, with no squashing or clipping (the step clamps voltages).
+ *   logp = sum_k (-z_k^2 / 2 - log_std_k) - 2 log(2 pi).  MGB_POLICY_MEAN: a = mean, and logp_out must be NULL.
+ *   act_out_dev [T][n][4] float32: the actions taken.  logp_out_dev [T][n] float32.  obs0_out_dev [n][obs_dim]: the
+ *   observation the policy acted on at t = 0, computed from the handle's state; at t > 0 it acted on obs[t-1].
+ *   obs, rew, done, final_obs, truncated: as mgb_quad_rollout_ex.  Every output may be NULL.
+ * The env side is bit for bit mgb_quad_rollout_ex fed act_out.  The step counter advances by T; nothing is allocated,
+ * and the call can be captured in a CUDA graph.  Refused (MGB_ERR_ARG, handle untouched): T <= 0, a NULL policy or
+ * params_dev, n_hidden / width / activation / mode out of range, logp_out in mean mode, output mirrors or multicast
+ * set, final_obs without auto_reset, and weights plus activations beyond the device's opt-in shared memory. */
+int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy *pol, uint64_t seed, float *act_out_dev,
+                            float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                            float *final_obs_dev, uint8_t *truncated_dev, void *stream);
+
 /* Quadrotor.step as the reference's numpy users call it (env.py:127-165: ndarray in, ndarray out).
  * Same as mgb_quad_step with HOST buffers: stages through pinned memory (or, for pinned caller buffers, lets the kernel
  * read/write host memory directly), copies inside the call, returns when the outputs are on the host (synchronous).
@@ -391,6 +433,26 @@ int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *act_dev, ui
                               void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
                               uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
                               void *stream);
+
+/* mgb_maze_rollout_ex (resample_cfg NULL) or mgb_maze_rollout_resample (resample_cfg set) of a MetaMaze2D handle with
+ * actions from a categorical MLP policy (mgb_policy, "policy-driven rollouts" above; input width (2 view_grid + 1)^2,
+ * the four outputs are the logits of actions 0..3, no log_std).
+ *   Sampling: u = (x >> 8) 2^-24 of the first Philox word; the float32 softmax of the logits is accumulated in index
+ *   order into c_0..c_2, and the action is the first k with u < c_k, else 3.  logp = l_a - logsumexp(l).
+ *   MGB_POLICY_MEAN: the argmax, ties to the lowest index, and logp_out must be NULL.
+ *   act_out_dev [T][n] int32, logp_out_dev [T][n] float32, obs0_out_dev [n][D] float32: the window the policy acted on
+ *   at t = 0, computed from the handle's state; at t > 0 it acted on obs[t-1] (post auto-reset and resampling).
+ *   obs, rew, done, final_obs, truncated: as mgb_maze_rollout_ex.  Every output may be NULL.
+ * The env side is bit for bit mgb_maze_rollout_ex / mgb_maze_rollout_resample fed act_out.  The step counter advances
+ * by T; nothing is allocated, and the call can be captured in a CUDA graph.  Refused (MGB_ERR_ARG, handle untouched):
+ * a 3-D handle, T <= 0, a NULL policy or params_dev, n_hidden / width / activation / mode out of range, logp_out in mean
+ * mode, output mirrors or multicast set, final_obs without auto_reset, resample_cfg where mgb_maze_rollout_resample
+ * refuses it (same reasons), and observation tiles, sampler workspaces, weights and activations of 128 envs beyond the
+ * device's opt-in shared memory (a large view_grid with wide layers). */
+int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
+                            const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, int32_t *act_out_dev,
+                            float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                            float *final_obs_dev, uint8_t *truncated_dev, void *stream);
 
 /* MetaMazeContinuous3D.step (maze_env.py:129-146 -> maze_continuous_3d.py:47-56, dynamics.py:58-92): act_dev [n][2]
  * float32 = (turn_rate, walk_speed), clipped to [-1, 1] like the reference; ten 10 ms sub-steps of turn/walk with the

@@ -24,4 +24,7 @@ def __getattr__(name):
                 "MetaMazeDiscrete3D", "MetaMazeContinuous3D", "TaskConfig", "MazeTaskSampler"):
         from . import metamaze
         return getattr(metamaze, name)
+    if name == "MLPPolicy":
+        from . import policy
+        return policy.MLPPolicy
     raise AttributeError(name)

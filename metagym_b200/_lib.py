@@ -49,6 +49,15 @@ class MazeCfg(ctypes.Structure):
                 ("max_vision", c_f64), ("fov", c_f64), ("l_focal", c_f64), ("text_size", c_f64)]
 
 
+class Policy(ctypes.Structure):
+    """mgb_policy (include/mgb200.h)."""
+    _fields_ = [("params_dev", vp), ("n_hidden", c_i32), ("width", c_i32 * 3), ("activation", c_i32), ("mode", c_i32)]
+
+
+ACT_TANH, ACT_RELU = 0, 1            # MGB_ACT_*
+POLICY_SAMPLE, POLICY_MEAN = 0, 1    # MGB_POLICY_*
+
+
 # name -> (restype, argtypes); every function include/mgb200.h declares (tests/test_abi.py checks the two agree)
 SIGNATURES = {
     "mgb_quad_create": (ctypes.c_int, [ctypes.POINTER(vp), c_i64, ctypes.POINTER(QuadCfg), ctypes.c_int, c_i64]),
@@ -66,6 +75,8 @@ SIGNATURES = {
     "mgb_quad_step_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_quad_step_host_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_quad_rollout_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_quad_rollout_policy": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_u64, vp, vp, vp, vp, vp, vp, vp, vp,
+                                               vp]),
     "mgb_quad_state": (ctypes.c_int, [vp, vp, vp, ctypes.c_int, vp]),
     "mgb_quad_launch_count": (c_i64, [vp]),
     "mgb_quad_step_kernel": (ctypes.c_char_p, [vp]),
@@ -105,6 +116,8 @@ SIGNATURES = {
                                                ctypes.POINTER(MazeSamplerCfg), c_u64, vp]),
     "mgb_maze_rollout_resample": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp,
                                                  ctypes.POINTER(MazeSamplerCfg), c_u64, vp]),
+    "mgb_maze_rollout_policy": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_u64, ctypes.POINTER(MazeSamplerCfg),
+                                               c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "mgb_common.cuh"
+#include "mgb_policy.cuh"
 
 namespace {
 
@@ -499,10 +500,16 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // slot with its workspace behind the two tiles, and after a __syncwarp each owner resets on its new blob.  Each warp then
 // publishes its own 32 rows of the tile with its own bulk store, so no step waits at a CTA barrier for another warp's
 // carving.
-template <int XM, bool FIN, bool REC, bool RS = false>
+// POL (XM == 0 only, mgb_maze_rollout_policy): the action of step t is drawn from the MLP policy `pol` (mgb_policy.cuh,
+// categorical head) on the window the env holds before step t.  Each step copies the window row it leaves in the tile
+// (post auto-reset and resampling) into the thread's column of the activation buffers, which follow the tiles and the
+// sampler workspaces in dynamic shared memory at pol.smem_off; at t = 0 the window of the loaded state.  The step
+// arithmetic after the action is the code the other instantiations run.
+template <int XM, bool FIN, bool REC, bool RS = false, bool POL = false>
 __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid_constant__ MazeConst c,
                                                                     const __grid_constant__ MazeArgs a,
-                                                                    const __grid_constant__ MazeResample rs)
+                                                                    const __grid_constant__ MazeResample rs,
+                                                                    const __grid_constant__ MgbMlp pol)
 {
     static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
@@ -526,6 +533,22 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
     const int n = c.n, g = c.view_grid;
+    float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the two activation buffers
+    if constexpr (POL) {
+        static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
+        pol_w = tile2d + pol.smem_off;
+        pol_x = pol_w + pol.staged;
+        pol_y = pol_x + pol.maxw * k2dThreads;
+        mgb_mlp_stage(pol, pol_w);
+        if (active) {       // the window of the loaded state: what the preceding reset() / step() returned
+            float *row = tile2d + threadIdx.x * D;
+            maze2d_window(c, blob, eaten, a.n_pad, s, row);
+            for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = row[k];
+            if (pol.obs0_out)
+                for (int k = 0; k < D; ++k) pol.obs0_out[e * D + k] = row[k];
+        }
+        __syncthreads();    // the staged weights (the RS loop has no CTA barrier)
+    }
     for (int t = 0; t < a.T; ++t) {
         float *tile = tile2d + (size_t)(t & 1) * k2dThreads * D;
         if constexpr (RS) {                                 // per warp: the warp's rows and their store are its own
@@ -538,7 +561,13 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
         uint32_t done_byte = 0;
         if (active) {
             int action;
-            if (a.act) action = a.act[(int64_t)t * a.n + e];
+            if constexpr (POL) {
+                float logits[4];
+                mgb_mlp_forward(pol, pol_w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
+                const float lp = mgb_categorical_action(pol, genv, a.t_base + (uint32_t)t, logits, action);
+                if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
+                if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
+            } else if (a.act) action = a.act[(int64_t)t * a.n + e];
             else {
                 const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
                                                              a.t_base + (uint32_t)t, MGB_STREAM_ACTION), akey);
@@ -570,7 +599,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
                 a.done[(int64_t)t * a.n + e] = (uint8_t)done;
                 if (XM == 1) mgb_mirror_store(a.mir, a.done + (int64_t)t * a.n + e, (uint8_t)done);
             }
-            if (a.obs) {
+            if (a.obs || POL) {     // POL: the row is also the policy's next input
                 float *row = tile + threadIdx.x * D;
                 for (int p = 0; p < W; ++p)
                     for (int q = 0; q < W; ++q) {
@@ -606,9 +635,13 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
                 if (done_byte) {
                     env_reset(c, blob, eaten, a.n_pad, s);
                     if (REC) path_store(c, a, e, s);
-                    if (a.obs) maze2d_window(c, blob, eaten, a.n_pad, s, tile + threadIdx.x * D);
+                    if (a.obs || POL) maze2d_window(c, blob, eaten, a.n_pad, s, tile + threadIdx.x * D);
                 }
             }
+        }
+        if constexpr (POL) {        // the policy's input at step t + 1: the row this thread left in the tile
+            if (active)
+                for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = tile[threadIdx.x * D + k];
         }
         if (XM == 2) {
             if (a.done) mgb_mc_st_bytes(mgb_shift(a.done + (int64_t)t * a.n + e, a.mir.delta[0]), done_byte, active);
@@ -4011,8 +4044,8 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
             MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false, REC, true>));
             MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC, true>));
         }
-        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs);
-        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs);
+        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{});
+        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{});
         MGB_CUDA(cudaGetLastError());
         return MGB_OK;
     }
@@ -4023,10 +4056,10 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC>));
     }
     const MazeResample none = {};
-    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
-    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
-    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
-    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none);
+    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
+    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
+    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
+    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -4174,6 +4207,85 @@ extern "C" int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *
     const cudaStream_t st = (cudaStream_t)stream;
     rc = h->path ? launch_2d_rollout<true>(h->c, 0, fin, a, blocks, sm, st, &r)
                  : launch_2d_rollout<false>(h->c, 0, fin, a, blocks, sm, st, &r);
+    if (rc) return rc;
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return MGB_OK;
+}
+
+// maze2d_rollout_kernel<0, fin, REC, RS, true>, sm bytes of dynamic shared memory; refused when the CTA would need more
+// shared memory than the device allows
+template <bool REC, bool RS>
+static int launch_2d_policy(const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r, const MgbMlp &m,
+                            unsigned blocks, size_t sm, cudaStream_t st)
+{
+    const auto kernel = fin ? maze2d_rollout_kernel<0, true, REC, RS, true> : maze2d_rollout_kernel<0, false, REC, RS, true>;
+    int optin = 0;
+    MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    cudaFuncAttributes fa;
+    MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    if (fa.sharedSizeBytes + sm > (size_t)optin) {
+        mgb_set_error("mgb_maze_rollout_policy: the policy rollout needs %zu bytes of shared memory per CTA (windows of "
+                      "view_grid %d, %sweights and activations of %d envs), more than the %d the device allows (use a "
+                      "smaller view_grid or narrower layers)", fa.sharedSizeBytes + sm, h->c.view_grid,
+                      RS ? "sampler workspaces, " : "", k2dThreads, optin);
+        return MGB_ERR_ARG;
+    }
+    MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m);
+    MGB_CUDA(cudaGetLastError());
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
+                                       const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                       int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                                       double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_policy");
+    SamplerCfg sc;
+    MgbMlp m;
+    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
+        if (h->c.kind != MGB_MAZE_2D) return "mgb_maze_rollout_policy serves MetaMaze2D (the 3-D envs observe frames)";
+        const int W = 2 * h->c.view_grid + 1;
+        if (const char *why = mgb_mlp_plan(pol, W * W, false, m)) return why;
+        if (logp_out_dev && m.mode != MGB_POLICY_SAMPLE) return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
+        if (h->mir.count != 0)
+            return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
+        if (!resample_cfg) return nullptr;
+        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout_resample
+        return sampler_cfg(h, resample_cfg, sc);
+    });
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    // two observation tiles, the sampler workspaces when resampling, then the policy's weights and activations
+    const int W = 2 * h->c.view_grid + 1;
+    size_t base = (size_t)2 * k2dThreads * W * W * 4;
+    if (resample_cfg) base += (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
+    base = (base + 15) / 16 * 16;
+    m.smem_off = (int)(base / 4);
+    m.seed = seed;
+    m.logp_out = logp_out_dev;
+    m.obs0_out = obs0_out_dev;
+    const size_t sm = base + mgb_mlp_smem_bytes(m, k2dThreads);
+    MazeArgs a = maze_args(h);
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+    MazeResample r = {};
+    if (resample_cfg) {
+        r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
+    }
+    const bool fin = final_obs_dev || truncated_dev;
+    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (resample_cfg)
+        rc = h->path ? launch_2d_policy<true, true>(h, fin, a, r, m, blocks, sm, st)
+                     : launch_2d_policy<false, true>(h, fin, a, r, m, blocks, sm, st);
+    else
+        rc = h->path ? launch_2d_policy<true, false>(h, fin, a, r, m, blocks, sm, st)
+                     : launch_2d_policy<false, false>(h, fin, a, r, m, blocks, sm, st);
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;

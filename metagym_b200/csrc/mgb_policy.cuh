@@ -1,0 +1,221 @@
+// MLP policies evaluated inside a rollout launch (mgb_quad_rollout_policy; DESIGN.md "Policy-driven rollouts").
+//
+// One thread owns one env.  The CTA stages the packed weights (mgb_policy.params_dev, torch.nn.Linear order) into shared
+// memory once per launch, regrouped so that a hidden layer's outputs are computed eight at a time: for output group g
+// and input i the eight weights W[8g .. 8g+7][i] are two consecutive float4, read by the whole warp as a broadcast, and
+// the thread's input x[i] is one conflict-free load from its own column of the activation buffers ([k][blockDim.x]).
+// The output layer (4 wide) is staged in groups of four.  Rows past a layer's width are zero.  Every output is a
+// fused multiply-add chain that starts at the bias and runs over the inputs in index order, in float32.
+#pragma once
+#include "mgb_common.cuh"
+
+constexpr int kPolicyMaxLayers = MGB_POLICY_MAX_HIDDEN + 1;
+
+// Launch-time plan of one policy: layer shapes and where each layer lives in the packed buffer and in shared memory.
+struct MgbMlp {
+    const float *params;          // packed buffer (global memory)
+    int n_layers;                 // n_hidden + 1
+    int in[kPolicyMaxLayers], out[kPolicyMaxLayers];
+    int gw[kPolicyMaxLayers];     // global float offset of W of layer l (b follows at gw + out * in)
+    int sw[kPolicyMaxLayers];     // shared float offset of the regrouped W of layer l
+    int sb[kPolicyMaxLayers];     // shared float offset of the bias of layer l (padded to the group width)
+    int g_log_std, s_log_std;     // log_std [4] (Gaussian policies), -1 if none
+    int staged;                   // floats of staged weights (a multiple of 8)
+    int maxw;                     // rows of each activation buffer: max(input width, hidden widths)
+    int smem_off;                 // float offset of the policy's region in the kernel's dynamic shared memory
+    int activation, mode;
+    uint64_t seed;
+    float *logp_out;              // [T][n] or null
+    float *obs0_out;              // [n][in[0]] or null
+};
+
+// Host: validate `p` and plan it for input width `in_dim` (output width 4; `log_std`: the buffer ends with log_std[4],
+// the Gaussian head of the quadrotor; without it the four outputs are the logits of the maze's categorical head).
+// Returns null, or the reason the policy is refused.
+static inline const char *mgb_mlp_plan(const mgb_policy *p, int in_dim, bool log_std, MgbMlp &m)
+{
+    if (!p) return "null policy";
+    if (!p->params_dev) return "null params_dev";
+    if (p->n_hidden < 0 || p->n_hidden > MGB_POLICY_MAX_HIDDEN) return "n_hidden must be 0..3";
+    for (int k = 0; k < p->n_hidden; ++k)
+        if (p->width[k] < 1 || p->width[k] > MGB_POLICY_MAX_WIDTH) return "hidden widths must be 1..64";
+    if (p->activation != MGB_ACT_TANH && p->activation != MGB_ACT_RELU) return "unknown activation";
+    if (p->mode != MGB_POLICY_SAMPLE && p->mode != MGB_POLICY_MEAN) return "unknown policy mode";
+    m = MgbMlp{};
+    m.params = p->params_dev;
+    m.n_layers = p->n_hidden + 1;
+    m.activation = p->activation;
+    m.mode = p->mode;
+    int g = 0, s = 0, maxw = in_dim;
+    for (int l = 0; l < m.n_layers; ++l) {
+        const bool last = l == m.n_layers - 1;
+        m.in[l] = l == 0 ? in_dim : p->width[l - 1];
+        m.out[l] = last ? 4 : p->width[l];
+        if (!last && m.out[l] > maxw) maxw = m.out[l];
+        const int gwid = last ? 4 : 8, rows = (m.out[l] + gwid - 1) / gwid * gwid;
+        m.gw[l] = g;
+        g += m.out[l] * (m.in[l] + 1);
+        m.sw[l] = s;
+        s += rows * m.in[l];
+        m.sb[l] = s;
+        s += rows;
+        s = (s + 7) / 8 * 8;
+    }
+    m.g_log_std = m.s_log_std = -1;
+    if (log_std) {
+        m.g_log_std = g;
+        m.s_log_std = s;
+        s += 8;
+    }
+    m.staged = s;
+    m.maxw = maxw;
+    return nullptr;
+}
+
+// floats of dynamic shared memory a CTA of `threads` needs: staged weights + two activation buffers
+static inline size_t mgb_mlp_smem_bytes(const MgbMlp &m, int threads)
+{
+    return ((size_t)m.staged + 2 * (size_t)m.maxw * (size_t)threads) * sizeof(float);
+}
+
+// Device: stage the weights of `m` into sm[0, m.staged) (all threads of the CTA; the caller synchronises)
+__device__ __forceinline__ void mgb_mlp_stage(const MgbMlp &m, float *sm)
+{
+    for (int l = 0; l < m.n_layers; ++l) {
+        const bool last = l == m.n_layers - 1;
+        const int gwid = last ? 4 : 8, in = m.in[l], out = m.out[l];
+        const int rows = (out + gwid - 1) / gwid * gwid;
+        const float *W = m.params + m.gw[l], *b = W + out * in;
+        for (int s = threadIdx.x; s < rows * in; s += blockDim.x) {
+            const int r = s % gwid, rest = s / gwid, i = rest % in, j = (rest / in) * gwid + r;
+            sm[m.sw[l] + s] = j < out ? __ldg(W + j * in + i) : 0.f;
+        }
+        for (int j = threadIdx.x; j < rows; j += blockDim.x) sm[m.sb[l] + j] = j < out ? __ldg(b + j) : 0.f;
+    }
+    if (m.s_log_std >= 0 && threadIdx.x < 4) sm[m.s_log_std + threadIdx.x] = __ldg(m.params + m.g_log_std + threadIdx.x);
+}
+
+__device__ __forceinline__ float mgb_mlp_activate(int activation, float x)
+{
+    return activation == MGB_ACT_TANH ? tanhf(x) : (x > 0.f ? x : 0.f);
+}
+
+// Device: forward pass of the thread's env.  Its input x[i] is a0[i * stride + col], i < m.in[0]; a0 and a1 are the
+// two activation buffers (each m.maxw rows of `stride` floats), both clobbered.  out4 receives the four outputs.
+__device__ __forceinline__ void mgb_mlp_forward(const MgbMlp &m, const float *sm, float *a0, float *a1, int stride,
+                                                int col, float out4[4])
+{
+    const float *x = a0 + col;
+    float *y = a1 + col;
+    for (int l = 0; l < m.n_layers - 1; ++l) {
+        const int in = m.in[l], out = m.out[l];
+        const float4 *W = reinterpret_cast<const float4 *>(sm + m.sw[l]);
+        const float4 *B = reinterpret_cast<const float4 *>(sm + m.sb[l]);
+        for (int g = 0; g < out; g += 8) {
+            const float4 b0 = B[g / 4], b1 = B[g / 4 + 1];
+            float acc[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+            const float4 *w = W + (g / 8) * in * 2;
+#pragma unroll 4
+            for (int i = 0; i < in; ++i) {
+                const float xi = x[i * stride];
+                const float4 w0 = w[2 * i], w1 = w[2 * i + 1];
+                acc[0] = fmaf(w0.x, xi, acc[0]); acc[1] = fmaf(w0.y, xi, acc[1]);
+                acc[2] = fmaf(w0.z, xi, acc[2]); acc[3] = fmaf(w0.w, xi, acc[3]);
+                acc[4] = fmaf(w1.x, xi, acc[4]); acc[5] = fmaf(w1.y, xi, acc[5]);
+                acc[6] = fmaf(w1.z, xi, acc[6]); acc[7] = fmaf(w1.w, xi, acc[7]);
+            }
+#pragma unroll
+            for (int r = 0; r < 8; ++r)
+                if (g + r < out) y[(g + r) * stride] = mgb_mlp_activate(m.activation, acc[r]);
+        }
+        const float *t = x;
+        x = y;
+        y = const_cast<float *>(t);
+    }
+    const int l = m.n_layers - 1, in = m.in[l];
+    const float4 *W = reinterpret_cast<const float4 *>(sm + m.sw[l]);
+    const float4 b = *reinterpret_cast<const float4 *>(sm + m.sb[l]);
+    float acc[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll 4
+    for (int i = 0; i < in; ++i) {
+        const float xi = x[i * stride];
+        const float4 w = W[i];
+        acc[0] = fmaf(w.x, xi, acc[0]); acc[1] = fmaf(w.y, xi, acc[1]);
+        acc[2] = fmaf(w.z, xi, acc[2]); acc[3] = fmaf(w.w, xi, acc[3]);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) out4[k] = acc[k];
+}
+
+// Device: Gaussian action of env genv at step counter t from the policy mean (MGB_POLICY_SAMPLE), or the mean itself
+// (MGB_POLICY_MEAN).  Returns log pi(a | obs) for the sampling mode (0 for the mean mode).
+__device__ __forceinline__ float mgb_gaussian_action(const MgbMlp &m, const float *sm, int64_t genv, uint32_t t,
+                                                     const float mean[4], float a[4])
+{
+    if (m.mode == MGB_POLICY_MEAN) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) a[k] = mean[k];
+        return 0.f;
+    }
+    const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32), t, MGB_STREAM_POLICY),
+                                      make_uint2((uint32_t)m.seed, (uint32_t)(m.seed >> 32)));
+    const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+    float z[4];
+#pragma unroll
+    for (int p = 0; p < 2; ++p) {
+        const float u1 = (float)((w[2 * p] >> 8) + 1u) * (1.0f / 16777216.0f);      // (0, 1]: log is finite
+        const float u2 = mgb_u01(w[2 * p + 1]);
+        const float rad = sqrtf(-2.f * logf(u1));
+        float sn, cs;
+        sincospif(2.f * u2, &sn, &cs);
+        z[2 * p] = rad * cs;
+        z[2 * p + 1] = rad * sn;
+    }
+    float logp = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float ls = sm[m.s_log_std + k];
+        a[k] = fmaf(expf(ls), z[k], mean[k]);
+        logp += -0.5f * z[k] * z[k] - ls;
+    }
+    return logp - 3.6757541328186907f;     // 2 log(2 pi)
+}
+
+// Device: categorical action over the four logits l (MetaMaze2D).  MGB_POLICY_SAMPLE: inverse CDF of the float32 softmax,
+// u = (x >> 8) 2^-24 of the first Philox word, the probabilities accumulated in index order; the action is the first k
+// with u < c_k, else 3.  MGB_POLICY_MEAN: the argmax, ties to the lowest index.  Returns l_a - logsumexp(l) for the
+// sampling mode (0 for the mean mode).
+__device__ __forceinline__ float mgb_categorical_action(const MgbMlp &m, int64_t genv, uint32_t t, const float l[4],
+                                                        int &action)
+{
+    float mx = l[0];
+    int am = 0;
+#pragma unroll
+    for (int k = 1; k < 4; ++k)
+        if (l[k] > mx) { mx = l[k]; am = k; }
+    if (m.mode == MGB_POLICY_MEAN) {
+        action = am;
+        return 0.f;
+    }
+    float ex[4], sum = 0.f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        ex[k] = expf(l[k] - mx);
+        sum += ex[k];
+    }
+    const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32), t, MGB_STREAM_POLICY),
+                                      make_uint2((uint32_t)m.seed, (uint32_t)(m.seed >> 32)));
+    const float u = mgb_u01(r.x);
+    float cdf = 0.f;
+    action = 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        cdf += ex[k] / sum;
+        if (u < cdf) { action = k; break; }
+    }
+    float la = l[0];
+#pragma unroll
+    for (int k = 1; k < 4; ++k)
+        if (action == k) la = l[k];
+    return (la - mx) - logf(sum);
+}

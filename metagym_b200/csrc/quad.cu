@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "mgb_common.cuh"
+#include "mgb_policy.cuh"
 #include "quad_lanes.cuh"
 
 namespace {
@@ -1144,9 +1145,14 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 // FIN (XM == 0 only, mgb_quad_rollout_ex): also store the truncation byte of every (t, e), and the terminal observation of
 // every env an auto-reset replaced at step t to final_obs + (t n + e) D, straight from registers before observe_reset
 // overwrites them.  Rows of envs that did not finish are not written.
-template <bool SIMPLE, int XM, bool FIN>
-__global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_constant__ QuadConst c,
-                                                                const __grid_constant__ QuadArgs a)
+// POL (XM == 0 only, mgb_quad_rollout_policy): the action of step t is drawn from the MLP policy `pol` (mgb_policy.cuh)
+// on the observation the env holds before step t, which each step leaves in the thread's column of the activation
+// buffers in dynamic shared memory (at t = 0: the observation of the loaded state).  The weights are staged once per
+// CTA.  The step arithmetic after the action is the code the other instantiations run.
+template <bool SIMPLE, int XM, bool FIN, bool POL = false>
+__global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(const __grid_constant__ QuadConst c,
+                                                                          const __grid_constant__ QuadArgs a,
+                                                                          const __grid_constant__ MgbMlp pol)
 {
     __shared__ __align__(128) float tiles[2][kThreads * kMaxObs];
     const int64_t e0 = (int64_t)blockIdx.x * kThreads;
@@ -1163,6 +1169,31 @@ __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
     const int task = active ? env_task(c, a, e) : 0;
+    float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the two activation buffers
+    if constexpr (POL) {
+        static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
+        extern __shared__ __align__(16) float pol_smem[];
+        pol_w = pol_smem;
+        pol_x = pol_w + pol.staged;
+        pol_y = pol_x + pol.maxw * kThreads;
+        mgb_mlp_stage(pol, pol_w);
+        if (active) {       // the observation of the loaded state: what the preceding reset() / step() returned
+            float o[kMaxObs], bv[3], Ri[9];
+            observe(c, s, adj, id, o, bv, Ri);
+            if (c.task == MGB_TASK_VELOCITY_CONTROL) {
+                const float4 q = target_row(a, task, s.ct[0] < c.nt - 1 ? s.ct[0] : c.nt - 1);
+                o[16] = q.x; o[17] = q.y; o[18] = q.z;
+            }
+#pragma unroll
+            for (int k = 0; k < kMaxObs; ++k)
+                if (k < D) pol_x[k * kThreads + threadIdx.x] = o[k];
+            if (pol.obs0_out) {
+#pragma unroll
+                for (int k = 0; k < kMaxObs; ++k)
+                    if (k < D) pol.obs0_out[e * D + k] = o[k];
+            }
+        }
+    }
     // software pipeline: the action of step t+1 is requested while step t integrates
     float4 act_next = make_float4(0.f, 0.f, 0.f, 0.f);
     if (active && a.act) act_next = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
@@ -1174,7 +1205,14 @@ __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_
         uint32_t done_byte = 0;
         if (active) {
             float4 act;
-            if (a.act) {
+            if constexpr (POL) {
+                float mean[4], av[4];
+                mgb_mlp_forward(pol, pol_w, pol_x, pol_y, kThreads, threadIdx.x, mean);
+                const float lp = mgb_gaussian_action(pol, pol_w, genv, a.t_base + (uint32_t)t, mean, av);
+                act = make_float4(av[0], av[1], av[2], av[3]);
+                if (a.act_out) reinterpret_cast<float4 *>(a.act_out)[(int64_t)t * a.n + e] = act;
+                if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
+            } else if (a.act) {
                 act = act_next;
                 if (t + 1 < a.T) act_next = __ldg(reinterpret_cast<const float4 *>(a.act) + (int64_t)(t + 1) * a.n + e);
             } else {
@@ -1232,6 +1270,11 @@ __global__ void __launch_bounds__(kThreads, 8) quad_rollout_kernel(const __grid_
 #pragma unroll
                 for (int k = 0; k < 16; ++k) orow[k] = o[k];
                 if (D == 19) { orow[16] = o[16]; orow[17] = o[17]; orow[18] = o[18]; }
+            }
+            if constexpr (POL) {       // the policy's input at step t + 1
+#pragma unroll
+                for (int k = 0; k < kMaxObs; ++k)
+                    if (k < D) pol_x[k * kThreads + threadIdx.x] = o[k];
             }
         }
         if (XM == 2) {
@@ -1780,7 +1823,55 @@ static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_se
         return xm == 2 ? quad_rollout_kernel<simple, 2, false> : xm == 1 ? quad_rollout_kernel<simple, 1, false>
                : fin   ? quad_rollout_kernel<simple, 0, true>  : quad_rollout_kernel<simple, 0, false>;
     });
-    kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a);
+    kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a, MgbMlp{});
+    MGB_CUDA(cudaGetLastError());
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return MGB_OK;
+}
+
+extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy *pol, uint64_t seed, float *act_out_dev,
+                                       float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev,
+                                       uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_policy");
+    MGB_REQUIRE(h, "null handle");
+    MGB_REQUIRE(T > 0, "T must be positive");
+    MgbMlp m;
+    const char *why = mgb_mlp_plan(pol, h->c.obs_dim, true, m);
+    MGB_REQUIRE(!why, why);
+    MGB_REQUIRE(!logp_out_dev || m.mode == MGB_POLICY_SAMPLE, "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)");
+    MGB_REQUIRE(h->mir.count == 0, "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)");
+    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal observation)");
+    MGB_REQUIRE((reinterpret_cast<uintptr_t>(act_out_dev) & 15u) == 0, "act_out_dev must be 16-byte aligned");
+    MGB_REQUIRE((reinterpret_cast<uintptr_t>(pol->params_dev) & 3u) == 0, "params_dev must be 4-byte aligned");
+    int rc = check_ready(h);
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    m.seed = seed;
+    m.logp_out = logp_out_dev;
+    m.obs0_out = obs0_out_dev;
+    const bool fin = final_obs_dev || truncated_dev;
+    const auto kernel = with_simple(h, [&](auto simple) {
+        return fin ? quad_rollout_kernel<simple, 0, true, true> : quad_rollout_kernel<simple, 0, false, true>;
+    });
+    const size_t smem = mgb_mlp_smem_bytes(m, kThreads);
+    int optin = 0;
+    MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    cudaFuncAttributes fa;
+    MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    if (fa.sharedSizeBytes + smem > (size_t)optin) {
+        mgb_set_error("%s: the policy needs %zu bytes of shared memory per CTA (weights and activations of %d envs), "
+                      "above the device's %d", __func__, fa.sharedSizeBytes + smem, kThreads, optin);
+        return MGB_ERR_ARG;
+    }
+    MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    QuadArgs a = base_args(h);
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev;
+    a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+    const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
+    kernel<<<blocks, kThreads, smem, (cudaStream_t)stream>>>(h->c, a, m);
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;

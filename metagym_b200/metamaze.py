@@ -684,7 +684,8 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         cfg.n_cells, cfg.max_steps, cfg.view_grid = n_cells, self.max_steps, self.view_grid
         return cfg
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, resample=None):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, resample=None, policy=None,
+                deterministic=False):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
         {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None).
 
@@ -698,8 +699,48 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         (mgb_maze_rollout_resample).  Every env whose episode ends at step t then gets the maze resample_tasks(done,
         **resample) would give it, in the same launch: obs[t] is its first window on the new maze, final_obs[t] the
         terminal window on the old one.  Needs auto_reset=True and set_task() with one table slot per env, like
-        resample_tasks; with n = 31 the view_grid may be at most 6."""
+        resample_tasks; with n = 31 the view_grid may be at most 6.
+
+        policy: an MLPPolicy (metagym_b200.policy) with (2 view_grid + 1)^2 inputs whose four outputs are the logits of
+        the actions (mgb_maze_rollout_policy): the action of step t is drawn from their softmax on the window before
+        step t, with the Philox stream keyed by act_seed; deterministic=True takes the argmax.  Composes with
+        `resample`.  The dict then also holds "act" [T,N] int32, "logp" [T,N] float32 (sampling only) and "obs0"
+        [N,<obs of one env>] (the window acted on at t = 0; at t > 0 it is obs[t-1]).  `actions` together with
+        `policy` is a ValueError."""
+        if policy is not None:
+            if actions is not None:
+                raise ValueError("rollout takes either actions or a policy, not both")
+            return self._rollout_policy(T, policy, act_seed, deterministic, out, resample)
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
+
+    def _rollout_policy(self, T, policy, act_seed, deterministic, out, resample):
+        if self.need_reset:
+            raise Exception("Must \"reset\" before doing any actions")
+        torch = self._torch
+        T, N, dev = int(T), self.num_envs, self.device
+        shape = tuple(self._obs.shape[1:])
+        D = int(np.prod(shape))
+        if policy.obs_dim != D:
+            raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
+        if policy.params.device != dev:
+            raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
+        if out is None:
+            out = {"obs": torch.empty((T, N) + shape, dtype=torch.float32, device=dev),
+                   "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
+                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
+                   "act": torch.empty((T, N), dtype=torch.int32, device=dev),
+                   "logp": None if deterministic else torch.empty((T, N), dtype=torch.float32, device=dev),
+                   "obs0": torch.empty((N,) + shape, dtype=torch.float32, device=dev)}
+            if self._want_final:
+                out["final_obs"] = torch.empty((T, N) + shape, dtype=torch.float32, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+        cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+        pol = policy.struct(deterministic)
+        keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
+        _lib.check(self._lib.mgb_maze_rollout_policy(self._h, T, ctypes.byref(pol), int(act_seed),
+                                                     None if cfg is None else ctypes.byref(cfg), seed,
+                                                     *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
+        return out
 
     def save_trajectory(self, file_name, envs=None, additional=None):
         """MetaMaze2D.save_trajectory(file_name, additional) (maze_env.py:211-212), file names as for the 3-D envs.

@@ -341,9 +341,15 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         _lib.check(self._lib.mgb_quad_step_host(self._h, _lib.ptr(act), _lib.ptr(obs), _lib.ptr(rew), _lib.ptr(done),
                                                 None, None, self._stream()))
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, policy=None, deterministic=False):
         """T steps in one launch (state stays in registers).  actions: [T,N,4] CUDA tensor or None (device-drawn
         U(min_voltage, max_voltage)).  Returns dict(obs [T,N,D], rew [T,N], done [T,N], act [T,N,4] or None).
+
+        policy: an MLPPolicy (metagym_b200.policy) whose actions drive the rollout (mgb_quad_rollout_policy): the
+        action of step t is drawn from N(mean, exp(log_std)^2), mean = policy(observation before step t), with the
+        Philox stream keyed by act_seed; deterministic=True takes the mean.  The dict then also holds "act" [T,N,4]
+        (the actions taken), "logp" [T,N] (their log-probabilities; sampling only) and "obs0" [N,D] (the observation
+        acted on at t = 0; at t > 0 it is obs[t-1]).  `actions` together with `policy` is a ValueError.
 
         With final_obs=True the dict also holds "final_obs" [T,N,D] float32: row (t, e) is the terminal observation
         of env e where done[t, e] (what step() reports as final_observation); it is allocated with torch.empty, and
@@ -352,6 +358,10 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         omit either entry, and that output is then not produced."""
         torch = self._torch
         N, D, dev = self.num_envs, self.obs_dim, self.device
+        if policy is not None:
+            if actions is not None:
+                raise ValueError("rollout takes either actions or a policy, not both")
+            return self._rollout_policy(T, policy, act_seed, deterministic, out)
         if out is None:
             out = {"obs": torch.empty((T, N, D), dtype=torch.float32, device=dev),
                    "rew": torch.empty((T, N), dtype=torch.float32, device=dev),
@@ -366,6 +376,31 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         keys = ("act", "obs", "rew", "done") + (("final_obs", "truncated") if self._want_final else ())
         _lib.check(self._rollout_fn(self._h, int(T), _lib.ptr(a), int(act_seed), *[_lib.ptr(out.get(k)) for k in keys],
                                     self._stream()))
+        return out
+
+    def _rollout_policy(self, T, policy, act_seed, deterministic, out):
+        torch = self._torch
+        N, D, dev = self.num_envs, self.obs_dim, self.device
+        if policy.obs_dim != D:
+            raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
+        if policy.params.device != dev:
+            raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
+        if not deterministic and not policy.has_log_std:
+            raise ValueError("a stochastic quadrotor policy needs log_std (or pass deterministic=True)")
+        if out is None:
+            out = {"obs": torch.empty((T, N, D), dtype=torch.float32, device=dev),
+                   "rew": torch.empty((T, N), dtype=torch.float32, device=dev),
+                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
+                   "act": torch.empty((T, N, 4), dtype=torch.float32, device=dev),
+                   "logp": None if deterministic else torch.empty((T, N), dtype=torch.float32, device=dev),
+                   "obs0": torch.empty((N, D), dtype=torch.float32, device=dev)}
+            if self._want_final:
+                out["final_obs"] = torch.empty((T, N, D), dtype=torch.float32, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+        pol = policy.struct(deterministic)
+        keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
+        _lib.check(self._lib.mgb_quad_rollout_policy(self._h, int(T), ctypes.byref(pol), int(act_seed),
+                                                     *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
         return out
 
     @property
