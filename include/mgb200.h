@@ -359,82 +359,75 @@ int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *task_slots_
 /* MazeBase.reset (maze_base.py:40-63, maze_discrete_3d.py:39-49).  mask_dev NULL = all.  obs_dev NULL = skip. */
 int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_dev, void *stream);
 
-/* MetaMaze*.step (maze_env.py:59-75,189-206): DISCRETE_ACTIONS[a] (maze_env.py:14) -> do_action -> evaluation_rule
- * (maze_base.py:65-95) -> update_observation (maze_2d.py:89-121 | maze_discrete_3d.py:113-127 + ray_caster_utils.py).
- *   act_dev [n] int32 in 0..3; obs_dev: 2-D float32 [n][2g+1][2g+1]; 3-D uint8|int32 [n][res_h][res_v][3];
+/* MetaMaze*.step (maze_env.py:59-75,129-146,189-206).  act_dev is typed by the handle kind:
+ *   MetaMaze2D, MetaMazeDiscrete3D: [n] int32 in 0..3; DISCRETE_ACTIONS[a] (maze_env.py:14) -> do_action ->
+ *   evaluation_rule (maze_base.py:65-95) -> update_observation (maze_2d.py:89-121 | maze_discrete_3d.py:113-127 +
+ *   ray_caster_utils.py).
+ *   MetaMazeContinuous3D: [n][2] float32 = (turn_rate, walk_speed), clipped to [-1, 1] like the reference
+ *   (maze_continuous_3d.py:47-56, dynamics.py:58-92); ten 10 ms sub-steps of turn/walk with the soft wall-repulsion
+ *   collision model, then evaluation_rule and the ray-cast observation (same renderer).  Typing follows what the reference
+ *   computes for float32 actions (its action_space.sample()): float32 position, float64 heading.
+ *   obs_dev: 2-D float32 [n][2g+1][2g+1]; 3-D uint8|int32|float32 [n][res_h][res_v][3];
  *   rew_dev [n] float64 (the reference returns python/np float64); done_dev [n] uint8.
  * With auto_reset on (mgb_maze_set_options) a finished env is reset in the same launch and obs holds the first
- * observation of the next episode. */
-int mgb_maze_step(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                  void *stream);
-/* mgb_maze_step with two optional outputs (NULL: not produced; both NULL is exactly mgb_maze_step):
+ * observation of the next episode.  Two optional outputs (NULL: not produced):
  *   final_obs_dev [n][obs of one env] in the obs dtype: for every env with done = 1 in this step, the observation an
  *     auto_reset-off handle would have returned (the terminal frame, life bar included).  Rows of envs that did not
  *     finish are left untouched.  Needs auto_reset on (MGB_ERR_ARG otherwise).
  *   truncated_dev [n] uint8, written for every env: 1 iff done and the episode ended only through the step limit
  *     (SURVIVAL: life >= 0; ESCAPE: not on the goal; steps > max_steps - 1), so terminated = done && !truncated.
- * obs, rew, done and the env state are bit for bit what mgb_maze_step gives.  The fused uint8 step (pose cache) moves the
- * terminal frames in the same launch (final_obs 16-byte aligned; otherwise the two-kernel path runs); the other 3-D paths
- * render them in one more launch, one frame per finished env.  Stream-ordered, no host synchronisation, capturable in a
- * CUDA graph. */
-int mgb_maze_step_ex(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                     void *final_obs_dev, uint8_t *truncated_dev, void *stream);
+ * obs, rew, done and the env state are bit for bit the same with or without them.  The fused uint8 step (pose cache)
+ * moves the terminal frames in the same launch (final_obs 16-byte aligned; otherwise the two-kernel path runs); the other
+ * 3-D paths render them in one more launch, one frame per finished env.  Stream-ordered, no host synchronisation,
+ * capturable in a CUDA graph. */
+int mgb_maze_step(mgb_maze *h, const void *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                  void *final_obs_dev, uint8_t *truncated_dev, void *stream);
 int mgb_maze_set_options(mgb_maze *h, int auto_reset);
 
-/* MetaMaze2D and MetaMazeDiscrete3D: T consecutive step() calls (maze_env.py:59-75,189-206; the random-action loops of
- * metamaze/test.py:9-47) in ONE launch (agent state in registers; auto-reset semantics
- * as configured; the 3-D form runs on the pose cache: one CTA per env, step logic by one thread, frame by the CTA).
- *   act_dev [T][n] int32 or NULL: NULL draws uniform {0..3} actions from the counter-based generator (stream id
- *   act_seed, keyed by the global env index), written to act_out_dev [T][n] if not NULL.
- *   obs_dev [T][n][obs of one env] (2-D: float32 [2g+1][2g+1]; 3-D: uint8 or int32 [res_h][res_v][3]),
- *   rew_dev [T][n] float64, done_dev [T][n] uint8 (any may be NULL). */
-int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                     void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream);
-/* mgb_maze_rollout with the two optional outputs of mgb_maze_step_ex, per step (both NULL: exactly mgb_maze_rollout).
- * MetaMaze2D only: a MetaMazeDiscrete3D handle given either one returns MGB_ERR_ARG.
- *   final_obs_dev [T][n][2g+1][2g+1] float32: row (t, e) is written only when done[t][e] = 1, with the terminal window
- *     (update_observation, maze_2d.py:89-121, on the state evaluation_rule left).  Rows with done = 0 are not written.
+/* T consecutive mgb_maze_step calls (the random-action loops of metamaze/test.py:9-67) in ONE launch; auto-reset
+ * semantics as configured, state left as T steps leave it.  The handle picks the engine:
+ *   MetaMaze2D: agent state in registers.
+ *   MetaMazeDiscrete3D without resample_cfg: the pose cache when it is in use (one CTA per env, step logic by one thread,
+ *   frame by the CTA); otherwise, and always with resample_cfg, the direct renderer (every frame ray-cast).  Both give
+ *   the same outputs, env state and step counter.
+ *   MetaMazeContinuous3D: the direct renderer.
+ *   act_dev [T][n] int32 in 0..3 (MetaMazeContinuous3D: float32 [T][n][2]) or NULL: NULL draws the actions from the
+ *   counter-based generator (stream id act_seed, keyed by the global env index, counted across calls) -- uniform {0..3},
+ *   or turn_rate and walk_speed uniform on [-1, 1) -- written to act_out_dev (same shape) if not NULL.
+ *   obs_dev [T][n][obs of one env] (2-D: float32 [2g+1][2g+1]; 3-D: uint8, int32 or float32 [res_h][res_v][3]),
+ *   rew_dev [T][n] float64, done_dev [T][n] uint8.  Any may be NULL, except on the direct renderer.
+ * Two optional outputs per step (NULL: not produced):
+ *   final_obs_dev [T][n][obs of one env] in the obs dtype: row (t, e) is written only when done[t][e] = 1, with the
+ *     observation an auto_reset-off handle would have returned at step t (update_observation on the state
+ *     evaluation_rule left: maze_2d.py:89-121; maze_discrete_3d.py:113-127 with the food it left and the life bar at the
+ *     terminal life; maze_continuous_3d.py:47-56 then the ray-cast observation).  Rows with done = 0 are not written.
  *     Needs auto_reset on (MGB_ERR_ARG otherwise).
  *   truncated_dev [T][n] uint8, written for every (t, e): 1 iff done and the episode ended only through the step limit
  *     (maze_base.py:80,91-95,191-192).
- * obs, rew, done, the drawn actions and the env state are bit for bit what mgb_maze_rollout gives.  Either output while
- * output mirrors or multicast are set is MGB_ERR_ARG. */
-int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                        void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
-                        void *stream);
-/* mgb_maze_rollout of a MetaMazeDiscrete3D handle (pose cache) with the two optional outputs of mgb_maze_step_ex, per step
- * (both NULL: exactly mgb_maze_rollout).  Any other handle kind is MGB_ERR_ARG.
- *   final_obs_dev [T][n][res_h][res_v][3] in the obs dtype: row (t, e) is written only when done[t][e] = 1, with the frame
- *     an auto_reset-off handle would have returned at step t (update_observation, maze_discrete_3d.py:113-127, on the state
- *     evaluation_rule left: the food it left and the life bar at the terminal life).  Rows with done = 0 are not written.
- *     Needs auto_reset on (MGB_ERR_ARG otherwise).
- *   truncated_dev [T][n] uint8, written for every (t, e): 1 iff done and the episode ended only through the step limit
- *     (maze_base.py:80,91-95,191-192).
- * obs_dev may be NULL (then only the terminal frames and the flags are produced).  obs, rew, done, the drawn actions, the
- * generator's step counter and the env state are bit for bit what mgb_maze_rollout gives.  Either output while output
- * mirrors or multicast are set is MGB_ERR_ARG; so is a handle without a pose cache.  Stream-ordered, no host
- * synchronisation, no allocation: capturable in a CUDA graph. */
-int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                                 void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
-                                 uint8_t *truncated_dev, void *stream);
-/* mgb_maze_rollout_ex of a MetaMaze2D handle that gives every env whose episode ends a freshly drawn maze in the same
- * launch -- the meta-RL data loop over an endless stream of tasks.  Actions (given or drawn) and the outputs (any may be
- * NULL) are those of mgb_maze_rollout_ex.  When env e finishes at step t, its reward, done, truncated[t][e] and the
- * terminal window final_obs[t][e] come from the old task; then it gets the task mgb_maze_resample_tasks(mask with only e
- * set, resample_cfg, resample_seed) would give it -- written into its table slot, resample count + 1 -- and starts its next
- * episode on it (start cell, initial_life, every food present): obs[t][e] is its first window on the NEW maze.  That equals,
- * step for step, step_ex + resample_tasks(done) + reset(mask = done).
- * Refused (MGB_ERR_ARG, handle untouched): a 3-D handle (use mgb_maze_rollout_direct), T <= 0, resample_cfg NULL,
- * auto-reset off, output mirrors or multicast set, shared memory per CTA (two tiles of 128 windows plus four sampler
- * workspaces) beyond the device's opt-in limit (n = 31 needs view_grid <= 6), and every refusal of
- * mgb_maze_resample_tasks (one slot per env, the cfg checks) with the same messages.
- * Advances the step counter by T.  Stream-ordered, no host synchronisation, no allocation: capturable in a CUDA graph. */
-int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                              void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
-                              uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
-                              void *stream);
+ * obs, rew, done, the drawn actions, the generator's step counter, the env state and the pose are bit for bit the same
+ * with or without them.  On the 3-D engines a finished env costs one more frame in the same launch.
+ *   resample_cfg NULL: no resampling; the outputs and the env state are bit for bit those of T step() calls.
+ *   resample_cfg set (the data-generation loop of meta-RL over an endless stream of tasks): when env e finishes at step t
+ *   (done, auto-reset on), its reward, done, truncated[t][e] and final_obs[t][e] come from the old task; then it gets the
+ *   task mgb_maze_resample_tasks(mask with only e set, resample_cfg, resample_seed) would give it -- written into its
+ *   table slot, resample count + 1 -- and starts its next episode on it (start cell, initial_life, every food present):
+ *   obs[t][e] is its first observation on the NEW maze.  That equals, step for step, step + resample_tasks(done) +
+ *   reset(mask = done) (without the extra render).
+ * MetaMaze2D without resample_cfg delivers obs, rew, done and act_out through output mirrors or multicast when they are
+ * set (mgb_maze_set_mirrors, mgb_maze_set_multicast below).
+ * Refused (MGB_ERR_ARG, handle untouched): T <= 0; final_obs without auto-reset; final_obs or truncated while output
+ * mirrors or multicast are set; output mirrors or multicast on a 3-D handle or with resample_cfg; NULL obs, rew or done on
+ * the direct renderer; a screen too large for the pose cache's group queue.  With resample_cfg also: auto-reset off,
+ * every refusal of mgb_maze_resample_tasks (one slot per env, a discrete handle whose pose cache is in use, the cfg
+ * checks) with the same messages, and on MetaMaze2D shared memory per CTA (two tiles of 128 windows plus four sampler
+ * workspaces) beyond the device's opt-in limit (n = 31 needs view_grid <= 6).
+ * Advances the step counter by T.  Stream-ordered, no host synchronisation, no allocation after the handle's first
+ * reset() (which builds the pose cache and sizes the renderer's scratch): capturable in a CUDA graph. */
+int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
+                     void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
+                     const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, void *stream);
 
-/* mgb_maze_rollout_ex (resample_cfg NULL) or mgb_maze_rollout_resample (resample_cfg set) of a MetaMaze2D handle with
+/* mgb_maze_rollout of a MetaMaze2D handle (resample_cfg NULL: no resampling; set: in-launch resampling) with
  * actions from a categorical MLP policy (mgb_policy, "policy-driven rollouts" above; input width (2 view_grid + 1)^2,
  * the four outputs are the logits of actions 0..3, no log_std).
  *   Sampling: u = (x >> 8) 2^-24 of the first Philox word; the float32 softmax of the logits is accumulated in index
@@ -442,11 +435,11 @@ int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *act_dev, ui
  *   MGB_POLICY_MEAN: the argmax, ties to the lowest index, and logp_out must be NULL.
  *   act_out_dev [T][n] int32, logp_out_dev [T][n] float32, obs0_out_dev [n][D] float32: the window the policy acted on
  *   at t = 0, computed from the handle's state; at t > 0 it acted on obs[t-1] (post auto-reset and resampling).
- *   obs, rew, done, final_obs, truncated: as mgb_maze_rollout_ex.  Every output may be NULL.
- * The env side is bit for bit mgb_maze_rollout_ex / mgb_maze_rollout_resample fed act_out.  The step counter advances
+ *   obs, rew, done, final_obs, truncated: as mgb_maze_rollout.  Every output may be NULL.
+ * The env side is bit for bit mgb_maze_rollout fed act_out.  The step counter advances
  * by T; nothing is allocated, and the call can be captured in a CUDA graph.  Refused (MGB_ERR_ARG, handle untouched):
  * a 3-D handle, T <= 0, a NULL policy or params_dev, n_hidden / width / activation / mode out of range, logp_out in mean
- * mode, output mirrors or multicast set, final_obs without auto_reset, resample_cfg where mgb_maze_rollout_resample
+ * mode, output mirrors or multicast set, final_obs without auto_reset, resample_cfg where mgb_maze_rollout
  * refuses it (same reasons), and observation tiles, sampler workspaces, weights and activations of 128 envs beyond the
  * device's opt-in shared memory (a large view_grid with wide layers). */
 int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
@@ -454,59 +447,6 @@ int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint6
                             float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev, uint8_t *done_dev,
                             float *final_obs_dev, uint8_t *truncated_dev, void *stream);
 
-/* MetaMazeContinuous3D.step (maze_env.py:129-146 -> maze_continuous_3d.py:47-56, dynamics.py:58-92): act_dev [n][2]
- * float32 = (turn_rate, walk_speed), clipped to [-1, 1] like the reference; ten 10 ms sub-steps of turn/walk with the
- * soft wall-repulsion collision model, then evaluation_rule and the ray-cast observation (same renderer).  Typing follows
- * what the reference computes for float32 actions (its action_space.sample()): float32 position, float64 heading. */
-int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                             void *stream);
-/* mgb_maze_step_continuous with the final_obs_dev and truncated_dev outputs of mgb_maze_step_ex. */
-int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                void *final_obs_dev, uint8_t *truncated_dev, void *stream);
-/* MetaMazeContinuous3D: T consecutive mgb_maze_step_continuous calls (the random-action loop of metamaze/test.py:49-67)
- * in ONE launch of the direct renderer; auto-reset semantics as configured, state left as T steps leave it.
- *   act_dev [T][n][2] float32 or NULL: NULL draws turn_rate and walk_speed uniform on [-1, 1) from the counter-based
- *   generator (seed act_seed, keyed by the global env index, counted across calls), written to act_out_dev [T][n][2]
- *   if not NULL.  obs_dev [T][n][res_h][res_v][3] (uint8, int32 or float32), rew_dev [T][n] float64,
- *   done_dev [T][n] uint8.  Refused while output mirrors are set.  Stream-ordered, no host synchronisation. */
-int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
-                                void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream);
-/* mgb_maze_rollout_continuous with the two optional outputs of mgb_maze_step_continuous_ex, per step (both NULL: exactly
- * mgb_maze_rollout_continuous).  Any other handle kind is MGB_ERR_ARG.
- *   final_obs_dev [T][n][res_h][res_v][3] in the obs dtype: row (t, e) is written only when done[t][e] = 1, with the frame
- *     an auto_reset-off handle would have returned at step t (maze_continuous_3d.py:47-56 then the ray-cast observation on
- *     the state evaluation_rule left, maze_base.py:65-95).  Rows with done = 0 are not written.  Needs auto_reset on.
- *   truncated_dev [T][n] uint8, written for every (t, e): 1 iff done and the episode ended only through the step limit
- *     (maze_base.py:80,91-95,191-192).
- * A finished env costs one more frame in the same launch.  obs, rew, done, the drawn actions, the generator's step counter,
- * the env state and the pose are bit for bit what mgb_maze_rollout_continuous gives.  Refused while output mirrors or
- * multicast are set.  Stream-ordered, no host synchronisation, no allocation after the first call of the handle's
- * renderer (reset() makes it): capturable in a CUDA graph. */
-int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,
-                                   void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
-                                   uint8_t *truncated_dev, void *stream);
-/* T consecutive steps of a MetaMazeDiscrete3D or MetaMazeContinuous3D handle in ONE launch of the direct renderer (every
- * frame ray-cast; a discrete handle's pose cache, if any, is not used), optionally giving every env whose episode ends a
- * freshly drawn maze in the same launch -- the data-generation loop of meta-RL over an endless stream of tasks.
- *   act_dev: discrete int32 [T][n] in 0..3, continuous float32 [T][n][2]; NULL draws the actions exactly as
- *   mgb_maze_rollout (discrete) or mgb_maze_rollout_continuous (continuous) do for the same act_seed and step counter,
- *   written to act_out_dev (same shape) if not NULL.  obs_dev [T][n][res_h][res_v][3], rew_dev [T][n] float64,
- *   done_dev [T][n] uint8; final_obs_dev / truncated_dev as in mgb_maze_rollout_discrete_ex (NULL: not produced).
- *   resample_cfg NULL: no resampling; this is then a plain rollout whose outputs and state are bit for bit those of T
- *   step() calls (discrete) or of mgb_maze_rollout_continuous_ex (continuous).
- *   resample_cfg set: when env e finishes at step t (done, auto-reset on), it gets the task mgb_maze_resample_tasks(mask
- *   with only e set, resample_cfg, resample_seed) would give it -- written into its table slot, resample count + 1 -- and
- *   starts its next episode on it: obs[t][e] is the first frame on the NEW maze, final_obs[t][e] the terminal frame on the
- *   old one.  That equals, step for step, step_ex + resample_tasks(done) + reset(mask = done) (without the extra render).
- * Refused (MGB_ERR_ARG, handle untouched): a MetaMaze2D handle, T <= 0, output mirrors or multicast set, final_obs without
- * auto-reset; with resample_cfg also auto-reset off and every refusal of mgb_maze_resample_tasks (one slot per env, a
- * discrete handle whose pose cache is in use, the cfg checks) with the same messages.
- * Advances the step counter by T.  Stream-ordered, no host synchronisation, no allocation after the handle's first
- * reset(): capturable in a CUDA graph. */
-int mgb_maze_rollout_direct(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
-                            void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
-                            uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
-                            void *stream);
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

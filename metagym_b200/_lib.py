@@ -91,8 +91,7 @@ SIGNATURES = {
     "mgb_maze_cache_info": (ctypes.c_int, [vp, vp]),
     "mgb_maze_update_tasks": (ctypes.c_int, [vp, c_i32, vp, vp, vp, vp, vp, ctypes.POINTER(MazeTaskScalars), vp]),
     "mgb_maze_reset": (ctypes.c_int, [vp, vp, vp, vp]),
-    "mgb_maze_step": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
-    "mgb_maze_step_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_step": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_set_options": (ctypes.c_int, [vp, ctypes.c_int]),
     "mgb_peer_alloc": (ctypes.c_int, [ctypes.c_int, c_u64, ctypes.POINTER(ctypes.c_void_p)]),
     "mgb_peer_free": (ctypes.c_int, [ctypes.c_int, vp]),
@@ -105,17 +104,8 @@ SIGNATURES = {
     "mgb_maze_set_mirror_window": (ctypes.c_int, [vp, vp, c_u64]),
     "mgb_quad_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
     "mgb_maze_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
-    "mgb_maze_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
-    "mgb_maze_rollout_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
-    "mgb_maze_step_continuous": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
-    "mgb_maze_step_continuous_ex": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
-    "mgb_maze_rollout_continuous": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp]),
-    "mgb_maze_rollout_discrete_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
-    "mgb_maze_rollout_continuous_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
-    "mgb_maze_rollout_direct": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp,
-                                               ctypes.POINTER(MazeSamplerCfg), c_u64, vp]),
-    "mgb_maze_rollout_resample": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp,
-                                                 ctypes.POINTER(MazeSamplerCfg), c_u64, vp]),
+    "mgb_maze_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, ctypes.POINTER(MazeSamplerCfg),
+                                        c_u64, vp]),
     "mgb_maze_rollout_policy": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_u64, ctypes.POINTER(MazeSamplerCfg),
                                                c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),

@@ -127,7 +127,7 @@ struct MazeArgs {
     int auto_reset;
     float *act_out_c;            // continuous-maze rollout: drawn actions [T][n][2] (last, so the other kernels' parameter
                                  // offsets do not move)
-    // terminal observations of auto-reset steps (mgb_maze_step_ex).  The step logic of a finished env appends its terminal
+    // terminal observations of auto-reset steps (mgb_maze_step).  The step logic of a finished env appends its terminal
     // state to a compact list before env_reset; a second pass renders the list into final_obs[fin_env[i]].
     uint8_t *truncated;          // [n] 1: done only through the step limit; nullptr: not produced
     void *final_obs;             // 2-D: [n][2g+1][2g+1] float32, written by the step kernel itself; 3-D: set on the list pass
@@ -155,8 +155,8 @@ struct MazeArgs {
     int var_bits;                // variant bits of the table: a task takes the largest bits <= var_bits whose frames fit V
 };
 
-// in-launch task resampling (maze3d_kernel<.., RS>, mgb_maze_rollout_direct; maze2d_rollout_kernel<0, .., RS>,
-// mgb_maze_rollout_resample): an env whose episode ends gets the task mgb_maze_resample_tasks would draw for it.  A
+// in-launch task resampling (maze3d_kernel<.., RS> and maze2d_rollout_kernel<0, .., RS>, mgb_maze_rollout with a
+// sampler cfg): an env whose episode ends gets the task mgb_maze_resample_tasks would draw for it.  A
 // parameter of those kernels after MazeArgs, so that no other parameter offsets move.
 struct MazeResample {
     SamplerCfg cfg;
@@ -489,11 +489,11 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 
 // T MetaMaze2D steps in one launch: the agent (cell, step counter, life) stays in registers, food stamps stay in their
 // SoA slots, each step's observation tile of the CTA leaves through double-buffered shared memory + one bulk store.
-// XM: 0 plain, 1 peer mirrors, 2 multicast-only stores (see quad_rollout_kernel).  FIN (XM == 0 only, mgb_maze_rollout_ex):
+// XM: 0 plain, 1 peer mirrors, 2 multicast-only stores (see quad_rollout_kernel).  FIN (XM == 0 only, final_obs / truncated):
 // also store the truncation byte of every (t, e), and the terminal window of every env that finished at step t to
 // final_obs + (t n + e) D, both before env_reset; rows of envs that did not finish are not written.  REC: path recording on
 // (a.path set); the instantiations without it have no store and no test of a.path in their loop.
-// RS (XM == 0 only, mgb_maze_rollout_resample): an env that finishes at step t gets the task mgb_maze_resample_tasks would
+// RS (XM == 0 only, a sampler cfg): an env that finishes at step t gets the task mgb_maze_resample_tasks would
 // draw for it (after its reward, done, truncation byte and terminal window, all on the old task) and restarts on it, so
 // obs[t] is its first window on the new maze.  The sampler is warp-collective: the done ballot is taken by all 32 lanes
 // (the tail warp's lanes past n included), the warp draws one task per finished lane in lane order into that lane's table
@@ -801,9 +801,9 @@ __device__ __forceinline__ void push_terminal_state(const MazeConst &c, const Ma
 //               env_reset, stores the state and builds the record set of the new episode's first frame for obs[t][env].
 //               The destination travels with the record set; whether a reset item follows is published in shared memory
 //               before the trip's closing barrier, so every thread takes the same next item.
-// ROLL entry points: mgb_maze_rollout_direct and mgb_maze_rollout_continuous[_ex]; a discrete item reads the action
+// ROLL: mgb_maze_rollout of a 3-D handle off the pose cache; a discrete item reads the action
 //               act[t][env] or draws it like maze3d_rollout_kernel.
-// RS (ROLL only, mgb_maze_rollout_direct with a sampler cfg): an item that resets its env (the item itself, or with FIN its
+// RS (ROLL only, mgb_maze_rollout with a sampler cfg): an item that resets its env (the item itself, or with FIN its
 //               reset item) first gives the env a new task: warp 0 of the geometry group draws it into the item's tile
 //               buffer (maze_sample_task), copies the tile to the env's table slot and fences the generic writes against
 //               the bulk copies that load the slot later; thread 0 then resets the env on the new tile.  The next item's
@@ -1681,7 +1681,7 @@ __device__ __forceinline__ EnvDyn make_dyn(const MazeConst &c, const MazeArgs &a
     return d;
 }
 
-// a finished env's terminal state joins the list pass of mgb_maze_step_ex (before env_reset): the pose cache keeps its EnvDyn,
+// a finished env's terminal state joins the list pass of mgb_maze_step (before env_reset): the pose cache keeps its EnvDyn,
 // the direct renderer everything geometry() reads
 __device__ __forceinline__ void push_terminal(const MazeConst &c, const MazeArgs &a, int64_t e, int task, const uint8_t *blob,
                                               const Env &s, const int32_t *eaten)
@@ -2138,7 +2138,7 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_compose_kernel(cons
     const int total_px = f.total_px;
     // slice boundaries stay 128-pixel aligned; the slices cover the frame even when it has fewer pixels than slices
     const int part_px = ((total_px + kParts - 1) / kParts + 127) / 128 * 128;
-  // list pass of mgb_maze_step_ex (final_obs set): item = (terminal list entry, slice), frame into final_obs[fin_env[entry]]
+  // list pass of mgb_maze_step (final_obs set): item = (terminal list entry, slice), frame into final_obs[fin_env[entry]]
   const int64_t n_items = (a.final_obs ? (int64_t)*a.fin_count : a.n) * kParts;
   // bake mode (pose-cache build): item = pose slot, every food present, no life bar, tintable groups only
   auto fetch = [&](int64_t idx) -> EnvDyn {
@@ -2377,7 +2377,7 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
 // T MetaMazeDiscrete3D steps in one launch (pose-cache path): one CTA per env; thread 0 runs the step logic and leaves the
 // env's EnvDyn in shared memory, then the whole CTA composes frame t straight into obs[t][env].  No logic launch, no
 // EnvDyn round trip through global memory, and the logic of one env overlaps the pixels of the others on the SM.
-// FIN (mgb_maze_rollout_discrete_ex): thread 0 also stores the truncation byte of every (t, env) and, for an env that
+// FIN (final_obs / truncated): thread 0 also stores the truncation byte of every (t, env) and, for an env that
 // finished at step t, publishes the EnvDyn of its terminal state in a second slot -- both before env_reset, which clears the
 // food stamps the terminal frame still shows.  The CTA then composes that frame into final_obs + (t n + env) frame, a
 // barrier later the usual observation: one compose_item per pass, one deferred-tint queue.
@@ -2496,7 +2496,7 @@ __global__ void maze_state_kernel(MazeArgs a, int32_t *agent_out, double *life_o
 // ---------------------------------------------------------------------------------------------------------------
 // handle + C ABI
 // ---------------------------------------------------------------------------------------------------------------
-struct MazeFinal {                 // the terminal list of mgb_maze_step_ex (MazeArgs::fin_*, 3-D kinds)
+struct MazeFinal {                 // the terminal list of mgb_maze_step (MazeArgs::fin_*, 3-D kinds)
     MgbDev<int32_t> count, env, task, eaten;
     MgbDev<EnvDyn> dyn;
     MgbDev<int4> agent;
@@ -3485,7 +3485,7 @@ static int maze_refuse(const char *fn, const char *msg)
     return MGB_ERR_ARG;
 }
 
-// What device resampling needs of the handle and of the sampler cfg (mgb_maze_resample_tasks, mgb_maze_rollout_direct):
+// What device resampling needs of the handle and of the sampler cfg (mgb_maze_resample_tasks, mgb_maze_rollout):
 // the refusal, or nullptr with sc derived from cfg
 static const char *sampler_cfg(const mgb_maze *h, const mgb_maze_sampler_cfg *cfg, SamplerCfg &sc)
 {
@@ -3847,7 +3847,7 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     return MGB_OK;
 }
 
-// Paths other than the fused step keep their terminal states in a list (mgb_maze_step_ex): clear its length, and leave
+// Paths other than the fused step keep their terminal states in a list (mgb_maze_step): clear its length, and leave
 // a.final_obs to the list pass, which step_ex launches after the step.  `listed`: a list was started.
 static int start_terminal_list(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t st)
 {
@@ -3939,7 +3939,7 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t s
     return MGB_OK;
 }
 
-// One step with the optional outputs of mgb_maze_step_ex (obs, rew, done and the state are exactly what they are without
+// One step with the optional outputs of mgb_maze_step (obs, rew, done and the state are exactly what they are without
 // them).  2-D: the step kernel writes the terminal windows itself.  Fused 3-D step: the terminal frames are extra frames of
 // the same launch.  Other 3-D paths: the step logic appends each finished env's terminal state to a list before resetting
 // it, then one more launch renders the list into final_obs: the compose kernel over the terminal EnvDyn records on the pose
@@ -3947,7 +3947,6 @@ static int launch_observe(mgb_maze *h, MazeArgs &a, bool &listed, cudaStream_t s
 // is fixed, and its work is one frame per finished env.
 static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated, cudaStream_t st)
 {
-    MGB_REQUIRE(!final_obs || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal frame)");
     a.truncated = truncated;
     a.final_obs = final_obs;
     const MazeFinal &fin = h->tasks.fin;
@@ -3979,23 +3978,6 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     return MGB_OK;
 }
 
-
-// The four single-step entry points: refusals are made as `fn`, with kind_msg for a handle of the other action type
-// (`continuous`: float [n][2] actions of a MGB_MAZE_CONTINUOUS_3D handle; otherwise int32 [n] actions).
-static int step(const char *fn, bool continuous, const char *kind_msg, mgb_maze *h, const void *act_dev, void *obs_dev,
-                double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev, void *stream)
-{
-    if (!(h && act_dev && obs_dev && rew_dev && done_dev)) return maze_refuse(fn, "null argument");
-    if ((h->c.kind == MGB_MAZE_CONTINUOUS_3D) != continuous) return maze_refuse(fn, kind_msg);
-    int rc = maze_ready(h);
-    if (rc) return rc;
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    if (continuous) a.act_c = static_cast<const float *>(act_dev);
-    else a.act = static_cast<const int32_t *>(act_dev);
-    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
-}
 
 extern "C" int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_dev, void *stream)
 {
@@ -4064,120 +4046,32 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
     return MGB_OK;
 }
 
-// Rollout of a MetaMaze2D or MetaMazeDiscrete3D handle; `own`: the entry point's kind checks (see check_rollout)
-template <class Own>
-static int rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                   void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
-                   void *stream, Own own)
+// The engine mgb_maze_rollout runs for the handle: the 2-D rollout kernel for MetaMaze2D; for MetaMazeDiscrete3D without
+// resampling the pose cache when ensure_pose_cache leaves it ready (the choice launch_observe makes for a step); the direct
+// raycaster otherwise.  It builds the pose cache when one is due, so it runs after every check that does not depend on
+// the engine.
+enum class RolloutEngine { grid2d, pose_cache, direct };
+
+static int rollout_engine(mgb_maze *h, bool resample, cudaStream_t st, RolloutEngine &eng)
 {
-    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, own);
-    if (rc) return rc;
-    const bool fin = final_obs_dev || truncated_dev;
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base; a.act_out = act_out_dev;
-    a.mir = h->mir;
-    if (h->mir.count != 0)
-        MGB_REQUIRE(h->mir_win.holds_rollout((uint64_t)T * h->n, obs_dev, (uint64_t)mgb_maze_obs_bytes_per_env(h), rew_dev, 8,
-                                             done_dev, act_out_dev, 4),
-                    "mirrors are on but an output lies outside the mirrored arena (set_mirrors([]) first)");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (h->c.kind == MGB_MAZE_DISCRETE_3D) {
-        MGB_REQUIRE(h->mir.count == 0, "output mirrors are implemented for the MetaMaze2D rollout only");
-        rc = ensure_pose_cache(h, st);
-        if (rc) return rc;
-        MGB_REQUIRE(h->cache_ready, "the fused 3-D rollout runs on the pose cache (MGB_MAZE_CACHE=0 or cache budget too small)");
-        bind_pose_cache(h->cache, a);
-        const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers
-        const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
-        MGB_REQUIRE(qbytes <= 200 * 1024, "screen too large for the fused rollout's group queue");
-        const unsigned grid = (unsigned)(h->n < resident ? h->n : resident);
-        if (fin) {
-            if (qbytes > 40 * 1024)
-                MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<true>));
-            a.final_obs = final_obs_dev;
-            a.truncated = truncated_dev;
-            maze3d_rollout_kernel<true><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
-        } else {
-            if (qbytes > 40 * 1024)
-                MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<false>));
-            maze3d_rollout_kernel<false><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
-        }
-        MGB_CUDA(cudaGetLastError());
-        h->t_base += (uint32_t)T;
-        h->launches += 1;
-        return MGB_OK;
-    }
-    const int W = 2 * h->c.view_grid + 1;
-    const size_t sm = (size_t)2 * k2dThreads * W * W * 4;
-    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
-    if (h->mir.count == MGB_MIRROR_MULTICAST) {
-        MGB_REQUIRE(h->n % 4 == 0, "multicast outputs need num_envs % 4 == 0");
-        MGB_REQUIRE((((uintptr_t)done_dev | (uintptr_t)obs_dev | (uintptr_t)act_out_dev) & 3) == 0 && ((uintptr_t)rew_dev & 7) == 0,
-                    "multicast outputs must be 4-byte (rewards: 8-byte) aligned");
-    }
-    if (fin) {
-        a.final_obs = final_obs_dev;
-        a.truncated = truncated_dev;
-    }
-    const int xm = h->mir.count == MGB_MIRROR_MULTICAST ? 2 : (h->mir.count > 0 ? 1 : 0);
-    rc = h->path ? launch_2d_rollout<true>(h->c, xm, fin, a, blocks, sm, st)
-                 : launch_2d_rollout<false>(h->c, xm, fin, a, blocks, sm, st);
-    if (rc) return rc;
-    h->t_base += (uint32_t)T;
-    h->launches += 1;
-    return MGB_OK;
+    eng = h->c.kind == MGB_MAZE_2D ? RolloutEngine::grid2d : RolloutEngine::direct;
+    if (h->c.kind != MGB_MAZE_DISCRETE_3D || resample) return MGB_OK;
+    const int rc = ensure_pose_cache(h, st);
+    if (rc == MGB_OK && h->cache_ready) eng = RolloutEngine::pose_cache;
+    return rc;
 }
 
-// The handle kinds of mgb_maze_rollout and mgb_maze_rollout_ex (fin: final_obs or truncated requested)
-static const char *grid_rollout_refusal(const mgb_maze *h, bool fin)
-{
-    if (h->c.kind != MGB_MAZE_2D && h->c.kind != MGB_MAZE_DISCRETE_3D)
-        return "mgb_maze_rollout serves MetaMaze2D and MetaMazeDiscrete3D";
-    return fin && h->c.kind != MGB_MAZE_2D ? "final_obs / truncated of a rollout are produced for MetaMaze2D only" : nullptr;
-}
-
-extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed, int32_t *act_out_dev,
-                                void *obs_dev, double *rew_dev, uint8_t *done_dev, void *stream)
+extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
+                                void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
+                                uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout");
-    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, nullptr, nullptr, stream,
-                   [h] { return grid_rollout_refusal(h, false); });
-}
-
-extern "C" int mgb_maze_rollout_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
-                                   int32_t *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                   void *final_obs_dev, uint8_t *truncated_dev, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_rollout_ex");
-    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
-                   stream, [=] { return grid_rollout_refusal(h, final_obs_dev || truncated_dev); });
-}
-
-extern "C" int mgb_maze_rollout_discrete_ex(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
-                                            int32_t *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                            void *final_obs_dev, uint8_t *truncated_dev, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_rollout_discrete_ex");
-    return rollout(h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
-                   stream, [h]() -> const char * {
-        if (h->c.kind != MGB_MAZE_DISCRETE_3D) return "mgb_maze_rollout_discrete_ex needs a MGB_MAZE_DISCRETE_3D handle";
-        return nullptr;
-    });
-}
-
-extern "C" int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *act_dev, uint64_t act_seed,
-                                         int32_t *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                         void *final_obs_dev, uint8_t *truncated_dev,
-                                         const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_rollout_resample");
     SamplerCfg sc;
     int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
-        if (h->c.kind != MGB_MAZE_2D)
-            return "mgb_maze_rollout_resample serves MetaMaze2D (the 3-D envs resample in mgb_maze_rollout_direct)";
-        if (!resample_cfg) return "null argument: resample_cfg is required";
+        if (h->c.kind != MGB_MAZE_2D && h->mir.count != 0)
+            return "output mirrors are not implemented for the 3-D rollouts (set_mirrors([]) first)";
+        if (!resample_cfg) return nullptr;
         if (!h->auto_reset) return "resampling finished envs needs auto_reset on";
         if (h->mir.count != 0)
             return "output mirrors and multicast are not implemented for the resampling rollout (set_mirrors([]) first)";
@@ -4185,28 +4079,79 @@ extern "C" int mgb_maze_rollout_resample(mgb_maze *h, int32_t T, const int32_t *
     });
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
-    // two observation tiles, then one sampler workspace per warp (16-byte multiples)
-    const int W = 2 * h->c.view_grid + 1;
-    const size_t sm = (size_t)2 * k2dThreads * W * W * 4 + (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
-    int optin = 0;
-    MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-    if (sm > (size_t)optin) {
-        mgb_set_error("%s: the resampling rollout needs %zu bytes of shared memory per CTA at n = %d and view_grid = %d, "
-                      "more than the %d the device allows (use a smaller view_grid)", __func__, sm, h->c.n, h->c.view_grid,
-                      optin);
-        return MGB_ERR_ARG;
-    }
-    MazeArgs a = maze_args(h);
-    a.act = act_dev; a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base; a.act_out = act_out_dev;
-    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
-    MazeResample r = {};
-    r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
-    const bool fin = final_obs_dev || truncated_dev;
-    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     const cudaStream_t st = (cudaStream_t)stream;
-    rc = h->path ? launch_2d_rollout<true>(h->c, 0, fin, a, blocks, sm, st, &r)
-                 : launch_2d_rollout<false>(h->c, 0, fin, a, blocks, sm, st, &r);
+    RolloutEngine eng;
+    rc = rollout_engine(h, resample_cfg != nullptr, st, eng);
+    if (rc) return rc;
+    if (eng == RolloutEngine::direct && !(obs_dev && rew_dev && done_dev)) return maze_refuse(__func__, "null argument");
+    MazeArgs a = maze_args(h);
+    if (h->c.kind == MGB_MAZE_CONTINUOUS_3D) {
+        a.act_c = static_cast<const float *>(act_dev); a.act_out_c = static_cast<float *>(act_out_dev);
+    } else {
+        a.act = static_cast<const int32_t *>(act_dev); a.act_out = static_cast<int32_t *>(act_out_dev);
+    }
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+    const bool fin = final_obs_dev || truncated_dev;
+    MazeResample r = {};
+    if (resample_cfg) { r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get(); }
+    if (eng == RolloutEngine::pose_cache) {
+        const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers
+        const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
+        MGB_REQUIRE(qbytes <= 200 * 1024, "screen too large for the fused rollout's group queue");
+        const unsigned grid = (unsigned)(h->n < resident ? h->n : resident);
+        if (fin) {
+            if (qbytes > 40 * 1024)
+                MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<true>));
+            maze3d_rollout_kernel<true><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
+        } else {
+            if (qbytes > 40 * 1024)
+                MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<false>));
+            maze3d_rollout_kernel<false><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
+        }
+        MGB_CUDA(cudaGetLastError());
+    } else if (eng == RolloutEngine::direct) {
+        const unsigned grid = (unsigned)(h->n < h->num_sms ? h->n : h->num_sms);
+        if (fin)
+            rc = resample_cfg ? launch_render<false, true, true, true>(h, a, grid, st, r)
+                              : launch_render<false, true, true>(h, a, grid, st);
+        else
+            rc = resample_cfg ? launch_render<false, true, false, true>(h, a, grid, st, r)
+                              : launch_render<false, true>(h, a, grid, st);
+    } else if (resample_cfg) {
+        // two observation tiles, then one sampler workspace per warp (16-byte multiples)
+        const int W = 2 * h->c.view_grid + 1;
+        const size_t sm = (size_t)2 * k2dThreads * W * W * 4 + (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
+        int optin = 0;
+        MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+        if (sm > (size_t)optin) {
+            mgb_set_error("%s: the resampling rollout needs %zu bytes of shared memory per CTA at n = %d and view_grid = %d, "
+                          "more than the %d the device allows (use a smaller view_grid)", __func__, sm, h->c.n,
+                          h->c.view_grid, optin);
+            return MGB_ERR_ARG;
+        }
+        const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
+        rc = h->path ? launch_2d_rollout<true>(h->c, 0, fin, a, blocks, sm, st, &r)
+                     : launch_2d_rollout<false>(h->c, 0, fin, a, blocks, sm, st, &r);
+    } else {
+        if (h->mir.count != 0)
+            MGB_REQUIRE(h->mir_win.holds_rollout((uint64_t)T * h->n, obs_dev, (uint64_t)mgb_maze_obs_bytes_per_env(h),
+                                                 rew_dev, 8, done_dev, act_out_dev, 4),
+                        "mirrors are on but an output lies outside the mirrored arena (set_mirrors([]) first)");
+        if (h->mir.count == MGB_MIRROR_MULTICAST) {
+            MGB_REQUIRE(h->n % 4 == 0, "multicast outputs need num_envs % 4 == 0");
+            MGB_REQUIRE((((uintptr_t)done_dev | (uintptr_t)obs_dev | (uintptr_t)act_out_dev) & 3) == 0 && ((uintptr_t)rew_dev & 7) == 0,
+                        "multicast outputs must be 4-byte (rewards: 8-byte) aligned");
+        }
+        a.mir = h->mir;
+        const int W = 2 * h->c.view_grid + 1;
+        const size_t sm = (size_t)2 * k2dThreads * W * W * 4;
+        const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
+        const int xm = h->mir.count == MGB_MIRROR_MULTICAST ? 2 : (h->mir.count > 0 ? 1 : 0);
+        rc = h->path ? launch_2d_rollout<true>(h->c, xm, fin, a, blocks, sm, st)
+                     : launch_2d_rollout<false>(h->c, xm, fin, a, blocks, sm, st);
+    }
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
@@ -4254,7 +4199,7 @@ extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy 
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
         if (!resample_cfg) return nullptr;
-        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout_resample
+        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout
         return sampler_cfg(h, resample_cfg, sc);
     });
     if (rc) return rc;
@@ -4313,106 +4258,6 @@ extern "C" int mgb_maze_set_multicast(mgb_maze *h, int64_t byte_delta)
     const char *why = h->mir.set_multicast(byte_delta);
     MGB_REQUIRE(!why, why);
     return MGB_OK;
-}
-
-extern "C" int mgb_maze_step_continuous(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev,
-                                        uint8_t *done_dev, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_step_continuous");
-    return step(__func__, true, "mgb_maze_step_continuous needs a MGB_MAZE_CONTINUOUS_3D handle", h, act_dev, obs_dev,
-                rew_dev, done_dev, nullptr, nullptr, stream);
-}
-
-extern "C" int mgb_maze_step_continuous_ex(mgb_maze *h, const float *act_dev, void *obs_dev, double *rew_dev,
-                                           uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_step_continuous_ex");
-    return step(__func__, true, "mgb_maze_step_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle", h, act_dev, obs_dev,
-                rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
-}
-
-// The rollouts on the direct renderer (maze3d_kernel<false, true, ..>): mgb_maze_rollout_direct (both 3-D kinds) and the
-// continuous-maze entry points.  Refusals are made as `fn`: own() makes the entry point's kind checks (see check_rollout),
-// mirror_msg refuses output mirrors.  act / act_out: int32 [T][n] (discrete) or float32 [T][n][2] (continuous).  With
-// final_obs or truncated: maze3d_kernel<.., FIN>; with rs (the derived sampler cfg): maze3d_kernel<.., RS>.
-template <class Own>
-static int rollout_continuous(const char *fn, const char *mirror_msg, mgb_maze *h, int32_t T, const void *act_dev,
-                              uint64_t act_seed, void *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                              void *final_obs_dev, uint8_t *truncated_dev, const SamplerCfg *rs, uint64_t rs_seed,
-                              void *stream, Own own)
-{
-    int rc = check_rollout(fn, h, T, final_obs_dev, truncated_dev, own);
-    if (rc) return rc;
-    if (h->mir.count != 0) return maze_refuse(fn, mirror_msg);
-    MgbDeviceGuard guard(h->device);
-    MazeArgs a = maze_args(h);
-    if (h->c.kind == MGB_MAZE_CONTINUOUS_3D) {
-        a.act_c = static_cast<const float *>(act_dev); a.act_out_c = static_cast<float *>(act_out_dev);
-    } else {
-        a.act = static_cast<const int32_t *>(act_dev); a.act_out = static_cast<int32_t *>(act_out_dev);
-    }
-    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    a.T = T; a.act_seed = act_seed; a.t_base = h->t_base;
-    MazeResample r = {};
-    if (rs) { r.cfg = *rs; r.seed = rs_seed; r.epoch = h->task_epoch.get(); }
-    const unsigned grid = (unsigned)(h->n < h->num_sms ? h->n : h->num_sms);
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (final_obs_dev || truncated_dev) {
-        a.final_obs = final_obs_dev;
-        a.truncated = truncated_dev;
-        rc = rs ? launch_render<false, true, true, true>(h, a, grid, st, r) : launch_render<false, true, true>(h, a, grid, st);
-    } else {
-        rc = rs ? launch_render<false, true, false, true>(h, a, grid, st, r) : launch_render<false, true>(h, a, grid, st);
-    }
-    if (rc) return rc;
-    h->t_base += (uint32_t)T;
-    h->launches += 1;
-    return MGB_OK;
-}
-
-static const char *const kContinuousMirrors =
-    "output mirrors are not implemented for the continuous-maze rollout (set_mirrors([]) first)";
-
-extern "C" int mgb_maze_rollout_continuous(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
-                                           float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                           void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_rollout_continuous");
-    return rollout_continuous(__func__, kContinuousMirrors, h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev,
-                              nullptr, nullptr, nullptr, 0, stream, [&]() -> const char * {
-        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
-        return h->c.kind == MGB_MAZE_CONTINUOUS_3D ? nullptr : "mgb_maze_rollout_continuous needs a MGB_MAZE_CONTINUOUS_3D handle";
-    });
-}
-
-extern "C" int mgb_maze_rollout_continuous_ex(mgb_maze *h, int32_t T, const float *act_dev, uint64_t act_seed,
-                                              float *act_out_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                              void *final_obs_dev, uint8_t *truncated_dev, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_rollout_continuous_ex");
-    return rollout_continuous(__func__, kContinuousMirrors, h, T, act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev,
-                              final_obs_dev, truncated_dev, nullptr, 0, stream, [&]() -> const char * {
-        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
-        return h->c.kind == MGB_MAZE_CONTINUOUS_3D ? nullptr : "mgb_maze_rollout_continuous_ex needs a MGB_MAZE_CONTINUOUS_3D handle";
-    });
-}
-
-extern "C" int mgb_maze_rollout_direct(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
-                                       void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
-                                       uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
-                                       void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_rollout_direct");
-    SamplerCfg sc;
-    return rollout_continuous(__func__, "output mirrors are not implemented for the 3-D rollouts (set_mirrors([]) first)", h, T,
-                              act_dev, act_seed, act_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev,
-                              resample_cfg ? &sc : nullptr, resample_seed, stream, [&]() -> const char * {
-        if (!(obs_dev && rew_dev && done_dev)) return "null argument";
-        if (h->c.kind == MGB_MAZE_2D) return "mgb_maze_rollout_direct serves MetaMazeDiscrete3D and MetaMazeContinuous3D";
-        if (!resample_cfg) return nullptr;
-        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";
-        return sampler_cfg(h, resample_cfg, sc);
-    });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -4878,20 +4723,22 @@ extern "C" int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void 
     return MGB_OK;
 }
 
-extern "C" int mgb_maze_step(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                             void *stream)
+// act_dev: float [n][2] for a MGB_MAZE_CONTINUOUS_3D handle, int32 [n] otherwise
+extern "C" int mgb_maze_step(mgb_maze *h, const void *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                             void *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_step");
-    return step(__func__, false, "use mgb_maze_step_continuous for the continuous maze", h, act_dev, obs_dev, rew_dev,
-                done_dev, nullptr, nullptr, stream);
-}
-
-extern "C" int mgb_maze_step_ex(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                void *final_obs_dev, uint8_t *truncated_dev, void *stream)
-{
-    MgbRange nvtx_range("mgb_maze_step_ex");
-    return step(__func__, false, "use mgb_maze_step_continuous_ex for the continuous maze", h, act_dev, obs_dev, rew_dev,
-                done_dev, final_obs_dev, truncated_dev, stream);
+    MGB_REQUIRE(h && act_dev && obs_dev && rew_dev && done_dev, "null argument");
+    int rc = maze_ready(h);
+    if (rc) return rc;
+    MGB_REQUIRE(!final_obs_dev || h->auto_reset,
+                "final_obs needs auto_reset on (without it obs already is the terminal frame)");
+    MgbDeviceGuard guard(h->device);
+    MazeArgs a = maze_args(h);
+    if (h->c.kind == MGB_MAZE_CONTINUOUS_3D) a.act_c = static_cast<const float *>(act_dev);
+    else a.act = static_cast<const int32_t *>(act_dev);
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
 }
 
 extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev, void *stream)

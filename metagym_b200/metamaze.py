@@ -438,29 +438,23 @@ class _BatchedMazeBase(Snapshots):
         if act.dtype is not act_dtype or not act.is_contiguous() or act.shape != shape:
             act = action.to(act_dtype).reshape(shape).contiguous()
         if self._own_ptrs is None or self._own_ptrs[0] != self._obs.data_ptr():
-            self._own_ptrs = (self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr())
-            if self._final is not None:
-                self._own_ptrs += (self._final.data_ptr(), self._trunc.data_ptr())
-            self._step_fn = getattr(self._lib, self._STEP_ENTRIES[self._final is not None])
+            self._own_ptrs = (self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr(),
+                              _lib.ptr(self._final), _lib.ptr(self._trunc))
             self._done_bool = self._done.view(torch.bool)
-        rc = self._step_fn(self._h, act.data_ptr(), *self._own_ptrs, self._stream())
+        rc = self._lib.mgb_maze_step(self._h, act.data_ptr(), *self._own_ptrs, self._stream())
         if rc:
             _lib.check(rc)
         info = _LazySteps(self)
         return self._out(self._obs), self._out(self._rew), self._out(self._done_bool), info
 
-    # step() and rollout(): the C entry points without / with the final_obs and truncated outputs, the layout of one
-    # env's action, the numpy dtype host actions are read as (None: as given), and whether the "act" output also
-    # records actions the caller passed in (or only device-drawn ones)
-    _STEP_ENTRIES = ("mgb_maze_step", "mgb_maze_step_ex")
-    _ROLLOUT_ENTRIES = ("mgb_maze_rollout", "mgb_maze_rollout_ex")
+    # step() and rollout(): the layout of one env's action, the numpy dtype host actions are read as (None: as given),
+    # and whether the "act" output also records actions the caller passed in (or only device-drawn ones)
     _ACT_DTYPE, _ACT_SHAPE, _ACT_HOST_DTYPE = "int32", (), None
     _RECORDS_GIVEN_ACTIONS = True
 
-    def _rollout(self, T, actions, act_seed, want_actions, out, final=False, direct=False, resample=None):
-        """final: also produce the "final_obs" / "truncated" entries (through _ROLLOUT_ENTRIES[1]).  direct (3-D kinds):
-        run mgb_maze_rollout_direct instead, resampling finished envs' tasks when `resample` (resample_tasks' keyword
-        arguments with seed) is given.  MetaMaze2D with `resample`: mgb_maze_rollout_resample."""
+    def _rollout(self, T, actions, act_seed, want_actions, out, final=False, resample=None):
+        """mgb_maze_rollout.  final: also produce the "final_obs" / "truncated" entries.  resample: resample_tasks'
+        keyword arguments with seed, to give finished envs a freshly drawn task in the same launch."""
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -478,18 +472,13 @@ class _BatchedMazeBase(Snapshots):
         a = None
         if actions is not None:
             a = torch.as_tensor(actions, dtype=act_dtype, device=dev).reshape(act_shape).contiguous()
-        args = [_lib.ptr(a), int(act_seed), _lib.ptr(out.get("act") if record else None), _lib.ptr(out.get("obs")),
-                _lib.ptr(out.get("rew")), _lib.ptr(out.get("done"))]
-        if direct or resample is not None:
-            cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
-            args += [_lib.ptr(out.get("final_obs") if final else None), _lib.ptr(out.get("truncated") if final else None),
-                     None if cfg is None else ctypes.byref(cfg), seed]
-            entry = self._lib.mgb_maze_rollout_direct if direct else self._lib.mgb_maze_rollout_resample
-            _lib.check(entry(self._h, T, *args, self._stream()))
-            return out
-        if final:
-            args += [_lib.ptr(out.get("final_obs")), _lib.ptr(out.get("truncated"))]
-        _lib.check(getattr(self._lib, self._ROLLOUT_ENTRIES[final])(self._h, T, *args, self._stream()))
+        cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+        _lib.check(self._lib.mgb_maze_rollout(self._h, T, _lib.ptr(a), int(act_seed),
+                                              _lib.ptr(out.get("act") if record else None), _lib.ptr(out.get("obs")),
+                                              _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
+                                              _lib.ptr(out.get("final_obs") if final else None),
+                                              _lib.ptr(out.get("truncated") if final else None),
+                                              None if cfg is None else ctypes.byref(cfg), seed, self._stream()))
         return out
 
     def _check_rollout_final(self, final_obs):
@@ -696,7 +685,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         caller-supplied `out` may omit either entry, and that output is then not produced.
 
         resample: None, or resample_tasks' keyword arguments with its seed, e.g. dict(seed=5, crowd_ratio=0.35)
-        (mgb_maze_rollout_resample).  Every env whose episode ends at step t then gets the maze resample_tasks(done,
+        Every env whose episode ends at step t then gets the maze resample_tasks(done,
         **resample) would give it, in the same launch: obs[t] is its first window on the new maze, final_obs[t] the
         terminal window on the old one.  Needs auto_reset=True and set_task() with one table slot per env, like
         resample_tasks; with n = 31 the view_grid may be at most 6.
@@ -756,7 +745,6 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     same values in the dtype the reference's observation_space declares (maze_env.py:37-39), 'uint8' = min(value, 255).
     textures: (grounds uint8 [n_tex,64,64,3], ceil uint8 [64,64,3]); default = procedural set."""
     KIND = 1
-    _ROLLOUT_ENTRIES = ("mgb_maze_rollout", "mgb_maze_rollout_discrete_ex")
 
     def __init__(self, enable_render=False, render_scale=480, resolution=(320, 320), max_steps=5000,
                  task_type="SURVIVAL", num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True,
@@ -792,22 +780,22 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False, resample=None):
         """T steps in one launch: obs [T,N,res_h,res_v,3] (uint8, int32 or float32), rew, done, act as for
-        BatchedMetaMaze2D.rollout.  Runs on the pose cache, or on the direct raycaster (mgb_maze_rollout_direct) for an
-        env created with cache=False or when `resample` is given; both give the same results.
+        BatchedMetaMaze2D.rollout (mgb_maze_rollout).  Runs on the pose cache when it is in use, otherwise (an env created
+        with cache=False, or when `resample` is given) on the direct raycaster; both give the same results.
 
         final_obs (per call, independent of the constructor's final_obs, which concerns step()): False returns only the
-        entries above.  True needs auto_reset=True (ValueError otherwise) and calls mgb_maze_rollout_discrete_ex: the
-        dict also holds "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e
-        if done[t, e] (what step() reports as final_observation; allocated with torch.empty, rows with done 0 are not
-        written), and "truncated" [T,N] uint8, written for every step: 1 iff done and the episode ended only through
-        max_steps.  A caller-supplied `out` may omit either entry, and that output is then not produced.
+        entries above.  True needs auto_reset=True (ValueError otherwise), and the dict also holds "final_obs"
+        [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e if done[t, e] (what
+        step() reports as final_observation; allocated with torch.empty, rows with done 0 are not written), and
+        "truncated" [T,N] uint8, written for every step: 1 iff done and the episode ended only through max_steps.  A
+        caller-supplied `out` may omit either entry, and that output is then not produced.
 
         resample: None, or resample_tasks' keyword arguments with its seed, e.g. dict(seed=5, crowd_ratio=0.35).  Every
         env whose episode ends at step t then gets the maze resample_tasks(done, **resample) would give it, in the same
         launch: obs[t] is its first frame on the new maze, final_obs[t] the terminal frame on the old one.  Needs
         auto_reset=True, cache=False and set_task() with one table slot per env, like resample_tasks."""
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs),
-                             direct=resample is not None or self.cache is False, resample=resample)
+                             resample=resample)
 
     def cache_info(self):
         """Pose-cache statistics (valid after the first reset()/step(); synchronises the device): dict(poses, variant_frames, variant_bits, bytes,
@@ -836,8 +824,6 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
     maze_continuous_3d.py:48-49); float32 position / float64 heading exactly as the reference computes them for
     float32 actions.  Every pose is unique, so this env always uses the direct float64 renderer."""
     KIND = 2
-    _STEP_ENTRIES = ("mgb_maze_step_continuous", "mgb_maze_step_continuous_ex")
-    _ROLLOUT_ENTRIES = ("mgb_maze_rollout_continuous", "mgb_maze_rollout_continuous_ex")
     _ACT_DTYPE, _ACT_SHAPE, _ACT_HOST_DTYPE = "float32", (2,), np.float32
     _RECORDS_GIVEN_ACTIONS = False
 
@@ -851,21 +837,21 @@ class BatchedMetaMazeContinuous3D(BatchedMetaMazeDiscrete3D):
         return cfg
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False, resample=None):
-        """T steps in one launch of the direct renderer (mgb_maze_rollout_continuous), exactly as T step() calls.
+        """T steps in one launch of the direct renderer (mgb_maze_rollout), exactly as T step() calls.
         actions: anything reshapeable to [T,N,2] (turn_rate, walk_speed), clipped to [-1, 1] like step(); None draws them
         on the device, uniform on [-1, 1) like action_space.sample().  Returns dict(obs [T,N,res_h,res_v,3] in the env's
         obs dtype, rew [T,N] f64, done [T,N] u8, act [T,N,2] f32: the drawn actions when want_actions, else None).
 
         final_obs (per call, independent of the constructor's final_obs, which concerns step()): True needs
-        auto_reset=True (ValueError otherwise) and calls mgb_maze_rollout_continuous_ex: the dict also holds
-        "final_obs" [T,N,res_h,res_v,3] in the obs dtype, where row (t, e) is the terminal frame of env e if done[t, e]
-        (allocated with torch.empty, rows with done 0 are not written), and "truncated" [T,N] uint8, written for every
-        step.  A caller-supplied `out` may omit either entry, and that output is then not produced.
+        auto_reset=True (ValueError otherwise), and the dict also holds "final_obs" [T,N,res_h,res_v,3] in the obs
+        dtype, where row (t, e) is the terminal frame of env e if done[t, e] (allocated with torch.empty, rows with done
+        0 are not written), and "truncated" [T,N] uint8, written for every step.  A caller-supplied `out` may omit either
+        entry, and that output is then not produced.
 
-        resample: as for BatchedMetaMazeDiscrete3D.rollout (mgb_maze_rollout_direct): every env whose episode ends at
-        step t gets a freshly drawn maze in the same launch, and obs[t] is its first frame on it."""
+        resample: as for BatchedMetaMazeDiscrete3D.rollout: every env whose episode ends at step t gets a freshly drawn
+        maze in the same launch, and obs[t] is its first frame on it."""
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs),
-                             direct=resample is not None, resample=resample)
+                             resample=resample)
 
     def pose(self):
         """-> (pos [N,2] float32 = _agent_loc, ori [N] float64 = _agent_ori)."""

@@ -1,4 +1,4 @@
-"""MetaMazeContinuous3D: T steps as one fused rollout launch (mgb_maze_rollout_continuous, device-drawn actions) against
+"""MetaMazeContinuous3D: T steps as one fused rollout launch (mgb_maze_rollout, device-drawn actions) against
 the same T steps as single step() launches replayed from a CUDA graph (pre-drawn actions).  Both run the direct renderer;
 the rollout saves the per-step launch and the step logic's round trip through a separate launch.
 

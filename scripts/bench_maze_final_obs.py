@@ -1,4 +1,4 @@
-"""Cost of terminal observations (final_obs=True: mgb_maze_step_ex / mgb_maze_step_continuous_ex) on auto-reset maze steps.
+"""Cost of terminal observations (final_obs=True: the optional outputs of mgb_maze_step) on auto-reset maze steps.
 
 Both arms replay T step() calls from a CUDA graph, like bench.py; one handle has final_obs off, the other on, with the
 same tasks and actions.  Cases: config 4 (1024 envs, 64 tasks, 15x15, 128x128 uint8, SURVIVAL, max_steps=200; the fused

@@ -1,5 +1,5 @@
 """Cost of the terminal observations and truncation flags of the fused rollouts (mgb_quad_rollout_ex,
-mgb_maze_rollout_ex, mgb_maze_rollout_discrete_ex, mgb_maze_rollout_continuous_ex) and of the quadrotor step's truncation
+and mgb_maze_rollout of the three maze kinds) and of the quadrotor step's truncation
 flag (mgb_quad_step_ex).
 
 Two handles per case, final_obs off and on, same configuration and seeds.  Each arm replays a CUDA graph, like bench.py:

@@ -1,6 +1,6 @@
 """GPU tests of time-limit truncation flags for quadrotor steps (mgb_quad_step_ex / mgb_quad_step_host_ex) and of
 terminal observations with truncation flags from the fused quadrotor and MetaMaze2D rollouts (mgb_quad_rollout_ex /
-mgb_maze_rollout_ex): against the CPU oracle, against step-driven twins bit for bit, and against handles without the new
+mgb_maze_rollout): against the CPU oracle, against step-driven twins bit for bit, and against handles without the new
 outputs, whose primary outputs must not move."""
 import numpy as np
 import pytest
@@ -388,7 +388,7 @@ def test_maze2d_rollout_ex_equals_steps(torch_mod, tasks, task_type, view_grid, 
 # --------------------------------------------------------------------------------------------------------------------
 # refusals
 # --------------------------------------------------------------------------------------------------------------------
-def test_refusals(torch_mod, tasks, textures):  # noqa: F811
+def test_final_obs_refusals(torch_mod, tasks, textures):  # noqa: F811
     torch = torch_mod
     from metagym_b200 import BatchedMetaMazeDiscrete3D, BatchedQuadrotor
     with pytest.raises(ValueError, match="auto_reset"):
@@ -416,29 +416,33 @@ def test_refusals(torch_mod, tasks, textures):  # noqa: F811
     m.set_task(tasks)
     m.reset()
     mfo = torch.zeros((T, n, 3, 3), device="cuda")
-    assert m._lib.mgb_maze_rollout_ex(m._h, T, None, 0, None, None, None, None, mfo.data_ptr(), None, m._stream()) \
-        == MGB_ERR_ARG
+    assert m._lib.mgb_maze_rollout(m._h, T, None, 0, None, None, None, None, mfo.data_ptr(), None, None, 0,
+                                   m._stream()) == MGB_ERR_ARG
     ma = _maze2d("SURVIVAL", 1, n, True)
     ma.set_task(tasks)
     ma.reset()
     for arm in (lambda: ma.set_mirrors([16]), lambda: ma.set_multicast(16)):
         arm()
         for f, tr in ((mfo, None), (None, u8)):
-            assert ma._lib.mgb_maze_rollout_ex(ma._h, T, None, 0, None, None, None, None, _ptr(f), _ptr(tr),
-                                               ma._stream()) == MGB_ERR_ARG
+            assert ma._lib.mgb_maze_rollout(ma._h, T, None, 0, None, None, None, None, _ptr(f), _ptr(tr), None, 0,
+                                            ma._stream()) == MGB_ERR_ARG
         ma.set_mirrors([])
-    # discrete 3-D: the new outputs do not exist for its rollout
-    d3 = BatchedMetaMazeDiscrete3D(resolution=(32, 32), obs_dtype="uint8", textures=textures, max_steps=MAX_STEPS,
-                                   num_envs=n, squeeze=False, auto_reset=True, final_obs=True)
-    d3.set_task(tasks)
-    d3.reset()
+    # discrete 3-D: the same call runs on the pose cache, as rollout(T, final_obs=True) of a twin does
+    d3, twin = (BatchedMetaMazeDiscrete3D(resolution=(32, 32), obs_dtype="uint8", textures=textures, max_steps=MAX_STEPS,
+                                          num_envs=n, squeeze=False, auto_reset=True, final_obs=True) for _ in range(2))
+    for e in (d3, twin):
+        e.set_task(tasks)
+        e.reset()
     f3 = torch.zeros((T, n, 32, 32, 3), dtype=torch.uint8, device="cuda")
     for f, tr in ((f3, None), (None, u8)):
-        assert d3._lib.mgb_maze_rollout_ex(d3._h, T, None, 0, None, None, None, None, _ptr(f), _ptr(tr),
-                                           d3._stream()) == MGB_ERR_ARG
+        assert d3._lib.mgb_maze_rollout(d3._h, T, None, 0, None, None, None, None, _ptr(f), _ptr(tr), None, 0,
+                                        d3._stream()) == 0
+        want = twin.rollout(T, final_obs=True)
+        d = want["done"].bool()
+        assert torch.equal(f3[d], want["final_obs"][d]) if tr is None else torch.equal(u8, want["truncated"])
     assert "final_obs" not in d3.rollout(T)
     torch.cuda.synchronize()
-    for e in (q, qa, m, ma, d3):
+    for e in (q, qa, m, ma, d3, twin):
         e.close()
 
 

@@ -1,5 +1,5 @@
-"""GPU tests of mgb_maze_rollout_resample: T MetaMaze2D steps in one launch of maze2d_rollout_kernel<0, FIN, REC, RS> that
-give every finished env a freshly drawn maze in the same launch (BatchedMetaMaze2D.rollout(T, resample=...)).
+"""GPU tests of mgb_maze_rollout with a sampler cfg: T MetaMaze2D steps in one launch of
+maze2d_rollout_kernel<0, FIN, REC, RS> that give every finished env a freshly drawn maze in the same launch (BatchedMetaMaze2D.rollout(T, resample=...)).
 
 Against the loop step + resample_tasks(done) + reset(mask=done) that returns the window on the new maze, against the CPU
 oracle fed the restated tasks (tests/maze_sampler_draws.py), across calls and a snapshot restore, refusals, and CUDA-graph
@@ -233,9 +233,9 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-def test_refusals_leave_the_handle_untouched(torch_mod, maze_golden):
-    """Each refusal of mgb_maze_rollout_resample returns MGB_ERR_ARG with its message (the sampler-cfg ones with the text
-    mgb_maze_resample_tasks gives for the same cfg) and leaves snapshot() as it was, and the handle runs afterwards;
+def test_resampling_refusals_leave_the_handle_untouched(torch_mod, maze_golden):
+    """Each refusal of mgb_maze_rollout with a sampler cfg returns MGB_ERR_ARG with its message (the sampler-cfg ones
+    with the text mgb_maze_resample_tasks gives for the same cfg) and leaves snapshot() as it was, and the handle runs afterwards;
     rollout(resample=dict(goal_reward=-1)) raises ValueError."""
     torch = torch_mod
     from metagym_b200 import BatchedMetaMaze2D, BatchedMetaMazeDiscrete3D, _lib
@@ -256,27 +256,29 @@ def test_refusals_leave_the_handle_untouched(torch_mod, maze_golden):
     def call(env, steps=T, f=False, tr=False, c="default"):
         obs, rew, done, fo, u8 = bufs(env)
         c = cfg() if c == "default" else c
-        return lib.mgb_maze_rollout_resample(env._h, steps, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(),
-                                             _ptr(fo) if f else None, _ptr(u8) if tr else None,
-                                             None if c is None else ctypes.byref(c), 9, env._stream())
+        return lib.mgb_maze_rollout(env._h, steps, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(),
+                                    _ptr(fo) if f else None, _ptr(u8) if tr else None,
+                                    None if c is None else ctypes.byref(c), 9, env._stream())
 
     def refused(env, text, **kw):
         before = records(env).clone()
         assert call(env, **kw) == MGB_ERR_ARG
         msg = lib.mgb_last_error().decode()
-        assert msg.startswith("mgb_maze_rollout_resample: ") and text in msg, msg
+        assert msg.startswith("mgb_maze_rollout: ") and text in msg, msg
         assert torch.equal(records(env), before)
-        return msg[len("mgb_maze_rollout_resample: "):]
+        return msg[len("mgb_maze_rollout: "):]
 
     env = make_env(N, n, table, max_steps=9, view_grid=2)
-    # a 3-D handle
+    # a 3-D handle resamples on the direct renderer (tests/test_maze3d_direct_rollout_gpu.py checks its outputs)
     d3 = BatchedMetaMazeDiscrete3D(resolution=(24, 16), max_steps=9, num_envs=N, squeeze=False, auto_reset=True, cache=False)
     d3.set_task(table, env2task=np.arange(N))
     d3.reset()
-    refused(d3, "mgb_maze_rollout_direct")
+    assert call(d3) == 0
+    torch.cuda.synchronize()
     for steps in (0, -1):
         refused(env, "T must be positive", steps=steps)
-    refused(env, "resample_cfg is required", c=None)
+    assert call(env, c=None) == 0                                           # without a cfg: the plain rollout
+    torch.cuda.synchronize()
     delta = np.array([16], np.int64)
     for arm in (lambda: lib.mgb_maze_set_mirrors(env._h, 1, delta.ctypes.data),
                 lambda: lib.mgb_maze_set_multicast(env._h, 16)):

@@ -1,5 +1,5 @@
-"""GPU tests of mgb_maze_rollout_direct: T steps of a MetaMazeDiscrete3D or MetaMazeContinuous3D handle in one launch of
-the direct raycaster (maze3d_kernel<false, true, FIN, RS>), optionally giving every finished env a freshly drawn maze in
+"""GPU tests of mgb_maze_rollout on the direct raycaster: T steps of a MetaMazeDiscrete3D or MetaMazeContinuous3D handle
+in one launch of maze3d_kernel<false, true, FIN, RS>, optionally giving every finished env a freshly drawn maze in
 the same launch (rollout(T, resample=...)).
 
 Against T step() calls of a cache=False twin, against the pose-cache rollout of a cached twin, against the loop
@@ -152,8 +152,8 @@ def test_discrete_direct_rollout_equals_single_steps(torch_mod, textures, tasks,
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype,task_type", [("uint8", "SURVIVAL"), ("int32", "ESCAPE")])
 def test_discrete_direct_rollout_equals_pose_cache_rollout(torch_mod, textures, tasks, monkeypatch, dtype, task_type):
-    """Drawn actions, two consecutive rollouts: the cache=False handle (mgb_maze_rollout_direct) and a cached twin
-    (mgb_maze_rollout_discrete_ex) give the same act_out, obs, rew, done, final_obs, truncated, state and step counter."""
+    """Drawn actions, two consecutive rollouts: the cache=False handle (direct renderer) and a cached twin (pose cache)
+    give the same act_out, obs, rew, done, final_obs, truncated, state and step counter."""
     torch = torch_mod
     n, res = 40, (32, 32)
     kw = dict(max_steps=11, task_type=task_type, auto_reset=True, env_index_base=BASE_HI)
@@ -308,10 +308,10 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-def test_refusals_leave_the_handle_untouched(torch_mod, textures, tasks, monkeypatch):
-    """Each refusal of mgb_maze_rollout_direct returns MGB_ERR_ARG with its message (the sampler-cfg ones with the text
-    mgb_maze_resample_tasks gives for the same cfg) and leaves snapshot() as it was; mgb_maze_rollout_discrete_ex on a
-    cache-less handle still refuses; rollout(resample=dict(goal_reward=-1)) raises ValueError."""
+def test_direct_rollout_refusals_leave_the_handle_untouched(torch_mod, textures, tasks, monkeypatch):
+    """Each refusal of mgb_maze_rollout on the direct renderer returns MGB_ERR_ARG with its message (the sampler-cfg
+    ones with the text mgb_maze_resample_tasks gives for the same cfg) and leaves snapshot() as it was; a MetaMaze2D
+    handle runs its own rollout; rollout(resample=dict(goal_reward=-1)) raises ValueError."""
     torch = torch_mod
     from metagym_b200 import BatchedMetaMaze2D, _lib
     n, T, res, N9 = 8, 3, (24, 16), 9
@@ -327,16 +327,16 @@ def test_refusals_leave_the_handle_untouched(torch_mod, textures, tasks, monkeyp
         return BatchedMetaMaze2D._sampler_cfg(**dict(dict(seed=3), **over))[0]
 
     def call(env, steps=T, f=None, tr=None, c=None):
-        return lib.mgb_maze_rollout_direct(env._h, steps, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(),
-                                           _ptr(f), _ptr(tr), None if c is None else ctypes.byref(c), 9, env._stream())
+        return lib.mgb_maze_rollout(env._h, steps, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(),
+                                    _ptr(f), _ptr(tr), None if c is None else ctypes.byref(c), 9, env._stream())
 
     def refused(env, text, **kw):
         before = env.snapshot()["records"].clone()
         assert call(env, **kw) == MGB_ERR_ARG
         msg = lib.mgb_last_error().decode()
-        assert msg.startswith("mgb_maze_rollout_direct: ") and text in msg, msg
+        assert msg.startswith("mgb_maze_rollout: ") and text in msg, msg
         assert torch.equal(env.snapshot()["records"], before)
-        return msg[len("mgb_maze_rollout_direct: "):]
+        return msg[len("mgb_maze_rollout: "):]
 
     def mk(kind, **kw):
         e = make_env(kind, n, res, "int32", textures, monkeypatch, **dict(dict(max_steps=9, auto_reset=True), **kw))
@@ -347,11 +347,20 @@ def test_refusals_leave_the_handle_untouched(torch_mod, textures, tasks, monkeyp
     m2 = BatchedMetaMaze2D(max_steps=9, num_envs=n, squeeze=False, auto_reset=True)
     m2.set_task(table, env2task=np.arange(n))
     m2.reset()
-    refused(m2, "serves MetaMazeDiscrete3D and MetaMazeContinuous3D")
+    assert call(m2) == 0                                                   # the 2-D rollout
+    torch.cuda.synchronize()
     envs = [mk("D3D", cache=False), mk("C3D")]
     for env in envs:
         for steps in (0, -1):
             refused(env, "T must be positive", steps=steps)
+        for k in range(3):                                                 # obs, rew or done missing
+            ptrs = [obs.data_ptr(), rew.data_ptr(), done.data_ptr()]
+            ptrs[k] = None
+            before = env.snapshot()["records"].clone()
+            rc = lib.mgb_maze_rollout(env._h, T, None, 0, None, *ptrs, None, None, None, 0, env._stream())
+            assert rc == MGB_ERR_ARG
+            assert lib.mgb_last_error().decode() == "mgb_maze_rollout: null argument"
+            assert torch.equal(env.snapshot()["records"], before)
         delta = np.array([16], np.int64)
         for arm in (lambda: lib.mgb_maze_set_mirrors(env._h, 1, delta.ctypes.data),
                     lambda: lib.mgb_maze_set_multicast(env._h, 16)):
@@ -388,11 +397,12 @@ def test_refusals_leave_the_handle_untouched(torch_mod, textures, tasks, monkeyp
     refused(cached, "the direct renderer", c=cfg())
     assert call(cached, f=fo, tr=u8) == 0
     torch.cuda.synchronize()
-    # the pose-cache entry point still refuses a cache-less handle
+    # a cache-less discrete handle without a cfg runs on the direct renderer: one launch, step counter + T
     nc = envs[0]
-    assert lib.mgb_maze_rollout_discrete_ex(nc._h, T, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(),
-                                            fo.data_ptr(), u8.data_ptr(), nc._stream()) == MGB_ERR_ARG
-    assert b"the fused 3-D rollout runs on the pose cache" in lib.mgb_last_error()
+    launches, t0 = nc.launch_count, t_base(nc)
+    assert call(nc, f=fo, tr=u8) == 0
+    torch.cuda.synchronize()
+    assert nc.launch_count == launches + 1 and t_base(nc) == t0 + T
     for e in envs + [m2, shared, cached]:
         e.close()
 

@@ -1,6 +1,6 @@
-"""GPU tests of terminal observations and truncation flags from the fused MetaMaze 3-D rollouts:
-mgb_maze_rollout_discrete_ex (maze3d_rollout_kernel<true>, pose cache) and mgb_maze_rollout_continuous_ex
-(maze3d_kernel<false, true, true>, direct renderer).  Against step() twins with final_obs=True bit for bit, against
+"""GPU tests of terminal observations and truncation flags from the fused MetaMaze 3-D rollouts (mgb_maze_rollout):
+maze3d_rollout_kernel<true> (discrete, pose cache) and maze3d_kernel<false, true, true> (continuous, direct
+renderer).  Against step() twins with final_obs=True bit for bit, against
 handles that run the plain rollout (whose outputs must not move), and against the CPU oracle."""
 import itertools
 
@@ -308,9 +308,10 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-def test_refusals(torch_mod, textures, tasks, monkeypatch):
-    """Wrong handle kind, T <= 0, final_obs without auto-reset (truncated alone is fine), either output with mirrors or
-    multicast, a discrete handle without a pose cache, and the Python ValueError; the rollout works afterwards."""
+def test_final_obs_rollout_refusals(torch_mod, textures, tasks, monkeypatch):
+    """T <= 0, final_obs without auto-reset (truncated alone is fine), either output with mirrors or multicast, and the
+    Python ValueError; the rollout works afterwards.  A MetaMaze2D handle runs its own rollout with the outputs, and a
+    discrete handle without a pose cache runs on the direct renderer, as its step() would."""
     torch = torch_mod
     from metagym_b200 import BatchedMetaMaze2D
     n, T, res = 8, 3, (32, 32)
@@ -323,29 +324,24 @@ def test_refusals(torch_mod, textures, tasks, monkeypatch):
     obs = torch.zeros_like(fo)
     rew = torch.zeros((T, n), dtype=torch.float64, device="cuda")
     done = torch.zeros((T, n), dtype=torch.uint8, device="cuda")
-    entry = {"D3D": lib.mgb_maze_rollout_discrete_ex, "C3D": lib.mgb_maze_rollout_continuous_ex}
 
-    def call(kind, h, steps, f, tr, stream):
-        return entry[kind](h, steps, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(), _ptr(f), _ptr(tr),
-                           stream)
+    def call(h, steps, f, tr, stream):
+        return lib.mgb_maze_rollout(h, steps, None, 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(), _ptr(f),
+                                    _ptr(tr), None, 0, stream)
 
-    # the wrong handle kind: 2-D, or the other 3-D kind
-    for kind in ("D3D", "C3D"):
-        other = envs["C3D" if kind == "D3D" else "D3D"]
-        for h in (m2, other):
-            assert call(kind, h._h, T, fo, u8, h._stream()) == MGB_ERR_ARG
-            assert b"MGB_MAZE_" in lib.mgb_last_error()
-    for kind, env in envs.items():
+    assert call(m2._h, T, fo, u8, m2._stream()) == 0                  # the 2-D rollout (test_final_obs_rollout_gpu.py)
+    torch.cuda.synchronize()
+    for env in envs.values():
         h, st = env._h, env._stream()
         for steps in (0, -1):
-            assert call(kind, h, steps, fo, u8, st) == MGB_ERR_ARG
+            assert call(h, steps, fo, u8, st) == MGB_ERR_ARG
             assert b"T must be positive" in lib.mgb_last_error()
         delta = np.array([16], np.int64)
         for arm in (lambda: lib.mgb_maze_set_mirrors(h, 1, delta.ctypes.data),
                     lambda: lib.mgb_maze_set_multicast(h, 16)):
             assert arm() == 0
             for f, tr in ((fo, None), (None, u8)):
-                assert call(kind, h, T, f, tr, st) == MGB_ERR_ARG
+                assert call(h, T, f, tr, st) == MGB_ERR_ARG
                 assert b"mirrors" in lib.mgb_last_error()
             assert lib.mgb_maze_set_mirrors(h, 0, None) == 0
         out = env.rollout(T, final_obs=True)                  # usable again
@@ -354,18 +350,23 @@ def test_refusals(torch_mod, textures, tasks, monkeypatch):
         # final_obs without auto-reset; truncated alone is fine
         assert lib.mgb_maze_set_options(h, 0) == 0
         env.auto_reset = False
-        assert call(kind, h, T, fo, None, st) == MGB_ERR_ARG
+        assert call(h, T, fo, None, st) == MGB_ERR_ARG
         assert b"auto_reset" in lib.mgb_last_error()
-        assert call(kind, h, T, None, u8, st) == 0
+        assert call(h, T, None, u8, st) == 0
         torch.cuda.synchronize()
         with pytest.raises(ValueError, match="auto_reset"):
             env.rollout(T, final_obs=True)
         assert "truncated" not in env.rollout(T)
         torch.cuda.synchronize()
-    # a discrete handle without a pose cache: the message of mgb_maze_rollout
+    # a discrete handle without a pose cache: the direct renderer, equal to step() with final_obs on a twin
     nc = ready(make_env("D3D", "SURVIVAL", n, res, "uint8", textures, monkeypatch, cache=False), tasks)
-    assert call("D3D", nc._h, T, fo, u8, nc._stream()) == MGB_ERR_ARG
-    assert b"the fused 3-D rollout runs on the pose cache" in lib.mgb_last_error()
-    torch.cuda.synchronize()
-    for e in list(envs.values()) + [m2, nc]:
+    twin = ready(make_env("D3D", "SURVIVAL", n, res, "uint8", textures, monkeypatch, cache=False, final_obs=True), tasks)
+    acts = random_actions(torch, "D3D", np.random.RandomState(4), T, n)
+    assert lib.mgb_maze_rollout(nc._h, T, acts.data_ptr(), 0, None, obs.data_ptr(), rew.data_ptr(), done.data_ptr(),
+                                fo.data_ptr(), u8.data_ptr(), None, 0, nc._stream()) == 0
+    for t in range(T):
+        o, r, d, _ = twin.step(acts[t])
+        assert torch.equal(obs[t], o) and torch.equal(rew[t], r) and torch.equal(done[t].bool(), d), t
+        assert torch.equal(u8[t].bool(), twin.truncated) and torch.equal(fo[t][d], twin.final_observation[d]), t
+    for e in list(envs.values()) + [m2, nc, twin]:
         e.close()

@@ -1,4 +1,4 @@
-"""GPU tests of the fused continuous-maze rollout (mgb_maze_rollout_continuous, maze3d_kernel<false, true>): T steps in one
+"""GPU tests of the fused continuous-maze rollout (mgb_maze_rollout, maze3d_kernel<false, true>): T steps in one
 launch equal T step() calls bit for bit, device-drawn actions equal their NumPy restatement, every env equals its own CPU
 oracle, sharding does not change a trajectory, and misuse is refused."""
 import itertools
@@ -205,9 +205,9 @@ def test_sharding_invariance(torch_mod, maze_golden, textures):
         h.close()
 
 
-def test_errors(torch_mod, maze_golden, textures):
-    """T = 0, a rollout before reset(), output mirrors or multicast switched on, a handle without a task, and
-    mgb_maze_rollout on a continuous handle are refused with a message; the rollout works again afterwards."""
+def test_rollout_errors(torch_mod, maze_golden, textures):
+    """T = 0, a rollout before reset(), output mirrors or multicast switched on, and a handle without a task are refused
+    with a message; the rollout works again afterwards, through Python and through the C call."""
     torch = torch_mod
     from metagym_b200 import BatchedMetaMazeContinuous3D, MgbError, _lib
     tasks = dense_tasks(maze_golden)
@@ -221,21 +221,20 @@ def test_errors(torch_mod, maze_golden, textures):
         env.rollout(0)
     delta = np.array([1 << 20], dtype=np.int64)
     _lib.check(env._lib.mgb_maze_set_mirrors(env._h, 1, delta.ctypes.data))
-    with pytest.raises(MgbError, match="mirrors are not implemented for the continuous-maze rollout"):
+    with pytest.raises(MgbError, match="mirrors are not implemented for the 3-D rollouts"):
         env.rollout(3)
     _lib.check(env._lib.mgb_maze_set_multicast(env._h, 1 << 20))
-    with pytest.raises(MgbError, match="mirrors are not implemented for the continuous-maze rollout"):
+    with pytest.raises(MgbError, match="mirrors are not implemented for the 3-D rollouts"):
         env.rollout(3)
     _lib.check(env._lib.mgb_maze_set_mirrors(env._h, 0, None))
     out = env.rollout(3)
-    with pytest.raises(MgbError, match="mgb_maze_rollout serves MetaMaze2D and MetaMazeDiscrete3D"):
-        _lib.check(env._lib.mgb_maze_rollout(env._h, 3, None, 0, None, out["obs"].data_ptr(), out["rew"].data_ptr(),
-                                             out["done"].data_ptr(), env._stream()))
+    _lib.check(env._lib.mgb_maze_rollout(env._h, 3, None, 0, None, out["obs"].data_ptr(), out["rew"].data_ptr(),
+                                         out["done"].data_ptr(), None, None, None, 0, env._stream()))
     torch.cuda.synchronize()
     env.close()
     bare = BatchedMetaMazeContinuous3D(resolution=res, max_steps=10, num_envs=n, squeeze=False, textures=textures)
     bare._create(15)                                          # a handle with textures but no task table
     with pytest.raises(MgbError, match="set_task"):
-        _lib.check(bare._lib.mgb_maze_rollout_continuous(bare._h, 3, None, 0, None, out["obs"].data_ptr(),
-                                                         out["rew"].data_ptr(), out["done"].data_ptr(), bare._stream()))
+        _lib.check(bare._lib.mgb_maze_rollout(bare._h, 3, None, 0, None, out["obs"].data_ptr(), out["rew"].data_ptr(),
+                                              out["done"].data_ptr(), None, None, None, 0, bare._stream()))
     bare.close()

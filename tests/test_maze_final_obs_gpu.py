@@ -1,5 +1,5 @@
-"""GPU tests of the terminal observations and truncation flags of auto-reset MetaMaze steps (final_obs=True,
-mgb_maze_step_ex / mgb_maze_step_continuous_ex) on every step path, against the CPU oracle (oracle/maze_oracle.c):
+"""GPU tests of the terminal observations and truncation flags of auto-reset MetaMaze steps (final_obs=True, the
+optional outputs of mgb_maze_step) on every step path, against the CPU oracle (oracle/maze_oracle.c):
 the terminal frame of every finished env, the first frame of its next episode, and why the episode ended."""
 import numpy as np
 import pytest
@@ -281,7 +281,7 @@ def test_sharded_handles_equal_one_handle(torch_mod, textures, tasks, monkeypatc
         e.close()
 
 
-def test_refusals(torch_mod, textures, tasks, monkeypatch):
+def test_final_obs_step_refusals(torch_mod, textures, tasks, monkeypatch):
     """final_obs needs auto_reset, in Python (ValueError) and in the C ABI (MGB_ERR_ARG)."""
     torch = torch_mod
     from metagym_b200 import BatchedMetaMaze2D, BatchedMetaMazeContinuous3D, BatchedMetaMazeDiscrete3D
@@ -299,10 +299,9 @@ def test_refusals(torch_mod, textures, tasks, monkeypatch):
         trunc = torch.zeros(2, dtype=torch.uint8, device="cuda")
         if PATHS[path][0] == "C3D":
             act = torch.zeros((2, 2), dtype=torch.float32, device="cuda")
-            fn = env._lib.mgb_maze_step_continuous_ex
         else:
             act = torch.zeros(2, dtype=torch.int32, device="cuda")
-            fn = env._lib.mgb_maze_step_ex
+        fn = env._lib.mgb_maze_step
         args = (env._h, act.data_ptr(), env._obs.data_ptr(), env._rew.data_ptr(), env._done.data_ptr())
         assert fn(*args, final.data_ptr(), trunc.data_ptr(), env._stream()) == -1       # MGB_ERR_ARG
         assert b"auto_reset" in env._lib.mgb_last_error()

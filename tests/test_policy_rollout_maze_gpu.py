@@ -1,7 +1,7 @@
 """GPU: MetaMaze2D rollouts driven by an on-device MLP policy with a categorical head (mgb_maze_rollout_policy,
 BatchedMetaMaze2D.rollout(policy=, resample=)).
 
-Env side: bit for bit the open-loop rollout (mgb_maze_rollout_ex, or mgb_maze_rollout_resample with `resample`) fed the
+Env side: bit for bit the open-loop rollout (mgb_maze_rollout, with a sampler cfg for `resample`) fed the
 actions the policy took, path recording included.  Policy side: the actions against the inverse-CDF draw restated in
 float64 from a torch forward pass of the same module on the windows the policy saw and the Philox uniforms of
 tests/policy_draws.py; the log-probabilities against log_softmax.
@@ -221,7 +221,7 @@ def test_graph_sees_updated_weights(tasks):  # noqa: F811
     assert check_policy_side(env, m2, got, 1, int(snap["counters"][0]))[0] <= 1.0
 
 
-def test_refusals_leave_the_handle_untouched(tasks, textures):  # noqa: F811
+def test_policy_refusals_leave_the_handle_untouched(tasks, textures):  # noqa: F811
     from metagym_b200 import BatchedMetaMazeDiscrete3D, _lib
     from metagym_b200.policy import MLPPolicy
     n, T = 128, 4
@@ -262,15 +262,15 @@ def test_refusals_leave_the_handle_untouched(tasks, textures):  # noqa: F811
     torch.cuda.synchronize()
     after = state(env)
     assert after[0] == before[0] and after[1] == before[1] + 1 and torch.equal(after[2], before[2])
-    # resample where mgb_maze_rollout_resample refuses it: the same reason
+    # resample where mgb_maze_rollout refuses it: the same reason
     plain = make_env(n, auto_reset=False, final_obs=False)
     plain.set_task(tasks)
     plain.reset()
     cfg, _ = plain._sampler_cfg(seed=1, **CFG)
     assert call(plain._h, good, cfg=cfg) == MGB_ERR_ARG
     why = lib.mgb_last_error().decode().split(": ", 1)[1]
-    assert lib.mgb_maze_rollout_resample(plain._h, T, None, 0, None, None, None, None, None, None, ctypes.byref(cfg), 0,
-                                         plain._stream()) == MGB_ERR_ARG
+    assert lib.mgb_maze_rollout(plain._h, T, None, 0, None, None, None, None, None, None, ctypes.byref(cfg), 0,
+                                plain._stream()) == MGB_ERR_ARG
     assert lib.mgb_last_error().decode().split(": ", 1)[1] == why
     # a 3-D handle
     d3 = BatchedMetaMazeDiscrete3D(resolution=(32, 32), textures=textures, max_steps=MAX_STEPS, num_envs=n,
