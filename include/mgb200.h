@@ -447,6 +447,61 @@ int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint6
                             float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev, uint8_t *done_dev,
                             float *final_obs_dev, uint8_t *truncated_dev, void *stream);
 
+/* ---- recurrent policies (DESIGN.md "Recurrent policies") ----------------------------------------------------------
+ * A GRU cell (torch.nn.GRUCell(in, H)) followed by a head, evaluated inside a MetaMaze2D rollout launch.  The policy's
+ * memory is a caller-owned float32 state [n][S], S = H + 5 feedback, row e = [c (H), onehot(prev action) (4),
+ * (float)prev reward (1)] (the last five only with feedback = 1).
+ *   Input of step t: x_t = [obs (D = (2 view_grid + 1)^2), then with feedback the five feedback entries of the state].
+ *   params_dev: float32 on the handle's device, read at every launch.  weight_ih [3H][in], weight_hh [3H][H], bias_ih
+ *     [3H], bias_hh [3H] (gate order r, z, n; a cell without bias packs zeros), then the head in torch.nn.Linear order:
+ *     W [4][H], b [4] (head_hidden = 0) or W1 [w][H], b1 [w], W2 [4][w], b2 [4] (head_hidden = 1, w = head_width,
+ *     hidden activation MGB_ACT_*).
+ *   Step t: h_t = GRU(x_t, c_t); the action is drawn from head(h_t) exactly as mgb_maze_rollout_policy draws it from
+ *     its logits (categorical head, MGB_STREAM_POLICY, counter (genv, t_base + t)).  Then, if done[t] and the reset rule
+ *     fires, the whole state row becomes zero; otherwise c_{t+1} = h_t and the feedback entries become
+ *     (onehot(a_t), (float)r_t).  MGB_RNN_RESET_EPISODE fires on every done; MGB_RNN_RESET_TASK fires where the env drew
+ *     a new maze in this launch (a rollout with resample_cfg), so without resampling it never fires inside a launch and
+ *     the caller zeroes the rows of envs it gives a new task (set_task, update_tasks, resample_tasks).
+ * Numerical contract (float32, no tensor cores, no approximate instructions; u = 2^-24):
+ *   gi_k[j] = fma chain from bias_ih[kH + j] over x_t[i], i = 0..in-1 in index order: acc = fmaf(W_ih[kH + j][i], x_i, acc);
+ *   gh_k[j] likewise from bias_hh[kH + j] over c_t[i], i = 0..H-1.  k = r, z, n.
+ *   r = 1 / (1 + expf(-(gi_r + gh_r))), z likewise: the two chains are added in one float32 add, then expf (at most 2
+ *     ulp), one add and one correctly rounded division.
+ *   n = tanhf(fmaf(r, gh_n, gi_n)) (one rounding inside, tanhf at most 2 ulp).
+ *   h' = fmaf(z, c, (1 - z) n): 1 - z and its product with n are rounded, then one fused multiply-add.
+ *   The head is the MLP of mgb_policy on h_t (fma chains from the bias, accurate tanhf). */
+#define MGB_RNN_RESET_EPISODE 0   /* zero the state row at every done */
+#define MGB_RNN_RESET_TASK 1      /* zero it where the env drew a new maze in this launch (in-launch resampling) */
+#define MGB_RNN_MAX_HIDDEN 64
+
+typedef struct mgb_rnn_policy {
+    const float *params_dev;  /* packed float32 on the handle's device, read at every launch */
+    int32_t hidden;           /* H, 1..64 */
+    int32_t feedback;         /* 0 or 1: the input ends with onehot(prev action) and prev reward */
+    int32_t reset;            /* MGB_RNN_RESET_* */
+    int32_t head_hidden;      /* 0: Linear(H, 4); 1: Linear(H, w), activation, Linear(w, 4) */
+    int32_t head_width;       /* w, 1..64 when head_hidden = 1 (ignored otherwise) */
+    int32_t activation;       /* MGB_ACT_* of the head's hidden layer */
+    int32_t mode;             /* MGB_POLICY_* */
+} mgb_rnn_policy;
+
+/* mgb_maze_rollout_policy with a recurrent policy (mgb_rnn_policy above) on a MetaMaze2D handle with auto_reset on.
+ *   state_dev [n][S] float32: read at launch start, written back in place at launch end (4-byte aligned, not NULL).
+ *   state0_out_dev [n][S]: the state as read.  hid_out_dev [T][n][H]: h_t.  Both may be NULL.
+ *   act_out, logp_out, obs0_out, obs, rew, done, final_obs, truncated, seed, resample_cfg, resample_seed: as
+ *   mgb_maze_rollout_policy.  The env side is bit for bit mgb_maze_rollout fed act_out.  The step counter advances by
+ *   T; nothing is allocated, and the call can be captured in a CUDA graph.  Refused (MGB_ERR_ARG; the handle, its step
+ *   counter and the state untouched): everything mgb_maze_rollout_policy refuses, a NULL or misaligned state_dev,
+ *   auto_reset off, hidden / feedback / reset / head_hidden / head_width / activation / mode out of range, and
+ *   observation tiles, sampler workspaces, weights and activations of 128 envs beyond the device's opt-in shared
+ *   memory (a large view_grid with a wide cell). */
+int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed,
+                         const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                         float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                         int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                         float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                         float *final_obs_dev, uint8_t *truncated_dev, void *stream);
+
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

@@ -24,7 +24,7 @@ def __getattr__(name):
                 "MetaMazeDiscrete3D", "MetaMazeContinuous3D", "TaskConfig", "MazeTaskSampler"):
         from . import metamaze
         return getattr(metamaze, name)
-    if name == "MLPPolicy":
+    if name in ("MLPPolicy", "GRUPolicy"):
         from . import policy
-        return policy.MLPPolicy
+        return getattr(policy, name)
     raise AttributeError(name)

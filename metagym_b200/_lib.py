@@ -54,8 +54,15 @@ class Policy(ctypes.Structure):
     _fields_ = [("params_dev", vp), ("n_hidden", c_i32), ("width", c_i32 * 3), ("activation", c_i32), ("mode", c_i32)]
 
 
+class RnnPolicy(ctypes.Structure):
+    """mgb_rnn_policy (include/mgb200.h)."""
+    _fields_ = [("params_dev", vp), ("hidden", c_i32), ("feedback", c_i32), ("reset", c_i32), ("head_hidden", c_i32),
+                ("head_width", c_i32), ("activation", c_i32), ("mode", c_i32)]
+
+
 ACT_TANH, ACT_RELU = 0, 1            # MGB_ACT_*
 POLICY_SAMPLE, POLICY_MEAN = 0, 1    # MGB_POLICY_*
+RNN_RESET_EPISODE, RNN_RESET_TASK = 0, 1     # MGB_RNN_RESET_*
 
 
 # name -> (restype, argtypes); every function include/mgb200.h declares (tests/test_abi.py checks the two agree)
@@ -108,6 +115,8 @@ SIGNATURES = {
                                         c_u64, vp]),
     "mgb_maze_rollout_policy": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_u64, ctypes.POINTER(MazeSamplerCfg),
                                                c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_rollout_rnn": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_u64, ctypes.POINTER(MazeSamplerCfg),
+                                            c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

@@ -21,6 +21,7 @@
 #include <string.h>
 #include <memory>
 #include <new>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -505,11 +506,17 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // (post auto-reset and resampling) into the thread's column of the activation buffers, which follow the tiles and the
 // sampler workspaces in dynamic shared memory at pol.smem_off; at t = 0 the window of the loaded state.  The step
 // arithmetic after the action is the code the other instantiations run.
-template <int XM, bool FIN, bool REC, bool RS = false, bool POL = false>
-__global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid_constant__ MazeConst c,
-                                                                    const __grid_constant__ MazeArgs a,
-                                                                    const __grid_constant__ MazeResample rs,
-                                                                    const __grid_constant__ MgbMlp pol)
+// POL == kPolGru (mgb_maze_rollout_rnn): the policy is the GRU `pol` (mgb_policy.cuh).  Its region at pol.smem_off holds
+// the staged cell and head, then the columns x [in], c [H], h [H] and the head's w.  The obs rows of x are filled as
+// POL == kPolMlp fills its input; at t = 0 the state row fills c and the feedback rows of x.  Step t computes h from
+// (x, c), acts on head(h), and after the step carries h into c (the two columns swap roles) and (onehot(a), (float)r)
+// into the feedback rows, or zeroes both where done and the reset rule fires; the state row is stored after step T - 1.
+constexpr int kPolMlp = 1, kPolGru = 2;
+
+template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0>
+__global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
+    const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
+    const __grid_constant__ std::conditional_t<POL == kPolGru, MgbGru, MgbMlp> pol)
 {
     static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
@@ -534,7 +541,8 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
     const int64_t genv = a.env_base + e;
     const int n = c.n, g = c.view_grid;
     float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the two activation buffers
-    if constexpr (POL) {
+    float *gru_c = nullptr, *gru_h = nullptr;                       // kPolGru: the carried and the new hidden state
+    if constexpr (POL == kPolMlp) {
         static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
         pol_w = tile2d + pol.smem_off;
         pol_x = pol_w + pol.staged;
@@ -549,6 +557,29 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
         }
         __syncthreads();    // the staged weights (the RS loop has no CTA barrier)
     }
+    if constexpr (POL == kPolGru) {
+        static_assert(XM == 0, "policy rollouts are not mirrored");
+        pol_w = tile2d + pol.smem_off;
+        pol_x = pol_w + pol.staged;
+        gru_c = pol_x + pol.in * k2dThreads;
+        gru_h = gru_c + pol.H * k2dThreads;
+        pol_y = gru_h + pol.H * k2dThreads;          // the head's hidden layer
+        mgb_gru_stage(pol, pol_w);
+        if (active) {
+            float *row = tile2d + threadIdx.x * D;
+            maze2d_window(c, blob, eaten, a.n_pad, s, row);
+            for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = row[k];
+            if (pol.head.obs0_out)
+                for (int k = 0; k < D; ++k) pol.head.obs0_out[e * D + k] = row[k];
+            const int S = pol.H + 5 * pol.feedback;
+            const float *st = pol.state + e * S;
+            for (int k = 0; k < pol.H; ++k) gru_c[k * k2dThreads + threadIdx.x] = st[k];
+            for (int k = pol.H; k < S; ++k) pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x] = st[k];
+            if (pol.state0_out)
+                for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
+        }
+        __syncthreads();    // the staged weights
+    }
     for (int t = 0; t < a.T; ++t) {
         float *tile = tile2d + (size_t)(t & 1) * k2dThreads * D;
         if constexpr (RS) {                                 // per warp: the warp's rows and their store are its own
@@ -561,12 +592,22 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
         uint32_t done_byte = 0;
         if (active) {
             int action;
-            if constexpr (POL) {
+            if constexpr (POL == kPolMlp) {
                 float logits[4];
                 mgb_mlp_forward(pol, pol_w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
                 const float lp = mgb_categorical_action(pol, genv, a.t_base + (uint32_t)t, logits, action);
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
                 if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
+            } else if constexpr (POL == kPolGru) {
+                mgb_gru_cell(pol, pol_w, pol_x, gru_c, gru_h, k2dThreads, threadIdx.x);
+                if (pol.hid_out)
+                    for (int k = 0; k < pol.H; ++k)
+                        pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = gru_h[k * k2dThreads + threadIdx.x];
+                float logits[4];
+                mgb_mlp_forward(pol.head, pol_w + pol.s_head, gru_h, pol_y, k2dThreads, threadIdx.x, logits);
+                const float lp = mgb_categorical_action(pol.head, genv, a.t_base + (uint32_t)t, logits, action);
+                if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
+                if (pol.head.logp_out) pol.head.logp_out[(int64_t)t * a.n + e] = lp;
             } else if (a.act) action = a.act[(int64_t)t * a.n + e];
             else {
                 const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
@@ -615,6 +656,20 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
                         row[p * W + q] = v;
                     }
                 if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
+            }
+            if constexpr (POL == kPolGru) {
+                // carry: with RS every finished env draws a new maze, so the task rule fires exactly where done does
+                const bool wipe = done && (RS || pol.reset == MGB_RNN_RESET_EPISODE);
+                if (wipe)
+                    for (int k = 0; k < pol.H; ++k) gru_h[k * k2dThreads + threadIdx.x] = 0.f;
+                if (pol.feedback) {
+                    float *fb = pol_x + D * k2dThreads + threadIdx.x;
+                    for (int k = 0; k < 4; ++k) fb[k * k2dThreads] = !wipe && k == action ? 1.f : 0.f;
+                    fb[4 * k2dThreads] = wipe ? 0.f : (float)reward;
+                }
+                float *const tmp = gru_c;
+                gru_c = gru_h;
+                gru_h = tmp;
             }
         }
         if constexpr (RS) {
@@ -693,6 +748,14 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(const __grid
     if (active) {
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
+    }
+    if constexpr (POL == kPolGru) {
+        if (active) {
+            const int S = pol.H + 5 * pol.feedback;
+            float *st = pol.state + e * S;
+            for (int k = 0; k < pol.H; ++k) st[k] = gru_c[k * k2dThreads + threadIdx.x];
+            for (int k = pol.H; k < S; ++k) st[k] = pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x];
+        }
     }
     if constexpr (RS) {
         if ((threadIdx.x & 31) == 0) mgb_bulk_wait_read<0>();
@@ -4158,21 +4221,21 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
     return MGB_OK;
 }
 
-// maze2d_rollout_kernel<0, fin, REC, RS, true>, sm bytes of dynamic shared memory; refused when the CTA would need more
-// shared memory than the device allows
-template <bool REC, bool RS>
-static int launch_2d_policy(const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r, const MgbMlp &m,
-                            unsigned blocks, size_t sm, cudaStream_t st)
+// maze2d_rollout_kernel<0, fin, REC, RS, POL>, sm bytes of dynamic shared memory; refused (as `fn`) when the CTA would
+// need more shared memory than the device allows
+template <bool REC, bool RS, int POL, class Plan>
+static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r,
+                            const Plan &m, unsigned blocks, size_t sm, cudaStream_t st)
 {
-    const auto kernel = fin ? maze2d_rollout_kernel<0, true, REC, RS, true> : maze2d_rollout_kernel<0, false, REC, RS, true>;
+    const auto kernel = fin ? maze2d_rollout_kernel<0, true, REC, RS, POL> : maze2d_rollout_kernel<0, false, REC, RS, POL>;
     int optin = 0;
     MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
     cudaFuncAttributes fa;
     MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
     if (fa.sharedSizeBytes + sm > (size_t)optin) {
-        mgb_set_error("mgb_maze_rollout_policy: the policy rollout needs %zu bytes of shared memory per CTA (windows of "
+        mgb_set_error("%s: the policy rollout needs %zu bytes of shared memory per CTA (windows of "
                       "view_grid %d, %sweights and activations of %d envs), more than the %d the device allows (use a "
-                      "smaller view_grid or narrower layers)", fa.sharedSizeBytes + sm, h->c.view_grid,
+                      "smaller view_grid or narrower layers)", fn, fa.sharedSizeBytes + sm, h->c.view_grid,
                       RS ? "sampler workspaces, " : "", k2dThreads, optin);
         return MGB_ERR_ARG;
     }
@@ -4226,11 +4289,73 @@ extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy 
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     const cudaStream_t st = (cudaStream_t)stream;
     if (resample_cfg)
-        rc = h->path ? launch_2d_policy<true, true>(h, fin, a, r, m, blocks, sm, st)
-                     : launch_2d_policy<false, true>(h, fin, a, r, m, blocks, sm, st);
+        rc = h->path ? launch_2d_policy<true, true, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st)
+                     : launch_2d_policy<false, true, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st);
     else
-        rc = h->path ? launch_2d_policy<true, false>(h, fin, a, r, m, blocks, sm, st)
-                     : launch_2d_policy<false, false>(h, fin, a, r, m, blocks, sm, st);
+        rc = h->path ? launch_2d_policy<true, false, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st)
+                     : launch_2d_policy<false, false, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st);
+    if (rc) return rc;
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed,
+                                    const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                    float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                                    int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                    float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                    float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_rnn");
+    SamplerCfg sc;
+    MgbGru g;
+    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
+        if (h->c.kind != MGB_MAZE_2D) return "mgb_maze_rollout_rnn serves MetaMaze2D (the 3-D envs observe frames)";
+        const int W = 2 * h->c.view_grid + 1;
+        if (const char *why = mgb_gru_plan(pol, W * W, g)) return why;
+        if (!state_dev) return "null state";
+        if ((uintptr_t)state_dev % sizeof(float)) return "state must be 4-byte aligned";
+        if (!h->auto_reset) return "the recurrent rollout needs auto_reset on (an episode boundary has no next step without it)";
+        if (logp_out_dev && g.head.mode != MGB_POLICY_SAMPLE)
+            return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
+        if (h->mir.count != 0)
+            return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
+        if (!resample_cfg) return nullptr;
+        return sampler_cfg(h, resample_cfg, sc);
+    });
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    // two observation tiles, the sampler workspaces when resampling, then the cell, the head and the columns
+    const int W = 2 * h->c.view_grid + 1;
+    size_t base = (size_t)2 * k2dThreads * W * W * 4;
+    if (resample_cfg) base += (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
+    base = (base + 15) / 16 * 16;
+    g.smem_off = (int)(base / 4);
+    g.head.seed = seed;
+    g.head.logp_out = logp_out_dev;
+    g.head.obs0_out = obs0_out_dev;
+    g.state = state_dev;
+    g.state0_out = state0_out_dev;
+    g.hid_out = hid_out_dev;
+    const size_t sm = base + mgb_gru_smem_bytes(g, k2dThreads);
+    MazeArgs a = maze_args(h);
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+    MazeResample r = {};
+    if (resample_cfg) {
+        r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
+    }
+    const bool fin = final_obs_dev || truncated_dev;
+    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (resample_cfg)
+        rc = h->path ? launch_2d_policy<true, true, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st)
+                     : launch_2d_policy<false, true, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st);
+    else
+        rc = h->path ? launch_2d_policy<true, false, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st)
+                     : launch_2d_policy<false, false, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st);
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;

@@ -219,3 +219,128 @@ __device__ __forceinline__ float mgb_categorical_action(const MgbMlp &m, int64_t
         if (action == k) la = l[k];
     return (la - mx) - logf(sum);
 }
+
+// ---------------------------------------------------------------------------------------------------------------
+// GRU policies (mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies").  The cell's weights are staged in groups of eight
+// hidden units: for group g and input i the 24 weights W[k H + 8g + r][i] (gate k = r, z, n; r < 8) are six consecutive
+// float4, read by the warp as broadcasts, for weight_ih over x and then weight_hh over c.  Group g's biases are 48
+// floats: bias_ih [3][8], then bias_hh [3][8].  Units past H are zero.  The head is an MgbMlp on h, staged behind the cell.
+// ---------------------------------------------------------------------------------------------------------------
+
+struct MgbGru {
+    const float *params;          // packed buffer (global memory)
+    int H, Hp, in, feedback, reset;   // Hp: H rounded up to 8
+    int g_hh, g_b;                // global float offsets of weight_hh and bias_ih (weight_ih at 0, bias_hh at g_b + 3H)
+    int s_hh, s_b, s_head;        // shared float offsets of the regrouped weight_hh, the biases and the head
+    int staged;                   // floats of staged weights, cell and head (a multiple of 8)
+    int head_width;               // rows of the head's activation buffer (0 without a hidden head layer)
+    int smem_off;                 // float offset of the policy's region in the kernel's dynamic shared memory
+    MgbMlp head;                  // the head (in[0] = H); its seed, mode, logp_out and obs0_out serve the whole policy
+    float *state, *state0_out, *hid_out;  // [n][H + 5 feedback], [n][H + 5 feedback] or null, [T][n][H] or null
+};
+
+// Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
+static inline const char *mgb_gru_plan(const mgb_rnn_policy *p, int obs_dim, MgbGru &g)
+{
+    if (!p) return "null policy";
+    if (!p->params_dev) return "null params_dev";
+    if (p->hidden < 1 || p->hidden > MGB_RNN_MAX_HIDDEN) return "hidden must be 1..64";
+    if (p->feedback != 0 && p->feedback != 1) return "feedback must be 0 or 1";
+    if (p->reset != MGB_RNN_RESET_EPISODE && p->reset != MGB_RNN_RESET_TASK) return "unknown reset rule";
+    if (p->head_hidden != 0 && p->head_hidden != 1) return "head_hidden must be 0 or 1";
+    if (p->head_hidden && (p->head_width < 1 || p->head_width > MGB_POLICY_MAX_WIDTH)) return "head_width must be 1..64";
+    g = MgbGru{};
+    g.params = p->params_dev;
+    g.H = p->hidden;
+    g.Hp = (g.H + 7) / 8 * 8;
+    g.in = obs_dim + 5 * p->feedback;
+    g.feedback = p->feedback;
+    g.reset = p->reset;
+    g.g_hh = 3 * g.H * g.in;
+    g.g_b = g.g_hh + 3 * g.H * g.H;
+    g.s_hh = 3 * g.Hp * g.in;
+    g.s_b = g.s_hh + 3 * g.Hp * g.H;
+    g.s_head = g.s_b + 6 * g.Hp;
+    const mgb_policy hp = {p->params_dev + g.g_b + 6 * g.H, p->head_hidden, {p->head_width, 0, 0}, p->activation, p->mode};
+    if (const char *why = mgb_mlp_plan(&hp, g.H, false, g.head)) return why;
+    g.staged = g.s_head + g.head.staged;
+    g.head_width = p->head_hidden ? p->head_width : 0;
+    return nullptr;
+}
+
+// bytes of dynamic shared memory a CTA of `threads` needs: staged weights + the columns x [in], c [H], h [H], w
+static inline size_t mgb_gru_smem_bytes(const MgbGru &g, int threads)
+{
+    return ((size_t)g.staged + (size_t)(g.in + 2 * g.H + g.head_width) * (size_t)threads) * sizeof(float);
+}
+
+// Device: stage the cell and the head into sm[0, g.staged) (all threads of the CTA; the caller synchronises)
+__device__ __forceinline__ void mgb_gru_stage(const MgbGru &g, float *sm)
+{
+    const int H = g.H;
+    for (int part = 0; part < 2; ++part) {
+        const int K = part ? H : g.in;
+        const float *W = g.params + (part ? g.g_hh : 0);
+        float *dst = sm + (part ? g.s_hh : 0);
+        for (int s = threadIdx.x; s < 3 * g.Hp * K; s += blockDim.x) {
+            const int r = s % 8, k = (s / 8) % 3, i = (s / 24) % K, j = (s / (24 * K)) * 8 + r;
+            dst[s] = j < H ? __ldg(W + (k * H + j) * K + i) : 0.f;
+        }
+    }
+    for (int s = threadIdx.x; s < 6 * g.Hp; s += blockDim.x) {
+        const int r = s % 8, k = (s / 8) % 3, kind = (s / 24) % 2, j = (s / 48) * 8 + r;
+        sm[g.s_b + s] = j < H ? __ldg(g.params + g.g_b + kind * 3 * H + k * H + j) : 0.f;
+    }
+    mgb_mlp_stage(g.head, sm + g.s_head);
+}
+
+// Device: h = GRU(x, c) for the thread's env (header "Recurrent policies" for the arithmetic).  x, c and h are the
+// column buffers (rows of `stride` floats; the thread's column is `col`); h must not alias x or c.
+__device__ __forceinline__ void mgb_gru_cell(const MgbGru &g, const float *sm, const float *xb, const float *cb, float *hb,
+                                             int stride, int col)
+{
+    const float *x = xb + col, *c = cb + col;
+    float *h = hb + col;
+    const int in = g.in, H = g.H;
+    const float4 *B = reinterpret_cast<const float4 *>(sm + g.s_b);
+    for (int u = 0; u < H; u += 8) {
+        const int grp = u / 8;
+        float gi[24], gh[24];
+#pragma unroll
+        for (int q = 0; q < 6; ++q) {
+            const float4 bi = B[grp * 12 + q], bh = B[grp * 12 + 6 + q];
+            gi[4 * q] = bi.x; gi[4 * q + 1] = bi.y; gi[4 * q + 2] = bi.z; gi[4 * q + 3] = bi.w;
+            gh[4 * q] = bh.x; gh[4 * q + 1] = bh.y; gh[4 * q + 2] = bh.z; gh[4 * q + 3] = bh.w;
+        }
+        const float4 *w = reinterpret_cast<const float4 *>(sm) + grp * in * 6;
+#pragma unroll 2
+        for (int i = 0; i < in; ++i) {
+            const float xi = x[i * stride];
+#pragma unroll
+            for (int q = 0; q < 6; ++q) {
+                const float4 wq = w[6 * i + q];
+                gi[4 * q] = fmaf(wq.x, xi, gi[4 * q]); gi[4 * q + 1] = fmaf(wq.y, xi, gi[4 * q + 1]);
+                gi[4 * q + 2] = fmaf(wq.z, xi, gi[4 * q + 2]); gi[4 * q + 3] = fmaf(wq.w, xi, gi[4 * q + 3]);
+            }
+        }
+        w = reinterpret_cast<const float4 *>(sm + g.s_hh) + grp * H * 6;
+#pragma unroll 2
+        for (int i = 0; i < H; ++i) {
+            const float ci = c[i * stride];
+#pragma unroll
+            for (int q = 0; q < 6; ++q) {
+                const float4 wq = w[6 * i + q];
+                gh[4 * q] = fmaf(wq.x, ci, gh[4 * q]); gh[4 * q + 1] = fmaf(wq.y, ci, gh[4 * q + 1]);
+                gh[4 * q + 2] = fmaf(wq.z, ci, gh[4 * q + 2]); gh[4 * q + 3] = fmaf(wq.w, ci, gh[4 * q + 3]);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 8; ++r)
+            if (u + r < H) {
+                const float rg = 1.f / (1.f + expf(-(gi[r] + gh[r])));
+                const float zg = 1.f / (1.f + expf(-(gi[8 + r] + gh[8 + r])));
+                const float ng = tanhf(fmaf(rg, gh[16 + r], gi[16 + r]));
+                h[(u + r) * stride] = fmaf(zg, c[(u + r) * stride], (1.f - zg) * ng);
+            }
+    }
+}

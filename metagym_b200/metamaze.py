@@ -674,7 +674,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         return cfg
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, resample=None, policy=None,
-                deterministic=False):
+                deterministic=False, state=None, want_hidden=False):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
         {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None).
 
@@ -695,12 +695,62 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         step t, with the Philox stream keyed by act_seed; deterministic=True takes the argmax.  Composes with
         `resample`.  The dict then also holds "act" [T,N] int32, "logp" [T,N] float32 (sampling only) and "obs0"
         [N,<obs of one env>] (the window acted on at t = 0; at t > 0 it is obs[t-1]).  `actions` together with
-        `policy` is a ValueError."""
+        `policy` is a ValueError.
+
+        policy may also be a GRUPolicy (mgb_maze_rollout_rnn; needs auto_reset=True), with state: its carried state
+        [N, policy.state_dim] float32 on the env's device (policy.initial_state(N) for fresh envs), read at the start
+        and updated in place at the end of the launch.  The dict then also holds "state0" (a copy of state as read),
+        "resampled" (whether the launch resampled, which unroll() needs for the "task" reset rule) and, with
+        want_hidden=True, "hid" [T,N,H] (the cell's output at every step)."""
+        from .policy import GRUPolicy
+        recurrent = isinstance(policy, GRUPolicy)
+        if recurrent and state is None:
+            raise ValueError("a GRUPolicy rollout needs its carried state (state=policy.initial_state(num_envs))")
+        if state is not None and not recurrent:
+            raise ValueError("state= goes with a GRUPolicy")
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
+            if recurrent:
+                return self._rollout_rnn(T, policy, state, act_seed, deterministic, out, resample, want_hidden)
             return self._rollout_policy(T, policy, act_seed, deterministic, out, resample)
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
+
+    def _rollout_rnn(self, T, policy, state, act_seed, deterministic, out, resample, want_hidden):
+        if self.need_reset:
+            raise Exception("Must \"reset\" before doing any actions")
+        torch = self._torch
+        T, N, dev = int(T), self.num_envs, self.device
+        shape = tuple(self._obs.shape[1:])
+        if policy.obs_dim != int(np.prod(shape)):
+            raise ValueError("the policy takes %d observation inputs, the env observes %d"
+                             % (policy.obs_dim, int(np.prod(shape))))
+        if policy.params.device != dev:
+            raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
+        if not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
+                and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
+            raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
+        if out is None:
+            out = {"obs": torch.empty((T, N) + shape, dtype=torch.float32, device=dev),
+                   "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
+                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
+                   "act": torch.empty((T, N), dtype=torch.int32, device=dev),
+                   "logp": None if deterministic else torch.empty((T, N), dtype=torch.float32, device=dev),
+                   "obs0": torch.empty((N,) + shape, dtype=torch.float32, device=dev),
+                   "state0": torch.empty((N, policy.state_dim), dtype=torch.float32, device=dev)}
+            if want_hidden:
+                out["hid"] = torch.empty((T, N, policy.hidden), dtype=torch.float32, device=dev)
+            if self._want_final:
+                out["final_obs"] = torch.empty((T, N) + shape, dtype=torch.float32, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+        out["resampled"] = resample is not None
+        cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+        pol = policy.struct(deterministic)
+        keys = ("state0", "hid", "act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
+        _lib.check(self._lib.mgb_maze_rollout_rnn(self._h, T, ctypes.byref(pol), int(act_seed),
+                                                  None if cfg is None else ctypes.byref(cfg), seed, _lib.ptr(state),
+                                                  *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
+        return out
 
     def _rollout_policy(self, T, policy, act_seed, deterministic, out, resample):
         if self.need_reset:
