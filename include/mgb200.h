@@ -448,9 +448,10 @@ int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint6
                             float *final_obs_dev, uint8_t *truncated_dev, void *stream);
 
 /* ---- recurrent policies (DESIGN.md "Recurrent policies") ----------------------------------------------------------
- * A GRU cell (torch.nn.GRUCell(in, H)) followed by a head, evaluated inside a MetaMaze2D rollout launch.  The policy's
- * memory is a caller-owned float32 state [n][S], S = H + 5 feedback, row e = [c (H), onehot(prev action) (4),
- * (float)prev reward (1)] (the last five only with feedback = 1).
+ * A GRU cell (torch.nn.GRUCell(in, H); cell = MGB_RNN_CELL_GRU) or an LSTM cell (torch.nn.LSTMCell(in, H); cell =
+ * MGB_RNN_CELL_LSTM, below) followed by a head, evaluated inside a MetaMaze2D rollout launch.  The GRU's memory is a
+ * caller-owned float32 state [n][S], S = H + 5 feedback, row e = [c (H), onehot(prev action) (4), (float)prev reward
+ * (1)] (the last five only with feedback = 1).
  *   Input of step t: x_t = [obs (D = (2 view_grid + 1)^2), then with feedback the five feedback entries of the state].
  *   params_dev: float32 on the handle's device, read at every launch.  weight_ih [3H][in], weight_hh [3H][H], bias_ih
  *     [3H], bias_hh [3H] (gate order r, z, n; a cell without bias packs zeros), then the head in torch.nn.Linear order:
@@ -469,10 +470,25 @@ int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint6
  *     ulp), one add and one correctly rounded division.
  *   n = tanhf(fmaf(r, gh_n, gi_n)) (one rounding inside, tanhf at most 2 ulp).
  *   h' = fmaf(z, c, (1 - z) n): 1 - z and its product with n are rounded, then one fused multiply-add.
- *   The head is the MLP of mgb_policy on h_t (fma chains from the bias, accurate tanhf). */
+ *   The head is the MLP of mgb_policy on h_t (fma chains from the bias, accurate tanhf).
+ * LSTM (cell = MGB_RNN_CELL_LSTM): everything above holds except the following.
+ *   State [n][S], S = 2H + 5 feedback, row e = [h (H), c (H), onehot(prev action) (4), (float)prev reward (1)].
+ *   params_dev: weight_ih [4H][in], weight_hh [4H][H], bias_ih [4H], bias_hh [4H] (torch's gate order i, f, g, o; a
+ *     cell without bias packs zeros), then the head as for the GRU.
+ *   Step t: (h_t, c'_t) = LSTM(x_t, (h_{t-1}, c_{t-1})); the action is drawn from head(h_t) as for the GRU.  Then, if
+ *     done[t] and the reset rule fires, the whole state row (h, c and feedback) becomes zero; otherwise h and c carry
+ *     and the feedback entries become (onehot(a_t), (float)r_t).  hid_out holds h_t.
+ *   gi_k[j] = fma chain from bias_ih[kH + j] over x_t[i], i = 0..in-1 in index order; gh_k[j] likewise from
+ *     bias_hh[kH + j] over h_{t-1}[i], i = 0..H-1.  k = i, f, g, o.  v_k = gi_k + gh_k in one float32 add.
+ *   i = 1 / (1 + expf(-v_i)), f and o likewise (expf at most 2 ulp, one add, one correctly rounded division);
+ *     g = tanhf(v_g) (at most 2 ulp).
+ *   c' = fmaf(f, c, i g): the product i g is rounded, then one fused multiply-add.
+ *   h' = o tanhf(c'): tanhf at most 2 ulp, then one rounded product. */
 #define MGB_RNN_RESET_EPISODE 0   /* zero the state row at every done */
 #define MGB_RNN_RESET_TASK 1      /* zero it where the env drew a new maze in this launch (in-launch resampling) */
 #define MGB_RNN_MAX_HIDDEN 64
+#define MGB_RNN_CELL_GRU 0        /* torch.nn.GRUCell */
+#define MGB_RNN_CELL_LSTM 1       /* torch.nn.LSTMCell */
 
 typedef struct mgb_rnn_policy {
     const float *params_dev;  /* packed float32 on the handle's device, read at every launch */
@@ -483,6 +499,7 @@ typedef struct mgb_rnn_policy {
     int32_t head_width;       /* w, 1..64 when head_hidden = 1 (ignored otherwise) */
     int32_t activation;       /* MGB_ACT_* of the head's hidden layer */
     int32_t mode;             /* MGB_POLICY_* */
+    int32_t cell;             /* MGB_RNN_CELL_* (0, the GRU, for callers that predate the field) */
 } mgb_rnn_policy;
 
 /* mgb_maze_rollout_policy with a recurrent policy (mgb_rnn_policy above) on a MetaMaze2D handle with auto_reset on.
@@ -492,9 +509,9 @@ typedef struct mgb_rnn_policy {
  *   mgb_maze_rollout_policy.  The env side is bit for bit mgb_maze_rollout fed act_out.  The step counter advances by
  *   T; nothing is allocated, and the call can be captured in a CUDA graph.  Refused (MGB_ERR_ARG; the handle, its step
  *   counter and the state untouched): everything mgb_maze_rollout_policy refuses, a NULL or misaligned state_dev,
- *   auto_reset off, hidden / feedback / reset / head_hidden / head_width / activation / mode out of range, and
- *   observation tiles, sampler workspaces, weights and activations of 128 envs beyond the device's opt-in shared
- *   memory (a large view_grid with a wide cell). */
+ *   auto_reset off, hidden / feedback / reset / head_hidden / head_width / activation / mode out of range, an unknown
+ *   cell, and observation tiles, sampler workspaces, weights and activations of 128 envs beyond the device's opt-in
+ *   shared memory (a large view_grid with a wide cell; DESIGN.md "Recurrent policies" lists what fits). */
 int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed,
                          const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
                          float *state_dev, float *state0_out_dev, float *hid_out_dev,

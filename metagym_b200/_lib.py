@@ -57,12 +57,13 @@ class Policy(ctypes.Structure):
 class RnnPolicy(ctypes.Structure):
     """mgb_rnn_policy (include/mgb200.h)."""
     _fields_ = [("params_dev", vp), ("hidden", c_i32), ("feedback", c_i32), ("reset", c_i32), ("head_hidden", c_i32),
-                ("head_width", c_i32), ("activation", c_i32), ("mode", c_i32)]
+                ("head_width", c_i32), ("activation", c_i32), ("mode", c_i32), ("cell", c_i32)]
 
 
 ACT_TANH, ACT_RELU = 0, 1            # MGB_ACT_*
 POLICY_SAMPLE, POLICY_MEAN = 0, 1    # MGB_POLICY_*
 RNN_RESET_EPISODE, RNN_RESET_TASK = 0, 1     # MGB_RNN_RESET_*
+RNN_CELL_GRU, RNN_CELL_LSTM = 0, 1           # MGB_RNN_CELL_*
 
 
 # name -> (restype, argtypes); every function include/mgb200.h declares (tests/test_abi.py checks the two agree)

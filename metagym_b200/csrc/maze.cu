@@ -511,13 +511,20 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // POL == kPolMlp fills its input; at t = 0 the state row fills c and the feedback rows of x.  Step t computes h from
 // (x, c), acts on head(h), and after the step carries h into c (the two columns swap roles) and (onehot(a), (float)r)
 // into the feedback rows, or zeroes both where done and the reset rule fires; the state row is stored after step T - 1.
-constexpr int kPolMlp = 1, kPolGru = 2;
+// POL == kPolLstm: the policy is the LSTM `pol`.  Its columns are x [in], the cell state c [H] and two h columns of Hr
+// rows.  Step t computes h from (x, h_{t-1}, c), updating c in place, then the head's hidden layer reuses the dead
+// h_{t-1} column; the carry swaps the two h columns as the GRU does, and a wipe zeroes c as well.
+constexpr int kPolMlp = 1, kPolGru = 2, kPolLstm = 3;
+
+template <int POL>
+using MazePolicyPlan = std::conditional_t<POL == kPolLstm, MgbLstm, std::conditional_t<POL == kPolGru, MgbGru, MgbMlp>>;
 
 template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0>
 __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
-    const __grid_constant__ std::conditional_t<POL == kPolGru, MgbGru, MgbMlp> pol)
+    const __grid_constant__ MazePolicyPlan<POL> pol)
 {
+    constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
     static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
     const int64_t e0 = (int64_t)blockIdx.x * k2dThreads;
@@ -541,7 +548,8 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     const int64_t genv = a.env_base + e;
     const int n = c.n, g = c.view_grid;
     float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the two activation buffers
-    float *gru_c = nullptr, *gru_h = nullptr;                       // kPolGru: the carried and the new hidden state
+    float *hid_prev = nullptr, *hid_new = nullptr;                  // RNN: the carried and the new hidden state
+    float *lstm_c = nullptr;                                        // kPolLstm: the cell state
     if constexpr (POL == kPolMlp) {
         static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
         pol_w = tile2d + pol.smem_off;
@@ -557,26 +565,43 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
         }
         __syncthreads();    // the staged weights (the RS loop has no CTA barrier)
     }
-    if constexpr (POL == kPolGru) {
+    if constexpr (RNN) {
         static_assert(XM == 0, "policy rollouts are not mirrored");
         pol_w = tile2d + pol.smem_off;
         pol_x = pol_w + pol.staged;
-        gru_c = pol_x + pol.in * k2dThreads;
-        gru_h = gru_c + pol.H * k2dThreads;
-        pol_y = gru_h + pol.H * k2dThreads;          // the head's hidden layer
-        mgb_gru_stage(pol, pol_w);
+        if constexpr (POL == kPolGru) {
+            hid_prev = pol_x + pol.in * k2dThreads;
+            hid_new = hid_prev + pol.H * k2dThreads;
+            pol_y = hid_new + pol.H * k2dThreads;      // the head's hidden layer
+            mgb_gru_stage(pol, pol_w);
+        } else {
+            lstm_c = pol_x + pol.in * k2dThreads;
+            hid_prev = lstm_c + pol.H * k2dThreads;
+            hid_new = hid_prev + pol.Hr * k2dThreads;
+            mgb_lstm_stage(pol, pol_w);
+        }
         if (active) {
             float *row = tile2d + threadIdx.x * D;
             maze2d_window(c, blob, eaten, a.n_pad, s, row);
             for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = row[k];
             if (pol.head.obs0_out)
                 for (int k = 0; k < D; ++k) pol.head.obs0_out[e * D + k] = row[k];
-            const int S = pol.H + 5 * pol.feedback;
-            const float *st = pol.state + e * S;
-            for (int k = 0; k < pol.H; ++k) gru_c[k * k2dThreads + threadIdx.x] = st[k];
-            for (int k = pol.H; k < S; ++k) pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x] = st[k];
-            if (pol.state0_out)
-                for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
+            if constexpr (POL == kPolGru) {
+                const int S = pol.H + 5 * pol.feedback;
+                const float *st = pol.state + e * S;
+                for (int k = 0; k < pol.H; ++k) hid_prev[k * k2dThreads + threadIdx.x] = st[k];
+                for (int k = pol.H; k < S; ++k) pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x] = st[k];
+                if (pol.state0_out)
+                    for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
+            } else {        // [h, c, feedback]
+                const int S = 2 * pol.H + 5 * pol.feedback;
+                const float *st = pol.state + e * S;
+                for (int k = 0; k < pol.H; ++k) hid_prev[k * k2dThreads + threadIdx.x] = st[k];
+                for (int k = 0; k < pol.H; ++k) lstm_c[k * k2dThreads + threadIdx.x] = st[pol.H + k];
+                for (int k = 2 * pol.H; k < S; ++k) pol_x[(D + k - 2 * pol.H) * k2dThreads + threadIdx.x] = st[k];
+                if (pol.state0_out)
+                    for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
+            }
         }
         __syncthreads();    // the staged weights
     }
@@ -598,13 +623,15 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                 const float lp = mgb_categorical_action(pol, genv, a.t_base + (uint32_t)t, logits, action);
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
                 if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
-            } else if constexpr (POL == kPolGru) {
-                mgb_gru_cell(pol, pol_w, pol_x, gru_c, gru_h, k2dThreads, threadIdx.x);
+            } else if constexpr (RNN) {
+                if constexpr (POL == kPolGru) mgb_gru_cell(pol, pol_w, pol_x, hid_prev, hid_new, k2dThreads, threadIdx.x);
+                else mgb_lstm_cell(pol, pol_w, pol_x, hid_prev, lstm_c, hid_new, k2dThreads, threadIdx.x);
                 if (pol.hid_out)
                     for (int k = 0; k < pol.H; ++k)
-                        pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = gru_h[k * k2dThreads + threadIdx.x];
+                        pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * k2dThreads + threadIdx.x];
+                if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
                 float logits[4];
-                mgb_mlp_forward(pol.head, pol_w + pol.s_head, gru_h, pol_y, k2dThreads, threadIdx.x, logits);
+                mgb_mlp_forward(pol.head, pol_w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits);
                 const float lp = mgb_categorical_action(pol.head, genv, a.t_base + (uint32_t)t, logits, action);
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
                 if (pol.head.logp_out) pol.head.logp_out[(int64_t)t * a.n + e] = lp;
@@ -657,19 +684,22 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                     }
                 if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
             }
-            if constexpr (POL == kPolGru) {
+            if constexpr (RNN) {
                 // carry: with RS every finished env draws a new maze, so the task rule fires exactly where done does
                 const bool wipe = done && (RS || pol.reset == MGB_RNN_RESET_EPISODE);
                 if (wipe)
-                    for (int k = 0; k < pol.H; ++k) gru_h[k * k2dThreads + threadIdx.x] = 0.f;
+                    for (int k = 0; k < pol.H; ++k) hid_new[k * k2dThreads + threadIdx.x] = 0.f;
+                if constexpr (POL == kPolLstm)
+                    if (wipe)
+                        for (int k = 0; k < pol.H; ++k) lstm_c[k * k2dThreads + threadIdx.x] = 0.f;
                 if (pol.feedback) {
                     float *fb = pol_x + D * k2dThreads + threadIdx.x;
                     for (int k = 0; k < 4; ++k) fb[k * k2dThreads] = !wipe && k == action ? 1.f : 0.f;
                     fb[4 * k2dThreads] = wipe ? 0.f : (float)reward;
                 }
-                float *const tmp = gru_c;
-                gru_c = gru_h;
-                gru_h = tmp;
+                float *const tmp = hid_prev;
+                hid_prev = hid_new;
+                hid_new = tmp;
             }
         }
         if constexpr (RS) {
@@ -749,12 +779,20 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
     }
-    if constexpr (POL == kPolGru) {
+    if constexpr (RNN) {
         if (active) {
-            const int S = pol.H + 5 * pol.feedback;
-            float *st = pol.state + e * S;
-            for (int k = 0; k < pol.H; ++k) st[k] = gru_c[k * k2dThreads + threadIdx.x];
-            for (int k = pol.H; k < S; ++k) st[k] = pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x];
+            if constexpr (POL == kPolGru) {
+                const int S = pol.H + 5 * pol.feedback;
+                float *st = pol.state + e * S;
+                for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * k2dThreads + threadIdx.x];
+                for (int k = pol.H; k < S; ++k) st[k] = pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x];
+            } else {
+                const int S = 2 * pol.H + 5 * pol.feedback;
+                float *st = pol.state + e * S;
+                for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * k2dThreads + threadIdx.x];
+                for (int k = 0; k < pol.H; ++k) st[pol.H + k] = lstm_c[k * k2dThreads + threadIdx.x];
+                for (int k = 2 * pol.H; k < S; ++k) st[k] = pol_x[(D + k - 2 * pol.H) * k2dThreads + threadIdx.x];
+            }
         }
     }
     if constexpr (RS) {
@@ -4310,14 +4348,16 @@ extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy
     MgbRange nvtx_range("mgb_maze_rollout_rnn");
     SamplerCfg sc;
     MgbGru g;
+    MgbLstm l;
+    const bool lstm = pol && pol->cell == MGB_RNN_CELL_LSTM;
     int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
         if (h->c.kind != MGB_MAZE_2D) return "mgb_maze_rollout_rnn serves MetaMaze2D (the 3-D envs observe frames)";
         const int W = 2 * h->c.view_grid + 1;
-        if (const char *why = mgb_gru_plan(pol, W * W, g)) return why;
+        if (const char *why = lstm ? mgb_lstm_plan(pol, W * W, l) : mgb_gru_plan(pol, W * W, g)) return why;
         if (!state_dev) return "null state";
         if ((uintptr_t)state_dev % sizeof(float)) return "state must be 4-byte aligned";
         if (!h->auto_reset) return "the recurrent rollout needs auto_reset on (an episode boundary has no next step without it)";
-        if (logp_out_dev && g.head.mode != MGB_POLICY_SAMPLE)
+        if (logp_out_dev && (lstm ? l.head.mode : g.head.mode) != MGB_POLICY_SAMPLE)
             return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
@@ -4331,14 +4371,6 @@ extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy
     size_t base = (size_t)2 * k2dThreads * W * W * 4;
     if (resample_cfg) base += (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
     base = (base + 15) / 16 * 16;
-    g.smem_off = (int)(base / 4);
-    g.head.seed = seed;
-    g.head.logp_out = logp_out_dev;
-    g.head.obs0_out = obs0_out_dev;
-    g.state = state_dev;
-    g.state0_out = state0_out_dev;
-    g.hid_out = hid_out_dev;
-    const size_t sm = base + mgb_gru_smem_bytes(g, k2dThreads);
     MazeArgs a = maze_args(h);
     a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
     a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
@@ -4350,12 +4382,26 @@ extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy
     const bool fin = final_obs_dev || truncated_dev;
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     const cudaStream_t st = (cudaStream_t)stream;
-    if (resample_cfg)
-        rc = h->path ? launch_2d_policy<true, true, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st)
-                     : launch_2d_policy<false, true, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st);
-    else
-        rc = h->path ? launch_2d_policy<true, false, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st)
-                     : launch_2d_policy<false, false, kPolGru>(__func__, h, fin, a, r, g, blocks, sm, st);
+    // the same launch for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>, p its plan
+    const char *const fn = __func__;    // (inside the lambda __func__ would name the lambda)
+    const auto launch = [&](auto kind, auto &p, size_t cell_bytes) {
+        constexpr int POL = decltype(kind)::value;
+        p.smem_off = (int)(base / 4);
+        p.head.seed = seed;
+        p.head.logp_out = logp_out_dev;
+        p.head.obs0_out = obs0_out_dev;
+        p.state = state_dev;
+        p.state0_out = state0_out_dev;
+        p.hid_out = hid_out_dev;
+        const size_t sm = base + cell_bytes;
+        if (resample_cfg)
+            return h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, p, blocks, sm, st)
+                           : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, p, blocks, sm, st);
+        return h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, p, blocks, sm, st)
+                       : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, p, blocks, sm, st);
+    };
+    rc = lstm ? launch(std::integral_constant<int, kPolLstm>{}, l, mgb_lstm_smem_bytes(l, k2dThreads))
+              : launch(std::integral_constant<int, kPolGru>{}, g, mgb_gru_smem_bytes(g, k2dThreads));
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;

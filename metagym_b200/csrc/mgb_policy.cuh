@@ -239,8 +239,8 @@ struct MgbGru {
     float *state, *state0_out, *hid_out;  // [n][H + 5 feedback], [n][H + 5 feedback] or null, [T][n][H] or null
 };
 
-// Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
-static inline const char *mgb_gru_plan(const mgb_rnn_policy *p, int obs_dim, MgbGru &g)
+// Host: the checks every recurrent cell shares.  Returns null, or the reason the policy is refused.
+static inline const char *mgb_rnn_check(const mgb_rnn_policy *p)
 {
     if (!p) return "null policy";
     if (!p->params_dev) return "null params_dev";
@@ -249,6 +249,14 @@ static inline const char *mgb_gru_plan(const mgb_rnn_policy *p, int obs_dim, Mgb
     if (p->reset != MGB_RNN_RESET_EPISODE && p->reset != MGB_RNN_RESET_TASK) return "unknown reset rule";
     if (p->head_hidden != 0 && p->head_hidden != 1) return "head_hidden must be 0 or 1";
     if (p->head_hidden && (p->head_width < 1 || p->head_width > MGB_POLICY_MAX_WIDTH)) return "head_width must be 1..64";
+    if (p->cell != MGB_RNN_CELL_GRU && p->cell != MGB_RNN_CELL_LSTM) return "unknown cell";
+    return nullptr;
+}
+
+// Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
+static inline const char *mgb_gru_plan(const mgb_rnn_policy *p, int obs_dim, MgbGru &g)
+{
+    if (const char *why = mgb_rnn_check(p)) return why;
     g = MgbGru{};
     g.params = p->params_dev;
     g.H = p->hidden;
@@ -341,6 +349,137 @@ __device__ __forceinline__ void mgb_gru_cell(const MgbGru &g, const float *sm, c
                 const float zg = 1.f / (1.f + expf(-(gi[8 + r] + gh[8 + r])));
                 const float ng = tanhf(fmaf(rg, gh[16 + r], gi[16 + r]));
                 h[(u + r) * stride] = fmaf(zg, c[(u + r) * stride], (1.f - zg) * ng);
+            }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// LSTM policies (mgb_maze_rollout_rnn with cell = MGB_RNN_CELL_LSTM).  The GRU's scheme with four gates: for group g of
+// kLstmGroup hidden units and input i the 4 kLstmGroup weights W[k H + kLstmGroup g + r][i] (gate k = i, f, g, o;
+// r < kLstmGroup) are consecutive float4, read by the warp as broadcasts, for weight_ih over x and then weight_hh over
+// the previous h.  Group g's biases are bias_ih [4][kLstmGroup], then bias_hh [4][kLstmGroup].  Units past H are zero.
+// The head is an MgbMlp on h, staged behind the cell.
+// ---------------------------------------------------------------------------------------------------------------
+
+constexpr int kLstmGroup = 8;     // hidden units per pass over the inputs: 8 gate accumulators per unit
+constexpr int kLstmQ = kLstmGroup;  // float4 weights per input of a group: 4 gates x kLstmGroup units / 4
+
+struct MgbLstm {
+    const float *params;          // packed buffer (global memory)
+    int H, Hp, in, feedback, reset;   // Hp: H rounded up to kLstmGroup
+    int Hr;                       // rows of each h column: max(H, head width); the head's hidden layer reuses the dead one
+    int g_hh, g_b;                // global float offsets of weight_hh and bias_ih (weight_ih at 0, bias_hh at g_b + 4H)
+    int s_hh, s_b, s_head;        // shared float offsets of the regrouped weight_hh, the biases and the head
+    int staged;                   // floats of staged weights, cell and head (a multiple of 8)
+    int smem_off;                 // float offset of the policy's region in the kernel's dynamic shared memory
+    MgbMlp head;                  // the head (in[0] = H); its seed, mode, logp_out and obs0_out serve the whole policy
+    float *state, *state0_out, *hid_out;  // [n][2H + 5 feedback], [n][2H + 5 feedback] or null, [T][n][H] or null
+};
+
+// Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
+static inline const char *mgb_lstm_plan(const mgb_rnn_policy *p, int obs_dim, MgbLstm &l)
+{
+    if (const char *why = mgb_rnn_check(p)) return why;
+    l = MgbLstm{};
+    l.params = p->params_dev;
+    l.H = p->hidden;
+    l.Hp = (l.H + kLstmGroup - 1) / kLstmGroup * kLstmGroup;
+    l.in = obs_dim + 5 * p->feedback;
+    l.feedback = p->feedback;
+    l.reset = p->reset;
+    l.Hr = p->head_hidden && p->head_width > l.H ? p->head_width : l.H;
+    l.g_hh = 4 * l.H * l.in;
+    l.g_b = l.g_hh + 4 * l.H * l.H;
+    l.s_hh = 4 * l.Hp * l.in;
+    l.s_b = l.s_hh + 4 * l.Hp * l.H;
+    l.s_head = l.s_b + 8 * l.Hp;
+    const mgb_policy hp = {p->params_dev + l.g_b + 8 * l.H, p->head_hidden, {p->head_width, 0, 0}, p->activation, p->mode};
+    if (const char *why = mgb_mlp_plan(&hp, l.H, false, l.head)) return why;
+    l.staged = l.s_head + l.head.staged;
+    return nullptr;
+}
+
+// bytes of dynamic shared memory a CTA of `threads` needs: staged weights + the columns x [in], c [H] and two h [Hr]
+static inline size_t mgb_lstm_smem_bytes(const MgbLstm &l, int threads)
+{
+    return ((size_t)l.staged + (size_t)(l.in + l.H + 2 * l.Hr) * (size_t)threads) * sizeof(float);
+}
+
+// Device: stage the cell and the head into sm[0, l.staged) (all threads of the CTA; the caller synchronises)
+__device__ __forceinline__ void mgb_lstm_stage(const MgbLstm &l, float *sm)
+{
+    constexpr int G = kLstmGroup;
+    const int H = l.H;
+    for (int part = 0; part < 2; ++part) {
+        const int K = part ? H : l.in;
+        const float *W = l.params + (part ? l.g_hh : 0);
+        float *dst = sm + (part ? l.s_hh : 0);
+        for (int s = threadIdx.x; s < 4 * l.Hp * K; s += blockDim.x) {
+            const int r = s % G, k = (s / G) % 4, i = (s / (4 * G)) % K, j = (s / (4 * G * K)) * G + r;
+            dst[s] = j < H ? __ldg(W + (k * H + j) * K + i) : 0.f;
+        }
+    }
+    for (int s = threadIdx.x; s < 8 * l.Hp; s += blockDim.x) {
+        const int r = s % G, k = (s / G) % 4, kind = (s / (4 * G)) % 2, j = (s / (8 * G)) * G + r;
+        sm[l.s_b + s] = j < H ? __ldg(l.params + l.g_b + kind * 4 * H + k * H + j) : 0.f;
+    }
+    mgb_mlp_stage(l.head, sm + l.s_head);
+}
+
+__device__ __forceinline__ float mgb_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }
+
+// Device: (h, c) = LSTM(x, (hp, c)) for the thread's env (header "Recurrent policies" for the arithmetic).  x, hp, c and
+// h are column buffers (rows of `stride` floats; the thread's column is `col`).  c is updated in place (unit j reads and
+// writes only c[j]); h must not alias x, hp or c.
+__device__ __forceinline__ void mgb_lstm_cell(const MgbLstm &l, const float *sm, const float *xb, const float *hpb,
+                                              float *cb, float *hb, int stride, int col)
+{
+    constexpr int G = kLstmGroup, Q = kLstmQ;
+    const float *x = xb + col, *hp = hpb + col;
+    float *c = cb + col, *h = hb + col;
+    const int in = l.in, H = l.H;
+    const float4 *B = reinterpret_cast<const float4 *>(sm + l.s_b);
+    for (int u = 0; u < H; u += G) {
+        const int grp = u / G;
+        float gi[4 * G], gh[4 * G];
+#pragma unroll
+        for (int q = 0; q < Q; ++q) {
+            const float4 bi = B[grp * 2 * Q + q], bh = B[grp * 2 * Q + Q + q];
+            gi[4 * q] = bi.x; gi[4 * q + 1] = bi.y; gi[4 * q + 2] = bi.z; gi[4 * q + 3] = bi.w;
+            gh[4 * q] = bh.x; gh[4 * q + 1] = bh.y; gh[4 * q + 2] = bh.z; gh[4 * q + 3] = bh.w;
+        }
+        const float4 *w = reinterpret_cast<const float4 *>(sm) + grp * in * Q;
+#pragma unroll 2
+        for (int i = 0; i < in; ++i) {
+            const float xi = x[i * stride];
+#pragma unroll
+            for (int q = 0; q < Q; ++q) {
+                const float4 wq = w[Q * i + q];
+                gi[4 * q] = fmaf(wq.x, xi, gi[4 * q]); gi[4 * q + 1] = fmaf(wq.y, xi, gi[4 * q + 1]);
+                gi[4 * q + 2] = fmaf(wq.z, xi, gi[4 * q + 2]); gi[4 * q + 3] = fmaf(wq.w, xi, gi[4 * q + 3]);
+            }
+        }
+        w = reinterpret_cast<const float4 *>(sm + l.s_hh) + grp * H * Q;
+#pragma unroll 2
+        for (int i = 0; i < H; ++i) {
+            const float hi = hp[i * stride];
+#pragma unroll
+            for (int q = 0; q < Q; ++q) {
+                const float4 wq = w[Q * i + q];
+                gh[4 * q] = fmaf(wq.x, hi, gh[4 * q]); gh[4 * q + 1] = fmaf(wq.y, hi, gh[4 * q + 1]);
+                gh[4 * q + 2] = fmaf(wq.z, hi, gh[4 * q + 2]); gh[4 * q + 3] = fmaf(wq.w, hi, gh[4 * q + 3]);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < G; ++r)
+            if (u + r < H) {
+                const float ig = mgb_sigmoid(gi[r] + gh[r]);
+                const float fg = mgb_sigmoid(gi[G + r] + gh[G + r]);
+                const float gg = tanhf(gi[2 * G + r] + gh[2 * G + r]);
+                const float og = mgb_sigmoid(gi[3 * G + r] + gh[3 * G + r]);
+                const float cn = fmaf(fg, c[(u + r) * stride], ig * gg);
+                c[(u + r) * stride] = cn;
+                h[(u + r) * stride] = og * tanhf(cn);
             }
     }
 }

@@ -697,17 +697,18 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         [N,<obs of one env>] (the window acted on at t = 0; at t > 0 it is obs[t-1]).  `actions` together with
         `policy` is a ValueError.
 
-        policy may also be a GRUPolicy (mgb_maze_rollout_rnn; needs auto_reset=True), with state: its carried state
-        [N, policy.state_dim] float32 on the env's device (policy.initial_state(N) for fresh envs), read at the start
-        and updated in place at the end of the launch.  The dict then also holds "state0" (a copy of state as read),
-        "resampled" (whether the launch resampled, which unroll() needs for the "task" reset rule) and, with
-        want_hidden=True, "hid" [T,N,H] (the cell's output at every step)."""
-        from .policy import GRUPolicy
-        recurrent = isinstance(policy, GRUPolicy)
+        policy may also be a GRUPolicy or an LSTMPolicy (mgb_maze_rollout_rnn; needs auto_reset=True), with state:
+        its carried state [N, policy.state_dim] float32 on the env's device (policy.initial_state(N) for fresh envs),
+        read at the start and updated in place at the end of the launch.  The dict then also holds "state0" (a copy
+        of state as read), "resampled" (whether the launch resampled, which unroll() needs for the "task" reset rule)
+        and, with want_hidden=True, "hid" [T,N,H] (the cell's output at every step)."""
+        from .policy import GRUPolicy, LSTMPolicy
+        recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy))
         if recurrent and state is None:
-            raise ValueError("a GRUPolicy rollout needs its carried state (state=policy.initial_state(num_envs))")
+            raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
+                             % type(policy).__name__)
         if state is not None and not recurrent:
-            raise ValueError("state= goes with a GRUPolicy")
+            raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")

@@ -7,9 +7,10 @@ then ``b [out]``, first hidden layer to output layer, then ``log_std [4]`` (the 
 MetaMaze2D rollout reads the four outputs as logits and ignores it).  The buffer lives on the env's device and is
 read at every launch, so ``update()`` after an optimiser step is seen by a rollout already captured in a CUDA graph.
 
-GRUPolicy packs an ``nn.GRUCell`` and a head for the recurrent MetaMaze2D rollout (mgb_maze_rollout_rnn; DESIGN.md
-"Recurrent policies"): ``weight_ih``, ``weight_hh``, ``bias_ih``, ``bias_hh``, then the head's layers as MLPPolicy packs
-them.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities through the torch modules.
+GRUPolicy and LSTMPolicy pack an ``nn.GRUCell`` or an ``nn.LSTMCell`` and a head for the recurrent MetaMaze2D rollout
+(mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies"): ``weight_ih``, ``weight_hh``, ``bias_ih``, ``bias_hh``, then the
+head's layers as MLPPolicy packs them.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities
+through the torch modules.
 """
 import ctypes
 
@@ -138,7 +139,7 @@ MAX_RNN_HIDDEN = 64  # MGB_RNN_MAX_HIDDEN
 _RESETS = {"episode": _lib.RNN_RESET_EPISODE, "task": _lib.RNN_RESET_TASK}
 
 
-def _head_layers(head, H):
+def _head_layers(head, H, name="GRUPolicy"):
     """(linears, activation code) of Linear(H, 4) or Linear(H, w) Act Linear(w, 4); ValueError for anything else."""
     import torch.nn as nn
     if type(head) is nn.Linear:
@@ -146,61 +147,60 @@ def _head_layers(head, H):
     try:
         lin, act = _layers(head)
     except ValueError as err:
-        raise ValueError("GRUPolicy head: %s" % err)
+        raise ValueError("%s head: %s" % (name, err))
     if len(lin) > 2:
-        raise ValueError("GRUPolicy: the head has at most one hidden layer")
+        raise ValueError("%s: the head has at most one hidden layer" % name)
     if lin[0].in_features != H:
-        raise ValueError("GRUPolicy: the head takes %d inputs, the cell has %d units" % (lin[0].in_features, H))
+        raise ValueError("%s: the head takes %d inputs, the cell has %d units" % (name, lin[0].in_features, H))
     return lin, act
 
 
-class GRUPolicy(object):
-    """A torch GRUCell and head packed for the recurrent MetaMaze2D rollout (BatchedMetaMaze2D.rollout(policy=, state=)).
-
-    cell: nn.GRUCell(obs_dim + 5 feedback, H), H 1..64.  head: nn.Linear(H, 4), or nn.Sequential(Linear(H, w), Tanh or
-    ReLU, Linear(w, 4)) with w 1..64; its four outputs are the logits of the actions.  feedback: the cell's input ends
-    with onehot(prev action) and the prev reward.  hidden_reset: "episode" zeroes an env's state at every done; "task"
-    only where the env drew a new maze inside the launch (rollout with resample=); after set_task / update_tasks /
-    resample_tasks the caller zeroes the rows itself.  log_std: the maze's categorical head has none; it must be None.
-    obs_mean / obs_std: optional [obs_dim] normalisation (x - mean) / std of the observation inputs, folded into the
-    obs columns of weight_ih and into bias_ih on the host in float64.  device: where the packed buffer lives.
-    """
+class _RecurrentPolicy(object):
+    """What GRUPolicy and LSTMPolicy share: validation, the head, packing, update() and the unroll skeleton.  A
+    subclass names its torch cell type (_torch_cell), its gate count, how many H-wide rows its carried memory has and
+    its MGB_RNN_CELL_* code, and runs one step of its cell in _step()."""
+    _gates = 0          # 3 (r, z, n) or 4 (i, f, g, o)
+    _memory = 0         # H-wide rows of the carried memory before the feedback: 1 (h) or 2 (h, c)
+    _cell_code = 0      # MGB_RNN_CELL_*
 
     def __init__(self, cell, head, log_std=None, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None,
                  device="cuda"):
         import torch
-        import torch.nn as nn
         self._torch = torch
-        if type(cell) is not nn.GRUCell:
-            raise ValueError("GRUPolicy takes an nn.GRUCell, got %s" % type(cell).__name__)
+        name, kind = type(self).__name__, self._torch_cell()
+        if type(cell) is not kind:
+            raise ValueError("%s takes an nn.%s, got %s" % (name, kind.__name__, type(cell).__name__))
         if log_std is not None:
-            raise ValueError("GRUPolicy: the MetaMaze2D head is categorical and has no log_std")
+            raise ValueError("%s: the MetaMaze2D head is categorical and has no log_std" % name)
         if feedback not in (True, False, 0, 1):
-            raise ValueError("GRUPolicy: feedback must be True or False")
+            raise ValueError("%s: feedback must be True or False" % name)
         if hidden_reset not in _RESETS:
-            raise ValueError("GRUPolicy: hidden_reset must be \"episode\" or \"task\"")
+            raise ValueError("%s: hidden_reset must be \"episode\" or \"task\"" % name)
         self.feedback = bool(feedback)
         self.hidden_reset = hidden_reset
         self.hidden = cell.hidden_size
         if not 1 <= self.hidden <= MAX_RNN_HIDDEN:
-            raise ValueError("GRUPolicy: the cell's hidden size must be 1..%d" % MAX_RNN_HIDDEN)
+            raise ValueError("%s: the cell's hidden size must be 1..%d" % (name, MAX_RNN_HIDDEN))
         self.obs_dim = cell.input_size - FEEDBACK * self.feedback
         if self.obs_dim < 1:
-            raise ValueError("GRUPolicy: with feedback the cell takes obs_dim + 5 inputs")
-        lin, self.activation = _head_layers(head, self.hidden)
+            raise ValueError("%s: with feedback the cell takes obs_dim + 5 inputs" % name)
+        lin, self.activation = _head_layers(head, self.hidden, name)
         self.head_width = lin[0].out_features if len(lin) == 2 else 0
-        self.state_dim = self.hidden + FEEDBACK * self.feedback
+        self.state_dim = self._memory * self.hidden + FEEDBACK * self.feedback
         H, n_in = self.hidden, cell.input_size
-        self.numel = 3 * H * (n_in + H + 2) + sum(m.out_features * (m.in_features + 1) for m in lin)
+        self.numel = self._gates * H * (n_in + H + 2) + sum(m.out_features * (m.in_features + 1) for m in lin)
         self.device = torch.device(device)
         self.params = torch.zeros(self.numel, dtype=torch.float32, device=self.device)
         self._cell, self._head, self._mean, self._std = cell, head, None, None
         self.update(cell, head, obs_mean, obs_std)
 
+    def _torch_cell(self):
+        raise NotImplementedError
+
     def _vec(self, x, n, what):
         t = self._torch.as_tensor(x).detach().to("cpu", self._torch.float64).reshape(-1)
         if t.numel() != n:
-            raise ValueError("GRUPolicy: %s must have %d entries" % (what, n))
+            raise ValueError("%s: %s must have %d entries" % (type(self).__name__, what, n))
         return t
 
     def pack(self):
@@ -208,7 +208,7 @@ class GRUPolicy(object):
         torch = self._torch
         cell, H, D = self._cell, self.hidden, self.obs_dim
         f64 = lambda t: t.detach().to("cpu", torch.float64)          # noqa: E731
-        zeros = torch.zeros(3 * H, dtype=torch.float64)
+        zeros = torch.zeros(self._gates * H, dtype=torch.float64)
         Wi, Wh = f64(cell.weight_ih).clone(), f64(cell.weight_hh)
         bi = f64(cell.bias_ih) if cell.bias_ih is not None else zeros
         bh = f64(cell.bias_hh) if cell.bias_hh is not None else zeros
@@ -219,7 +219,7 @@ class GRUPolicy(object):
             bi = bi - Wi[:, :D] @ (mean / std)
             Wi[:, :D] = Wi[:, :D] / std
         parts = [Wi.reshape(-1), Wh.reshape(-1), bi, bh]
-        lin, _ = _head_layers(self._head, H)
+        lin, _ = _head_layers(self._head, H, type(self).__name__)
         for m in lin:
             parts += [f64(m.weight).reshape(-1), f64(m.bias) if m.bias is not None else
                       torch.zeros(m.out_features, dtype=torch.float64)]
@@ -228,20 +228,20 @@ class GRUPolicy(object):
     def update(self, cell=None, head=None, obs_mean=None, obs_std=None):
         """Repack into the same device buffer (copy_, stream-ordered): a graph captured on this policy sees the new
         weights.  Arguments left None keep their previous values; cell and head must keep their shapes."""
-        import torch.nn as nn
-        if cell is not None and (type(cell) is not nn.GRUCell or cell.input_size != self._cell.input_size
+        name = type(self).__name__
+        if cell is not None and (type(cell) is not self._torch_cell() or cell.input_size != self._cell.input_size
                                  or cell.hidden_size != self.hidden):
-            raise ValueError("GRUPolicy.update: the cell must keep its input and hidden sizes")
+            raise ValueError("%s.update: the cell must keep its input and hidden sizes" % name)
         if head is not None:
-            lin, act = _head_layers(head, self.hidden)
+            lin, act = _head_layers(head, self.hidden, name)
             if (lin[0].out_features if len(lin) == 2 else 0) != self.head_width or act != self.activation:
-                raise ValueError("GRUPolicy.update: the head must keep its layer shapes and activation")
+                raise ValueError("%s.update: the head must keep its layer shapes and activation" % name)
         mean = None if obs_mean is None else self._vec(obs_mean, self.obs_dim, "obs_mean")
         std = None if obs_std is None else self._vec(obs_std, self.obs_dim, "obs_std")
         if mean is not None and not self._torch.isfinite(mean).all():
-            raise ValueError("GRUPolicy: obs_mean must be finite")
+            raise ValueError("%s: obs_mean must be finite" % name)
         if std is not None and not (self._torch.isfinite(std).all() and (std > 0).all()):
-            raise ValueError("GRUPolicy: obs_std must be finite and strictly positive")
+            raise ValueError("%s: obs_std must be finite and strictly positive" % name)
         if cell is not None:
             self._cell = cell
         if head is not None:
@@ -257,19 +257,23 @@ class GRUPolicy(object):
         """The mgb_rnn_policy the C entry point takes."""
         return _lib.RnnPolicy(self.params.data_ptr(), self.hidden, int(self.feedback), _RESETS[self.hidden_reset],
                               int(self.head_width > 0), self.head_width, self.activation,
-                              _lib.POLICY_MEAN if deterministic else _lib.POLICY_SAMPLE)
+                              _lib.POLICY_MEAN if deterministic else _lib.POLICY_SAMPLE, self._cell_code)
 
     def initial_state(self, num_envs):
-        """[num_envs, H + 5 feedback] float32 zeros on the policy's device: the state of envs that start fresh."""
+        """[num_envs, state_dim] float32 zeros on the policy's device: the state of envs that start fresh."""
         return self._torch.zeros((int(num_envs), self.state_dim), dtype=self._torch.float32, device=self.device)
+
+    def _step(self, x, mem):
+        """(h, memory carried to the next step) of one cell step; mem holds the _memory H-wide rows of the state."""
+        raise NotImplementedError
 
     def unroll(self, out):
         """Recompute a recurrent rollout with autograd through the cell and head: returns (logits [T, N, 4],
         logp [T, N]), logp the log-probability of out["act"].  Uses out's obs0, obs, act, rew, done, state0 and
         resampled, and applies the kernel's input construction and reset rule, in the cell's dtype and device."""
         torch = self._torch
-        cell, head, H, D = self._cell, self._head, self.hidden, self.obs_dim
-        w = cell.weight_ih
+        head, D = self._head, self.obs_dim
+        w = self._cell.weight_ih
         dt, dev = w.dtype, w.device
         act = out["act"].to(dev).long()
         T, N = act.shape
@@ -282,17 +286,60 @@ class GRUPolicy(object):
         done = out["done"].to(dev).bool()
         state0 = out["state0"].to(dev, dt)
         wipe_on_done = self.hidden_reset == "episode" or bool(out.get("resampled", False))
-        c, fb = state0[:, :H], state0[:, H:]
+        nm = self._memory * self.hidden
+        mem, fb = state0[:, :nm], state0[:, nm:]
         logits, logp = [], []
         for t in range(T):
             x = torch.cat([obs[t], fb], 1) if self.feedback else obs[t]
-            h = cell(x, c)
+            h, new_mem = self._step(x, mem)
             lg = head(h)
             logits.append(lg)
             logp.append(torch.log_softmax(lg, -1).gather(1, act[t][:, None])[:, 0])
             keep = ~(done[t] & wipe_on_done)
-            c = torch.where(keep[:, None], h, torch.zeros_like(h))
+            mem = torch.where(keep[:, None], new_mem, torch.zeros_like(new_mem))
             if self.feedback:
                 new_fb = torch.cat([torch.nn.functional.one_hot(act[t], 4).to(dt), rew[t][:, None]], 1)
                 fb = torch.where(keep[:, None], new_fb, torch.zeros_like(new_fb))
         return torch.stack(logits), torch.stack(logp)
+
+
+class GRUPolicy(_RecurrentPolicy):
+    """A torch GRUCell and head packed for the recurrent MetaMaze2D rollout (BatchedMetaMaze2D.rollout(policy=, state=)).
+
+    cell: nn.GRUCell(obs_dim + 5 feedback, H), H 1..64.  head: nn.Linear(H, 4), or nn.Sequential(Linear(H, w), Tanh or
+    ReLU, Linear(w, 4)) with w 1..64; its four outputs are the logits of the actions.  feedback: the cell's input ends
+    with onehot(prev action) and the prev reward.  hidden_reset: "episode" zeroes an env's state at every done; "task"
+    only where the env drew a new maze inside the launch (rollout with resample=); after set_task / update_tasks /
+    resample_tasks the caller zeroes the rows itself.  log_std: the maze's categorical head has none; it must be None.
+    obs_mean / obs_std: optional [obs_dim] normalisation (x - mean) / std of the observation inputs, folded into the
+    obs columns of weight_ih and into bias_ih on the host in float64.  device: where the packed buffer lives.
+    The carried state is [N, H + 5 feedback] = [h, onehot(prev action), prev reward].
+    """
+    _gates, _memory, _cell_code = 3, 1, _lib.RNN_CELL_GRU
+
+    def _torch_cell(self):
+        return self._torch.nn.GRUCell
+
+    def _step(self, x, mem):
+        h = self._cell(x, mem)
+        return h, h
+
+
+class LSTMPolicy(_RecurrentPolicy):
+    """A torch LSTMCell and head packed for the recurrent MetaMaze2D rollout (BatchedMetaMaze2D.rollout(policy=,
+    state=)): GRUPolicy's interface and semantics with nn.LSTMCell(obs_dim + 5 feedback, H), H 1..64, whose four gates
+    (i, f, g, o) are packed in torch's order.  The carried state is [N, 2H + 5 feedback] = [h, c, onehot(prev action),
+    prev reward]; the reset rule zeroes the whole row, h and c included.
+    """
+    _gates, _memory, _cell_code = 4, 2, _lib.RNN_CELL_LSTM
+
+    def __init__(self, cell, head, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None, device="cuda"):
+        super().__init__(cell, head, None, feedback, hidden_reset, obs_mean, obs_std, device)
+
+    def _torch_cell(self):
+        return self._torch.nn.LSTMCell
+
+    def _step(self, x, mem):
+        H = self.hidden
+        h, c = self._cell(x, (mem[:, :H], mem[:, H:]))
+        return h, self._torch.cat([h, c], 1)

@@ -361,8 +361,8 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
-            from .policy import GRUPolicy
-            if isinstance(policy, GRUPolicy):
+            from .policy import GRUPolicy, LSTMPolicy
+            if isinstance(policy, (GRUPolicy, LSTMPolicy)):
                 raise ValueError("recurrent policies run on MetaMaze2D only; the quadrotor takes an MLPPolicy")
             return self._rollout_policy(T, policy, act_seed, deterministic, out)
         if out is None:
