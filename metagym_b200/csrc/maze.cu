@@ -506,18 +506,16 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // (post auto-reset and resampling) into the thread's column of the activation buffers, which follow the tiles and the
 // sampler workspaces in dynamic shared memory at pol.smem_off; at t = 0 the window of the loaded state.  The step
 // arithmetic after the action is the code the other instantiations run.
-// POL == kPolGru (mgb_maze_rollout_rnn): the policy is the GRU `pol` (mgb_policy.cuh).  Its region at pol.smem_off holds
-// the staged cell and head, then the columns x [in], c [H], h [H] and the head's w.  The obs rows of x are filled as
-// POL == kPolMlp fills its input; at t = 0 the state row fills c and the feedback rows of x.  Step t computes h from
-// (x, c), acts on head(h), and after the step carries h into c (the two columns swap roles) and (onehot(a), (float)r)
-// into the feedback rows, or zeroes both where done and the reset rule fires; the state row is stored after step T - 1.
-// POL == kPolLstm: the policy is the LSTM `pol`.  Its columns are x [in], the cell state c [H] and two h columns of Hr
-// rows.  Step t computes h from (x, h_{t-1}, c), updating c in place, then the head's hidden layer reuses the dead
-// h_{t-1} column; the carry swaps the two h columns as the GRU does, and a wipe zeroes c as well.
+// POL == kPolGru or kPolLstm (mgb_maze_rollout_rnn): the policy is the recurrent `pol` (MgbRnn, mgb_policy.cuh).  Its
+// region at pol.smem_off holds the staged cell and head, then the columns x, c, h0, h1 and w.  The obs rows of x are
+// filled as for the MLP; at t = 0 the state row fills h0, c and the feedback rows of x.  Step t computes h1 from
+// (x, h0, c), updating c in place, and acts on head(h1), whose hidden layer goes to w (GRU) or the dead h0 (LSTM).
+// After the step the carry swaps h0 and h1 and writes (onehot(a), (float)r) into the feedback rows, or zeroes h, c and
+// the feedback where done and the reset rule fires; the state row is stored after step T - 1.
 constexpr int kPolMlp = 1, kPolGru = 2, kPolLstm = 3;
 
 template <int POL>
-using MazePolicyPlan = std::conditional_t<POL == kPolLstm, MgbLstm, std::conditional_t<POL == kPolGru, MgbGru, MgbMlp>>;
+using MazePolicyPlan = std::conditional_t<POL == kPolLstm, MgbRnn<4>, std::conditional_t<POL == kPolGru, MgbRnn<3>, MgbMlp>>;
 
 template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0>
 __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
@@ -547,63 +545,40 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
     const int n = c.n, g = c.view_grid;
-    float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the two activation buffers
-    float *hid_prev = nullptr, *hid_new = nullptr;                  // RNN: the carried and the new hidden state
-    float *lstm_c = nullptr;                                        // kPolLstm: the cell state
-    if constexpr (POL == kPolMlp) {
-        static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
+    float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the input, the hidden layer
+    float *hid_prev = nullptr, *hid_new = nullptr, *cst = nullptr;  // RNN: the columns h0, h1 and c
+    const MgbMlp &head = mgb_policy_head(pol);                      // the plan of the categorical head
+    if constexpr (POL) {
+        static_assert(XM == 0, "policy rollouts are not mirrored");
         pol_w = tile2d + pol.smem_off;
         pol_x = pol_w + pol.staged;
-        pol_y = pol_x + pol.maxw * k2dThreads;
-        mgb_mlp_stage(pol, pol_w);
+        if constexpr (RNN) {
+            cst = pol_x + pol.in * k2dThreads;
+            hid_prev = cst + pol.C() * k2dThreads;
+            hid_new = hid_prev + pol.Hr * k2dThreads;
+            pol_y = hid_new + pol.Hr * k2dThreads;     // w; the LSTM's head uses the dead h0 instead
+            mgb_rnn_stage(pol, pol_w);
+        } else {
+            pol_y = pol_x + pol.maxw * k2dThreads;
+            mgb_mlp_stage(pol, pol_w);
+        }
         if (active) {       // the window of the loaded state: what the preceding reset() / step() returned
             float *row = tile2d + threadIdx.x * D;
             maze2d_window(c, blob, eaten, a.n_pad, s, row);
             for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = row[k];
-            if (pol.obs0_out)
-                for (int k = 0; k < D; ++k) pol.obs0_out[e * D + k] = row[k];
-        }
-        __syncthreads();    // the staged weights (the RS loop has no CTA barrier)
-    }
-    if constexpr (RNN) {
-        static_assert(XM == 0, "policy rollouts are not mirrored");
-        pol_w = tile2d + pol.smem_off;
-        pol_x = pol_w + pol.staged;
-        if constexpr (POL == kPolGru) {
-            hid_prev = pol_x + pol.in * k2dThreads;
-            hid_new = hid_prev + pol.H * k2dThreads;
-            pol_y = hid_new + pol.H * k2dThreads;      // the head's hidden layer
-            mgb_gru_stage(pol, pol_w);
-        } else {
-            lstm_c = pol_x + pol.in * k2dThreads;
-            hid_prev = lstm_c + pol.H * k2dThreads;
-            hid_new = hid_prev + pol.Hr * k2dThreads;
-            mgb_lstm_stage(pol, pol_w);
-        }
-        if (active) {
-            float *row = tile2d + threadIdx.x * D;
-            maze2d_window(c, blob, eaten, a.n_pad, s, row);
-            for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = row[k];
-            if (pol.head.obs0_out)
-                for (int k = 0; k < D; ++k) pol.head.obs0_out[e * D + k] = row[k];
-            if constexpr (POL == kPolGru) {
-                const int S = pol.H + 5 * pol.feedback;
+            if (head.obs0_out)
+                for (int k = 0; k < D; ++k) head.obs0_out[e * D + k] = row[k];
+            if constexpr (RNN) {        // [h, c, feedback]
+                const int S = pol.HC() + 5 * pol.feedback;
                 const float *st = pol.state + e * S;
                 for (int k = 0; k < pol.H; ++k) hid_prev[k * k2dThreads + threadIdx.x] = st[k];
-                for (int k = pol.H; k < S; ++k) pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x] = st[k];
-                if (pol.state0_out)
-                    for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
-            } else {        // [h, c, feedback]
-                const int S = 2 * pol.H + 5 * pol.feedback;
-                const float *st = pol.state + e * S;
-                for (int k = 0; k < pol.H; ++k) hid_prev[k * k2dThreads + threadIdx.x] = st[k];
-                for (int k = 0; k < pol.H; ++k) lstm_c[k * k2dThreads + threadIdx.x] = st[pol.H + k];
-                for (int k = 2 * pol.H; k < S; ++k) pol_x[(D + k - 2 * pol.H) * k2dThreads + threadIdx.x] = st[k];
+                for (int k = 0; k < pol.C(); ++k) cst[k * k2dThreads + threadIdx.x] = st[pol.H + k];
+                for (int k = pol.HC(); k < S; ++k) pol_x[(D + k - pol.HC()) * k2dThreads + threadIdx.x] = st[k];
                 if (pol.state0_out)
                     for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
             }
         }
-        __syncthreads();    // the staged weights
+        __syncthreads();    // the staged weights (the RS loop has no CTA barrier)
     }
     for (int t = 0; t < a.T; ++t) {
         float *tile = tile2d + (size_t)(t & 1) * k2dThreads * D;
@@ -617,24 +592,21 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
         uint32_t done_byte = 0;
         if (active) {
             int action;
-            if constexpr (POL == kPolMlp) {
+            if constexpr (POL) {
                 float logits[4];
-                mgb_mlp_forward(pol, pol_w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
-                const float lp = mgb_categorical_action(pol, genv, a.t_base + (uint32_t)t, logits, action);
+                if constexpr (RNN) {
+                    mgb_rnn_cell(pol, pol_w, pol_x, hid_prev, cst, hid_new, k2dThreads, threadIdx.x);
+                    if (pol.hid_out)
+                        for (int k = 0; k < pol.H; ++k)
+                            pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * k2dThreads + threadIdx.x];
+                    if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
+                    mgb_mlp_forward(head, pol_w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits);
+                } else {
+                    mgb_mlp_forward(pol, pol_w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
+                }
+                const float lp = mgb_categorical_action(head, genv, a.t_base + (uint32_t)t, logits, action);
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
-                if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
-            } else if constexpr (RNN) {
-                if constexpr (POL == kPolGru) mgb_gru_cell(pol, pol_w, pol_x, hid_prev, hid_new, k2dThreads, threadIdx.x);
-                else mgb_lstm_cell(pol, pol_w, pol_x, hid_prev, lstm_c, hid_new, k2dThreads, threadIdx.x);
-                if (pol.hid_out)
-                    for (int k = 0; k < pol.H; ++k)
-                        pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * k2dThreads + threadIdx.x];
-                if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
-                float logits[4];
-                mgb_mlp_forward(pol.head, pol_w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits);
-                const float lp = mgb_categorical_action(pol.head, genv, a.t_base + (uint32_t)t, logits, action);
-                if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
-                if (pol.head.logp_out) pol.head.logp_out[(int64_t)t * a.n + e] = lp;
+                if (head.logp_out) head.logp_out[(int64_t)t * a.n + e] = lp;
             } else if (a.act) action = a.act[(int64_t)t * a.n + e];
             else {
                 const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
@@ -687,11 +659,10 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
             if constexpr (RNN) {
                 // carry: with RS every finished env draws a new maze, so the task rule fires exactly where done does
                 const bool wipe = done && (RS || pol.reset == MGB_RNN_RESET_EPISODE);
-                if (wipe)
+                if (wipe) {
                     for (int k = 0; k < pol.H; ++k) hid_new[k * k2dThreads + threadIdx.x] = 0.f;
-                if constexpr (POL == kPolLstm)
-                    if (wipe)
-                        for (int k = 0; k < pol.H; ++k) lstm_c[k * k2dThreads + threadIdx.x] = 0.f;
+                    for (int k = 0; k < pol.C(); ++k) cst[k * k2dThreads + threadIdx.x] = 0.f;
+                }
                 if (pol.feedback) {
                     float *fb = pol_x + D * k2dThreads + threadIdx.x;
                     for (int k = 0; k < 4; ++k) fb[k * k2dThreads] = !wipe && k == action ? 1.f : 0.f;
@@ -781,18 +752,11 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     }
     if constexpr (RNN) {
         if (active) {
-            if constexpr (POL == kPolGru) {
-                const int S = pol.H + 5 * pol.feedback;
-                float *st = pol.state + e * S;
-                for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * k2dThreads + threadIdx.x];
-                for (int k = pol.H; k < S; ++k) st[k] = pol_x[(D + k - pol.H) * k2dThreads + threadIdx.x];
-            } else {
-                const int S = 2 * pol.H + 5 * pol.feedback;
-                float *st = pol.state + e * S;
-                for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * k2dThreads + threadIdx.x];
-                for (int k = 0; k < pol.H; ++k) st[pol.H + k] = lstm_c[k * k2dThreads + threadIdx.x];
-                for (int k = 2 * pol.H; k < S; ++k) st[k] = pol_x[(D + k - 2 * pol.H) * k2dThreads + threadIdx.x];
-            }
+            const int S = pol.HC() + 5 * pol.feedback;
+            float *st = pol.state + e * S;
+            for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * k2dThreads + threadIdx.x];
+            for (int k = 0; k < pol.C(); ++k) st[pol.H + k] = cst[k * k2dThreads + threadIdx.x];
+            for (int k = pol.HC(); k < S; ++k) st[k] = pol_x[(D + k - pol.HC()) * k2dThreads + threadIdx.x];
         }
     }
     if constexpr (RS) {
@@ -4162,6 +4126,16 @@ static int rollout_engine(mgb_maze *h, bool resample, cudaStream_t st, RolloutEn
     return rc;
 }
 
+// Dynamic shared memory of a 2-D rollout CTA in front of a policy's region: two observation tiles and, when resampling,
+// one sampler workspace per warp (16-byte multiples), rounded up to 16 bytes
+static size_t maze2d_tiles_bytes(const mgb_maze *h, bool resample)
+{
+    const int W = 2 * h->c.view_grid + 1;
+    size_t sm = (size_t)2 * k2dThreads * W * W * 4;
+    if (resample) sm += (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
+    return (sm + 15) / 16 * 16;
+}
+
 extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_seed, void *act_out_dev,
                                 void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev,
                                 uint8_t *truncated_dev, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
@@ -4221,9 +4195,7 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
             rc = resample_cfg ? launch_render<false, true, false, true>(h, a, grid, st, r)
                               : launch_render<false, true>(h, a, grid, st);
     } else if (resample_cfg) {
-        // two observation tiles, then one sampler workspace per warp (16-byte multiples)
-        const int W = 2 * h->c.view_grid + 1;
-        const size_t sm = (size_t)2 * k2dThreads * W * W * 4 + (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
+        const size_t sm = maze2d_tiles_bytes(h, true);
         int optin = 0;
         MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
         if (sm > (size_t)optin) {
@@ -4246,8 +4218,7 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
                         "multicast outputs must be 4-byte (rewards: 8-byte) aligned");
         }
         a.mir = h->mir;
-        const int W = 2 * h->c.view_grid + 1;
-        const size_t sm = (size_t)2 * k2dThreads * W * W * 4;
+        const size_t sm = maze2d_tiles_bytes(h, false);
         const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
         const int xm = h->mir.count == MGB_MIRROR_MULTICAST ? 2 : (h->mir.count > 0 ? 1 : 0);
         rc = h->path ? launch_2d_rollout<true>(h->c, xm, fin, a, blocks, sm, st)
@@ -4261,9 +4232,9 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
 
 // maze2d_rollout_kernel<0, fin, REC, RS, POL>, sm bytes of dynamic shared memory; refused (as `fn`) when the CTA would
 // need more shared memory than the device allows
-template <bool REC, bool RS, int POL, class Plan>
+template <bool REC, bool RS, int POL>
 static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r,
-                            const Plan &m, unsigned blocks, size_t sm, cudaStream_t st)
+                            const MazePolicyPlan<POL> &m, unsigned blocks, size_t sm, cudaStream_t st)
 {
     const auto kernel = fin ? maze2d_rollout_kernel<0, true, REC, RS, POL> : maze2d_rollout_kernel<0, false, REC, RS, POL>;
     int optin = 0;
@@ -4283,20 +4254,26 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
     return MGB_OK;
 }
 
-extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
-                                       const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
-                                       int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
-                                       double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
-                                       void *stream)
+// A policy rollout of kind POL (mgb_maze_rollout_policy, mgb_maze_rollout_rnn) with the plan `pol`.  The checks, in
+// order: the handle, T, the handle kind, then own(observation width) (the entry point plans the policy into pol and
+// makes its own checks; it returns the refusal, or nullptr), logp_out in the mean mode, mirrors, resampling, the
+// optional outputs and the handle's state.  The policy's region of dynamic shared memory follows the tiles and the
+// sampler workspaces.
+template <int POL, class Own>
+static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolicyPlan<POL> &pol, Own own, uint64_t seed,
+                               const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, int32_t *act_out_dev,
+                               float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev,
+                               uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
-    MgbRange nvtx_range("mgb_maze_rollout_policy");
+    MgbMlp &head = mgb_policy_head(pol);
     SamplerCfg sc;
-    MgbMlp m;
-    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
-        if (h->c.kind != MGB_MAZE_2D) return "mgb_maze_rollout_policy serves MetaMaze2D (the 3-D envs observe frames)";
+    int rc = check_rollout(fn, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
+        if (h->c.kind != MGB_MAZE_2D)
+            return POL == kPolMlp ? "mgb_maze_rollout_policy serves MetaMaze2D (the 3-D envs observe frames)"
+                                  : "mgb_maze_rollout_rnn serves MetaMaze2D (the 3-D envs observe frames)";
         const int W = 2 * h->c.view_grid + 1;
-        if (const char *why = mgb_mlp_plan(pol, W * W, false, m)) return why;
-        if (logp_out_dev && m.mode != MGB_POLICY_SAMPLE) return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
+        if (const char *why = own(W * W)) return why;
+        if (logp_out_dev && head.mode != MGB_POLICY_SAMPLE) return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
         if (!resample_cfg) return nullptr;
@@ -4305,16 +4282,14 @@ extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy 
     });
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
-    // two observation tiles, the sampler workspaces when resampling, then the policy's weights and activations
-    const int W = 2 * h->c.view_grid + 1;
-    size_t base = (size_t)2 * k2dThreads * W * W * 4;
-    if (resample_cfg) base += (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
-    base = (base + 15) / 16 * 16;
-    m.smem_off = (int)(base / 4);
-    m.seed = seed;
-    m.logp_out = logp_out_dev;
-    m.obs0_out = obs0_out_dev;
-    const size_t sm = base + mgb_mlp_smem_bytes(m, k2dThreads);
+    const size_t base = maze2d_tiles_bytes(h, resample_cfg != nullptr);
+    pol.smem_off = (int)(base / 4);
+    head.seed = seed;
+    head.logp_out = logp_out_dev;
+    head.obs0_out = obs0_out_dev;
+    size_t sm = base;
+    if constexpr (POL == kPolMlp) sm += mgb_mlp_smem_bytes(pol, k2dThreads);
+    else sm += mgb_rnn_smem_bytes(pol, k2dThreads);
     MazeArgs a = maze_args(h);
     a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
     a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
@@ -4327,15 +4302,29 @@ extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy 
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     const cudaStream_t st = (cudaStream_t)stream;
     if (resample_cfg)
-        rc = h->path ? launch_2d_policy<true, true, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st)
-                     : launch_2d_policy<false, true, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st);
+        rc = h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st)
+                     : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st);
     else
-        rc = h->path ? launch_2d_policy<true, false, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st)
-                     : launch_2d_policy<false, false, kPolMlp>(__func__, h, fin, a, r, m, blocks, sm, st);
+        rc = h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st)
+                     : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st);
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
+}
+
+extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
+                                       const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                       int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                                       double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_policy");
+    MgbMlp m;
+    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m); };
+    return maze_rollout_policy<kPolMlp>(__func__, h, T, m, own, seed, resample_cfg, resample_seed, act_out_dev,
+                                        logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev,
+                                        truncated_dev, stream);
 }
 
 extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed,
@@ -4346,66 +4335,26 @@ extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy
                                     float *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout_rnn");
-    SamplerCfg sc;
-    MgbGru g;
-    MgbLstm l;
-    const bool lstm = pol && pol->cell == MGB_RNN_CELL_LSTM;
-    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
-        if (h->c.kind != MGB_MAZE_2D) return "mgb_maze_rollout_rnn serves MetaMaze2D (the 3-D envs observe frames)";
-        const int W = 2 * h->c.view_grid + 1;
-        if (const char *why = lstm ? mgb_lstm_plan(pol, W * W, l) : mgb_gru_plan(pol, W * W, g)) return why;
-        if (!state_dev) return "null state";
-        if ((uintptr_t)state_dev % sizeof(float)) return "state must be 4-byte aligned";
-        if (!h->auto_reset) return "the recurrent rollout needs auto_reset on (an episode boundary has no next step without it)";
-        if (logp_out_dev && (lstm ? l.head.mode : g.head.mode) != MGB_POLICY_SAMPLE)
-            return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
-        if (h->mir.count != 0)
-            return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
-        if (!resample_cfg) return nullptr;
-        return sampler_cfg(h, resample_cfg, sc);
-    });
-    if (rc) return rc;
-    MgbDeviceGuard guard(h->device);
-    // two observation tiles, the sampler workspaces when resampling, then the cell, the head and the columns
-    const int W = 2 * h->c.view_grid + 1;
-    size_t base = (size_t)2 * k2dThreads * W * W * 4;
-    if (resample_cfg) base += (size_t)(k2dThreads / 32) * sampler_ws_bytes(h->c.n);
-    base = (base + 15) / 16 * 16;
-    MazeArgs a = maze_args(h);
-    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
-    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
-    MazeResample r = {};
-    if (resample_cfg) {
-        r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
-    }
-    const bool fin = final_obs_dev || truncated_dev;
-    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
-    const cudaStream_t st = (cudaStream_t)stream;
-    // the same launch for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>, p its plan
-    const char *const fn = __func__;    // (inside the lambda __func__ would name the lambda)
-    const auto launch = [&](auto kind, auto &p, size_t cell_bytes) {
+    // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
+    const auto run = [&](auto kind) {
         constexpr int POL = decltype(kind)::value;
-        p.smem_off = (int)(base / 4);
-        p.head.seed = seed;
-        p.head.logp_out = logp_out_dev;
-        p.head.obs0_out = obs0_out_dev;
-        p.state = state_dev;
-        p.state0_out = state0_out_dev;
-        p.hid_out = hid_out_dev;
-        const size_t sm = base + cell_bytes;
-        if (resample_cfg)
-            return h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, p, blocks, sm, st)
-                           : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, p, blocks, sm, st);
-        return h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, p, blocks, sm, st)
-                       : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, p, blocks, sm, st);
+        MazePolicyPlan<POL> p;
+        const auto own = [&](int obs_dim) -> const char * {
+            if (const char *why = mgb_rnn_plan(pol, obs_dim, p)) return why;
+            p.state = state_dev;
+            p.state0_out = state0_out_dev;
+            p.hid_out = hid_out_dev;
+            if (!state_dev) return "null state";
+            if ((uintptr_t)state_dev % sizeof(float)) return "state must be 4-byte aligned";
+            if (!h->auto_reset) return "the recurrent rollout needs auto_reset on (an episode boundary has no next step without it)";
+            return nullptr;
+        };
+        return maze_rollout_policy<POL>("mgb_maze_rollout_rnn", h, T, p, own, seed, resample_cfg, resample_seed,
+                                        act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
+                                        final_obs_dev, truncated_dev, stream);
     };
-    rc = lstm ? launch(std::integral_constant<int, kPolLstm>{}, l, mgb_lstm_smem_bytes(l, k2dThreads))
-              : launch(std::integral_constant<int, kPolGru>{}, g, mgb_gru_smem_bytes(g, k2dThreads));
-    if (rc) return rc;
-    h->t_base += (uint32_t)T;
-    h->launches += 1;
-    return MGB_OK;
+    return pol && pol->cell == MGB_RNN_CELL_LSTM ? run(std::integral_constant<int, kPolLstm>{})
+                                                 : run(std::integral_constant<int, kPolGru>{});
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)

@@ -1,4 +1,5 @@
-// MLP policies evaluated inside a rollout launch (mgb_quad_rollout_policy; DESIGN.md "Policy-driven rollouts").
+// MLP policies evaluated inside a rollout launch (mgb_quad_rollout_policy, mgb_maze_rollout_policy; DESIGN.md
+// "Policy-driven rollouts"), and the recurrent policies of mgb_maze_rollout_rnn below.
 //
 // One thread owns one env.  The CTA stages the packed weights (mgb_policy.params_dev, torch.nn.Linear order) into shared
 // memory once per launch, regrouped so that a hidden layer's outputs are computed eight at a time: for output group g
@@ -7,6 +8,7 @@
 // The output layer (4 wide) is staged in groups of four.  Rows past a layer's width are zero.  Every output is a
 // fused multiply-add chain that starts at the bias and runs over the inputs in index order, in float32.
 #pragma once
+#include <type_traits>
 #include "mgb_common.cuh"
 
 constexpr int kPolicyMaxLayers = MGB_POLICY_MAX_HIDDEN + 1;
@@ -221,23 +223,47 @@ __device__ __forceinline__ float mgb_categorical_action(const MgbMlp &m, int64_t
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// GRU policies (mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies").  The cell's weights are staged in groups of eight
-// hidden units: for group g and input i the 24 weights W[k H + 8g + r][i] (gate k = r, z, n; r < 8) are six consecutive
-// float4, read by the warp as broadcasts, for weight_ih over x and then weight_hh over c.  Group g's biases are 48
-// floats: bias_ih [3][8], then bias_hh [3][8].  Units past H are zero.  The head is an MgbMlp on h, staged behind the cell.
+// Recurrent policies (mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies"): a cell of NG gates, the GRU (NG = 3, gates
+// r, z, n) or the LSTM (NG = 4, gates i, f, g, o), then a head.  The cell's weights are staged in groups of kRnnGroup
+// hidden units: for group g and input i the NG kRnnGroup weights W[k H + kRnnGroup g + r][i] (gate k, r < kRnnGroup)
+// are consecutive float4, read by the warp as broadcasts, for weight_ih over x and then weight_hh over the previous h.
+// Group g's biases are bias_ih [NG][kRnnGroup], then bias_hh [NG][kRnnGroup].  Units past H are zero.  The head is an
+// MgbMlp on h, staged behind the cell.
+//
+// Per env the policy keeps the columns x [in], c [C], h0 [Hr], h1 [Hr], w [Hw] (rows of the CTA's env count floats):
+// the input, the LSTM's cell state (C = H; the GRU has none, C = 0), the previous and the new h, which swap roles every
+// step, and the head's hidden layer.  The GRU has Hr = H and Hw = its head width; the LSTM writes its head's hidden
+// layer into the dead previous-h column instead, so Hr = max(H, head width) and Hw = 0.  The carried state row is
+// [h (H), c (C), feedback (5 feedback)].
 // ---------------------------------------------------------------------------------------------------------------
 
-struct MgbGru {
+constexpr int kRnnGroup = 8;      // hidden units per pass over the inputs
+
+template <int NG>
+struct MgbRnn {
+    static_assert(NG == 3 || NG == 4, "the GRU has three gates, the LSTM four");
     const float *params;          // packed buffer (global memory)
-    int H, Hp, in, feedback, reset;   // Hp: H rounded up to 8
-    int g_hh, g_b;                // global float offsets of weight_hh and bias_ih (weight_ih at 0, bias_hh at g_b + 3H)
+    int H, Hp, in, feedback, reset;   // Hp: H rounded up to kRnnGroup
+    int Hr;                       // rows of each h column
+    int g_hh, g_b;                // global float offsets of weight_hh and bias_ih (weight_ih at 0, bias_hh at g_b + NG H)
     int s_hh, s_b, s_head;        // shared float offsets of the regrouped weight_hh, the biases and the head
     int staged;                   // floats of staged weights, cell and head (a multiple of 8)
-    int head_width;               // rows of the head's activation buffer (0 without a hidden head layer)
     int smem_off;                 // float offset of the policy's region in the kernel's dynamic shared memory
+    int Hw;                       // rows of the w column
     MgbMlp head;                  // the head (in[0] = H); its seed, mode, logp_out and obs0_out serve the whole policy
-    float *state, *state0_out, *hid_out;  // [n][H + 5 feedback], [n][H + 5 feedback] or null, [T][n][H] or null
+    float *state, *state0_out, *hid_out;  // [n][H + C + 5 feedback], the same or null, [T][n][H] or null
+
+    __host__ __device__ int C() const { return NG == 4 ? H : 0; }             // rows of the c column
+    __host__ __device__ int HC() const { return NG == 4 ? 2 * H : H; }        // H + C: floats of h and c in a state row
 };
+
+// The plan of the categorical head: an MLP policy's own, or a recurrent policy's head
+template <class Plan>
+__host__ __device__ __forceinline__ auto &mgb_policy_head(Plan &p)
+{
+    if constexpr (std::is_same_v<std::remove_const_t<Plan>, MgbMlp>) return p;
+    else return p.head;
+}
 
 // Host: the checks every recurrent cell shares.  Returns null, or the reason the policy is refused.
 static inline const char *mgb_rnn_check(const mgb_rnn_policy *p)
@@ -254,197 +280,81 @@ static inline const char *mgb_rnn_check(const mgb_rnn_policy *p)
 }
 
 // Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
-static inline const char *mgb_gru_plan(const mgb_rnn_policy *p, int obs_dim, MgbGru &g)
+template <int NG>
+static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, MgbRnn<NG> &r)
 {
     if (const char *why = mgb_rnn_check(p)) return why;
-    g = MgbGru{};
-    g.params = p->params_dev;
-    g.H = p->hidden;
-    g.Hp = (g.H + 7) / 8 * 8;
-    g.in = obs_dim + 5 * p->feedback;
-    g.feedback = p->feedback;
-    g.reset = p->reset;
-    g.g_hh = 3 * g.H * g.in;
-    g.g_b = g.g_hh + 3 * g.H * g.H;
-    g.s_hh = 3 * g.Hp * g.in;
-    g.s_b = g.s_hh + 3 * g.Hp * g.H;
-    g.s_head = g.s_b + 6 * g.Hp;
-    const mgb_policy hp = {p->params_dev + g.g_b + 6 * g.H, p->head_hidden, {p->head_width, 0, 0}, p->activation, p->mode};
-    if (const char *why = mgb_mlp_plan(&hp, g.H, false, g.head)) return why;
-    g.staged = g.s_head + g.head.staged;
-    g.head_width = p->head_hidden ? p->head_width : 0;
+    r = MgbRnn<NG>{};
+    r.params = p->params_dev;
+    r.H = p->hidden;
+    r.Hp = (r.H + kRnnGroup - 1) / kRnnGroup * kRnnGroup;
+    r.in = obs_dim + 5 * p->feedback;
+    r.feedback = p->feedback;
+    r.reset = p->reset;
+    const int head_width = p->head_hidden ? p->head_width : 0;
+    r.Hr = NG == 4 && head_width > r.H ? head_width : r.H;
+    r.Hw = NG == 4 ? 0 : head_width;
+    r.g_hh = NG * r.H * r.in;
+    r.g_b = r.g_hh + NG * r.H * r.H;
+    r.s_hh = NG * r.Hp * r.in;
+    r.s_b = r.s_hh + NG * r.Hp * r.H;
+    r.s_head = r.s_b + 2 * NG * r.Hp;
+    const mgb_policy hp = {p->params_dev + r.g_b + 2 * NG * r.H, p->head_hidden, {p->head_width, 0, 0}, p->activation,
+                           p->mode};
+    if (const char *why = mgb_mlp_plan(&hp, r.H, false, r.head)) return why;
+    r.staged = r.s_head + r.head.staged;
     return nullptr;
 }
 
-// bytes of dynamic shared memory a CTA of `threads` needs: staged weights + the columns x [in], c [H], h [H], w
-static inline size_t mgb_gru_smem_bytes(const MgbGru &g, int threads)
+// bytes of dynamic shared memory a CTA of `threads` needs: staged weights + the columns x, c, h0, h1 and w
+template <int NG>
+static inline size_t mgb_rnn_smem_bytes(const MgbRnn<NG> &r, int threads)
 {
-    return ((size_t)g.staged + (size_t)(g.in + 2 * g.H + g.head_width) * (size_t)threads) * sizeof(float);
+    return ((size_t)r.staged + (size_t)(r.in + r.C() + 2 * r.Hr + r.Hw) * (size_t)threads) * sizeof(float);
 }
 
-// Device: stage the cell and the head into sm[0, g.staged) (all threads of the CTA; the caller synchronises)
-__device__ __forceinline__ void mgb_gru_stage(const MgbGru &g, float *sm)
+// Device: stage the cell and the head into sm[0, r.staged) (all threads of the CTA; the caller synchronises)
+template <int NG>
+__device__ __forceinline__ void mgb_rnn_stage(const MgbRnn<NG> &r, float *sm)
 {
-    const int H = g.H;
+    constexpr int G = kRnnGroup;
+    const int H = r.H;
     for (int part = 0; part < 2; ++part) {
-        const int K = part ? H : g.in;
-        const float *W = g.params + (part ? g.g_hh : 0);
-        float *dst = sm + (part ? g.s_hh : 0);
-        for (int s = threadIdx.x; s < 3 * g.Hp * K; s += blockDim.x) {
-            const int r = s % 8, k = (s / 8) % 3, i = (s / 24) % K, j = (s / (24 * K)) * 8 + r;
+        const int K = part ? H : r.in;
+        const float *W = r.params + (part ? r.g_hh : 0);
+        float *dst = sm + (part ? r.s_hh : 0);
+        for (int s = threadIdx.x; s < NG * r.Hp * K; s += blockDim.x) {
+            const int u = s % G, k = (s / G) % NG, i = (s / (NG * G)) % K, j = (s / (NG * G * K)) * G + u;
             dst[s] = j < H ? __ldg(W + (k * H + j) * K + i) : 0.f;
         }
     }
-    for (int s = threadIdx.x; s < 6 * g.Hp; s += blockDim.x) {
-        const int r = s % 8, k = (s / 8) % 3, kind = (s / 24) % 2, j = (s / 48) * 8 + r;
-        sm[g.s_b + s] = j < H ? __ldg(g.params + g.g_b + kind * 3 * H + k * H + j) : 0.f;
+    for (int s = threadIdx.x; s < 2 * NG * r.Hp; s += blockDim.x) {
+        const int u = s % G, k = (s / G) % NG, kind = (s / (NG * G)) % 2, j = (s / (2 * NG * G)) * G + u;
+        sm[r.s_b + s] = j < H ? __ldg(r.params + r.g_b + kind * NG * H + k * H + j) : 0.f;
     }
-    mgb_mlp_stage(g.head, sm + g.s_head);
-}
-
-// Device: h = GRU(x, c) for the thread's env (header "Recurrent policies" for the arithmetic).  x, c and h are the
-// column buffers (rows of `stride` floats; the thread's column is `col`); h must not alias x or c.
-__device__ __forceinline__ void mgb_gru_cell(const MgbGru &g, const float *sm, const float *xb, const float *cb, float *hb,
-                                             int stride, int col)
-{
-    const float *x = xb + col, *c = cb + col;
-    float *h = hb + col;
-    const int in = g.in, H = g.H;
-    const float4 *B = reinterpret_cast<const float4 *>(sm + g.s_b);
-    for (int u = 0; u < H; u += 8) {
-        const int grp = u / 8;
-        float gi[24], gh[24];
-#pragma unroll
-        for (int q = 0; q < 6; ++q) {
-            const float4 bi = B[grp * 12 + q], bh = B[grp * 12 + 6 + q];
-            gi[4 * q] = bi.x; gi[4 * q + 1] = bi.y; gi[4 * q + 2] = bi.z; gi[4 * q + 3] = bi.w;
-            gh[4 * q] = bh.x; gh[4 * q + 1] = bh.y; gh[4 * q + 2] = bh.z; gh[4 * q + 3] = bh.w;
-        }
-        const float4 *w = reinterpret_cast<const float4 *>(sm) + grp * in * 6;
-#pragma unroll 2
-        for (int i = 0; i < in; ++i) {
-            const float xi = x[i * stride];
-#pragma unroll
-            for (int q = 0; q < 6; ++q) {
-                const float4 wq = w[6 * i + q];
-                gi[4 * q] = fmaf(wq.x, xi, gi[4 * q]); gi[4 * q + 1] = fmaf(wq.y, xi, gi[4 * q + 1]);
-                gi[4 * q + 2] = fmaf(wq.z, xi, gi[4 * q + 2]); gi[4 * q + 3] = fmaf(wq.w, xi, gi[4 * q + 3]);
-            }
-        }
-        w = reinterpret_cast<const float4 *>(sm + g.s_hh) + grp * H * 6;
-#pragma unroll 2
-        for (int i = 0; i < H; ++i) {
-            const float ci = c[i * stride];
-#pragma unroll
-            for (int q = 0; q < 6; ++q) {
-                const float4 wq = w[6 * i + q];
-                gh[4 * q] = fmaf(wq.x, ci, gh[4 * q]); gh[4 * q + 1] = fmaf(wq.y, ci, gh[4 * q + 1]);
-                gh[4 * q + 2] = fmaf(wq.z, ci, gh[4 * q + 2]); gh[4 * q + 3] = fmaf(wq.w, ci, gh[4 * q + 3]);
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < 8; ++r)
-            if (u + r < H) {
-                const float rg = 1.f / (1.f + expf(-(gi[r] + gh[r])));
-                const float zg = 1.f / (1.f + expf(-(gi[8 + r] + gh[8 + r])));
-                const float ng = tanhf(fmaf(rg, gh[16 + r], gi[16 + r]));
-                h[(u + r) * stride] = fmaf(zg, c[(u + r) * stride], (1.f - zg) * ng);
-            }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// LSTM policies (mgb_maze_rollout_rnn with cell = MGB_RNN_CELL_LSTM).  The GRU's scheme with four gates: for group g of
-// kLstmGroup hidden units and input i the 4 kLstmGroup weights W[k H + kLstmGroup g + r][i] (gate k = i, f, g, o;
-// r < kLstmGroup) are consecutive float4, read by the warp as broadcasts, for weight_ih over x and then weight_hh over
-// the previous h.  Group g's biases are bias_ih [4][kLstmGroup], then bias_hh [4][kLstmGroup].  Units past H are zero.
-// The head is an MgbMlp on h, staged behind the cell.
-// ---------------------------------------------------------------------------------------------------------------
-
-constexpr int kLstmGroup = 8;     // hidden units per pass over the inputs: 8 gate accumulators per unit
-constexpr int kLstmQ = kLstmGroup;  // float4 weights per input of a group: 4 gates x kLstmGroup units / 4
-
-struct MgbLstm {
-    const float *params;          // packed buffer (global memory)
-    int H, Hp, in, feedback, reset;   // Hp: H rounded up to kLstmGroup
-    int Hr;                       // rows of each h column: max(H, head width); the head's hidden layer reuses the dead one
-    int g_hh, g_b;                // global float offsets of weight_hh and bias_ih (weight_ih at 0, bias_hh at g_b + 4H)
-    int s_hh, s_b, s_head;        // shared float offsets of the regrouped weight_hh, the biases and the head
-    int staged;                   // floats of staged weights, cell and head (a multiple of 8)
-    int smem_off;                 // float offset of the policy's region in the kernel's dynamic shared memory
-    MgbMlp head;                  // the head (in[0] = H); its seed, mode, logp_out and obs0_out serve the whole policy
-    float *state, *state0_out, *hid_out;  // [n][2H + 5 feedback], [n][2H + 5 feedback] or null, [T][n][H] or null
-};
-
-// Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
-static inline const char *mgb_lstm_plan(const mgb_rnn_policy *p, int obs_dim, MgbLstm &l)
-{
-    if (const char *why = mgb_rnn_check(p)) return why;
-    l = MgbLstm{};
-    l.params = p->params_dev;
-    l.H = p->hidden;
-    l.Hp = (l.H + kLstmGroup - 1) / kLstmGroup * kLstmGroup;
-    l.in = obs_dim + 5 * p->feedback;
-    l.feedback = p->feedback;
-    l.reset = p->reset;
-    l.Hr = p->head_hidden && p->head_width > l.H ? p->head_width : l.H;
-    l.g_hh = 4 * l.H * l.in;
-    l.g_b = l.g_hh + 4 * l.H * l.H;
-    l.s_hh = 4 * l.Hp * l.in;
-    l.s_b = l.s_hh + 4 * l.Hp * l.H;
-    l.s_head = l.s_b + 8 * l.Hp;
-    const mgb_policy hp = {p->params_dev + l.g_b + 8 * l.H, p->head_hidden, {p->head_width, 0, 0}, p->activation, p->mode};
-    if (const char *why = mgb_mlp_plan(&hp, l.H, false, l.head)) return why;
-    l.staged = l.s_head + l.head.staged;
-    return nullptr;
-}
-
-// bytes of dynamic shared memory a CTA of `threads` needs: staged weights + the columns x [in], c [H] and two h [Hr]
-static inline size_t mgb_lstm_smem_bytes(const MgbLstm &l, int threads)
-{
-    return ((size_t)l.staged + (size_t)(l.in + l.H + 2 * l.Hr) * (size_t)threads) * sizeof(float);
-}
-
-// Device: stage the cell and the head into sm[0, l.staged) (all threads of the CTA; the caller synchronises)
-__device__ __forceinline__ void mgb_lstm_stage(const MgbLstm &l, float *sm)
-{
-    constexpr int G = kLstmGroup;
-    const int H = l.H;
-    for (int part = 0; part < 2; ++part) {
-        const int K = part ? H : l.in;
-        const float *W = l.params + (part ? l.g_hh : 0);
-        float *dst = sm + (part ? l.s_hh : 0);
-        for (int s = threadIdx.x; s < 4 * l.Hp * K; s += blockDim.x) {
-            const int r = s % G, k = (s / G) % 4, i = (s / (4 * G)) % K, j = (s / (4 * G * K)) * G + r;
-            dst[s] = j < H ? __ldg(W + (k * H + j) * K + i) : 0.f;
-        }
-    }
-    for (int s = threadIdx.x; s < 8 * l.Hp; s += blockDim.x) {
-        const int r = s % G, k = (s / G) % 4, kind = (s / (4 * G)) % 2, j = (s / (8 * G)) * G + r;
-        sm[l.s_b + s] = j < H ? __ldg(l.params + l.g_b + kind * 4 * H + k * H + j) : 0.f;
-    }
-    mgb_mlp_stage(l.head, sm + l.s_head);
+    mgb_mlp_stage(r.head, sm + r.s_head);
 }
 
 __device__ __forceinline__ float mgb_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }
 
-// Device: (h, c) = LSTM(x, (hp, c)) for the thread's env (header "Recurrent policies" for the arithmetic).  x, hp, c and
-// h are column buffers (rows of `stride` floats; the thread's column is `col`).  c is updated in place (unit j reads and
-// writes only c[j]); h must not alias x, hp or c.
-__device__ __forceinline__ void mgb_lstm_cell(const MgbLstm &l, const float *sm, const float *xb, const float *hpb,
-                                              float *cb, float *hb, int stride, int col)
+// Device: one step of the cell for the thread's env (header "Recurrent policies" for the arithmetic): h = GRU(x, hp),
+// or (h, c) = LSTM(x, (hp, c)) with c updated in place (unit j reads and writes only c[j]; the GRU ignores c).  x, hp,
+// c and h are column buffers (rows of `stride` floats; the thread's column is `col`); h must not alias x, hp or c.
+template <int NG>
+__device__ __forceinline__ void mgb_rnn_cell(const MgbRnn<NG> &r, const float *sm, const float *xb, const float *hpb,
+                                             float *cb, float *hb, int stride, int col)
 {
-    constexpr int G = kLstmGroup, Q = kLstmQ;
+    constexpr int G = kRnnGroup, Q = NG * G / 4;     // Q: float4 weights per input of a group
     const float *x = xb + col, *hp = hpb + col;
     float *c = cb + col, *h = hb + col;
-    const int in = l.in, H = l.H;
-    const float4 *B = reinterpret_cast<const float4 *>(sm + l.s_b);
+    const int in = r.in, H = r.H;
+    const float4 *B = reinterpret_cast<const float4 *>(sm + r.s_b);
     for (int u = 0; u < H; u += G) {
         const int grp = u / G;
-        float gi[4 * G], gh[4 * G];
+        float gi[NG * G], gh[NG * G];
 #pragma unroll
         for (int q = 0; q < Q; ++q) {
-            const float4 bi = B[grp * 2 * Q + q], bh = B[grp * 2 * Q + Q + q];
+            const float4 bi = B[grp * (2 * Q) + q], bh = B[grp * (2 * Q) + Q + q];
             gi[4 * q] = bi.x; gi[4 * q + 1] = bi.y; gi[4 * q + 2] = bi.z; gi[4 * q + 3] = bi.w;
             gh[4 * q] = bh.x; gh[4 * q + 1] = bh.y; gh[4 * q + 2] = bh.z; gh[4 * q + 3] = bh.w;
         }
@@ -459,7 +369,7 @@ __device__ __forceinline__ void mgb_lstm_cell(const MgbLstm &l, const float *sm,
                 gi[4 * q + 2] = fmaf(wq.z, xi, gi[4 * q + 2]); gi[4 * q + 3] = fmaf(wq.w, xi, gi[4 * q + 3]);
             }
         }
-        w = reinterpret_cast<const float4 *>(sm + l.s_hh) + grp * H * Q;
+        w = reinterpret_cast<const float4 *>(sm + r.s_hh) + grp * H * Q;
 #pragma unroll 2
         for (int i = 0; i < H; ++i) {
             const float hi = hp[i * stride];
@@ -471,15 +381,22 @@ __device__ __forceinline__ void mgb_lstm_cell(const MgbLstm &l, const float *sm,
             }
         }
 #pragma unroll
-        for (int r = 0; r < G; ++r)
-            if (u + r < H) {
-                const float ig = mgb_sigmoid(gi[r] + gh[r]);
-                const float fg = mgb_sigmoid(gi[G + r] + gh[G + r]);
-                const float gg = tanhf(gi[2 * G + r] + gh[2 * G + r]);
-                const float og = mgb_sigmoid(gi[3 * G + r] + gh[3 * G + r]);
-                const float cn = fmaf(fg, c[(u + r) * stride], ig * gg);
-                c[(u + r) * stride] = cn;
-                h[(u + r) * stride] = og * tanhf(cn);
+        for (int v = 0; v < G; ++v)
+            if (u + v < H) {
+                if constexpr (NG == 3) {
+                    const float rg = mgb_sigmoid(gi[v] + gh[v]);
+                    const float zg = mgb_sigmoid(gi[G + v] + gh[G + v]);
+                    const float ng = tanhf(fmaf(rg, gh[2 * G + v], gi[2 * G + v]));
+                    h[(u + v) * stride] = fmaf(zg, hp[(u + v) * stride], (1.f - zg) * ng);
+                } else {
+                    const float ig = mgb_sigmoid(gi[v] + gh[v]);
+                    const float fg = mgb_sigmoid(gi[G + v] + gh[G + v]);
+                    const float gg = tanhf(gi[2 * G + v] + gh[2 * G + v]);
+                    const float og = mgb_sigmoid(gi[3 * G + v] + gh[3 * G + v]);
+                    const float cn = fmaf(fg, c[(u + v) * stride], ig * gg);
+                    c[(u + v) * stride] = cn;
+                    h[(u + v) * stride] = og * tanhf(cn);
+                }
             }
     }
 }

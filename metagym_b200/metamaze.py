@@ -712,48 +712,10 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
-            if recurrent:
-                return self._rollout_rnn(T, policy, state, act_seed, deterministic, out, resample, want_hidden)
-            return self._rollout_policy(T, policy, act_seed, deterministic, out, resample)
+            return self._rollout_policy(T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden)
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
 
-    def _rollout_rnn(self, T, policy, state, act_seed, deterministic, out, resample, want_hidden):
-        if self.need_reset:
-            raise Exception("Must \"reset\" before doing any actions")
-        torch = self._torch
-        T, N, dev = int(T), self.num_envs, self.device
-        shape = tuple(self._obs.shape[1:])
-        if policy.obs_dim != int(np.prod(shape)):
-            raise ValueError("the policy takes %d observation inputs, the env observes %d"
-                             % (policy.obs_dim, int(np.prod(shape))))
-        if policy.params.device != dev:
-            raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
-        if not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
-                and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
-            raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
-        if out is None:
-            out = {"obs": torch.empty((T, N) + shape, dtype=torch.float32, device=dev),
-                   "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
-                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev),
-                   "act": torch.empty((T, N), dtype=torch.int32, device=dev),
-                   "logp": None if deterministic else torch.empty((T, N), dtype=torch.float32, device=dev),
-                   "obs0": torch.empty((N,) + shape, dtype=torch.float32, device=dev),
-                   "state0": torch.empty((N, policy.state_dim), dtype=torch.float32, device=dev)}
-            if want_hidden:
-                out["hid"] = torch.empty((T, N, policy.hidden), dtype=torch.float32, device=dev)
-            if self._want_final:
-                out["final_obs"] = torch.empty((T, N) + shape, dtype=torch.float32, device=dev)
-                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
-        out["resampled"] = resample is not None
-        cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
-        pol = policy.struct(deterministic)
-        keys = ("state0", "hid", "act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
-        _lib.check(self._lib.mgb_maze_rollout_rnn(self._h, T, ctypes.byref(pol), int(act_seed),
-                                                  None if cfg is None else ctypes.byref(cfg), seed, _lib.ptr(state),
-                                                  *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
-        return out
-
-    def _rollout_policy(self, T, policy, act_seed, deterministic, out, resample):
+    def _rollout_policy(self, T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden):
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -761,9 +723,12 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         shape = tuple(self._obs.shape[1:])
         D = int(np.prod(shape))
         if policy.obs_dim != D:
-            raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
+            raise ValueError("the policy takes %d observation inputs, the env observes %d" % (policy.obs_dim, D))
         if policy.params.device != dev:
             raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
+        if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
+                              and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
+            raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
         if out is None:
             out = {"obs": torch.empty((T, N) + shape, dtype=torch.float32, device=dev),
                    "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
@@ -771,15 +736,23 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
                    "act": torch.empty((T, N), dtype=torch.int32, device=dev),
                    "logp": None if deterministic else torch.empty((T, N), dtype=torch.float32, device=dev),
                    "obs0": torch.empty((N,) + shape, dtype=torch.float32, device=dev)}
+            if recurrent:
+                out["state0"] = torch.empty((N, policy.state_dim), dtype=torch.float32, device=dev)
+            if recurrent and want_hidden:
+                out["hid"] = torch.empty((T, N, policy.hidden), dtype=torch.float32, device=dev)
             if self._want_final:
                 out["final_obs"] = torch.empty((T, N) + shape, dtype=torch.float32, device=dev)
                 out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+        if recurrent:
+            out["resampled"] = resample is not None
         cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
         pol = policy.struct(deterministic)
+        args = [self._h, T, ctypes.byref(pol), int(act_seed), None if cfg is None else ctypes.byref(cfg), seed]
+        if recurrent:
+            args += [_lib.ptr(state), _lib.ptr(out.get("state0")), _lib.ptr(out.get("hid"))]
         keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
-        _lib.check(self._lib.mgb_maze_rollout_policy(self._h, T, ctypes.byref(pol), int(act_seed),
-                                                     None if cfg is None else ctypes.byref(cfg), seed,
-                                                     *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
+        entry = self._lib.mgb_maze_rollout_rnn if recurrent else self._lib.mgb_maze_rollout_policy
+        _lib.check(entry(*args, *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
         return out
 
     def save_trajectory(self, file_name, envs=None, additional=None):
