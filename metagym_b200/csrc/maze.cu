@@ -4999,7 +4999,8 @@ static int64_t record_bytes(const mgb_maze *h)
     return record_path_off(h) + (h->path ? (path_cap(h) * 2 + 15) / 16 * 16 : 0);
 }
 
-// snapshot (LOAD false) or restore the path entries of the records
+// snapshot (LOAD false) or restore the path entries of the records.  A snapshot also zeroes the padding behind each
+// record's entries, so that the same state always gives the same record bytes.
 static int record_paths(mgb_maze *h, bool load, const uint8_t *rec_dev, int64_t n_rec, const int64_t *row, cudaStream_t st)
 {
     if (!h->path) return MGB_OK;
@@ -5014,6 +5015,10 @@ static int record_paths(mgb_maze *h, bool load, const uint8_t *rec_dev, int64_t 
                                                                       record_bytes(h), record_path_off(h), 0, nullptr);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
+    const int64_t used = path_cap(h) * 2, pad = (used + 15) / 16 * 16 - used;
+    if (!load && pad)
+        MGB_CUDA(cudaMemset2DAsync(rec + record_path_off(h) + used, (size_t)record_bytes(h), 0, (size_t)pad,
+                                   (size_t)h->n, st));
     return MGB_OK;
 }
 
