@@ -384,6 +384,25 @@ int mgb_maze_step(mgb_maze *h, const void *act_dev, void *obs_dev, double *rew_d
                   void *final_obs_dev, uint8_t *truncated_dev, void *stream);
 int mgb_maze_set_options(mgb_maze *h, int auto_reset);
 
+/* Trials of k episodes per maze (RL^2: the agent's memory is carried across the episodes of one maze).  k >= 1 makes
+ * the handle a TRIAL handle; k = 0 (the default) leaves it as it is.  Must be called before the first mgb_maze_set_task,
+ * which fixes the record layout; refused (MGB_ERR_ARG) afterwards and for k < 0.  Synchronous.
+ * A trial handle keeps task_episodes[e]: the episodes env e has finished (done = 1) since it was last given a maze.
+ *   Every done adds 1: mgb_maze_step, mgb_maze_rollout, mgb_maze_rollout_policy and mgb_maze_rollout_rnn.
+ *   It goes to 0 where the env gets a maze: mgb_maze_set_task (all envs), mgb_maze_update_tasks (envs of the replaced
+ *   slots), mgb_maze_resample_tasks (masked envs) and an in-launch draw.  mgb_maze_reset does not change it.
+ *   With resample_cfg, an env that finishes at step t draws a new maze only when its count after step t reaches k (and
+ *   the count returns to 0); otherwise it auto-resets on its old maze exactly as without resample_cfg, and its resample
+ *   count is unchanged.  The rollout then equals, step for step, step + resample_tasks(m) + reset(mask = m) with
+ *   m = done && task_episodes >= k.  The recurrent "task" reset rule zeroes the state where the env drew.
+ *   Without resample_cfg a step or rollout takes the counts from done_dev, which may then not be NULL (MGB_ERR_ARG,
+ *   handle untouched); one more small kernel follows the launch.  k = 1 gives exactly the outputs of a handle without
+ *   trials.  Snapshot records gain one 16-byte block (mgb_maze_snapshot below).
+ *   mgb_maze_task_episodes: the counts as int32 [n] into out_dev; stream-ordered, capturable in a CUDA graph.  Refused on
+ *   a handle that is not a trial handle. */
+int mgb_maze_set_episodes_per_task(mgb_maze *h, int32_t k);
+int mgb_maze_task_episodes(mgb_maze *h, int32_t *out_dev, void *stream);
+
 /* T consecutive mgb_maze_step calls (the random-action loops of metamaze/test.py:9-67) in ONE launch; auto-reset
  * semantics as configured, state left as T steps leave it.  The handle picks the engine:
  *   MetaMaze2D: agent state in registers.
@@ -566,8 +585,11 @@ int mgb_maze_path(mgb_maze *h, int32_t count, const int32_t *envs_dev, int8_t *c
  * slot.  Restore then writes that task into the destination env's own slot; otherwise the table is shared, the fingerprint
  * covers it, and restore points env2task[e] at the record's slot.  mgb_maze_restore is synchronous the first time it
  * finds the pose cache to be built (like the first reset); after that it is stream-ordered.  A recording handle
- * (mgb_maze_set_path) appends the env's path entries to its records (2 (max_steps + 1) bytes, padded to 16).
- *   mgb_maze_fingerprint: out[0] config (mgb_maze_cfg, auto_reset, table shape, path recording, record layout), out[1] textures,
+ * (mgb_maze_set_path) appends the env's path entries to its records (2 (max_steps + 1) bytes, padded to 16).  A trial
+ * handle (mgb_maze_set_episodes_per_task) has one more 16-byte block after the food stamps: its episode count (u32) and
+ * zero padding; the task and the path entries follow it.
+ *   mgb_maze_fingerprint: out[0] config (mgb_maze_cfg, auto_reset, table shape, path recording, episodes per task,
+ *     record layout), out[1] textures,
  *     out[2] the shared task table (0 when records carry their tasks), out[3] 1 when records carry their tasks. */
 int64_t mgb_maze_record_bytes(const mgb_maze *h);
 int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream);

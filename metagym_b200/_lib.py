@@ -101,6 +101,8 @@ SIGNATURES = {
     "mgb_maze_reset": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_step": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_set_options": (ctypes.c_int, [vp, ctypes.c_int]),
+    "mgb_maze_set_episodes_per_task": (ctypes.c_int, [vp, c_i32]),
+    "mgb_maze_task_episodes": (ctypes.c_int, [vp, vp, vp]),
     "mgb_peer_alloc": (ctypes.c_int, [ctypes.c_int, c_u64, ctypes.POINTER(ctypes.c_void_p)]),
     "mgb_peer_free": (ctypes.c_int, [ctypes.c_int, vp]),
     "mgb_peer_export": (ctypes.c_int, [ctypes.c_int, vp, vp]),

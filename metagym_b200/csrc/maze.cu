@@ -158,12 +158,26 @@ struct MazeArgs {
 
 // in-launch task resampling (maze3d_kernel<.., RS> and maze2d_rollout_kernel<0, .., RS>, mgb_maze_rollout with a
 // sampler cfg): an env whose episode ends gets the task mgb_maze_resample_tasks would draw for it.  A
-// parameter of those kernels after MazeArgs, so that no other parameter offsets move.
+// parameter of those kernels after MazeArgs, so that no other parameter offsets move.  Trial handles
+// (mgb_maze_set_episodes_per_task) also pass `count`: an env then draws only when it finishes its k-th episode on its
+// maze (rs_draws); with count null every finished env draws.
 struct MazeResample {
     SamplerCfg cfg;
     uint64_t seed;
     uint32_t *epoch;             // [n] resample count of every env
+    uint32_t *count;             // [n] episodes each env has finished on its current maze, or null
+    int32_t k;                   // episodes per maze (count set)
 };
+
+// A finished env's trial bookkeeping: its count goes up by one, and it draws a new maze (count back to 0) at the k-th
+__device__ __forceinline__ bool rs_draws(const MazeResample &rs, uint32_t &cnt)
+{
+    if (!rs.count) return true;
+    cnt += 1;
+    const bool draw = cnt >= (uint32_t)rs.k;
+    if (draw) cnt = 0;
+    return draw;
+}
 
 __device__ __noinline__ void maze_sample_task(const MazeConst &c, const SamplerCfg &sc, uint64_t seed, int64_t genv,
                                               uint32_t *epoch, uint8_t *ws, uint8_t *b);
@@ -534,6 +548,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     const TaskHdr *th = nullptr;
     const int8_t *walls = nullptr;
     Env s = {0, 0, 0, 0, 0.0};
+    uint32_t tcount = 0;                                // RS on a trial handle: episodes finished on the current maze
     int32_t *eaten = a.eaten + e;
     if (active) {
         blob = a.blobs + (int64_t)a.env2task[e] * c.blob_bytes;
@@ -541,6 +556,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
         walls = reinterpret_cast<const int8_t *>(blob + c.off_walls);
         const int4 ag = a.agent[e];
         s.gx = ag.x; s.gy = ag.y; s.ori = ag.z; s.steps = ag.w; s.life = a.life[e];
+        if (RS && rs.count) tcount = rs.count[e];
     }
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
@@ -589,7 +605,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
             if (threadIdx.x == 0) mgb_bulk_wait_read<1>();  // the store issued two steps ago has read this tile
             __syncthreads();
         }
-        uint32_t done_byte = 0;
+        uint32_t done_byte = 0, draw = 0;                  // draw (RS): the env finished and draws a new maze
         if (active) {
             int action;
             if constexpr (POL) {
@@ -628,6 +644,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                     maze2d_window(c, blob, eaten, a.n_pad, s, reinterpret_cast<float *>(a.final_obs) + ((int64_t)t * a.n + e) * D);
             }
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
+            if (RS && done) draw = (uint32_t)rs_draws(rs, tcount);
             if (REC) path_store(c, a, e, s);
             if (a.rew) {
                 if (XM == 2) mgb_mc_st(mgb_shift(a.rew + (int64_t)t * a.n + e, a.mir.delta[0]), reward);
@@ -657,8 +674,8 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                 if (c.task_type == MGB_MAZE_SURVIVAL) row[g * W + g] = (float)s.life;
             }
             if constexpr (RNN) {
-                // carry: with RS every finished env draws a new maze, so the task rule fires exactly where done does
-                const bool wipe = done && (RS || pol.reset == MGB_RNN_RESET_EPISODE);
+                // carry: the task rule fires where the env draws a new maze, which only RS does
+                const bool wipe = done && (pol.reset == MGB_RNN_RESET_EPISODE || draw);
                 if (wipe) {
                     for (int k = 0; k < pol.H; ++k) hid_new[k * k2dThreads + threadIdx.x] = 0.f;
                     for (int k = 0; k < pol.C(); ++k) cst[k * k2dThreads + threadIdx.x] = 0.f;
@@ -676,8 +693,9 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
         if constexpr (RS) {
             // auto-reset is on (the host requires it).  The step above left every finished env reset on its old task, with
             // that task's window in the tile and its path entry 0 stored; that step code stays as the other instantiations
-            // compile it, and the few finished envs redo the three on the new task here.
-            uint32_t fin = __ballot_sync(0xffffffffu, done_byte != 0);
+            // compile it, and the few envs that draw redo the three on the new task here.  A finished env of a trial
+            // handle that does not draw keeps what the step left: its next episode on the old maze.
+            uint32_t fin = __ballot_sync(0xffffffffu, draw != 0);
             if (fin) {
                 uint8_t *ws = reinterpret_cast<uint8_t *>(tile2d + 2 * k2dThreads * D) +
                               (threadIdx.x >> 5) * sampler_ws_bytes(c.n);
@@ -688,7 +706,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                                      const_cast<uint8_t *>(a.blobs) + (int64_t)a.env2task[el] * c.blob_bytes);
                 }
                 __syncwarp();   // the new blobs, written by every lane, are read by their owners below
-                if (done_byte) {
+                if (draw) {
                     env_reset(c, blob, eaten, a.n_pad, s);
                     if (REC) path_store(c, a, e, s);
                     if (a.obs || POL) maze2d_window(c, blob, eaten, a.n_pad, s, tile + threadIdx.x * D);
@@ -749,6 +767,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     if (active) {
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
+        if (RS && rs.count) rs.count[e] = tcount;
     }
     if constexpr (RNN) {
         if (active) {
@@ -1048,7 +1067,11 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                     split = FIN && done && a.final_obs && a.auto_reset;
                 }
                 if (done && a.auto_reset && !split) {
-                    rs_env = RS;
+                    if (RS) {       // the episode ends here (with FIN, at its reset item): count it, and draw at the k-th
+                        uint32_t cnt = rs.count ? rs.count[e] : 0u;
+                        rs_env = rs_draws(rs, cnt);
+                        if (rs.count) rs.count[e] = cnt;
+                    }
                     env_reset(c, s_blob, eaten, a.n_pad, s);
                     if (cont) {
                         cp[0] = (float)(s.gx * th->cell_size + 0.5 * th->cell_size);
@@ -2620,6 +2643,8 @@ struct mgb_maze {
     int64_t n_poses = 0;
     MazePoseCache cache;
     MgbDev<uint32_t> task_epoch;              // [n_pad] how often each env's task has been resampled on the device
+    int32_t trial_k = 0;                      // mgb_maze_set_episodes_per_task: episodes per maze (0: not a trial handle)
+    MgbDev<uint32_t> task_count;              // trial handle: [n_pad] episodes each env has finished on its current maze
     bool slot_per_env = false;                // env2task is injective: every env owns its task-table slot
     MgbDev<uint8_t> task_flags;               // [n_tasks] scratch of mgb_maze_update_tasks
     bool cache_would_fit = true;              // last ensure_pose_cache decision (false: over budget -> direct renderer)
@@ -2817,6 +2842,32 @@ extern "C" int64_t mgb_maze_obs_bytes_per_env(const mgb_maze *h)
 }
 
 extern "C" int64_t mgb_maze_launch_count(const mgb_maze *h) { return h ? h->launches : MGB_ERR_ARG; }
+
+extern "C" int mgb_maze_set_episodes_per_task(mgb_maze *h, int32_t k)
+{
+    MGB_REQUIRE(h, "null handle");
+    MGB_REQUIRE(k >= 0, "episodes_per_task must be >= 0 (0: off)");
+    MGB_REQUIRE(!h->task_epoch, "call mgb_maze_set_episodes_per_task before mgb_maze_set_task (it fixes the record layout)");
+    MgbDeviceGuard guard(h->device);
+    MgbDev<uint32_t> count;
+    if (k > 0) {
+        MGB_CUDA(count.alloc(sizeof(uint32_t) * (size_t)h->n_pad));
+        MGB_CUDA(cudaMemset(count.get(), 0, sizeof(uint32_t) * (size_t)h->n_pad));
+    }
+    h->task_count = std::move(count);
+    h->trial_k = k;
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_task_episodes(mgb_maze *h, int32_t *out_dev, void *stream)
+{
+    MGB_REQUIRE(h && out_dev, "null argument");
+    MGB_REQUIRE(h->trial_k > 0, "not a trial handle (mgb_maze_set_episodes_per_task)");
+    MgbDeviceGuard guard(h->device);
+    MGB_CUDA(cudaMemcpyAsync(out_dev, h->task_count.get(), sizeof(uint32_t) * (size_t)h->n, cudaMemcpyDeviceToDevice,
+                             (cudaStream_t)stream));
+    return MGB_OK;
+}
 
 extern "C" int mgb_maze_set_options(mgb_maze *h, int auto_reset)
 {
@@ -3159,6 +3210,7 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     }
     // set_task leaves the env in "need reset" state (maze_env.py:44-50): initialise it so a stray step is harmless
     MazeArgs a = maze_args(h);
+    if (h->trial_k) MGB_CUDA(cudaMemset(h->task_count.get(), 0, sizeof(uint32_t) * (size_t)h->n_pad));   // every env has a new maze
     maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256>>>(h->c, a, nullptr);
     MGB_CUDA(cudaDeviceSynchronize());
     h->launches += 1;
@@ -3345,7 +3397,8 @@ __device__ __noinline__ void maze_sample_task(const MazeConst &c, const SamplerC
 __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(const __grid_constant__ MazeConst c,
                                                                               const __grid_constant__ MazeArgs a,
                                                                               uint8_t *blobs, const uint8_t *mask, uint32_t *epoch,
-                                                                              const __grid_constant__ SamplerCfg sc, uint64_t seed)
+                                                                              const __grid_constant__ SamplerCfg sc, uint64_t seed,
+                                                                              uint32_t *count)
 {
     __shared__ __align__(16) uint8_t s_ws[kSamplerWarps][kSamplerWsMax];
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -3355,6 +3408,7 @@ __global__ void __launch_bounds__(32 * kSamplerWarps) maze_sample_tasks_kernel(c
     uint8_t *b = blobs + (size_t)a.env2task[e] * c.blob_bytes;
     maze_sample_task(c, sc, seed, a.env_base + e, epoch + e, s_ws[w], b);
     if (lane != 0) return;
+    if (count) count[e] = 0;                                       // trial handle: no episode finished on the new maze yet
     // ---- the env starts an episode on its new task (set_task + reset of that env, maze_env.py:44-57)
     Env s;
     env_reset(c, b, a.eaten + e, a.n_pad, s);
@@ -3396,6 +3450,24 @@ __global__ void maze_clear_flags_kernel(uint8_t *task_flags, int n)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) task_flags[i] = 0;
+}
+
+// Trial handles: the envs whose table slot mgb_maze_update_tasks just replaced have finished no episode on their new maze
+__global__ void maze_zero_counts_kernel(int64_t n, const int32_t *env2task, const uint8_t *task_flags, uint32_t *count)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n && task_flags[env2task[e]]) count[e] = 0;
+}
+
+// Trial handles, after a step (T = 1) or a rollout without resampling: every done of done [T][n] is one more episode
+// finished on the env's maze.  The kernels that write done stay as every other handle runs them.
+__global__ void maze_count_done_kernel(int64_t n, int T, const uint8_t *__restrict__ done, uint32_t *count)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    uint32_t k = 0;
+    for (int t = 0; t < T; ++t) k += done[(int64_t)t * n + e] != 0;
+    if (k) count[e] += k;
 }
 
 // Lay the host pose lists out at the larger stride S (a handle on the direct renderer took a task with more free cells
@@ -3527,6 +3599,11 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     }
     MazeArgs a = maze_args(h);
     maze_reset_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(c, a, h->task_flags.get());
+    if (h->trial_k) {
+        maze_zero_counts_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->n, h->env2task.get(), h->task_flags.get(),
+                                                                               h->task_count.get());
+        h->launches += 1;
+    }
     maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags.get(), h->n_tasks);
     MGB_CUDA(cudaGetLastError());
     h->launches += 2;
@@ -3590,7 +3667,7 @@ extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, con
     const MazeConst &c = h->c;
     MazeArgs a = maze_args(h);
     maze_sample_tasks_kernel<<<(unsigned)((h->n + kSamplerWarps - 1) / kSamplerWarps), 32 * kSamplerWarps, 0, (cudaStream_t)stream>>>(c, a, h->tasks.blobs.get(), mask_dev, h->task_epoch.get(),
-                                                                                        sc, seed);
+                                                                                        sc, seed, h->task_count.get());
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     return MGB_OK;
@@ -4043,6 +4120,22 @@ static int step_ex(mgb_maze *h, MazeArgs &a, void *final_obs, uint8_t *truncated
     return MGB_OK;
 }
 
+// A trial handle's counts after a launch that wrote done [T][n] without resampling (maze_count_done_kernel)
+static int count_done(mgb_maze *h, const uint8_t *done_dev, int32_t T, cudaStream_t st)
+{
+    if (!h->trial_k) return MGB_OK;
+    maze_count_done_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->n, T, done_dev, h->task_count.get());
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
+// What a trial handle needs of a step or rollout without resampling: the refusal, or nullptr
+static const char *trial_needs_done(const mgb_maze *h, const void *done_dev)
+{
+    return h->trial_k && !done_dev ? "a trial handle counts episodes from done: done_dev may not be null without resampling"
+                                   : nullptr;
+}
 
 extern "C" int mgb_maze_reset(mgb_maze *h, const uint8_t *mask_dev, void *obs_dev, void *stream)
 {
@@ -4146,7 +4239,7 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
     int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
         if (h->c.kind != MGB_MAZE_2D && h->mir.count != 0)
             return "output mirrors are not implemented for the 3-D rollouts (set_mirrors([]) first)";
-        if (!resample_cfg) return nullptr;
+        if (!resample_cfg) return trial_needs_done(h, done_dev);
         if (!h->auto_reset) return "resampling finished envs needs auto_reset on";
         if (h->mir.count != 0)
             return "output mirrors and multicast are not implemented for the resampling rollout (set_mirrors([]) first)";
@@ -4170,7 +4263,10 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
     a.final_obs = final_obs_dev; a.truncated = truncated_dev;
     const bool fin = final_obs_dev || truncated_dev;
     MazeResample r = {};
-    if (resample_cfg) { r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get(); }
+    if (resample_cfg) {
+        r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
+        r.count = h->task_count.get(); r.k = h->trial_k;
+    }
     if (eng == RolloutEngine::pose_cache) {
         const int64_t resident = (int64_t)h->num_sms * 5;          // __launch_bounds__(256, 5): 48 registers
         const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
@@ -4227,7 +4323,7 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
-    return MGB_OK;
+    return resample_cfg ? MGB_OK : count_done(h, done_dev, T, st);
 }
 
 // maze2d_rollout_kernel<0, fin, REC, RS, POL>, sm bytes of dynamic shared memory; refused (as `fn`) when the CTA would
@@ -4276,7 +4372,7 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
         if (logp_out_dev && head.mode != MGB_POLICY_SAMPLE) return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
-        if (!resample_cfg) return nullptr;
+        if (!resample_cfg) return trial_needs_done(h, done_dev);
         if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout
         return sampler_cfg(h, resample_cfg, sc);
     });
@@ -4297,6 +4393,7 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
     MazeResample r = {};
     if (resample_cfg) {
         r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
+        r.count = h->task_count.get(); r.k = h->trial_k;
     }
     const bool fin = final_obs_dev || truncated_dev;
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
@@ -4310,7 +4407,7 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
-    return MGB_OK;
+    return resample_cfg ? MGB_OK : count_done(h, done_dev, T, st);
 }
 
 extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
@@ -4858,7 +4955,8 @@ extern "C" int mgb_maze_step(mgb_maze *h, const void *act_dev, void *obs_dev, do
     if (h->c.kind == MGB_MAZE_CONTINUOUS_3D) a.act_c = static_cast<const float *>(act_dev);
     else a.act = static_cast<const int32_t *>(act_dev);
     a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
-    return step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
+    rc = step_ex(h, a, final_obs_dev, truncated_dev, (cudaStream_t)stream);
+    return rc ? rc : count_done(h, done_dev, 1, (cudaStream_t)stream);
 }
 
 extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev, void *stream)
@@ -4878,6 +4976,7 @@ extern "C" int mgb_maze_state(mgb_maze *h, int32_t *agent_dev, double *life_dev,
 //   [16, 32)  life f64 | resample count u32 | task-table slot i32
 //   [32, 48)  continuous position f32 x 2 | heading f64 (zero for the other kinds)
 //   [48, ..)  food stamps int32 [f_max], in groups of four (16 bytes each, unused tail zero)
+//   [.., +16) trial handles only: the env's episode count u32 | zero padding
 //   [tail, ..) the task of the env's slot, blob_bytes, when records carry their tasks
 //   [.., ..)  path recording on: the path entries char2 [max_steps + 1], padded to 16 bytes
 // ---------------------------------------------------------------------------------------------------------------
@@ -4886,7 +4985,7 @@ namespace {
 constexpr int64_t kMazeRecHead = 48;
 
 __global__ void maze_snapshot_kernel(int f_max, const __grid_constant__ MazeArgs a, const uint32_t *__restrict__ epoch,
-                                     uint8_t *__restrict__ rec, int64_t rec_bytes)
+                                     const uint32_t *__restrict__ count, uint8_t *__restrict__ rec, int64_t rec_bytes)
 {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= a.n) return;
@@ -4905,11 +5004,12 @@ __global__ void maze_snapshot_kernel(int f_max, const __grid_constant__ MazeArgs
         for (int j = 0; j < 4; ++j) v[j] = f + j < f_max ? (uint32_t)a.eaten[(int64_t)(f + j) * a.n_pad + e] : 0u;
         r[3 + f / 4] = make_uint4(v[0], v[1], v[2], v[3]);
     }
+    if (count) r[3 + (f_max + 3) / 4] = make_uint4(count[e], 0u, 0u, 0u);
 }
 
 // env2task_w: null when records carry their tasks (the env keeps its own slot)
 __global__ void maze_restore_kernel(int f_max, const __grid_constant__ MazeArgs a, uint32_t *__restrict__ epoch,
-                                    int32_t *__restrict__ env2task_w, int n_tasks, const uint8_t *__restrict__ rec,
+                                    uint32_t *__restrict__ count, int32_t *__restrict__ env2task_w, int n_tasks, const uint8_t *__restrict__ rec,
                                     int64_t rec_bytes, int64_t n_rec, const int64_t *__restrict__ row)
 {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -4933,6 +5033,7 @@ __global__ void maze_restore_kernel(int f_max, const __grid_constant__ MazeArgs 
         for (int j = 0; j < 4; ++j)
             if (f + j < f_max) a.eaten[(int64_t)(f + j) * a.n_pad + e] = (int32_t)v[j];
     }
+    if (count) count[e] = s[3 + (f_max + 3) / 4].x;
 }
 
 // The task of every env's own slot <-> the tail of its record: one uint4 per thread over all (env, uint4) pairs, so that
@@ -4986,7 +5087,10 @@ static bool records_carry_tasks(const mgb_maze *h)
     return h->slot_per_env && !cached;
 }
 
-static int64_t record_tail(const mgb_maze *h) { return kMazeRecHead + (int64_t)(h->c.f_max + 3) / 4 * 16; }
+static int64_t record_tail(const mgb_maze *h)
+{
+    return kMazeRecHead + (int64_t)(h->c.f_max + 3) / 4 * 16 + (h->trial_k ? 16 : 0);
+}
 
 // where the path entries start in a record (recording on)
 static int64_t record_path_off(const mgb_maze *h)
@@ -5039,7 +5143,8 @@ extern "C" int mgb_maze_snapshot(mgb_maze *h, uint8_t *rec_dev, void *stream)
     cudaStream_t st = (cudaStream_t)stream;
     const MazeArgs a = maze_args(h);
     const int64_t rb = record_bytes(h);
-    maze_snapshot_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch.get(), rec_dev, rb);
+    maze_snapshot_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch.get(),
+                                                                         h->task_count.get(), rec_dev, rb);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
     if (records_carry_tasks(h)) {
@@ -5071,7 +5176,7 @@ extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_r
     const int64_t rb = record_bytes(h);
     const MazeArgs a = maze_args(h);
     maze_restore_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, st>>>(h->c.f_max, a, h->task_epoch.get(),
-                                                                        carry ? nullptr : h->env2task.get(), h->n_tasks, rec_dev,
+                                                                        h->task_count.get(), carry ? nullptr : h->env2task.get(), h->n_tasks, rec_dev,
                                                                         rb, n_rec, row_of_env_dev);
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
@@ -5113,6 +5218,10 @@ extern "C" int mgb_maze_fingerprint(const mgb_maze *h, uint64_t *out)
         const int64_t cap = path_cap(h);
         f = mgb_fnv(f, "path", 4);
         f = mgb_fnv(f, &cap, sizeof(cap));
+    }
+    if (h->trial_k) {                           // episodes per maze (a handle without trials hashes as before)
+        f = mgb_fnv(f, "trial", 5);
+        f = mgb_fnv(f, &h->trial_k, sizeof(h->trial_k));
     }
     out[0] = mgb_fnv(f, &rb, sizeof(rb));
     out[1] = h->fp_tex;

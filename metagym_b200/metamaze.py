@@ -196,14 +196,36 @@ def MazeTaskSampler(n=15, allow_loops=True, cell_size=2.0, wall_height=3.2, agen
                       food_interval=interval)
 
 
+def new_tasks(out):
+    """[T, N] bool CUDA tensor: True where env e drew a new maze at step t of the rollout that returned `out` (the
+    "task" reset rule of the recurrent policies fires exactly there).  False everywhere when the rollout did not
+    resample; `done` for a resampling rollout of a handle without trials; on a trial handle (episodes_per_task=k) the
+    finished episodes that were the k-th on their maze, counted from out["task_episodes0"].  `out` is the dict of a
+    recurrent rollout or of any rollout of a trial handle (both record whether the launch resampled)."""
+    import torch
+    done = out["done"].bool()
+    if not out.get("resampled", False):
+        return torch.zeros_like(done)
+    k = out.get("episodes_per_task")
+    if k is None:
+        return done
+    count = out["task_episodes0"].to(done.device, torch.int64)
+    drew = torch.empty_like(done)
+    for t in range(done.shape[0]):
+        count = count + done[t]
+        drew[t] = done[t] & (count >= k)
+        count = count.masked_fill(drew[t], 0)
+    return drew
+
+
 class _BatchedMazeBase(Snapshots):
     """snapshot() / restore() / clone_envs() (metagym_b200/snapshot.py): exact checkpoint and resume of agent, life, food,
-    resample counts, continuous pose, task slot (and, for one table slot per env on the direct renderer, the task itself)
-    and the rollout action counter.  A restore clears need_reset."""
+    resample counts, trial episode counts, continuous pose, task slot (and, for one table slot per env on the direct
+    renderer, the task itself) and the rollout action counter.  A restore clears need_reset."""
     KIND = None
     _SNAP_PREFIX = "mgb_maze"
     _FINGERPRINT_PARTS = ("configuration (kind, task type, max_steps, view, resolution, obs dtype, optics, auto_reset, "
-                          "table shape, path recording)", "textures", "task table", "record mode (per-env tasks or a shared table)")
+                          "table shape, path recording, episodes_per_task)", "textures", "task table", "record mode (per-env tasks or a shared table)")
 
     def _snap_kind(self):
         return ("maze2d", "maze_discrete_3d", "maze_continuous_3d")[self.KIND]
@@ -217,11 +239,14 @@ class _BatchedMazeBase(Snapshots):
                                                  dtype=np.int32)
 
     def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs=False,
-               record_path=False):
+               record_path=False, episodes_per_task=None):
         import torch
         assert task_type in ("SURVIVAL", "ESCAPE")
         if final_obs and not auto_reset:
             raise ValueError("final_obs=True needs auto_reset=True (without auto-reset obs already is the terminal frame)")
+        if episodes_per_task is not None and not (int(episodes_per_task) == episodes_per_task and episodes_per_task >= 1):
+            raise ValueError("episodes_per_task must be None or an integer >= 1, got %r" % (episodes_per_task,))
+        self.episodes_per_task = None if episodes_per_task is None else int(episodes_per_task)
         self._want_final = bool(final_obs)
         self.record_path = bool(record_path)
         self._torch = torch
@@ -267,6 +292,32 @@ class _BatchedMazeBase(Snapshots):
         limit (max_steps), so terminated = done & ~truncated.  None with final_obs=False."""
         return None if self._trunc is None else self._out(self._trunc.view(self._torch.bool))
 
+    @property
+    def task_episodes(self):
+        """Trial handles (episodes_per_task=k): CUDA int32 [N], the episodes each env has finished (done) since it was
+        last given a maze (set_task, update_tasks, resample_tasks or an in-launch draw); reset() leaves it alone.  A copy,
+        stream-ordered.  None for a handle without trials."""
+        if self.episodes_per_task is None:
+            return None
+        if self.need_set_task:
+            raise Exception("Must call \"set_task\" before reset")
+        out = self._torch.empty((self.num_envs,), dtype=self._torch.int32, device=self.device)
+        _lib.check(self._lib.mgb_maze_task_episodes(self._h, out.data_ptr(), self._stream()))
+        return out
+
+    def _trial_entries(self, out, resample):
+        """A trial handle's rollout dict gains "task_episodes0" (the counts at launch start, copied on the stream before
+        the launch; a caller-supplied tensor is filled in place), "episodes_per_task" and "resampled"."""
+        if self.episodes_per_task is None:
+            return
+        te = out.get("task_episodes0")
+        if te is None:
+            te = self._torch.empty((self.num_envs,), dtype=self._torch.int32, device=self.device)
+        _lib.check(self._lib.mgb_maze_task_episodes(self._h, te.data_ptr(), self._stream()))
+        out["task_episodes0"] = te
+        out["episodes_per_task"] = self.episodes_per_task
+        out["resampled"] = resample is not None
+
     def _stream(self):
         return _lib.current_stream(self._torch, self.device)
 
@@ -290,6 +341,8 @@ class _BatchedMazeBase(Snapshots):
         _lib.check(self._lib.mgb_maze_set_options(self._h, int(self.auto_reset)))
         if self.record_path:
             _lib.check(self._lib.mgb_maze_set_path(self._h, 1))
+        if self.episodes_per_task is not None:
+            _lib.check(self._lib.mgb_maze_set_episodes_per_task(self._h, self.episodes_per_task))
         self._after_create()
 
     @staticmethod
@@ -473,6 +526,7 @@ class _BatchedMazeBase(Snapshots):
         if actions is not None:
             a = torch.as_tensor(actions, dtype=act_dtype, device=dev).reshape(act_shape).contiguous()
         cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+        self._trial_entries(out, resample)
         _lib.check(self._lib.mgb_maze_rollout(self._h, T, _lib.ptr(a), int(act_seed),
                                               _lib.ptr(out.get("act") if record else None), _lib.ptr(out.get("obs")),
                                               _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")),
@@ -648,19 +702,28 @@ class _LazySteps(dict):
 
 
 class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
-    """MetaMaze2D(enable_render, render_scale, max_steps, task_type, view_grid) x num_envs (maze_env.py:155-172)."""
+    """MetaMaze2D(enable_render, render_scale, max_steps, task_type, view_grid) x num_envs (maze_env.py:155-172).
+
+    episodes_per_task=k (all three maze kinds; default None: no trials) makes a trial handle for RL^2: each env counts
+    the episodes it finishes on its current maze (task_episodes), and a rollout with resample= gives a finished env a
+    new maze only when that episode was its k-th there; the others restart on the same maze, and a recurrent policy
+    with hidden_reset="task" keeps its state across them.  k = 1 behaves exactly like None.  Without resample= step()
+    and rollout() only count; combine task_episodes with resample_tasks(mask) to re-task from the host.  k is fixed for
+    the handle's life; a trial handle's snapshot records are 16 bytes longer and restore only into a handle with the
+    same k."""
     KIND = 0
     _MIRROR_PREFIX = "mgb_maze"
 
     def __init__(self, enable_render=False, render_scale=480, max_steps=5000, task_type="SURVIVAL", view_grid=2,
                  num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True, final_obs=False,
-                 record_path=False):
+                 record_path=False, episodes_per_task=None):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
         self.render_scale = int(render_scale)
         self.view_grid = int(view_grid)
-        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path)
+        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path,
+                    episodes_per_task)
         w = 2 * self.view_grid + 1
         # the reference declares Box(-1, 1, (3,3), int32) but returns float32 (2g+1)^2 arrays (maze_2d.py:92)
         self.observation_space = Box(low=-1, high=1, shape=(w, w), dtype=np.float32)
@@ -688,7 +751,11 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         Every env whose episode ends at step t then gets the maze resample_tasks(done,
         **resample) would give it, in the same launch: obs[t] is its first window on the new maze, final_obs[t] the
         terminal window on the old one.  Needs auto_reset=True and set_task() with one table slot per env, like
-        resample_tasks; with n = 31 the view_grid may be at most 6.
+        resample_tasks; with n = 31 the view_grid may be at most 6.  On a trial handle (episodes_per_task=k) only an
+        episode that is the env's k-th on its maze draws; new_tasks(out) marks where envs drew.
+
+        A trial handle's dict also holds "task_episodes0" [N] int32 (task_episodes at launch start),
+        "episodes_per_task" (k) and "resampled".
 
         policy: an MLPPolicy (metagym_b200.policy) with (2 view_grid + 1)^2 inputs whose four outputs are the logits of
         the actions (mgb_maze_rollout_policy): the action of step t is drawn from their softmax on the window before
@@ -746,6 +813,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         if recurrent:
             out["resampled"] = resample is not None
         cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+        self._trial_entries(out, resample)
         pol = policy.struct(deterministic)
         args = [self._h, T, ctypes.byref(pol), int(act_seed), None if cfg is None else ctypes.byref(cfg), seed]
         if recurrent:
@@ -773,7 +841,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     def __init__(self, enable_render=False, render_scale=480, resolution=(320, 320), max_steps=5000,
                  task_type="SURVIVAL", num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True,
                  obs_dtype="int32", textures=None, max_vision_range=12.0, fol_angle=0.6 * PI, cache=None,
-                 final_obs=False, record_path=False):
+                 final_obs=False, record_path=False, episodes_per_task=None):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
@@ -784,7 +852,8 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         self.max_vision_range, self.fol_angle = max_vision_range, fol_angle
         self.cache = cache                  # None: library default (on, MGB_MAZE_CACHE); False: direct renderer only
         self.textures = textures if textures is not None else synthetic_textures(seed=0)
-        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path)
+        self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path,
+                    episodes_per_task)
         torch = self._torch
         h, v = self.resolution
         self.observation_space = Box(low=0, high=256, shape=(h, v, 3), dtype=np.float32)     # maze_env.py:37-39
@@ -817,7 +886,8 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         resample: None, or resample_tasks' keyword arguments with its seed, e.g. dict(seed=5, crowd_ratio=0.35).  Every
         env whose episode ends at step t then gets the maze resample_tasks(done, **resample) would give it, in the same
         launch: obs[t] is its first frame on the new maze, final_obs[t] the terminal frame on the old one.  Needs
-        auto_reset=True, cache=False and set_task() with one table slot per env, like resample_tasks."""
+        auto_reset=True, cache=False and set_task() with one table slot per env, like resample_tasks.  Trial handles
+        (episodes_per_task=k): as for BatchedMetaMaze2D.rollout."""
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs),
                              resample=resample)
 

@@ -270,7 +270,9 @@ class _RecurrentPolicy(object):
     def unroll(self, out):
         """Recompute a recurrent rollout with autograd through the cell and head: returns (logits [T, N, 4],
         logp [T, N]), logp the log-probability of out["act"].  Uses out's obs0, obs, act, rew, done, state0 and
-        resampled, and applies the kernel's input construction and reset rule, in the cell's dtype and device."""
+        resampled (and on a trial handle task_episodes0 and episodes_per_task), and applies the kernel's input
+        construction and reset rule, in the cell's dtype and device."""
+        from .metamaze import new_tasks
         torch = self._torch
         head, D = self._head, self.obs_dim
         w = self._cell.weight_ih
@@ -285,7 +287,7 @@ class _RecurrentPolicy(object):
         rew = out["rew"].to(dev).float().to(dt)          # the kernel feeds (float)r back
         done = out["done"].to(dev).bool()
         state0 = out["state0"].to(dev, dt)
-        wipe_on_done = self.hidden_reset == "episode" or bool(out.get("resampled", False))
+        wipe = done if self.hidden_reset == "episode" else new_tasks(out).to(dev)
         nm = self._memory * self.hidden
         mem, fb = state0[:, :nm], state0[:, nm:]
         logits, logp = [], []
@@ -295,7 +297,7 @@ class _RecurrentPolicy(object):
             lg = head(h)
             logits.append(lg)
             logp.append(torch.log_softmax(lg, -1).gather(1, act[t][:, None])[:, 0])
-            keep = ~(done[t] & wipe_on_done)
+            keep = ~wipe[t]
             mem = torch.where(keep[:, None], new_mem, torch.zeros_like(new_mem))
             if self.feedback:
                 new_fb = torch.cat([torch.nn.functional.one_hot(act[t], 4).to(dt), rew[t][:, None]], 1)
@@ -309,7 +311,8 @@ class GRUPolicy(_RecurrentPolicy):
     cell: nn.GRUCell(obs_dim + 5 feedback, H), H 1..64.  head: nn.Linear(H, 4), or nn.Sequential(Linear(H, w), Tanh or
     ReLU, Linear(w, 4)) with w 1..64; its four outputs are the logits of the actions.  feedback: the cell's input ends
     with onehot(prev action) and the prev reward.  hidden_reset: "episode" zeroes an env's state at every done; "task"
-    only where the env drew a new maze inside the launch (rollout with resample=); after set_task / update_tasks /
+    only where the env drew a new maze inside the launch (rollout with resample=; on a trial handle the k-th episode on
+    a maze, metamaze.new_tasks); after set_task / update_tasks /
     resample_tasks the caller zeroes the rows itself.  log_std: the maze's categorical head has none; it must be None.
     obs_mean / obs_std: optional [obs_dim] normalisation (x - mean) / std of the observation inputs, folded into the
     obs columns of weight_ih and into bias_ih on the host in float64.  device: where the packed buffer lives.
