@@ -173,6 +173,11 @@ int mgb_quad_rollout_ex(mgb_quad *h, int32_t T, const float *act_dev, uint64_t a
 #define MGB_POLICY_MEAN 1     /* deterministic: the mean (quadrotor) / argmax of the logits (maze 2-D) */
 #define MGB_POLICY_MAX_HIDDEN 3
 #define MGB_POLICY_MAX_WIDTH 64
+/* Populations (the *_population entry points): envs per member are a multiple of MGB_POLICY_MEMBER_WARP and either
+ * divide the policy kernel's CTA env count or are a multiple of it. */
+#define MGB_POLICY_MEMBER_WARP 32
+#define MGB_QUAD_POLICY_CTA_ENVS 64      /* quadrotor: 32 or a multiple of 64 envs per member */
+#define MGB_MAZE2D_POLICY_CTA_ENVS 128   /* MetaMaze2D: 32, 64 or a multiple of 128 envs per member */
 
 typedef struct mgb_policy {
     const float *params_dev;  /* packed float32 on the handle's device, read at every launch */
@@ -197,6 +202,18 @@ typedef struct mgb_policy {
 int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy *pol, uint64_t seed, float *act_out_dev,
                             float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
                             float *final_obs_dev, uint8_t *truncated_dev, void *stream);
+
+/* mgb_quad_rollout_policy with a population of `members` policies of pol's shape (DESIGN.md "Populations"): member m's
+ * packed buffer starts at pol->params_dev + m member_stride floats, and with E = n / members it drives the envs
+ * [m E, (m + 1) E) of the handle.  Every other input, output, draw (keyed by the global env index) and refusal is
+ * mgb_quad_rollout_policy's, and members = 1 is that call exactly (the stride is then not read).  Also refused
+ * (MGB_ERR_ARG, handle untouched): members < 1, n not a multiple of members, E neither 32 nor a multiple of
+ * MGB_QUAD_POLICY_CTA_ENVS, member_stride below the packed length (with log_std), and the staged members of one CTA
+ * with the activations beyond the device's opt-in shared memory. */
+int mgb_quad_rollout_population(mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members, int64_t member_stride,
+                                uint64_t seed, float *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                                uint8_t *truncated_dev, void *stream);
 
 /* Quadrotor.step as the reference's numpy users call it (env.py:127-165: ndarray in, ndarray out).
  * Same as mgb_quad_step with HOST buffers: stages through pinned memory (or, for pinned caller buffers, lets the kernel
@@ -537,6 +554,26 @@ int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint
                          int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
                          float *obs_dev, double *rew_dev, uint8_t *done_dev,
                          float *final_obs_dev, uint8_t *truncated_dev, void *stream);
+
+/* mgb_maze_rollout_policy and mgb_maze_rollout_rnn with a population of `members` policies of pol's shape (DESIGN.md
+ * "Populations"): member m's packed buffer starts at pol->params_dev + m member_stride floats, and with E = n / members
+ * it drives the envs [m E, (m + 1) E) of the handle (its rows of state_dev too).  Every other input, output, draw
+ * (keyed by the global env index) and refusal is that of the single-policy call, and members = 1 is that call exactly
+ * (the stride is then not read).  Also refused (MGB_ERR_ARG; the handle, its step counter and the state untouched):
+ * members < 1, n not a multiple of members, E not 32, 64 or a multiple of MGB_MAZE2D_POLICY_CTA_ENVS, member_stride
+ * below the packed length, and the staged members of one CTA with the tiles and activations beyond the device's opt-in
+ * shared memory. */
+int mgb_maze_rollout_population(mgb_maze *h, int32_t T, const mgb_policy *pol, int32_t members, int64_t member_stride,
+                                uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                                double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                void *stream);
+int mgb_maze_rollout_rnn_population(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                    int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
+                                    uint64_t resample_seed, float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                                    int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                                    double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                    void *stream);
 
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */

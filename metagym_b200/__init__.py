@@ -24,7 +24,7 @@ def __getattr__(name):
                 "MetaMazeDiscrete3D", "MetaMazeContinuous3D", "TaskConfig", "MazeTaskSampler"):
         from . import metamaze
         return getattr(metamaze, name)
-    if name in ("MLPPolicy", "GRUPolicy", "LSTMPolicy"):
+    if name in ("MLPPolicy", "GRUPolicy", "LSTMPolicy", "PolicyPopulation"):
         from . import policy
         return getattr(policy, name)
     raise AttributeError(name)

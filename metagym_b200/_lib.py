@@ -64,6 +64,9 @@ ACT_TANH, ACT_RELU = 0, 1            # MGB_ACT_*
 POLICY_SAMPLE, POLICY_MEAN = 0, 1    # MGB_POLICY_*
 RNN_RESET_EPISODE, RNN_RESET_TASK = 0, 1     # MGB_RNN_RESET_*
 RNN_CELL_GRU, RNN_CELL_LSTM = 0, 1           # MGB_RNN_CELL_*
+POLICY_MEMBER_WARP = 32                      # MGB_POLICY_MEMBER_WARP
+QUAD_POLICY_CTA_ENVS = 64                    # MGB_QUAD_POLICY_CTA_ENVS
+MAZE2D_POLICY_CTA_ENVS = 128                 # MGB_MAZE2D_POLICY_CTA_ENVS
 
 
 # name -> (restype, argtypes); every function include/mgb200.h declares (tests/test_abi.py checks the two agree)
@@ -85,6 +88,8 @@ SIGNATURES = {
     "mgb_quad_rollout_ex": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_quad_rollout_policy": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_u64, vp, vp, vp, vp, vp, vp, vp, vp,
                                                vp]),
+    "mgb_quad_rollout_population": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_i32, c_i64, c_u64, vp, vp, vp,
+                                                   vp, vp, vp, vp, vp, vp]),
     "mgb_quad_state": (ctypes.c_int, [vp, vp, vp, ctypes.c_int, vp]),
     "mgb_quad_launch_count": (c_i64, [vp]),
     "mgb_quad_step_kernel": (ctypes.c_char_p, [vp]),
@@ -120,6 +125,12 @@ SIGNATURES = {
                                                c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_rollout_rnn": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_u64, ctypes.POINTER(MazeSamplerCfg),
                                             c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_rollout_population": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_i32, c_i64, c_u64,
+                                                   ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp, vp,
+                                                   vp, vp]),
+    "mgb_maze_rollout_rnn_population": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64,
+                                                       ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp,
+                                                       vp, vp, vp, vp, vp, vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

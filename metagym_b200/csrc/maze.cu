@@ -411,6 +411,7 @@ __global__ void maze_reset_kernel(const __grid_constant__ MazeConst c, const __g
 // 2-D: one thread per env; observation tile of the CTA leaves through shared memory + one bulk store
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int k2dThreads = 128;
+static_assert(k2dThreads == MGB_MAZE2D_POLICY_CTA_ENVS, "include/mgb200.h publishes the policy CTA's env count");
 
 __global__ void __launch_bounds__(k2dThreads) maze2d_kernel(const __grid_constant__ MazeConst c,
                                                             const __grid_constant__ MazeArgs a)
@@ -518,10 +519,12 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // POL (XM == 0 only, mgb_maze_rollout_policy): the action of step t is drawn from the MLP policy `pol` (mgb_policy.cuh,
 // categorical head) on the window the env holds before step t.  Each step copies the window row it leaves in the tile
 // (post auto-reset and resampling) into the thread's column of the activation buffers, which follow the tiles and the
-// sampler workspaces in dynamic shared memory at pol.smem_off; at t = 0 the window of the loaded state.  The step
-// arithmetic after the action is the code the other instantiations run.
+// sampler workspaces in dynamic shared memory at pol.smem_off, behind the staged weights; at t = 0 the window of the
+// loaded state.  A population's CTA stages the one member that drives its envs, or its head.copies members back to back,
+// each warp reading its own (mgb_population_stage).  The step arithmetic after the action is the code the other
+// instantiations run.
 // POL == kPolGru or kPolLstm (mgb_maze_rollout_rnn): the policy is the recurrent `pol` (MgbRnn, mgb_policy.cuh).  Its
-// region at pol.smem_off holds the staged cell and head, then the columns x, c, h0, h1 and w.  The obs rows of x are
+// region at pol.smem_off holds the staged cell and head (of each staged member), then the columns x, c, h0, h1 and w.  The obs rows of x are
 // filled as for the MLP; at t = 0 the state row fills h0, c and the feedback rows of x.  Step t computes h1 from
 // (x, h0, c), updating c in place, and acts on head(h1), whose hidden layer goes to w (GRU) or the dead h0 (LSTM).
 // After the step the carry swaps h0 and h1 and writes (onehot(a), (float)r) into the feedback rows, or zeroes h, c and
@@ -561,23 +564,23 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
     const int n = c.n, g = c.view_grid;
-    float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the input, the hidden layer
+    const float *pol_w = nullptr;                                   // the staged weights (mgb_population_weights)
+    float *pol_x = nullptr, *pol_y = nullptr;                       // the input, the hidden layer
     float *hid_prev = nullptr, *hid_new = nullptr, *cst = nullptr;  // RNN: the columns h0, h1 and c
     const MgbMlp &head = mgb_policy_head(pol);                      // the plan of the categorical head
     if constexpr (POL) {
         static_assert(XM == 0, "policy rollouts are not mirrored");
-        pol_w = tile2d + pol.smem_off;
-        pol_x = pol_w + pol.staged;
+        pol_x = tile2d + pol.smem_off + head.copies * pol.staged;
         if constexpr (RNN) {
             cst = pol_x + pol.in * k2dThreads;
             hid_prev = cst + pol.C() * k2dThreads;
             hid_new = hid_prev + pol.Hr * k2dThreads;
             pol_y = hid_new + pol.Hr * k2dThreads;     // w; the LSTM's head uses the dead h0 instead
-            mgb_rnn_stage(pol, pol_w);
         } else {
             pol_y = pol_x + pol.maxw * k2dThreads;
-            mgb_mlp_stage(pol, pol_w);
         }
+        pol_w = tile2d + pol.smem_off;
+        mgb_population_stage(pol, tile2d + pol.smem_off, e0, rows, k2dThreads);
         if (active) {       // the window of the loaded state: what the preceding reset() / step() returned
             float *row = tile2d + threadIdx.x * D;
             maze2d_window(c, blob, eaten, a.n_pad, s, row);
@@ -610,16 +613,18 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
             int action;
             if constexpr (POL) {
                 float logits[4];
-                if constexpr (RNN) {
-                    mgb_rnn_cell(pol, pol_w, pol_x, hid_prev, cst, hid_new, k2dThreads, threadIdx.x);
-                    if (pol.hid_out)
-                        for (int k = 0; k < pol.H; ++k)
-                            pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * k2dThreads + threadIdx.x];
-                    if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
-                    mgb_mlp_forward(head, pol_w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits);
-                } else {
-                    mgb_mlp_forward(pol, pol_w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
-                }
+                mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
+                    if constexpr (RNN) {
+                        mgb_rnn_cell(pol, w, pol_x, hid_prev, cst, hid_new, k2dThreads, threadIdx.x);
+                        if (pol.hid_out)
+                            for (int k = 0; k < pol.H; ++k)
+                                pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * k2dThreads + threadIdx.x];
+                        if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
+                        mgb_mlp_forward(head, w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits);
+                    } else {
+                        mgb_mlp_forward(pol, w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
+                    }
+                });
                 const float lp = mgb_categorical_action(head, genv, a.t_base + (uint32_t)t, logits, action);
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
                 if (head.logp_out) head.logp_out[(int64_t)t * a.n + e] = lp;
@@ -4352,11 +4357,13 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
 
 // A policy rollout of kind POL (mgb_maze_rollout_policy, mgb_maze_rollout_rnn) with the plan `pol`.  The checks, in
 // order: the handle, T, the handle kind, then own(observation width) (the entry point plans the policy into pol and
-// makes its own checks; it returns the refusal, or nullptr), logp_out in the mean mode, mirrors, resampling, the
+// makes its own checks; it returns the refusal, or nullptr), the population (one member: nothing to refuse), logp_out
+// in the mean mode, mirrors, resampling, the
 // optional outputs and the handle's state.  The policy's region of dynamic shared memory follows the tiles and the
 // sampler workspaces.
 template <int POL, class Own>
-static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolicyPlan<POL> &pol, Own own, uint64_t seed,
+static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolicyPlan<POL> &pol, Own own,
+                               int32_t members, int64_t member_stride, uint64_t seed,
                                const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, int32_t *act_out_dev,
                                float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev,
                                uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
@@ -4369,6 +4376,7 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
                                   : "mgb_maze_rollout_rnn serves MetaMaze2D (the 3-D envs observe frames)";
         const int W = 2 * h->c.view_grid + 1;
         if (const char *why = own(W * W)) return why;
+        if (const char *why = mgb_population_plan(head, h->n, members, member_stride, k2dThreads)) return why;
         if (logp_out_dev && head.mode != MGB_POLICY_SAMPLE) return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
@@ -4410,6 +4418,20 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
     return resample_cfg ? MGB_OK : count_done(h, done_dev, T, st);
 }
 
+// mgb_maze_rollout_policy of `members` policies (one: mgb_maze_rollout_policy), refused as `fn`
+static int maze_rollout_mlp(const char *fn, mgb_maze *h, int32_t T, const mgb_policy *pol, int32_t members,
+                            int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
+                            uint64_t resample_seed, int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                            float *obs_dev, double *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                            uint8_t *truncated_dev, void *stream)
+{
+    MgbMlp m;
+    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m); };
+    return maze_rollout_policy<kPolMlp>(fn, h, T, m, own, members, member_stride, seed, resample_cfg, resample_seed,
+                                        act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
+                                        final_obs_dev, truncated_dev, stream);
+}
+
 extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
                                        const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
                                        int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
@@ -4417,21 +4439,29 @@ extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy 
                                        void *stream)
 {
     MgbRange nvtx_range("mgb_maze_rollout_policy");
-    MgbMlp m;
-    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m); };
-    return maze_rollout_policy<kPolMlp>(__func__, h, T, m, own, seed, resample_cfg, resample_seed, act_out_dev,
-                                        logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev,
-                                        truncated_dev, stream);
+    return maze_rollout_mlp(__func__, h, T, pol, 1, 0, seed, resample_cfg, resample_seed, act_out_dev, logp_out_dev,
+                            obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
 }
 
-extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed,
-                                    const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
-                                    float *state_dev, float *state0_out_dev, float *hid_out_dev,
-                                    int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
-                                    float *obs_dev, double *rew_dev, uint8_t *done_dev,
-                                    float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+extern "C" int mgb_maze_rollout_population(mgb_maze *h, int32_t T, const mgb_policy *pol, int32_t members,
+                                           int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
+                                           uint64_t resample_seed, int32_t *act_out_dev, float *logp_out_dev,
+                                           float *obs0_out_dev, float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                           float *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
-    MgbRange nvtx_range("mgb_maze_rollout_rnn");
+    MgbRange nvtx_range("mgb_maze_rollout_population");
+    return maze_rollout_mlp(__func__, h, T, pol, members, member_stride, seed, resample_cfg, resample_seed, act_out_dev,
+                            logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
+}
+
+// mgb_maze_rollout_rnn of `members` policies (one: mgb_maze_rollout_rnn), refused as `fn`
+static int maze_rollout_rnn(const char *fn, mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                            int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
+                            uint64_t resample_seed, float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                            int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                            double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                            void *stream)
+{
     // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
     const auto run = [&](auto kind) {
         constexpr int POL = decltype(kind)::value;
@@ -4446,12 +4476,39 @@ extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy
             if (!h->auto_reset) return "the recurrent rollout needs auto_reset on (an episode boundary has no next step without it)";
             return nullptr;
         };
-        return maze_rollout_policy<POL>("mgb_maze_rollout_rnn", h, T, p, own, seed, resample_cfg, resample_seed,
+        return maze_rollout_policy<POL>(fn, h, T, p, own, members, member_stride, seed, resample_cfg, resample_seed,
                                         act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
                                         final_obs_dev, truncated_dev, stream);
     };
     return pol && pol->cell == MGB_RNN_CELL_LSTM ? run(std::integral_constant<int, kPolLstm>{})
                                                  : run(std::integral_constant<int, kPolGru>{});
+}
+
+extern "C" int mgb_maze_rollout_rnn(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed,
+                                    const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                    float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                                    int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                    float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                    float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_rnn");
+    return maze_rollout_rnn(__func__, h, T, pol, 1, 0, seed, resample_cfg, resample_seed, state_dev, state0_out_dev,
+                            hid_out_dev, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
+                            final_obs_dev, truncated_dev, stream);
+}
+
+extern "C" int mgb_maze_rollout_rnn_population(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                               int64_t member_stride, uint64_t seed,
+                                               const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                               float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                                               int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                               float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                               float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_rnn_population");
+    return maze_rollout_rnn(__func__, h, T, pol, members, member_stride, seed, resample_cfg, resample_seed, state_dev,
+                            state0_out_dev, hid_out_dev, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
+                            done_dev, final_obs_dev, truncated_dev, stream);
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)

@@ -29,6 +29,12 @@ struct MgbMlp {
     uint64_t seed;
     float *logp_out;              // [T][n] or null
     float *obs0_out;              // [n][in[0]] or null
+    // populations (DESIGN.md "Populations"); a plan's head holds them for the whole policy, as it does seed and mode
+    int packed;                   // floats of one packed buffer that the plan reads
+    int copies;                   // members staged per CTA: CTA envs / member_envs when that is above 1, else 1
+    int64_t member_envs;          // envs per member: member m drives the envs [m E, (m + 1) E); INT64_MAX: one policy
+    int64_t member_stride;        // floats from one member's packed buffer to the next
+    int member_shift;             // the warp's staged copy is threadIdx.x >> member_shift (31: the only one)
 };
 
 // Host: validate `p` and plan it for input width `in_dim` (output width 4; `log_std`: the buffer ends with log_std[4],
@@ -71,30 +77,36 @@ static inline const char *mgb_mlp_plan(const mgb_policy *p, int in_dim, bool log
     }
     m.staged = s;
     m.maxw = maxw;
+    m.packed = g + (log_std ? 4 : 0);
+    m.copies = 1;
+    m.member_envs = INT64_MAX;
+    m.member_shift = 31;
     return nullptr;
 }
 
-// floats of dynamic shared memory a CTA of `threads` needs: staged weights + two activation buffers
+// bytes of dynamic shared memory a CTA of `threads` needs: staged weights of m.copies members + two activation buffers
 static inline size_t mgb_mlp_smem_bytes(const MgbMlp &m, int threads)
 {
-    return ((size_t)m.staged + 2 * (size_t)m.maxw * (size_t)threads) * sizeof(float);
+    return ((size_t)m.staged * (size_t)m.copies + 2 * (size_t)m.maxw * (size_t)threads) * sizeof(float);
 }
 
-// Device: stage the weights of `m` into sm[0, m.staged) (all threads of the CTA; the caller synchronises)
-__device__ __forceinline__ void mgb_mlp_stage(const MgbMlp &m, float *sm)
+// Device: stage the weights of `m` read at m.params + off into sm[0, m.staged) (all threads of the CTA; the caller
+// synchronises)
+__device__ __forceinline__ void mgb_mlp_stage(const MgbMlp &m, float *sm, int64_t off)
 {
     for (int l = 0; l < m.n_layers; ++l) {
         const bool last = l == m.n_layers - 1;
         const int gwid = last ? 4 : 8, in = m.in[l], out = m.out[l];
         const int rows = (out + gwid - 1) / gwid * gwid;
-        const float *W = m.params + m.gw[l], *b = W + out * in;
+        const float *W = m.params + off + m.gw[l], *b = W + out * in;
         for (int s = threadIdx.x; s < rows * in; s += blockDim.x) {
             const int r = s % gwid, rest = s / gwid, i = rest % in, j = (rest / in) * gwid + r;
             sm[m.sw[l] + s] = j < out ? __ldg(W + j * in + i) : 0.f;
         }
         for (int j = threadIdx.x; j < rows; j += blockDim.x) sm[m.sb[l] + j] = j < out ? __ldg(b + j) : 0.f;
     }
-    if (m.s_log_std >= 0 && threadIdx.x < 4) sm[m.s_log_std + threadIdx.x] = __ldg(m.params + m.g_log_std + threadIdx.x);
+    if (m.s_log_std >= 0 && threadIdx.x < 4)
+        sm[m.s_log_std + threadIdx.x] = __ldg(m.params + off + m.g_log_std + threadIdx.x);
 }
 
 __device__ __forceinline__ float mgb_mlp_activate(int activation, float x)
@@ -303,25 +315,29 @@ static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, Mgb
                            p->mode};
     if (const char *why = mgb_mlp_plan(&hp, r.H, false, r.head)) return why;
     r.staged = r.s_head + r.head.staged;
+    r.head.packed += r.g_b + 2 * NG * r.H;
     return nullptr;
 }
 
-// bytes of dynamic shared memory a CTA of `threads` needs: staged weights + the columns x, c, h0, h1 and w
+// bytes of dynamic shared memory a CTA of `threads` needs: staged weights of head.copies members + the columns x, c,
+// h0, h1 and w
 template <int NG>
 static inline size_t mgb_rnn_smem_bytes(const MgbRnn<NG> &r, int threads)
 {
-    return ((size_t)r.staged + (size_t)(r.in + r.C() + 2 * r.Hr + r.Hw) * (size_t)threads) * sizeof(float);
+    return ((size_t)r.staged * (size_t)r.head.copies + (size_t)(r.in + r.C() + 2 * r.Hr + r.Hw) * (size_t)threads) *
+           sizeof(float);
 }
 
-// Device: stage the cell and the head into sm[0, r.staged) (all threads of the CTA; the caller synchronises)
+// Device: stage the cell and the head read at r.params + off into sm[0, r.staged) (all threads of the CTA; the caller
+// synchronises)
 template <int NG>
-__device__ __forceinline__ void mgb_rnn_stage(const MgbRnn<NG> &r, float *sm)
+__device__ __forceinline__ void mgb_rnn_stage(const MgbRnn<NG> &r, float *sm, int64_t off)
 {
     constexpr int G = kRnnGroup;
     const int H = r.H;
     for (int part = 0; part < 2; ++part) {
         const int K = part ? H : r.in;
-        const float *W = r.params + (part ? r.g_hh : 0);
+        const float *W = r.params + off + (part ? r.g_hh : 0);
         float *dst = sm + (part ? r.s_hh : 0);
         for (int s = threadIdx.x; s < NG * r.Hp * K; s += blockDim.x) {
             const int u = s % G, k = (s / G) % NG, i = (s / (NG * G)) % K, j = (s / (NG * G * K)) * G + u;
@@ -330,9 +346,66 @@ __device__ __forceinline__ void mgb_rnn_stage(const MgbRnn<NG> &r, float *sm)
     }
     for (int s = threadIdx.x; s < 2 * NG * r.Hp; s += blockDim.x) {
         const int u = s % G, k = (s / G) % NG, kind = (s / (NG * G)) % 2, j = (s / (2 * NG * G)) * G + u;
-        sm[r.s_b + s] = j < H ? __ldg(r.params + r.g_b + kind * NG * H + k * H + j) : 0.f;
+        sm[r.s_b + s] = j < H ? __ldg(r.params + off + r.g_b + kind * NG * H + k * H + j) : 0.f;
     }
-    mgb_mlp_stage(r.head, sm + r.s_head);
+    mgb_mlp_stage(r.head, sm + r.s_head, off);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Populations (DESIGN.md "Populations"): `members` packed policies of one plan, `member_stride` floats apart; with
+// E = n / members, member m drives the envs [m E, (m + 1) E) of the handle.  E is a multiple of a warp's 32 envs and
+// either divides the CTA's env count or is a multiple of it.  A CTA whose envs belong to one member stages it once;
+// a CTA of CTA / E members stages them back to back, `staged` floats apart, and every warp reads its own member.
+// ---------------------------------------------------------------------------------------------------------------
+
+// Host: spread the population over the n envs of a handle whose policy CTA holds `cta` envs, into the plan's head.
+// Returns null, or the reason the population is refused.  One member reads no stride and leaves the plan as it is.
+static inline const char *mgb_population_plan(MgbMlp &head, int64_t n, int32_t members, int64_t member_stride, int cta)
+{
+    if (members < 1) return "members must be at least 1";
+    if (n % members != 0) return "num_envs must be a multiple of members";
+    if (members == 1) return nullptr;
+    const int64_t E = n / members;
+    if (E % MGB_POLICY_MEMBER_WARP != 0 || (E < cta ? cta % E : E % cta) != 0)
+        return "envs per member (num_envs / members) must be a multiple of 32 that divides the policy CTA's envs or is a "
+               "multiple of them (MGB_QUAD_POLICY_CTA_ENVS, MGB_MAZE2D_POLICY_CTA_ENVS)";
+    if (member_stride < head.packed) return "member_stride is shorter than one member's packed policy";
+    head.member_envs = E;
+    head.member_stride = member_stride;
+    head.copies = E < cta ? (int)(cta / E) : 1;
+    if (E < cta) head.member_shift = E == 32 ? 5 : 6;        // E divides a CTA of 64 or 128: 32 or 64
+    return nullptr;
+}
+
+// Device: stage the members that drive the CTA's envs [e0, e0 + rows) into sm, `staged` floats apart (all threads of
+// the CTA; the caller synchronises).  One policy (member_stride 0) stages from the buffer's start.
+template <class Plan>
+__device__ __forceinline__ void mgb_population_stage(const Plan &p, float *sm, int64_t e0, int rows, int cta)
+{
+    const MgbMlp &head = mgb_policy_head(p);
+    const int64_t E = head.member_envs, m0 = head.member_stride ? e0 / E : 0;
+    const int here = E < cta ? (int)((rows + E - 1) / E) : 1;      // a partial last CTA holds fewer members
+    for (int j = 0; j < here; ++j) {
+        if constexpr (std::is_same_v<Plan, MgbMlp>) mgb_mlp_stage(p, sm + j * p.staged, (m0 + j) * head.member_stride);
+        else mgb_rnn_stage(p, sm + j * p.staged, (m0 + j) * head.member_stride);
+    }
+}
+
+// Device: f(w) with w the staged copy the thread's warp reads, of the copies mgb_population_stage left at sm.  With one
+// copy per CTA (one policy, or a member per CTA or more) w is sm itself, and the compiler keeps the weight addresses in
+// uniform registers; it cannot for the warp's copy (threadIdx.x >> member_shift), and a single-policy MetaMaze2D MLP
+// rollout through that address alone measured 6.5 % slower.  So f is compiled for both.  The empty asm ends the two
+// arms differently, so that the compiler does not sink their common code below the branch and make w one per-thread
+// value again.
+template <class F>
+__device__ __forceinline__ void mgb_population_weights(const MgbMlp &head, const float *sm, int staged, F &&f)
+{
+    if (head.copies == 1) {
+        f(sm);
+    } else {
+        f(sm + ((int)threadIdx.x >> head.member_shift) * staged);
+        asm volatile("");
+    }
 }
 
 __device__ __forceinline__ float mgb_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }

@@ -34,6 +34,7 @@
 namespace {
 
 constexpr int kThreads = 64;   // scalar tile kernel / rollout kernel: envs per CTA
+static_assert(kThreads == MGB_QUAD_POLICY_CTA_ENVS, "include/mgb200.h publishes the policy CTA's env count");
 constexpr int kMaxObs = 19;
 
 // Constants derived on the host (double arithmetic, rounded once to float32 -- numpy's "weak python scalar" rule).
@@ -1148,7 +1149,9 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 // POL (XM == 0 only, mgb_quad_rollout_policy): the action of step t is drawn from the MLP policy `pol` (mgb_policy.cuh)
 // on the observation the env holds before step t, which each step leaves in the thread's column of the activation
 // buffers in dynamic shared memory (at t = 0: the observation of the loaded state).  The weights are staged once per
-// CTA.  The step arithmetic after the action is the code the other instantiations run.
+// CTA: the one member of a population that drives the CTA's envs, or its pol.copies members back to back, each warp
+// reading its own (mgb_population_stage).  The step arithmetic after the action is the code the other instantiations
+// run.
 template <bool SIMPLE, int XM, bool FIN, bool POL = false>
 __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(const __grid_constant__ QuadConst c,
                                                                           const __grid_constant__ QuadArgs a,
@@ -1169,14 +1172,15 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
     const uint2 akey = make_uint2((uint32_t)a.act_seed, (uint32_t)(a.act_seed >> 32));
     const int64_t genv = a.env_base + e;
     const int task = active ? env_task(c, a, e) : 0;
-    float *pol_w = nullptr, *pol_x = nullptr, *pol_y = nullptr;    // staged weights, the two activation buffers
+    const float *pol_w = nullptr;           // the staged weights (mgb_population_weights)
+    float *pol_x = nullptr, *pol_y = nullptr;   // the two activation buffers
     if constexpr (POL) {
         static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
         extern __shared__ __align__(16) float pol_smem[];
-        pol_w = pol_smem;
-        pol_x = pol_w + pol.staged;
+        pol_x = pol_smem + pol.copies * pol.staged;
         pol_y = pol_x + pol.maxw * kThreads;
-        mgb_mlp_stage(pol, pol_w);
+        pol_w = pol_smem;
+        mgb_population_stage(pol, pol_smem, e0, rows, kThreads);
         if (active) {       // the observation of the loaded state: what the preceding reset() / step() returned
             float o[kMaxObs], bv[3], Ri[9];
             observe(c, s, adj, id, o, bv, Ri);
@@ -1206,9 +1210,11 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
         if (active) {
             float4 act;
             if constexpr (POL) {
-                float mean[4], av[4];
-                mgb_mlp_forward(pol, pol_w, pol_x, pol_y, kThreads, threadIdx.x, mean);
-                const float lp = mgb_gaussian_action(pol, pol_w, genv, a.t_base + (uint32_t)t, mean, av);
+                float mean[4], av[4], lp;
+                mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
+                    mgb_mlp_forward(pol, w, pol_x, pol_y, kThreads, threadIdx.x, mean);
+                    lp = mgb_gaussian_action(pol, w, genv, a.t_base + (uint32_t)t, mean, av);
+                });
                 act = make_float4(av[0], av[1], av[2], av[3]);
                 if (a.act_out) reinterpret_cast<float4 *>(a.act_out)[(int64_t)t * a.n + e] = act;
                 if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
@@ -1830,21 +1836,29 @@ static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_se
     return MGB_OK;
 }
 
-extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy *pol, uint64_t seed, float *act_out_dev,
-                                       float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev,
-                                       uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+// A policy rollout of `members` policies (one: mgb_quad_rollout_policy), refused as `fn`
+static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
+                          int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
+                          float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                          uint8_t *truncated_dev, void *stream)
 {
-    MgbRange nvtx_range("mgb_quad_rollout_policy");
-    MGB_REQUIRE(h, "null handle");
-    MGB_REQUIRE(T > 0, "T must be positive");
+    const auto refuse = [&](const char *why) {
+        mgb_set_error("%s: %s", fn, why);
+        return MGB_ERR_ARG;
+    };
+    if (!h) return refuse("null handle");
+    if (T <= 0) return refuse("T must be positive");
     MgbMlp m;
-    const char *why = mgb_mlp_plan(pol, h->c.obs_dim, true, m);
-    MGB_REQUIRE(!why, why);
-    MGB_REQUIRE(!logp_out_dev || m.mode == MGB_POLICY_SAMPLE, "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)");
-    MGB_REQUIRE(h->mir.count == 0, "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)");
-    MGB_REQUIRE(!final_obs_dev || h->auto_reset, "final_obs needs auto_reset on (without it obs already is the terminal observation)");
-    MGB_REQUIRE((reinterpret_cast<uintptr_t>(act_out_dev) & 15u) == 0, "act_out_dev must be 16-byte aligned");
-    MGB_REQUIRE((reinterpret_cast<uintptr_t>(pol->params_dev) & 3u) == 0, "params_dev must be 4-byte aligned");
+    if (const char *why = mgb_mlp_plan(pol, h->c.obs_dim, true, m)) return refuse(why);
+    if (const char *why = mgb_population_plan(m, h->n, members, member_stride, kThreads)) return refuse(why);
+    if (logp_out_dev && m.mode != MGB_POLICY_SAMPLE)
+        return refuse("logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)");
+    if (h->mir.count != 0)
+        return refuse("policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)");
+    if (final_obs_dev && !h->auto_reset)
+        return refuse("final_obs needs auto_reset on (without it obs already is the terminal observation)");
+    if ((reinterpret_cast<uintptr_t>(act_out_dev) & 15u) != 0) return refuse("act_out_dev must be 16-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(pol->params_dev) & 3u) != 0) return refuse("params_dev must be 4-byte aligned");
     int rc = check_ready(h);
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
@@ -1862,7 +1876,7 @@ extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy 
     MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
     if (fa.sharedSizeBytes + smem > (size_t)optin) {
         mgb_set_error("%s: the policy needs %zu bytes of shared memory per CTA (weights and activations of %d envs), "
-                      "above the device's %d", __func__, fa.sharedSizeBytes + smem, kThreads, optin);
+                      "above the device's %d", fn, fa.sharedSizeBytes + smem, kThreads, optin);
         return MGB_ERR_ARG;
     }
     MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1876,6 +1890,25 @@ extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy 
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
+}
+
+extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy *pol, uint64_t seed, float *act_out_dev,
+                                       float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev,
+                                       uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_policy");
+    return rollout_policy(__func__, h, T, pol, 1, 0, seed, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
+                          done_dev, final_obs_dev, truncated_dev, stream);
+}
+
+extern "C" int mgb_quad_rollout_population(mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
+                                           int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
+                                           float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                                           float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_population");
+    return rollout_policy(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
+                          obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
 }
 
 extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,

@@ -768,9 +768,14 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         its carried state [N, policy.state_dim] float32 on the env's device (policy.initial_state(N) for fresh envs),
         read at the start and updated in place at the end of the launch.  The dict then also holds "state0" (a copy
         of state as read), "resampled" (whether the launch resampled, which unroll() needs for the "task" reset rule)
-        and, with want_hidden=True, "hid" [T,N,H] (the cell's output at every step)."""
-        from .policy import GRUPolicy, LSTMPolicy
-        recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy))
+        and, with want_hidden=True, "hid" [T,N,H] (the cell's output at every step).
+
+        policy may also be a PolicyPopulation of any of the three kinds (mgb_maze_rollout_population,
+        mgb_maze_rollout_rnn_population): member m drives the envs [m E, (m + 1) E), E = N / members, which must be
+        32, 64 or a multiple of 128; a recurrent population takes state= as its members would."""
+        from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
+        recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation)
+                                                                      and policy.recurrent)
         if recurrent and state is None:
             raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
                              % type(policy).__name__)
@@ -783,10 +788,14 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
 
     def _rollout_policy(self, T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden):
+        from .policy import PolicyPopulation
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
         T, N, dev = int(T), self.num_envs, self.device
+        population = isinstance(policy, PolicyPopulation)
+        if population:
+            policy.check_envs(N, _lib.MAZE2D_POLICY_CTA_ENVS)
         shape = tuple(self._obs.shape[1:])
         D = int(np.prod(shape))
         if policy.obs_dim != D:
@@ -815,11 +824,15 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
         self._trial_entries(out, resample)
         pol = policy.struct(deterministic)
-        args = [self._h, T, ctypes.byref(pol), int(act_seed), None if cfg is None else ctypes.byref(cfg), seed]
+        args = [self._h, T, ctypes.byref(pol)] + ([policy.members, policy.member_stride] if population else [])
+        args += [int(act_seed), None if cfg is None else ctypes.byref(cfg), seed]
         if recurrent:
             args += [_lib.ptr(state), _lib.ptr(out.get("state0")), _lib.ptr(out.get("hid"))]
         keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
-        entry = self._lib.mgb_maze_rollout_rnn if recurrent else self._lib.mgb_maze_rollout_policy
+        if population:
+            entry = self._lib.mgb_maze_rollout_rnn_population if recurrent else self._lib.mgb_maze_rollout_population
+        else:
+            entry = self._lib.mgb_maze_rollout_rnn if recurrent else self._lib.mgb_maze_rollout_policy
         _lib.check(entry(*args, *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
         return out
 

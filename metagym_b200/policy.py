@@ -11,7 +11,11 @@ GRUPolicy and LSTMPolicy pack an ``nn.GRUCell`` or an ``nn.LSTMCell`` and a head
 (mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies"): ``weight_ih``, ``weight_hh``, ``bias_ih``, ``bias_hh``, then the
 head's layers as MLPPolicy packs them.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities
 through the torch modules.
+
+PolicyPopulation holds M policies of one shape as the rows of one [M, numel] device tensor, and one rollout launch
+drives each block of num_envs / M envs with its own member (DESIGN.md "Populations").
 """
+import copy
 import ctypes
 
 from . import _lib
@@ -346,3 +350,138 @@ class LSTMPolicy(_RecurrentPolicy):
         H = self.hidden
         h, c = self._cell(x, (mem[:, :H], mem[:, H:]))
         return h, self._torch.cat([h, c], 1)
+
+
+class PolicyPopulation(object):
+    """M policies of one shape that drive one fused rollout together (DESIGN.md "Populations"): with E = N / M, member
+    m acts for the envs [m E, (m + 1) E) of the handle, and everything else (draws keyed by the global env index, reset
+    rules, trials, resampling, the optional outputs, the carried state) is what a handle of those E envs with
+    env_index_base + m E would see with member m alone.
+
+    policies: M MLPPolicy, GRUPolicy or LSTMPolicy objects of one class and one shape: the same layer widths,
+    activation, feedback and hidden_reset, and all or none with log_std.  The observation normalisation may differ,
+    since it is folded into each member's row.  The population owns `params`, a [M, numel] float32 tensor on the
+    members' device; each member's `params` becomes the view of its row, so pop.policies[m].update(...) writes into the
+    population, and a rollout captured in a CUDA graph sees that write and any direct write into pop.params.
+
+    E must be a multiple of 32 that divides the kernel's CTA env count or is a multiple of it: 32 or a multiple of 64
+    on the quadrotor, 32, 64 or a multiple of 128 on MetaMaze2D.  With M = 1 any N is accepted.
+    """
+
+    def __init__(self, policies):
+        import torch
+        self._torch = torch
+        policies = list(policies)
+        if not policies:
+            raise ValueError("PolicyPopulation needs at least one policy")
+        kind = type(policies[0])
+        if kind not in (MLPPolicy, GRUPolicy, LSTMPolicy):
+            raise ValueError("PolicyPopulation takes MLPPolicy, GRUPolicy or LSTMPolicy members, got %s" % kind.__name__)
+        if any(type(p) is not kind for p in policies):
+            raise ValueError("PolicyPopulation: every member must be a %s" % kind.__name__)
+        if len({id(p) for p in policies}) != len(policies):
+            raise ValueError("PolicyPopulation: a policy may be a member once")
+        shapes = {self._shape(p) for p in policies}
+        if len(shapes) != 1:
+            raise ValueError("PolicyPopulation: the members must have one shape (layer widths, activation, feedback, "
+                             "hidden_reset, log_std) and one device")
+        self.policies = policies
+        self.kind = kind
+        self.recurrent = kind is not MLPPolicy
+        first = policies[0]
+        self.numel, self.obs_dim, self.device = first.numel, first.obs_dim, first.device
+        if self.recurrent:
+            self.hidden, self.state_dim = first.hidden, first.state_dim
+        self.params = torch.empty((len(policies), self.numel), dtype=torch.float32, device=self.device)
+        for m, p in enumerate(policies):
+            self.params[m].copy_(p.params)
+            p.params = self.params[m]
+
+    @staticmethod
+    def _shape(p):
+        if isinstance(p, MLPPolicy):
+            return (p.obs_dim, tuple(p.widths), p.activation, p.has_log_std, p.device)
+        return (p.obs_dim, p.hidden, p.head_width, p.activation, p.feedback, p.hidden_reset, p.device)
+
+    @classmethod
+    def from_template(cls, policy, members):
+        """`members` copies of one policy, for evolution strategies: each row starts as policy's packed buffer, and an
+        ES step is one torch op on pop.params followed by one launch.  For an MLPPolicy or a cell and head whose layers
+        all have biases and that has no normalisation, a row equals torch.nn.utils.parameters_to_vector over the
+        module's parameters (MLPPolicy: the Sequential's; GRUPolicy / LSTMPolicy: the cell's, then the head's), followed
+        on an MLPPolicy by its 4 log_std floats (zeros without log_std; the maze does not read them).  The copies share
+        the template's torch modules until a member's update() gives it its own, so unroll() describes the rows only
+        while they hold what the modules pack."""
+        members = int(members)
+        if members < 1:
+            raise ValueError("PolicyPopulation.from_template: members must be at least 1")
+        return cls([policy] + [copy.copy(policy) for _ in range(members - 1)])
+
+    @property
+    def members(self):
+        return len(self.policies)
+
+    @property
+    def has_log_std(self):
+        return all(p.has_log_std for p in self.policies)
+
+    def envs_per_member(self, num_envs):
+        """E = num_envs / members; ValueError when num_envs is not a multiple of members."""
+        num_envs = int(num_envs)
+        if num_envs % self.members:
+            raise ValueError("a population of %d members needs num_envs (%d) to be a multiple of it"
+                             % (self.members, num_envs))
+        return num_envs // self.members
+
+    def check_envs(self, num_envs, cta_envs):
+        """E for a handle of num_envs envs whose policy kernel runs cta_envs envs per CTA; ValueError naming the
+        granularity rule when E is not a multiple of 32 that divides cta_envs or is a multiple of it."""
+        E = self.envs_per_member(num_envs)
+        if self.members > 1 and (E % _lib.POLICY_MEMBER_WARP or (cta_envs % E if E < cta_envs else E % cta_envs)):
+            raise ValueError("a population needs envs per member (num_envs / members = %d) to be a multiple of %d that "
+                             "divides %d or is a multiple of it" % (E, _lib.POLICY_MEMBER_WARP, cta_envs))
+        return E
+
+    def struct(self, deterministic=False):
+        """The policy struct of the C entry points, pointing at row 0; the rows are member_stride floats apart."""
+        st = self.policies[0].struct(deterministic)
+        st.params_dev = self.params.data_ptr()
+        return st
+
+    @property
+    def member_stride(self):
+        return self.params.stride(0)
+
+    _ENV_ROWS = ("obs0", "state0", "task_episodes0")     # [N, ...]; every other tensor entry is [T, N, ...]
+
+    def member_slice(self, out, m):
+        """Member m's env columns of a rollout dict (every [T, N, ...] output, and the rows of obs0, state0 and
+        task_episodes0; other entries are copied), or its rows of an [N, ...] tensor such as the carried state."""
+        torch = self._torch
+        if isinstance(out, torch.Tensor):
+            E = self.envs_per_member(out.shape[0])
+            return out[m * E:(m + 1) * E]
+        E = self.envs_per_member(out["done"].shape[1])
+        sl = slice(m * E, (m + 1) * E)
+        res = {}
+        for k, v in out.items():
+            if isinstance(v, torch.Tensor):
+                res[k] = v[sl] if k in self._ENV_ROWS else v[:, sl]
+            else:
+                res[k] = v
+        return res
+
+    def initial_state(self, num_envs):
+        """[num_envs, state_dim] float32 zeros on the population's device (recurrent populations)."""
+        if not self.recurrent:
+            raise ValueError("initial_state: an MLP population carries no state")
+        return self.policies[0].initial_state(num_envs)
+
+    def unroll(self, out):
+        """The members' unroll() over their env slices of `out`, concatenated along the env axis: (logits [T, N, 4],
+        logp [T, N]) (recurrent populations)."""
+        if not self.recurrent:
+            raise ValueError("unroll: an MLP population has nothing to unroll")
+        parts = [p.unroll(self.member_slice(out, m)) for m, p in enumerate(self.policies)]
+        torch = self._torch
+        return torch.cat([lg for lg, _ in parts], 1), torch.cat([lp for _, lp in parts], 1)

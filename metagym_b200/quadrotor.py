@@ -350,6 +350,8 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         Philox stream keyed by act_seed; deterministic=True takes the mean.  The dict then also holds "act" [T,N,4]
         (the actions taken), "logp" [T,N] (their log-probabilities; sampling only) and "obs0" [N,D] (the observation
         acted on at t = 0; at t > 0 it is obs[t-1]).  `actions` together with `policy` is a ValueError.
+        policy may also be a PolicyPopulation of MLPPolicy members (mgb_quad_rollout_population): member m drives the
+        envs [m E, (m + 1) E), E = N / members, which must be 32 or a multiple of 64.
 
         With final_obs=True the dict also holds "final_obs" [T,N,D] float32: row (t, e) is the terminal observation
         of env e where done[t, e] (what step() reports as final_observation); it is allocated with torch.empty, and
@@ -361,8 +363,8 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
-            from .policy import GRUPolicy, LSTMPolicy
-            if isinstance(policy, (GRUPolicy, LSTMPolicy)):
+            from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
+            if isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation) and policy.recurrent):
                 raise ValueError("recurrent policies run on MetaMaze2D only; the quadrotor takes an MLPPolicy")
             return self._rollout_policy(T, policy, act_seed, deterministic, out)
         if out is None:
@@ -382,8 +384,12 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         return out
 
     def _rollout_policy(self, T, policy, act_seed, deterministic, out):
+        from .policy import PolicyPopulation
         torch = self._torch
         N, D, dev = self.num_envs, self.obs_dim, self.device
+        population = isinstance(policy, PolicyPopulation)
+        if population:
+            policy.check_envs(N, _lib.QUAD_POLICY_CTA_ENVS)
         if policy.obs_dim != D:
             raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
         if policy.params.device != dev:
@@ -402,8 +408,13 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                 out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
         pol = policy.struct(deterministic)
         keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
-        _lib.check(self._lib.mgb_quad_rollout_policy(self._h, int(T), ctypes.byref(pol), int(act_seed),
-                                                     *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
+        outs = [_lib.ptr(out.get(k)) for k in keys]
+        if population:
+            _lib.check(self._lib.mgb_quad_rollout_population(self._h, int(T), ctypes.byref(pol), policy.members,
+                                                             policy.member_stride, int(act_seed), *outs, self._stream()))
+        else:
+            _lib.check(self._lib.mgb_quad_rollout_policy(self._h, int(T), ctypes.byref(pol), int(act_seed), *outs,
+                                                         self._stream()))
         return out
 
     @property
