@@ -575,6 +575,55 @@ int mgb_maze_rollout_rnn_population(mgb_maze *h, int32_t T, const mgb_rnn_policy
                                     double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
                                     void *stream);
 
+/* ---- value heads and GAE (DESIGN.md "Value heads and GAE") -------------------------------------------------------
+ * The *_critic entry points are the population calls (members = 1: the single policy) with a critic: the packed
+ * buffer's output layer has 5 rows, W [5][k] then b [5], rows 0..3 the actor's outputs and row 4 the value V (k: the
+ * last hidden width, the obs dim with no hidden layer, H or the head's hidden width for the recurrent head).  The
+ * quadrotor's log_std [4] still follows.  Rows 0..3, and with them every action, logp and env output, are bit for bit
+ * those of the same call on the buffer without row 4.  V is the fma chain of row 4 from its bias, like the others.
+ *   value_dev [T][n] float32 (not NULL): V(s_t) on the input step t acts on (obs0 at t = 0).
+ *   value_last_dev [n]: V(s_T) on the observation and carried state the launch leaves behind; it equals value[0] of the
+ *     next launch bit for bit when nothing touches the handle or the state in between.
+ *   final_value_dev [T][n]: V of the terminal observation, written only where the cut fires (below) on a truncated step;
+ *     other entries keep what they held.  Recurrent: the cell steps once more from the memory before the wipe (h_t, and
+ *     the LSTM's c'_t) on [terminal window, onehot(a_t), (float)r_t].
+ *   The cut is where the policy's memory is wiped: every done for an MLP and MGB_RNN_RESET_EPISODE, and where the env drew
+ *     a new maze in this launch for MGB_RNN_RESET_TASK.
+ *   adv_dev, ret_dev [T][n] (both or neither; they need rew, done, truncated and final_value): GAE(gamma, lambda) over
+ *     the launch, float32, each operation rounded to nearest, no contraction; r_t is the reward rounded once to float32.
+ *     gl = gamma lambda; for t = T-1 .. 0: nv = cut_t ? (truncated_t ? final_value_t : 0)
+ *     : (t = T-1 ? value_last : value_{t+1}); delta = (r_t + gamma nv) - v_t; A_t = delta + (cut_t ? 0 : gl A_{t+1}),
+ *     A_T = 0; ret_t = A_t + v_t.
+ *   Every other argument is the population call's.  Refused (MGB_ERR_ARG; the handle, its step counter and the state
+ *   untouched): everything the population call refuses, a NULL critic, auto_reset off, a NULL value_dev, adv / ret
+ *   without each other or without rew, done, truncated and final_value, gamma or lambda not finite or outside [0, 1],
+ *   and the footprint beyond the device's opt-in shared memory. */
+typedef struct mgb_critic {
+    float *value_dev;         /* [T][n], not NULL */
+    float *value_last_dev;    /* [n] or NULL */
+    float *final_value_dev;   /* [T][n] or NULL */
+    float *adv_dev;           /* [T][n] or NULL */
+    float *ret_dev;           /* [T][n] or NULL */
+    float gamma;              /* discount, [0, 1] */
+    float lambda;             /* GAE lambda, [0, 1] */
+} mgb_critic;
+
+int mgb_quad_rollout_critic(mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members, int64_t member_stride,
+                            uint64_t seed, float *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                            float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                            uint8_t *truncated_dev, const mgb_critic *critic, void *stream);
+int mgb_maze_rollout_critic(mgb_maze *h, int32_t T, const mgb_policy *pol, int32_t members, int64_t member_stride,
+                            uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                            int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                            double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                            const mgb_critic *critic, void *stream);
+int mgb_maze_rollout_rnn_critic(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
+                                uint64_t resample_seed, float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                                int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
+                                double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                const mgb_critic *critic, void *stream);
+
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

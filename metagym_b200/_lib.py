@@ -60,6 +60,11 @@ class RnnPolicy(ctypes.Structure):
                 ("head_width", c_i32), ("activation", c_i32), ("mode", c_i32), ("cell", c_i32)]
 
 
+class Critic(ctypes.Structure):       # mgb_critic
+    _fields_ = [("value_dev", vp), ("value_last_dev", vp), ("final_value_dev", vp), ("adv_dev", vp), ("ret_dev", vp),
+                ("gamma", ctypes.c_float), ("lam", ctypes.c_float)]
+
+
 ACT_TANH, ACT_RELU = 0, 1            # MGB_ACT_*
 POLICY_SAMPLE, POLICY_MEAN = 0, 1    # MGB_POLICY_*
 RNN_RESET_EPISODE, RNN_RESET_TASK = 0, 1     # MGB_RNN_RESET_*
@@ -90,6 +95,8 @@ SIGNATURES = {
                                                vp]),
     "mgb_quad_rollout_population": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_i32, c_i64, c_u64, vp, vp, vp,
                                                    vp, vp, vp, vp, vp, vp]),
+    "mgb_quad_rollout_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_i32, c_i64, c_u64, vp, vp, vp, vp,
+                                               vp, vp, vp, vp, ctypes.POINTER(Critic), vp]),
     "mgb_quad_state": (ctypes.c_int, [vp, vp, vp, ctypes.c_int, vp]),
     "mgb_quad_launch_count": (c_i64, [vp]),
     "mgb_quad_step_kernel": (ctypes.c_char_p, [vp]),
@@ -131,6 +138,12 @@ SIGNATURES = {
     "mgb_maze_rollout_rnn_population": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64,
                                                        ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp,
                                                        vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_rollout_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_i32, c_i64, c_u64,
+                                               ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp, vp, vp,
+                                               ctypes.POINTER(Critic), vp]),
+    "mgb_maze_rollout_rnn_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64,
+                                                   ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp, vp,
+                                                   vp, vp, vp, vp, ctypes.POINTER(Critic), vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

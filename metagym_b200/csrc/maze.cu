@@ -529,17 +529,67 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // (x, h0, c), updating c in place, and acts on head(h1), whose hidden layer goes to w (GRU) or the dead h0 (LSTM).
 // After the step the carry swaps h0 and h1 and writes (onehot(a), (float)r) into the feedback rows, or zeroes h, c and
 // the feedback where done and the reset rule fires; the state row is stored after step T - 1.
+// VAL (POL and FIN only, mgb_maze_rollout_critic / mgb_maze_rollout_rnn_critic): the head's output layer has the value
+// row.  Step t stores V(s_t).  Where the cut (the carry's wipe) fires on a truncated step, the terminal window goes into
+// the x column and the policy runs once more on it, before the wipe (the recurrent cell from h_t and c'_t with the
+// step's feedback, writing into the dead h0 column; the LSTM's head then uses the dead h1): that is final_value.  The task rule's cut is stored in adv for the epilogue.  After the loop (and after the state row is
+// stored, since the LSTM cell updates c in place) one more pass gives value_last, and the epilogue (mgb_gae) walks the
+// thread's column.
 constexpr int kPolMlp = 1, kPolGru = 2, kPolLstm = 3;
 
 template <int POL>
 using MazePolicyPlan = std::conditional_t<POL == kPolLstm, MgbRnn<4>, std::conditional_t<POL == kPolGru, MgbRnn<3>, MgbMlp>>;
 
-template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0>
-__global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
-    const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
-    const __grid_constant__ MazePolicyPlan<POL> pol)
+// VAL, step t of the thread's active env, after maze_logic and before env_reset: decides the cut from done and the
+// trial draw, stores the task rule's cut into adv, and where the cut fires on a truncated step stores V of the terminal
+// window (written into `row`, then the x column) into final_value.  Besides `row` and the x column's obs rows, which
+// the step refills, it clobbers only what the carry then wipes: the h columns, c and the feedback rows.
+template <int POL>
+__device__ __forceinline__ void maze2d_terminal_value(const MazeConst &c, const MazeArgs &a, const mgb_critic &cr,
+                                                      const MazePolicyPlan<POL> &pol, const float *pol_w, float *pol_x,
+                                                      float *pol_y, float *hid_prev, float *hid_new, float *cst,
+                                                      const uint8_t *blob, const int32_t *eaten, const Env &s, int t,
+                                                      int64_t e, int D, int done, int action, double reward,
+                                                      uint32_t draw, float *row)
 {
     constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
+    bool cut = done;
+    if constexpr (RNN) {
+        cut = done && (pol.reset == MGB_RNN_RESET_EPISODE || draw);
+        if (pol.reset == MGB_RNN_RESET_TASK && cr.adv_dev) cr.adv_dev[(int64_t)t * a.n + e] = cut ? 1.f : 0.f;
+    }
+    if (!(cut && maze_truncated(c, blob, s))) return;
+    maze2d_window(c, blob, eaten, a.n_pad, s, row);
+    for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = row[k];
+    const MgbMlp &head = mgb_policy_head(pol);
+    float logits[4], v;
+    mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
+        if constexpr (RNN) {
+            if (pol.feedback) {
+                float *fb = pol_x + D * k2dThreads + threadIdx.x;
+                for (int k = 0; k < 4; ++k) fb[k * k2dThreads] = k == action ? 1.f : 0.f;
+                fb[4 * k2dThreads] = (float)reward;
+            }
+            mgb_rnn_cell(pol, w, pol_x, hid_new, cst, hid_prev, k2dThreads, threadIdx.x);
+            mgb_mlp_forward<true>(head, w + pol.s_head, hid_prev, POL == kPolLstm ? hid_new : pol_y, k2dThreads,
+                                  threadIdx.x, logits, &v);
+        } else {
+            mgb_mlp_forward<true>(pol, w, pol_x, pol_y, k2dThreads, threadIdx.x, logits, &v);
+        }
+    });
+    if (cr.final_value_dev) cr.final_value_dev[(int64_t)t * a.n + e] = v;
+}
+
+// VAL declares a minimum of one resident CTA per SM (.minnctapersm 1; 0 emits nothing, so the other instantiations are
+// compiled as before): with ptxas's default register target the MLP kernel without RS spilled 8 bytes and the LSTM one
+// with RS 84 bytes, where their value-less counterparts do not spill; with it none spills.
+template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0, bool VAL = false>
+__global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel(
+    const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
+    const __grid_constant__ MazePolicyPlan<POL> pol, const __grid_constant__ mgb_critic cr)
+{
+    constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
+    static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
     static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
     const int64_t e0 = (int64_t)blockIdx.x * k2dThreads;
@@ -612,7 +662,7 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
         if (active) {
             int action;
             if constexpr (POL) {
-                float logits[4];
+                float logits[4], v;
                 mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
                     if constexpr (RNN) {
                         mgb_rnn_cell(pol, w, pol_x, hid_prev, cst, hid_new, k2dThreads, threadIdx.x);
@@ -620,14 +670,15 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                             for (int k = 0; k < pol.H; ++k)
                                 pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * k2dThreads + threadIdx.x];
                         if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
-                        mgb_mlp_forward(head, w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits);
+                        mgb_mlp_forward<VAL>(head, w + pol.s_head, hid_new, pol_y, k2dThreads, threadIdx.x, logits, &v);
                     } else {
-                        mgb_mlp_forward(pol, w, pol_x, pol_y, k2dThreads, threadIdx.x, logits);
+                        mgb_mlp_forward<VAL>(pol, w, pol_x, pol_y, k2dThreads, threadIdx.x, logits, &v);
                     }
                 });
                 const float lp = mgb_categorical_action(head, genv, a.t_base + (uint32_t)t, logits, action);
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
                 if (head.logp_out) head.logp_out[(int64_t)t * a.n + e] = lp;
+                if constexpr (VAL) cr.value_dev[(int64_t)t * a.n + e] = v;
             } else if (a.act) action = a.act[(int64_t)t * a.n + e];
             else {
                 const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
@@ -648,8 +699,13 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
                 if (done && a.final_obs)
                     maze2d_window(c, blob, eaten, a.n_pad, s, reinterpret_cast<float *>(a.final_obs) + ((int64_t)t * a.n + e) * D);
             }
+            if constexpr (VAL) {    // the cut needs the trial draw before the reset
+                if (RS && done) draw = (uint32_t)rs_draws(rs, tcount);
+                maze2d_terminal_value<POL>(c, a, cr, pol, pol_w, pol_x, pol_y, hid_prev, hid_new, cst, blob, eaten, s, t,
+                                           e, D, done, action, reward, draw, tile + threadIdx.x * D);
+            }
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
-            if (RS && done) draw = (uint32_t)rs_draws(rs, tcount);
+            if (!VAL && RS && done) draw = (uint32_t)rs_draws(rs, tcount);
             if (REC) path_store(c, a, e, s);
             if (a.rew) {
                 if (XM == 2) mgb_mc_st(mgb_shift(a.rew + (int64_t)t * a.n + e, a.mir.delta[0]), reward);
@@ -781,6 +837,24 @@ __global__ void __launch_bounds__(k2dThreads) maze2d_rollout_kernel(
             for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * k2dThreads + threadIdx.x];
             for (int k = 0; k < pol.C(); ++k) st[pol.H + k] = cst[k * k2dThreads + threadIdx.x];
             for (int k = pol.HC(); k < S; ++k) st[k] = pol_x[(D + k - pol.HC()) * k2dThreads + threadIdx.x];
+        }
+    }
+    if constexpr (VAL) {
+        if (active) {       // V(s_T), then GAE over the thread's column
+            float logits[4], v;
+            mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
+                if constexpr (RNN) {
+                    mgb_rnn_cell(pol, w, pol_x, hid_prev, cst, hid_new, k2dThreads, threadIdx.x);
+                    mgb_mlp_forward<true>(head, w + pol.s_head, hid_new, POL == kPolLstm ? hid_prev : pol_y, k2dThreads,
+                                          threadIdx.x, logits, &v);
+                } else {
+                    mgb_mlp_forward<true>(pol, w, pol_x, pol_y, k2dThreads, threadIdx.x, logits, &v);
+                }
+            });
+            if (cr.value_last_dev) cr.value_last_dev[e] = v;
+            bool task_rule = false;
+            if constexpr (RNN) task_rule = pol.reset == MGB_RNN_RESET_TASK;
+            if (cr.adv_dev) mgb_gae(cr, a.T, a.n, e, v, a.rew, a.done, a.truncated, task_rule);
         }
     }
     if constexpr (RS) {
@@ -4189,8 +4263,8 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
             MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false, REC, true>));
             MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC, true>));
         }
-        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{});
-        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{});
+        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{}, mgb_critic{});
+        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{}, mgb_critic{});
         MGB_CUDA(cudaGetLastError());
         return MGB_OK;
     }
@@ -4201,10 +4275,10 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC>));
     }
     const MazeResample none = {};
-    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
-    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
-    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
-    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{});
+    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
+    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
+    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
+    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -4333,11 +4407,15 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
 
 // maze2d_rollout_kernel<0, fin, REC, RS, POL>, sm bytes of dynamic shared memory; refused (as `fn`) when the CTA would
 // need more shared memory than the device allows
+// (with a critic: maze2d_rollout_kernel<0, true, REC, RS, POL, true>)
 template <bool REC, bool RS, int POL>
 static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r,
-                            const MazePolicyPlan<POL> &m, unsigned blocks, size_t sm, cudaStream_t st)
+                            const MazePolicyPlan<POL> &m, unsigned blocks, size_t sm, cudaStream_t st,
+                            const mgb_critic *critic)
 {
-    const auto kernel = fin ? maze2d_rollout_kernel<0, true, REC, RS, POL> : maze2d_rollout_kernel<0, false, REC, RS, POL>;
+    const auto kernel = critic ? maze2d_rollout_kernel<0, true, REC, RS, POL, true>
+                        : fin  ? maze2d_rollout_kernel<0, true, REC, RS, POL>
+                               : maze2d_rollout_kernel<0, false, REC, RS, POL>;
     int optin = 0;
     MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
     cudaFuncAttributes fa;
@@ -4350,7 +4428,7 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
         return MGB_ERR_ARG;
     }
     MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m);
+    kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m, critic ? *critic : mgb_critic{});
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -4361,12 +4439,14 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
 // in the mean mode, mirrors, resampling, the
 // optional outputs and the handle's state.  The policy's region of dynamic shared memory follows the tiles and the
 // sampler workspaces.
+// A critic (the *_critic entry points, whose own() plans the value row; null for the others) is checked last.
 template <int POL, class Own>
 static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolicyPlan<POL> &pol, Own own,
                                int32_t members, int64_t member_stride, uint64_t seed,
                                const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, int32_t *act_out_dev,
                                float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev,
-                               uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+                               uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream,
+                               bool val = false, const mgb_critic *critic = nullptr)
 {
     MgbMlp &head = mgb_policy_head(pol);
     SamplerCfg sc;
@@ -4380,9 +4460,13 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
         if (logp_out_dev && head.mode != MGB_POLICY_SAMPLE) return "logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)";
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
-        if (!resample_cfg) return trial_needs_done(h, done_dev);
-        if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout
-        return sampler_cfg(h, resample_cfg, sc);
+        if (!resample_cfg) {
+            if (const char *why = trial_needs_done(h, done_dev)) return why;
+        } else {
+            if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout
+            if (const char *why = sampler_cfg(h, resample_cfg, sc)) return why;
+        }
+        return val ? mgb_critic_check(critic, h->auto_reset, rew_dev, done_dev, truncated_dev) : nullptr;
     });
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
@@ -4406,12 +4490,13 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolic
     const bool fin = final_obs_dev || truncated_dev;
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     const cudaStream_t st = (cudaStream_t)stream;
+    const mgb_critic *cr = val ? critic : nullptr;
     if (resample_cfg)
-        rc = h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st)
-                     : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st);
+        rc = h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr)
+                     : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr);
     else
-        rc = h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st)
-                     : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st);
+        rc = h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr)
+                     : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr);
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
@@ -4423,13 +4508,13 @@ static int maze_rollout_mlp(const char *fn, mgb_maze *h, int32_t T, const mgb_po
                             int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
                             uint64_t resample_seed, int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
                             float *obs_dev, double *rew_dev, uint8_t *done_dev, float *final_obs_dev,
-                            uint8_t *truncated_dev, void *stream)
+                            uint8_t *truncated_dev, void *stream, bool val = false, const mgb_critic *critic = nullptr)
 {
     MgbMlp m;
-    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m); };
+    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m, val); };
     return maze_rollout_policy<kPolMlp>(fn, h, T, m, own, members, member_stride, seed, resample_cfg, resample_seed,
                                         act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
-                                        final_obs_dev, truncated_dev, stream);
+                                        final_obs_dev, truncated_dev, stream, val, critic);
 }
 
 extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
@@ -4460,14 +4545,14 @@ static int maze_rollout_rnn(const char *fn, mgb_maze *h, int32_t T, const mgb_rn
                             uint64_t resample_seed, float *state_dev, float *state0_out_dev, float *hid_out_dev,
                             int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
                             double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
-                            void *stream)
+                            void *stream, bool val = false, const mgb_critic *critic = nullptr)
 {
     // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
     const auto run = [&](auto kind) {
         constexpr int POL = decltype(kind)::value;
         MazePolicyPlan<POL> p;
         const auto own = [&](int obs_dim) -> const char * {
-            if (const char *why = mgb_rnn_plan(pol, obs_dim, p)) return why;
+            if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val)) return why;
             p.state = state_dev;
             p.state0_out = state0_out_dev;
             p.hid_out = hid_out_dev;
@@ -4478,7 +4563,7 @@ static int maze_rollout_rnn(const char *fn, mgb_maze *h, int32_t T, const mgb_rn
         };
         return maze_rollout_policy<POL>(fn, h, T, p, own, members, member_stride, seed, resample_cfg, resample_seed,
                                         act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
-                                        final_obs_dev, truncated_dev, stream);
+                                        final_obs_dev, truncated_dev, stream, val, critic);
     };
     return pol && pol->cell == MGB_RNN_CELL_LSTM ? run(std::integral_constant<int, kPolLstm>{})
                                                  : run(std::integral_constant<int, kPolGru>{});
@@ -4509,6 +4594,33 @@ extern "C" int mgb_maze_rollout_rnn_population(mgb_maze *h, int32_t T, const mgb
     return maze_rollout_rnn(__func__, h, T, pol, members, member_stride, seed, resample_cfg, resample_seed, state_dev,
                             state0_out_dev, hid_out_dev, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
                             done_dev, final_obs_dev, truncated_dev, stream);
+}
+
+extern "C" int mgb_maze_rollout_critic(mgb_maze *h, int32_t T, const mgb_policy *pol, int32_t members,
+                                       int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
+                                       uint64_t resample_seed, int32_t *act_out_dev, float *logp_out_dev,
+                                       float *obs0_out_dev, float *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                       float *final_obs_dev, uint8_t *truncated_dev, const mgb_critic *critic,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_critic");
+    return maze_rollout_mlp(__func__, h, T, pol, members, member_stride, seed, resample_cfg, resample_seed, act_out_dev,
+                            logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream,
+                            true, critic);
+}
+
+extern "C" int mgb_maze_rollout_rnn_critic(mgb_maze *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                           int64_t member_stride, uint64_t seed,
+                                           const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed,
+                                           float *state_dev, float *state0_out_dev, float *hid_out_dev,
+                                           int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                           float *obs_dev, double *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                                           uint8_t *truncated_dev, const mgb_critic *critic, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_rnn_critic");
+    return maze_rollout_rnn(__func__, h, T, pol, members, member_stride, seed, resample_cfg, resample_seed, state_dev,
+                            state0_out_dev, hid_out_dev, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
+                            done_dev, final_obs_dev, truncated_dev, stream, true, critic);
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)

@@ -5,8 +5,9 @@
 // memory once per launch, regrouped so that a hidden layer's outputs are computed eight at a time: for output group g
 // and input i the eight weights W[8g .. 8g+7][i] are two consecutive float4, read by the whole warp as a broadcast, and
 // the thread's input x[i] is one conflict-free load from its own column of the activation buffers ([k][blockDim.x]).
-// The output layer (4 wide) is staged in groups of four.  Rows past a layer's width are zero.  Every output is a
-// fused multiply-add chain that starts at the bias and runs over the inputs in index order, in float32.
+// The output layer (4 wide, or 5 with a value head: row 4 is the critic's V) is staged in groups of four, so 5 rows pad
+// to 8.  Rows past a layer's width are zero.  Every output is a fused multiply-add chain that starts at the bias and runs
+// over the inputs in index order, in float32, so rows 0..3 do not depend on whether row 4 exists.
 #pragma once
 #include <type_traits>
 #include "mgb_common.cuh"
@@ -38,9 +39,10 @@ struct MgbMlp {
 };
 
 // Host: validate `p` and plan it for input width `in_dim` (output width 4; `log_std`: the buffer ends with log_std[4],
-// the Gaussian head of the quadrotor; without it the four outputs are the logits of the maze's categorical head).
+// the Gaussian head of the quadrotor; without it the four outputs are the logits of the maze's categorical head;
+// `value`: the output layer has a fifth row, the value head of the critic entry points).
 // Returns null, or the reason the policy is refused.
-static inline const char *mgb_mlp_plan(const mgb_policy *p, int in_dim, bool log_std, MgbMlp &m)
+static inline const char *mgb_mlp_plan(const mgb_policy *p, int in_dim, bool log_std, MgbMlp &m, bool value = false)
 {
     if (!p) return "null policy";
     if (!p->params_dev) return "null params_dev";
@@ -58,7 +60,7 @@ static inline const char *mgb_mlp_plan(const mgb_policy *p, int in_dim, bool log
     for (int l = 0; l < m.n_layers; ++l) {
         const bool last = l == m.n_layers - 1;
         m.in[l] = l == 0 ? in_dim : p->width[l - 1];
-        m.out[l] = last ? 4 : p->width[l];
+        m.out[l] = last ? (value ? 5 : 4) : p->width[l];
         if (!last && m.out[l] > maxw) maxw = m.out[l];
         const int gwid = last ? 4 : 8, rows = (m.out[l] + gwid - 1) / gwid * gwid;
         m.gw[l] = g;
@@ -115,9 +117,11 @@ __device__ __forceinline__ float mgb_mlp_activate(int activation, float x)
 }
 
 // Device: forward pass of the thread's env.  Its input x[i] is a0[i * stride + col], i < m.in[0]; a0 and a1 are the
-// two activation buffers (each m.maxw rows of `stride` floats), both clobbered.  out4 receives the four outputs.
+// two activation buffers (each m.maxw rows of `stride` floats), both clobbered.  out4 receives the four outputs, and
+// with VAL (a plan of 5 outputs) *value receives the fifth, the first row of the output layer's second group.
+template <bool VAL = false>
 __device__ __forceinline__ void mgb_mlp_forward(const MgbMlp &m, const float *sm, float *a0, float *a1, int stride,
-                                                int col, float out4[4])
+                                                int col, float out4[4], float *value = nullptr)
 {
     const float *x = a0 + col;
     float *y = a1 + col;
@@ -150,15 +154,19 @@ __device__ __forceinline__ void mgb_mlp_forward(const MgbMlp &m, const float *sm
     const float4 *W = reinterpret_cast<const float4 *>(sm + m.sw[l]);
     const float4 b = *reinterpret_cast<const float4 *>(sm + m.sb[l]);
     float acc[4] = {b.x, b.y, b.z, b.w};
+    float accv = 0.f;
+    if constexpr (VAL) accv = sm[m.sb[l] + 4];
 #pragma unroll 4
     for (int i = 0; i < in; ++i) {
         const float xi = x[i * stride];
         const float4 w = W[i];
         acc[0] = fmaf(w.x, xi, acc[0]); acc[1] = fmaf(w.y, xi, acc[1]);
         acc[2] = fmaf(w.z, xi, acc[2]); acc[3] = fmaf(w.w, xi, acc[3]);
+        if constexpr (VAL) accv = fmaf(sm[m.sw[l] + 4 * (in + i)], xi, accv);
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) out4[k] = acc[k];
+    if constexpr (VAL) *value = accv;
 }
 
 // Device: Gaussian action of env genv at step counter t from the policy mean (MGB_POLICY_SAMPLE), or the mean itself
@@ -291,9 +299,10 @@ static inline const char *mgb_rnn_check(const mgb_rnn_policy *p)
     return nullptr;
 }
 
-// Host: validate `p` and plan it for observation width `obs_dim`.  Returns null, or the reason the policy is refused.
+// Host: validate `p` and plan it for observation width `obs_dim` (`value`: the head's output layer has the value row).
+// Returns null, or the reason the policy is refused.
 template <int NG>
-static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, MgbRnn<NG> &r)
+static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, MgbRnn<NG> &r, bool value = false)
 {
     if (const char *why = mgb_rnn_check(p)) return why;
     r = MgbRnn<NG>{};
@@ -313,7 +322,7 @@ static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, Mgb
     r.s_head = r.s_b + 2 * NG * r.Hp;
     const mgb_policy hp = {p->params_dev + r.g_b + 2 * NG * r.H, p->head_hidden, {p->head_width, 0, 0}, p->activation,
                            p->mode};
-    if (const char *why = mgb_mlp_plan(&hp, r.H, false, r.head)) return why;
+    if (const char *why = mgb_mlp_plan(&hp, r.H, false, r.head, value)) return why;
     r.staged = r.s_head + r.head.staged;
     r.head.packed += r.g_b + 2 * NG * r.H;
     return nullptr;
@@ -405,6 +414,52 @@ __device__ __forceinline__ void mgb_population_weights(const MgbMlp &head, const
     } else {
         f(sm + ((int)threadIdx.x >> head.member_shift) * staged);
         asm volatile("");
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Value heads and GAE (DESIGN.md "Value heads and GAE", header "value heads and GAE")
+// ---------------------------------------------------------------------------------------------------------------
+
+// Host: the checks of a critic (header "value heads and GAE") that the entry point's own checks do not make.  Returns
+// null, or the reason the call is refused.
+static inline const char *mgb_critic_check(const mgb_critic *cr, bool auto_reset, const void *rew, const void *done,
+                                           const void *truncated)
+{
+    if (!cr) return "null critic";
+    if (!auto_reset) return "a critic needs auto_reset on (the value of a finished env's next state is a new episode's)";
+    if (!cr->value_dev) return "null value_dev";
+    if (!cr->adv_dev != !cr->ret_dev) return "adv_dev and ret_dev go together";
+    if (cr->adv_dev && !(rew && done && truncated && cr->final_value_dev))
+        return "adv / ret need rew, done, truncated and final_value";
+    if (!(cr->gamma >= 0.f && cr->gamma <= 1.f)) return "gamma must be finite and in [0, 1]";
+    if (!(cr->lambda >= 0.f && cr->lambda <= 1.f)) return "lambda must be finite and in [0, 1]";
+    return nullptr;
+}
+
+// Device: GAE(gamma, lambda) of the thread's env e, walking its column backwards from v_last = V(s_T).  It reads back
+// only what the thread itself stored in this launch with ordinary stores (rew, done, truncated, value, final_value, and
+// with cut_in_adv the cut flags the loop left in adv), so no fence is needed.  Every operation is rounded to nearest
+// with no contraction, so that a float32 NumPy restatement is bit exact.
+template <class R>
+__device__ __forceinline__ void mgb_gae(const mgb_critic &cr, int T, int64_t n, int64_t e, float v_last, const R *rew,
+                                        const uint8_t *done, const uint8_t *truncated, bool cut_in_adv)
+{
+    const float gamma = cr.gamma, gl = __fmul_rn(cr.gamma, cr.lambda);
+    float nv_next = v_last, A = 0.f;
+    for (int t = T - 1; t >= 0; --t) {
+        const int64_t i = (int64_t)t * n + e;
+        const float v = cr.value_dev[i];
+        const bool cut = cut_in_adv ? cr.adv_dev[i] != 0.f : done[i] != 0;
+        const float nv = cut ? (truncated[i] ? cr.final_value_dev[i] : 0.f) : nv_next;
+        float r;
+        if constexpr (std::is_same_v<R, double>) r = __double2float_rn(rew[i]);
+        else r = rew[i];
+        const float delta = __fsub_rn(__fadd_rn(r, __fmul_rn(gamma, nv)), v);
+        A = __fadd_rn(delta, cut ? 0.f : __fmul_rn(gl, A));
+        cr.adv_dev[i] = A;
+        if (cr.ret_dev) cr.ret_dev[i] = __fadd_rn(A, v);
+        nv_next = v;
     }
 }
 

@@ -1152,11 +1152,16 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 // CTA: the one member of a population that drives the CTA's envs, or its pol.copies members back to back, each warp
 // reading its own (mgb_population_stage).  The step arithmetic after the action is the code the other instantiations
 // run.
-template <bool SIMPLE, int XM, bool FIN, bool POL = false>
+// VAL (POL and FIN only, mgb_quad_rollout_critic): the output layer has the value row (mgb_mlp_forward<true>).  Step t
+// stores V(s_t); a truncated step's terminal observation o[] goes through the policy once more before observe_reset
+// (final_value); after the loop one more pass gives value_last, and the epilogue (mgb_gae) walks the thread's column.
+template <bool SIMPLE, int XM, bool FIN, bool POL = false, bool VAL = false>
 __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(const __grid_constant__ QuadConst c,
                                                                           const __grid_constant__ QuadArgs a,
-                                                                          const __grid_constant__ MgbMlp pol)
+                                                                          const __grid_constant__ MgbMlp pol,
+                                                                          const __grid_constant__ mgb_critic cr)
 {
+    static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
     __shared__ __align__(128) float tiles[2][kThreads * kMaxObs];
     const int64_t e0 = (int64_t)blockIdx.x * kThreads;
     const int64_t e = e0 + threadIdx.x;
@@ -1210,11 +1215,12 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
         if (active) {
             float4 act;
             if constexpr (POL) {
-                float mean[4], av[4], lp;
+                float mean[4], av[4], lp, v;
                 mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
-                    mgb_mlp_forward(pol, w, pol_x, pol_y, kThreads, threadIdx.x, mean);
+                    mgb_mlp_forward<VAL>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, mean, &v);
                     lp = mgb_gaussian_action(pol, w, genv, a.t_base + (uint32_t)t, mean, av);
                 });
+                if constexpr (VAL) cr.value_dev[(int64_t)t * a.n + e] = v;
                 act = make_float4(av[0], av[1], av[2], av[3]);
                 if (a.act_out) reinterpret_cast<float4 *>(a.act_out)[(int64_t)t * a.n + e] = act;
                 if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
@@ -1257,6 +1263,19 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
                     if (D == 19) { frow[16] = o[16]; frow[17] = o[17]; frow[18] = o[18]; }
                 }
             }
+            if constexpr (VAL) {
+                // the cut is every done (auto_reset is on): V of the terminal observation where it was truncated
+                if (wf[0] && trunc[0]) {
+#pragma unroll
+                    for (int k = 0; k < kMaxObs; ++k)
+                        if (k < D) pol_x[k * kThreads + threadIdx.x] = o[k];
+                    float out4[4], v;
+                    mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
+                        mgb_mlp_forward<true>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, out4, &v);
+                    });
+                    if (cr.final_value_dev) cr.final_value_dev[(int64_t)t * a.n + e] = v;
+                }
+            }
             if (wf[0]) {
                 observe_reset(c, a, task, s, 0, o);
                 adjugate(s.R, adj, id);
@@ -1297,6 +1316,16 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
         }
     }
     if (active) store_state(a, e, s);
+    if constexpr (VAL) {
+        if (active) {
+            float out4[4], v;
+            mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
+                mgb_mlp_forward<true>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, out4, &v);
+            });
+            if (cr.value_last_dev) cr.value_last_dev[e] = v;
+            if (cr.adv_dev) mgb_gae(cr, a.T, a.n, e, v, a.rew, a.done, a.truncated, false);
+        }
+    }
     if (threadIdx.x == 0) mgb_bulk_wait_read<0>();   // smem must outlive the copy; the kernel boundary flushes the writes
 }
 
@@ -1829,18 +1858,19 @@ static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_se
         return xm == 2 ? quad_rollout_kernel<simple, 2, false> : xm == 1 ? quad_rollout_kernel<simple, 1, false>
                : fin   ? quad_rollout_kernel<simple, 0, true>  : quad_rollout_kernel<simple, 0, false>;
     });
-    kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a, MgbMlp{});
+    kernel<<<blocks, kThreads, 0, (cudaStream_t)stream>>>(h->c, a, MgbMlp{}, mgb_critic{});
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
 }
 
-// A policy rollout of `members` policies (one: mgb_quad_rollout_policy), refused as `fn`
+// A policy rollout of `members` policies (one: mgb_quad_rollout_policy), refused as `fn`; with a critic (the value
+// heads of mgb_quad_rollout_critic, null for the other entry points) the policy has the value row
 static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
                           int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
                           float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
-                          uint8_t *truncated_dev, void *stream)
+                          uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
 {
     const auto refuse = [&](const char *why) {
         mgb_set_error("%s: %s", fn, why);
@@ -1849,7 +1879,7 @@ static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_poli
     if (!h) return refuse("null handle");
     if (T <= 0) return refuse("T must be positive");
     MgbMlp m;
-    if (const char *why = mgb_mlp_plan(pol, h->c.obs_dim, true, m)) return refuse(why);
+    if (const char *why = mgb_mlp_plan(pol, h->c.obs_dim, true, m, val)) return refuse(why);
     if (const char *why = mgb_population_plan(m, h->n, members, member_stride, kThreads)) return refuse(why);
     if (logp_out_dev && m.mode != MGB_POLICY_SAMPLE)
         return refuse("logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)");
@@ -1859,6 +1889,9 @@ static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_poli
         return refuse("final_obs needs auto_reset on (without it obs already is the terminal observation)");
     if ((reinterpret_cast<uintptr_t>(act_out_dev) & 15u) != 0) return refuse("act_out_dev must be 16-byte aligned");
     if ((reinterpret_cast<uintptr_t>(pol->params_dev) & 3u) != 0) return refuse("params_dev must be 4-byte aligned");
+    if (val) {
+        if (const char *why = mgb_critic_check(critic, h->auto_reset, rew_dev, done_dev, truncated_dev)) return refuse(why);
+    }
     int rc = check_ready(h);
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
@@ -1867,7 +1900,8 @@ static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_poli
     m.obs0_out = obs0_out_dev;
     const bool fin = final_obs_dev || truncated_dev;
     const auto kernel = with_simple(h, [&](auto simple) {
-        return fin ? quad_rollout_kernel<simple, 0, true, true> : quad_rollout_kernel<simple, 0, false, true>;
+        return val ? quad_rollout_kernel<simple, 0, true, true, true>
+               : fin ? quad_rollout_kernel<simple, 0, true, true> : quad_rollout_kernel<simple, 0, false, true>;
     });
     const size_t smem = mgb_mlp_smem_bytes(m, kThreads);
     int optin = 0;
@@ -1885,7 +1919,7 @@ static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_poli
     a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
     a.final_obs = final_obs_dev; a.truncated = truncated_dev;
     const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
-    kernel<<<blocks, kThreads, smem, (cudaStream_t)stream>>>(h->c, a, m);
+    kernel<<<blocks, kThreads, smem, (cudaStream_t)stream>>>(h->c, a, m, val ? *critic : mgb_critic{});
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;
@@ -1909,6 +1943,17 @@ extern "C" int mgb_quad_rollout_population(mgb_quad *h, int32_t T, const mgb_pol
     MgbRange nvtx_range("mgb_quad_rollout_population");
     return rollout_policy(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
                           obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
+}
+
+extern "C" int mgb_quad_rollout_critic(mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
+                                       int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
+                                       float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                                       float *final_obs_dev, uint8_t *truncated_dev, const mgb_critic *critic,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_critic");
+    return rollout_policy(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
+                          obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream, critic, true);
 }
 
 extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,

@@ -737,7 +737,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         return cfg
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, resample=None, policy=None,
-                deterministic=False, state=None, want_hidden=False):
+                deterministic=False, state=None, want_hidden=False, gae=None):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
         {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None).
 
@@ -772,7 +772,15 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
 
         policy may also be a PolicyPopulation of any of the three kinds (mgb_maze_rollout_population,
         mgb_maze_rollout_rnn_population): member m drives the envs [m E, (m + 1) E), E = N / members, which must be
-        32, 64 or a multiple of 128; a recurrent population takes state= as its members would."""
+        32, 64 or a multiple of 128; a recurrent population takes state= as its members would.
+
+        A policy or population with a value head (value=nn.Linear(k, 1); mgb_maze_rollout_critic,
+        mgb_maze_rollout_rnn_critic; needs auto_reset=True) also yields "value" [T,N] float32 (V on the input step t
+        acts on), "value_last" [N] (V after the last step, with the carried state the launch leaves: the next launch's
+        value[0]) and, with final_obs=True or gae, "final_value" [T,N]: V of the terminal window where an episode ended
+        truncated and the policy's memory is wiped (every done, or new_tasks(out) under hidden_reset="task"), from the
+        memory before the wipe; other entries are not written.  gae=(gamma, lam) also yields "adv" and "ret" [T,N]
+        float32, GAE(gamma, lam) cut where the memory is wiped (DESIGN.md "Value heads and GAE")."""
         from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
         recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation)
                                                                       and policy.recurrent)
@@ -784,11 +792,15 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
-            return self._rollout_policy(T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden)
+            return self._rollout_policy(T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden,
+                                        gae)
+        if gae is not None:
+            raise ValueError("gae= needs a policy with a value head")
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
 
-    def _rollout_policy(self, T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden):
-        from .policy import PolicyPopulation
+    def _rollout_policy(self, T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden,
+                        gae=None):
+        from .policy import PolicyPopulation, critic_args, critic_struct
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")
         torch = self._torch
@@ -805,6 +817,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
                               and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
             raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
+        critic = critic_args(policy, gae)
         if out is None:
             out = {"obs": torch.empty((T, N) + shape, dtype=torch.float32, device=dev),
                    "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
@@ -824,16 +837,23 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
         self._trial_entries(out, resample)
         pol = policy.struct(deterministic)
-        args = [self._h, T, ctypes.byref(pol)] + ([policy.members, policy.member_stride] if population else [])
+        tail = []
+        if critic is not None:
+            tail = [ctypes.byref(critic_struct(torch, out, T, N, dev, critic, self._want_final))]
+            members = [policy.members, policy.member_stride] if population else [1, 0]
+            entry = self._lib.mgb_maze_rollout_rnn_critic if recurrent else self._lib.mgb_maze_rollout_critic
+        elif population:
+            members = [policy.members, policy.member_stride]
+            entry = self._lib.mgb_maze_rollout_rnn_population if recurrent else self._lib.mgb_maze_rollout_population
+        else:
+            members = []
+            entry = self._lib.mgb_maze_rollout_rnn if recurrent else self._lib.mgb_maze_rollout_policy
+        args = [self._h, T, ctypes.byref(pol)] + members
         args += [int(act_seed), None if cfg is None else ctypes.byref(cfg), seed]
         if recurrent:
             args += [_lib.ptr(state), _lib.ptr(out.get("state0")), _lib.ptr(out.get("hid"))]
         keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
-        if population:
-            entry = self._lib.mgb_maze_rollout_rnn_population if recurrent else self._lib.mgb_maze_rollout_population
-        else:
-            entry = self._lib.mgb_maze_rollout_rnn if recurrent else self._lib.mgb_maze_rollout_policy
-        _lib.check(entry(*args, *[_lib.ptr(out.get(k)) for k in keys], self._stream()))
+        _lib.check(entry(*args, *[_lib.ptr(out.get(k)) for k in keys], *tail, self._stream()))
         return out
 
     def save_trajectory(self, file_name, envs=None, additional=None):

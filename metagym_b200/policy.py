@@ -12,6 +12,11 @@ GRUPolicy and LSTMPolicy pack an ``nn.GRUCell`` or an ``nn.LSTMCell`` and a head
 head's layers as MLPPolicy packs them.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities
 through the torch modules.
 
+Each of the three takes an optional value head, value = nn.Linear(k, 1) reading what the output layer reads: the
+critic of the *_critic entry points (DESIGN.md "Value heads and GAE").  It packs as a fifth row of the output layer,
+W [5][k] then b [5] (torch.cat of the actor's rows and the critic's), so the rollouts also return V(s_t), the bootstrap
+values and, on request, GAE advantages.
+
 PolicyPopulation holds M policies of one shape as the rows of one [M, numel] device tensor, and one rollout launch
 drives each block of num_envs / M envs with its own member (DESIGN.md "Populations").
 """
@@ -53,6 +58,26 @@ def _layers(module):
     return lin, act
 
 
+def _value_head(value, k, name):
+    """value (an nn.Linear(k, 1)) or None; ValueError for anything else."""
+    import torch.nn as nn
+    if value is None:
+        return None
+    if type(value) is not nn.Linear or value.out_features != 1 or value.in_features != k:
+        raise ValueError("%s: value must be an nn.Linear(%d, 1) reading what the output layer reads" % (name, k))
+    return value
+
+
+def _cat_value(W, b, value):
+    """The output layer W [4][k], b [4] (float64) with the value row appended when there is one."""
+    import torch
+    if value is None:
+        return W, b
+    f64 = lambda t: t.detach().to("cpu", torch.float64)          # noqa: E731
+    bv = f64(value.bias) if value.bias is not None else torch.zeros(1, dtype=torch.float64)
+    return torch.cat([W, f64(value.weight)], 0), torch.cat([b, bv])
+
+
 class MLPPolicy(object):
     """A torch MLP packed for the fused policy rollouts.
 
@@ -60,17 +85,21 @@ class MLPPolicy(object):
     width 1..64, ending in a Linear with 4 outputs.  log_std: [4] log standard deviations of the quadrotor's Gaussian
     policy (None: no stochastic quadrotor rollouts).  obs_mean / obs_std: optional [obs_dim] observation normalisation
     (x - mean) / std, folded into the first layer's W and b on the host in float64.  device: where the packed buffer
-    lives (the env's CUDA device).
+    lives (the env's CUDA device).  value: an optional nn.Linear(k, 1) value head, k the last hidden width (obs_dim
+    with no hidden layer); it packs as row 4 of the output layer, where the normalisation folds into it too.
     """
 
-    def __init__(self, module, log_std=None, obs_mean=None, obs_std=None, device="cuda"):
+    def __init__(self, module, log_std=None, obs_mean=None, obs_std=None, device="cuda", value=None):
         import torch
         self._torch = torch
         lin, self.activation = _layers(module)
         self.obs_dim = lin[0].in_features
         self.widths = [m.out_features for m in lin[:-1]]
         self.n_hidden = len(self.widths)
-        self.numel = sum(m.out_features * (m.in_features + 1) for m in lin) + N_OUT
+        self._value = _value_head(value, lin[-1].in_features, "MLPPolicy")
+        self.has_value = self._value is not None
+        self.numel = (sum(m.out_features * (m.in_features + 1) for m in lin) + N_OUT
+                      + (lin[-1].in_features + 1 if self.has_value else 0))
         self.device = torch.device(device)
         self.params = torch.zeros(self.numel, dtype=torch.float32, device=self.device)
         self.has_log_std = False
@@ -92,6 +121,8 @@ class MLPPolicy(object):
             W = m.weight.detach().to("cpu", torch.float64)
             b = m.bias.detach().to("cpu", torch.float64) if m.bias is not None else torch.zeros(m.out_features,
                                                                                                 dtype=torch.float64)
+            if k == len(lin) - 1:
+                W, b = _cat_value(W, b, self._value)
             if k == 0 and (self._mean is not None or self._std is not None):
                 mean = self._mean if self._mean is not None else torch.zeros(self.obs_dim, dtype=torch.float64)
                 std = self._std if self._std is not None else torch.ones(self.obs_dim, dtype=torch.float64)
@@ -102,14 +133,19 @@ class MLPPolicy(object):
         parts.append(self._log_std if self._log_std is not None else torch.zeros(N_OUT, dtype=torch.float64))
         return torch.cat(parts).to(torch.float32)
 
-    def update(self, module=None, log_std=None, obs_mean=None, obs_std=None):
+    def update(self, module=None, log_std=None, obs_mean=None, obs_std=None, value=None):
         """Repack into the same device buffer (copy_, stream-ordered): a graph captured on this policy sees the new
-        weights.  Arguments left None keep their previous values; the module must keep its layer shapes."""
+        weights.  Arguments left None keep their previous values; the module must keep its layer shapes, and a value
+        head can only replace the policy's own."""
         if module is not None:
             lin, act = _layers(module)
             if (lin[0].in_features != self.obs_dim or [m.out_features for m in lin[:-1]] != self.widths
                     or act != self.activation):
                 raise ValueError("MLPPolicy.update: the module must keep the layer shapes and the activation")
+        if value is not None:
+            if not self.has_value:
+                raise ValueError("MLPPolicy.update: this policy was built without a value head")
+            _value_head(value, self.widths[-1] if self.widths else self.obs_dim, "MLPPolicy")
         if log_std is not None:
             self._vec(log_std, N_OUT, "log_std")
         # normalisation is checked before anything changes: a zero or non-finite std would fold into inf / NaN weights
@@ -128,8 +164,29 @@ class MLPPolicy(object):
             self._mean = mean
         if std is not None:
             self._std = std
+        if value is not None:
+            self._value = value
         self.params.copy_(self.pack(), non_blocking=False)
         return self
+
+    def evaluate(self, obs):
+        """(out [..., 4], value [...]) of observations obs [..., obs_dim] through the torch modules, with the
+        observation normalisation, in the module's dtype and device (autograd flows): the reference of the value
+        the critic rollouts return, and what a PPO update evaluates."""
+        if not self.has_value:
+            raise ValueError("MLPPolicy.evaluate needs a value head")
+        torch = self._torch
+        lin, _ = _layers(self._module)
+        w = lin[0].weight
+        x = torch.as_tensor(obs).to(w.device, w.dtype)
+        if self._mean is not None:
+            x = x - self._mean.to(w.device, w.dtype)
+        if self._std is not None:
+            x = x / self._std.to(w.device, w.dtype)
+        mods = list(self._module)
+        for m in mods[:-1]:
+            x = m(x)
+        return mods[-1](x), self._value(x)[..., 0]
 
     def struct(self, deterministic=False):
         """The mgb_policy the C entry points take."""
@@ -168,7 +225,7 @@ class _RecurrentPolicy(object):
     _cell_code = 0      # MGB_RNN_CELL_*
 
     def __init__(self, cell, head, log_std=None, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None,
-                 device="cuda"):
+                 device="cuda", value=None):
         import torch
         self._torch = torch
         name, kind = type(self).__name__, self._torch_cell()
@@ -192,7 +249,10 @@ class _RecurrentPolicy(object):
         self.head_width = lin[0].out_features if len(lin) == 2 else 0
         self.state_dim = self._memory * self.hidden + FEEDBACK * self.feedback
         H, n_in = self.hidden, cell.input_size
-        self.numel = self._gates * H * (n_in + H + 2) + sum(m.out_features * (m.in_features + 1) for m in lin)
+        self._value = _value_head(value, lin[-1].in_features, name)
+        self.has_value = self._value is not None
+        self.numel = (self._gates * H * (n_in + H + 2) + sum(m.out_features * (m.in_features + 1) for m in lin)
+                      + (lin[-1].in_features + 1 if self.has_value else 0))
         self.device = torch.device(device)
         self.params = torch.zeros(self.numel, dtype=torch.float32, device=self.device)
         self._cell, self._head, self._mean, self._std = cell, head, None, None
@@ -224,14 +284,17 @@ class _RecurrentPolicy(object):
             Wi[:, :D] = Wi[:, :D] / std
         parts = [Wi.reshape(-1), Wh.reshape(-1), bi, bh]
         lin, _ = _head_layers(self._head, H, type(self).__name__)
-        for m in lin:
-            parts += [f64(m.weight).reshape(-1), f64(m.bias) if m.bias is not None else
-                      torch.zeros(m.out_features, dtype=torch.float64)]
+        for k, m in enumerate(lin):
+            W, b = f64(m.weight), f64(m.bias) if m.bias is not None else torch.zeros(m.out_features, dtype=torch.float64)
+            if k == len(lin) - 1:
+                W, b = _cat_value(W, b, self._value)
+            parts += [W.reshape(-1), b]
         return torch.cat(parts).to(torch.float32)
 
-    def update(self, cell=None, head=None, obs_mean=None, obs_std=None):
+    def update(self, cell=None, head=None, obs_mean=None, obs_std=None, value=None):
         """Repack into the same device buffer (copy_, stream-ordered): a graph captured on this policy sees the new
-        weights.  Arguments left None keep their previous values; cell and head must keep their shapes."""
+        weights.  Arguments left None keep their previous values; cell and head must keep their shapes, and a value
+        head can only replace the policy's own."""
         name = type(self).__name__
         if cell is not None and (type(cell) is not self._torch_cell() or cell.input_size != self._cell.input_size
                                  or cell.hidden_size != self.hidden):
@@ -240,6 +303,10 @@ class _RecurrentPolicy(object):
             lin, act = _head_layers(head, self.hidden, name)
             if (lin[0].out_features if len(lin) == 2 else 0) != self.head_width or act != self.activation:
                 raise ValueError("%s.update: the head must keep its layer shapes and activation" % name)
+        if value is not None:
+            if not self.has_value:
+                raise ValueError("%s.update: this policy was built without a value head" % name)
+            _value_head(value, self.head_width or self.hidden, name)
         mean = None if obs_mean is None else self._vec(obs_mean, self.obs_dim, "obs_mean")
         std = None if obs_std is None else self._vec(obs_std, self.obs_dim, "obs_std")
         if mean is not None and not self._torch.isfinite(mean).all():
@@ -254,6 +321,8 @@ class _RecurrentPolicy(object):
             self._mean = mean
         if std is not None:
             self._std = std
+        if value is not None:
+            self._value = value
         self.params.copy_(self.pack(), non_blocking=False)
         return self
 
@@ -271,11 +340,14 @@ class _RecurrentPolicy(object):
         """(h, memory carried to the next step) of one cell step; mem holds the _memory H-wide rows of the state."""
         raise NotImplementedError
 
-    def unroll(self, out):
+    def unroll(self, out, value=False):
         """Recompute a recurrent rollout with autograd through the cell and head: returns (logits [T, N, 4],
-        logp [T, N]), logp the log-probability of out["act"].  Uses out's obs0, obs, act, rew, done, state0 and
+        logp [T, N]), logp the log-probability of out["act"], and with value=True (a policy with a value head) also
+        value [T, N], V(s_t).  Uses out's obs0, obs, act, rew, done, state0 and
         resampled (and on a trial handle task_episodes0 and episodes_per_task), and applies the kernel's input
         construction and reset rule, in the cell's dtype and device."""
+        if value and not self.has_value:
+            raise ValueError("unroll(value=True) needs a value head")
         from .metamaze import new_tasks
         torch = self._torch
         head, D = self._head, self.obs_dim
@@ -294,11 +366,17 @@ class _RecurrentPolicy(object):
         wipe = done if self.hidden_reset == "episode" else new_tasks(out).to(dev)
         nm = self._memory * self.hidden
         mem, fb = state0[:, :nm], state0[:, nm:]
-        logits, logp = [], []
+        logits, logp, vals = [], [], []
+        mods = list(head) if isinstance(head, torch.nn.Sequential) else [head]
         for t in range(T):
             x = torch.cat([obs[t], fb], 1) if self.feedback else obs[t]
             h, new_mem = self._step(x, mem)
-            lg = head(h)
+            z = h
+            for m in mods[:-1]:
+                z = m(z)
+            lg = mods[-1](z)
+            if value:
+                vals.append(self._value(z)[:, 0])
             logits.append(lg)
             logp.append(torch.log_softmax(lg, -1).gather(1, act[t][:, None])[:, 0])
             keep = ~wipe[t]
@@ -306,6 +384,8 @@ class _RecurrentPolicy(object):
             if self.feedback:
                 new_fb = torch.cat([torch.nn.functional.one_hot(act[t], 4).to(dt), rew[t][:, None]], 1)
                 fb = torch.where(keep[:, None], new_fb, torch.zeros_like(new_fb))
+        if value:
+            return torch.stack(logits), torch.stack(logp), torch.stack(vals)
         return torch.stack(logits), torch.stack(logp)
 
 
@@ -340,8 +420,9 @@ class LSTMPolicy(_RecurrentPolicy):
     """
     _gates, _memory, _cell_code = 4, 2, _lib.RNN_CELL_LSTM
 
-    def __init__(self, cell, head, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None, device="cuda"):
-        super().__init__(cell, head, None, feedback, hidden_reset, obs_mean, obs_std, device)
+    def __init__(self, cell, head, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None, device="cuda",
+                 value=None):
+        super().__init__(cell, head, None, feedback, hidden_reset, obs_mean, obs_std, device, value)
 
     def _torch_cell(self):
         return self._torch.nn.LSTMCell
@@ -350,6 +431,36 @@ class LSTMPolicy(_RecurrentPolicy):
         H = self.hidden
         h, c = self._cell(x, (mem[:, :H], mem[:, H:]))
         return h, self._torch.cat([h, c], 1)
+
+
+def critic_args(policy, gae):
+    """(gamma, lam) for a rollout of `policy` that goes to a *_critic entry point, or None for one that does not.  A
+    policy or population with a value head always goes there (gamma = lam = 1 without gae: the launch computes no GAE
+    then and does not read them); gae without a value head is a ValueError."""
+    if not policy.has_value:
+        if gae is not None:
+            raise ValueError("gae= needs a policy with a value head (value=nn.Linear(k, 1))")
+        return None
+    if gae is None:
+        return None, None
+    gamma, lam = gae
+    return float(gamma), float(lam)
+
+
+def critic_struct(torch, out, T, N, dev, critic, want_final):
+    """The mgb_critic of a rollout whose outputs are `out`: allocates (torch.empty) the entries out lacks, "value" [T, N]
+    and "value_last" [N], with want_final or gae "final_value" [T, N], and with gae "adv", "ret" [T, N] and the
+    "truncated" [T, N] GAE reads."""
+    gamma, lam = critic
+    gae = gamma is not None
+    keys = ["value", "value_last"] + (["final_value"] if want_final or gae else []) + (["adv", "ret"] if gae else [])
+    for k in keys:
+        if out.get(k) is None:
+            out[k] = torch.empty((N,) if k == "value_last" else (T, N), dtype=torch.float32, device=dev)
+    if gae and out.get("truncated") is None:
+        out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+    return _lib.Critic(*[_lib.ptr(out.get(k)) for k in ("value", "value_last", "final_value", "adv", "ret")],
+                       1.0 if gamma is None else gamma, 1.0 if lam is None else lam)
 
 
 class PolicyPopulation(object):
@@ -384,7 +495,7 @@ class PolicyPopulation(object):
         shapes = {self._shape(p) for p in policies}
         if len(shapes) != 1:
             raise ValueError("PolicyPopulation: the members must have one shape (layer widths, activation, feedback, "
-                             "hidden_reset, log_std) and one device")
+                             "hidden_reset, log_std, value head) and one device")
         self.policies = policies
         self.kind = kind
         self.recurrent = kind is not MLPPolicy
@@ -400,8 +511,8 @@ class PolicyPopulation(object):
     @staticmethod
     def _shape(p):
         if isinstance(p, MLPPolicy):
-            return (p.obs_dim, tuple(p.widths), p.activation, p.has_log_std, p.device)
-        return (p.obs_dim, p.hidden, p.head_width, p.activation, p.feedback, p.hidden_reset, p.device)
+            return (p.obs_dim, tuple(p.widths), p.activation, p.has_log_std, p.has_value, p.device)
+        return (p.obs_dim, p.hidden, p.head_width, p.activation, p.feedback, p.hidden_reset, p.has_value, p.device)
 
     @classmethod
     def from_template(cls, policy, members):
@@ -424,6 +535,10 @@ class PolicyPopulation(object):
     @property
     def has_log_std(self):
         return all(p.has_log_std for p in self.policies)
+
+    @property
+    def has_value(self):
+        return self.policies[0].has_value
 
     def envs_per_member(self, num_envs):
         """E = num_envs / members; ValueError when num_envs is not a multiple of members."""
@@ -452,11 +567,11 @@ class PolicyPopulation(object):
     def member_stride(self):
         return self.params.stride(0)
 
-    _ENV_ROWS = ("obs0", "state0", "task_episodes0")     # [N, ...]; every other tensor entry is [T, N, ...]
+    _ENV_ROWS = ("obs0", "state0", "task_episodes0", "value_last")   # [N, ...]; every other tensor entry is [T, N, ...]
 
     def member_slice(self, out, m):
-        """Member m's env columns of a rollout dict (every [T, N, ...] output, and the rows of obs0, state0 and
-        task_episodes0; other entries are copied), or its rows of an [N, ...] tensor such as the carried state."""
+        """Member m's env columns of a rollout dict (every [T, N, ...] output, and the rows of obs0, state0,
+        task_episodes0 and value_last; other entries are copied), or its rows of an [N, ...] tensor such as the carried state."""
         torch = self._torch
         if isinstance(out, torch.Tensor):
             E = self.envs_per_member(out.shape[0])
@@ -477,11 +592,11 @@ class PolicyPopulation(object):
             raise ValueError("initial_state: an MLP population carries no state")
         return self.policies[0].initial_state(num_envs)
 
-    def unroll(self, out):
+    def unroll(self, out, value=False):
         """The members' unroll() over their env slices of `out`, concatenated along the env axis: (logits [T, N, 4],
-        logp [T, N]) (recurrent populations)."""
+        logp [T, N]), and with value=True value [T, N] (recurrent populations)."""
         if not self.recurrent:
             raise ValueError("unroll: an MLP population has nothing to unroll")
-        parts = [p.unroll(self.member_slice(out, m)) for m, p in enumerate(self.policies)]
+        parts = [p.unroll(self.member_slice(out, m), value) for m, p in enumerate(self.policies)]
         torch = self._torch
-        return torch.cat([lg for lg, _ in parts], 1), torch.cat([lp for _, lp in parts], 1)
+        return tuple(torch.cat([q[i] for q in parts], 1) for i in range(len(parts[0])))

@@ -341,7 +341,8 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         _lib.check(self._lib.mgb_quad_step_host(self._h, _lib.ptr(act), _lib.ptr(obs), _lib.ptr(rew), _lib.ptr(done),
                                                 None, None, self._stream()))
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, policy=None, deterministic=False):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, policy=None, deterministic=False,
+                gae=None):
         """T steps in one launch (state stays in registers).  actions: [T,N,4] CUDA tensor or None (device-drawn
         U(min_voltage, max_voltage)).  Returns dict(obs [T,N,D], rew [T,N], done [T,N], act [T,N,4] or None).
 
@@ -352,6 +353,11 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         acted on at t = 0; at t > 0 it is obs[t-1]).  `actions` together with `policy` is a ValueError.
         policy may also be a PolicyPopulation of MLPPolicy members (mgb_quad_rollout_population): member m drives the
         envs [m E, (m + 1) E), E = N / members, which must be 32 or a multiple of 64.
+        A policy or population with a value head (MLPPolicy(value=...); mgb_quad_rollout_critic) also yields "value"
+        [T,N] (V on the observation step t acts on), "value_last" [N] (V after the last step: the next launch's
+        value[0]) and, with final_obs=True or gae, "final_value" [T,N] (V of the terminal observation where an episode
+        ended truncated; other entries are not written).  gae=(gamma, lam) also yields "adv" and "ret" [T,N] float32,
+        GAE(gamma, lam) computed in the launch (DESIGN.md "Value heads and GAE"); it needs a value head and auto_reset.
 
         With final_obs=True the dict also holds "final_obs" [T,N,D] float32: row (t, e) is the terminal observation
         of env e where done[t, e] (what step() reports as final_observation); it is allocated with torch.empty, and
@@ -366,7 +372,9 @@ class BatchedQuadrotor(Snapshots, Mirrored):
             from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
             if isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation) and policy.recurrent):
                 raise ValueError("recurrent policies run on MetaMaze2D only; the quadrotor takes an MLPPolicy")
-            return self._rollout_policy(T, policy, act_seed, deterministic, out)
+            return self._rollout_policy(T, policy, act_seed, deterministic, out, gae)
+        if gae is not None:
+            raise ValueError("gae= needs a policy with a value head")
         if out is None:
             out = {"obs": torch.empty((T, N, D), dtype=torch.float32, device=dev),
                    "rew": torch.empty((T, N), dtype=torch.float32, device=dev),
@@ -383,8 +391,8 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                                     self._stream()))
         return out
 
-    def _rollout_policy(self, T, policy, act_seed, deterministic, out):
-        from .policy import PolicyPopulation
+    def _rollout_policy(self, T, policy, act_seed, deterministic, out, gae=None):
+        from .policy import PolicyPopulation, critic_args, critic_struct
         torch = self._torch
         N, D, dev = self.num_envs, self.obs_dim, self.device
         population = isinstance(policy, PolicyPopulation)
@@ -396,6 +404,7 @@ class BatchedQuadrotor(Snapshots, Mirrored):
             raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
         if not deterministic and not policy.has_log_std:
             raise ValueError("a stochastic quadrotor policy needs log_std (or pass deterministic=True)")
+        critic = critic_args(policy, gae)
         if out is None:
             out = {"obs": torch.empty((T, N, D), dtype=torch.float32, device=dev),
                    "rew": torch.empty((T, N), dtype=torch.float32, device=dev),
@@ -408,6 +417,13 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                 out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
         pol = policy.struct(deterministic)
         keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
+        if critic is not None:
+            cr = critic_struct(torch, out, T, N, dev, critic, self._want_final)
+            outs = [_lib.ptr(out.get(k)) for k in keys]
+            members, stride = (policy.members, policy.member_stride) if population else (1, 0)
+            _lib.check(self._lib.mgb_quad_rollout_critic(self._h, int(T), ctypes.byref(pol), members, stride,
+                                                         int(act_seed), *outs, ctypes.byref(cr), self._stream()))
+            return out
         outs = [_lib.ptr(out.get(k)) for k in keys]
         if population:
             _lib.check(self._lib.mgb_quad_rollout_population(self._h, int(T), ctypes.byref(pol), policy.members,
