@@ -624,6 +624,54 @@ int mgb_maze_rollout_rnn_critic(mgb_maze *h, int32_t T, const mgb_rnn_policy *po
                                 double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
                                 const mgb_critic *critic, void *stream);
 
+/* ---- recurrent cell sequences (DESIGN.md "Fused unroll") ----------------------------------------------------------
+ * The learner's side of the recurrent policies: the cell of mgb_rnn_policy run over T given steps of n envs, forward and
+ * backward, with no env and no head.  A PPO update recomputes h_t with autograd from a rollout's inputs; the head, the
+ * log-softmax and the weight gradients are batched GEMMs over all T n rows and stay with the caller.
+ *   params_dev: weight_ih [G H][in], weight_hh [G H][H], bias_ih [G H], bias_hh [G H] (G = 3 for the GRU, 4 for the LSTM;
+ *     zeros for a cell without bias): the cell part of mgb_rnn_policy's packed buffer.
+ *   x_dev [T][in][n]: the cell's input of step t for env e at (t in + i) n + e.
+ *   wipe_dev [T][n] uint8: nonzero where the state is zeroed after step t (the reset rule of the rollout that made x).
+ *   state0_dev [n][HC]: the memory going into step 0, HC = H (GRU: h) or 2H (LSTM: h, c).
+ *   h_dev [T][n][H]: h_t.
+ * mgb_rnn_seq_forward: for t = 0 .. T-1, (h, c) = cell(x_t, memory), the memory being state0 at t = 0, zeros where
+ *   wipe[t-1] and (h_{t-1}, c_{t-1}) otherwise; the arithmetic of "Recurrent policies" above, so h_t equals the rollout's
+ *   hid_out bit for bit on equal inputs.  With gates_dev [T][S][H][n] (S = 4) it also saves what the backward reads, unit
+ *   j of env e at ((t S + s) H + j) n + e: the GRU's r, z, n and W_hn h_{t-1} + b_hn, the LSTM's i, f, g, o; the LSTM
+ *   saves c_t as s = 4 (S = 5).  gates_dev NULL saves nothing.  Reads params, x, wipe, state0; writes h (and gates).
+ * mgb_rnn_seq_backward: from dh_dev [T][n][H] = dL/dh_t and the saved gates (and h for the GRU), walks t = T-1 .. 0 and
+ *   writes the gate pre-activation gradients dgi_dev [T][G H][n] (gate block k, unit j of env e at ((t G + k) H + j) n + e;
+ *   = dL/d(W_ih x + b_ih)), for the GRU dghn_dev [T][H][n], the n block of dL/d(W_hh h + b_hh), whose r and z blocks
+ *   equal dgi's, and dstate0_dev [n][HC].  The gradient carried into step t-1 is dropped where wipe[t-1].  Each env is
+ *   summed in a fixed order by one thread: no atomics, the result is deterministic.  Reads params, wipe, state0, h (GRU),
+ *   gates and dh; writes dgi, dghn and dstate0.
+ * Both are stream-ordered, allocate nothing and can be captured in a CUDA graph; offsets are 64-bit.  The CTA holds
+ * MGB_RNN_SEQ_CTA_ENVS envs.  Refused (MGB_ERR_ARG, nothing written): a NULL seq, an unknown cell, hidden outside 1..64,
+ * in, T or n below 1, a NULL pointer the call reads or writes, and a footprint beyond the current device's opt-in shared
+ * memory (forward: the cell's staged weights and the columns x, c, h of the CTA's envs; backward: weight_hh and two
+ * columns; DESIGN.md "Fused unroll" restates both). */
+#define MGB_RNN_SEQ_CTA_ENVS 128
+typedef struct mgb_rnn_seq {
+    int32_t cell;             /* MGB_RNN_CELL_* */
+    int32_t hidden;           /* H, 1..64 */
+    int32_t in;               /* inputs per step, >= 1 */
+    int32_t T;                /* steps, >= 1 */
+    int64_t n;                /* envs, >= 1 */
+    const float *params_dev;  /* cell weights, above */
+    const float *x_dev;       /* [T][in][n] (forward) */
+    const uint8_t *wipe_dev;  /* [T][n] */
+    const float *state0_dev;  /* [n][HC] */
+    float *h_dev;             /* [T][n][H]: written by the forward, read by the GRU's backward */
+    float *gates_dev;         /* [T][S][H][n]: written by the forward (or NULL), read by the backward */
+    const float *dh_dev;      /* [T][n][H] (backward) */
+    float *dgi_dev;           /* [T][G H][n] (backward) */
+    float *dghn_dev;          /* [T][H][n] (backward, GRU) */
+    float *dstate0_dev;       /* [n][HC] (backward) */
+} mgb_rnn_seq;
+
+int mgb_rnn_seq_forward(const mgb_rnn_seq *seq, void *stream);
+int mgb_rnn_seq_backward(const mgb_rnn_seq *seq, void *stream);
+
 /* Continuous pose (maze_continuous_3d.py:47-56, dynamics.py:71-92): pos_dev [n][2] float32 (_agent_loc), ori_dev [n]
  * float64 (_agent_ori). */
 int mgb_maze_pose(mgb_maze *h, float *pos_dev, double *ori_dev, void *stream);

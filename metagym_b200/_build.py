@@ -38,7 +38,8 @@ def needs_build():
 
 # per-file extra flags: the maze renderer must reproduce float64 results of code that never fuses multiply-add
 # quad.cu: every FMA is written out (fmaf / dot3 / det2) so that all kernel variants compute the same bits
-PER_FILE_FLAGS = {"maze.cu": ["-fmad=false"], "quad.cu": ["-fmad=false"]}
+# rnn_seq.cu: the forward runs the rollout's cell and must compile it exactly as maze.cu does
+PER_FILE_FLAGS = {"maze.cu": ["-fmad=false"], "quad.cu": ["-fmad=false"], "rnn_seq.cu": ["-fmad=false"]}
 
 
 def build(force=False, verbose=False):

@@ -65,6 +65,13 @@ class Critic(ctypes.Structure):       # mgb_critic
                 ("gamma", ctypes.c_float), ("lam", ctypes.c_float)]
 
 
+class RnnSeq(ctypes.Structure):
+    """mgb_rnn_seq (include/mgb200.h)."""
+    _fields_ = [("cell", c_i32), ("hidden", c_i32), ("in_", c_i32), ("T", c_i32), ("n", c_i64), ("params_dev", vp),
+                ("x_dev", vp), ("wipe_dev", vp), ("state0_dev", vp), ("h_dev", vp), ("gates_dev", vp), ("dh_dev", vp),
+                ("dgi_dev", vp), ("dghn_dev", vp), ("dstate0_dev", vp)]
+
+
 ACT_TANH, ACT_RELU = 0, 1            # MGB_ACT_*
 POLICY_SAMPLE, POLICY_MEAN = 0, 1    # MGB_POLICY_*
 RNN_RESET_EPISODE, RNN_RESET_TASK = 0, 1     # MGB_RNN_RESET_*
@@ -72,6 +79,7 @@ RNN_CELL_GRU, RNN_CELL_LSTM = 0, 1           # MGB_RNN_CELL_*
 POLICY_MEMBER_WARP = 32                      # MGB_POLICY_MEMBER_WARP
 QUAD_POLICY_CTA_ENVS = 64                    # MGB_QUAD_POLICY_CTA_ENVS
 MAZE2D_POLICY_CTA_ENVS = 128                 # MGB_MAZE2D_POLICY_CTA_ENVS
+RNN_SEQ_CTA_ENVS = 128                       # MGB_RNN_SEQ_CTA_ENVS
 
 
 # name -> (restype, argtypes); every function include/mgb200.h declares (tests/test_abi.py checks the two agree)
@@ -144,6 +152,8 @@ SIGNATURES = {
     "mgb_maze_rollout_rnn_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64,
                                                    ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp, vp,
                                                    vp, vp, vp, vp, ctypes.POINTER(Critic), vp]),
+    "mgb_rnn_seq_forward": (ctypes.c_int, [ctypes.POINTER(RnnSeq), vp]),
+    "mgb_rnn_seq_backward": (ctypes.c_int, [ctypes.POINTER(RnnSeq), vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_state": (ctypes.c_int, [vp, vp, vp, vp]),
     "mgb_maze_launch_count": (c_i64, [vp]),

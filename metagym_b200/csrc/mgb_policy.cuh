@@ -338,8 +338,9 @@ static inline size_t mgb_rnn_smem_bytes(const MgbRnn<NG> &r, int threads)
 }
 
 // Device: stage the cell and the head read at r.params + off into sm[0, r.staged) (all threads of the CTA; the caller
-// synchronises)
-template <int NG>
+// synchronises).  HEAD = false stages the cell alone, into sm[0, r.s_head): the sequence kernels of rnn_seq.cu, whose
+// packed buffer ends with bias_hh.
+template <int NG, bool HEAD = true>
 __device__ __forceinline__ void mgb_rnn_stage(const MgbRnn<NG> &r, float *sm, int64_t off)
 {
     constexpr int G = kRnnGroup;
@@ -357,7 +358,7 @@ __device__ __forceinline__ void mgb_rnn_stage(const MgbRnn<NG> &r, float *sm, in
         const int u = s % G, k = (s / G) % NG, kind = (s / (NG * G)) % 2, j = (s / (2 * NG * G)) * G + u;
         sm[r.s_b + s] = j < H ? __ldg(r.params + off + r.g_b + kind * NG * H + k * H + j) : 0.f;
     }
-    mgb_mlp_stage(r.head, sm + r.s_head, off);
+    if constexpr (HEAD) mgb_mlp_stage(r.head, sm + r.s_head, off);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -465,12 +466,20 @@ __device__ __forceinline__ void mgb_gae(const mgb_critic &cr, int T, int64_t n, 
 
 __device__ __forceinline__ float mgb_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }
 
+// What mgb_rnn_cell hands its `save` for unit j: nothing by default (the rollouts)
+struct MgbRnnNoSave {
+    template <class... V>
+    __device__ __forceinline__ void operator()(int, V...) const {}
+};
+
 // Device: one step of the cell for the thread's env (header "Recurrent policies" for the arithmetic): h = GRU(x, hp),
 // or (h, c) = LSTM(x, (hp, c)) with c updated in place (unit j reads and writes only c[j]; the GRU ignores c).  x, hp,
 // c and h are column buffers (rows of `stride` floats; the thread's column is `col`); h must not alias x, hp or c.
-template <int NG>
+// save(j, ...) receives unit j's values the backward pass of mgb_rnn_seq_backward needs: the GRU's r, z, n and
+// W_hn hp + b_hn, the LSTM's i, f, g, o and c'.
+template <int NG, class Save = MgbRnnNoSave>
 __device__ __forceinline__ void mgb_rnn_cell(const MgbRnn<NG> &r, const float *sm, const float *xb, const float *hpb,
-                                             float *cb, float *hb, int stride, int col)
+                                             float *cb, float *hb, int stride, int col, Save save = {})
 {
     constexpr int G = kRnnGroup, Q = NG * G / 4;     // Q: float4 weights per input of a group
     const float *x = xb + col, *hp = hpb + col;
@@ -516,6 +525,7 @@ __device__ __forceinline__ void mgb_rnn_cell(const MgbRnn<NG> &r, const float *s
                     const float zg = mgb_sigmoid(gi[G + v] + gh[G + v]);
                     const float ng = tanhf(fmaf(rg, gh[2 * G + v], gi[2 * G + v]));
                     h[(u + v) * stride] = fmaf(zg, hp[(u + v) * stride], (1.f - zg) * ng);
+                    save(u + v, rg, zg, ng, gh[2 * G + v]);
                 } else {
                     const float ig = mgb_sigmoid(gi[v] + gh[v]);
                     const float fg = mgb_sigmoid(gi[G + v] + gh[G + v]);
@@ -524,6 +534,7 @@ __device__ __forceinline__ void mgb_rnn_cell(const MgbRnn<NG> &r, const float *s
                     const float cn = fmaf(fg, c[(u + v) * stride], ig * gg);
                     c[(u + v) * stride] = cn;
                     h[(u + v) * stride] = og * tanhf(cn);
+                    save(u + v, ig, fg, gg, og, cn);
                 }
             }
     }

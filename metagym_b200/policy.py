@@ -10,7 +10,8 @@ read at every launch, so ``update()`` after an optimiser step is seen by a rollo
 GRUPolicy and LSTMPolicy pack an ``nn.GRUCell`` or an ``nn.LSTMCell`` and a head for the recurrent MetaMaze2D rollout
 (mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies"): ``weight_ih``, ``weight_hh``, ``bias_ih``, ``bias_hh``, then the
 head's layers as MLPPolicy packs them.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities
-through the torch modules.
+with autograd, running a float32 CUDA cell through the fused cell sequence (metagym_b200.cell_seq; DESIGN.md "Fused
+unroll") and any other cell through a torch loop over the steps.
 
 Each of the three takes an optional value head, value = nn.Linear(k, 1) reading what the output layer reads: the
 critic of the *_critic entry points (DESIGN.md "Value heads and GAE").  It packs as a fifth row of the output layer,
@@ -345,12 +346,34 @@ class _RecurrentPolicy(object):
         logp [T, N]), logp the log-probability of out["act"], and with value=True (a policy with a value head) also
         value [T, N], V(s_t).  Uses out's obs0, obs, act, rew, done, state0 and
         resampled (and on a trial handle task_episodes0 and episodes_per_task), and applies the kernel's input
-        construction and reset rule, in the cell's dtype and device."""
+        construction and reset rule, in the cell's dtype and device.  A float32 cell on CUDA runs through the fused
+        cell sequence (metagym_b200.cell_seq; DESIGN.md "Fused unroll"), with the head batched over all T N rows; any
+        other cell, or one whose footprint the device's shared memory cannot hold, runs the torch step loop."""
         if value and not self.has_value:
             raise ValueError("unroll(value=True) needs a value head")
+        from . import cell_seq
+        if not cell_seq.fits(self._cell):
+            return self._unroll_reference(out, value)
+        torch = self._torch
+        obs, act, rew, wipe, state0 = self._unroll_inputs(out)
+        X = self._cell_input(obs, act, rew, wipe, state0).detach().transpose(1, 2).contiguous()
+        h = cell_seq.run(self._cell, self._cell_code, X, wipe.contiguous(), state0[:, :self._memory * self.hidden])
+        z = h
+        mods = list(self._head) if isinstance(self._head, torch.nn.Sequential) else [self._head]
+        for m in mods[:-1]:
+            z = m(z)
+        logits = mods[-1](z)
+        logp = torch.log_softmax(logits, -1).gather(2, act[..., None])[..., 0]
+        if value:
+            return logits, logp, self._value(z)[..., 0]
+        return logits, logp
+
+    def _unroll_inputs(self, out):
+        """(obs [T, N, D] normalised, act [T, N] int64, rew [T, N] as the kernel feeds it back, wipe [T, N] bool, state0
+        [N, state_dim]) of a rollout dict, in the cell's dtype and device."""
         from .metamaze import new_tasks
         torch = self._torch
-        head, D = self._head, self.obs_dim
+        D = self.obs_dim
         w = self._cell.weight_ih
         dt, dev = w.dtype, w.device
         act = out["act"].to(dev).long()
@@ -364,6 +387,28 @@ class _RecurrentPolicy(object):
         done = out["done"].to(dev).bool()
         state0 = out["state0"].to(dev, dt)
         wipe = done if self.hidden_reset == "episode" else new_tasks(out).to(dev)
+        return obs, act, rew, wipe, state0
+
+    def _cell_input(self, obs, act, rew, wipe, state0):
+        """x [T, N, in] of every step at once: the observation, then with feedback state0's feedback at t = 0 and
+        (onehot(a_{t-1}), r_{t-1}) after, zeros where wipe[t-1]."""
+        if not self.feedback:
+            return obs
+        torch = self._torch
+        fb = torch.cat([torch.nn.functional.one_hot(act, 4).to(obs.dtype), rew[..., None]], 2)
+        fb = fb.masked_fill(wipe[..., None], 0.)
+        return torch.cat([obs, torch.cat([state0[None, :, self._memory * self.hidden:], fb[:-1]], 0)], 2)
+
+    def _unroll_reference(self, out, value=False):
+        """unroll() as a torch loop over the steps: the path of CPU and float64 cells and of cells beyond the kernels'
+        footprint, and the reference the fused path is tested against."""
+        if value and not self.has_value:
+            raise ValueError("unroll(value=True) needs a value head")
+        torch = self._torch
+        head = self._head
+        dt = self._cell.weight_ih.dtype
+        obs, act, rew, wipe, state0 = self._unroll_inputs(out)
+        T, N = act.shape
         nm = self._memory * self.hidden
         mem, fb = state0[:, :nm], state0[:, nm:]
         logits, logp, vals = [], [], []
