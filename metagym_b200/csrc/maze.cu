@@ -2726,7 +2726,6 @@ struct mgb_maze {
     MgbDev<uint32_t> task_count;              // trial handle: [n_pad] episodes each env has finished on its current maze
     bool slot_per_env = false;                // env2task is injective: every env owns its task-table slot
     MgbDev<uint8_t> task_flags;               // [n_tasks] scratch of mgb_maze_update_tasks
-    bool cache_would_fit = true;              // last ensure_pose_cache decision (false: over budget -> direct renderer)
     std::vector<double> cls_heights;          // eff-table classes of the current task table
     double min_cell = 0.0;                    // smallest cell_size of the table (bounds the crossings a ray can record)
     MazeStage stage[2];
@@ -3265,7 +3264,6 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     h->n_tasks = n_tasks;
     h->has_task = true;
     h->task_flags.reset();
-    h->cache_would_fit = true;
     // pose list of the cache: every free cell x 4 headings of every task, S = 4 x the most free cells of a task per task
     // slot, so that update_tasks can rebuild one task's poses in place
     h->host_poses.clear();
@@ -3565,6 +3563,7 @@ static void relayout_poses(mgb_maze *h, int S)
 
 static int render_region(mgb_maze *h, const MazeArgs &a, int K, int64_t n_fill, cudaStream_t st);
 static int bake_region(mgb_maze *h, MazePoseCache &pc, MazeArgs a, int K, cudaStream_t st);
+static bool pose_cache_serves(const mgb_maze *h);
 
 extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *task_slots_host, const int8_t *walls_host,
                                      const int8_t *texts_host, const double *food_rewards_host,
@@ -3582,7 +3581,7 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
     // discrete 3-D tables keep the cache's pose lists; a handle that serves (or will serve) them from the pose cache
     // rebuilds the replaced tasks' region in place, which needs every task within the table's S / 4 free cells
     const bool poses_kept = c.kind == MGB_MAZE_DISCRETE_3D && !h->host_poses.empty();
-    const bool cached = poses_kept && h->cache_enabled && h->cache_would_fit;
+    const bool cached = pose_cache_serves(h);
     int most = 0;
     int64_t n_fill = 0;
     for (int t = 0; t < count; ++t) {
@@ -3715,7 +3714,7 @@ static const char *sampler_cfg(const mgb_maze *h, const mgb_maze_sampler_cfg *cf
         return "device resampling needs one task-table slot per env (mgb_maze_set_task with n_tasks >= n_envs and an injective "
                "env2task)";
     const MazeConst &c = h->c;
-    if (c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() && h->cache_would_fit)
+    if (pose_cache_serves(h))
         return "device resampling needs the direct renderer: create the env with the pose cache off (cache=False)";
     if (!(c.n % 2 == 1 && c.n > 6)) return "Cell Numbers can only be odd, minimum 7 (maze_task.py:57-58)";
     if (!(cfg->step_reward < 0)) return "step_reward must be < 0 (maze_task.py:59)";
@@ -3887,6 +3886,15 @@ static bool pose_cache_fits(const mgb_maze *h, double &bytes)
     return bytes <= h->cache_budget_gb * 1e9 && packs;
 }
 
+// Whether the pose cache draws the handle's frames: a discrete 3-D table, the cache on, and pose_cache_fits.  Everything
+// it reads is host state that set_task, set_textures, update_tasks and set_cache keep current, so every call decides the
+// same way before and after the first reset() builds the cache.
+static bool pose_cache_serves(const mgb_maze *h)
+{
+    double bytes;
+    return h->c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() && pose_cache_fits(h, bytes);
+}
+
 // screens whose columns are whole 4-pixel groups get signatures, baked all-present frames and (uint8 SURVIVAL) variant frames
 static bool cache_bakes(const MazeConst &c)
 {
@@ -3966,10 +3974,14 @@ static int ensure_pose_cache(mgb_maze *h, cudaStream_t st)
     if (!h->cache_dirty) return MGB_OK;
     h->cache_ready = false;
     MazeConst &c = h->c;
-    if (!h->cache_enabled || c.kind != MGB_MAZE_DISCRETE_3D || h->host_poses.empty()) { h->cache_dirty = false; return MGB_OK; }
+    if (!pose_cache_serves(h)) {          // a decision, not a failure: cache_info then reports no cache
+        h->cache_dirty = false;
+        h->variant_bits_used = 0; h->var_stride = 0; h->var_planned = false; h->cache_bytes = 0.0;
+        return MGB_OK;
+    }
     const size_t slots = h->host_poses.size(), px = (size_t)c.res_h * c.res_v;
     double bytes;
-    if (!pose_cache_fits(h, bytes)) { h->cache_dirty = false; h->cache_would_fit = false; return MGB_OK; }   // a decision, not a failure
+    pose_cache_fits(h, bytes);
     // From here on a failure (capture in progress, out of memory) leaves cache_dirty set: the next call retries instead of
     // silently rendering every frame with the slow direct renderer (round-1 advice).
     // cudaMalloc/cudaFree synchronise; a capture in progress cannot build the cache
@@ -5250,10 +5262,7 @@ __global__ void maze_record_path_kernel(int64_t n, int64_t n_pad, int64_t cap, c
 // (resample_tasks needs the direct renderer).  Otherwise the table is shared, and fingerprinted.
 static bool records_carry_tasks(const mgb_maze *h)
 {
-    double bytes;
-    const bool cached = h->c.kind == MGB_MAZE_DISCRETE_3D && h->cache_enabled && !h->host_poses.empty() &&
-                        pose_cache_fits(h, bytes);
-    return h->slot_per_env && !cached;
+    return h->slot_per_env && !pose_cache_serves(h);
 }
 
 static int64_t record_tail(const mgb_maze *h)
