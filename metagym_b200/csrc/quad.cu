@@ -234,7 +234,8 @@ template <class T> __device__ __forceinline__ T fast_atan2(T y, T x)
     T out;
 #pragma unroll
     for (int h = 0; h < Lanes<T>::N; ++h) {
-        const bool swap = lane(ay, h) > lane(ax, h), neg = lane(x, h) < 0.f;
+        // the sign bit, not x < 0: atan2(+-0, -0) = +-pi like np.arctan2 (gimbal lock, an inverted vehicle)
+        const bool swap = lane(ay, h) > lane(ax, h), neg = signbit(lane(x, h));
         const float v = swap ? (neg ? lane(r2b, h) : lane(r1, h)) : (neg ? lane(r2a, h) : lane(r, h));
         set_lane(out, h, copysignf(v, lane(y, h)));
     }

@@ -30,6 +30,8 @@ static int qo_any_obstacle(double xo, double yo, double xn, double yn)
     const int W = qo_cols + 1;
     return (qo_sat[ye * W + xe] - qo_sat[ys * W + xe] - qo_sat[ye * W + xs] + qo_sat[ys * W + xs]) > 0;
 }
+/* the same, exported for tests that check the window against a literal numpy slice of the map */
+int qo_map_any_obstacle(double xo, double yo, double xn, double yn) { return qo_any_obstacle(xo, yo, xn, yn); }
 
 #define QO_CAT2(a, b) a##b
 #define QO_CAT(a, b) QO_CAT2(a, b)

@@ -287,3 +287,10 @@ def set_map(map_matrix):
     lib().qo_set_map(_ptr(sat, ctypes.c_int), ctypes.c_int(m.shape[0]), ctypes.c_int(m.shape[1]),
                      ctypes.c_int(int(xs[0])), ctypes.c_int(int(ys[0])))
     return int(xs[0]), int(ys[0])
+
+
+def map_any_obstacle(xo, yo, xn, yn):
+    """Whether the window env_step sweeps between map coordinates (xo, yo) and (xn, yn) (position + start cell, as
+    float64) holds an obstacle of the map set_map() installed."""
+    return bool(lib().qo_map_any_obstacle(ctypes.c_double(xo), ctypes.c_double(yo), ctypes.c_double(xn),
+                                          ctypes.c_double(yn)))
