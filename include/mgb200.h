@@ -178,6 +178,7 @@ int mgb_quad_rollout_ex(mgb_quad *h, int32_t T, const float *act_dev, uint64_t a
 #define MGB_POLICY_MEMBER_WARP 32
 #define MGB_QUAD_POLICY_CTA_ENVS 64      /* quadrotor: 32 or a multiple of 64 envs per member */
 #define MGB_MAZE2D_POLICY_CTA_ENVS 128   /* MetaMaze2D: 32, 64 or a multiple of 128 envs per member */
+#define MGB_QUAD_RNN_CTA_ENVS 128        /* quadrotor, recurrent policies: 32, 64 or a multiple of 128 envs per member */
 
 typedef struct mgb_policy {
     const float *params_dev;  /* packed float32 on the handle's device, read at every launch */
@@ -623,6 +624,46 @@ int mgb_maze_rollout_rnn_critic(mgb_maze *h, int32_t T, const mgb_rnn_policy *po
                                 int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
                                 double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
                                 const mgb_critic *critic, void *stream);
+
+/* ---- recurrent quadrotor policies (DESIGN.md "Recurrent quadrotor policies") ---------------------------------------
+ * The cells of "recurrent policies" above (mgb_rnn_policy, unchanged) with a Gaussian head, driving a quadrotor handle
+ * with auto_reset on.  The packed buffer is the maze's (the cell, then the head, with its value row for the critic)
+ * followed by log_std [4], always, as for mgb_quad_rollout_policy.
+ *   Input of step t: x_t = [obs_t (D = 16, or 19 for velocity_control), then with feedback a_{t-1} (4), r_{t-1} (1)]:
+ *     the raw action the policy drew (as stored in act_out, not clamped) and the float32 reward.  The feedback entries
+ *     of the state row hold them; S = H + 5 (GRU) or 2H + 5 (LSTM), as on the maze.
+ *   Step t: h_t from the cell exactly as on the maze; mean = head(h_t); the action is drawn exactly as
+ *     mgb_quad_rollout_policy draws it (Philox counter (genv, t_base + t, MGB_STREAM_POLICY), Box-Muller, the same
+ *     logp), so one seed gives the same z for every quadrotor policy.  Then the whole state row (h, c and feedback) is
+ *     zeroed at every done (reset must be MGB_RNN_RESET_EPISODE: a quadrotor task never changes inside a launch);
+ *     otherwise h and c carry and the feedback becomes (a_t, r_t).
+ *   state_dev [n][S] float32: read at launch start, written back in place at launch end (4-byte aligned, not NULL).
+ *   state0_out_dev [n][S]: the state as read.  hid_out_dev [T][n][H]: h_t.  Both may be NULL.
+ *   act_out, logp_out, obs0_out, obs, rew, done, final_obs, truncated, seed: as mgb_quad_rollout_policy.  The env side
+ *   is bit for bit mgb_quad_rollout_ex fed act_out.  The step counter advances by T; nothing is allocated, and the call
+ *   can be captured in a CUDA graph.
+ *   Populations: as mgb_quad_rollout_population, with E = n / members 32, 64 or a multiple of MGB_QUAD_RNN_CTA_ENVS.
+ *   Critic: as mgb_quad_rollout_critic; final_value comes from the memory before the wipe (h_t, and the LSTM's c'_t):
+ *     the cell steps once more on [terminal obs, a_t, r_t].
+ * Refused (MGB_ERR_ARG; the handle, its step counter and the state untouched): everything mgb_quad_rollout_policy (and
+ * the population and critic calls) refuse, reset other than MGB_RNN_RESET_EPISODE, auto_reset off, a NULL or
+ * misaligned state_dev, hidden / feedback / head_hidden / head_width / activation / mode out of range, an unknown cell,
+ * and weights, observation tiles and columns of MGB_QUAD_RNN_CTA_ENVS envs beyond the device's opt-in shared memory
+ * (the message gives the byte count; DESIGN.md "Recurrent quadrotor policies" lists what fits). */
+int mgb_quad_rollout_rnn(mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed, float *state_dev,
+                         float *state0_out_dev, float *hid_out_dev, float *act_out_dev, float *logp_out_dev,
+                         float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                         uint8_t *truncated_dev, void *stream);
+int mgb_quad_rollout_rnn_population(mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                    int64_t member_stride, uint64_t seed, float *state_dev, float *state0_out_dev,
+                                    float *hid_out_dev, float *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                    float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                                    uint8_t *truncated_dev, void *stream);
+int mgb_quad_rollout_rnn_critic(mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                int64_t member_stride, uint64_t seed, float *state_dev, float *state0_out_dev,
+                                float *hid_out_dev, float *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                                float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                                uint8_t *truncated_dev, const mgb_critic *critic, void *stream);
 
 /* ---- recurrent cell sequences (DESIGN.md "Fused unroll") ----------------------------------------------------------
  * The learner's side of the recurrent policies: the cell of mgb_rnn_policy run over T given steps of n envs, forward and

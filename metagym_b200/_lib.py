@@ -79,6 +79,7 @@ RNN_CELL_GRU, RNN_CELL_LSTM = 0, 1           # MGB_RNN_CELL_*
 POLICY_MEMBER_WARP = 32                      # MGB_POLICY_MEMBER_WARP
 QUAD_POLICY_CTA_ENVS = 64                    # MGB_QUAD_POLICY_CTA_ENVS
 MAZE2D_POLICY_CTA_ENVS = 128                 # MGB_MAZE2D_POLICY_CTA_ENVS
+QUAD_RNN_CTA_ENVS = 128                      # MGB_QUAD_RNN_CTA_ENVS
 RNN_SEQ_CTA_ENVS = 128                       # MGB_RNN_SEQ_CTA_ENVS
 
 
@@ -105,6 +106,12 @@ SIGNATURES = {
                                                    vp, vp, vp, vp, vp, vp]),
     "mgb_quad_rollout_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_i32, c_i64, c_u64, vp, vp, vp, vp,
                                                vp, vp, vp, vp, ctypes.POINTER(Critic), vp]),
+    "mgb_quad_rollout_rnn": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_u64, vp, vp, vp, vp, vp, vp, vp,
+                                            vp, vp, vp, vp, vp]),
+    "mgb_quad_rollout_rnn_population": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64, vp,
+                                                       vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_quad_rollout_rnn_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64, vp, vp,
+                                                   vp, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.POINTER(Critic), vp]),
     "mgb_quad_state": (ctypes.c_int, [vp, vp, vp, ctypes.c_int, vp]),
     "mgb_quad_launch_count": (c_i64, [vp]),
     "mgb_quad_step_kernel": (ctypes.c_char_p, [vp]),

@@ -535,18 +535,13 @@ __device__ __forceinline__ void maze2d_window(const MazeConst &c, const uint8_t 
 // step's feedback, writing into the dead h0 column; the LSTM's head then uses the dead h1): that is final_value.  The task rule's cut is stored in adv for the epilogue.  After the loop (and after the state row is
 // stored, since the LSTM cell updates c in place) one more pass gives value_last, and the epilogue (mgb_gae) walks the
 // thread's column.
-constexpr int kPolMlp = 1, kPolGru = 2, kPolLstm = 3;
-
-template <int POL>
-using MazePolicyPlan = std::conditional_t<POL == kPolLstm, MgbRnn<4>, std::conditional_t<POL == kPolGru, MgbRnn<3>, MgbMlp>>;
-
 // VAL, step t of the thread's active env, after maze_logic and before env_reset: decides the cut from done and the
 // trial draw, stores the task rule's cut into adv, and where the cut fires on a truncated step stores V of the terminal
 // window (written into `row`, then the x column) into final_value.  Besides `row` and the x column's obs rows, which
 // the step refills, it clobbers only what the carry then wipes: the h columns, c and the feedback rows.
 template <int POL>
 __device__ __forceinline__ void maze2d_terminal_value(const MazeConst &c, const MazeArgs &a, const mgb_critic &cr,
-                                                      const MazePolicyPlan<POL> &pol, const float *pol_w, float *pol_x,
+                                                      const MgbPolicyPlan<POL> &pol, const float *pol_w, float *pol_x,
                                                       float *pol_y, float *hid_prev, float *hid_new, float *cst,
                                                       const uint8_t *blob, const int32_t *eaten, const Env &s, int t,
                                                       int64_t e, int D, int done, int action, double reward,
@@ -586,7 +581,7 @@ __device__ __forceinline__ void maze2d_terminal_value(const MazeConst &c, const 
 template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0, bool VAL = false>
 __global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel(
     const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
-    const __grid_constant__ MazePolicyPlan<POL> pol, const __grid_constant__ mgb_critic cr)
+    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ mgb_critic cr)
 {
     constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
     static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
@@ -4422,7 +4417,7 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
 // (with a critic: maze2d_rollout_kernel<0, true, REC, RS, POL, true>)
 template <bool REC, bool RS, int POL>
 static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r,
-                            const MazePolicyPlan<POL> &m, unsigned blocks, size_t sm, cudaStream_t st,
+                            const MgbPolicyPlan<POL> &m, unsigned blocks, size_t sm, cudaStream_t st,
                             const mgb_critic *critic)
 {
     const auto kernel = critic ? maze2d_rollout_kernel<0, true, REC, RS, POL, true>
@@ -4453,7 +4448,7 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
 // sampler workspaces.
 // A critic (the *_critic entry points, whose own() plans the value row; null for the others) is checked last.
 template <int POL, class Own>
-static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MazePolicyPlan<POL> &pol, Own own,
+static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MgbPolicyPlan<POL> &pol, Own own,
                                int32_t members, int64_t member_stride, uint64_t seed,
                                const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, int32_t *act_out_dev,
                                float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev,
@@ -4562,7 +4557,7 @@ static int maze_rollout_rnn(const char *fn, mgb_maze *h, int32_t T, const mgb_rn
     // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
     const auto run = [&](auto kind) {
         constexpr int POL = decltype(kind)::value;
-        MazePolicyPlan<POL> p;
+        MgbPolicyPlan<POL> p;
         const auto own = [&](int obs_dim) -> const char * {
             if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val)) return why;
             p.state = state_dev;

@@ -1,5 +1,5 @@
 // MLP policies evaluated inside a rollout launch (mgb_quad_rollout_policy, mgb_maze_rollout_policy; DESIGN.md
-// "Policy-driven rollouts"), and the recurrent policies of mgb_maze_rollout_rnn below.
+// "Policy-driven rollouts"), and the recurrent policies of mgb_maze_rollout_rnn and mgb_quad_rollout_rnn below.
 //
 // One thread owns one env.  The CTA stages the packed weights (mgb_policy.params_dev, torch.nn.Linear order) into shared
 // memory once per launch, regrouped so that a hidden layer's outputs are computed eight at a time: for output group g
@@ -277,7 +277,13 @@ struct MgbRnn {
     __host__ __device__ int HC() const { return NG == 4 ? 2 * H : H; }        // H + C: floats of h and c in a state row
 };
 
-// The plan of the categorical head: an MLP policy's own, or a recurrent policy's head
+// The policy kinds of the rollout kernels: none (0, open-loop), an MLP, a GRU or an LSTM, and the plan type of each
+constexpr int kPolMlp = 1, kPolGru = 2, kPolLstm = 3;
+
+template <int POL>
+using MgbPolicyPlan = std::conditional_t<POL == kPolLstm, MgbRnn<4>, std::conditional_t<POL == kPolGru, MgbRnn<3>, MgbMlp>>;
+
+// The plan of the action head: an MLP policy's own, or a recurrent policy's head
 template <class Plan>
 __host__ __device__ __forceinline__ auto &mgb_policy_head(Plan &p)
 {
@@ -299,10 +305,12 @@ static inline const char *mgb_rnn_check(const mgb_rnn_policy *p)
     return nullptr;
 }
 
-// Host: validate `p` and plan it for observation width `obs_dim` (`value`: the head's output layer has the value row).
-// Returns null, or the reason the policy is refused.
+// Host: validate `p` and plan it for observation width `obs_dim` (`value`: the head's output layer has the value row;
+// `log_std`: the buffer ends with log_std [4], the quadrotor's Gaussian head).  Returns null, or the reason the policy
+// is refused.
 template <int NG>
-static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, MgbRnn<NG> &r, bool value = false)
+static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, MgbRnn<NG> &r, bool value = false,
+                                       bool log_std = false)
 {
     if (const char *why = mgb_rnn_check(p)) return why;
     r = MgbRnn<NG>{};
@@ -322,7 +330,7 @@ static inline const char *mgb_rnn_plan(const mgb_rnn_policy *p, int obs_dim, Mgb
     r.s_head = r.s_b + 2 * NG * r.Hp;
     const mgb_policy hp = {p->params_dev + r.g_b + 2 * NG * r.H, p->head_hidden, {p->head_width, 0, 0}, p->activation,
                            p->mode};
-    if (const char *why = mgb_mlp_plan(&hp, r.H, false, r.head, value)) return why;
+    if (const char *why = mgb_mlp_plan(&hp, r.H, log_std, r.head, value)) return why;
     r.staged = r.s_head + r.head.staged;
     r.head.packed += r.g_b + 2 * NG * r.H;
     return nullptr;
@@ -378,7 +386,7 @@ static inline const char *mgb_population_plan(MgbMlp &head, int64_t n, int32_t m
     const int64_t E = n / members;
     if (E % MGB_POLICY_MEMBER_WARP != 0 || (E < cta ? cta % E : E % cta) != 0)
         return "envs per member (num_envs / members) must be a multiple of 32 that divides the policy CTA's envs or is a "
-               "multiple of them (MGB_QUAD_POLICY_CTA_ENVS, MGB_MAZE2D_POLICY_CTA_ENVS)";
+               "multiple of them (MGB_QUAD_POLICY_CTA_ENVS, MGB_QUAD_RNN_CTA_ENVS, MGB_MAZE2D_POLICY_CTA_ENVS)";
     if (member_stride < head.packed) return "member_stride is shorter than one member's packed policy";
     head.member_envs = E;
     head.member_stride = member_stride;

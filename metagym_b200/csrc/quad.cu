@@ -35,6 +35,8 @@ namespace {
 
 constexpr int kThreads = 64;   // scalar tile kernel / rollout kernel: envs per CTA
 static_assert(kThreads == MGB_QUAD_POLICY_CTA_ENVS, "include/mgb200.h publishes the policy CTA's env count");
+constexpr int kRnnThreads = 128;   // rollout kernel with a recurrent policy: envs per CTA (DESIGN.md "Recurrent quadrotor policies")
+static_assert(kRnnThreads == MGB_QUAD_RNN_CTA_ENVS, "include/mgb200.h publishes the recurrent policy CTA's env count");
 constexpr int kMaxObs = 19;
 
 // Constants derived on the host (double arithmetic, rounded once to float32 -- numpy's "weak python scalar" rule).
@@ -1153,20 +1155,30 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 // CTA: the one member of a population that drives the CTA's envs, or its pol.copies members back to back, each warp
 // reading its own (mgb_population_stage).  The step arithmetic after the action is the code the other instantiations
 // run.
-// VAL (POL and FIN only, mgb_quad_rollout_critic): the output layer has the value row (mgb_mlp_forward<true>).  Step t
-// stores V(s_t); a truncated step's terminal observation o[] goes through the policy once more before observe_reset
-// (final_value); after the loop one more pass gives value_last, and the epilogue (mgb_gae) walks the thread's column.
-template <bool SIMPLE, int XM, bool FIN, bool POL = false, bool VAL = false>
-__global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(const __grid_constant__ QuadConst c,
-                                                                          const __grid_constant__ QuadArgs a,
-                                                                          const __grid_constant__ MgbMlp pol,
-                                                                          const __grid_constant__ mgb_critic cr)
+// POL == kPolGru or kPolLstm (mgb_quad_rollout_rnn): the policy is the recurrent `pol` (MgbRnn, mgb_policy.cuh) with a
+// Gaussian head, in CTAs of kRnnThreads envs.  Its dynamic shared memory holds the staged cell, head and log_std (of each
+// staged member), then the columns x, c, h0, h1 and w (mgb_policy.cuh).  The obs rows of x are filled as for the MLP; at
+// t = 0 the state row fills h0, c and the feedback rows of x.  Step t computes h1 from (x, h0, c), updating c in place,
+// and acts on head(h1), whose hidden layer goes to w (GRU) or the dead h0 (LSTM).  Right after the step the carry
+// zeroes h1 and c where done, writes the feedback rows (a_t, r_t) (zeros where done) and swaps h0 and h1; the state row
+// is stored once, after step T - 1.
+// VAL (POL and FIN only, mgb_quad_rollout_critic, mgb_quad_rollout_rnn_critic): the output layer has the value row
+// (mgb_mlp_forward<true>).  Step t stores V(s_t); a truncated step's terminal observation o[] goes through the policy
+// once more before observe_reset (final_value; a recurrent cell steps from h_t and c'_t on [o, a_t, r_t] into the dead
+// h0, before the carry wipes); after the loop (and after the state row is stored, since the LSTM cell updates c in
+// place) one more pass gives value_last, and the epilogue (mgb_gae) walks the thread's column.
+template <bool SIMPLE, int XM, bool FIN, int POL = 0, bool VAL = false>
+__global__ void __launch_bounds__(POL >= kPolGru ? kRnnThreads : kThreads, POL >= kPolGru ? 1 : POL ? 3 : 8)
+quad_rollout_kernel(const __grid_constant__ QuadConst c, const __grid_constant__ QuadArgs a,
+                    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ mgb_critic cr)
 {
+    constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
+    constexpr int CTA = RNN ? kRnnThreads : kThreads;
     static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
-    __shared__ __align__(128) float tiles[2][kThreads * kMaxObs];
-    const int64_t e0 = (int64_t)blockIdx.x * kThreads;
+    __shared__ __align__(128) float tiles[2][CTA * kMaxObs];
+    const int64_t e0 = (int64_t)blockIdx.x * CTA;
     const int64_t e = e0 + threadIdx.x;
-    const int rows = (int)((a.n - e0) < kThreads ? (a.n - e0) : kThreads);
+    const int rows = (int)((a.n - e0) < CTA ? (a.n - e0) : CTA);
     const int D = c.obs_dim;
     const bool active = e < a.n;
     QState s;
@@ -1179,14 +1191,23 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
     const int64_t genv = a.env_base + e;
     const int task = active ? env_task(c, a, e) : 0;
     const float *pol_w = nullptr;           // the staged weights (mgb_population_weights)
-    float *pol_x = nullptr, *pol_y = nullptr;   // the two activation buffers
+    float *pol_x = nullptr, *pol_y = nullptr;   // the two activation buffers (RNN: the input and the w column)
+    float *hid_prev = nullptr, *hid_new = nullptr, *cst = nullptr;  // RNN: the columns h0, h1 and c
+    const MgbMlp &head = mgb_policy_head(pol);  // the plan of the Gaussian head
     if constexpr (POL) {
         static_assert(!POL || XM == 0, "policy rollouts are not mirrored");
         extern __shared__ __align__(16) float pol_smem[];
-        pol_x = pol_smem + pol.copies * pol.staged;
-        pol_y = pol_x + pol.maxw * kThreads;
+        pol_x = pol_smem + head.copies * pol.staged;
+        if constexpr (RNN) {
+            cst = pol_x + pol.in * CTA;
+            hid_prev = cst + pol.C() * CTA;
+            hid_new = hid_prev + pol.Hr * CTA;
+            pol_y = hid_new + pol.Hr * CTA;     // w; the LSTM's head uses the dead h0 instead
+        } else {
+            pol_y = pol_x + pol.maxw * kThreads;
+        }
         pol_w = pol_smem;
-        mgb_population_stage(pol, pol_smem, e0, rows, kThreads);
+        mgb_population_stage(pol, pol_smem, e0, rows, CTA);
         if (active) {       // the observation of the loaded state: what the preceding reset() / step() returned
             float o[kMaxObs], bv[3], Ri[9];
             observe(c, s, adj, id, o, bv, Ri);
@@ -1196,11 +1217,20 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
             }
 #pragma unroll
             for (int k = 0; k < kMaxObs; ++k)
-                if (k < D) pol_x[k * kThreads + threadIdx.x] = o[k];
-            if (pol.obs0_out) {
+                if (k < D) pol_x[k * CTA + threadIdx.x] = o[k];
+            if (head.obs0_out) {
 #pragma unroll
                 for (int k = 0; k < kMaxObs; ++k)
-                    if (k < D) pol.obs0_out[e * D + k] = o[k];
+                    if (k < D) head.obs0_out[e * D + k] = o[k];
+            }
+            if constexpr (RNN) {        // [h, c, feedback]
+                const int S = pol.HC() + 5 * pol.feedback;
+                const float *st = pol.state + e * S;
+                for (int k = 0; k < pol.H; ++k) hid_prev[k * CTA + threadIdx.x] = st[k];
+                for (int k = 0; k < pol.C(); ++k) cst[k * CTA + threadIdx.x] = st[pol.H + k];
+                for (int k = pol.HC(); k < S; ++k) pol_x[(D + k - pol.HC()) * CTA + threadIdx.x] = st[k];
+                if (pol.state0_out)
+                    for (int k = 0; k < S; ++k) pol.state0_out[e * S + k] = st[k];
             }
         }
     }
@@ -1217,14 +1247,24 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
             float4 act;
             if constexpr (POL) {
                 float mean[4], av[4], lp, v;
-                mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
-                    mgb_mlp_forward<VAL>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, mean, &v);
-                    lp = mgb_gaussian_action(pol, w, genv, a.t_base + (uint32_t)t, mean, av);
+                mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
+                    if constexpr (RNN) {
+                        mgb_rnn_cell(pol, w, pol_x, hid_prev, cst, hid_new, CTA, threadIdx.x);
+                        if (pol.hid_out)
+                            for (int k = 0; k < pol.H; ++k)
+                                pol.hid_out[((int64_t)t * a.n + e) * pol.H + k] = hid_new[k * CTA + threadIdx.x];
+                        if constexpr (POL == kPolLstm) pol_y = hid_prev;   // dead until the carry makes it the next h
+                        mgb_mlp_forward<VAL>(head, w + pol.s_head, hid_new, pol_y, CTA, threadIdx.x, mean, &v);
+                        lp = mgb_gaussian_action(head, w + pol.s_head, genv, a.t_base + (uint32_t)t, mean, av);
+                    } else {
+                        mgb_mlp_forward<VAL>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, mean, &v);
+                        lp = mgb_gaussian_action(pol, w, genv, a.t_base + (uint32_t)t, mean, av);
+                    }
                 });
                 if constexpr (VAL) cr.value_dev[(int64_t)t * a.n + e] = v;
                 act = make_float4(av[0], av[1], av[2], av[3]);
                 if (a.act_out) reinterpret_cast<float4 *>(a.act_out)[(int64_t)t * a.n + e] = act;
-                if (pol.logp_out) pol.logp_out[(int64_t)t * a.n + e] = lp;
+                if (head.logp_out) head.logp_out[(int64_t)t * a.n + e] = lp;
             } else if (a.act) {
                 act = act_next;
                 if (t + 1 < a.T) act_next = __ldg(reinterpret_cast<const float4 *>(a.act) + (int64_t)(t + 1) * a.n + e);
@@ -1269,10 +1309,21 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
                 if (wf[0] && trunc[0]) {
 #pragma unroll
                     for (int k = 0; k < kMaxObs; ++k)
-                        if (k < D) pol_x[k * kThreads + threadIdx.x] = o[k];
+                        if (k < D) pol_x[k * CTA + threadIdx.x] = o[k];
                     float out4[4], v;
-                    mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
-                        mgb_mlp_forward<true>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, out4, &v);
+                    mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
+                        if constexpr (RNN) {
+                            if (pol.feedback) {
+                                float *fb = pol_x + D * CTA + threadIdx.x;
+                                fb[0] = act.x; fb[CTA] = act.y; fb[2 * CTA] = act.z; fb[3 * CTA] = act.w;
+                                fb[4 * CTA] = reward;
+                            }
+                            mgb_rnn_cell(pol, w, pol_x, hid_new, cst, hid_prev, CTA, threadIdx.x);
+                            mgb_mlp_forward<true>(head, w + pol.s_head, hid_prev, POL == kPolLstm ? hid_new : pol_y, CTA,
+                                                  threadIdx.x, out4, &v);
+                        } else {
+                            mgb_mlp_forward<true>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, out4, &v);
+                        }
                     });
                     if (cr.final_value_dev) cr.final_value_dev[(int64_t)t * a.n + e] = v;
                 }
@@ -1300,7 +1351,23 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
             if constexpr (POL) {       // the policy's input at step t + 1
 #pragma unroll
                 for (int k = 0; k < kMaxObs; ++k)
-                    if (k < D) pol_x[k * kThreads + threadIdx.x] = o[k];
+                    if (k < D) pol_x[k * CTA + threadIdx.x] = o[k];
+            }
+            if constexpr (RNN) {       // the carry: every done wipes the whole row (MGB_RNN_RESET_EPISODE)
+                const bool wipe = done[0] != 0;
+                if (wipe) {
+                    for (int k = 0; k < pol.H; ++k) hid_new[k * CTA + threadIdx.x] = 0.f;
+                    for (int k = 0; k < pol.C(); ++k) cst[k * CTA + threadIdx.x] = 0.f;
+                }
+                if (pol.feedback) {
+                    float *fb = pol_x + D * CTA + threadIdx.x;
+                    fb[0] = wipe ? 0.f : act.x; fb[CTA] = wipe ? 0.f : act.y;
+                    fb[2 * CTA] = wipe ? 0.f : act.z; fb[3 * CTA] = wipe ? 0.f : act.w;
+                    fb[4 * CTA] = wipe ? 0.f : reward;
+                }
+                float *const tmp = hid_prev;
+                hid_prev = hid_new;
+                hid_new = tmp;
             }
         }
         if (XM == 2) {
@@ -1317,11 +1384,26 @@ __global__ void __launch_bounds__(kThreads, POL ? 3 : 8) quad_rollout_kernel(con
         }
     }
     if (active) store_state(a, e, s);
+    if constexpr (RNN) {
+        if (active) {
+            const int S = pol.HC() + 5 * pol.feedback;
+            float *st = pol.state + e * S;
+            for (int k = 0; k < pol.H; ++k) st[k] = hid_prev[k * CTA + threadIdx.x];
+            for (int k = 0; k < pol.C(); ++k) st[pol.H + k] = cst[k * CTA + threadIdx.x];
+            for (int k = pol.HC(); k < S; ++k) st[k] = pol_x[(D + k - pol.HC()) * CTA + threadIdx.x];
+        }
+    }
     if constexpr (VAL) {
         if (active) {
             float out4[4], v;
-            mgb_population_weights(pol, pol_w, pol.staged, [&](const float *w) {
-                mgb_mlp_forward<true>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, out4, &v);
+            mgb_population_weights(head, pol_w, pol.staged, [&](const float *w) {
+                if constexpr (RNN) {
+                    mgb_rnn_cell(pol, w, pol_x, hid_prev, cst, hid_new, CTA, threadIdx.x);
+                    mgb_mlp_forward<true>(head, w + pol.s_head, hid_new, POL == kPolLstm ? hid_prev : pol_y, CTA,
+                                          threadIdx.x, out4, &v);
+                } else {
+                    mgb_mlp_forward<true>(pol, w, pol_x, pol_y, kThreads, threadIdx.x, out4, &v);
+                }
             });
             if (cr.value_last_dev) cr.value_last_dev[e] = v;
             if (cr.adv_dev) mgb_gae(cr, a.T, a.n, e, v, a.rew, a.done, a.truncated, false);
@@ -1866,52 +1948,59 @@ static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_se
     return MGB_OK;
 }
 
-// A policy rollout of `members` policies (one: mgb_quad_rollout_policy), refused as `fn`; with a critic (the value
-// heads of mgb_quad_rollout_critic, null for the other entry points) the policy has the value row
-static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
+// A policy rollout of kind POL with `members` policies of the plan `m` (one: mgb_quad_rollout_policy,
+// mgb_quad_rollout_rnn), refused as `fn`.  The checks, in order: the handle, T, then own() (the entry point plans the
+// policy into m and makes its own checks; it returns the refusal, or nullptr), the population, logp_out in the mean mode,
+// mirrors, final_obs, the alignments, the critic (with `val`, the *_critic entry points, whose own() plans the value row),
+// the handle's state and the footprint.
+template <int POL, class Own>
+static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, MgbPolicyPlan<POL> &m, Own own, int32_t members,
                           int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
                           float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
                           uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
 {
+    constexpr int CTA = POL >= kPolGru ? kRnnThreads : kThreads;
     const auto refuse = [&](const char *why) {
         mgb_set_error("%s: %s", fn, why);
         return MGB_ERR_ARG;
     };
     if (!h) return refuse("null handle");
     if (T <= 0) return refuse("T must be positive");
-    MgbMlp m;
-    if (const char *why = mgb_mlp_plan(pol, h->c.obs_dim, true, m, val)) return refuse(why);
-    if (const char *why = mgb_population_plan(m, h->n, members, member_stride, kThreads)) return refuse(why);
-    if (logp_out_dev && m.mode != MGB_POLICY_SAMPLE)
+    if (const char *why = own(h->c.obs_dim)) return refuse(why);
+    MgbMlp &head = mgb_policy_head(m);
+    if (const char *why = mgb_population_plan(head, h->n, members, member_stride, CTA)) return refuse(why);
+    if (logp_out_dev && head.mode != MGB_POLICY_SAMPLE)
         return refuse("logp_out needs MGB_POLICY_SAMPLE (the mean mode draws nothing)");
     if (h->mir.count != 0)
         return refuse("policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)");
     if (final_obs_dev && !h->auto_reset)
         return refuse("final_obs needs auto_reset on (without it obs already is the terminal observation)");
     if ((reinterpret_cast<uintptr_t>(act_out_dev) & 15u) != 0) return refuse("act_out_dev must be 16-byte aligned");
-    if ((reinterpret_cast<uintptr_t>(pol->params_dev) & 3u) != 0) return refuse("params_dev must be 4-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(m.params) & 3u) != 0) return refuse("params_dev must be 4-byte aligned");
     if (val) {
         if (const char *why = mgb_critic_check(critic, h->auto_reset, rew_dev, done_dev, truncated_dev)) return refuse(why);
     }
     int rc = check_ready(h);
     if (rc) return rc;
     MgbDeviceGuard guard(h->device);
-    m.seed = seed;
-    m.logp_out = logp_out_dev;
-    m.obs0_out = obs0_out_dev;
+    head.seed = seed;
+    head.logp_out = logp_out_dev;
+    head.obs0_out = obs0_out_dev;
     const bool fin = final_obs_dev || truncated_dev;
     const auto kernel = with_simple(h, [&](auto simple) {
-        return val ? quad_rollout_kernel<simple, 0, true, true, true>
-               : fin ? quad_rollout_kernel<simple, 0, true, true> : quad_rollout_kernel<simple, 0, false, true>;
+        return val ? quad_rollout_kernel<simple, 0, true, POL, true>
+               : fin ? quad_rollout_kernel<simple, 0, true, POL> : quad_rollout_kernel<simple, 0, false, POL>;
     });
-    const size_t smem = mgb_mlp_smem_bytes(m, kThreads);
+    size_t smem;
+    if constexpr (POL == kPolMlp) smem = mgb_mlp_smem_bytes(m, CTA);
+    else smem = mgb_rnn_smem_bytes(m, CTA);
     int optin = 0;
     MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
     cudaFuncAttributes fa;
     MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
     if (fa.sharedSizeBytes + smem > (size_t)optin) {
         mgb_set_error("%s: the policy needs %zu bytes of shared memory per CTA (weights and activations of %d envs), "
-                      "above the device's %d", fn, fa.sharedSizeBytes + smem, kThreads, optin);
+                      "above the device's %d", fn, fa.sharedSizeBytes + smem, CTA, optin);
         return MGB_ERR_ARG;
     }
     MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1919,12 +2008,94 @@ static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, const mgb_poli
     a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev;
     a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
     a.final_obs = final_obs_dev; a.truncated = truncated_dev;
-    const unsigned blocks = (unsigned)((a.n + kThreads - 1) / kThreads);
-    kernel<<<blocks, kThreads, smem, (cudaStream_t)stream>>>(h->c, a, m, val ? *critic : mgb_critic{});
+    const unsigned blocks = (unsigned)((a.n + CTA - 1) / CTA);
+    kernel<<<blocks, CTA, smem, (cudaStream_t)stream>>>(h->c, a, m, val ? *critic : mgb_critic{});
     MGB_CUDA(cudaGetLastError());
     h->t_base += (uint32_t)T;
     h->launches += 1;
     return MGB_OK;
+}
+
+// mgb_quad_rollout_policy of `members` MLP policies (one: mgb_quad_rollout_policy), refused as `fn`
+static int rollout_mlp(const char *fn, mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
+                       int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
+                       float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                       uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
+{
+    MgbMlp m;
+    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, true, m, val); };
+    return rollout_policy<kPolMlp>(fn, h, T, m, own, members, member_stride, seed, act_out_dev, logp_out_dev,
+                                   obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream,
+                                   critic, val);
+}
+
+// mgb_quad_rollout_rnn of `members` recurrent policies (one: mgb_quad_rollout_rnn), refused as `fn`
+static int rollout_rnn(const char *fn, mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                       int64_t member_stride, uint64_t seed, float *state_dev, float *state0_out_dev,
+                       float *hid_out_dev, float *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
+                       float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
+                       uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
+{
+    // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
+    const auto run = [&](auto kind) {
+        constexpr int POL = decltype(kind)::value;
+        MgbPolicyPlan<POL> p;
+        const auto own = [&](int obs_dim) -> const char * {
+            if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val, true)) return why;
+            if (pol->reset != MGB_RNN_RESET_EPISODE)
+                return "the quadrotor's recurrent rollout needs reset = MGB_RNN_RESET_EPISODE (its tasks never change "
+                       "inside a launch)";
+            if (!state_dev) return "null state";
+            if ((uintptr_t)state_dev % sizeof(float)) return "state must be 4-byte aligned";
+            if (!h->auto_reset)
+                return "the recurrent rollout needs auto_reset on (an episode boundary has no next step without it)";
+            p.state = state_dev;
+            p.state0_out = state0_out_dev;
+            p.hid_out = hid_out_dev;
+            return nullptr;
+        };
+        return rollout_policy<POL>(fn, h, T, p, own, members, member_stride, seed, act_out_dev, logp_out_dev,
+                                   obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream,
+                                   critic, val);
+    };
+    return pol && pol->cell == MGB_RNN_CELL_LSTM ? run(std::integral_constant<int, kPolLstm>{})
+                                                 : run(std::integral_constant<int, kPolGru>{});
+}
+
+extern "C" int mgb_quad_rollout_rnn(mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, uint64_t seed, float *state_dev,
+                                    float *state0_out_dev, float *hid_out_dev, float *act_out_dev, float *logp_out_dev,
+                                    float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev,
+                                    float *final_obs_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_rnn");
+    return rollout_rnn(__func__, h, T, pol, 1, 0, seed, state_dev, state0_out_dev, hid_out_dev, act_out_dev,
+                       logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
+}
+
+extern "C" int mgb_quad_rollout_rnn_population(mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                               int64_t member_stride, uint64_t seed, float *state_dev,
+                                               float *state0_out_dev, float *hid_out_dev, float *act_out_dev,
+                                               float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev,
+                                               uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                               void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_rnn_population");
+    return rollout_rnn(__func__, h, T, pol, members, member_stride, seed, state_dev, state0_out_dev, hid_out_dev,
+                       act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev,
+                       truncated_dev, stream);
+}
+
+extern "C" int mgb_quad_rollout_rnn_critic(mgb_quad *h, int32_t T, const mgb_rnn_policy *pol, int32_t members,
+                                           int64_t member_stride, uint64_t seed, float *state_dev,
+                                           float *state0_out_dev, float *hid_out_dev, float *act_out_dev,
+                                           float *logp_out_dev, float *obs0_out_dev, float *obs_dev, float *rew_dev,
+                                           uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
+                                           const mgb_critic *critic, void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_rollout_rnn_critic");
+    return rollout_rnn(__func__, h, T, pol, members, member_stride, seed, state_dev, state0_out_dev, hid_out_dev,
+                       act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev,
+                       truncated_dev, stream, critic, true);
 }
 
 extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy *pol, uint64_t seed, float *act_out_dev,
@@ -1932,8 +2103,8 @@ extern "C" int mgb_quad_rollout_policy(mgb_quad *h, int32_t T, const mgb_policy 
                                        uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_quad_rollout_policy");
-    return rollout_policy(__func__, h, T, pol, 1, 0, seed, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
-                          done_dev, final_obs_dev, truncated_dev, stream);
+    return rollout_mlp(__func__, h, T, pol, 1, 0, seed, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
+                       done_dev, final_obs_dev, truncated_dev, stream);
 }
 
 extern "C" int mgb_quad_rollout_population(mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
@@ -1942,8 +2113,8 @@ extern "C" int mgb_quad_rollout_population(mgb_quad *h, int32_t T, const mgb_pol
                                            float *final_obs_dev, uint8_t *truncated_dev, void *stream)
 {
     MgbRange nvtx_range("mgb_quad_rollout_population");
-    return rollout_policy(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
-                          obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
+    return rollout_mlp(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
+                       obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
 }
 
 extern "C" int mgb_quad_rollout_critic(mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
@@ -1953,8 +2124,8 @@ extern "C" int mgb_quad_rollout_critic(mgb_quad *h, int32_t T, const mgb_policy 
                                        void *stream)
 {
     MgbRange nvtx_range("mgb_quad_rollout_critic");
-    return rollout_policy(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
-                          obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream, critic, true);
+    return rollout_mlp(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
+                       obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream, critic, true);
 }
 
 extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,

@@ -789,6 +789,8 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
                              % type(policy).__name__)
         if state is not None and not recurrent:
             raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
+        if recurrent and policy.dist != "categorical":
+            raise ValueError("a Gaussian recurrent policy drives the quadrotor; MetaMaze2D takes dist=\"categorical\"")
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")

@@ -9,7 +9,9 @@ read at every launch, so ``update()`` after an optimiser step is seen by a rollo
 
 GRUPolicy and LSTMPolicy pack an ``nn.GRUCell`` or an ``nn.LSTMCell`` and a head for the recurrent MetaMaze2D rollout
 (mgb_maze_rollout_rnn; DESIGN.md "Recurrent policies"): ``weight_ih``, ``weight_hh``, ``bias_ih``, ``bias_hh``, then the
-head's layers as MLPPolicy packs them.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities
+head's layers as MLPPolicy packs them.  With dist="gaussian" they drive the quadrotor instead (mgb_quad_rollout_rnn;
+DESIGN.md "Recurrent quadrotor policies"): the head's four outputs are the mean of a Gaussian, the feedback is the raw
+previous action and reward, and ``log_std [4]`` goes last, as MLPPolicy packs it.  ``unroll()`` recomputes a recurrent rollout's logits and log-probabilities
 with autograd, running a float32 CUDA cell through the fused cell sequence (metagym_b200.cell_seq; DESIGN.md "Fused
 unroll") and any other cell through a torch loop over the steps.
 
@@ -196,9 +198,18 @@ class MLPPolicy(object):
                            _lib.POLICY_MEAN if deterministic else _lib.POLICY_SAMPLE)
 
 
-FEEDBACK = 5        # onehot(prev action) (4) + prev reward (1)
+FEEDBACK = 5        # onehot(prev action) or the raw prev action (4) + prev reward (1)
 MAX_RNN_HIDDEN = 64  # MGB_RNN_MAX_HIDDEN
 _RESETS = {"episode": _lib.RNN_RESET_EPISODE, "task": _lib.RNN_RESET_TASK}
+_DISTS = ("categorical", "gaussian")
+LOG_2PI_2 = 3.6757541328186907    # 2 log(2 pi): the constant of a 4-dimensional Gaussian log-density
+
+
+def gaussian_logp(act, mean, log_std):
+    """log N(act; mean, exp(log_std)^2) summed over the last axis of four: sum_k (-((a - mean) / sigma)^2 / 2 - log_std_k)
+    - 2 log(2 pi), the logp of the quadrotor's policy rollouts (autograd flows through mean and log_std)."""
+    z = (act - mean) / log_std.exp()
+    return (-0.5 * z * z - log_std).sum(-1) - LOG_2PI_2
 
 
 def _head_layers(head, H, name="GRUPolicy"):
@@ -226,18 +237,25 @@ class _RecurrentPolicy(object):
     _cell_code = 0      # MGB_RNN_CELL_*
 
     def __init__(self, cell, head, log_std=None, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None,
-                 device="cuda", value=None):
+                 device="cuda", value=None, dist="categorical"):
         import torch
         self._torch = torch
         name, kind = type(self).__name__, self._torch_cell()
         if type(cell) is not kind:
             raise ValueError("%s takes an nn.%s, got %s" % (name, kind.__name__, type(cell).__name__))
-        if log_std is not None:
+        if dist not in _DISTS:
+            raise ValueError("%s: dist must be \"categorical\" (MetaMaze2D) or \"gaussian\" (the quadrotor)" % name)
+        if log_std is not None and dist != "gaussian":
             raise ValueError("%s: the MetaMaze2D head is categorical and has no log_std" % name)
         if feedback not in (True, False, 0, 1):
             raise ValueError("%s: feedback must be True or False" % name)
         if hidden_reset not in _RESETS:
             raise ValueError("%s: hidden_reset must be \"episode\" or \"task\"" % name)
+        if dist == "gaussian" and hidden_reset != "episode":
+            raise ValueError("%s: a Gaussian (quadrotor) policy needs hidden_reset=\"episode\" (a quadrotor task never "
+                             "changes inside a launch)" % name)
+        self.dist = dist
+        self.gaussian = dist == "gaussian"
         self.feedback = bool(feedback)
         self.hidden_reset = hidden_reset
         self.hidden = cell.hidden_size
@@ -253,11 +271,13 @@ class _RecurrentPolicy(object):
         self._value = _value_head(value, lin[-1].in_features, name)
         self.has_value = self._value is not None
         self.numel = (self._gates * H * (n_in + H + 2) + sum(m.out_features * (m.in_features + 1) for m in lin)
-                      + (lin[-1].in_features + 1 if self.has_value else 0))
+                      + (lin[-1].in_features + 1 if self.has_value else 0) + (N_OUT if self.gaussian else 0))
         self.device = torch.device(device)
         self.params = torch.zeros(self.numel, dtype=torch.float32, device=self.device)
+        self.has_log_std = False
         self._cell, self._head, self._mean, self._std = cell, head, None, None
-        self.update(cell, head, obs_mean, obs_std)
+        self._log_std, self._log_std_arg = None, None
+        self.update(cell, head, obs_mean, obs_std, log_std=log_std)
 
     def _torch_cell(self):
         raise NotImplementedError
@@ -290,13 +310,20 @@ class _RecurrentPolicy(object):
             if k == len(lin) - 1:
                 W, b = _cat_value(W, b, self._value)
             parts += [W.reshape(-1), b]
+        if self.gaussian:
+            parts.append(self._log_std if self._log_std is not None else torch.zeros(N_OUT, dtype=torch.float64))
         return torch.cat(parts).to(torch.float32)
 
-    def update(self, cell=None, head=None, obs_mean=None, obs_std=None, value=None):
+    def update(self, cell=None, head=None, obs_mean=None, obs_std=None, value=None, log_std=None):
         """Repack into the same device buffer (copy_, stream-ordered): a graph captured on this policy sees the new
         weights.  Arguments left None keep their previous values; cell and head must keep their shapes, and a value
-        head can only replace the policy's own."""
+        head can only replace the policy's own.  log_std [4]: a Gaussian policy's log standard deviations (unroll()
+        differentiates through the tensor passed here)."""
         name = type(self).__name__
+        if log_std is not None:
+            if not self.gaussian:
+                raise ValueError("%s: the MetaMaze2D head is categorical and has no log_std" % name)
+            self._vec(log_std, N_OUT, "log_std")
         if cell is not None and (type(cell) is not self._torch_cell() or cell.input_size != self._cell.input_size
                                  or cell.hidden_size != self.hidden):
             raise ValueError("%s.update: the cell must keep its input and hidden sizes" % name)
@@ -324,6 +351,10 @@ class _RecurrentPolicy(object):
             self._std = std
         if value is not None:
             self._value = value
+        if log_std is not None:
+            self._log_std = self._vec(log_std, N_OUT, "log_std")
+            self._log_std_arg = log_std
+            self.has_log_std = True
         self.params.copy_(self.pack(), non_blocking=False)
         return self
 
@@ -344,7 +375,8 @@ class _RecurrentPolicy(object):
     def unroll(self, out, value=False):
         """Recompute a recurrent rollout with autograd through the cell and head: returns (logits [T, N, 4],
         logp [T, N]), logp the log-probability of out["act"], and with value=True (a policy with a value head) also
-        value [T, N], V(s_t).  Uses out's obs0, obs, act, rew, done, state0 and
+        value [T, N], V(s_t).  A Gaussian policy returns (mean [T, N, 4], logp [T, N]) instead, and autograd also
+        reaches the log_std tensor it was given.  Uses out's obs0, obs, act, rew, done, state0 and
         resampled (and on a trial handle task_episodes0 and episodes_per_task), and applies the kernel's input
         construction and reset rule, in the cell's dtype and device.  A float32 cell on CUDA runs through the fused
         cell sequence (metagym_b200.cell_seq; DESIGN.md "Fused unroll"), with the head batched over all T N rows; any
@@ -363,10 +395,19 @@ class _RecurrentPolicy(object):
         for m in mods[:-1]:
             z = m(z)
         logits = mods[-1](z)
-        logp = torch.log_softmax(logits, -1).gather(2, act[..., None])[..., 0]
+        logp = self._logp(logits, act)
         if value:
             return logits, logp, self._value(z)[..., 0]
         return logits, logp
+
+    def _logp(self, out4, act):
+        """log pi(act) of the head's outputs out4 [..., 4]: the categorical logits, or the Gaussian mean with log_std."""
+        torch = self._torch
+        if not self.gaussian:
+            return torch.log_softmax(out4, -1).gather(-1, act[..., None])[..., 0]
+        ls = self._log_std_arg if self._log_std_arg is not None else torch.zeros(N_OUT)
+        ls = torch.as_tensor(ls).reshape(N_OUT).to(out4.device, out4.dtype)
+        return gaussian_logp(act, out4, ls)
 
     def _unroll_inputs(self, out):
         """(obs [T, N, D] normalised, act [T, N] int64, rew [T, N] as the kernel feeds it back, wipe [T, N] bool, state0
@@ -376,8 +417,8 @@ class _RecurrentPolicy(object):
         D = self.obs_dim
         w = self._cell.weight_ih
         dt, dev = w.dtype, w.device
-        act = out["act"].to(dev).long()
-        T, N = act.shape
+        act = out["act"].to(dev, dt) if self.gaussian else out["act"].to(dev).long()
+        T, N = act.shape[:2]
         obs = torch.cat([out["obs0"].reshape(1, N, -1), out["obs"][:T - 1].reshape(T - 1, N, -1)], 0).to(dev, dt)
         if self._mean is not None or self._std is not None:
             mean = self._mean if self._mean is not None else torch.zeros(D, dtype=torch.float64)
@@ -391,13 +432,17 @@ class _RecurrentPolicy(object):
 
     def _cell_input(self, obs, act, rew, wipe, state0):
         """x [T, N, in] of every step at once: the observation, then with feedback state0's feedback at t = 0 and
-        (onehot(a_{t-1}), r_{t-1}) after, zeros where wipe[t-1]."""
+        (onehot(a_{t-1}) or the Gaussian's raw a_{t-1}, r_{t-1}) after, zeros where wipe[t-1]."""
         if not self.feedback:
             return obs
         torch = self._torch
-        fb = torch.cat([torch.nn.functional.one_hot(act, 4).to(obs.dtype), rew[..., None]], 2)
+        fb = torch.cat([self._action_feedback(act).to(obs.dtype), rew[..., None]], -1)
         fb = fb.masked_fill(wipe[..., None], 0.)
         return torch.cat([obs, torch.cat([state0[None, :, self._memory * self.hidden:], fb[:-1]], 0)], 2)
+
+    def _action_feedback(self, act):
+        """The four feedback entries of the actions act: onehot(act), or the Gaussian's raw actions."""
+        return act if self.gaussian else self._torch.nn.functional.one_hot(act, 4)
 
     def _unroll_reference(self, out, value=False):
         """unroll() as a torch loop over the steps: the path of CPU and float64 cells and of cells beyond the kernels'
@@ -408,7 +453,7 @@ class _RecurrentPolicy(object):
         head = self._head
         dt = self._cell.weight_ih.dtype
         obs, act, rew, wipe, state0 = self._unroll_inputs(out)
-        T, N = act.shape
+        T, N = act.shape[:2]
         nm = self._memory * self.hidden
         mem, fb = state0[:, :nm], state0[:, nm:]
         logits, logp, vals = [], [], []
@@ -423,11 +468,11 @@ class _RecurrentPolicy(object):
             if value:
                 vals.append(self._value(z)[:, 0])
             logits.append(lg)
-            logp.append(torch.log_softmax(lg, -1).gather(1, act[t][:, None])[:, 0])
+            logp.append(self._logp(lg, act[t]))
             keep = ~wipe[t]
             mem = torch.where(keep[:, None], new_mem, torch.zeros_like(new_mem))
             if self.feedback:
-                new_fb = torch.cat([torch.nn.functional.one_hot(act[t], 4).to(dt), rew[t][:, None]], 1)
+                new_fb = torch.cat([self._action_feedback(act[t]).to(dt), rew[t][:, None]], 1)
                 fb = torch.where(keep[:, None], new_fb, torch.zeros_like(new_fb))
         if value:
             return torch.stack(logits), torch.stack(logp), torch.stack(vals)
@@ -446,6 +491,11 @@ class GRUPolicy(_RecurrentPolicy):
     obs_mean / obs_std: optional [obs_dim] normalisation (x - mean) / std of the observation inputs, folded into the
     obs columns of weight_ih and into bias_ih on the host in float64.  device: where the packed buffer lives.
     The carried state is [N, H + 5 feedback] = [h, onehot(prev action), prev reward].
+
+    dist="gaussian" makes it a quadrotor policy (BatchedQuadrotor.rollout(policy=, state=); mgb_quad_rollout_rnn): the
+    head's four outputs are the mean of the Gaussian the actions are drawn from, log_std [4] (optional; without it only
+    deterministic rollouts run) is packed last, the feedback is (a_{t-1}, r_{t-1}) with the raw action drawn, and
+    hidden_reset must be "episode".  The cell then takes obs_dim (16, or 19 for velocity_control) + 5 inputs.
     """
     _gates, _memory, _cell_code = 3, 1, _lib.RNN_CELL_GRU
 
@@ -461,13 +511,15 @@ class LSTMPolicy(_RecurrentPolicy):
     """A torch LSTMCell and head packed for the recurrent MetaMaze2D rollout (BatchedMetaMaze2D.rollout(policy=,
     state=)): GRUPolicy's interface and semantics with nn.LSTMCell(obs_dim + 5 feedback, H), H 1..64, whose four gates
     (i, f, g, o) are packed in torch's order.  The carried state is [N, 2H + 5 feedback] = [h, c, onehot(prev action),
-    prev reward]; the reset rule zeroes the whole row, h and c included.
+    prev reward]; the reset rule zeroes the whole row, h and c included.  log_std and dist="gaussian": as GRUPolicy.
     """
     _gates, _memory, _cell_code = 4, 2, _lib.RNN_CELL_LSTM
 
     def __init__(self, cell, head, feedback=True, hidden_reset="episode", obs_mean=None, obs_std=None, device="cuda",
-                 value=None):
-        super().__init__(cell, head, None, feedback, hidden_reset, obs_mean, obs_std, device, value)
+                 value=None, log_std=None, dist="categorical"):
+        if log_std is not None and dist != "gaussian":
+            raise TypeError("LSTMPolicy: log_std goes with dist=\"gaussian\" (the MetaMaze2D head is categorical)")
+        super().__init__(cell, head, log_std, feedback, hidden_reset, obs_mean, obs_std, device, value, dist)
 
     def _torch_cell(self):
         return self._torch.nn.LSTMCell
@@ -521,7 +573,8 @@ class PolicyPopulation(object):
     population, and a rollout captured in a CUDA graph sees that write and any direct write into pop.params.
 
     E must be a multiple of 32 that divides the kernel's CTA env count or is a multiple of it: 32 or a multiple of 64
-    on the quadrotor, 32, 64 or a multiple of 128 on MetaMaze2D.  With M = 1 any N is accepted.
+    on the quadrotor with MLP members, 32, 64 or a multiple of 128 with recurrent members and on MetaMaze2D.  With
+    M = 1 any N is accepted.
     """
 
     def __init__(self, policies):
@@ -557,7 +610,8 @@ class PolicyPopulation(object):
     def _shape(p):
         if isinstance(p, MLPPolicy):
             return (p.obs_dim, tuple(p.widths), p.activation, p.has_log_std, p.has_value, p.device)
-        return (p.obs_dim, p.hidden, p.head_width, p.activation, p.feedback, p.hidden_reset, p.has_value, p.device)
+        return (p.obs_dim, p.hidden, p.head_width, p.activation, p.feedback, p.hidden_reset, p.has_value, p.device,
+                p.dist, p.has_log_std)
 
     @classmethod
     def from_template(cls, policy, members):
@@ -584,6 +638,12 @@ class PolicyPopulation(object):
     @property
     def has_value(self):
         return self.policies[0].has_value
+
+    @property
+    def dist(self):
+        """The members' action distribution: "gaussian" for MLP members and Gaussian recurrent ones, else
+        "categorical"."""
+        return getattr(self.policies[0], "dist", "gaussian")
 
     def envs_per_member(self, num_envs):
         """E = num_envs / members; ValueError when num_envs is not a multiple of members."""

@@ -342,7 +342,7 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                                                 None, None, self._stream()))
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, policy=None, deterministic=False,
-                gae=None):
+                gae=None, state=None, want_hidden=False):
         """T steps in one launch (state stays in registers).  actions: [T,N,4] CUDA tensor or None (device-drawn
         U(min_voltage, max_voltage)).  Returns dict(obs [T,N,D], rew [T,N], done [T,N], act [T,N,4] or None).
 
@@ -358,6 +358,12 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         value[0]) and, with final_obs=True or gae, "final_value" [T,N] (V of the terminal observation where an episode
         ended truncated; other entries are not written).  gae=(gamma, lam) also yields "adv" and "ret" [T,N] float32,
         GAE(gamma, lam) computed in the launch (DESIGN.md "Value heads and GAE"); it needs a value head and auto_reset.
+        policy may also be a GRUPolicy or an LSTMPolicy with dist="gaussian", or a population of them
+        (mgb_quad_rollout_rnn; DESIGN.md "Recurrent quadrotor policies"; needs auto_reset=True), with state: the carried
+        state [N, state_dim] float32, contiguous, on the env's device (policy.initial_state(N) to start fresh), read at
+        the start and updated in place at the end of the launch.  The dict then also holds "state0" (a copy of state as
+        read) and, with want_hidden=True, "hid" [T,N,H] (the cell's output at every step); a population's E must be
+        32, 64 or a multiple of 128.
 
         With final_obs=True the dict also holds "final_obs" [T,N,D] float32: row (t, e) is the terminal observation
         of env e where done[t, e] (what step() reports as final_observation); it is allocated with torch.empty, and
@@ -370,9 +376,20 @@ class BatchedQuadrotor(Snapshots, Mirrored):
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
             from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
-            if isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation) and policy.recurrent):
-                raise ValueError("recurrent policies run on MetaMaze2D only; the quadrotor takes an MLPPolicy")
-            return self._rollout_policy(T, policy, act_seed, deterministic, out, gae)
+            recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation)
+                                                                          and policy.recurrent)
+            if recurrent and policy.dist != "gaussian":
+                raise ValueError("a categorical recurrent policy drives MetaMaze2D; the quadrotor takes "
+                                 "dist=\"gaussian\"")
+            if recurrent and state is None:
+                raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
+                                 % type(policy).__name__)
+            if state is not None and not recurrent:
+                raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
+            return self._rollout_policy(T, policy, act_seed, deterministic, out, gae, state if recurrent else None,
+                                        want_hidden)
+        if state is not None:
+            raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
         if gae is not None:
             raise ValueError("gae= needs a policy with a value head")
         if out is None:
@@ -391,19 +408,23 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                                     self._stream()))
         return out
 
-    def _rollout_policy(self, T, policy, act_seed, deterministic, out, gae=None):
+    def _rollout_policy(self, T, policy, act_seed, deterministic, out, gae=None, state=None, want_hidden=False):
         from .policy import PolicyPopulation, critic_args, critic_struct
         torch = self._torch
         N, D, dev = self.num_envs, self.obs_dim, self.device
+        recurrent = state is not None
         population = isinstance(policy, PolicyPopulation)
         if population:
-            policy.check_envs(N, _lib.QUAD_POLICY_CTA_ENVS)
+            policy.check_envs(N, _lib.QUAD_RNN_CTA_ENVS if recurrent else _lib.QUAD_POLICY_CTA_ENVS)
         if policy.obs_dim != D:
             raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
         if policy.params.device != dev:
             raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
         if not deterministic and not policy.has_log_std:
             raise ValueError("a stochastic quadrotor policy needs log_std (or pass deterministic=True)")
+        if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
+                              and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
+            raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
         critic = critic_args(policy, gae)
         if out is None:
             out = {"obs": torch.empty((T, N, D), dtype=torch.float32, device=dev),
@@ -412,11 +433,17 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                    "act": torch.empty((T, N, 4), dtype=torch.float32, device=dev),
                    "logp": None if deterministic else torch.empty((T, N), dtype=torch.float32, device=dev),
                    "obs0": torch.empty((N, D), dtype=torch.float32, device=dev)}
+            if recurrent:
+                out["state0"] = torch.empty((N, policy.state_dim), dtype=torch.float32, device=dev)
+            if recurrent and want_hidden:
+                out["hid"] = torch.empty((T, N, policy.hidden), dtype=torch.float32, device=dev)
             if self._want_final:
                 out["final_obs"] = torch.empty((T, N, D), dtype=torch.float32, device=dev)
                 out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
         pol = policy.struct(deterministic)
         keys = ("act", "logp", "obs0", "obs", "rew", "done", "final_obs", "truncated")
+        if recurrent:
+            return self._rollout_rnn(T, policy, pol, population, critic, act_seed, state, out, keys)
         if critic is not None:
             cr = critic_struct(torch, out, T, N, dev, critic, self._want_final)
             outs = [_lib.ptr(out.get(k)) for k in keys]
@@ -431,6 +458,26 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         else:
             _lib.check(self._lib.mgb_quad_rollout_policy(self._h, int(T), ctypes.byref(pol), int(act_seed), *outs,
                                                          self._stream()))
+        return out
+
+    def _rollout_rnn(self, T, policy, pol, population, critic, act_seed, state, out, keys):
+        """mgb_quad_rollout_rnn, its population or its critic call: the entry point's arguments from the checked
+        policy, its struct, the carried state and the output dict."""
+        from .policy import critic_struct
+        members = [policy.members, policy.member_stride] if population else [1, 0]
+        tail = []
+        if critic is not None:
+            tail = [ctypes.byref(critic_struct(self._torch, out, T, self.num_envs, self.device, critic,
+                                               self._want_final))]
+            entry = self._lib.mgb_quad_rollout_rnn_critic
+        elif population:
+            entry = self._lib.mgb_quad_rollout_rnn_population
+        else:
+            members = []
+            entry = self._lib.mgb_quad_rollout_rnn
+        args = [self._h, int(T), ctypes.byref(pol)] + members + [int(act_seed)]
+        args += [_lib.ptr(state), _lib.ptr(out.get("state0")), _lib.ptr(out.get("hid"))]
+        _lib.check(entry(*args, *[_lib.ptr(out.get(k)) for k in keys], *tail, self._stream()))
         return out
 
     @property
