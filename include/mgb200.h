@@ -665,6 +665,40 @@ int mgb_quad_rollout_rnn_critic(mgb_quad *h, int32_t T, const mgb_rnn_policy *po
                                 float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
                                 uint8_t *truncated_dev, const mgb_critic *critic, void *stream);
 
+/* ---- whole-episode evaluation (DESIGN.md "Whole-episode evaluation") -----------------------------------------------
+ * Per-episode returns of a policy in ONE launch: every env steps until its `episodes`-th done and then stops.  One entry
+ * point per engine serves every policy kind.
+ *   Policy: exactly one of mlp (as mgb_*_rollout_policy) and rnn (as mgb_*_rollout_rnn) is set.  members = 1: a single
+ *     policy; otherwise member m drives the envs [m E, (m + 1) E), E = n / members under the population calls' rules
+ *     (member_stride as there).  state_dev [n][S] goes with rnn only, read at launch start and written back at launch
+ *     end as in mgb_*_rollout_rnn.  value_row = 1: the packed output layer has the critic's fifth row (the *_critic
+ *     layout); it is skipped, never evaluated.  seed keys the policy's draws; mode MGB_POLICY_MEAN draws nothing.
+ *   Stopping rule: let t = 0, 1, ... count env e's steps in this launch.  Step t is, bit for bit, step t of the policy
+ *     rollout with the same handle state, policy, seed, carried state and resample_cfg: the same Philox counter
+ *     (genv, t_base + t), auto-reset, in-launch resampling (MetaMaze2D), trial counting and path recording.  Env e stops
+ *     after its episodes-th done, at step L_e; its state (the quadrotor's rigid body, ct and episode counter; the
+ *     maze's agent, life, food, steps, task slot, resample count, trial count and path) and its row of state_dev are
+ *     then what a rollout of exactly L_e steps leaves, so successive calls score consecutive episodes.
+ *   Outputs, [episodes][n] (episode-major, like the rollouts' [T][n]), none NULL:
+ *     return_dev: the float64 sum in step order of episode j's rewards (the steps after done number j - 1, up to and
+ *       including done number j; episode 0 starts at launch start).  Quadrotor rewards are float32 widened one by one.
+ *     length_dev: the steps of episode j.  truncated_dev: the rollout's truncated flag at that done (1 only when the
+ *       episode ended through the time limit alone).
+ *   Episode 0 is counted from whatever state the env holds at launch start: reset() first for clean episodes (the
+ *   quadrotor's reset() leaves ct alone, as the reference's does).  Each episode ends within the time limit (nt on the
+ *   quadrotor, max_steps on the maze), so the launch takes at most B = episodes x limit steps, and the step counter
+ *   advances by B.  No host synchronisation and no allocation; the call can be captured in a CUDA graph.
+ * Refused (MGB_ERR_ARG; the handle, its step counter and the state untouched): everything the matching rollout call
+ * refuses, auto_reset off, episodes < 1, B above 2^31 - 1, both or neither of mlp / rnn, state_dev NULL with rnn or set
+ * with mlp, value_row other than 0 or 1, a NULL output, a 3-D maze handle, and output mirrors or multicast set. */
+int mgb_quad_evaluate(mgb_quad *h, int32_t episodes, const mgb_policy *mlp, const mgb_rnn_policy *rnn,
+                      int32_t value_row, int32_t members, int64_t member_stride, uint64_t seed, float *state_dev,
+                      double *return_dev, int32_t *length_dev, uint8_t *truncated_dev, void *stream);
+int mgb_maze_evaluate(mgb_maze *h, int32_t episodes, const mgb_policy *mlp, const mgb_rnn_policy *rnn,
+                      int32_t value_row, int32_t members, int64_t member_stride, uint64_t seed,
+                      const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, float *state_dev,
+                      double *return_dev, int32_t *length_dev, uint8_t *truncated_dev, void *stream);
+
 /* ---- recurrent cell sequences (DESIGN.md "Fused unroll") ----------------------------------------------------------
  * The learner's side of the recurrent policies: the cell of mgb_rnn_policy run over T given steps of n envs, forward and
  * backward, with no env and no head.  A PPO update recomputes h_t with autograd from a rollout's inputs; the head, the

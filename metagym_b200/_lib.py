@@ -159,6 +159,10 @@ SIGNATURES = {
     "mgb_maze_rollout_rnn_critic": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_i32, c_i64, c_u64,
                                                    ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp, vp, vp,
                                                    vp, vp, vp, vp, ctypes.POINTER(Critic), vp]),
+    "mgb_quad_evaluate": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), ctypes.POINTER(RnnPolicy), c_i32, c_i32,
+                                         c_i64, c_u64, vp, vp, vp, vp, vp]),
+    "mgb_maze_evaluate": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), ctypes.POINTER(RnnPolicy), c_i32, c_i32,
+                                         c_i64, c_u64, ctypes.POINTER(MazeSamplerCfg), c_u64, vp, vp, vp, vp, vp]),
     "mgb_rnn_seq_forward": (ctypes.c_int, [ctypes.POINTER(RnnSeq), vp]),
     "mgb_rnn_seq_backward": (ctypes.c_int, [ctypes.POINTER(RnnSeq), vp]),
     "mgb_maze_pose": (ctypes.c_int, [vp, vp, vp, vp]),

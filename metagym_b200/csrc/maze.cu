@@ -578,13 +578,23 @@ __device__ __forceinline__ void maze2d_terminal_value(const MazeConst &c, const 
 // VAL declares a minimum of one resident CTA per SM (.minnctapersm 1; 0 emits nothing, so the other instantiations are
 // compiled as before): with ptxas's default register target the MLP kernel without RS spilled 8 bytes and the LSTM one
 // with RS 84 bytes, where their value-less counterparts do not spill; with it none spills.
-template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0, bool VAL = false>
-__global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel(
+// EVAL (POL only, not FIN or VAL; mgb_maze_evaluate): whole-episode evaluation.  a.T is the step bound; the thread
+// steps its env until its cr.episodes-th done and then stops, its state as that step left it.  It keeps the episode's
+// return, length and index in registers and stores them at each done (mgb_eval_step); no per-step output is stored.  The
+// window row in the tile is the thread's own scratch (the policy's next input), so the loop has no CTA barrier; a warp
+// leaves it when all its envs have finished.  With RS a finished lane still takes part in the warp's draws (maze_sample_task
+// is warp-cooperative) and changes nothing.  Without RS a trial handle's counts go up by the episodes at the end.
+// EVAL keeps the counterpart's bounds, except with RS and the LSTM: at ptxas's default register target it took 128
+// registers and spilled 80 bytes, where its counterpart takes 143 and does not spill; with one resident CTA per SM
+// declared, as VAL does, it takes 168 and none spills.
+template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0, bool VAL = false, bool EVAL = false>
+__global__ void __launch_bounds__(k2dThreads, VAL || (EVAL && RS && POL == kPolLstm) ? 1 : 0) maze2d_rollout_kernel(
     const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
-    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ mgb_critic cr)
+    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ MgbCriticOrEval<EVAL> cr)
 {
     constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
     static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
+    static_assert(!EVAL || (POL && !FIN && !VAL), "evaluation runs a policy and stores only per-episode results");
     static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
     const int64_t e0 = (int64_t)blockIdx.x * k2dThreads;
@@ -644,9 +654,14 @@ __global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel
         }
         __syncthreads();    // the staged weights (the RS loop has no CTA barrier)
     }
+    bool live = active;                 // EVAL: the env has episodes left
+    double ev_ret = 0.0;                // EVAL: the return, length and index of the current episode
+    int ev_len = 0, ev_ep = 0;
     for (int t = 0; t < a.T; ++t) {
         float *tile = tile2d + (size_t)(t & 1) * k2dThreads * D;
-        if constexpr (RS) {                                 // per warp: the warp's rows and their store are its own
+        if constexpr (EVAL) {
+            if (!__any_sync(0xffffffffu, live)) break;
+        } else if constexpr (RS) {                          // per warp: the warp's rows and their store are its own
             if ((threadIdx.x & 31) == 0) mgb_bulk_wait_read<1>();
             __syncwarp();
         } else {
@@ -654,7 +669,7 @@ __global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel
             __syncthreads();
         }
         uint32_t done_byte = 0, draw = 0;                  // draw (RS): the env finished and draws a new maze
-        if (active) {
+        if (EVAL ? live : active) {
             int action;
             if constexpr (POL) {
                 float logits[4], v;
@@ -699,16 +714,18 @@ __global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel
                 maze2d_terminal_value<POL>(c, a, cr, pol, pol_w, pol_x, pol_y, hid_prev, hid_new, cst, blob, eaten, s, t,
                                            e, D, done, action, reward, draw, tile + threadIdx.x * D);
             }
+            if constexpr (EVAL) live = mgb_eval_step(cr, a.n, e, reward, done, done && maze_truncated(c, blob, s), ev_ret,
+                                                     ev_len, ev_ep);
             if (done && a.auto_reset) env_reset(c, blob, eaten, a.n_pad, s);
             if (!VAL && RS && done) draw = (uint32_t)rs_draws(rs, tcount);
             if (REC) path_store(c, a, e, s);
-            if (a.rew) {
+            if (a.rew && !EVAL) {
                 if (XM == 2) mgb_mc_st(mgb_shift(a.rew + (int64_t)t * a.n + e, a.mir.delta[0]), reward);
                 else a.rew[(int64_t)t * a.n + e] = reward;
                 if (XM == 1) mgb_mirror_store(a.mir, a.rew + (int64_t)t * a.n + e, reward);
             }
             done_byte = (uint32_t)done;
-            if (a.done && XM != 2) {
+            if (a.done && XM != 2 && !EVAL) {
                 a.done[(int64_t)t * a.n + e] = (uint8_t)done;
                 if (XM == 1) mgb_mirror_store(a.mir, a.done + (int64_t)t * a.n + e, (uint8_t)done);
             }
@@ -770,10 +787,11 @@ __global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel
             }
         }
         if constexpr (POL) {        // the policy's input at step t + 1: the row this thread left in the tile
-            if (active)
+            if (EVAL ? live : active)
                 for (int k = 0; k < D; ++k) pol_x[k * k2dThreads + threadIdx.x] = tile[threadIdx.x * D + k];
         }
-        if (XM == 2) {
+        if (EVAL) {                 // no observation leaves the CTA
+        } else if (XM == 2) {
             if (a.done) mgb_mc_st_bytes(mgb_shift(a.done + (int64_t)t * a.n + e, a.mir.delta[0]), done_byte, active);
             if (a.obs) {
                 __syncthreads();
@@ -824,6 +842,7 @@ __global__ void __launch_bounds__(k2dThreads, VAL ? 1 : 0) maze2d_rollout_kernel
         a.agent[e] = make_int4(s.gx, s.gy, s.ori, s.steps);
         a.life[e] = s.life;
         if (RS && rs.count) rs.count[e] = tcount;
+        if (EVAL && !RS && rs.count) rs.count[e] += (uint32_t)ev_ep;     // what maze_count_done_kernel adds
     }
     if constexpr (RNN) {
         if (active) {
@@ -4414,30 +4433,36 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
 
 // maze2d_rollout_kernel<0, fin, REC, RS, POL>, sm bytes of dynamic shared memory; refused (as `fn`) when the CTA would
 // need more shared memory than the device allows
-// (with a critic: maze2d_rollout_kernel<0, true, REC, RS, POL, true>)
+// (with a critic: maze2d_rollout_kernel<0, true, REC, RS, POL, true>; with ev, mgb_maze_evaluate:
+// maze2d_rollout_kernel<0, false, REC, RS, POL, false, true>)
 template <bool REC, bool RS, int POL>
 static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const MazeArgs &a, const MazeResample &r,
                             const MgbPolicyPlan<POL> &m, unsigned blocks, size_t sm, cudaStream_t st,
-                            const mgb_critic *critic)
+                            const mgb_critic *critic, const MgbEval *ev = nullptr)
 {
+    // the launch of `kernel`, whose last parameter is `last` (the critic, or the evaluation's outputs)
+    const auto launch = [&](auto kernel, const auto &last) -> int {
+        int optin = 0;
+        MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+        cudaFuncAttributes fa;
+        MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
+        if (fa.sharedSizeBytes + sm > (size_t)optin) {
+            mgb_set_error("%s: the policy rollout needs %zu bytes of shared memory per CTA (windows of "
+                          "view_grid %d, %sweights and activations of %d envs), more than the %d the device allows (use a "
+                          "smaller view_grid or narrower layers)", fn, fa.sharedSizeBytes + sm, h->c.view_grid,
+                          RS ? "sampler workspaces, " : "", k2dThreads, optin);
+            return MGB_ERR_ARG;
+        }
+        MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+        kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m, last);
+        MGB_CUDA(cudaGetLastError());
+        return MGB_OK;
+    };
+    if (ev) return launch(maze2d_rollout_kernel<0, false, REC, RS, POL, false, true>, *ev);
     const auto kernel = critic ? maze2d_rollout_kernel<0, true, REC, RS, POL, true>
                         : fin  ? maze2d_rollout_kernel<0, true, REC, RS, POL>
                                : maze2d_rollout_kernel<0, false, REC, RS, POL>;
-    int optin = 0;
-    MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-    cudaFuncAttributes fa;
-    MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
-    if (fa.sharedSizeBytes + sm > (size_t)optin) {
-        mgb_set_error("%s: the policy rollout needs %zu bytes of shared memory per CTA (windows of "
-                      "view_grid %d, %sweights and activations of %d envs), more than the %d the device allows (use a "
-                      "smaller view_grid or narrower layers)", fn, fa.sharedSizeBytes + sm, h->c.view_grid,
-                      RS ? "sampler workspaces, " : "", k2dThreads, optin);
-        return MGB_ERR_ARG;
-    }
-    MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m, critic ? *critic : mgb_critic{});
-    MGB_CUDA(cudaGetLastError());
-    return MGB_OK;
+    return launch(kernel, critic ? *critic : mgb_critic{});
 }
 
 // A policy rollout of kind POL (mgb_maze_rollout_policy, mgb_maze_rollout_rnn) with the plan `pol`.  The checks, in
@@ -4447,13 +4472,15 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
 // optional outputs and the handle's state.  The policy's region of dynamic shared memory follows the tiles and the
 // sampler workspaces.
 // A critic (the *_critic entry points, whose own() plans the value row; null for the others) is checked last.
+// With ev (mgb_maze_evaluate, which passes no per-step output) the launch is the EVAL instantiation over the step bound
+// T, and a trial handle without resampling has its episodes counted in the launch instead of from done.
 template <int POL, class Own>
 static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MgbPolicyPlan<POL> &pol, Own own,
                                int32_t members, int64_t member_stride, uint64_t seed,
                                const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, int32_t *act_out_dev,
                                float *logp_out_dev, float *obs0_out_dev, float *obs_dev, double *rew_dev,
                                uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev, void *stream,
-                               bool val = false, const mgb_critic *critic = nullptr)
+                               bool val = false, const mgb_critic *critic = nullptr, const MgbEval *ev = nullptr)
 {
     MgbMlp &head = mgb_policy_head(pol);
     SamplerCfg sc;
@@ -4468,7 +4495,7 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MgbPolicy
         if (h->mir.count != 0)
             return "policy rollouts are not delivered through output mirrors or multicast (set_mirrors([]) first)";
         if (!resample_cfg) {
-            if (const char *why = trial_needs_done(h, done_dev)) return why;
+            if (const char *why = ev ? nullptr : trial_needs_done(h, done_dev)) return why;
         } else {
             if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout
             if (const char *why = sampler_cfg(h, resample_cfg, sc)) return why;
@@ -4493,21 +4520,23 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MgbPolicy
     if (resample_cfg) {
         r.cfg = sc; r.seed = resample_seed; r.epoch = h->task_epoch.get();
         r.count = h->task_count.get(); r.k = h->trial_k;
+    } else if (ev && h->trial_k) {
+        r.count = h->task_count.get();
     }
     const bool fin = final_obs_dev || truncated_dev;
     const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
     const cudaStream_t st = (cudaStream_t)stream;
     const mgb_critic *cr = val ? critic : nullptr;
     if (resample_cfg)
-        rc = h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr)
-                     : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr);
+        rc = h->path ? launch_2d_policy<true, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr, ev)
+                     : launch_2d_policy<false, true, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr, ev);
     else
-        rc = h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr)
-                     : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr);
+        rc = h->path ? launch_2d_policy<true, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr, ev)
+                     : launch_2d_policy<false, false, POL>(fn, h, fin, a, r, pol, blocks, sm, st, cr, ev);
     if (rc) return rc;
     h->t_base += (uint32_t)T;
     h->launches += 1;
-    return resample_cfg ? MGB_OK : count_done(h, done_dev, T, st);
+    return resample_cfg || ev ? MGB_OK : count_done(h, done_dev, T, st);
 }
 
 // mgb_maze_rollout_policy of `members` policies (one: mgb_maze_rollout_policy), refused as `fn`
@@ -4515,13 +4544,14 @@ static int maze_rollout_mlp(const char *fn, mgb_maze *h, int32_t T, const mgb_po
                             int64_t member_stride, uint64_t seed, const mgb_maze_sampler_cfg *resample_cfg,
                             uint64_t resample_seed, int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
                             float *obs_dev, double *rew_dev, uint8_t *done_dev, float *final_obs_dev,
-                            uint8_t *truncated_dev, void *stream, bool val = false, const mgb_critic *critic = nullptr)
+                            uint8_t *truncated_dev, void *stream, bool val = false, const mgb_critic *critic = nullptr,
+                            const MgbEval *ev = nullptr, bool value_row = false)
 {
     MgbMlp m;
-    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m, val); };
+    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, false, m, val || value_row); };
     return maze_rollout_policy<kPolMlp>(fn, h, T, m, own, members, member_stride, seed, resample_cfg, resample_seed,
                                         act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
-                                        final_obs_dev, truncated_dev, stream, val, critic);
+                                        final_obs_dev, truncated_dev, stream, val, critic, ev);
 }
 
 extern "C" int mgb_maze_rollout_policy(mgb_maze *h, int32_t T, const mgb_policy *pol, uint64_t seed,
@@ -4552,14 +4582,15 @@ static int maze_rollout_rnn(const char *fn, mgb_maze *h, int32_t T, const mgb_rn
                             uint64_t resample_seed, float *state_dev, float *state0_out_dev, float *hid_out_dev,
                             int32_t *act_out_dev, float *logp_out_dev, float *obs0_out_dev, float *obs_dev,
                             double *rew_dev, uint8_t *done_dev, float *final_obs_dev, uint8_t *truncated_dev,
-                            void *stream, bool val = false, const mgb_critic *critic = nullptr)
+                            void *stream, bool val = false, const mgb_critic *critic = nullptr,
+                            const MgbEval *ev = nullptr, bool value_row = false)
 {
     // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
     const auto run = [&](auto kind) {
         constexpr int POL = decltype(kind)::value;
         MgbPolicyPlan<POL> p;
         const auto own = [&](int obs_dim) -> const char * {
-            if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val)) return why;
+            if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val || value_row)) return why;
             p.state = state_dev;
             p.state0_out = state0_out_dev;
             p.hid_out = hid_out_dev;
@@ -4570,7 +4601,7 @@ static int maze_rollout_rnn(const char *fn, mgb_maze *h, int32_t T, const mgb_rn
         };
         return maze_rollout_policy<POL>(fn, h, T, p, own, members, member_stride, seed, resample_cfg, resample_seed,
                                         act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev, done_dev,
-                                        final_obs_dev, truncated_dev, stream, val, critic);
+                                        final_obs_dev, truncated_dev, stream, val, critic, ev);
     };
     return pol && pol->cell == MGB_RNN_CELL_LSTM ? run(std::integral_constant<int, kPolLstm>{})
                                                  : run(std::integral_constant<int, kPolGru>{});
@@ -4628,6 +4659,28 @@ extern "C" int mgb_maze_rollout_rnn_critic(mgb_maze *h, int32_t T, const mgb_rnn
     return maze_rollout_rnn(__func__, h, T, pol, members, member_stride, seed, resample_cfg, resample_seed, state_dev,
                             state0_out_dev, hid_out_dev, act_out_dev, logp_out_dev, obs0_out_dev, obs_dev, rew_dev,
                             done_dev, final_obs_dev, truncated_dev, stream, true, critic);
+}
+
+extern "C" int mgb_maze_evaluate(mgb_maze *h, int32_t episodes, const mgb_policy *mlp, const mgb_rnn_policy *rnn,
+                                 int32_t value_row, int32_t members, int64_t member_stride, uint64_t seed,
+                                 const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, float *state_dev,
+                                 double *return_dev, int32_t *length_dev, uint8_t *truncated_dev, void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_evaluate");
+    int32_t T = 0;
+    const char *why = !h ? "null handle"
+                      : h->c.kind != MGB_MAZE_2D ? "mgb_maze_evaluate serves MetaMaze2D (the 3-D envs have no policy path)"
+                      : mgb_eval_check(episodes, h->c.max_steps, h->auto_reset, mlp, rnn, state_dev, value_row,
+                                       return_dev, length_dev, truncated_dev, T);
+    if (why) return maze_refuse(__func__, why);
+    const MgbEval ev = {return_dev, length_dev, truncated_dev, episodes};
+    if (mlp)
+        return maze_rollout_mlp(__func__, h, T, mlp, members, member_stride, seed, resample_cfg, resample_seed, nullptr,
+                                nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream, false, nullptr,
+                                &ev, value_row != 0);
+    return maze_rollout_rnn(__func__, h, T, rnn, members, member_stride, seed, resample_cfg, resample_seed, state_dev,
+                            nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                            stream, false, nullptr, &ev, value_row != 0);
 }
 
 extern "C" int mgb_maze_set_mirrors(mgb_maze *h, int count, const int64_t *byte_delta)

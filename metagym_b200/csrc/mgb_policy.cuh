@@ -472,6 +472,58 @@ __device__ __forceinline__ void mgb_gae(const mgb_critic &cr, int T, int64_t n, 
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Whole-episode evaluation (mgb_quad_evaluate, mgb_maze_evaluate; DESIGN.md "Whole-episode evaluation").  The EVAL
+// instantiations of the policy rollout kernels take this in place of the critic: each env steps until its
+// `episodes`-th done and stores one entry per episode, at the done that ends it.
+// ---------------------------------------------------------------------------------------------------------------
+
+struct MgbEval {
+    double *ret;          // [episodes][n]: the float64 sum of the episode's rewards, in step order
+    int32_t *len;         // [episodes][n]: its steps
+    uint8_t *trunc;       // [episodes][n]: the rollout's truncated flag at the done that ended it
+    int episodes;
+};
+
+// The last kernel parameter of a policy rollout: the critic, or with EVAL the evaluation's outputs
+template <bool EVAL>
+using MgbCriticOrEval = std::conditional_t<EVAL, MgbEval, mgb_critic>;
+
+// Host: the checks an evaluation makes besides the rollout's; `limit` is the time limit in steps.  Returns null, or
+// the reason the call is refused, and sets T to the step bound episodes * limit.
+static inline const char *mgb_eval_check(int32_t episodes, int64_t limit, bool auto_reset, const void *mlp,
+                                         const void *rnn, const float *state, int32_t value_row, const void *ret,
+                                         const void *len, const void *trunc, int32_t &T)
+{
+    if (!auto_reset) return "evaluation needs auto_reset on (an env steps on into its next episode)";
+    if (episodes < 1) return "episodes must be at least 1";
+    if ((int64_t)episodes * limit > INT32_MAX) return "episodes * the time limit must be at most 2^31 - 1 steps";
+    if (!mlp == !rnn) return "exactly one of mlp and rnn must be set";
+    if (rnn && !state) return "null state (a recurrent policy carries its state)";
+    if (mlp && state) return "state goes with a recurrent policy";
+    if (value_row != 0 && value_row != 1) return "value_row must be 0 or 1";
+    if (!ret || !len || !trunc) return "null output";
+    T = (int32_t)((int64_t)episodes * limit);
+    return nullptr;
+}
+
+// Device: one step's reward into the thread's episode.  At a done it stores the episode and starts the next; returns
+// false once the env has finished its last episode.
+__device__ __forceinline__ bool mgb_eval_step(const MgbEval &ev, int64_t n, int64_t e, double reward, bool done,
+                                              bool truncated, double &ret, int &len, int &ep)
+{
+    ret += reward;
+    len += 1;
+    if (!done) return true;
+    const int64_t i = (int64_t)ep * n + e;
+    ev.ret[i] = ret;
+    ev.len[i] = len;
+    ev.trunc[i] = truncated ? 1 : 0;
+    ret = 0.0;
+    len = 0;
+    return ++ep < ev.episodes;
+}
+
 __device__ __forceinline__ float mgb_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }
 
 // What mgb_rnn_cell hands its `save` for unit j: nothing by default (the rollouts)

@@ -1167,14 +1167,19 @@ __global__ void __launch_bounds__(kStreamThreads, 4) quad_stream_kernel(const __
 // once more before observe_reset (final_value; a recurrent cell steps from h_t and c'_t on [o, a_t, r_t] into the dead
 // h0, before the carry wipes); after the loop (and after the state row is stored, since the LSTM cell updates c in
 // place) one more pass gives value_last, and the epilogue (mgb_gae) walks the thread's column.
-template <bool SIMPLE, int XM, bool FIN, int POL = 0, bool VAL = false>
+// EVAL (POL only, not FIN or VAL; mgb_quad_evaluate): whole-episode evaluation.  a.T is the step bound; the thread
+// steps its env until its cr.episodes-th done and then stops, its state as that step left it.  It keeps the episode's
+// return, length and index in registers and stores them at each done (mgb_eval_step); no per-step output is stored and
+// no observation tile is written, so the loop has no CTA barrier (one barrier after staging publishes the weights).
+template <bool SIMPLE, int XM, bool FIN, int POL = 0, bool VAL = false, bool EVAL = false>
 __global__ void __launch_bounds__(POL >= kPolGru ? kRnnThreads : kThreads, POL >= kPolGru ? 1 : POL ? 3 : 8)
 quad_rollout_kernel(const __grid_constant__ QuadConst c, const __grid_constant__ QuadArgs a,
-                    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ mgb_critic cr)
+                    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ MgbCriticOrEval<EVAL> cr)
 {
     constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
     constexpr int CTA = RNN ? kRnnThreads : kThreads;
     static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
+    static_assert(!EVAL || (POL && !FIN && !VAL), "evaluation runs a policy and stores only per-episode results");
     __shared__ __align__(128) float tiles[2][CTA * kMaxObs];
     const int64_t e0 = (int64_t)blockIdx.x * CTA;
     const int64_t e = e0 + threadIdx.x;
@@ -1237,11 +1242,19 @@ quad_rollout_kernel(const __grid_constant__ QuadConst c, const __grid_constant__
     // software pipeline: the action of step t+1 is requested while step t integrates
     float4 act_next = make_float4(0.f, 0.f, 0.f, 0.f);
     if (active && a.act) act_next = __ldg(reinterpret_cast<const float4 *>(a.act) + e);
+    bool live = active;                 // EVAL: the env has episodes left
+    double ev_ret = 0.0;                // EVAL: the return, length and index of the current episode
+    int ev_len = 0, ev_ep = 0;
+    if constexpr (EVAL) __syncthreads();    // the staged weights
     for (int t = 0; t < a.T; ++t) {
         float *tile = tiles[t & 1];
-        // the bulk store issued two steps ago must have finished READING this tile before we overwrite it
-        if (threadIdx.x == 0) mgb_bulk_wait_read<1>();
-        __syncthreads();
+        if constexpr (EVAL) {
+            if (!live) break;
+        } else {
+            // the bulk store issued two steps ago must have finished READING this tile before we overwrite it
+            if (threadIdx.x == 0) mgb_bulk_wait_read<1>();
+            __syncthreads();
+        }
         uint32_t done_byte = 0;
         if (active) {
             float4 act;
@@ -1328,21 +1341,22 @@ quad_rollout_kernel(const __grid_constant__ QuadConst c, const __grid_constant__
                     if (cr.final_value_dev) cr.final_value_dev[(int64_t)t * a.n + e] = v;
                 }
             }
+            if constexpr (EVAL) live = mgb_eval_step(cr, a.n, e, (double)reward, done[0], trunc[0], ev_ret, ev_len, ev_ep);
             if (wf[0]) {
                 observe_reset(c, a, task, s, 0, o);
                 adjugate(s.R, adj, id);
             }
-            if (a.rew) {
+            if (a.rew && !EVAL) {
                 if (XM == 2) mgb_mc_st(mgb_shift(a.rew + (int64_t)t * a.n + e, a.mir.delta[0]), reward);
                 else a.rew[(int64_t)t * a.n + e] = reward;
                 if (XM == 1) mgb_mirror_store(a.mir, a.rew + (int64_t)t * a.n + e, reward);
             }
             done_byte = (uint32_t)done[0];
-            if (a.done && XM != 2) {
+            if (a.done && XM != 2 && !EVAL) {
                 a.done[(int64_t)t * a.n + e] = (uint8_t)done[0];
                 if (XM == 1) mgb_mirror_store(a.mir, a.done + (int64_t)t * a.n + e, (uint8_t)done[0]);
             }
-            if (a.obs) {
+            if (a.obs && !EVAL) {
                 float *orow = tile + threadIdx.x * D;
 #pragma unroll
                 for (int k = 0; k < 16; ++k) orow[k] = o[k];
@@ -1378,7 +1392,7 @@ quad_rollout_kernel(const __grid_constant__ QuadConst c, const __grid_constant__
                 mgb_mc_copy_tile(mgb_shift(a.obs + ((int64_t)t * a.n + e0) * D, a.mir.delta[0]), tile,
                                  (uint32_t)rows * (uint32_t)D * 4u);
             }
-        } else if (a.obs) {
+        } else if (a.obs && !EVAL) {
             if (XM == 1) publish_tile_mirrored(a.mir, a.obs + (int64_t)t * a.n * D, tile, e0, rows, D);
             else publish_tile(a.obs + (int64_t)t * a.n * D, tile, e0, rows, D);
         }
@@ -1952,12 +1966,14 @@ static int rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_se
 // mgb_quad_rollout_rnn), refused as `fn`.  The checks, in order: the handle, T, then own() (the entry point plans the
 // policy into m and makes its own checks; it returns the refusal, or nullptr), the population, logp_out in the mean mode,
 // mirrors, final_obs, the alignments, the critic (with `val`, the *_critic entry points, whose own() plans the value row),
-// the handle's state and the footprint.
+// the handle's state and the footprint.  With `ev` (mgb_quad_evaluate, which passes no per-step output) the launch is
+// the EVAL instantiation over the step bound T.
 template <int POL, class Own>
 static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, MgbPolicyPlan<POL> &m, Own own, int32_t members,
                           int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
                           float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
-                          uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
+                          uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false,
+                          const MgbEval *ev = nullptr)
 {
     constexpr int CTA = POL >= kPolGru ? kRnnThreads : kThreads;
     const auto refuse = [&](const char *why) {
@@ -1987,46 +2003,54 @@ static int rollout_policy(const char *fn, mgb_quad *h, int32_t T, MgbPolicyPlan<
     head.logp_out = logp_out_dev;
     head.obs0_out = obs0_out_dev;
     const bool fin = final_obs_dev || truncated_dev;
+    size_t smem;
+    if constexpr (POL == kPolMlp) smem = mgb_mlp_smem_bytes(m, CTA);
+    else smem = mgb_rnn_smem_bytes(m, CTA);
+    // the launch of `kernel`, whose last parameter is `last` (the critic, or the evaluation's outputs)
+    const auto launch = [&](auto kernel, const auto &last) -> int {
+        int optin = 0;
+        MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+        cudaFuncAttributes fa;
+        MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
+        if (fa.sharedSizeBytes + smem > (size_t)optin) {
+            mgb_set_error("%s: the policy needs %zu bytes of shared memory per CTA (weights and activations of %d envs), "
+                          "above the device's %d", fn, fa.sharedSizeBytes + smem, CTA, optin);
+            return MGB_ERR_ARG;
+        }
+        MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        QuadArgs a = base_args(h);
+        a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev;
+        a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
+        a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+        const unsigned blocks = (unsigned)((a.n + CTA - 1) / CTA);
+        kernel<<<blocks, CTA, smem, (cudaStream_t)stream>>>(h->c, a, m, last);
+        MGB_CUDA(cudaGetLastError());
+        h->t_base += (uint32_t)T;
+        h->launches += 1;
+        return MGB_OK;
+    };
+    if (ev)
+        return with_simple(h, [&](auto simple) { return launch(quad_rollout_kernel<simple, 0, false, POL, false, true>, *ev); });
     const auto kernel = with_simple(h, [&](auto simple) {
         return val ? quad_rollout_kernel<simple, 0, true, POL, true>
                : fin ? quad_rollout_kernel<simple, 0, true, POL> : quad_rollout_kernel<simple, 0, false, POL>;
     });
-    size_t smem;
-    if constexpr (POL == kPolMlp) smem = mgb_mlp_smem_bytes(m, CTA);
-    else smem = mgb_rnn_smem_bytes(m, CTA);
-    int optin = 0;
-    MGB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
-    cudaFuncAttributes fa;
-    MGB_CUDA(cudaFuncGetAttributes(&fa, kernel));
-    if (fa.sharedSizeBytes + smem > (size_t)optin) {
-        mgb_set_error("%s: the policy needs %zu bytes of shared memory per CTA (weights and activations of %d envs), "
-                      "above the device's %d", fn, fa.sharedSizeBytes + smem, CTA, optin);
-        return MGB_ERR_ARG;
-    }
-    MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    QuadArgs a = base_args(h);
-    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev;
-    a.T = T; a.t_base = h->t_base; a.act_out = act_out_dev;
-    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
-    const unsigned blocks = (unsigned)((a.n + CTA - 1) / CTA);
-    kernel<<<blocks, CTA, smem, (cudaStream_t)stream>>>(h->c, a, m, val ? *critic : mgb_critic{});
-    MGB_CUDA(cudaGetLastError());
-    h->t_base += (uint32_t)T;
-    h->launches += 1;
-    return MGB_OK;
+    return launch(kernel, val ? *critic : mgb_critic{});
 }
 
 // mgb_quad_rollout_policy of `members` MLP policies (one: mgb_quad_rollout_policy), refused as `fn`
+// (with `ev`, mgb_quad_evaluate: the value row is planned when value_row is set, and skipped)
 static int rollout_mlp(const char *fn, mgb_quad *h, int32_t T, const mgb_policy *pol, int32_t members,
                        int64_t member_stride, uint64_t seed, float *act_out_dev, float *logp_out_dev,
                        float *obs0_out_dev, float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
-                       uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
+                       uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false,
+                       const MgbEval *ev = nullptr, bool value_row = false)
 {
     MgbMlp m;
-    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, true, m, val); };
+    const auto own = [&](int obs_dim) { return mgb_mlp_plan(pol, obs_dim, true, m, val || value_row); };
     return rollout_policy<kPolMlp>(fn, h, T, m, own, members, member_stride, seed, act_out_dev, logp_out_dev,
                                    obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream,
-                                   critic, val);
+                                   critic, val, ev);
 }
 
 // mgb_quad_rollout_rnn of `members` recurrent policies (one: mgb_quad_rollout_rnn), refused as `fn`
@@ -2034,14 +2058,15 @@ static int rollout_rnn(const char *fn, mgb_quad *h, int32_t T, const mgb_rnn_pol
                        int64_t member_stride, uint64_t seed, float *state_dev, float *state0_out_dev,
                        float *hid_out_dev, float *act_out_dev, float *logp_out_dev, float *obs0_out_dev,
                        float *obs_dev, float *rew_dev, uint8_t *done_dev, float *final_obs_dev,
-                       uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false)
+                       uint8_t *truncated_dev, void *stream, const mgb_critic *critic = nullptr, bool val = false,
+                       const MgbEval *ev = nullptr, bool value_row = false)
 {
     // the same rollout for either cell: kind is std::integral_constant<int, kPolGru or kPolLstm>
     const auto run = [&](auto kind) {
         constexpr int POL = decltype(kind)::value;
         MgbPolicyPlan<POL> p;
         const auto own = [&](int obs_dim) -> const char * {
-            if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val, true)) return why;
+            if (const char *why = mgb_rnn_plan(pol, obs_dim, p, val || value_row, true)) return why;
             if (pol->reset != MGB_RNN_RESET_EPISODE)
                 return "the quadrotor's recurrent rollout needs reset = MGB_RNN_RESET_EPISODE (its tasks never change "
                        "inside a launch)";
@@ -2056,7 +2081,7 @@ static int rollout_rnn(const char *fn, mgb_quad *h, int32_t T, const mgb_rnn_pol
         };
         return rollout_policy<POL>(fn, h, T, p, own, members, member_stride, seed, act_out_dev, logp_out_dev,
                                    obs0_out_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream,
-                                   critic, val);
+                                   critic, val, ev);
     };
     return pol && pol->cell == MGB_RNN_CELL_LSTM ? run(std::integral_constant<int, kPolLstm>{})
                                                  : run(std::integral_constant<int, kPolGru>{});
@@ -2126,6 +2151,29 @@ extern "C" int mgb_quad_rollout_critic(mgb_quad *h, int32_t T, const mgb_policy 
     MgbRange nvtx_range("mgb_quad_rollout_critic");
     return rollout_mlp(__func__, h, T, pol, members, member_stride, seed, act_out_dev, logp_out_dev, obs0_out_dev,
                        obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream, critic, true);
+}
+
+extern "C" int mgb_quad_evaluate(mgb_quad *h, int32_t episodes, const mgb_policy *mlp, const mgb_rnn_policy *rnn,
+                                 int32_t value_row, int32_t members, int64_t member_stride, uint64_t seed,
+                                 float *state_dev, double *return_dev, int32_t *length_dev, uint8_t *truncated_dev,
+                                 void *stream)
+{
+    MgbRange nvtx_range("mgb_quad_evaluate");
+    int32_t T = 0;
+    const char *why = h ? mgb_eval_check(episodes, h->c.nt, h->auto_reset, mlp, rnn, state_dev, value_row, return_dev,
+                                         length_dev, truncated_dev, T)
+                        : "null handle";
+    if (why) {
+        mgb_set_error("%s: %s", __func__, why);
+        return MGB_ERR_ARG;
+    }
+    const MgbEval ev = {return_dev, length_dev, truncated_dev, episodes};
+    if (mlp)
+        return rollout_mlp(__func__, h, T, mlp, members, member_stride, seed, nullptr, nullptr, nullptr, nullptr,
+                           nullptr, nullptr, nullptr, nullptr, stream, nullptr, false, &ev, value_row != 0);
+    return rollout_rnn(__func__, h, T, rnn, members, member_stride, seed, state_dev, nullptr, nullptr, nullptr, nullptr,
+                       nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream, nullptr, false, &ev,
+                       value_row != 0);
 }
 
 extern "C" int mgb_quad_rollout(mgb_quad *h, int32_t T, const float *act_dev, uint64_t act_seed, float *act_out_dev,

@@ -701,6 +701,37 @@ class _LazySteps(dict):
         return k == "steps"
 
 
+def _check_policy(env, policy, state):
+    """The checks of every policy launch of the MetaMaze2D handle `env` (rollout, evaluate), made before anything
+    reaches the device: the kind, the input width, the device, the carried state and a population's envs per member.
+    Returns (recurrent, population)."""
+    from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
+    torch = env._torch
+    N, dev = env.num_envs, env.device
+    population = isinstance(policy, PolicyPopulation)
+    recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (population and policy.recurrent)
+    if recurrent and state is None:
+        raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
+                         % type(policy).__name__)
+    if state is not None and not recurrent:
+        raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
+    if recurrent and policy.dist != "categorical":
+        raise ValueError("a Gaussian recurrent policy drives the quadrotor; MetaMaze2D takes dist=\"categorical\"")
+    if env.need_reset:
+        raise Exception("Must \"reset\" before doing any actions")
+    if population:
+        policy.check_envs(N, _lib.MAZE2D_POLICY_CTA_ENVS)
+    D = int(np.prod(env._obs.shape[1:]))
+    if policy.obs_dim != D:
+        raise ValueError("the policy takes %d observation inputs, the env observes %d" % (policy.obs_dim, D))
+    if policy.params.device != dev:
+        raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
+    if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
+                          and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
+        raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
+    return recurrent, population
+
+
 class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
     """MetaMaze2D(enable_render, render_scale, max_steps, task_type, view_grid) x num_envs (maze_env.py:155-172).
 
@@ -781,44 +812,59 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         truncated and the policy's memory is wiped (every done, or new_tasks(out) under hidden_reset="task"), from the
         memory before the wipe; other entries are not written.  gae=(gamma, lam) also yields "adv" and "ret" [T,N]
         float32, GAE(gamma, lam) cut where the memory is wiped (DESIGN.md "Value heads and GAE")."""
-        from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
-        recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation)
-                                                                      and policy.recurrent)
-        if recurrent and state is None:
-            raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
-                             % type(policy).__name__)
-        if state is not None and not recurrent:
-            raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
-        if recurrent and policy.dist != "categorical":
-            raise ValueError("a Gaussian recurrent policy drives the quadrotor; MetaMaze2D takes dist=\"categorical\"")
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
-            return self._rollout_policy(T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden,
-                                        gae)
+            recurrent, population = _check_policy(self, policy, state)
+            return self._rollout_policy(T, policy, recurrent, population, state, act_seed, deterministic, out, resample,
+                                        want_hidden, gae)
+        if state is not None:
+            raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
         if gae is not None:
             raise ValueError("gae= needs a policy with a value head")
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._want_final, resample=resample)
 
-    def _rollout_policy(self, T, policy, recurrent, state, act_seed, deterministic, out, resample, want_hidden,
-                        gae=None):
-        from .policy import PolicyPopulation, critic_args, critic_struct
-        if self.need_reset:
-            raise Exception("Must \"reset\" before doing any actions")
+    def evaluate(self, policy, episodes=1, act_seed=0, deterministic=False, state=None, resample=None):
+        """Whole-episode evaluation in one launch (mgb_maze_evaluate; DESIGN.md "Whole-episode evaluation"): every env
+        steps under `policy` until its `episodes`-th done, then stops.  Step t is, bit for bit, step t of
+        rollout(T, policy=policy, act_seed=act_seed, deterministic=deterministic, state=state, resample=resample),
+        with its auto-reset, in-launch resampling, trial counting and path recording, and each env is left as such a
+        rollout of its own length leaves it (state, if given, included), so successive calls score consecutive
+        episodes.  Episode 0 counts from the state the env holds now: reset() first for clean episodes.  policy is any
+        policy rollout() takes, including populations and policies with a value head (never evaluated).  Needs
+        auto_reset=True.  The step counter advances by episodes * max_steps.  On a trial handle (episodes_per_task=k,
+        with resample and hidden_reset="task") res["return"].mean(1) is the adaptation curve over a trial's episodes.
+
+        Returns {"return": [episodes, N] float64 (the rewards of each episode summed in step order), "length":
+        [episodes, N] int32 (its steps; zero-filled first, so an episode the launch did not finish, which the time limit
+        rules out, would show as length 0), "truncated": [episodes, N] uint8 (1 iff it ended through max_steps alone)}.
+        A population's fitness, member by member: res["return"].mean(0).view(M, -1).mean(1)."""
+        recurrent, population = _check_policy(self, policy, state)
+        episodes = int(episodes)
+        if episodes < 1 or episodes * self.max_steps > 2 ** 31 - 1:
+            raise ValueError("episodes must be at least 1, and episodes * max_steps at most 2^31 - 1 steps")
+        torch = self._torch
+        shape = (episodes, self.num_envs)
+        out = {"return": torch.empty(shape, dtype=torch.float64, device=self.device),
+               "length": torch.zeros(shape, dtype=torch.int32, device=self.device),
+               "truncated": torch.empty(shape, dtype=torch.uint8, device=self.device)}
+        cfg, seed = (None, 0) if resample is None else self._sampler_cfg(**resample)
+        pol = ctypes.byref(policy.struct(deterministic))
+        members, stride = (policy.members, policy.member_stride) if population else (1, 0)
+        mlp, rnn = (None, pol) if recurrent else (pol, None)
+        _lib.check(self._lib.mgb_maze_evaluate(self._h, episodes, mlp, rnn,
+                                               int(policy.has_value), members, stride, int(act_seed),
+                                               None if cfg is None else ctypes.byref(cfg), seed, _lib.ptr(state),
+                                               *[_lib.ptr(out[k]) for k in ("return", "length", "truncated")],
+                                               self._stream()))
+        return out
+
+    def _rollout_policy(self, T, policy, recurrent, population, state, act_seed, deterministic, out, resample,
+                        want_hidden, gae=None):
+        from .policy import critic_args, critic_struct
         torch = self._torch
         T, N, dev = int(T), self.num_envs, self.device
-        population = isinstance(policy, PolicyPopulation)
-        if population:
-            policy.check_envs(N, _lib.MAZE2D_POLICY_CTA_ENVS)
         shape = tuple(self._obs.shape[1:])
-        D = int(np.prod(shape))
-        if policy.obs_dim != D:
-            raise ValueError("the policy takes %d observation inputs, the env observes %d" % (policy.obs_dim, D))
-        if policy.params.device != dev:
-            raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
-        if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
-                              and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
-            raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
         critic = critic_args(policy, gae)
         if out is None:
             out = {"obs": torch.empty((T, N) + shape, dtype=torch.float32, device=dev),

@@ -126,6 +126,37 @@ class QuadInfo(dict):
         return list(self._keys)
 
 
+def _check_policy(env, policy, state, deterministic):
+    """The checks of every policy launch of the quadrotor handle `env` (rollout, evaluate), made before anything reaches
+    the device: the kind, the input width, the device, log_std, the carried state and a population's envs per member.
+    Returns (recurrent, population)."""
+    from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
+    torch = env._torch
+    N, D, dev = env.num_envs, env.obs_dim, env.device
+    population = isinstance(policy, PolicyPopulation)
+    recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (population and policy.recurrent)
+    if recurrent and policy.dist != "gaussian":
+        raise ValueError("a categorical recurrent policy drives MetaMaze2D; the quadrotor takes "
+                         "dist=\"gaussian\"")
+    if recurrent and state is None:
+        raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
+                         % type(policy).__name__)
+    if state is not None and not recurrent:
+        raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
+    if population:
+        policy.check_envs(N, _lib.QUAD_RNN_CTA_ENVS if recurrent else _lib.QUAD_POLICY_CTA_ENVS)
+    if policy.obs_dim != D:
+        raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
+    if policy.params.device != dev:
+        raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
+    if not deterministic and not policy.has_log_std:
+        raise ValueError("a stochastic quadrotor policy needs log_std (or pass deterministic=True)")
+    if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
+                          and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
+        raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
+    return recurrent, population
+
+
 class BatchedQuadrotor(Snapshots, Mirrored):
     """`Quadrotor(dt, nt, seed, task, map_file, simulator_conf, healthy_reward)` x num_envs on one H100.
 
@@ -375,18 +406,8 @@ class BatchedQuadrotor(Snapshots, Mirrored):
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
-            from .policy import GRUPolicy, LSTMPolicy, PolicyPopulation
-            recurrent = isinstance(policy, (GRUPolicy, LSTMPolicy)) or (isinstance(policy, PolicyPopulation)
-                                                                          and policy.recurrent)
-            if recurrent and policy.dist != "gaussian":
-                raise ValueError("a categorical recurrent policy drives MetaMaze2D; the quadrotor takes "
-                                 "dist=\"gaussian\"")
-            if recurrent and state is None:
-                raise ValueError("a %s rollout needs its carried state (state=policy.initial_state(num_envs))"
-                                 % type(policy).__name__)
-            if state is not None and not recurrent:
-                raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
-            return self._rollout_policy(T, policy, act_seed, deterministic, out, gae, state if recurrent else None,
+            recurrent, population = _check_policy(self, policy, state, deterministic)
+            return self._rollout_policy(T, policy, recurrent, population, act_seed, deterministic, out, gae, state,
                                         want_hidden)
         if state is not None:
             raise ValueError("state= goes with a GRUPolicy or an LSTMPolicy")
@@ -408,23 +429,42 @@ class BatchedQuadrotor(Snapshots, Mirrored):
                                     self._stream()))
         return out
 
-    def _rollout_policy(self, T, policy, act_seed, deterministic, out, gae=None, state=None, want_hidden=False):
-        from .policy import PolicyPopulation, critic_args, critic_struct
+    def evaluate(self, policy, episodes=1, act_seed=0, deterministic=False, state=None):
+        """Whole-episode evaluation in one launch (mgb_quad_evaluate; DESIGN.md "Whole-episode evaluation"): every env
+        steps under `policy` until its `episodes`-th done, then stops.  Step t is, bit for bit, step t of
+        rollout(T, policy=policy, act_seed=act_seed, deterministic=deterministic, state=state), and each env is left as
+        such a rollout of its own length leaves it (state, if given, included), so successive calls score consecutive
+        episodes.  Episode 0 counts from the state the env holds now: reset() first for clean episodes.  policy is any
+        policy rollout() takes, including populations and policies with a value head (never evaluated).  Needs
+        auto_reset=True.  The step counter advances by episodes * nt.
+
+        Returns {"return": [episodes, N] float64 (the rewards of each episode summed in step order), "length":
+        [episodes, N] int32 (its steps; zero-filled first, so an episode the launch did not finish, which the time limit
+        rules out, would show as length 0), "truncated": [episodes, N] uint8 (1 iff it ended through nt alone)}.  A
+        population's fitness, member by member: res["return"].mean(0).view(M, -1).mean(1)."""
+        recurrent, population = _check_policy(self, policy, state, deterministic)
+        episodes = int(episodes)
+        if episodes < 1 or episodes * self.nt > 2 ** 31 - 1:
+            raise ValueError("episodes must be at least 1, and episodes * nt at most 2^31 - 1 steps")
+        torch = self._torch
+        shape = (episodes, self.num_envs)
+        out = {"return": torch.empty(shape, dtype=torch.float64, device=self.device),
+               "length": torch.zeros(shape, dtype=torch.int32, device=self.device),
+               "truncated": torch.empty(shape, dtype=torch.uint8, device=self.device)}
+        pol = ctypes.byref(policy.struct(deterministic))
+        members, stride = (policy.members, policy.member_stride) if population else (1, 0)
+        mlp, rnn = (None, pol) if recurrent else (pol, None)
+        _lib.check(self._lib.mgb_quad_evaluate(self._h, episodes, mlp, rnn,
+                                               int(policy.has_value), members, stride, int(act_seed), _lib.ptr(state),
+                                               *[_lib.ptr(out[k]) for k in ("return", "length", "truncated")],
+                                               self._stream()))
+        return out
+
+    def _rollout_policy(self, T, policy, recurrent, population, act_seed, deterministic, out, gae=None, state=None,
+                        want_hidden=False):
+        from .policy import critic_args, critic_struct
         torch = self._torch
         N, D, dev = self.num_envs, self.obs_dim, self.device
-        recurrent = state is not None
-        population = isinstance(policy, PolicyPopulation)
-        if population:
-            policy.check_envs(N, _lib.QUAD_RNN_CTA_ENVS if recurrent else _lib.QUAD_POLICY_CTA_ENVS)
-        if policy.obs_dim != D:
-            raise ValueError("the policy takes %d inputs, the env observes %d" % (policy.obs_dim, D))
-        if policy.params.device != dev:
-            raise ValueError("the policy's buffer is on %s, the env on %s" % (policy.params.device, dev))
-        if not deterministic and not policy.has_log_std:
-            raise ValueError("a stochastic quadrotor policy needs log_std (or pass deterministic=True)")
-        if recurrent and not (isinstance(state, torch.Tensor) and state.dtype == torch.float32 and state.device == dev
-                              and tuple(state.shape) == (N, policy.state_dim) and state.is_contiguous()):
-            raise ValueError("state must be a contiguous float32 tensor [%d, %d] on %s" % (N, policy.state_dim, dev))
         critic = critic_args(policy, gae)
         if out is None:
             out = {"obs": torch.empty((T, N, D), dtype=torch.float32, device=dev),
