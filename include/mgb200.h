@@ -464,6 +464,56 @@ int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uint64_t act_s
                      void *obs_dev, double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
                      const mgb_maze_sampler_cfg *resample_cfg, uint64_t resample_seed, void *stream);
 
+/* Expert (ESCAPE on MetaMaze2D and MetaMazeDiscrete3D; DESIGN.md §4d "Expert").  Per task slot, a breadth-first search
+ * backwards from the goal over the step's own action model:
+ *   MetaMaze2D: the states are the cells, the actions the four of DISCRETE_ACTIONS (maze_2d.py:21-34); a move into a
+ *   wall or off the grid leaves the agent in place and still takes a step.  One heading plane.
+ *   MetaMazeDiscrete3D: the states are (heading, cell), 4 n^2 of them; an action turns, then moves
+ *   (maze_discrete_3d.py:51-81).
+ *   dist(s): the fewest actions from s after which the agent stands on the goal cell (evaluation_rule ends the episode
+ *   there, maze_base.py:90-93); 0 on the goal, 0xFFFF where the goal cannot be reached.
+ *   mask(s): bit a set iff dist(next(s, a)) = dist(s) - 1; 0 on the goal and on unreachable states.
+ * Tables: dist uint16 and mask uint8 [slot][planes][n][n] (planes: 1 for MetaMaze2D, 4 indexed by heading), entry
+ * ((slot planes + ori) n + gx) n + gy.  Every integer, so the tables are exact.  They are rebuilt on the stream of the
+ * call that changes the task table, for exactly the slots it changes: mgb_maze_set_task (every slot),
+ * mgb_maze_update_tasks (the replaced slots), mgb_maze_resample_tasks (the drawn slots) and mgb_maze_restore (the slots
+ * of the restored envs, when records carry their tasks).  None of them gains a host synchronisation.
+ * Decision of step t of env e (global index genv = env_index_base + e) on a state with mask m: Philox4x32-10 counter
+ * (genv lo, genv hi, t_base + t, MGB_STREAM_EXPERT = 0x800), key = seed, words r.x, r.y.  The choice set C is {0..3}
+ * when (r.x >> 8) 2^-24 < eps (float32 compare) or m = 0, else the bits of m; the action is the j-th lowest member of
+ * C, j = floor(r.y |C| / 2^32).  Mean mode (mode 1): no draw and no eps; the lowest member of m, or 0 where m = 0.
+ *
+ * mgb_maze_set_expert(h, on): makes h an expert handle.  Before the first mgb_maze_set_task only, like
+ *   mgb_maze_set_episodes_per_task; refused afterwards, and with on for SURVIVAL or MetaMazeContinuous3D.
+ * mgb_maze_rollout_expert: mgb_maze_rollout without resampling whose action at step t is act_dev[t] when act_dev is
+ *   given, else the expert's decision on the state the env holds before step t (written to act_out_dev if not NULL).
+ *   expert_out_dev [T][n] uint8 (or NULL): the mask of that state (DAgger labels).  The env side is bit for bit
+ *   mgb_maze_rollout fed act_out: auto-reset, final_obs / truncated, trial counts, path recording; every engine
+ *   (MetaMaze2D, the pose cache, the direct renderer) gives the same outputs.  mode 0 samples, mode 1 is the mean mode.
+ *   obs_dev, rew_dev and done_dev are required.  Advances the step counter by T.
+ * mgb_maze_step_expert: mgb_maze_step, then expert_out_dev [n] uint8: the mask of every env's state after the step,
+ *   the one its next action acts on (what mgb_maze_expert returns then).
+ * mgb_maze_expert: the mask (uint8 [n]) and, if dist_out_dev is not NULL, the dist (uint16 [n]) of every env's state.
+ * mgb_maze_expert_table: the tables of slots [slot0, slot0 + count), mask uint8 and (if not NULL) dist uint16
+ *   [count][planes][n][n].
+ * All of them are stream-ordered, allocate nothing after the first reset() and can be captured in a CUDA graph.
+ * Refused (MGB_ERR_ARG, handle untouched), with a message naming the reason: a handle that is not an expert handle,
+ * SURVIVAL, MetaMazeContinuous3D, output mirrors or multicast set, eps not finite or outside [0, 1], a mode other than
+ * 0 or 1, T <= 0, a NULL required output, final_obs without auto_reset, a slot range outside the table.
+ * In-launch resampling is not offered: the kernels that draw a new maze into a slot cannot rebuild its tables.  So on an
+ * expert handle every call with a resample_cfg (mgb_maze_rollout, mgb_maze_rollout_policy, mgb_maze_rollout_rnn, their
+ * population and critic forms, mgb_maze_evaluate) is refused (MGB_ERR_ARG, handle untouched); mgb_maze_resample_tasks
+ * between launches keeps the tables current. */
+int mgb_maze_set_expert(mgb_maze *h, int on);
+int mgb_maze_rollout_expert(mgb_maze *h, int32_t T, const int32_t *act_dev, float eps, int32_t mode, uint64_t seed,
+                            int32_t *act_out_dev, uint8_t *expert_out_dev, void *obs_dev, double *rew_dev,
+                            uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev, void *stream);
+int mgb_maze_step_expert(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                         void *final_obs_dev, uint8_t *truncated_dev, uint8_t *expert_out_dev, void *stream);
+int mgb_maze_expert(mgb_maze *h, uint8_t *mask_out_dev, uint16_t *dist_out_dev, void *stream);
+int mgb_maze_expert_table(mgb_maze *h, int32_t slot0, int32_t count, uint8_t *mask_out_dev, uint16_t *dist_out_dev,
+                          void *stream);
+
 /* mgb_maze_rollout of a MetaMaze2D handle (resample_cfg NULL: no resampling; set: in-launch resampling) with
  * actions from a categorical MLP policy (mgb_policy, "policy-driven rollouts" above; input width (2 view_grid + 1)^2,
  * the four outputs are the logits of actions 0..3, no log_std).

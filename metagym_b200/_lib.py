@@ -143,6 +143,12 @@ SIGNATURES = {
     "mgb_maze_set_multicast": (ctypes.c_int, [vp, ctypes.c_int64]),
     "mgb_maze_rollout": (ctypes.c_int, [vp, c_i32, vp, c_u64, vp, vp, vp, vp, vp, vp, ctypes.POINTER(MazeSamplerCfg),
                                         c_u64, vp]),
+    "mgb_maze_set_expert": (ctypes.c_int, [vp, ctypes.c_int]),
+    "mgb_maze_rollout_expert": (ctypes.c_int, [vp, c_i32, vp, ctypes.c_float, c_i32, c_u64, vp, vp, vp, vp, vp, vp, vp,
+                                               vp]),
+    "mgb_maze_step_expert": (ctypes.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "mgb_maze_expert": (ctypes.c_int, [vp, vp, vp, vp]),
+    "mgb_maze_expert_table": (ctypes.c_int, [vp, c_i32, c_i32, vp, vp, vp]),
     "mgb_maze_rollout_policy": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(Policy), c_u64, ctypes.POINTER(MazeSamplerCfg),
                                                c_u64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "mgb_maze_rollout_rnn": (ctypes.c_int, [vp, c_i32, ctypes.POINTER(RnnPolicy), c_u64, ctypes.POINTER(MazeSamplerCfg),

@@ -290,6 +290,170 @@ __device__ __forceinline__ double food_now(const MazeConst &c, const uint8_t *bl
     return visible ? reinterpret_cast<const double *>(blob + c.off_fval)[f] : 0.0;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// ESCAPE expert (include/mgb200.h "Expert", DESIGN.md §4d): per task slot, the fewest actions to the goal from every
+// state and the set of actions that realise it, by breadth-first search backwards from the goal over the step's own move
+// rules.  A state is s = (ori n + gx) n + gy (MetaMaze2D: ori = 0, one plane).
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kExpertWarps = 2;
+constexpr int kExpertStates = 4 * kMaxN * kMaxN;
+constexpr uint16_t kExpertFar = 0xFFFF;      // the goal cannot be reached
+
+__host__ __device__ constexpr int expert_planes(int kind) { return kind == MGB_MAZE_2D ? 1 : 4; }
+
+// The state action `action` leads to from s: the move of maze_logic, restated on a state index
+__device__ __forceinline__ int expert_next(const MazeConst &c, const int8_t *walls, int s, int action)
+{
+    const int n = c.n, nn = n * n;
+    int ori = s / nn, gx = (s - ori * nn) / n, gy = s - ori * nn - gx * n;
+    if (c.kind == MGB_MAZE_2D) {
+        int tx = gx + (action == 0 ? -1 : (action == 1 ? 1 : 0));
+        int ty = gy + (action == 2 ? -1 : (action == 3 ? 1 : 0));
+        if (tx < 0) tx += n;
+        if (ty < 0) ty += n;
+        if (tx < n && ty < n && walls[tx * n + ty] < 1) { gx = tx; gy = ty; }
+    } else {
+        const int turn = action == 0 ? -1 : (action == 1 ? 1 : 0);
+        const int mv = action == 2 ? -1 : (action == 3 ? 1 : 0);
+        ori = (ori + turn + 4) & 3;
+        int tx = gx, ty = gy;
+        if (ori == 0) tx += mv; else if (ori == 1) ty += mv; else if (ori == 2) tx -= mv; else ty -= mv;
+        if (tx >= 0 && tx < n && ty >= 0 && ty < n && walls[tx * n + ty] == 0) { gx = tx; gy = ty; }
+    }
+    return (ori * n + gx) * n + gy;
+}
+
+// The states from which `action` may lead to t, or -1: `which` 0 is the state that stays (3-D: the turned heading on
+// t's cell), 1 the state that moved into t.  A superset: the caller keeps a candidate only if expert_next maps it to t.
+__device__ __forceinline__ int expert_pred(const MazeConst &c, int t, int action, int which)
+{
+    const int n = c.n, nn = n * n;
+    const int ot = t / nn, x = (t - ot * nn) / n, y = t - ot * nn - x * n;
+    if (c.kind == MGB_MAZE_2D) {       // staying in place reaches t from t itself, which the search has already visited
+        if (which == 0) return -1;
+        const int dx = action == 0 ? -1 : (action == 1 ? 1 : 0), dy = action == 2 ? -1 : (action == 3 ? 1 : 0);
+        return ((x - dx + n) % n) * n + (y - dy + n) % n;     // the wrap of a negative index (maze_logic) included
+    }
+    const int turn = action == 0 ? -1 : (action == 1 ? 1 : 0);
+    const int mv = action == 2 ? -1 : (action == 3 ? 1 : 0);
+    const int o = (ot - turn + 4) & 3;
+    if (which == 0) return (o * n + x) * n + y;
+    if (mv == 0) return -1;
+    const int sx = x - mv * (ot == 0 ? 1 : (ot == 2 ? -1 : 0)), sy = y - mv * (ot == 1 ? 1 : (ot == 3 ? -1 : 0));
+    return sx >= 0 && sx < n && sy >= 0 && sy < n ? (o * n + sx) * n + sy : -1;
+}
+
+// One warp per item: the tables of task slot map[i] (map null: slot i), for the items with sel[i] set (sel null: all)
+// whose record row[i] lies in [0, n_rec) (row null: all).  Breadth-first from the goal's states with the queue, the
+// distance plane and the walls in shared memory: each state enters the queue once, when a lane claims it (16-bit
+// compare-and-swap) as a verified predecessor of a state of the level before.
+__global__ void __launch_bounds__(32 * kExpertWarps) maze_expert_kernel(const __grid_constant__ MazeConst c,
+                                                                        const uint8_t *blobs, int64_t count,
+                                                                        const int32_t *map, const uint8_t *sel,
+                                                                        const int64_t *row, int64_t n_rec,
+                                                                        uint16_t *dist, uint8_t *mask)
+{
+    __shared__ uint16_t s_dist[kExpertWarps][kExpertStates];
+    __shared__ uint16_t s_queue[kExpertWarps][kExpertStates];
+    __shared__ int8_t s_walls[kExpertWarps][kMaxN * kMaxN];
+    __shared__ int s_tail[kExpertWarps];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t i = (int64_t)blockIdx.x * kExpertWarps + w;
+    if (i >= count) return;                                        // warp-uniform exits
+    if (sel && !sel[i]) return;
+    if (row && (row[i] < 0 || row[i] >= n_rec)) return;
+    const int64_t slot = map ? map[i] : i;
+    const uint8_t *blob = blobs + slot * c.blob_bytes;
+    const int n = c.n, nn = n * n, P = expert_planes(c.kind), S = P * nn;
+    const int goal = blob_hdr(blob)->goal[0] * n + blob_hdr(blob)->goal[1];
+    uint16_t *d = s_dist[w], *q = s_queue[w];
+    int8_t *walls = s_walls[w];
+    for (int k = lane; k < nn; k += 32) walls[k] = reinterpret_cast<const int8_t *>(blob + c.off_walls)[k];
+    for (int k = lane; k < S; k += 32) d[k] = k % nn == goal ? 0 : kExpertFar;
+    if (lane < P) q[lane] = (uint16_t)(lane * nn + goal);
+    if (lane == 0) s_tail[w] = P;
+    __syncwarp();
+    for (int lo = 0, hi = P; lo < hi;) {
+        for (int k = lo + lane; k < hi; k += 32) {
+            const int t = q[k];
+            const uint16_t nd = (uint16_t)(d[t] + 1);
+            for (int act = 0; act < 4; ++act)
+                for (int which = 0; which < 2; ++which) {
+                    const int sp = expert_pred(c, t, act, which);
+                    if (sp < 0 || d[sp] != kExpertFar || expert_next(c, walls, sp, act) != t) continue;
+                    if (atomicCAS(reinterpret_cast<unsigned short *>(d + sp), kExpertFar, nd) == kExpertFar)
+                        q[atomicAdd(&s_tail[w], 1)] = (uint16_t)sp;
+                }
+        }
+        __syncwarp();
+        lo = hi;
+        hi = *reinterpret_cast<volatile int *>(&s_tail[w]);
+        __syncwarp();                                              // every lane has read the level's end
+    }
+    for (int k = lane; k < S; k += 32) {
+        const uint16_t dk = d[k];
+        uint8_t m = 0;
+        if (dk != 0 && dk != kExpertFar)
+            for (int act = 0; act < 4; ++act) m |= (uint8_t)(d[expert_next(c, walls, k, act)] == dk - 1) << act;
+        dist[slot * S + k] = dk;
+        mask[slot * S + k] = m;
+    }
+}
+
+// What an expert rollout (the EXP instantiations) reads and writes besides MazeArgs: a parameter after the others, empty
+// in every other instantiation, so that no existing parameter offset moves
+struct MazeExpert {
+    const uint8_t *mask;         // [slots][planes][n][n]
+    uint8_t *out;                // [T][n]: the mask of the state acted on, or null
+    float eps;                   // mixing rate
+    int mean;                    // 1: the lowest action of the choice set, no draw
+    uint64_t seed;
+};
+struct MazeNoExpert {};
+template <bool EXP>
+using MazeExpertOr = std::conditional_t<EXP, MazeExpert, MazeNoExpert>;
+
+// the entry of an env in state s on task slot `slot`
+__device__ __forceinline__ int64_t expert_index(const MazeConst &c, int64_t slot, const Env &s)
+{
+    const int P = expert_planes(c.kind);
+    return ((slot * P + (P == 4 ? s.ori : 0)) * c.n + s.gx) * c.n + s.gy;
+}
+
+__device__ __forceinline__ uint8_t expert_mask(const MazeConst &c, const uint8_t *mask, int64_t slot, const Env &s)
+{
+    return mask[expert_index(c, slot, s)];
+}
+
+// the tables' entries of every env's current state (mgb_maze_expert, mgb_maze_step_expert)
+__global__ void maze_expert_state_kernel(const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a,
+                                         const uint8_t *mask, const uint16_t *dist, uint8_t *mask_out, uint16_t *dist_out)
+{
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n) return;
+    const int4 ag = a.agent[e];
+    const Env s = {ag.x, ag.y, ag.z, ag.w, 0.0};
+    const int64_t k = expert_index(c, a.env2task[e], s);
+    mask_out[e] = mask[k];
+    if (dist_out) dist_out[e] = dist[k];
+}
+
+// The expert's action on a state with mask m (include/mgb200.h): the choice set is {0..3} when r.x's 24-bit uniform is
+// below eps or m is empty, else m; the action is set bit number floor(r.y k / 2^32) of the k in the choice set, or its
+// lowest bit in mean mode
+__device__ __forceinline__ int expert_action(const MazeExpert &x, uint8_t m, int64_t genv, uint32_t t)
+{
+    uint32_t set = m ? m : 0xFu, j = 0;
+    if (!x.mean) {
+        const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32), t, MGB_STREAM_EXPERT),
+                                          make_uint2((uint32_t)x.seed, (uint32_t)(x.seed >> 32)));
+        if (mgb_u01(r.x) < x.eps) set = 0xFu;
+        j = (uint32_t)(((uint64_t)r.y * (uint32_t)__popc(set)) >> 32);
+    }
+    for (; j; --j) set &= set - 1;
+    return __ffs(set) - 1;
+}
+
 
 // ---------------------------------------------------------------------------------------------------------------
 // MetaMazeContinuous3D dynamics (dynamics.py:16-92), float32/float64 typing of the numba + numpy original for float32
@@ -587,14 +751,18 @@ __device__ __forceinline__ void maze2d_terminal_value(const MazeConst &c, const 
 // EVAL keeps the counterpart's bounds, except with RS and the LSTM: at ptxas's default register target it took 128
 // registers and spilled 80 bytes, where its counterpart takes 143 and does not spill; with one resident CTA per SM
 // declared, as VAL does, it takes 168 and none spills.
-template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0, bool VAL = false, bool EVAL = false>
+// EXP (XM == 0, not RS or POL; mgb_maze_rollout_expert): the action of step t is act[t] when given, else the expert's
+// (expert_action, from the mask of the state the env holds before step t); the mask goes to x.out [T][n].
+template <int XM, bool FIN, bool REC, bool RS = false, int POL = 0, bool VAL = false, bool EVAL = false, bool EXP = false>
 __global__ void __launch_bounds__(k2dThreads, VAL || (EVAL && RS && POL == kPolLstm) ? 1 : 0) maze2d_rollout_kernel(
     const __grid_constant__ MazeConst c, const __grid_constant__ MazeArgs a, const __grid_constant__ MazeResample rs,
-    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ MgbCriticOrEval<EVAL> cr)
+    const __grid_constant__ MgbPolicyPlan<POL> pol, const __grid_constant__ MgbCriticOrEval<EVAL> cr,
+    const __grid_constant__ MazeExpertOr<EXP> x)
 {
     constexpr bool RNN = POL == kPolGru || POL == kPolLstm;
     static_assert(!VAL || (POL && FIN), "value heads run on the policy rollouts with terminal outputs");
     static_assert(!EVAL || (POL && !FIN && !VAL), "evaluation runs a policy and stores only per-episode results");
+    static_assert(!EXP || (XM == 0 && !RS && !POL), "expert rollouts are not mirrored, resampled or policy-driven");
     static_assert(!RS || XM == 0, "resampling rollouts are not mirrored");
     extern __shared__ __align__(128) float tile2d[];
     const int64_t e0 = (int64_t)blockIdx.x * k2dThreads;
@@ -689,6 +857,14 @@ __global__ void __launch_bounds__(k2dThreads, VAL || (EVAL && RS && POL == kPolL
                 if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
                 if (head.logp_out) head.logp_out[(int64_t)t * a.n + e] = lp;
                 if constexpr (VAL) cr.value_dev[(int64_t)t * a.n + e] = v;
+            } else if constexpr (EXP) {
+                const uint8_t m = expert_mask(c, x.mask, a.env2task[e], s);
+                if (a.act) action = a.act[(int64_t)t * a.n + e];
+                else {
+                    action = expert_action(x, m, genv, a.t_base + (uint32_t)t);
+                    if (a.act_out) a.act_out[(int64_t)t * a.n + e] = action;
+                }
+                if (x.out) x.out[(int64_t)t * a.n + e] = m;
             } else if (a.act) action = a.act[(int64_t)t * a.n + e];
             else {
                 const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
@@ -985,13 +1161,18 @@ __device__ __forceinline__ void push_terminal_state(const MazeConst &c, const Ma
 //               buffer (maze_sample_task), copies the tile to the env's table slot and fences the generic writes against
 //               the bulk copies that load the slot later; thread 0 then resets the env on the new tile.  The next item's
 //               tile is requested only after that (sequential mode), since it may be the same env.
-template <bool FILL, bool ROLL, bool FIN = false, bool RS = false>
+// EXP (ROLL, not RS; mgb_maze_rollout_expert): the step logic of (e, t), which runs in the geometry phase, takes act[t]
+// when given, else the expert's action on the state env e holds before step t, and stores that state's mask into
+// x.out [T][n]; the pipeline order is the open-loop rollout's.
+template <bool FILL, bool ROLL, bool FIN = false, bool RS = false, bool EXP = false>
 __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_constant__ MazeConst c,
                                                                    const __grid_constant__ MazeArgs a,
-                                                                   const __grid_constant__ MazeResample rs)
+                                                                   const __grid_constant__ MazeResample rs,
+                                                                   const __grid_constant__ MazeExpertOr<EXP> x)
 {
     static_assert(!FIN || (ROLL && !FILL), "terminal frames are a rollout output");
     static_assert(!RS || (ROLL && !FILL), "tasks are resampled in a rollout");
+    static_assert(!EXP || (ROLL && !FILL && !RS), "expert rollouts run without resampling");
     extern __shared__ __align__(128) uint8_t smem[];
     // list pass (final_obs set): items are the entries of the terminal list the step logic just wrote; a CTA without one
     // leaves before it stages the textures
@@ -1142,7 +1323,15 @@ __global__ void __launch_bounds__(kRenderThreads, 1) maze3d_kernel(const __grid_
                         maze_logic(c, s_blob, eaten, a.n_pad, s, a.act[e], reward, done);
                     } else {
                         int action;
-                        if (a.act) action = a.act[o];
+                        if constexpr (EXP) {
+                            const uint8_t m = expert_mask(c, x.mask, a.env2task[e], s);
+                            if (a.act) action = a.act[o];
+                            else {
+                                action = expert_action(x, m, a.env_base + e, a.t_base + (uint32_t)t);
+                                if (a.act_out) a.act_out[o] = action;
+                            }
+                            if (x.out) x.out[o] = m;
+                        } else if (a.act) action = a.act[o];
                         else {      // the draw of maze3d_rollout_kernel / maze2d_rollout_kernel
                             const int64_t genv = a.env_base + e;
                             const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
@@ -2562,9 +2751,12 @@ __global__ void __launch_bounds__(kStepThreads, 2) maze3d_step_kernel(const __gr
 // finished at step t, publishes the EnvDyn of its terminal state in a second slot -- both before env_reset, which clears the
 // food stamps the terminal frame still shows.  The CTA then composes that frame into final_obs + (t n + env) frame, a
 // barrier later the usual observation: one compose_item per pass, one deferred-tint queue.
-template <bool FIN>
+// EXP (mgb_maze_rollout_expert): thread 0 takes act[t] when given, else the expert's action (expert_action) on the state
+// it holds before step t, and stores that state's mask into x.out [T][n].
+template <bool FIN, bool EXP = false>
 __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(const __grid_constant__ MazeConst c,
-                                                                            const __grid_constant__ MazeArgs a)
+                                                                            const __grid_constant__ MazeArgs a,
+                                                                            const __grid_constant__ MazeExpertOr<EXP> x)
 {
     __shared__ EnvDyn s_dyn;
     __shared__ int s_nslow;
@@ -2586,7 +2778,15 @@ __global__ void __launch_bounds__(kComposeThreads, 5) maze3d_rollout_kernel(cons
         for (int t = 0; t < a.T; ++t) {
             if (threadIdx.x == 0) {
                 int action;
-                if (a.act) action = a.act[(int64_t)t * a.n + env];
+                if constexpr (EXP) {
+                    const uint8_t m = expert_mask(c, x.mask, task, s);
+                    if (a.act) action = a.act[(int64_t)t * a.n + env];
+                    else {
+                        action = expert_action(x, m, genv, a.t_base + (uint32_t)t);
+                        if (a.act_out) a.act_out[(int64_t)t * a.n + env] = action;
+                    }
+                    if (x.out) x.out[(int64_t)t * a.n + env] = m;
+                } else if (a.act) action = a.act[(int64_t)t * a.n + env];
                 else {
                     const uint4 r = mgb_philox4x32_10(make_uint4((uint32_t)genv, (uint32_t)((uint64_t)genv >> 32),
                                                                  a.t_base + (uint32_t)t, MGB_STREAM_ACTION), akey);
@@ -2761,8 +2961,9 @@ struct mgb_maze {
     int auto_reset = 0;
     bool has_task = false, has_tex = false;
     size_t smem3d = 0;
-    int render_attr_set[8] = {};             // maze3d_kernel<false / true / rollout / rollout with terminal frames>, then the
-                                             // two rollouts with resampling (4 + ...): shared-memory opt-in raised by this handle
+    int render_attr_set[16] = {};            // maze3d_kernel<false / true / rollout / rollout with terminal frames>, then the
+                                             // two rollouts with resampling (4 + ...), then the expert rollouts (8 + ...):
+                                             // shared-memory opt-in raised by this handle
     int compose_ctas_per_sm = 0;       // occupancy of maze3d_compose_kernel (queried once per handle)
     int num_sms = 0;
     int64_t launches = 0;
@@ -2772,7 +2973,29 @@ struct mgb_maze {
     MgbMirrors mir = {};         // mgb_maze_set_mirrors
     MgbMirrorWindow mir_win;     // mgb_maze_set_mirror_window
     MgbDev<char2> path;            // mgb_maze_set_path: [max_steps + 1][n_pad] recorded cells, empty when not recording
+    bool expert = false;           // mgb_maze_set_expert: the tables below follow every change of the task table, so
+                                   // the rollouts that draw new mazes inside the launch refuse an expert handle
+    MgbDev<uint16_t> exp_dist;     // [n_tasks][planes][n][n] (maze_expert_kernel)
+    MgbDev<uint8_t> exp_mask;      // [n_tasks][planes][n][n]
 };
+
+// The refusal of in-launch resampling on an expert handle: the kernels that draw a new maze into a slot cannot rebuild
+// the slot's expert tables, which would then describe the old maze
+static const char *const kExpertNoInLaunchResampling =
+    "in-launch resampling is not available on an expert handle (its tables would keep the old mazes): call "
+    "mgb_maze_resample_tasks between launches instead";
+
+// Rebuild the expert tables of the task slots a table change touched, on st (maze_expert_kernel's items, map, sel, row)
+static int build_expert(mgb_maze *h, int64_t count, const int32_t *map, const uint8_t *sel, const int64_t *row,
+                        int64_t n_rec, cudaStream_t st)
+{
+    if (!h->expert) return MGB_OK;
+    maze_expert_kernel<<<(unsigned)((count + kExpertWarps - 1) / kExpertWarps), 32 * kExpertWarps, 0, st>>>(
+        h->c, h->tasks.blobs.get(), count, map, sel, row, n_rec, h->exp_dist.get(), h->exp_mask.get());
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
 
 // entries of one env's path record: an episode ends at steps <= max_steps
 static int64_t path_cap(const mgb_maze *h) { return (int64_t)h->c.max_steps + 1; }
@@ -2948,6 +3171,18 @@ extern "C" int mgb_maze_set_episodes_per_task(mgb_maze *h, int32_t k)
     }
     h->task_count = std::move(count);
     h->trial_k = k;
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_set_expert(mgb_maze *h, int on)
+{
+    MGB_REQUIRE(h, "null handle");
+    MGB_REQUIRE(!h->task_epoch, "call mgb_maze_set_expert before mgb_maze_set_task (the task table then builds the expert's tables)");
+    MGB_REQUIRE(!on || h->c.task_type == MGB_MAZE_ESCAPE,
+                "the expert is defined for ESCAPE only (SURVIVAL has no single shortest-path target)");
+    MGB_REQUIRE(!on || h->c.kind != MGB_MAZE_CONTINUOUS_3D,
+                "the expert is defined for the grid mazes only (MetaMazeContinuous3D has continuous actions)");
+    h->expert = on != 0;
     return MGB_OK;
 }
 
@@ -3233,6 +3468,7 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     // The old table goes before the new one is allocated (HBM never holds both); until the new one is complete every
     // step refuses with "Must call set_task" instead of reading a half-built table.
     h->has_task = false; h->tasks = MazeTasks();
+    h->exp_dist.reset(); h->exp_mask.reset();
     const size_t eaten_bytes = sizeof(int32_t) * (size_t)(f_max > 0 ? f_max : 1) * h->n_pad;
     MazeTasks tasks;
     MGB_CUDA(tasks.blobs.alloc(blobs.size()));
@@ -3276,6 +3512,13 @@ extern "C" int mgb_maze_set_task(mgb_maze *h, int32_t n_tasks, const int8_t *wal
     for (int t = 0; t < n_tasks; ++t)
         h->slot_fp[t] = mgb_fnv(MGB_FNV_BASIS, blobs.data() + (size_t)t * c.blob_bytes, (size_t)c.blob_bytes);
     h->n_tasks = n_tasks;
+    if (h->expert) {
+        const size_t states = (size_t)n_tasks * expert_planes(c.kind) * nn;
+        MGB_CUDA(h->exp_dist.alloc(states * sizeof(uint16_t)));
+        MGB_CUDA(h->exp_mask.alloc(states));
+        const int rc = build_expert(h, n_tasks, nullptr, nullptr, nullptr, 0, nullptr);
+        if (rc) return rc;
+    }
     h->has_task = true;
     h->task_flags.reset();
     // pose list of the cache: every free cell x 4 headings of every task, S = 4 x the most free cells of a task per task
@@ -3696,6 +3939,7 @@ extern "C" int mgb_maze_update_tasks(mgb_maze *h, int32_t count, const int32_t *
                                                                                h->task_count.get());
         h->launches += 1;
     }
+    if (const int rc = build_expert(h, h->n_tasks, nullptr, h->task_flags.get(), nullptr, 0, st)) return rc;
     maze_clear_flags_kernel<<<(unsigned)((h->n_tasks + 255) / 256), 256, 0, st>>>(h->task_flags.get(), h->n_tasks);
     MGB_CUDA(cudaGetLastError());
     h->launches += 2;
@@ -3762,7 +4006,7 @@ extern "C" int mgb_maze_resample_tasks(mgb_maze *h, const uint8_t *mask_dev, con
                                                                                         sc, seed, h->task_count.get());
     MGB_CUDA(cudaGetLastError());
     h->launches += 1;
-    return MGB_OK;
+    return build_expert(h, h->n, h->env2task.get(), mask_dev, nullptr, 0, (cudaStream_t)stream);
 }
 
 extern "C" int mgb_maze_get_tasks(mgb_maze *h, int32_t count, const int32_t *task_slots_host, int8_t *walls_host,
@@ -3839,8 +4083,9 @@ template <class F> static cudaError_t maze_allow_max_dynamic_smem(F *kernel)
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
 }
 
-template <bool FILL, bool ROLL = false, bool FIN = false, bool RS = false>
-static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStream_t st, const MazeResample &rs = {})
+template <bool FILL, bool ROLL = false, bool FIN = false, bool RS = false, bool EXP = false>
+static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStream_t st, const MazeResample &rs = {},
+                         const MazeExpertOr<EXP> &x = {})
 {
     MazeConst &c = h->c;
     // shared-memory plan, most wanted first: (direct renderer) two record sets with the crossing lists in shared memory,
@@ -3875,13 +4120,13 @@ static int launch_render(mgb_maze *h, const MazeArgs &a, unsigned grid, cudaStre
     }
     // The opt-in limit is a property of the kernel on a device, shared by every handle: each handle raises it once to the
     // device maximum (the same value from every handle and thread, so there is no ordering to get wrong and no global state).
-    const int attr = (RS ? 4 : 0) + (FIN ? 3 : (ROLL ? 2 : (FILL ? 1 : 0)));
+    const int attr = (EXP ? 8 : 0) + (RS ? 4 : 0) + (FIN ? 3 : (ROLL ? 2 : (FILL ? 1 : 0)));
     if (!h->render_attr_set[attr]) {
-        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL, FIN, RS>));
+        MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_kernel<FILL, ROLL, FIN, RS, EXP>));
         h->render_attr_set[attr] = 1;
     }
     h->smem3d = sm;
-    maze3d_kernel<FILL, ROLL, FIN, RS><<<grid, kRenderThreads, sm, st>>>(c, a2, rs);
+    maze3d_kernel<FILL, ROLL, FIN, RS, EXP><<<grid, kRenderThreads, sm, st>>>(c, a2, rs, x);
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -4289,8 +4534,8 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
             MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, false, REC, true>));
             MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC, true>));
         }
-        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{}, mgb_critic{});
-        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{}, mgb_critic{});
+        if (fin) maze2d_rollout_kernel<0, true, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{}, mgb_critic{}, MazeNoExpert{});
+        else maze2d_rollout_kernel<0, false, REC, true><<<blocks, k2dThreads, sm, st>>>(c, a, *rs, MgbMlp{}, mgb_critic{}, MazeNoExpert{});
         MGB_CUDA(cudaGetLastError());
         return MGB_OK;
     }
@@ -4301,10 +4546,10 @@ static int launch_2d_rollout(const MazeConst &c, int xm, bool fin, const MazeArg
         MGB_CUDA(maze_allow_max_dynamic_smem(maze2d_rollout_kernel<0, true, REC>));
     }
     const MazeResample none = {};
-    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
-    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
-    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
-    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{});
+    if (xm == 2) maze2d_rollout_kernel<2, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{}, MazeNoExpert{});
+    else if (xm == 1) maze2d_rollout_kernel<1, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{}, MazeNoExpert{});
+    else if (fin) maze2d_rollout_kernel<0, true, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{}, MazeNoExpert{});
+    else maze2d_rollout_kernel<0, false, REC><<<blocks, k2dThreads, sm, st>>>(c, a, none, MgbMlp{}, mgb_critic{}, MazeNoExpert{});
     MGB_CUDA(cudaGetLastError());
     return MGB_OK;
 }
@@ -4345,6 +4590,7 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
         if (h->c.kind != MGB_MAZE_2D && h->mir.count != 0)
             return "output mirrors are not implemented for the 3-D rollouts (set_mirrors([]) first)";
         if (!resample_cfg) return trial_needs_done(h, done_dev);
+        if (h->expert) return kExpertNoInLaunchResampling;
         if (!h->auto_reset) return "resampling finished envs needs auto_reset on";
         if (h->mir.count != 0)
             return "output mirrors and multicast are not implemented for the resampling rollout (set_mirrors([]) first)";
@@ -4380,11 +4626,11 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
         if (fin) {
             if (qbytes > 40 * 1024)
                 MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<true>));
-            maze3d_rollout_kernel<true><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
+            maze3d_rollout_kernel<true><<<grid, kComposeThreads, qbytes, st>>>(h->c, a, MazeNoExpert{});
         } else {
             if (qbytes > 40 * 1024)
                 MGB_CUDA(maze_allow_max_dynamic_smem(maze3d_rollout_kernel<false>));
-            maze3d_rollout_kernel<false><<<grid, kComposeThreads, qbytes, st>>>(h->c, a);
+            maze3d_rollout_kernel<false><<<grid, kComposeThreads, qbytes, st>>>(h->c, a, MazeNoExpert{});
         }
         MGB_CUDA(cudaGetLastError());
     } else if (eng == RolloutEngine::direct) {
@@ -4431,6 +4677,124 @@ extern "C" int mgb_maze_rollout(mgb_maze *h, int32_t T, const void *act_dev, uin
     return resample_cfg ? MGB_OK : count_done(h, done_dev, T, st);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// ESCAPE expert entry points (include/mgb200.h "Expert")
+// ---------------------------------------------------------------------------------------------------------------
+// What every expert entry point needs of the handle: the refusal, or nullptr
+static const char *expert_refusal(const mgb_maze *h)
+{
+    if (h->c.task_type != MGB_MAZE_ESCAPE) return "the expert is defined for ESCAPE only (SURVIVAL has no single shortest-path target)";
+    if (h->c.kind == MGB_MAZE_CONTINUOUS_3D)
+        return "the expert is defined for the grid mazes only (MetaMazeContinuous3D has continuous actions)";
+    if (!h->expert) return "not an expert handle (mgb_maze_set_expert before mgb_maze_set_task)";
+    if (h->mir.count != 0) return "expert outputs are not delivered through output mirrors or multicast (set_mirrors([]) first)";
+    return nullptr;
+}
+
+template <bool FIN>
+static int launch_2d_expert(mgb_maze *h, const MazeArgs &a, const MazeExpert &x, cudaStream_t st)
+{
+    const size_t sm = maze2d_tiles_bytes(h, false);
+    const unsigned blocks = (unsigned)((h->n + k2dThreads - 1) / k2dThreads);
+    const auto kernel = h->path ? maze2d_rollout_kernel<0, FIN, true, false, 0, false, false, true>
+                                : maze2d_rollout_kernel<0, FIN, false, false, 0, false, false, true>;
+    if (sm > 48 * 1024) MGB_CUDA(maze_allow_max_dynamic_smem(kernel));
+    kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, MazeResample{}, MgbMlp{}, mgb_critic{}, x);
+    MGB_CUDA(cudaGetLastError());
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_rollout_expert(mgb_maze *h, int32_t T, const int32_t *act_dev, float eps, int32_t mode,
+                                       uint64_t seed, int32_t *act_out_dev, uint8_t *expert_out_dev, void *obs_dev,
+                                       double *rew_dev, uint8_t *done_dev, void *final_obs_dev, uint8_t *truncated_dev,
+                                       void *stream)
+{
+    MgbRange nvtx_range("mgb_maze_rollout_expert");
+    int rc = check_rollout(__func__, h, T, final_obs_dev, truncated_dev, [&]() -> const char * {
+        if (const char *why = expert_refusal(h)) return why;
+        if (!(eps >= 0.0f && eps <= 1.0f)) return "eps must be finite and in [0, 1]";
+        if (mode != 0 && mode != 1) return "mode must be 0 (sample) or 1 (mean)";
+        if (!(obs_dev && rew_dev && done_dev)) return "null argument (obs, rew and done are required)";
+        return nullptr;
+    });
+    if (rc) return rc;
+    MgbDeviceGuard guard(h->device);
+    const cudaStream_t st = (cudaStream_t)stream;
+    RolloutEngine eng;
+    if ((rc = rollout_engine(h, false, st, eng))) return rc;
+    MazeArgs a = maze_args(h);
+    a.act = act_dev; a.act_out = act_out_dev;
+    a.obs = obs_dev; a.rew = rew_dev; a.done = done_dev; a.do_step = 1;
+    a.T = T; a.t_base = h->t_base;
+    a.final_obs = final_obs_dev; a.truncated = truncated_dev;
+    const bool fin = final_obs_dev || truncated_dev;
+    MazeExpert x;
+    x.mask = h->exp_mask.get(); x.out = expert_out_dev; x.eps = eps; x.mean = mode; x.seed = seed;
+    if (eng == RolloutEngine::pose_cache) {
+        const int64_t resident = (int64_t)h->num_sms * 5;
+        const size_t qbytes = ((size_t)h->c.res_h * h->c.res_v / 4 + 1) * sizeof(int);
+        MGB_REQUIRE(qbytes <= 200 * 1024, "screen too large for the fused rollout's group queue");
+        const unsigned grid = (unsigned)(h->n < resident ? h->n : resident);
+        const auto kernel = fin ? maze3d_rollout_kernel<true, true> : maze3d_rollout_kernel<false, true>;
+        if (qbytes > 40 * 1024) MGB_CUDA(maze_allow_max_dynamic_smem(kernel));
+        kernel<<<grid, kComposeThreads, qbytes, st>>>(h->c, a, x);
+        MGB_CUDA(cudaGetLastError());
+    } else if (eng == RolloutEngine::direct) {
+        const unsigned grid = (unsigned)(h->n < h->num_sms ? h->n : h->num_sms);
+        rc = fin ? launch_render<false, true, true, false, true>(h, a, grid, st, {}, x)
+                 : launch_render<false, true, false, false, true>(h, a, grid, st, {}, x);
+    } else {
+        rc = fin ? launch_2d_expert<true>(h, a, x, st) : launch_2d_expert<false>(h, a, x, st);
+    }
+    if (rc) return rc;
+    h->t_base += (uint32_t)T;
+    h->launches += 1;
+    return count_done(h, done_dev, T, st);
+}
+
+extern "C" int mgb_maze_expert(mgb_maze *h, uint8_t *mask_out_dev, uint16_t *dist_out_dev, void *stream)
+{
+    if (!h) return maze_refuse(__func__, "null handle");
+    if (const char *why = expert_refusal(h)) return maze_refuse(__func__, why);
+    if (!mask_out_dev) return maze_refuse(__func__, "null argument (mask_out is required)");
+    if (int rc = maze_ready(h)) return rc;
+    MgbDeviceGuard guard(h->device);
+    maze_expert_state_kernel<<<(unsigned)((h->n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        h->c, maze_args(h), h->exp_mask.get(), h->exp_dist.get(), mask_out_dev, dist_out_dev);
+    MGB_CUDA(cudaGetLastError());
+    h->launches += 1;
+    return MGB_OK;
+}
+
+extern "C" int mgb_maze_step_expert(mgb_maze *h, const int32_t *act_dev, void *obs_dev, double *rew_dev, uint8_t *done_dev,
+                                    void *final_obs_dev, uint8_t *truncated_dev, uint8_t *expert_out_dev, void *stream)
+{
+    if (!h) return maze_refuse(__func__, "null handle");
+    if (const char *why = expert_refusal(h)) return maze_refuse(__func__, why);
+    if (!expert_out_dev) return maze_refuse(__func__, "null argument (expert_out is required)");
+    int rc = mgb_maze_step(h, act_dev, obs_dev, rew_dev, done_dev, final_obs_dev, truncated_dev, stream);
+    return rc ? rc : mgb_maze_expert(h, expert_out_dev, nullptr, stream);
+}
+
+extern "C" int mgb_maze_expert_table(mgb_maze *h, int32_t slot0, int32_t count, uint8_t *mask_out_dev,
+                                     uint16_t *dist_out_dev, void *stream)
+{
+    if (!h) return maze_refuse(__func__, "null handle");
+    if (const char *why = expert_refusal(h)) return maze_refuse(__func__, why);
+    if (!mask_out_dev) return maze_refuse(__func__, "null argument (mask_out is required)");
+    if (int rc = maze_ready(h)) return rc;
+    if (!(slot0 >= 0 && count > 0 && (int64_t)slot0 + count <= h->n_tasks))
+        return maze_refuse(__func__, "slots [slot0, slot0 + count) must lie in the task table");
+    MgbDeviceGuard guard(h->device);
+    const size_t per = (size_t)expert_planes(h->c.kind) * h->c.n * h->c.n;
+    const cudaStream_t st = (cudaStream_t)stream;
+    MGB_CUDA(cudaMemcpyAsync(mask_out_dev, h->exp_mask.get() + slot0 * per, count * per, cudaMemcpyDeviceToDevice, st));
+    if (dist_out_dev)
+        MGB_CUDA(cudaMemcpyAsync(dist_out_dev, h->exp_dist.get() + slot0 * per, count * per * sizeof(uint16_t),
+                                 cudaMemcpyDeviceToDevice, st));
+    return MGB_OK;
+}
+
 // maze2d_rollout_kernel<0, fin, REC, RS, POL>, sm bytes of dynamic shared memory; refused (as `fn`) when the CTA would
 // need more shared memory than the device allows
 // (with a critic: maze2d_rollout_kernel<0, true, REC, RS, POL, true>; with ev, mgb_maze_evaluate:
@@ -4454,7 +4818,7 @@ static int launch_2d_policy(const char *fn, const mgb_maze *h, bool fin, const M
             return MGB_ERR_ARG;
         }
         MGB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-        kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m, last);
+        kernel<<<blocks, k2dThreads, sm, st>>>(h->c, a, r, m, last, MazeNoExpert{});
         MGB_CUDA(cudaGetLastError());
         return MGB_OK;
     };
@@ -4497,6 +4861,7 @@ static int maze_rollout_policy(const char *fn, mgb_maze *h, int32_t T, MgbPolicy
         if (!resample_cfg) {
             if (const char *why = ev ? nullptr : trial_needs_done(h, done_dev)) return why;
         } else {
+            if (h->expert) return kExpertNoInLaunchResampling;                            // as mgb_maze_rollout
             if (!h->auto_reset) return "resampling finished envs needs auto_reset on";     // as mgb_maze_rollout
             if (const char *why = sampler_cfg(h, resample_cfg, sc)) return why;
         }
@@ -5414,6 +5779,7 @@ extern "C" int mgb_maze_restore(mgb_maze *h, const uint8_t *rec_dev, int64_t n_r
                                                                       n_rec, row_of_env_dev);
         MGB_CUDA(cudaGetLastError());
         h->launches += 1;
+        if ((rc = build_expert(h, h->n, h->env2task.get(), nullptr, row_of_env_dev, n_rec, st))) return rc;
     }
     return record_paths(h, true, rec_dev, n_rec, row_of_env_dev, st);
 }

@@ -174,6 +174,7 @@ __host__ __device__ __forceinline__ float mgb_u01(uint32_t x) { return (float)(x
 #define MGB_STREAM_RESET 0x100u   // + j, j = 0..2: twelve reset draws
 #define MGB_STREAM_ACTION 0x200u  // rollout actions
 #define MGB_STREAM_POLICY 0x400u  // draws of policy-driven rollouts (mgb_policy.cuh)
+#define MGB_STREAM_EXPERT 0x800u  // draws of the maze expert (maze.cu, expert_action)
 
 // ---------------------------------------------------------------------------------------------------------------
 // Bulk asynchronous copies (the TMA engine's 1-D form: cp.async.bulk, SASS UBLKCP)

@@ -7,6 +7,7 @@ reference's `TaskConfig` namedtuple (metagym/metamaze/envs/maze_task.py:15-17); 
 `MazeTaskSampler` are accepted as they are (duck-typed by field name).
 """
 import ctypes
+import math
 from collections import namedtuple
 
 import numpy as np
@@ -239,9 +240,15 @@ class _BatchedMazeBase(Snapshots):
                                                  dtype=np.int32)
 
     def _setup(self, num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs=False,
-               record_path=False, episodes_per_task=None):
+               record_path=False, episodes_per_task=None, expert=False):
         import torch
         assert task_type in ("SURVIVAL", "ESCAPE")
+        if expert and task_type != "ESCAPE":
+            raise ValueError("expert=True is defined for ESCAPE only (SURVIVAL has no single shortest-path target)")
+        if expert and self.KIND == 2:
+            raise ValueError("expert=True is defined for the grid mazes only (MetaMazeContinuous3D has continuous actions)")
+        self.with_expert = bool(expert)
+        self._exp = None
         if final_obs and not auto_reset:
             raise ValueError("final_obs=True needs auto_reset=True (without auto-reset obs already is the terminal frame)")
         if episodes_per_task is not None and not (int(episodes_per_task) == episodes_per_task and episodes_per_task >= 1):
@@ -343,6 +350,8 @@ class _BatchedMazeBase(Snapshots):
             _lib.check(self._lib.mgb_maze_set_path(self._h, 1))
         if self.episodes_per_task is not None:
             _lib.check(self._lib.mgb_maze_set_episodes_per_task(self._h, self.episodes_per_task))
+        if self.with_expert:
+            _lib.check(self._lib.mgb_maze_set_expert(self._h, 1))
         self._after_create()
 
     @staticmethod
@@ -478,7 +487,12 @@ class _BatchedMazeBase(Snapshots):
         self.need_reset = False
         return self._out(self._obs)
 
-    def step(self, action=None):
+    def step(self, action=None, want_expert=False):
+        """want_expert=True (an expert=True env): info["expert"] is the expert's action mask [N] uint8 of the state each
+        env holds after the step, the one its next action acts on (mgb_maze_step_expert; a persistent buffer, so that
+        the step can be captured in a CUDA graph)."""
+        if want_expert:
+            self._require_expert()
         if self.need_reset:
             raise Exception("Must \"reset\" before doing any actions")              # maze_env.py:60-61
         if action is None:
@@ -494,10 +508,18 @@ class _BatchedMazeBase(Snapshots):
             self._own_ptrs = (self._obs.data_ptr(), self._rew.data_ptr(), self._done.data_ptr(),
                               _lib.ptr(self._final), _lib.ptr(self._trunc))
             self._done_bool = self._done.view(torch.bool)
-        rc = self._lib.mgb_maze_step(self._h, act.data_ptr(), *self._own_ptrs, self._stream())
+        if want_expert:
+            if self._exp is None:
+                self._exp = torch.empty((self.num_envs,), dtype=torch.uint8, device=self.device)
+            rc = self._lib.mgb_maze_step_expert(self._h, act.data_ptr(), *self._own_ptrs, self._exp.data_ptr(),
+                                                self._stream())
+        else:
+            rc = self._lib.mgb_maze_step(self._h, act.data_ptr(), *self._own_ptrs, self._stream())
         if rc:
             _lib.check(rc)
         info = _LazySteps(self)
+        if want_expert:
+            info["expert"] = self._out(self._exp)
         return self._out(self._obs), self._out(self._rew), self._out(self._done_bool), info
 
     # step() and rollout(): the layout of one env's action, the numpy dtype host actions are read as (None: as given),
@@ -534,6 +556,78 @@ class _BatchedMazeBase(Snapshots):
                                               _lib.ptr(out.get("truncated") if final else None),
                                               None if cfg is None else ctypes.byref(cfg), seed, self._stream()))
         return out
+
+    def _require_expert(self):
+        if not self.with_expert:
+            raise ValueError("the expert needs an env created with expert=True")
+        if self.need_set_task:
+            raise Exception("Must call \"set_task\" before reset")
+
+    def _expert_rollout(self, T, actions, eps, deterministic, act_seed, want_expert, out, final, resample):
+        """mgb_maze_rollout_expert: rollout() with expert= or want_expert=True."""
+        self._require_expert()
+        if resample is not None:
+            raise ValueError("expert rollouts do not resample in the launch (resample_tasks between rollouts instead)")
+        if actions is not None and eps is not None:
+            raise ValueError("rollout takes either actions or expert=eps, not both")
+        if actions is None and eps is None:
+            raise ValueError("want_expert=True without actions needs expert=eps to choose the actions")
+        if eps is not None and not (math.isfinite(eps) and 0.0 <= eps <= 1.0):
+            raise ValueError("expert=eps must be a finite mixing rate in [0, 1], got %r" % (eps,))
+        if self.need_reset:
+            raise Exception("Must \"reset\" before doing any actions")
+        torch = self._torch
+        T, N, dev = int(T), self.num_envs, self.device
+        if out is None:
+            out = {"obs": torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev),
+                   "rew": torch.empty((T, N), dtype=torch.float64, device=dev),
+                   "done": torch.empty((T, N), dtype=torch.uint8, device=dev)}
+            if actions is None:
+                out["act"] = torch.empty((T, N), dtype=torch.int32, device=dev)
+            out["expert"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+            if final:
+                out["final_obs"] = torch.empty((T, N) + tuple(self._obs.shape[1:]), dtype=self._obs.dtype, device=dev)
+                out["truncated"] = torch.empty((T, N), dtype=torch.uint8, device=dev)
+        a = None
+        if actions is not None:
+            a = torch.as_tensor(actions, dtype=torch.int32, device=dev).reshape(T, N).contiguous()
+        self._trial_entries(out, None)
+        _lib.check(self._lib.mgb_maze_rollout_expert(
+            self._h, T, _lib.ptr(a), float(0.0 if eps is None else eps), int(bool(deterministic)), int(act_seed),
+            _lib.ptr(out.get("act") if a is None else None), _lib.ptr(out.get("expert")), _lib.ptr(out.get("obs")),
+            _lib.ptr(out.get("rew")), _lib.ptr(out.get("done")), _lib.ptr(out.get("final_obs") if final else None),
+            _lib.ptr(out.get("truncated") if final else None), self._stream()))
+        return out
+
+    def expert(self):
+        """An expert=True env's expert on the state every env holds now (mgb_maze_expert): (mask [N] uint8, bit a set
+        iff action a starts a shortest path to the goal; dist [N] int32, the fewest actions to the goal, 65535 where it
+        cannot be reached).  Stream-ordered."""
+        self._require_expert()
+        torch = self._torch
+        mask = torch.empty((self.num_envs,), dtype=torch.uint8, device=self.device)
+        dist = torch.empty((self.num_envs,), dtype=torch.int16, device=self.device)
+        _lib.check(self._lib.mgb_maze_expert(self._h, mask.data_ptr(), dist.data_ptr(), self._stream()))
+        return self._out(mask), self._out(dist.to(torch.int32) & 0xFFFF)
+
+    def expert_table(self, slots=None):
+        """The expert's tables of task-table slots `slots` (None: every slot; mgb_maze_expert_table): (mask [K,P,n,n]
+        uint8, dist [K,P,n,n] int32), P = 1 heading plane for MetaMaze2D and 4 (indexed by ori) for MetaMazeDiscrete3D,
+        entry [k, ori, gx, gy]."""
+        self._require_expert()
+        torch = self._torch
+        n, P = self._n_cells, 1 if self.KIND == 0 else 4
+        sl = list(range(len(self.tasks))) if slots is None else [int(k) for k in np.asarray(slots).reshape(-1)]
+        mask = torch.empty((len(sl), P, n, n), dtype=torch.uint8, device=self.device)
+        dist = torch.empty((len(sl), P, n, n), dtype=torch.int16, device=self.device)
+        if slots is None:
+            _lib.check(self._lib.mgb_maze_expert_table(self._h, 0, len(sl), mask.data_ptr(), dist.data_ptr(),
+                                                       self._stream()))
+        else:
+            for k, s in enumerate(sl):
+                _lib.check(self._lib.mgb_maze_expert_table(self._h, s, 1, mask[k].data_ptr(), dist[k].data_ptr(),
+                                                           self._stream()))
+        return mask, dist.to(torch.int32) & 0xFFFF
 
     def _check_rollout_final(self, final_obs):
         """rollout(..., final_obs=True) of the 3-D envs: the constructor's rule, per call."""
@@ -698,7 +792,7 @@ class _LazySteps(dict):
         return self[k]
 
     def __contains__(self, k):
-        return k == "steps"
+        return k == "steps" or dict.__contains__(self, k)
 
 
 def _check_policy(env, policy, state):
@@ -747,14 +841,14 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
 
     def __init__(self, enable_render=False, render_scale=480, max_steps=5000, task_type="SURVIVAL", view_grid=2,
                  num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True, final_obs=False,
-                 record_path=False, episodes_per_task=None):
+                 record_path=False, episodes_per_task=None, expert=False):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
         self.render_scale = int(render_scale)
         self.view_grid = int(view_grid)
         self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path,
-                    episodes_per_task)
+                    episodes_per_task, expert)
         w = 2 * self.view_grid + 1
         # the reference declares Box(-1, 1, (3,3), int32) but returns float32 (2g+1)^2 arrays (maze_2d.py:92)
         self.observation_space = Box(low=-1, high=1, shape=(w, w), dtype=np.float32)
@@ -768,7 +862,7 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         return cfg
 
     def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, resample=None, policy=None,
-                deterministic=False, state=None, want_hidden=False, gae=None):
+                deterministic=False, state=None, want_hidden=False, gae=None, expert=None, want_expert=False):
         """T steps in one launch (mgb_maze_rollout).  actions: [T,N] int32 CUDA tensor or None (device-drawn uniform
         {0..3}).  Returns dict(obs [T,N,<obs of one env>], rew [T,N] f64, done [T,N] u8, act [T,N] i32 or None).
 
@@ -811,7 +905,19 @@ class BatchedMetaMaze2D(_BatchedMazeBase, Mirrored):
         value[0]) and, with final_obs=True or gae, "final_value" [T,N]: V of the terminal window where an episode ended
         truncated and the policy's memory is wiped (every done, or new_tasks(out) under hidden_reset="task"), from the
         memory before the wipe; other entries are not written.  gae=(gamma, lam) also yields "adv" and "ret" [T,N]
-        float32, GAE(gamma, lam) cut where the memory is wiped (DESIGN.md "Value heads and GAE")."""
+        float32, GAE(gamma, lam) cut where the memory is wiped (DESIGN.md "Value heads and GAE").
+
+        expert=eps (an env created with expert=True; mgb_maze_rollout_expert): the action of step t is the shortest-path
+        expert's on the state before step t, mixed with uniform actions at rate eps; deterministic=True takes the lowest
+        optimal action.  act_seed keys the expert's draws.  The dict also holds "act" [T,N] int32 and "expert" [T,N]
+        uint8, the mask of optimal actions of the state each step acted on.  actions=a with want_expert=True steps the
+        given actions and labels them.  The env side is bit for bit rollout(T, actions=out["act"]).  Not with resample
+        or a policy."""
+        if expert is not None or want_expert:
+            if policy is not None:
+                raise ValueError("rollout takes either a policy or the expert, not both")
+            return self._expert_rollout(T, actions, expert, deterministic, act_seed, want_expert, out, self._want_final,
+                                        resample)
         if policy is not None:
             if actions is not None:
                 raise ValueError("rollout takes either actions or a policy, not both")
@@ -922,7 +1028,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
     def __init__(self, enable_render=False, render_scale=480, resolution=(320, 320), max_steps=5000,
                  task_type="SURVIVAL", num_envs=1, device=0, auto_reset=False, env_index_base=0, squeeze=True,
                  obs_dtype="int32", textures=None, max_vision_range=12.0, fol_angle=0.6 * PI, cache=None,
-                 final_obs=False, record_path=False, episodes_per_task=None):
+                 final_obs=False, record_path=False, episodes_per_task=None, expert=False):
         if enable_render:
             raise NotImplementedError("enable_render=True needs a display; the batched engine is headless")
         self.enable_render = False
@@ -934,7 +1040,7 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         self.cache = cache                  # None: library default (on, MGB_MAZE_CACHE); False: direct renderer only
         self.textures = textures if textures is not None else synthetic_textures(seed=0)
         self._setup(num_envs, device, task_type, max_steps, auto_reset, env_index_base, squeeze, final_obs, record_path,
-                    episodes_per_task)
+                    episodes_per_task, expert)
         torch = self._torch
         h, v = self.resolution
         self.observation_space = Box(low=0, high=256, shape=(h, v, 3), dtype=np.float32)     # maze_env.py:37-39
@@ -952,7 +1058,8 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         cfg.l_focal, cfg.text_size = 0.20, 1.0                                # maze_discrete_3d.py:116
         return cfg
 
-    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False, resample=None):
+    def rollout(self, T, actions=None, act_seed=0, want_actions=False, out=None, final_obs=False, resample=None,
+                expert=None, deterministic=False, want_expert=False):
         """T steps in one launch: obs [T,N,res_h,res_v,3] (uint8, int32 or float32), rew, done, act as for
         BatchedMetaMaze2D.rollout (mgb_maze_rollout).  Runs on the pose cache when it is in use, otherwise (an env created
         with cache=False, or when `resample` is given) on the direct raycaster; both give the same results.
@@ -968,7 +1075,13 @@ class BatchedMetaMazeDiscrete3D(_BatchedMazeBase):
         env whose episode ends at step t then gets the maze resample_tasks(done, **resample) would give it, in the same
         launch: obs[t] is its first frame on the new maze, final_obs[t] the terminal frame on the old one.  Needs
         auto_reset=True, cache=False and set_task() with one table slot per env, like resample_tasks.  Trial handles
-        (episodes_per_task=k): as for BatchedMetaMaze2D.rollout."""
+        (episodes_per_task=k): as for BatchedMetaMaze2D.rollout.
+
+        expert=eps, deterministic, want_expert (an env created with expert=True): as for BatchedMetaMaze2D.rollout, on
+        the pose cache and on the direct renderer alike."""
+        if expert is not None or want_expert:
+            return self._expert_rollout(T, actions, expert, deterministic, act_seed, want_expert, out,
+                                        self._check_rollout_final(final_obs), resample)
         return self._rollout(T, actions, act_seed, want_actions, out, final=self._check_rollout_final(final_obs),
                              resample=resample)
 
